@@ -2,7 +2,7 @@
 """bench.py -- headline benchmark: 256-channel fir_decimate_cc bank (decim 10, 199-tap HAMMING), BASELINE config 2,
 plus one leg per other BASELINE config (3: fastddc, 4: fused NFM bank, 5: overlap-add bank) in `extra`.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one pass of the hot path over one batch: 256 channels x 2.4 M cf32 samples per GPU (1 s of a
@@ -11,17 +11,22 @@ no data-path collective (independent inputs, SURVEY 8(e)) -> weak scaling.
 
 Prints ONE JSON line (rank 0):
   value      whole-job Msamples/s of complex input, inputs resident in HBM, device-timed (CUDA events), max over ranks;
-             the K timed steps follow a >= 0.7 s pre-heat of the same kernel, so they run at the power-capped clock the
-             `clocks` record shows; `sustained` repeats the measurement over >= 1 s
+             the K timed steps follow a pre-heat of the same kernel that lasts until its rate has settled (0.7 to 10 s,
+             `clocks.preheat_s`), so they run at the power-capped clock the `clocks` record shows; `sustained` repeats the
+             measurement over >= 1 s
   e2e        same metric through the host-buffer C-ABI call (csdrb_fir_decimate_bank_cc_host): pinned host input,
              H2D + kernel + D2H of the outputs inside the timed region, every step;  e2e_u8: the same bank fed with
              rtl_sdr-style u8 IQ (csdrb_fir_decimate_bank_u8_host, conversion fused into the FIR kernel)
   roofline   algorithmic bytes (8 B/sample in + 8 B/output) / measured kernel time vs MEASURED_PEAKS.json hbm_gbs
+             (else the H100 SXM data sheet's 3.35 TB/s)
   extra      configs 3, 4, 5 (and the strong-scaling split of config 2 at N > 1): value, kernel_ms, roofline, clocks per leg,
              timed with CUDA events around the C-ABI calls over >= 1 s each.  Config 4 at N > 1 moves the wideband block from
              rank 0 to every rank with an NCCL broadcast per step (double-buffered against the previous block's kernel)
   cpu_baseline  the compiled reference (oracle/_ref) or the oracle port on this box's host cores, bounded sample
 --impl reference: the reference's own CPU implementation of the same step on all host threads (rank 0 only).
+--dump-outputs DIR: after the timed steps, rank 0 writes what the last timed step computed to DIR/fir_decimate_bank_cc.npy:
+             float32 [DUMP_CHANNELS, n_out, 2] (I, Q), the output rows of a fixed, seeded choice of channels (the whole bank is
+             ~490 MB).  The inputs come from a seeded generator, so two builds given the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -44,41 +49,31 @@ CHANNELS, N_IN, TAPS, DECIM = 256, 2_400_000, 199, 10
 WORKLOAD = "256-channel fir_decimate_cc bank, decim=10, 199-tap HAMMING, 2.4 Msps/ch synthetic cf32 (BASELINE configs[1])"
 METRIC = "Msamples/s in, 256-ch fir_decimate_cc d=10"
 ALGO_BYTES_PER_SAMPLE = 8.0 + 8.0 / DECIM            # SURVEY 8(d): 8 B read per input sample + 8 B written per output
+DUMP_CHANNELS, DUMP_SEED = 24, 2024                  # --dump-outputs: 24 rows x 240 k outputs x 8 B = 46 MB (< 64 MB)
 
 
 def base_config(world: int) -> dict:
     """the `config` object of BOTH arms (the driver compares the key sets)"""
     return {"workload": WORKLOAD, "channels_per_gpu": CHANNELS, "samples_per_channel": N_IN, "taps": TAPS, "decimation": DECIM,
             "parallelism": f"channel slices, {CHANNELS} per GPU x {world} GPUs, no collective",
-            "l2": "inputs (4.9 GB per GPU) exceed the 126 MB L2; no flush needed", "timing": "CUDA events on the launch stream, max over ranks"}
+            "l2": "inputs (4.9 GB per GPU) exceed the 50 MB L2; no flush needed", "timing": "CUDA events on the launch stream, max over ranks"}
 
 
 def peaks():
     p = ROOT / "MEASURED_PEAKS.json"
     if p.exists():
-        return json.loads(p.read_text()).get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return json.loads(p.read_text()).get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json hbm_gbs, copy read+write)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
-FP32_PEAK_TFLOPS = 72.0      # 148 SMs x 128 lanes x 2 flop x 1.9 GHz: context for the FP32-bound legs (tools/bin/microbench measured 71 with FFMA)
-
-
-def ncu_traffic():
-    for name in ("r02_fir_bank_ncu_summary.json", "fir_bank_ncu_summary.json"):
-        p = ROOT / "profiles" / name
-        if p.exists():
-            try:
-                return json.loads(p.read_text()).get("dram_bytes_per_launch"), f"ncu --set full capture, profiles/{name} (static: not re-measured in this run)"
-            except Exception:
-                pass
-    return None, None
+FP32_PEAK_TFLOPS = 67.0      # H100 SXM data sheet (132 SMs x 128 lanes x 2 flop x ~1.98 GHz): context for the FP32-bound legs
 
 
 # ----------------------------------------------------------------------------------------------------
 class ClockSampler:
     """nvidia-smi clocks / throttle reasons sampled every 100 ms while the timed region runs."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, index):
         self.index, self.proc, self.lines = index, None, []
@@ -104,13 +99,13 @@ class ClockSampler:
             self.t.join(timeout=2)
 
     def summary(self):
-        sm, mx, pw, reasons = [], 0, [], set()
+        sm, mx, pw, reasons, limit = [], 0, [], set(), None
         for ln in self.lines:
             f = [x.strip() for x in ln.split(",")]
-            if len(f) < 8:
+            if len(f) < 9:
                 continue
             try:
-                sm.append(float(f[1])); mx = max(mx, float(f[2])); pw.append(float(f[3]))
+                sm.append(float(f[1])); mx = max(mx, float(f[2])); pw.append(float(f[3])); limit = float(f[8])
             except ValueError:
                 continue
             for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), f[4:8]):
@@ -119,7 +114,7 @@ class ClockSampler:
         if not sm:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["unavailable"]}
         busy = [s for s, p in zip(sm, pw) if p > 0.5 * max(pw)] or sm          # samples taken under load (power), not the idle edges
-        return {"sm_mhz": float(np.median(busy)), "sm_max_mhz": mx, "reasons": sorted(reasons), "samples": len(sm), "power_w_max": max(pw)}
+        return {"sm_mhz": float(np.median(busy)), "sm_max_mhz": mx, "reasons": sorted(reasons), "samples": len(sm), "power_w_max": max(pw), "power_limit_w": limit}
 
 
 def physical_gpu_index(local: int) -> int:
@@ -272,7 +267,7 @@ def run_b200(args):
             roof.update(achieved=gbs, peak=peak, frac=gbs / peak, fp32_tflops=tf, peak_source=peak_src)
         else:
             roof.update(achieved=tf, peak=FP32_PEAK_TFLOPS, frac=tf / FP32_PEAK_TFLOPS, algorithmic_gbs=gbs, frac_of_hbm=gbs / peak,
-                        peak_source="FP32 FMA peak 148 SMs x 128 lanes x 2 x 1.9 GHz (nominal; no tensor cores on this path)")
+                        peak_source="FP32 FMA peak of the H100 SXM data sheet (nominal; no tensor cores on this path)")
         return {"name": name, "value": total_units_factor * units_per_step / ms / 1e3, "unit": "Msamples/s", "kernel_ms": ms, "steps": n,
                 "gpu_launches": int(launches), "roofline": roof, "clocks": clk.summary(), "config": config, "note": note}
 
@@ -281,7 +276,7 @@ def run_b200(args):
     n_out = csdr_b200.fir_out_len(N_IN, DECIM, TAPS)
     ostride = n_out + (n_out & 1)
     g = torch.Generator(device=dev).manual_seed(1000 + rank)
-    x = torch.rand((CHANNELS, N_IN, 2), generator=g, device=dev, dtype=torch.float32) * 2 - 1      # 4.9 GB >> 126 MB L2
+    x = torch.rand((CHANNELS, N_IN, 2), generator=g, device=dev, dtype=torch.float32) * 2 - 1      # 4.9 GB >> 50 MB L2
     y = torch.empty((CHANNELS, ostride), dtype=torch.complex64, device=dev)
 
     # ---- config 2, device-resident leg (the headline) ---------------------------------------------------
@@ -292,25 +287,42 @@ def run_b200(args):
         fir_step(k)
     barrier()              # the first collective sets the communicator up (hundreds of ms): do it here, or the timed loop's own barrier lets the GPU cool off after the pre-heat
     with ClockSampler(physical_gpu_index(local)) as clk:
+        preheat_s = 0.0
         if not args.quick:
-            t_hold = time.perf_counter()                         # pre-heat: the timed steps below run at the clock the GPU settles to under this kernel
-            while time.perf_counter() - t_hold < 0.7:
-                for k in range(8):
-                    fir_step(k)
-                torch.cuda.synchronize()
+            # pre-heat: the timed steps below run at the clock the GPU settles to under this kernel.  A power-capped H100 keeps lowering
+            # its clock for seconds after the load starts, so hold until three ~100 ms windows agree within 0.5 % (0.7 s at least, 10 s at most).
+            t_hold = time.perf_counter()
+            rates = []
+            while True:
+                t_w, n_w = time.perf_counter(), 0
+                while time.perf_counter() - t_w < 0.1:
+                    for k in range(8):
+                        fir_step(k)
+                    torch.cuda.synchronize()
+                    n_w += 8
+                rates = (rates + [n_w / (time.perf_counter() - t_w)])[-3:]
+                preheat_s = time.perf_counter() - t_hold
+                if preheat_s >= 10.0 or (preheat_s >= 0.7 and len(rates) == 3 and max(rates) <= 1.005 * min(rates)):
+                    break
         launches0 = csdr_b200.kernel_launches()
         total_ms, per_kernel_ms = timed_loop(fir_step, args.steps)
         launches = csdr_b200.kernel_launches() - launches0
+        if args.dump_outputs and rank == 0:
+            rows = np.sort(np.random.default_rng(DUMP_SEED).choice(CHANNELS, DUMP_CHANNELS, replace=False))
+            dump = torch.view_as_real(y[torch.from_numpy(rows).to(dev), :n_out]).cpu().numpy()
         sus_ms, sus_n = (per_kernel_ms, args.steps) if args.quick else sustained(fir_step)
     samples_per_step = CHANNELS * N_IN
     value = world * samples_per_step * args.steps / total_ms / 1e3                                   # Msamples/s, whole job
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "fir_decimate_bank_cc.npy"), np.ascontiguousarray(dump, np.float32))
     if args.quick:
         if rank == 0:
             print(json.dumps({"quick": True, "value": value, "unit": "Msamples/s", "kernel_ms": per_kernel_ms, "gpu_launches": int(launches)}), flush=True)
         if world > 1:
             dist.destroy_process_group()
         return
-    main_clocks = clk.summary()
+    main_clocks = dict(clk.summary(), preheat_s=preheat_s)
 
     # ---- config 2, strong-scaling split (256 / N channels per GPU): SURVEY 8(e)'s partition next to the weak one ----------
     if world > 1 and not args.no_extra:
@@ -373,7 +385,6 @@ def run_b200(args):
     if rank == 0:
         algo_bytes = samples_per_step * 8.0 + CHANNELS * n_out * 8.0
         achieved = algo_bytes / (per_kernel_ms * 1e-3) / 1e9
-        traffic, traffic_src = ncu_traffic()
         line = {"metric": METRIC, "value": value, "unit": "Msamples/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
                 "ms_per_step": total_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
                 "dtype": "f32", "data": "synthetic",
@@ -385,7 +396,7 @@ def run_b200(args):
                            "steps": e2e_steps, "api": "csdrb_fir_decimate_bank_u8_host (u8 IQ in, convert_u8_f fused into the FIR kernel; csdr-fm:41)",
                            "checksum": checksum_u8, "vs_cf32_e2e": e2e_u8_value / e2e_value},
                 "gpu_launches": int(launches),
-                "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src,
+                "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                              "peak_source": peak_src, "algorithmic_bytes_per_launch": algo_bytes, "kernel_ms": per_kernel_ms,
                              "fp32_tflops": CHANNELS * n_out * TAPS * 4 / (per_kernel_ms * 1e-3) / 1e12,
                              "note": "8.8 algorithmic B/sample at 79.6 flop/sample sits on the FP32/HBM ridge; both are reported"},
@@ -485,7 +496,7 @@ def other_configs(torch, dist, cb, L, dev, world, rank, local, leg, check, cur_s
     bw3, dec3, C3 = 0.002, 64, 64
     c3 = max(1, C3 // world)
     ddc = cb.fastddc_init(bw3, dec3, 0.0)
-    nblocks = 592                                                          # 4 x 148 SMs: whole waves for the forward FFT (a CTA per block) and for the fold (a CTA per 16 blocks x 16 ch x 64 bins)
+    nblocks = 528                                                          # 4 x 132 SMs: whole waves for the forward FFT (a CTA per block) and for the fold (a CTA per 16 blocks x 16 ch x 64 bins)
     nsamp = nblocks * ddc.input_size
     gen = torch.Generator(device=dev).manual_seed(3)
     xw = torch.view_as_complex(torch.rand((nsamp, 2), generator=gen, device=dev) * 2 - 1)
@@ -562,7 +573,8 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extra", action="store_true", help="skip the config 3/4/5 legs")
-    ap.add_argument("--quick", action="store_true", help="device-resident leg only (for ncu runs): no clock hold loop, no e2e, no CPU baseline")
+    ap.add_argument("--quick", action="store_true", help="device-resident leg only: no clock hold loop, no e2e, no CPU baseline")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs (a fixed sample of the bank) as DIR/*.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else max(args.warmup, 1)
     if args.impl == "reference":

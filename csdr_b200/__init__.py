@@ -1,4 +1,4 @@
-"""csdr_b200 -- B200-native csdr block-DSP hot path.
+"""csdr_b200 -- H100-native csdr block-DSP hot path.
 
 This package is a thin Python mirror of the C ABI in ``include/csdr_b200.h`` (ctypes; no torch types cross
 the boundary -- tensors are passed as raw device pointers + the current CUDA stream handle).  PyTorch is

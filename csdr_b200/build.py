@@ -1,5 +1,5 @@
-"""Builds csdr_b200/libcsdr_b200.so in-tree: nvcc for the kernels + C ABI (sm_100a only), gcc for the
-host-side C (filter design, geometry).  The .so is git-ignored but travels to the GPU box with gpurun."""
+"""Builds csdr_b200/libcsdr_b200.so in-tree: nvcc for the kernels + C ABI (sm_90a only), gcc for the
+host-side C (filter design, geometry).  The .so is git-ignored: build() makes it."""
 from __future__ import annotations
 
 import hashlib
@@ -15,7 +15,7 @@ HOST = PKG / "host"
 OBJ = PKG / "build"
 LIB = PKG / "libcsdr_b200.so"
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xptxas", "-v", "--fmad=true", "--expt-relaxed-constexpr", "-diag-suppress", "20281", f"-I{ROOT / 'include'}", f"-I{CSRC}"]
 GCC_FLAGS = ["-std=gnu99", "-O2", "-fno-fast-math", "-ffp-contract=off", "-fPIC", f"-I{ROOT / 'include'}"]
 
@@ -78,7 +78,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         stale = OBJ / "bankd.host.o"
         if stale.exists():
             stale.unlink()
-        cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-Xlinker", f"--version-script={vs}", "-o", str(LIB)] + [str(o) for o in objs] + ["-lm", "-ldl"]
+        cmd = [_nvcc(), "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-Xlinker", f"--version-script={vs}", "-o", str(LIB)] + [str(o) for o in objs] + ["-lm", "-ldl"]
         subprocess.run(cmd, check=True)
     cli_src = HOST / "csdr_cli.c"
     cli = PKG / "csdr"

@@ -104,7 +104,7 @@ extern "C" {
 // Part B
 // =====================================================================================================
 const char* csdrb_last_error(void) { return g_err; }
-const char* csdrb_version(void) { return "csdr_b200 0.1 (sm_100a)"; }
+const char* csdrb_version(void) { return "csdr_b200 0.1 (sm_90a)"; }
 int csdrb_device_count(void)
 {
     int n = 0;
@@ -232,9 +232,8 @@ static HostBank& host_bank()                                     // one per devi
 }
 
 // Page-locked memory on the NUMA node the current device hangs off.  cudaHostAlloc places the pages where the calling thread runs; with one
-// process per GPU on a two-socket host half the ranks would otherwise stream their H2D traffic across the socket interconnect (SCALE_r01: e2e
-// efficiency 0.56 at 8 GPUs).  The thread is moved onto the device's node for the duration of the allocation (sysfs: the PCI device's
-// numa_node and that node's cpulist), then gets its old affinity back.  Any failure along the way just leaves the default placement.
+// process per GPU on a two-socket host half the ranks would otherwise stream their H2D traffic across the socket interconnect.
+// The thread is moved onto the device's node for the duration of the allocation (sysfs: the PCI device's numa_node and that node's cpulist), then gets its old affinity back.  Any failure along the way just leaves the default placement.
 static bool cpus_of_device_node(cpu_set_t* set)
 {
     int dev = 0; char bus[32] = "";

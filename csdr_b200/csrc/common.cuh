@@ -1,10 +1,10 @@
-// common.cuh -- shared device helpers for the csdr_b200 kernels (sm_100a only).
+// common.cuh -- shared device helpers for the csdr_b200 kernels (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "csdr_b200 kernels are written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "csdr_b200 kernels are written for sm_90a (H100) only"
 #endif
 
 // dynamic shared memory of a kernel; the CPU-tier emulator (tests/host_shim/cuda_emul.h) supplies its own definition
@@ -13,6 +13,9 @@
 #endif
 
 namespace csdrb {
+
+// SMs of an H100 SXM: the launch-size heuristics aim at whole waves of this many SMs
+constexpr long kSmCount = 132;
 
 // ---- error plumbing (host) ---------------------------------------------------------------------
 // Every C-ABI entry point returns >= 0 on success and a negative csdrb_status on failure; the text of
@@ -27,36 +30,17 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line);
 
 // The inline-PTX helpers below have C++ models in tests/host_shim/cuda_emul.h (CPU test tier); the product never defines this macro.
 #ifndef CSDRB_HOST_EMULATION
-// ---- packed FP32 (Blackwell FFMA2 / FADD2 / FMUL2) --------------------------------------------
-// One instruction does the I and the Q lane of a complex sample.  Each half is an IEEE-754 fp32
-// operation (round-to-nearest-even), so results are identical to two scalar FFMA/FADD/FMUL.
-// CAUTION: ptxas (12.9) contracts fadd2(fmul2(a, b), c) into ONE FFMA2 despite the explicit .rn and even under --fmad=false,
-// unlike the scalar __fmul_rn/__fadd_rn pair.  Where a product has to be rounded on its own, add with scalar __fadd_rn.
+// ---- complex-lane FP32 pairs ------------------------------------------------------------------
+// The I and the Q lane of a complex sample.  Hopper has no packed FP32 instruction, so each helper is two
+// scalar IEEE-754 fp32 operations (round-to-nearest-even); the _rn intrinsics keep ptxas from contracting
+// a separately rounded product into a later add.
 __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c)
 {
-    uint64_t ra = *reinterpret_cast<uint64_t*>(&a), rb = *reinterpret_cast<uint64_t*>(&b),
-             rc = *reinterpret_cast<uint64_t*>(&c), rd;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-    return *reinterpret_cast<float2*>(&rd);
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
 }
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b)
-{
-    uint64_t ra = *reinterpret_cast<uint64_t*>(&a), rb = *reinterpret_cast<uint64_t*>(&b), rd;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-    return *reinterpret_cast<float2*>(&rd);
-}
-__device__ __forceinline__ float2 fsub2(float2 a, float2 b)
-{
-    uint64_t ra = *reinterpret_cast<uint64_t*>(&a), rb = *reinterpret_cast<uint64_t*>(&b), rd;
-    asm("sub.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-    return *reinterpret_cast<float2*>(&rd);
-}
-__device__ __forceinline__ float2 fmul2(float2 a, float2 b)
-{
-    uint64_t ra = *reinterpret_cast<uint64_t*>(&a), rb = *reinterpret_cast<uint64_t*>(&b), rd;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-    return *reinterpret_cast<float2*>(&rd);
-}
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fsub2(float2 a, float2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 // ---- mbarrier + bulk async copy (the 1-D TMA path: SASS UBLKCP) ----------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }

@@ -5,17 +5,17 @@
 // Mapping: LANE = CHANNEL.  All 32 lanes of a warp walk the same wideband samples in the same order, so
 //   * the wideband sample is one broadcast load per warp (shared input: 8 B per sample, L1/L2 resident),
 //   * the FIR tap for sample n and output o is the same for every lane -> taps live in uniform registers
-//     (kernel parameter, duplicated (h,h) for FFMA2), exactly like the independent-input bank kernel,
+//     (kernel parameter, duplicated (h,h) for FFMA pair), exactly like the independent-input bank kernel,
 //   * each lane keeps its own NCO phasor (the reference's float recursion, re-seeded at every chunk boundary from the
 //     replayed float phase chain) and its own M = ceil(T/D) running output accumulators in registers.
-// Per wideband sample and channel: 4 flop rotation + 6 flop recursion + 2*M FFMA2 lanes; nothing goes through shared memory,
+// Per wideband sample and channel: 4 flop rotation + 6 flop recursion + 2*M FFMA pair lanes; nothing goes through shared memory,
 // the shifted stream never exists in HBM (the unfused chain writes and re-reads 8*C bytes per wideband sample).
 // A warp owns a time segment of SEG outputs (plus M-1 trailing periods to finish its last outputs); segments are independent
 // because the phasor of any sample depends only on its chunk's seed and its position inside the chunk.
 //
 // The float phase chain is a separate one-thread-per-channel pre-pass.  Folding it into this kernel as a ticketed producer CTA was
-// tried and measured SLOWER (2.27 ms vs 2.06 ms at 2 M samples x 128 ch): the whole grid is resident at once, so every segment needs
-// its chunk phase at t = 0 and nothing overlaps, while the producer runs ~3x slower on a shared SM.  The remaining lever is to run the
+// tried and was slower: the whole grid is resident at once, so every segment needs
+// its chunk phase at t = 0 and nothing overlaps, while the producer runs several times slower on a shared SM.  The remaining lever is to run the
 // pre-pass of block k+1 on a side stream during the main kernel of block k (it only depends on the previous pre-pass).
 //
 // Bound: FP32 issue (SURVEY 8(d) cfg4): ~ (10 + 4*M) FMA-lane slots per (sample, channel).
@@ -61,11 +61,11 @@ ddc_wrap_tables_kernel(const float3* __restrict__ params, int chunk, WrapTable* 
     if (c < channels && threadIdx.x == 0) wrap_table_build(__fmul_rn(__fmul_rn(params[c].z, 3.14159265358979323846f), (float)chunk), tables + c);
 }
 
-// One warp walks DDC_CHAIN_CPW channels (1: more than one per warp does not interleave -- the wrap's branches and votes keep the chains in program order;
-// measured on the fastddc and shift chains, r02 call 19).
+// One warp walks DDC_CHAIN_CPW channels (1: more than one per warp does not interleave -- the wrap's branches and votes keep the chains in program order,
+// as on the fastddc and shift chains).
 constexpr int DDC_CHAIN_CPW = 1;
 constexpr int DDC_CHAIN_WARPS = 1;                 // chains per CTA.  The pre-pass of block k+1 runs NEXT TO block k's main kernel, whose three CTAs leave ~10 K registers per SM: a one-warp
-                                                   // CTA slips in, an eight-warp CTA has to wait for an SM to drain and the pre-pass serialises behind the main kernel (0.88 instead of 0.64 ms per block)
+                                                   // CTA slips in, an eight-warp CTA has to wait for an SM to drain and the pre-pass serialises behind the main kernel
 
 __global__ void __launch_bounds__(32 * DDC_CHAIN_WARPS)
 ddc_phase_chain_kernel(const float3* __restrict__ params, float* __restrict__ phase_io, float* __restrict__ chunk_phase,
@@ -122,8 +122,8 @@ __global__ void ddc_rechunk_kernel(const float3* __restrict__ params, float* __r
 }
 
 // CPL = channels per lane.  A tap pair is loaded once per warp and sample phase (LDCU.128 fetches two of them: taps are stored
-// [p][j] so the M taps that one sample meets are contiguous); with CPL = 2 every loaded tap feeds two FFMA2 and every wideband
-// sample load feeds two channels, which halves the non-FMA issue slots per channel-sample (ncu r01: 868 LDCU per 850 FFMA2 at CPL = 1).
+// [p][j] so the M taps that one sample meets are contiguous); with CPL = 2 every loaded tap feeds the FMAs of two channels and every
+// wideband sample load feeds two channels, which halves the non-FMA issue slots per channel-sample (at CPL = 1 there is about one tap load per FMA pair).
 template <int D, int M, int CPL, bool DEMOD>
 __global__ void __launch_bounds__(128)
 ddc_bank_fused_kernel(const float2* __restrict__ wide, int n_in, int offset, int chunk, int nchunks,
@@ -239,15 +239,15 @@ ddc_bank_fused_kernel(const float2* __restrict__ wide, int n_in, int offset, int
 // ---- v2 (round 2): taps in shared memory, packed phasor arithmetic, ramp-aware tap ranges ---------------------------------------
 // What the round-1 ncu profile of the kernel above showed: FMA pipe 29 %, issue 45 % -- neither saturated.  Three structural costs:
 //  (1) every tap pair was an LDCU from a 7.2 KB kernel parameter walked once per period: far more than the uniform/constant L0 holds, so the
-//      FFMA2 stream waited on constant-cache refills.  Here the CTA copies the taps once into shared memory ((h,h) pairs, [p][j] layout) and a
+//      FFMA pair stream waited on constant-cache refills.  Here the CTA copies the taps once into shared memory ((h,h) pairs, [p][j] layout) and a
 //      warp fetches two taps with one broadcast LDS.128 (one wavefront, 29-cycle fixed latency the compiler pipelines).
 //  (2) rotation and recursion cost 10 scalar FMA-pipe slots per (sample, channel).  With the phasor kept twice, P = (c, s) and Q = (-s, c),
-//          shifted = x.i * P + x.q * Q                        (FMUL2 + FFMA2 -- libcsdr_gpl.c:39-40 up to one fused product)
-//          P'      = cosd * P + sind * Q                      (FMUL2, FMUL2, FADD, FADD: the reference's two rounded products and their sum, :42-45)
+//          shifted = x.i * P + x.q * Q                        (FMUL pair + FFMA pair -- libcsdr_gpl.c:39-40 up to one fused product)
+//          P'      = cosd * P + sind * Q                      (FMUL pair, FMUL pair, FADD, FADD: the reference's two rounded products and their sum, :42-45)
 //          Q'      = (-P'.y, P'.x)                            (operand swizzle / negate modifiers of the packed instructions: free)
 //      it is 6 slots; the phasor state stays bit-identical to the scalar sequence (negation commutes with rounding).
 //  (3) a warp's time segment spends M-1 periods filling and M-1 periods draining its accumulators; with ~40-output segments that was a third of
-//      all FFMA2.  Here the head and tail periods only touch the accumulators that belong to emitted outputs, in groups of four taps
+//      all FFMA pair.  Here the head and tail periods only touch the accumulators that belong to emitted outputs, in groups of four taps
 //      (template <JLO, JHI>), which removes ~80 % of that waste.
 // Work decomposition: warp-granular 1-D grid; warp w owns (segment, channel set) = (w / sets, w % sets), a channel set = 32*CPL channels.
 template <int D, int M, int CPL, bool DEMOD>
@@ -263,17 +263,15 @@ struct DdcWalk {
     }
     __device__ __forceinline__ void advance(int u)
     {
-        // ptxas contracts mul.rn.f32x2 + add.rn.f32x2 into FFMA2 (even with --fmad=false), which would drop one of the reference's two
-        // product roundings: the sum is two scalar FADDs, which it leaves alone (SASS: FMUL2, FMUL2, FADD, FADD)
+        // two rounded products and their rounded sum, as in the reference (the _rn helpers keep ptxas from fusing a product into the add)
         const float2 a = fmul2(P[u], cd2[u]), b = fmul2(Q[u], sd2[u]);
         const float2 pn = make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y));
         P[u] = pn;
         Q[u] = make_float2(__uint_as_float(__float_as_uint(pn.y) ^ 0x80000000u), pn.x);
     }
     // one wideband sample against the taps of its phase p (tp = taps of phase p, MP/2 float4), accumulators JLO..JHI-1 only
-    // The taps come as SCALARS (two per 64-bit shared load) and enter the FFMA2 as (h, h) built from one register: ptxas turns that into the .F32 broadcast
-    // modifier, so the tap operand is one register (and sits in the reuse latch for both channels of the lane) and four taps come with one 128-bit shared load;
-    // the first form kept every tap duplicated (h, h) in shared memory and in a register pair (207 LDS in the kernel instead of 134).
+    // The taps come as SCALARS (two per 64-bit shared load) and multiply the I and the Q lane of the shifted sample: the tap operand is one register
+    // for both channels of the lane, and four taps come with one 128-bit shared load (a copy duplicated (h, h) in shared memory needs twice the loads).
     template <int JLO, int JHI>
     __device__ __forceinline__ void sample(float xi, float xq, const float2* __restrict__ tp)
     {
@@ -360,7 +358,7 @@ ddc_bank_fused2_kernel(const float2* __restrict__ wide, int n_in, int offset, in
         constexpr int JLO = decltype(jlo)::value, JHI = decltype(jhi)::value;
         constexpr int UU = (JLO == 0 && JHI == MP) ? U : 2;             // the steady-state body is unrolled deeper than the ramps
         const long base = (long)q * D;
-        // (fetching the next group's samples into registers while this one is multiplied was measured: 762 vs 724 us -- the extra registers cost more
+        // (fetching the next group's samples into registers while this one is multiplied was slower: the extra registers cost more
         // than the exposed L1 round trip)
 #pragma unroll 1
         for (int p0 = 0; p0 < D; p0 += UU) {
@@ -450,7 +448,7 @@ static int launch_fused(const float2* wide, int n_in, int offset, int chunk, int
                         int demod, void* out, long out_stride, int n_out, const float2* last_in, float2* last_out, const float* h_taps, int T, cudaStream_t st)
 {
     constexpr int MP = (M + 1) & ~1;
-    DdcTaps<D * MP> tp;                                                 // tap k = jD + p stored at [p][j], duplicated for FFMA2
+    DdcTaps<D * MP> tp;                                                 // tap k = jD + p stored at [p][j], duplicated for FFMA pair
     for (int p = 0; p < D; p++)
         for (int j = 0; j < MP; j++) {
             const int k = j * D + p; const float h = (j < M && k < T) ? h_taps[k] : 0.f;
@@ -465,7 +463,7 @@ static int launch_fused(const float2* wide, int n_in, int offset, int chunk, int
     const int cpl = cpl_env == 2 ? 2 : 1;
     const int warps_per_seg = (channels + 32 * cpl - 1) / (32 * cpl);
     // enough warps to fill the machine while keeping the M-1 trailing periods of every segment a small fraction
-    long want_segments = (148L * wps_env + warps_per_seg - 1) / warps_per_seg;
+    long want_segments = (kSmCount * wps_env + warps_per_seg - 1) / warps_per_seg;
     int seg = (int)((n_out + want_segments - 1) / want_segments);
     if (seg < 2 * M) seg = 2 * M;
     const int nsegs = (n_out + seg - 1) / seg;

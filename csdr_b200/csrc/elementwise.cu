@@ -154,7 +154,7 @@ __global__ void compress_fft_adpcm_rows_kernel(const float* __restrict__ in, lon
 static int grid_for(long work_items, int block)
 {
     long g = (work_items + block - 1) / block;
-    const long cap = 148L * 16;                               // 16 resident CTAs of 256 threads per SM is plenty
+    const long cap = kSmCount * 16;                              // 16 resident CTAs of 256 threads per SM is plenty
     return (int)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 

@@ -24,8 +24,8 @@
 
 namespace csdrb {
 
-// Radix-16 passes (fft16.cuh) are the default since the round-2 A/B on a B200 (profiles/r02_ab_*): 4096-pt 313 -> 379 Gsamples/s, 16384-pt 188 -> 211,
-// fastddc forward 101 -> 113, config-5 overlap-add 84.6 -> 97.5.  CSDRB_FFT_RADIX16=0 selects the radix-8 kernels (kept for A/B runs and for sizes
+// Radix-16 passes (fft16.cuh) are the default: fewer passes over shared memory than radix 8 for the 4096- and 16384-point
+// transforms, the fastddc forward FFT and the config-5 overlap-add bank.  CSDRB_FFT_RADIX16=0 selects the radix-8 kernels (kept for A/B runs and for sizes
 // without a radix-16 plan).
 static bool fft_radix16_enabled()
 {
@@ -142,12 +142,12 @@ int launch_olafir_bank(const float2* d_in, long in_stride, float2* d_out, long o
     if (int rc = get_twiddles(fft_size, &tw, st)) return rc;
     if (blocks_per_cta <= 0) {
         // enough CTAs to fill the machine a few times over, but runs long enough that the recomputed lead-in block stays cheap
-        long want = (148L * 8 + channels - 1) / channels;
+        long want = (kSmCount * 8 + channels - 1) / channels;
         blocks_per_cta = (int)((nblocks + want - 1) / want);
         if (blocks_per_cta < 16) blocks_per_cta = nblocks < 16 ? nblocks : 16;
     }
     const dim3 grid((nblocks + blocks_per_cta - 1) / blocks_per_cta, channels);
-    static const bool staged = getenv("CSDRB_OLAFIR_STAGED") != nullptr;            // A/B switch: the r01 kernel with staged copies
+    static const bool staged = getenv("CSDRB_OLAFIR_STAGED") != nullptr;            // A/B switch: the first kernel, with staged copies
     static const bool radix16 = fft_radix16_enabled();
     if (radix16 && !staged && (fft_size == 256 || fft_size == 4096)) {
         const float2* tw16 = nullptr;
@@ -387,11 +387,11 @@ int launch_fastddc_inv_bank(const float2* d_spectra, int nblocks, const float2* 
     CSDRB_CUDA(cudaGetLastError());
     if (fft_inv_size <= 1024 && fft_inv_size >= 8 && (fft_size / fft_inv_size) % 2 == 0) {
         // Tile = CT channels x BT blocks per CTA (each spectrum bin fetched once per CT channels, each tap once per BT blocks).  Big tiles
-        // save L2 traffic but a bank of 64 channels x 16 blocks is only 64 CTAs of 4x4 on 148 SMs (r01: the launch was latency-bound),
+        // save L2 traffic but a bank of 64 channels x 16 blocks is only 64 CTAs of 4x4 on the whole GPU (the launch is latency-bound),
         // so the tile shrinks until the grid covers the machine about twice.  CSDRB_INV_TILE=44|22 forces one for A/B runs.
         static const char* forced = getenv("CSDRB_INV_TILE");
         const long ctas44 = (long)((nblocks + 3) / 4) * ((channels + 3) / 4);
-        const bool small_tile = forced ? (forced[0] == '2') : (ctas44 < 2 * 148);
+        const bool small_tile = forced ? (forced[0] == '2') : (ctas44 < 2 * kSmCount);
         const int CTv = small_tile ? 2 : 4, BTv = small_tile ? 2 : 4;
         const dim3 tgrid((nblocks + BTv - 1) / BTv, (channels + CTv - 1) / CTv);
         const size_t smem = sizeof(float2) * (size_t)CTv * BTv * fft_smem_elems(fft_inv_size);
@@ -424,8 +424,8 @@ int launch_fastddc_inv_bank(const float2* d_spectra, int nblocks, const float2* 
 
 
 // ---- fastddc inverse bank with look-ahead ---------------------------------------------------------------------------------------------
-// The stateless call above has the chain + phasor walk (57 + 10..57 us for 64 channels x 256 blocks) inside every call, next to a fold that
-// keeps the FMA pipe busy: r02 timeline, the post step waits ~115 us for them while the fold is done after 90..108.  They depend on nothing
+// The stateless call above has the chain + phasor walk inside every call, next to a fold that
+// keeps the FMA pipe busy: the post step waits for them after the fold is done.  They depend on nothing
 // but the channel parameters and the carried state, so a plan object that OWNS that state prepares call k+1 while call k's IFFT/post step
 // and the caller's next forward FFT run: two sets of {state, per-block arrays, phasors}, set q is written by the side stream while set p is
 // read by the main stream.  Same kernels, same order of operations per channel: the outputs are those of the stateless call, bit for bit
@@ -551,7 +551,7 @@ int fastddc_inv_plan_run(void* plan, const float2* d_spectra, const float2* d_ta
     const int q = 1 - p;
     CSDRB_CUDA(cudaStreamWaitEvent(pl->side, pl->post_done[q], 0));       // set q was last read two runs ago (a never-recorded event does not block)
     if (trace) CSDRB_CUDA(cudaEventRecord(tev[3], pl->side));
-    // Measured at 592 blocks (r02 call 18): a chain walked NEXT TO the fold stretches the fold from 168 to 205 us (one chain warp per channel, 64 SMs with a guest
+    // A chain walked NEXT TO the fold stretches the fold (one chain warp per channel, 64 SMs with a guest
     // that holds up every barrier of the fold CTA there), so chain and walk go behind the fold, next to the IFFT step and the caller's next forward FFT
     // ('f', the default).  CSDRB_PLAN_ORDER for A/B: 'd' = chain at once, walk behind the fold; 'i' = chain at once, walk behind the IFFT step; 's' = both behind the IFFT step.
     static const char order = getenv("CSDRB_PLAN_ORDER") ? getenv("CSDRB_PLAN_ORDER")[0] : 'f';

@@ -3,7 +3,7 @@
 // Stands behind the reference's FFT abstraction (fft_fftw.c:6-41: unnormalised DFT, exponent sign -1
 // forward / +1 backward).  One CTA transforms one N-point signal that already sits in shared memory.
 //
-// Pass structure (validated against numpy in the design notes, DESIGN.md section K7): radices are
+// Pass structure (validated against numpy): radices are
 // [2 or 4 (if log2 N is not a multiple of 3)] followed by radix-8 passes.  For a pass of radix R over
 // sub-transforms of size Ns (Ns = product of the previous radices), butterfly j in [0, N/R):
 //     k = j mod Ns;   v[r] = s[j + r*N/R] * W_N^(k*r*N/(Ns*R));   V = DFT_R(v);   s'[(j/Ns)*Ns*R + k + r*Ns] = V[r]
@@ -11,8 +11,8 @@
 // (a thread holds at most 16 points per pass, so NT >= N/16 threads are required).
 // Twiddles: for a radix-8 pass over sub-transforms of size NS the butterfly with k = j mod NS needs w^r, w = exp(-2*pi*i*k/(8*NS)).
 // Three planes of a per-size table hold w^1, w^2, w^4 at index NS + k (the ranges [NS, 2NS) of the different passes do not
-// overlap), computed in double on the host and rounded once to float; lanes with consecutive k read consecutive entries (the r01
-// profile showed seven scattered LDGs per butterfly saturating L1TEX).  w^3, w^5, w^6, w^7 are one float product each, so every
+// overlap), computed in double on the host and rounded once to float; lanes with consecutive k read consecutive entries (seven
+// scattered LDGs per butterfly would saturate L1TEX).  w^3, w^5, w^6, w^7 are one float product each, so every
 // twiddle is within ~2 ulp and the whole transform stays ~1e-7*log2 N from the exact DFT.
 #pragma once
 #include "common.cuh"
@@ -353,8 +353,8 @@ __device__ __forceinline__ void block_fft_io(float2* __restrict__ s, const float
     }
 }
 
-// Prologue copy global -> padded shared array.  All of a thread's loads are issued before the first store: the r01 source-level
-// profile had 58 % of the 4096-point kernel's stall samples on the first STS of a load-then-store loop (16 serial DRAM round trips).
+// Prologue copy global -> padded shared array.  All of a thread's loads are issued before the first store: a load-then-store loop
+// serialises one DRAM round trip per element (16 for the 4096-point kernel).
 template <int N, int NT, typename Fetch>
 __device__ __forceinline__ void fft_stage_in(float2* __restrict__ s, int tid, Fetch fetch)
 {

@@ -306,12 +306,12 @@ __device__ __forceinline__ float ddc_wrap(float ph) { return wrap_phase_pm_pi(ph
 
 // Walk the block-to-block state of decimating_shift_addition_cc (libcsdr_gpl.c:154-158), one WARP per CHAIN_CPW channels.  A chain is sequential and a step
 // is ~400 cycles of dependent latency; letting one warp carry four channels "side by side" did NOT interleave them -- the wrap's warp-uniform branches and
-// votes keep the steps of different chains in program order, so four chains per warp ran four times as long on a quarter of the SMs (592 blocks: 211 us
-// against 130 us; r02 call 19).  The code stays generic, the constant is 1.
+// votes keep the steps of different chains in program order, so four chains per warp run four times as long on a quarter of the SMs.  The code stays
+// generic, the constant is 1.
 constexpr int CHAIN_CPW = 1;
 
 // CHAIN_WARPS chains per CTA: the chains run NEXT TO other kernels (the fold, the IFFT step), and a guest warp slows its host SM's CTAs down -- eight warps per CTA put the 64
-// chains of config 3 on 8 SMs instead of 64 (forward + plan loop at 592 blocks: 0.349 -> 0.331 ms; the fold's one CTA per SM leaves room for a 256-thread guest, which
+// chains of config 3 on 8 SMs instead of 64 (the fold's one CTA per SM leaves room for a 256-thread guest, which
 // the fused NFM bank's three CTAs per SM do not: its chain kernel keeps one warp per CTA).
 constexpr int CHAIN_WARPS = 8;
 
@@ -441,7 +441,7 @@ fastddc_inv_kernel(const float2* __restrict__ spectra /*[nblocks][N]*/, const fl
 }
 
 // Tiled variant for M <= 1024: one CTA folds CT channels x BT blocks at once, so every spectrum bin is fetched once per CT
-// channels and every tap once per BT blocks (r01: the untiled kernel moved 256 KB of L2 traffic per (channel, block) and ran
+// channels and every tap once per BT blocks (the untiled kernel moves 256 KB of L2 traffic per (channel, block) and runs
 // at the L2 bandwidth limit).  The CT*BT inverse FFTs run four at a time (64 threads each); the CT*BT sequential post-shift
 // chains run on CT*BT different lanes in parallel.  Summation order per destination bin is still ascending, as in the reference.
 template <int M, int CT, int BT>
@@ -535,22 +535,20 @@ fastddc_inv_tiled_kernel(const float2* __restrict__ spectra, const float2* __res
 
 
 // ---- fastddc inverse, round 2: fold as a batched complex contraction + a separate IFFT / post-shift kernel ------------------------------
-// Round 1's tiled kernel above reached 10 Gsamples/s (2.7 % of the HBM roof, 8 % of FP32): ncu showed 13 warps per issue waiting on the
-// fold's global loads, and a 4x4 tile still pulls 1.07 GB through L2 per 64 ch x 256 blocks.  The fold is, per residue r of M,
+// The tiled kernel above waits on the fold's global loads, and a 4x4 tile still pulls 1.07 GB through L2 per 64 ch x 256 blocks.  The fold is, per residue r of M,
 //     F[c][b][r] = sum_{k < P}  Xs[b][r + k*M] * H[c][r + k*M],           P = N / M  (= pre_decimation)
 // i.e. M independent complex (C x P) * (P x B) products.  fastddc_fold_kernel runs it like a GEMM: a CTA owns 64 residues x 16 channels x
 // 16 blocks; per k-step the 16 spectrum rows and 16 tap rows (8 KB each) arrive by cp.async into a 4-stage ring, every value is read from
-// shared memory by two thread groups, and a thread keeps an 8 x 8 accumulator tile for its residue (128 FFMA2 per 16 LDS.64).  L2 traffic
+// shared memory by two thread groups, and a thread keeps an 8 x 8 accumulator tile for its residue (128 FFMA pair per 16 LDS.64).  L2 traffic
 // drops to 0.27 GB, the inner loop is FMA-pipe bound.  Summation per destination bin is still ascending in the bin index, as in
-// fastddc.c:126-141 (k ascending = bin index ascending); products and sums are fused (FFMA2), inside the 1e-5 budget.
+// fastddc.c:126-141 (k ascending = bin index ascending); products and sums are fused (FFMA pair), inside the 1e-5 budget.
 // The folded bins go to a scratch array (L2-sized: 64 ch x 256 blocks x 512 bins = 67 MB), fastddc_ifft_rows_kernel does IFFT_M, /M,
 // scrap and the post shift; the block-to-block state chain runs on a side stream meanwhile (it is data-independent).
 constexpr int FOLD_R = 64, FOLD_CT = 8, FOLD_BT = 8, FOLD_ST = 3;     // residues per CTA, thread tile (channels x blocks), pipeline stages
 
 // BT = blocks per thread tile: 8 -> 256 threads (8 warps per SM), 4 -> 512 threads (16 warps, half the accumulators per thread: more latency hiding, more
 // shared-memory reads per FMA).  The CTA tile is 64 residues x 16 channels x 16 blocks either way.
-// HFIRST = the tap pair is the FIRST multiplicand of the packed FMA (ptxas keeps the first operand in the reuse cache across consecutive FFMA2: with the
-// pair there an instruction reads 3 registers instead of 4, and swap + negate become modifiers of that slot -- no MOV/FADD to build (-hi, hr)).
+// HFIRST = the tap pair is the FIRST multiplicand of each FMA pair (operand order only; both forms compute the same values).
 template <int BT, bool HFIRST>
 __global__ void __launch_bounds__(64 * 2 * (2 * FOLD_BT / BT), 1)
 fastddc_fold_kernel(const float2* __restrict__ spectra /*[nblocks][N]*/, const float2* __restrict__ taps_fft /*[C][N]*/, const DdcChan* __restrict__ chan,
@@ -578,7 +576,7 @@ fastddc_fold_kernel(const float2* __restrict__ spectra /*[nblocks][N]*/, const f
 #pragma unroll
         for (int q = 0; q < CPT; q++) cp_async16(sm + stage * STAGE + dsto[q], src[q] + (long)(q < CPT / 2 ? kx : k) * M);
     };
-    // (a 4-stage ring with the next step's operands pulled into registers during the FMAs was measured slower: 96 vs 88 us, 233 registers)
+    // (a 4-stage ring with the next step's operands pulled into registers during the FMAs was slower: it needs ~230 registers)
     float2 acc[FOLD_CT][BT];
 #pragma unroll
     for (int u = 0; u < FOLD_CT; u++)
@@ -599,7 +597,7 @@ fastddc_fold_kernel(const float2* __restrict__ spectra /*[nblocks][N]*/, const f
 #pragma unroll
         for (int u = 0; u < FOLD_CT; u++) h[u] = hs[u * FOLD_R];
         // acc += x*h = xr*(hr, hi) + xi*(-hi, hr): two packed FMAs per accumulator, scalar-broadcast x against h and against h swapped/negated
-        // (operand modifiers of FFMA2: no register moves).  Two sweeps over the tile, so the two FMAs of one accumulator sit 64 instructions apart.
+        // (operand modifiers of FFMA pair: no register moves).  Two sweeps over the tile, so the two FMAs of one accumulator sit 64 instructions apart.
 #pragma unroll
         for (int u = 0; u < FOLD_CT; u++)
 #pragma unroll
@@ -633,7 +631,7 @@ fastddc_fold_kernel(const float2* __restrict__ spectra /*[nblocks][N]*/, const f
 // phasor[pair][k] is written 32 steps at a time through a padded shared tile, so both this kernel's stores and the IFFT kernel's loads are coalesced rows.
 // The IFFT kernel then only multiplies -- every output in parallel instead of one lane per row.
 // (Walking the recursion on the FP64 pipe instead -- bit-identical, 53 >= 2*24 + 2 bits make the double rounding innocuous -- to stay out of the fold kernel's
-// FFMA2 stream was measured slower: 113 us under the fold against 57 us for this form, 9.7 us alone; r02 call 13.)
+// FMA stream was slower under the fold than this form.)
 __global__ void __launch_bounds__(128)
 fastddc_phasor_kernel(const DdcChan* __restrict__ chan, const float* __restrict__ blk_phase, float2* __restrict__ phasor, int channels, int nblocks, int kmax)
 {
@@ -667,8 +665,8 @@ fastddc_phasor_kernel(const DdcChan* __restrict__ chan, const float* __restrict_
 // IFFT_M of the folded (channel, block) rows, /M, drop the scrap, decimate, post shift (the phasors come from fastddc_phasor_kernel; pairs are p = c * nblocks + b).
 // A row is M/8 threads, a CTA is 128 threads = 1024/M rows; the first pass reads the folded row from global memory, the last pass hands every finished element
 // to the sink below, which multiplies by the phasor fetched BEFORE the middle passes and stores: two shared-memory round trips per row, no staging copy, 8 KB of
-// shared memory per CTA.  History (64 ch x 256 blocks, M = 512): a warp per row walking the recursion 113 us; sixteen rows per CTA, a lane per row 58 us; phasors
-// precomputed, flat (row, output) items 54.5 us (three 74 KB CTAs per SM, half of the stall samples on global loads); this form 41.5 us.
+// shared memory per CTA.  Earlier forms (a warp per row walking the recursion; sixteen rows per CTA,
+// a lane per row; flat (row, output) items with precomputed phasors) were slower.
 template <int M>
 struct FastddcPostSink {
     float2* y; float2 ph[8]; int kk[8]; float inv_m;

@@ -5,14 +5,14 @@
 // for C independent channels in one launch (the reference runs one process per channel).
 //
 // Fast path (D % 4 == 2, e.g. 10 and 50; T <= D*M): polyphase register tiling, no tensor cores.
-//   * taps travel as a __grid_constant__ kernel parameter, duplicated (h,h) so that one FFMA2
+//   * taps travel as a __grid_constant__ kernel parameter, duplicated (h,h) so that one FFMA pair
 //     (fma.rn.f32x2) multiplies the I and Q of a sample by the same real tap; ptxas keeps them in
-//     UNIFORM registers (LDCU -> UR operand of FFMA2): no vector registers, no shared-memory traffic.
+//     UNIFORM registers (LDCU -> UR operand of FFMA pair): no vector registers, no shared-memory traffic.
 //   * the input tile is copied global->shared by ONE bulk async copy (cp.async.bulk, SASS UBLKCP)
 //     completing on an mbarrier; the layout in shared memory is the plain stream order.
 //   * a thread owns R consecutive outputs.  Writing tap index k = m*D + p (phase p, sub-tap m), its
 //     outputs need x[(r+m)*D + p]: for one phase that is a contiguous-in-(r+m) window of R+M-1 samples,
-//     each reused by up to min(R,M) FFMA2.  Phases are taken in PAIRS (p, p+1) so every window element
+//     each reused by up to min(R,M) FFMA pair.  Phases are taken in PAIRS (p, p+1) so every window element
 //     is one 128-bit LDS.  With D/2 odd and R odd the lane stride R*D/2 (in 16-byte units) is odd, so
 //     the eight lanes of a quarter-warp hit eight different 16-byte bank groups: conflict-free, no padding.
 //   * the tap range is split in two halves across the two warps of a warp pair (more resident warps per

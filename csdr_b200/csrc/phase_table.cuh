@@ -2,9 +2,9 @@
 //
 // Every NCO block of the reference carries a float phase from call to call:   ph += rate*PI*n;  while (ph > PI) ph -= 2*PI;  ...
 // (libcsdr_gpl.c:48-50, :154-157; libcsdr.c:300-304).  The subtractions round, so the chain ph[k+1] = wrap(fl(ph[k] + inc)) has to be
-// replayed step by step; wrap_phase_pm_pi (common.cuh) does one step bit-exactly in ~1 200 dependent cycles (nine binade levels), and
-// with a few thousand steps per block that serial chain -- not the data path -- set the pace of the shift bank (2.0 of 2.1 ms), of the
-// fused DDC bank's pre-pass (1.8 ms per 2 Mi samples) and of the fastddc inverse bank (0.16 of 0.36 ms) in round 1.
+// replayed step by step; wrap_phase_pm_pi (common.cuh) does one step bit-exactly in about a thousand dependent cycles (nine binade levels),
+// and with a few thousand steps per block that serial chain -- not the data path -- sets the pace of the shift bank, of the fused DDC
+// bank's pre-pass and of the fastddc inverse bank.
 //
 // Observation.  With inc fixed, x = fl(ph + inc) only ever lies in [|inc| - pi, |inc| + pi].  Over such a window the loop is a piecewise
 // translation:  wrap16(a) = a - K(a)  with K a step function of a few dozen pieces, where wrap16 runs the loop until the value drops below
@@ -150,7 +150,7 @@ __device__ __forceinline__ float wrap_after_add(float x, const WrapTable* __rest
 
 #if defined(__CUDACC__) || defined(CSDRB_HOST_EMULATION)
 // ---- one warp per chain: the table lives in registers, a step is two votes and a shuffle ------------------------------------------------
-// Thread-per-channel lookups read 32 different tables per load instruction (32 L1 wavefronts each; measured 1 100 cycles per step).  With a
+// Thread-per-channel lookups read 32 different tables per load instruction (32 L1 wavefronts each).  With a
 // whole warp on ONE chain every lane keeps two thresholds and their K's, the piece index is popc(ballot(a >= thr)), K comes by shuffle:
 // no memory traffic at all inside the chain.  All 32 lanes pass the same x and get the same result.
 struct WrapLanes { float thr0, thr1, lo, hi; double K0, K1; int n; };
@@ -188,8 +188,8 @@ static __device__ __noinline__ float wrap_after_add_warp_generic(float x, const 
     return (__float_as_uint(x) >> 31) ? -a : a;
 }
 
-// The chain kernels' step.  A chain is pure latency, and the r02 SASS of the loop had seven branches per step (>= 16? in the window? more than 32 pieces?
-// the wrap loop's three iterations ...) at ~0.2 us per step; here the common case -- the value inside the table's window or already below 16 -- is
+// The chain kernels' step.  A chain is pure latency, and a looped step has seven branches (>= 16? in the window? more than 32 pieces?
+// the wrap loop's three iterations ...); here the common case -- the value inside the table's window or already below 16 -- is
 // straight-line code: two votes, popc, shuffles, one double subtraction, three predicated subtractions (below 16 at most three are left:
 // 16 - 3*2pi < pi).  Same operations in the same order as the generic form, which takes everything else.
 __device__ __forceinline__ float wrap_after_add_warp(float x, const WrapLanes& w)

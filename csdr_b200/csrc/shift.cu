@@ -41,8 +41,8 @@ constexpr int kChainTableMin = 96;
 
 // chains of nchunks starting phases, one WARP per CHAIN_CPW channels: steps with the full-chunk increment go through the register-resident wrap tables
 // (phase_table.cuh), the last, shorter chunk has its own increment (direct); 32 phases per channel are stored at a time.  `step(slot, ph, len)` is the direct
-// form for slot's channel.  (Four channels per warp were measured: the wrap's branches and votes keep the chains in program order, 526 us per slice of 782
-// chunks against 115 us with a warp per channel -- r02 call 19; the constant stays 1.)
+// form for slot's channel.  (Four channels per warp do not interleave: the wrap's branches and votes keep the chains in program order, so a
+// warp per channel is faster; the constant stays 1.)
 constexpr int CHAIN_CPW = 1;
 constexpr int CHAIN_WARPS = 1;                    // chains per CTA: a chain slice runs next to the main kernel of the previous slice and must fit into what that leaves of an SM (see ddc_bank.cu)
 
@@ -113,8 +113,7 @@ shift_phase_chain_kernel(const float3* __restrict__ params, float* __restrict__ 
 constexpr int SH_TILE = 32;                       // samples per lane per sub-step
 
 // Load `rows` rows of 32 consecutive samples into the padded tile: row r covers stream positions (k0 + r)*seg + t0 .. +31 (zeros past the row's
-// length).  Eight rows' loads are issued before the first shared store -- a load-then-store loop serialises one DRAM/L2 round trip per row
-// (the r01 FFT profile showed exactly that pattern costing 58 % of the stall samples).
+// length).  Eight rows' loads are issued before the first shared store -- a load-then-store loop serialises one DRAM/L2 round trip per row.
 __device__ __forceinline__ void tile_load_rows(float2* __restrict__ tile, const float2* __restrict__ x, int rows, int k0, int seg, int n, int t0, int lane, int pitch)
 {
     for (int r0 = 0; r0 < rows; r0 += 8) {
@@ -131,9 +130,9 @@ __device__ __forceinline__ void tile_load_rows(float2* __restrict__ tile, const 
 }
 constexpr int SH_PITCH = SH_TILE + 1;             // odd pitch in 8-byte units: row-wise walks are conflict-free
 
-// (Two double-buffered forms were measured against this kernel in round 2 -- the tile of step t+1 arriving by 8-byte cp.async while step t is rotated: 32 x 32
-// tiles, 67 KB per CTA, 715 us for 64 x 2.4 M; 32 x 16 tiles in the same shared memory as here with the rotation in registers, 740 us -- against 616 us for this
-// plain load / rotate / store form with its 24 resident warps per SM.  profiles/r02_shift_bank_*_ncu_summary.json.)
+// (Two double-buffered forms were slower than this kernel -- the tile of step t+1 arriving by 8-byte cp.async while step t is rotated: 32 x 32
+// tiles, 67 KB per CTA; 32 x 16 tiles in the same shared memory as here with the rotation in registers -- against this
+// plain load / rotate / store form with its 24 resident warps per SM.)
 __global__ void __launch_bounds__(128)
 shift_bank_kernel(const float2* __restrict__ in, long in_stride, float2* __restrict__ out, long out_stride,
                   const float3* __restrict__ params, const float* __restrict__ chunk_phase, int n, int chunk, int nchunks, int k_first, int k_end)
@@ -501,9 +500,9 @@ int launch_shift_addition_bank(const float2* d_in, long in_stride, float2* d_out
     const float3* prm = reinterpret_cast<const float3*>(d_params);
     WrapTable* tables = chain_tables(d_scratch, scratch_bytes, channels, nchunks);
     constexpr size_t smem = 0;                                          // the tiles are static shared memory
-    // The chain is one warp per channel and sequential (150 ns per chunk): a long one is cut into up to three slices that run on a side stream, the main
-    // kernel follows slice by slice on the caller's stream.  A slice must still fill the machine (a warp walks its 32 chunks tile after tile, ~3 us per tile:
-    // eight slices of 384 chunks x 64 channels ran the main kernel at 0.43 waves and gained nothing; r02 call 14).  CSDRB_SHIFT_SLICES=1: one stream.
+    // The chain is one warp per channel and sequential: a long one is cut into up to three slices that run on a side stream, the main
+    // kernel follows slice by slice on the caller's stream.  A slice must still fill the machine (a warp walks its 32 chunks tile after tile:
+    // eight slices of 384 chunks x 64 channels run the main kernel at under half a wave and gain nothing).  CSDRB_SHIFT_SLICES=1: one stream.
     static const int max_slices = getenv("CSDRB_SHIFT_SLICES") ? atoi(getenv("CSDRB_SHIFT_SLICES")) : 3;
     static const long slice_min = getenv("CSDRB_SHIFT_SLICE_MIN") ? atol(getenv("CSDRB_SHIFT_SLICE_MIN")) : 768L * 64;   // chunk-channels a slice needs to fill the machine (the CPU tier lowers it)
     int slices = (int)(((long)nchunks * channels) / (slice_min > 0 ? slice_min : 1));

@@ -24,8 +24,8 @@ static SideStream* side_stream()
               cudaEventCreateWithFlags(&s->join, cudaEventDisableTiming) == cudaSuccess;
     for (int i = 0; i < kSideSlices && ok; i++) ok = cudaEventCreateWithFlags(&s->slice[i], cudaEventDisableTiming) == cudaSuccess;
     if (!ok) { set_error("side stream: CUDA object creation failed"); delete s; return nullptr; }
-    // stream-ordered scratch (cudaMallocAsync) must not go back to the OS at every synchronisation: keep the pool's memory (r02: re-mapping 67 MB per
-    // fastddc call cost more than the kernels)
+    // stream-ordered scratch (cudaMallocAsync) must not go back to the OS at every synchronisation: keep the pool's memory (re-mapping the fastddc
+    // scratch at every call costs more than the kernels)
     cudaMemPool_t pool = nullptr;
     if (cudaDeviceGetDefaultMemPool(&pool, dev) == cudaSuccess) { unsigned long long keep = ~0ULL; cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &keep); }
     per_dev[dev] = s;

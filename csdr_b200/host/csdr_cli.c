@@ -737,7 +737,7 @@ static const struct { const char *name; int (*run)(int, char **); const char *sy
 
 static int usage(void)
 {
-    fprintf(stderr, "csdr (B200 hot-path build) - DSP blocks on stdin/stdout, computed by libcsdr_b200 on a CUDA device\nusage:\n");
+    fprintf(stderr, "csdr (H100 hot-path build) - DSP blocks on stdin/stdout, computed by libcsdr_b200 on a CUDA device\nusage:\n");
     for (size_t k = 0; k < sizeof kCommands / sizeof kCommands[0]; k++) fprintf(stderr, "    csdr %s\n", kCommands[k].syntax);
     fprintf(stderr, "commands of the reference CLI outside this list are not part of this build\n");
     return -1;

@@ -1,5 +1,5 @@
 /*
- * csdr_b200.h -- public C ABI of libcsdr_b200.so (B200 / sm_100a implementation of the csdr block-DSP hot path).
+ * csdr_b200.h -- public C ABI of libcsdr_b200.so (H100 / sm_90a implementation of the csdr block-DSP hot path).
  *
  * Two layers, both plain C (System V x86-64, no C++ or torch types in any signature):
  *

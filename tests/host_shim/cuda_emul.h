@@ -7,7 +7,7 @@
 // arrived); the order in which fibers run between barriers alternates / reverses / is shuffled (CUDA_EMUL_ORDER) so that a missing
 // barrier shows as a wrong result; threadIdx/blockIdx/blockDim/gridDim are per-fiber values; dynamic shared memory is one buffer per CTA
 // pre-filled with a NaN pattern; IEEE single-precision intrinsics map onto the same operations (fmaf is a true FMA on the host too);
-// __shfl_xor_sync goes through a per-warp exchange; the inline-PTX helpers of csrc/common.cuh have C++ models here (FFMA2 = two FMAs,
+// __shfl_xor_sync goes through a per-warp exchange; the inline-PTX helpers of csrc/common.cuh have C++ models here (ffma2 = two FMAs,
 // cp.async.bulk = alignment-checked memcpy that completes an mbarrier, st.global.L1::no_allocate = alignment-checked store); launch
 // configurations the hardware would refuse (gridDim.y/z > 65535, > 1024 threads, > 227 KB shared) fail like they would on the GPU.
 // Not modelled: the memory model (fibers switch only at barriers, so a race that needs true concurrency can go unnoticed), occupancy and
@@ -113,7 +113,7 @@ template <typename K, typename... A>
 void launch(dim3 grid, dim3 block, size_t smem_bytes, K kernel, A... args)
 {
     State& s = st();
-    // what cudaLaunchKernel would refuse on sm_100 (cudaErrorInvalidConfiguration / invalid value): recorded for cudaGetLastError()
+    // what cudaLaunchKernel would refuse on sm_90 (cudaErrorInvalidConfiguration / invalid value): recorded for cudaGetLastError()
     if (grid.x == 0 || grid.y == 0 || grid.z == 0 || grid.y > 65535u || grid.z > 65535u || grid.x > 2147483647u || block.x * block.y * block.z == 0 ||
         block.x * block.y * block.z > 1024u || block.x > 1024u || block.y > 1024u || block.z > 64u || smem_bytes > 227u * 1024u) {
         s.launch_error = true;
@@ -263,7 +263,7 @@ static inline int __popc(unsigned v) { return __builtin_popcount(v); }
 
 // ---- C++ models of the inline-PTX helpers of csdr_b200/csrc/common.cuh (which steps aside under CSDRB_HOST_EMULATION) ------------
 namespace csdrb {
-static inline float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }     // two IEEE FMAs, like FFMA2
+static inline float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }     // two IEEE FMAs
 static inline float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 static inline float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 static inline float2 fsub2(float2 a, float2 b) { return make_float2(__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y)); }

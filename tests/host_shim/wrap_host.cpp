@@ -11,6 +11,7 @@ static inline unsigned __float_as_uint(float f) { unsigned u; std::memcpy(&u, &f
 static inline float __fsub_rn(float a, float b) { volatile float r = a - b; return r; }
 static inline float __fadd_rn(float a, float b) { volatile float r = a + b; return r; }
 static inline float __fmul_rn(float a, float b) { volatile float r = a * b; return r; }
+static inline float __fmaf_rn(float a, float b, float c) { return std::fmaf(a, b, c); }
 static inline size_t __cvta_generic_to_shared(const void*) { return 0; }
 static inline int __float2int_rz(float f) { return (int)f; }
 static inline float __int_as_float(int i) { float f; std::memcpy(&f, &i, 4); return f; }

@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on the B200 box): the CUDA path, called through the C ABI of
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called through the C ABI of
 libcsdr_b200.so, against the CPU oracle (oracle/liboracle.so), the committed golden vectors and -- when
 present as a prebuilt binary -- the compiled reference itself (oracle/_ref/libcsdr_ref.so).
 

@@ -1,4 +1,4 @@
-"""GPU parity tests added in round 2 (run with -m gpu on the B200 box), all through the C ABI of libcsdr_b200.so:
+"""GPU parity tests added in round 2 (run with -m gpu on an H100), all through the C ABI of libcsdr_b200.so:
   * the u8 front end fused into the FIR bank (convert_u8_f | fir_decimate_cc, csdr-fm:41), device and host (end-to-end) calls;
   * the table-driven phase chains (csrc/phase_table.cuh): long chains, every rate class, bit-exact carried phases vs the oracle's loops;
   * the fold-based fastddc inverse bank on ragged channel / block counts, against the round-1 kernels and the oracle;

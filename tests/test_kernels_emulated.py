@@ -348,7 +348,7 @@ def test_nfm_deemphasis_fir_and_fused_limiter(audio, oracle, rate):
 @pytest.mark.parametrize("D,T,n,variant", [(10, 199, 9_999, -1), (10, 199, 30_011, 0), (10, 199, 30_011, 3), (10, 199, 4_000, 7), (10, 79, 20_000, -1),
                                            (50, 801, 70_000, -1), (7, 79, 5_001, -1), (10, 199, 199, -1), (10, 199, 208, -1), (10, 199, 150, -1)])
 def test_k3_fir_decimate_bank(fir, oracle, D, T, n, variant):
-    """bulk-copy tile loads on an mbarrier, polyphase register tiling, FFMA2, pair reduction through named barriers, streaming stores --
+    """bulk-copy tile loads on an mbarrier, polyphase register tiling, FMA pairs, pair reduction through named barriers, streaming stores --
     executed on the host against the oracle; n == T, n < T and ragged ends included."""
     rng = np.random.default_rng(D * 1000 + T + n)
     ch = 3

@@ -1,4 +1,4 @@
-"""Throughput of the non-headline BASELINE configs and of the standalone streaming kernels on one B200 (device-resident data).
+"""Throughput of the non-headline BASELINE configs and of the standalone streaming kernels on one H100 (device-resident data).
 Prints one line per measurement and writes gpurun_out/configs.json.  Parity for all of these is in tests/ (-m gpu)."""
 import json, os, sys, time
 from pathlib import Path
@@ -6,7 +6,7 @@ import numpy as np, torch
 sys.path.insert(0, str(Path(__file__).resolve().parents[1]))
 import csdr_b200 as cb
 
-PEAK = json.loads(Path("MEASURED_PEAKS.json").read_text())["hbm_gbs"] if Path("MEASURED_PEAKS.json").exists() else 6650.0
+PEAK = json.loads(Path("MEASURED_PEAKS.json").read_text())["hbm_gbs"] if Path("MEASURED_PEAKS.json").exists() else 3350.0
 res = {}
 
 

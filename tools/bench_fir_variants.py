@@ -11,7 +11,7 @@ taps = csdr_b200.firdes_lowpass_f(T, 0.5 / D)
 x = torch.rand((C, N, 2), device="cuda") * 2 - 1
 n_out = csdr_b200.fir_out_len(N, D, T)
 out = torch.empty((C, n_out + (n_out & 1)), dtype=torch.complex64, device="cuda")
-peaks = json.loads(Path("MEASURED_PEAKS.json").read_text()) if Path("MEASURED_PEAKS.json").exists() else {"hbm_gbs": 6650.0}
+peaks = json.loads(Path("MEASURED_PEAKS.json").read_text()) if Path("MEASURED_PEAKS.json").exists() else {"hbm_gbs": 3350.0}
 res = {}
 nv = csdr_b200.lib().csdrb_fir_bank_variants()
 for v in range(nv):
