@@ -2,14 +2,14 @@
 //     shift_addition_cc(rate_c)  ->  fir_decimate_cc(D, taps)  ->  [fmdemod_quadri_cf]        for C channels of ONE wideband stream
 // i.e. what ddcd_old.h:51-57 runs as one `csdr shift_addition_cc --fd N | csdr fir_decimate_cc D bw` process chain per client.
 //
-// Mapping: LANE = CHANNEL.  All 32 lanes of a warp walk the same wideband samples in the same order, so
+// Mapping: LANE = CHANNELS.  All 32 lanes of a warp walk the same wideband samples in the same order, so
 //   * the wideband sample is one broadcast load per warp (shared input: 8 B per sample, L1/L2 resident),
-//   * the FIR tap for sample n and output o is the same for every lane -> taps live in uniform registers
-//     (kernel parameter, duplicated (h,h) for FFMA pair), exactly like the independent-input bank kernel,
-//   * each lane keeps its own NCO phasor (the reference's float recursion, re-seeded at every chunk boundary from the
-//     replayed float phase chain) and its own M = ceil(T/D) running output accumulators in registers.
-// Per wideband sample and channel: 4 flop rotation + 6 flop recursion + 2*M FFMA pair lanes; nothing goes through shared memory,
-// the shifted stream never exists in HBM (the unfused chain writes and re-reads 8*C bytes per wideband sample).
+//   * the FIR tap for sample n and output o is the same for every lane -> the CTA copies the taps into shared memory once and
+//     a warp reads them with broadcast loads,
+//   * each lane carries kDdcChannelsPerLane channels, each with its own NCO phasor (the reference's float recursion, re-seeded at
+//     every chunk boundary from the replayed float phase chain) and its own M = ceil(T/D) running output accumulators in registers.
+// Per wideband sample and channel: 4 flop rotation + 6 flop recursion + 2*M FFMA pair lanes; the shifted stream never exists in HBM
+// (the unfused chain writes and re-reads 8*C bytes per wideband sample).
 // A warp owns a time segment of SEG outputs (plus M-1 trailing periods to finish its last outputs); segments are independent
 // because the phasor of any sample depends only on its chunk's seed and its position inside the chunk.
 //
@@ -28,7 +28,7 @@
 namespace csdrb {
 
 template <int TPAD>
-struct alignas(16) DdcTaps { float4 hh2[TPAD / 2]; };               // rows of MP = M rounded up to even; one float4 = taps (j, j+1), each duplicated (h,h)
+struct alignas(16) DdcTaps { float2 h2[TPAD / 2]; };                // [p][j / 2] = taps (j, j+1) of phase p; rows of MP = M rounded up to even
 
 #define FMDEMOD_K_D 0.340447550238101026565118445432744920253753662109375
 
@@ -61,9 +61,8 @@ ddc_wrap_tables_kernel(const float3* __restrict__ params, int chunk, WrapTable* 
     if (c < channels && threadIdx.x == 0) wrap_table_build(__fmul_rn(__fmul_rn(params[c].z, 3.14159265358979323846f), (float)chunk), tables + c);
 }
 
-// One warp walks DDC_CHAIN_CPW channels (1: more than one per warp does not interleave -- the wrap's branches and votes keep the chains in program order,
+// One warp walks one channel (more than one per warp does not interleave -- the wrap's branches and votes keep the chains in program order,
 // as on the fastddc and shift chains).
-constexpr int DDC_CHAIN_CPW = 1;
 constexpr int DDC_CHAIN_WARPS = 1;                 // chains per CTA.  The pre-pass of block k+1 runs NEXT TO block k's main kernel, whose three CTAs leave ~10 K registers per SM: a one-warp
                                                    // CTA slips in, an eight-warp CTA has to wait for an SM to drain and the pre-pass serialises behind the main kernel
 
@@ -71,47 +70,24 @@ __global__ void __launch_bounds__(32 * DDC_CHAIN_WARPS)
 ddc_phase_chain_kernel(const float3* __restrict__ params, float* __restrict__ phase_io, float* __restrict__ chunk_phase,
                        int channels, int nchunks, int chunk, int next_chunk, const WrapTable* __restrict__ tables)
 {
-    const int c0 = (blockIdx.x * DDC_CHAIN_WARPS + (threadIdx.x >> 5)) * DDC_CHAIN_CPW, lane = threadIdx.x & 31;
-    if (c0 >= channels) return;
-    const int nc = min(DDC_CHAIN_CPW, channels - c0);
-    float inc[DDC_CHAIN_CPW], ph[DDC_CHAIN_CPW], keep[DDC_CHAIN_CPW], mine[DDC_CHAIN_CPW];
-    WrapLanes w[DDC_CHAIN_CPW];
-#pragma unroll
-    for (int i = 0; i < DDC_CHAIN_CPW; i++) {
-        const int c = min(c0 + i, channels - 1);                        // slots past the bank shadow its last channel (they compute, they do not store)
-        inc[i] = __fmul_rn(__fmul_rn(params[c].z, 3.14159265358979323846f), (float)chunk);
-        w[i] = wrap_lanes_load(tables + c, lane);
-        ph[i] = phase_io[c]; keep[i] = ph[i]; mine[i] = 0.f;
-    }
-    __syncwarp();                                      // every lane has read the carried phases before lane 0 overwrites them
+    const int c = blockIdx.x * DDC_CHAIN_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (c >= channels) return;
+    const float inc = __fmul_rn(__fmul_rn(params[c].z, 3.14159265358979323846f), (float)chunk);
+    const WrapLanes w = wrap_lanes_load(tables + c, lane);
+    float ph = phase_io[c], keep = ph, mine = 0.f;
+    __syncwarp();                                      // every lane has read the carried phase before lane 0 overwrites it
     for (int k = 0; k < nchunks; k++) {
-        if ((k & 31) == lane) {
-#pragma unroll
-            for (int i = 0; i < DDC_CHAIN_CPW; i++) mine[i] = ph[i];
-        }
-        if (((k & 31) == 31 || k == nchunks - 1) && (k & ~31) + lane <= k) {                             // one coalesced store per channel and 32 steps
-#pragma unroll
-            for (int i = 0; i < DDC_CHAIN_CPW; i++) if (i < nc) chunk_phase[(long)(c0 + i) * nchunks + (k & ~31) + lane] = mine[i];
-        }
-        if (k == next_chunk) {
-#pragma unroll
-            for (int i = 0; i < DDC_CHAIN_CPW; i++) keep[i] = ph[i];
-        }
-#pragma unroll
-        for (int i = 0; i < DDC_CHAIN_CPW; i++) ph[i] = wrap_after_add_warp(__fadd_rn(ph[i], inc[i]), w[i]);
+        if ((k & 31) == lane) mine = ph;
+        if (((k & 31) == 31 || k == nchunks - 1) && (k & ~31) + lane <= k)                               // one coalesced store per 32 steps
+            chunk_phase[(long)c * nchunks + (k & ~31) + lane] = mine;
+        if (k == next_chunk) keep = ph;
+        ph = wrap_after_add_warp(__fadd_rn(ph, inc), w);
     }
     if (next_chunk >= nchunks) {                       // the next block starts beyond the chunks this block touched
-        for (int k = nchunks; k < next_chunk; k++) {
-#pragma unroll
-            for (int i = 0; i < DDC_CHAIN_CPW; i++) ph[i] = wrap_after_add_warp(__fadd_rn(ph[i], inc[i]), w[i]);
-        }
-#pragma unroll
-        for (int i = 0; i < DDC_CHAIN_CPW; i++) keep[i] = ph[i];
+        for (int k = nchunks; k < next_chunk; k++) ph = wrap_after_add_warp(__fadd_rn(ph, inc), w);
+        keep = ph;
     }
-    if (lane == 0) {
-#pragma unroll
-        for (int i = 0; i < DDC_CHAIN_CPW; i++) if (i < nc) phase_io[c0 + i] = keep[i];
-    }
+    if (lane == 0) phase_io[c] = keep;
 }
 
 // retune support: close the current chunk `n` samples in (every channel advances by n samples at its present rate), see csdrb_ddc_bank_process
@@ -121,135 +97,26 @@ __global__ void ddc_rechunk_kernel(const float3* __restrict__ params, float* __r
     if (c < channels) phase_io[c] = wrap_phase_pm_pi(__fadd_rn(phase_io[c], __fmul_rn(__fmul_rn(params[c].z, 3.14159265358979323846f), (float)n)));
 }
 
-// CPL = channels per lane.  A tap pair is loaded once per warp and sample phase (LDCU.128 fetches two of them: taps are stored
-// [p][j] so the M taps that one sample meets are contiguous); with CPL = 2 every loaded tap feeds the FMAs of two channels and every
-// wideband sample load feeds two channels, which halves the non-FMA issue slots per channel-sample (at CPL = 1 there is about one tap load per FMA pair).
-template <int D, int M, int CPL, bool DEMOD>
-__global__ void __launch_bounds__(128)
-ddc_bank_fused_kernel(const float2* __restrict__ wide, int n_in, int offset, int chunk, int nchunks,
-                      const float3* __restrict__ params, const float2* __restrict__ seeds, int channels,
-                      void* __restrict__ out_v, long out_stride, int n_out, int seg_outputs,
-                      const float2* __restrict__ last_in, float2* __restrict__ last_out,
-                      const __grid_constant__ DdcTaps<D * ((M + 1) & ~1)> taps)
-{
-    constexpr int MP = (M + 1) & ~1;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int ch0 = (blockIdx.y * 4 + warp) * (32 * CPL) + lane;        // this lane's channels: ch0 + 32*u
-    if (ch0 - lane >= channels) return;                                 // whole warp beyond the bank
-    const int o_first = blockIdx.x * seg_outputs;                       // first output this warp emits
-    if (o_first >= n_out) return;
-    const int o_end = min(n_out, o_first + seg_outputs);
-    // an output's window starts at its own first sample, so the walk can begin right at o_first (outputs before it are the
-    // partial ones and are simply not emitted); the demodulator needs the previous baseband sample: start one output early.
-    int o_start = o_first - (DEMOD ? 1 : 0);
-    if (o_start < 0) o_start = 0;
-    int chs[CPL]; bool live[CPL];
-    float sind[CPL], cosd[CPL], c[CPL], s[CPL];
-    float2 acc[CPL][M], prev[CPL];
-    long n = (long)o_start * D;                                         // absolute chunk position = offset + n
-    int kchunk = (int)((offset + n) / chunk);
-    const int into = (int)((offset + n) % chunk);                       // samples already consumed in this chunk
-#pragma unroll
-    for (int u = 0; u < CPL; u++) {
-        live[u] = ch0 + 32 * u < channels;
-        chs[u] = live[u] ? ch0 + 32 * u : channels - 1;                 // dead lanes shadow a real channel (no divergence), never store
-        const float3 p = params[chs[u]];
-        sind[u] = p.x; cosd[u] = p.y;
-#pragma unroll
-        for (int j = 0; j < M; j++) acc[u][j] = make_float2(0.f, 0.f);
-        prev[u] = (DEMOD && last_in) ? last_in[chs[u]] : make_float2(0.f, 0.f);
-        const float2 cs = seeds[(long)chs[u] * nchunks + kchunk];
-        c[u] = cs.x; s[u] = cs.y;
-    }
-    for (int t = 0; t < into; t++) {                                    // replay the recursion up to the segment start (< chunk steps, no data)
-#pragma unroll
-        for (int u = 0; u < CPL; u++) {
-            const float cn = __fsub_rn(__fmul_rn(c[u], cosd[u]), __fmul_rn(s[u], sind[u]));
-            const float sn = __fadd_rn(__fmul_rn(s[u], cosd[u]), __fmul_rn(c[u], sind[u]));
-            c[u] = cn; s[u] = sn;
-        }
-    }
-    int left = chunk - into;
-    // acc[.][j] collects output q-j while the walk is in period q (samples qD .. qD+D-1): sample qD+p meets tap p + jD.
-    for (int q = o_start; q < o_end + M - 1; q++) {
-        const long base = (long)q * D;
-        const bool inside = base + D <= n_in;                           // whole period inside the block: no per-load checks
-        const float4* src = reinterpret_cast<const float4*>(wide + base);   // D even, base even: 16-byte aligned
-#pragma unroll
-        for (int pp = 0; pp < D; pp += 2) {
-            float4 xx;                                                  // two wideband samples per 128-bit broadcast load
-            if (inside) xx = __ldg(src + pp / 2);
-            else {                                                      // samples past n_in only ever meet zero-padded taps: read as zeros
-                const float2 a = base + pp < n_in ? wide[base + pp] : make_float2(0.f, 0.f);
-                const float2 b = base + pp + 1 < n_in ? wide[base + pp + 1] : make_float2(0.f, 0.f);
-                xx = make_float4(a.x, a.y, b.x, b.y);
-            }
-#pragma unroll
-            for (int e = 0; e < 2; e++) {
-                const int pidx = pp + e;
-                const float xi = e ? xx.z : xx.x, xq = e ? xx.w : xx.y;
-                if (left == 0) {                                        // chunk boundary: re-seed the phasors (warp-uniform branch)
-                    if (kchunk < nchunks - 1) kchunk++;                 // (beyond the block the data are zeros; any phasor will do)
-#pragma unroll
-                    for (int u = 0; u < CPL; u++) { const float2 cs = seeds[(long)chs[u] * nchunks + kchunk]; c[u] = cs.x; s[u] = cs.y; }
-                    left = chunk;
-                }
-                left--;
-                float2 sh[CPL];
-#pragma unroll
-                for (int u = 0; u < CPL; u++) {
-                    sh[u] = make_float2(fmaf(c[u], xi, -s[u] * xq), fmaf(s[u], xi, c[u] * xq));
-                    const float cn = __fsub_rn(__fmul_rn(c[u], cosd[u]), __fmul_rn(s[u], sind[u]));
-                    const float sn = __fadd_rn(__fmul_rn(s[u], cosd[u]), __fmul_rn(c[u], sind[u]));
-                    c[u] = cn; s[u] = sn;
-                }
-#pragma unroll
-                for (int j = 0; j < M; j += 2) {
-                    const float4 h2 = taps.hh2[(pidx * MP + j) / 2];    // [p][j] layout, one 128-bit uniform load = two taps
-#pragma unroll
-                    for (int u = 0; u < CPL; u++) {
-                        acc[u][j] = ffma2(sh[u], make_float2(h2.x, h2.y), acc[u][j]);
-                        if (j + 1 < M) acc[u][j + 1] = ffma2(sh[u], make_float2(h2.z, h2.w), acc[u][j + 1]);
-                    }
-                }
-            }
-        }
-        // period q done: output q-(M-1) is complete (its last tap block was j = M-1)
-        const int o = q - (M - 1);
-#pragma unroll
-        for (int u = 0; u < CPL; u++) {
-            const float2 y = acc[u][M - 1];
-#pragma unroll
-            for (int j = M - 1; j > 0; j--) acc[u][j] = acc[u][j - 1];
-            acc[u][0] = make_float2(0.f, 0.f);
-            if (o >= o_start) {
-                if (DEMOD) {
-                    if (o >= o_first && live[u]) static_cast<float*>(out_v)[(long)chs[u] * out_stride + o] = quadri_d(y, prev[u]);
-                    prev[u] = y;
-                    if (last_out && live[u] && o == n_out - 1) last_out[chs[u]] = y;
-                } else if (o >= o_first && live[u]) {
-                    static_cast<float2*>(out_v)[(long)chs[u] * out_stride + o] = y;
-                }
-            }
-        }
-    }
-}
-
-
-// ---- v2 (round 2): taps in shared memory, packed phasor arithmetic, ramp-aware tap ranges ---------------------------------------
-// What the round-1 ncu profile of the kernel above showed: FMA pipe 29 %, issue 45 % -- neither saturated.  Three structural costs:
-//  (1) every tap pair was an LDCU from a 7.2 KB kernel parameter walked once per period: far more than the uniform/constant L0 holds, so the
-//      FFMA pair stream waited on constant-cache refills.  Here the CTA copies the taps once into shared memory ((h,h) pairs, [p][j] layout) and a
-//      warp fetches two taps with one broadcast LDS.128 (one wavefront, 29-cycle fixed latency the compiler pipelines).
-//  (2) rotation and recursion cost 10 scalar FMA-pipe slots per (sample, channel).  With the phasor kept twice, P = (c, s) and Q = (-s, c),
+// ---- the bank kernel: taps in shared memory, packed phasor arithmetic, ramp-aware tap ranges ---------------------------------------
+//  (1) The taps (7.2 KB at D = 50) are walked once per period: far more than the uniform/constant cache holds, so read from a kernel parameter the
+//      FFMA pair stream would wait on constant-cache refills.  The CTA copies them once into shared memory ([p][j] layout) and a warp fetches
+//      several taps with one broadcast shared load.
+//  (2) With the phasor kept twice, P = (c, s) and Q = (-s, c), rotation and recursion are packed operations:
 //          shifted = x.i * P + x.q * Q                        (FMUL pair + FFMA pair -- libcsdr_gpl.c:39-40 up to one fused product)
 //          P'      = cosd * P + sind * Q                      (FMUL pair, FMUL pair, FADD, FADD: the reference's two rounded products and their sum, :42-45)
 //          Q'      = (-P'.y, P'.x)                            (operand swizzle / negate modifiers of the packed instructions: free)
-//      it is 6 slots; the phasor state stays bit-identical to the scalar sequence (negation commutes with rounding).
-//  (3) a warp's time segment spends M-1 periods filling and M-1 periods draining its accumulators; with ~40-output segments that was a third of
-//      all FFMA pair.  Here the head and tail periods only touch the accumulators that belong to emitted outputs, in groups of four taps
-//      (template <JLO, JHI>), which removes ~80 % of that waste.
+//      and the phasor state stays bit-identical to the scalar sequence (negation commutes with rounding).
+//  (3) A warp's time segment spends M-1 periods filling and M-1 periods draining its accumulators; with ~40-output segments a full-width walk
+//      would spend a third of all FFMA pair there.  The head and tail periods only touch the accumulators that belong to emitted outputs, in
+//      groups of four taps (template <JLO, JHI>), which removes ~80 % of that waste.
 // Work decomposition: warp-granular 1-D grid; warp w owns (segment, channel set) = (w / sets, w % sets), a channel set = 32*CPL channels.
+// CPL = channels per lane: with two, every loaded tap and every wideband sample feeds the FMAs of two channels, which halves the non-FMA issue
+// slots per channel-sample against one channel per lane.  CSDRB_DDC_CPL=1 selects one channel per lane (DESIGN.md 8b: faster on an H100).
+constexpr int kDdcChannelsPerLane = 2;
+// Resident warps per SM the launcher sizes its segments for: three 4-warp CTAs at the ~165 registers per thread of the D = 50 and D = 10 / 20-tap
+// kernels.  Fewer, longer segments would leave SMs idle; more, shorter ones spend a larger share on the M-1 trailing periods of each.
+constexpr int kDdcWarpsPerSm = 12;
+
 template <int D, int M, int CPL, bool DEMOD>
 struct DdcWalk {
     static constexpr int MP = (M + 1) & ~1;
@@ -269,7 +136,7 @@ struct DdcWalk {
         P[u] = pn;
         Q[u] = make_float2(__uint_as_float(__float_as_uint(pn.y) ^ 0x80000000u), pn.x);
     }
-    // one wideband sample against the taps of its phase p (tp = taps of phase p, MP/2 float4), accumulators JLO..JHI-1 only
+    // one wideband sample against the taps of its phase p (tp = taps of phase p, MP/2 float2), accumulators JLO..JHI-1 only
     // The taps come as SCALARS (two per 64-bit shared load) and multiply the I and the Q lane of the shifted sample: the tap operand is one register
     // for both channels of the lane, and four taps come with one 128-bit shared load (a copy duplicated (h, h) in shared memory needs twice the loads).
     template <int JLO, int JHI>
@@ -305,7 +172,7 @@ ddc_bank_fused2_kernel(const float2* __restrict__ wide, int n_in, int offset, in
     constexpr int MP = (M + 1) & ~1;
     constexpr int U = (D % 10 == 0) ? 10 : 2;                           // samples per unchecked group
     __shared__ float2 staps[D * MP / 2];                               // [p][j / 2] = taps (j, j+1) of phase p
-    for (int i = threadIdx.x; i < D * MP / 2; i += 128) { const float4 hh = taps.hh2[i]; staps[i] = make_float2(hh.x, hh.z); }
+    for (int i = threadIdx.x; i < D * MP / 2; i += 128) staps[i] = taps.h2[i];
     __syncthreads();
     const int lane = threadIdx.x & 31;
     const long wid = (long)blockIdx.x * 4 + (threadIdx.x >> 5);
@@ -448,39 +315,24 @@ static int launch_fused(const float2* wide, int n_in, int offset, int chunk, int
                         int demod, void* out, long out_stride, int n_out, const float2* last_in, float2* last_out, const float* h_taps, int T, cudaStream_t st)
 {
     constexpr int MP = (M + 1) & ~1;
-    DdcTaps<D * MP> tp;                                                 // tap k = jD + p stored at [p][j], duplicated for FFMA pair
+    DdcTaps<D * MP> tp;                                                 // tap k = jD + p stored at [p][j]
     for (int p = 0; p < D; p++)
         for (int j = 0; j < MP; j++) {
             const int k = j * D + p; const float h = (j < M && k < T) ? h_taps[k] : 0.f;
-            float4& slot = tp.hh2[(p * MP + j) / 2];
-            if (j & 1) { slot.z = h; slot.w = h; } else { slot.x = h; slot.y = h; }
+            float2& slot = tp.h2[(p * MP + j) / 2];
+            if (j & 1) slot.y = h; else slot.x = h;
         }
-    // tuning knobs: kernel generation (2 = shared-memory taps / packed phasor / ramp-aware, 1 = the round-1 kernel kept for A/B runs),
-    // channels per lane and resident-warp target per SM
-    static const int ver_env = getenv("CSDRB_DDC_V") ? atoi(getenv("CSDRB_DDC_V")) : 2;
-    static const int cpl_env = getenv("CSDRB_DDC_CPL") ? atoi(getenv("CSDRB_DDC_CPL")) : (ver_env == 1 ? 1 : 2);
-    static const int wps_env = getenv("CSDRB_DDC_WPS") ? atoi(getenv("CSDRB_DDC_WPS")) : (ver_env == 1 ? 24 : 12);
-    const int cpl = cpl_env == 2 ? 2 : 1;
+    static const int cpl = getenv("CSDRB_DDC_CPL") && atoi(getenv("CSDRB_DDC_CPL")) != kDdcChannelsPerLane ? 1 : kDdcChannelsPerLane;
     const int warps_per_seg = (channels + 32 * cpl - 1) / (32 * cpl);
     // enough warps to fill the machine while keeping the M-1 trailing periods of every segment a small fraction
-    long want_segments = (kSmCount * wps_env + warps_per_seg - 1) / warps_per_seg;
+    long want_segments = (kSmCount * kDdcWarpsPerSm + warps_per_seg - 1) / warps_per_seg;
     int seg = (int)((n_out + want_segments - 1) / want_segments);
     if (seg < 2 * M) seg = 2 * M;
     const int nsegs = (n_out + seg - 1) / seg;
-    if (ver_env != 1) {
-        const long warps = (long)nsegs * warps_per_seg;
-        const unsigned ctas = (unsigned)((warps + 3) / 4);
-#define CSDRB_DDC_LAUNCH2(CPLV, DM) ddc_bank_fused2_kernel<D, M, CPLV, DM><<<ctas, 128, 0, st>>>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, warps_per_seg, out, out_stride, n_out, seg, nsegs, last_in, last_out, tp)
-        if (cpl == 2) { if (demod) CSDRB_DDC_LAUNCH2(2, true); else CSDRB_DDC_LAUNCH2(2, false); }
-        else { if (demod) CSDRB_DDC_LAUNCH2(1, true); else CSDRB_DDC_LAUNCH2(1, false); }
-#undef CSDRB_DDC_LAUNCH2
-        CSDRB_CUDA(cudaGetLastError());
-        return 0;
-    }
-    const int groups = (warps_per_seg + 3) / 4;
-    dim3 grid(nsegs, groups);
-#define CSDRB_DDC_LAUNCH(CPLV, DM) ddc_bank_fused_kernel<D, M, CPLV, DM><<<grid, 128, 0, st>>>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, out, out_stride, n_out, seg, last_in, last_out, tp)
-    if (cpl == 2) { if (demod) CSDRB_DDC_LAUNCH(2, true); else CSDRB_DDC_LAUNCH(2, false); }
+    const long warps = (long)nsegs * warps_per_seg;
+    const unsigned ctas = (unsigned)((warps + 3) / 4);
+#define CSDRB_DDC_LAUNCH(CPLV, DM) ddc_bank_fused2_kernel<D, M, CPLV, DM><<<ctas, 128, 0, st>>>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, warps_per_seg, out, out_stride, n_out, seg, nsegs, last_in, last_out, tp)
+    if (cpl == kDdcChannelsPerLane) { if (demod) CSDRB_DDC_LAUNCH(kDdcChannelsPerLane, true); else CSDRB_DDC_LAUNCH(kDdcChannelsPerLane, false); }
     else { if (demod) CSDRB_DDC_LAUNCH(1, true); else CSDRB_DDC_LAUNCH(1, false); }
 #undef CSDRB_DDC_LAUNCH
     CSDRB_CUDA(cudaGetLastError());
@@ -509,7 +361,7 @@ int launch_ddc_prepass(int input_size, int channels, const float* d_params, floa
     }
     const long advance = (long)n_out * decimation;                      // the next block starts here (the caller re-presents the tail)
     const int next_chunk = (int)((offset + advance) / chunk);
-    ddc_phase_chain_kernel<<<(channels + DDC_CHAIN_CPW * DDC_CHAIN_WARPS - 1) / (DDC_CHAIN_CPW * DDC_CHAIN_WARPS), 32 * DDC_CHAIN_WARPS, 0, st>>>(reinterpret_cast<const float3*>(d_params), d_phase_io, chunk_phase, channels, nchunks, chunk, next_chunk,
+    ddc_phase_chain_kernel<<<(channels + DDC_CHAIN_WARPS - 1) / DDC_CHAIN_WARPS, 32 * DDC_CHAIN_WARPS, 0, st>>>(reinterpret_cast<const float3*>(d_params), d_phase_io, chunk_phase, channels, nchunks, chunk, next_chunk,
                                                              static_cast<const WrapTable*>(d_tables));
     CSDRB_CUDA(cudaGetLastError());
     const long total = (long)channels * nchunks;

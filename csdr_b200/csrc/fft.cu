@@ -24,15 +24,6 @@
 
 namespace csdrb {
 
-// Radix-16 passes (fft16.cuh) are the default: fewer passes over shared memory than radix 8 for the 4096- and 16384-point
-// transforms, the fastddc forward FFT and the config-5 overlap-add bank.  CSDRB_FFT_RADIX16=0 selects the radix-8 kernels (kept for A/B runs and for sizes
-// without a radix-16 plan).
-static bool fft_radix16_enabled()
-{
-    const char* e = getenv("CSDRB_FFT_RADIX16");
-    return !(e && e[0] == '0');
-}
-
 // ---- twiddle tables ------------------------------------------------------------------------------
 static std::map<int, float2*> g_tw;
 static std::mutex g_tw_mu;
@@ -111,8 +102,8 @@ int launch_fft_c2c_batch(const float2* d_in, long in_stride, float2* d_out, long
 {
     if (batch <= 0) return 0;
     if (n < 2 || n > FFT_MAX_N || (n & (n - 1))) { set_error("fft: size %d unsupported (power of two, 2..%d)", n, FFT_MAX_N); return -1; }
-    static const bool radix16 = fft_radix16_enabled();
-    if (radix16 && n >= 32) {
+    // radix-16 passes (fft16.cuh) from 32 points on: fewer passes over shared memory than radix 8 (4096: three instead of four, 16384: four instead of five)
+    if (n >= 32) {
         const float2* tw16 = nullptr;
         if (int rc = get_twiddles16(n, &tw16, st)) return rc;
         switch (n) {
@@ -124,7 +115,7 @@ int launch_fft_c2c_batch(const float2* d_in, long in_stride, float2* d_out, long
     const float2* tw = nullptr;
     if (int rc = get_twiddles(n, &tw, st)) return rc;
     switch (n) {
-#define X(N) case N: return launch_c2c_n<N>(d_in, in_stride, d_out, out_stride, batch, inverse != 0, tw, st);
+#define X(N) case N: if constexpr (N < 32) return launch_c2c_n<N>(d_in, in_stride, d_out, out_stride, batch, inverse != 0, tw, st); break;
         CSDRB_FFT_SIZES(X)
 #undef X
     }
@@ -147,9 +138,8 @@ int launch_olafir_bank(const float2* d_in, long in_stride, float2* d_out, long o
         if (blocks_per_cta < 16) blocks_per_cta = nblocks < 16 ? nblocks : 16;
     }
     const dim3 grid((nblocks + blocks_per_cta - 1) / blocks_per_cta, channels);
-    static const bool staged = getenv("CSDRB_OLAFIR_STAGED") != nullptr;            // A/B switch: the first kernel, with staged copies
-    static const bool radix16 = fft_radix16_enabled();
-    if (radix16 && !staged && (fft_size == 256 || fft_size == 4096)) {
+    // fused kernels: radix-16 passes at 256 and 4096 points, radix-8 passes at the other sizes from 16 on; 4 and 8 points take the staged kernel
+    if (fft_size == 256 || fft_size == 4096) {
         const float2* tw16 = nullptr;
         if (int rc = get_twiddles16(fft_size, &tw16, st)) return rc;
         const size_t fsmem = sizeof(float2) * ((size_t)fft_smem_elems(fft_size) + 2 * (size_t)(fft_size - input_size));
@@ -164,10 +154,10 @@ int launch_olafir_bank(const float2* d_in, long in_stride, float2* d_out, long o
         CSDRB_CUDA(cudaGetLastError());
         return 1;
     }
-    if (fft_size >= 16 && !staged) {
+    if (fft_size >= 16) {
         const size_t fsmem = sizeof(float2) * ((size_t)fft_smem_elems(fft_size) + 2 * (size_t)(fft_size - input_size));
         switch (fft_size) {
-#define X(N) case N: if constexpr (N >= 16 && N <= 8192) { auto k = olafir_bank_fused_kernel<N>; \
+#define X(N) case N: if constexpr (N >= 16 && N <= 8192 && N != 256 && N != 4096) { auto k = olafir_bank_fused_kernel<N>; \
             if (fsmem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem)); \
             k<<<grid, fft_threads(N), fsmem, st>>>(d_in, in_stride, d_out, out_stride, d_taps_fft, taps_stride, d_tail_io, input_size, nblocks, blocks_per_cta, tw); } break;
             CSDRB_FFT_SIZES(X)
@@ -178,7 +168,7 @@ int launch_olafir_bank(const float2* d_in, long in_stride, float2* d_out, long o
     }
     const size_t smem = sizeof(float2) * ((size_t)fft_smem_elems(fft_size) + (size_t)fft_size);
     switch (fft_size) {
-#define X(N) case N: if constexpr (N >= 4 && N <= 8192) { auto k = olafir_bank_kernel<N>; \
+#define X(N) case N: if constexpr (N == 4 || N == 8) { auto k = olafir_bank_kernel<N>; \
         if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
         k<<<grid, fft_threads(N), smem, st>>>(d_in, in_stride, d_out, out_stride, d_taps_fft, taps_stride, d_tail_io, input_size, nblocks, blocks_per_cta, tw); } break;
         CSDRB_FFT_SIZES(X)
@@ -193,8 +183,7 @@ int launch_fastddc_fwd(const float2* d_in, float2* d_spectra, float2* d_overlap_
 {
     if (nblocks <= 0) return 0;
     if (fft_size < 4 || fft_size > FFT_MAX_N || (fft_size & (fft_size - 1))) { set_error("fastddc_fwd: fft_size %d unsupported", fft_size); return -1; }
-    static const bool radix16 = fft_radix16_enabled();
-    if (radix16 && fft_size >= 32) {
+    if (fft_size >= 32) {                                               // radix-16 passes, as in launch_fft_c2c_batch
         const float2* tw16 = nullptr;
         if (int rc = get_twiddles16(fft_size, &tw16, st)) return rc;
         const size_t smem16 = sizeof(float2) * (size_t)fft_smem_elems(fft_size);
@@ -218,7 +207,7 @@ int launch_fastddc_fwd(const float2* d_in, float2* d_spectra, float2* d_overlap_
     if (int rc = get_twiddles(fft_size, &tw, st)) return rc;
     const size_t smem = sizeof(float2) * (size_t)fft_smem_elems(fft_size);
     switch (fft_size) {
-#define X(N) case N: if constexpr (N >= 4) { auto k = fastddc_fwd_kernel<N>; \
+#define X(N) case N: if constexpr (N >= 4 && N < 32) { auto k = fastddc_fwd_kernel<N>; \
         if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
         k<<<nblocks, fft_threads(N), smem, st>>>(d_in, d_spectra, d_overlap_io, input_size, tw); } break;
         CSDRB_FFT_SIZES(X)
@@ -258,11 +247,10 @@ int launch_apply_fir_fft(const float2* d_in, const float2* d_taps_fft, const flo
 struct InvPrep { int* blk_remain; float* blk_phase; int* blk_offset; WrapTable* tables; float2* phasor; int kmax; };
 
 // Geometries the fold path covers: whole 64-residue CTAs and an even pre-decimation (the half swap of the spectrum is then a rotation of the
-// fold's k index).  CSDRB_INV_FOLD=0 sends everything to the round-1 kernels.
+// fold's k index).
 bool fastddc_inv_fold_ok(int fft_size, int fft_inv_size)
 {
-    static const bool fold_off = getenv("CSDRB_INV_FOLD") && getenv("CSDRB_INV_FOLD")[0] == '0';
-    if (fold_off || fft_inv_size < 64 || fft_inv_size > 1024 || (fft_inv_size & (fft_inv_size - 1)) || fft_size % fft_inv_size) return false;
+    if (fft_inv_size < 64 || fft_inv_size > 1024 || (fft_inv_size & (fft_inv_size - 1)) || fft_size % fft_inv_size) return false;
     const int P = fft_size / fft_inv_size;
     return P >= 2 && P % 2 == 0;
 }
@@ -270,14 +258,11 @@ bool fastddc_inv_fold_ok(int fft_size, int fft_inv_size)
 // The data-independent half of a call: block-to-block {remain, phase} chain (updates the carried state, writes the per-block state and the
 // output counts) and the post-shift phasors of every (channel, block) row.  Everything on stream `s`.
 int launch_fastddc_inv_prepare(const void* d_chan, int channels, int nblocks, int post_input_size, int post_decimation, int* d_remain_io, float* d_phase_io,
-                               int* d_out_total, const InvPrep& p, cudaStream_t s, cudaEvent_t before_phasors = nullptr, bool build_tables = true)
+                               int* d_out_total, const InvPrep& p, cudaStream_t s, bool build_tables = true)
 {
     fastddc_state_chain_kernel<<<(channels + CHAIN_CPW * CHAIN_WARPS - 1) / (CHAIN_CPW * CHAIN_WARPS), 32 * CHAIN_WARPS, 0, s>>>(static_cast<const DdcChan*>(d_chan), d_remain_io, d_phase_io, p.blk_remain, p.blk_phase,
                                                        p.blk_offset, d_out_total, channels, nblocks, post_input_size, post_decimation, p.tables, build_tables ? 1 : 0);
     CSDRB_CUDA(cudaGetLastError());
-    // the chain (votes, shuffles, a double add per step) shares an SM with a running fold at no cost to either; the phasor walk is FMUL/FADD and does not --
-    // a caller that has a fold in flight passes the event behind it
-    if (before_phasors) CSDRB_CUDA(cudaStreamWaitEvent(s, before_phasors, 0));
     fastddc_phasor_kernel<<<(unsigned)(((long)channels * nblocks + 127) / 128), 128, 0, s>>>(static_cast<const DdcChan*>(d_chan), p.blk_phase, p.phasor, channels, nblocks, p.kmax);
     CSDRB_CUDA(cudaGetLastError());
     return 0;
@@ -291,19 +276,13 @@ int launch_fastddc_inv_apply(const float2* d_spectra, int nblocks, const float2*
     const float2* tw = nullptr;
     if (int rc = get_twiddles(fft_inv_size, &tw, st)) return rc;
     const size_t fsmem = sizeof(float2) * (size_t)FOLD_ST * 2 * (2 * FOLD_BT) * FOLD_R;
-    static const bool wide_cta = getenv("CSDRB_FOLD_BT") && getenv("CSDRB_FOLD_BT")[0] == '4';     // A/B: 512-thread CTAs with 8 x 4 thread tiles
-    static const bool x_first = getenv("CSDRB_FOLD_HFIRST") && getenv("CSDRB_FOLD_HFIRST")[0] == '0';   // A/B: the sample, not the tap pair, as first multiplicand
     const dim3 fgrid(fft_inv_size / FOLD_R, (channels + 2 * FOLD_CT - 1) / (2 * FOLD_CT), (nblocks + 2 * FOLD_BT - 1) / (2 * FOLD_BT));
     if (fgrid.y > 65535u || fgrid.z > 65535u) { set_error("fastddc_inv: bank too large for one call"); return -1; }
     const float inv_pre = 1.0f / (float)pre_decimation;
     const DdcChan* dc = static_cast<const DdcChan*>(d_chan);
     // (the attribute belongs to the current device's context: set per call, not latched per process)
-    if (wide_cta) CSDRB_CUDA(cudaFuncSetAttribute(fastddc_fold_kernel<4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
-    else if (x_first) CSDRB_CUDA(cudaFuncSetAttribute(fastddc_fold_kernel<8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
-    else CSDRB_CUDA(cudaFuncSetAttribute(fastddc_fold_kernel<8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
-    if (wide_cta) fastddc_fold_kernel<4, true><<<fgrid, 512, fsmem, st>>>(d_spectra, d_taps_fft, dc, folded, fft_size, fft_inv_size, nblocks, channels, inv_pre);
-    else if (x_first) fastddc_fold_kernel<8, false><<<fgrid, 256, fsmem, st>>>(d_spectra, d_taps_fft, dc, folded, fft_size, fft_inv_size, nblocks, channels, inv_pre);
-    else fastddc_fold_kernel<8, true><<<fgrid, 256, fsmem, st>>>(d_spectra, d_taps_fft, dc, folded, fft_size, fft_inv_size, nblocks, channels, inv_pre);
+    CSDRB_CUDA(cudaFuncSetAttribute(fastddc_fold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
+    fastddc_fold_kernel<<<fgrid, FOLD_NT, fsmem, st>>>(d_spectra, d_taps_fft, dc, folded, fft_size, fft_inv_size, nblocks, channels, inv_pre);
     CSDRB_CUDA(cudaGetLastError());
     if (after_fold) CSDRB_CUDA(cudaEventRecord(after_fold, st));
     if (prepared) CSDRB_CUDA(cudaStreamWaitEvent(st, prepared, 0));
@@ -343,8 +322,8 @@ int launch_fastddc_inv_bank(const float2* d_spectra, int nblocks, const float2* 
     float* blk_phase = reinterpret_cast<float*>(blk_remain + (size_t)channels * nblocks);
     int* blk_offset = reinterpret_cast<int*>(blk_phase + (size_t)channels * nblocks);
     WrapTable* tables = nblocks > 96 ? reinterpret_cast<WrapTable*>(static_cast<char*>(d_scratch) + (((size_t)channels * nblocks * 12 + 64 + 15) & ~(size_t)15)) : nullptr;
-    // Round-2 path: fold as a batched contraction (fastddc_fold_kernel), IFFT + post shift in a second kernel, and the data-independent
-    // block-to-block state chain + phasor walk on a side stream meanwhile.  Anything fastddc_inv_fold_ok() refuses takes the round-1 kernels below.
+    // Fold path: fold as a batched contraction (fastddc_fold_kernel), IFFT + post shift in a second kernel, and the data-independent
+    // block-to-block state chain + phasor walk on a side stream meanwhile.  Anything fastddc_inv_fold_ok() refuses takes the single-kernel forms below.
     if (fastddc_inv_fold_ok(fft_size, fft_inv_size)) {
         SideStream* ss = side_stream();
         if (!ss) return -1;
@@ -385,18 +364,17 @@ int launch_fastddc_inv_bank(const float2* d_spectra, int nblocks, const float2* 
     fastddc_state_chain_kernel<<<(channels + CHAIN_CPW * CHAIN_WARPS - 1) / (CHAIN_CPW * CHAIN_WARPS), 32 * CHAIN_WARPS, 0, st>>>(static_cast<const DdcChan*>(d_chan), d_remain_io, d_phase_io, blk_remain, blk_phase,
                                                                     blk_offset, d_out_total, channels, nblocks, post_input_size, post_decimation, tables, 1);
     CSDRB_CUDA(cudaGetLastError());
-    if (fft_inv_size <= 1024 && fft_inv_size >= 8 && (fft_size / fft_inv_size) % 2 == 0) {
+    if (fft_inv_size >= 8 && fft_inv_size <= 32 && (fft_size / fft_inv_size) % 2 == 0) {          // (64..1024 with an even P is the fold path's)
         // Tile = CT channels x BT blocks per CTA (each spectrum bin fetched once per CT channels, each tap once per BT blocks).  Big tiles
         // save L2 traffic but a bank of 64 channels x 16 blocks is only 64 CTAs of 4x4 on the whole GPU (the launch is latency-bound),
-        // so the tile shrinks until the grid covers the machine about twice.  CSDRB_INV_TILE=44|22 forces one for A/B runs.
-        static const char* forced = getenv("CSDRB_INV_TILE");
+        // so the tile shrinks until the grid covers the machine about twice.
         const long ctas44 = (long)((nblocks + 3) / 4) * ((channels + 3) / 4);
-        const bool small_tile = forced ? (forced[0] == '2') : (ctas44 < 2 * kSmCount);
+        const bool small_tile = ctas44 < 2 * kSmCount;
         const int CTv = small_tile ? 2 : 4, BTv = small_tile ? 2 : 4;
         const dim3 tgrid((nblocks + BTv - 1) / BTv, (channels + CTv - 1) / CTv);
         const size_t smem = sizeof(float2) * (size_t)CTv * BTv * fft_smem_elems(fft_inv_size);
         switch (fft_inv_size) {
-#define X(M) case M: if constexpr (M >= 8 && M <= 1024) { \
+#define X(M) case M: if constexpr (M >= 8 && M <= 32) { \
             if (small_tile) { auto k = fastddc_inv_tiled_kernel<M, 2, 2>; \
                 if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
                 k<<<tgrid, 256, smem, st>>>(d_spectra, d_taps_fft, static_cast<const DdcChan*>(d_chan), blk_remain, blk_phase, blk_offset, d_out, out_stride, \
@@ -452,13 +430,13 @@ static size_t plan_prep_bytes(int channels, int nblocks, int kmax)
     return fastddc_inv_scratch_bytes(channels, nblocks) + 16 + sizeof(float2) * (size_t)channels * nblocks * (size_t)kmax;
 }
 
-static int plan_enqueue_prepare(FastddcInvPlan* pl, int q, cudaEvent_t before_phasors = nullptr)
+static int plan_enqueue_prepare(FastddcInvPlan* pl, int q)
 {
     // state of set q := state of the other set (what the previous preparation left), then the chain advances it in place
     CSDRB_CUDA(cudaMemcpyAsync(pl->d_remain[q], pl->d_remain[1 - q], sizeof(int) * pl->channels, cudaMemcpyDeviceToDevice, pl->side));
     CSDRB_CUDA(cudaMemcpyAsync(pl->d_phase[q], pl->d_phase[1 - q], sizeof(float) * pl->channels, cudaMemcpyDeviceToDevice, pl->side));
     if (int rc = launch_fastddc_inv_prepare(pl->d_chan, pl->channels, pl->nblocks, pl->post_input_size, pl->post_decimation, pl->d_remain[q], pl->d_phase[q],
-                                            pl->d_total[q], pl->prep[q], pl->side, before_phasors, !pl->tables_built)) return rc;
+                                            pl->d_total[q], pl->prep[q], pl->side, !pl->tables_built)) return rc;
     pl->tables_built = true;
     CSDRB_CUDA(cudaEventRecord(pl->ready[q], pl->side));
     return 0;
@@ -552,12 +530,9 @@ int fastddc_inv_plan_run(void* plan, const float2* d_spectra, const float2* d_ta
     CSDRB_CUDA(cudaStreamWaitEvent(pl->side, pl->post_done[q], 0));       // set q was last read two runs ago (a never-recorded event does not block)
     if (trace) CSDRB_CUDA(cudaEventRecord(tev[3], pl->side));
     // A chain walked NEXT TO the fold stretches the fold (one chain warp per channel, 64 SMs with a guest
-    // that holds up every barrier of the fold CTA there), so chain and walk go behind the fold, next to the IFFT step and the caller's next forward FFT
-    // ('f', the default).  CSDRB_PLAN_ORDER for A/B: 'd' = chain at once, walk behind the fold; 'i' = chain at once, walk behind the IFFT step; 's' = both behind the IFFT step.
-    static const char order = getenv("CSDRB_PLAN_ORDER") ? getenv("CSDRB_PLAN_ORDER")[0] : 'f';
-    if (order == 'f') CSDRB_CUDA(cudaStreamWaitEvent(pl->side, pl->fold_done, 0));
-    if (order == 's') CSDRB_CUDA(cudaStreamWaitEvent(pl->side, pl->post_done[p], 0));
-    if (int rc = plan_enqueue_prepare(pl, q, order == 'i' ? pl->post_done[p] : (order == 'd' ? pl->fold_done : nullptr))) return rc;
+    // that holds up every barrier of the fold CTA there), so chain and walk go behind the fold, next to the IFFT step and the caller's next forward FFT.
+    CSDRB_CUDA(cudaStreamWaitEvent(pl->side, pl->fold_done, 0));
+    if (int rc = plan_enqueue_prepare(pl, q)) return rc;
     pl->cur = q; pl->ahead = true;
     if (trace) {
         CSDRB_CUDA(cudaEventRecord(tev[4], pl->side));

@@ -1,4 +1,4 @@
-// fft16.cuh -- EXPERIMENT (branch r2-prep): radix-16 passes for the block FFT.
+// fft16.cuh -- radix-16 passes for the block FFT.
 //
 // N = R0 * 16^k with R0 in {2, 4, 8, 16}: 4096 = 16*16*16 is three passes instead of four, 16384 = 4*16*16*16 four instead of five.  With the
 // first pass reading the caller's data and the last pass writing it (fft.cuh: block_fft_io) a 4096-point transform touches shared memory

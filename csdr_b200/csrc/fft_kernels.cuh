@@ -85,7 +85,7 @@ olafir_bank_kernel(const float2* __restrict__ in, long in_stride, float2* __rest
     if (b_last == nblocks) for (int i = tid; i < overlap; i += NT) tail_io[(long)ch * N + i] = tail[i];
 }
 
-// EXPERIMENT: the fused overlap-add kernel on radix-16 passes, sizes 16^k (config 5's 4096): 4R+4W shared accesses per point and block
+// The fused overlap-add kernel on radix-16 passes, sizes 16^k (config 5's 4096): 4R+4W shared accesses per point and block
 template <int N>
 __global__ void __launch_bounds__(fft16_threads(N), (N <= 4096 ? 2 : 1))
 olafir_bank_fused16_kernel(const float2* __restrict__ in, long in_stride, float2* __restrict__ out, long out_stride,
@@ -141,7 +141,7 @@ olafir_bank_fused16_kernel(const float2* __restrict__ in, long in_stride, float2
     if (b_last == nblocks) for (int i = tid; i < overlap; i += NT) tail_io[(long)ch * N + i] = tail_cur[i];
 }
 
-// EXPERIMENT: the batched transform with radix-16 passes (fft16.cuh); tw16 = the four-plane table of fft16_fill_twiddles
+// The batched transform with radix-16 passes (fft16.cuh); tw16 = the four-plane table of fft16_fill_twiddles
 template <int N, bool INV>
 __global__ void __launch_bounds__(fft16_threads(N))
 fft_c2c_batch16_kernel(const float2* __restrict__ in, long in_stride, float2* __restrict__ out, long out_stride, const float2* __restrict__ tw16)
@@ -237,7 +237,7 @@ fastddc_fwd_kernel(const float2* __restrict__ in, float2* __restrict__ spectra, 
     block_fft_io<N, NT, false>(s, tw, tid, src, dst);
 }
 
-// EXPERIMENT: the same forward step on radix-16 passes (16384 = 4*16^3: four passes instead of five)
+// The same forward step on radix-16 passes (16384 = 4*16^3: four passes instead of five)
 template <int N>
 __global__ void __launch_bounds__(fft16_threads(N))
 fastddc_fwd16_kernel(const float2* __restrict__ in, float2* __restrict__ spectra, const float2* __restrict__ overlap_in,
@@ -534,7 +534,7 @@ fastddc_inv_tiled_kernel(const float2* __restrict__ spectra, const float2* __res
 }
 
 
-// ---- fastddc inverse, round 2: fold as a batched complex contraction + a separate IFFT / post-shift kernel ------------------------------
+// ---- fastddc inverse: fold as a batched complex contraction + a separate IFFT / post-shift kernel ------------------------------------
 // The tiled kernel above waits on the fold's global loads, and a 4x4 tile still pulls 1.07 GB through L2 per 64 ch x 256 blocks.  The fold is, per residue r of M,
 //     F[c][b][r] = sum_{k < P}  Xs[b][r + k*M] * H[c][r + k*M],           P = N / M  (= pre_decimation)
 // i.e. M independent complex (C x P) * (P x B) products.  fastddc_fold_kernel runs it like a GEMM: a CTA owns 64 residues x 16 channels x
@@ -545,19 +545,16 @@ fastddc_inv_tiled_kernel(const float2* __restrict__ spectra, const float2* __res
 // The folded bins go to a scratch array (L2-sized: 64 ch x 256 blocks x 512 bins = 67 MB), fastddc_ifft_rows_kernel does IFFT_M, /M,
 // scrap and the post shift; the block-to-block state chain runs on a side stream meanwhile (it is data-independent).
 constexpr int FOLD_R = 64, FOLD_CT = 8, FOLD_BT = 8, FOLD_ST = 3;     // residues per CTA, thread tile (channels x blocks), pipeline stages
+constexpr int FOLD_NT = 64 * 2 * 2;                                   // threads: a residue each, times two channel halves, times two block halves of the CTA tile
 
-// BT = blocks per thread tile: 8 -> 256 threads (8 warps per SM), 4 -> 512 threads (16 warps, half the accumulators per thread: more latency hiding, more
-// shared-memory reads per FMA).  The CTA tile is 64 residues x 16 channels x 16 blocks either way.
-// HFIRST = the tap pair is the FIRST multiplicand of each FMA pair (operand order only; both forms compute the same values).
-template <int BT, bool HFIRST>
-__global__ void __launch_bounds__(64 * 2 * (2 * FOLD_BT / BT), 1)
+__global__ void __launch_bounds__(FOLD_NT, 1)
 fastddc_fold_kernel(const float2* __restrict__ spectra /*[nblocks][N]*/, const float2* __restrict__ taps_fft /*[C][N]*/, const DdcChan* __restrict__ chan,
                     float2* __restrict__ folded /*[C][nblocks][M]*/, int N, int M, int nblocks, int channels, float inv_pre)
 {
     CSDRB_DYN_SMEM(smem_raw);
     float2* sm = reinterpret_cast<float2*>(smem_raw);                   // FOLD_ST stages of { x[16][64], h[16][64] }
     constexpr int ROWS = 2 * FOLD_BT, STAGE = 2 * ROWS * FOLD_R;        // float2 per stage
-    constexpr int NT = 64 * 2 * (ROWS / BT), CPT = (2 * ROWS * (FOLD_R / 2)) / NT;   // threads; 16-byte copies per thread and k-step
+    constexpr int NT = FOLD_NT, CPT = (2 * ROWS * (FOLD_R / 2)) / NT;  // 16-byte copies per thread and k-step
     const int tid = threadIdx.x;
     const int rl = tid & 63, g = tid >> 6, gc = g & 1, gb = g >> 1;
     const int r0 = blockIdx.x * FOLD_R, c0 = blockIdx.y * (2 * FOLD_CT), b0 = blockIdx.z * (2 * FOLD_BT);
@@ -577,11 +574,11 @@ fastddc_fold_kernel(const float2* __restrict__ spectra /*[nblocks][N]*/, const f
         for (int q = 0; q < CPT; q++) cp_async16(sm + stage * STAGE + dsto[q], src[q] + (long)(q < CPT / 2 ? kx : k) * M);
     };
     // (a 4-stage ring with the next step's operands pulled into registers during the FMAs was slower: it needs ~230 registers)
-    float2 acc[FOLD_CT][BT];
+    float2 acc[FOLD_CT][FOLD_BT];
 #pragma unroll
     for (int u = 0; u < FOLD_CT; u++)
 #pragma unroll
-        for (int v = 0; v < BT; v++) acc[u][v] = make_float2(0.f, 0.f);
+        for (int v = 0; v < FOLD_BT; v++) acc[u][v] = make_float2(0.f, 0.f);
 #pragma unroll
     for (int s = 0; s < FOLD_ST - 1; s++) { if (s < P) issue(s, s); cp_async_commit(); }
     for (int k = 0; k < P; k++) {
@@ -589,11 +586,11 @@ fastddc_fold_kernel(const float2* __restrict__ spectra /*[nblocks][N]*/, const f
         __syncthreads();                                                // stage k has landed for everyone; stage (k-1) is free again
         if (k + FOLD_ST - 1 < P) issue(k + FOLD_ST - 1, (k + FOLD_ST - 1) % FOLD_ST);
         cp_async_commit();
-        const float2* xs = sm + (k % FOLD_ST) * STAGE + (gb * BT) * FOLD_R + rl;
+        const float2* xs = sm + (k % FOLD_ST) * STAGE + (gb * FOLD_BT) * FOLD_R + rl;
         const float2* hs = sm + (k % FOLD_ST) * STAGE + (ROWS + gc * FOLD_CT) * FOLD_R + rl;
-        float2 x[BT], h[FOLD_CT];
+        float2 x[FOLD_BT], h[FOLD_CT];
 #pragma unroll
-        for (int v = 0; v < BT; v++) x[v] = xs[v * FOLD_R];
+        for (int v = 0; v < FOLD_BT; v++) x[v] = xs[v * FOLD_R];
 #pragma unroll
         for (int u = 0; u < FOLD_CT; u++) h[u] = hs[u * FOLD_R];
         // acc += x*h = xr*(hr, hi) + xi*(-hi, hr): two packed FMAs per accumulator, scalar-broadcast x against h and against h swapped/negated
@@ -601,14 +598,12 @@ fastddc_fold_kernel(const float2* __restrict__ spectra /*[nblocks][N]*/, const f
 #pragma unroll
         for (int u = 0; u < FOLD_CT; u++)
 #pragma unroll
-            for (int v = 0; v < BT; v++)
-                acc[u][v] = HFIRST ? ffma2(h[u], make_float2(x[v].x, x[v].x), acc[u][v]) : ffma2(make_float2(x[v].x, x[v].x), h[u], acc[u][v]);
+            for (int v = 0; v < FOLD_BT; v++) acc[u][v] = ffma2(h[u], make_float2(x[v].x, x[v].x), acc[u][v]);
 #pragma unroll
         for (int u = 0; u < FOLD_CT; u++)
 #pragma unroll
-            for (int v = 0; v < BT; v++)
-                acc[u][v] = HFIRST ? ffma2(make_float2(__uint_as_float(__float_as_uint(h[u].y) ^ 0x80000000u), h[u].x), make_float2(x[v].y, x[v].y), acc[u][v])
-                                   : ffma2(make_float2(x[v].y, x[v].y), make_float2(__uint_as_float(__float_as_uint(h[u].y) ^ 0x80000000u), h[u].x), acc[u][v]);
+            for (int v = 0; v < FOLD_BT; v++)
+                acc[u][v] = ffma2(make_float2(__uint_as_float(__float_as_uint(h[u].y) ^ 0x80000000u), h[u].x), make_float2(x[v].y, x[v].y), acc[u][v]);
     }
     // /pre_decimation, and both half swaps (fastddc.c:143-150) folded into the destination index (r - offsetbin) mod M
     const int r = r0 + rl;
@@ -619,8 +614,8 @@ fastddc_fold_kernel(const float2* __restrict__ spectra /*[nblocks][N]*/, const f
         int d2 = (r - chan[c].offsetbin) % M;
         if (d2 < 0) d2 += M;
 #pragma unroll
-        for (int v = 0; v < BT; v++) {
-            const int b = b0 + gb * BT + v;
+        for (int v = 0; v < FOLD_BT; v++) {
+            const int b = b0 + gb * FOLD_BT + v;
             if (b < nblocks) folded[((long)c * nblocks + b) * M + d2] = make_float2(acc[u][v].x * inv_pre, acc[u][v].y * inv_pre);
         }
     }

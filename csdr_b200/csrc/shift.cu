@@ -502,12 +502,14 @@ int launch_shift_addition_bank(const float2* d_in, long in_stride, float2* d_out
     constexpr size_t smem = 0;                                          // the tiles are static shared memory
     // The chain is one warp per channel and sequential: a long one is cut into up to three slices that run on a side stream, the main
     // kernel follows slice by slice on the caller's stream.  A slice must still fill the machine (a warp walks its 32 chunks tile after tile:
-    // eight slices of 384 chunks x 64 channels run the main kernel at under half a wave and gain nothing).  CSDRB_SHIFT_SLICES=1: one stream.
-    static const int max_slices = getenv("CSDRB_SHIFT_SLICES") ? atoi(getenv("CSDRB_SHIFT_SLICES")) : 3;
-    static const long slice_min = getenv("CSDRB_SHIFT_SLICE_MIN") ? atol(getenv("CSDRB_SHIFT_SLICE_MIN")) : 768L * 64;   // chunk-channels a slice needs to fill the machine (the CPU tier lowers it)
+    // eight slices of 384 chunks x 64 channels run the main kernel at under half a wave and gain nothing).
+    constexpr int max_slices = 3;
+    static_assert(max_slices <= kSideSlices, "one side-stream event per slice");
+    // Chunk-channels a slice needs to fill the machine.  CSDRB_SHIFT_SLICE_MIN lowers it for the emulated CPU tests
+    // (tests/test_kernels_emulated.py), whose banks are far too small to reach the sliced path otherwise.
+    static const long slice_min = getenv("CSDRB_SHIFT_SLICE_MIN") ? atol(getenv("CSDRB_SHIFT_SLICE_MIN")) : 768L * 64;
     int slices = (int)(((long)nchunks * channels) / (slice_min > 0 ? slice_min : 1));
     if (slices > max_slices) slices = max_slices;
-    if (slices > kSideSlices) slices = kSideSlices;
     if (slices < 2) {
         shift_phase_chain_kernel<<<(channels + CHAIN_CPW * CHAIN_WARPS - 1) / (CHAIN_CPW * CHAIN_WARPS), 32 * CHAIN_WARPS, 0, st>>>(prm, d_phase_io, chunk_phase, channels, n, chunk, nchunks, tables, 0, nchunks);
         CSDRB_CUDA(cudaGetLastError());

@@ -1,7 +1,7 @@
 """GPU parity tests added in round 2 (run with -m gpu on an H100), all through the C ABI of libcsdr_b200.so:
   * the u8 front end fused into the FIR bank (convert_u8_f | fir_decimate_cc, csdr-fm:41), device and host (end-to-end) calls;
   * the table-driven phase chains (csrc/phase_table.cuh): long chains, every rate class, bit-exact carried phases vs the oracle's loops;
-  * the fold-based fastddc inverse bank on ragged channel / block counts, against the round-1 kernels and the oracle;
+  * the fold-based fastddc inverse bank on ragged channel / block counts against the oracle, in one call and carried into a second;
   * config 2 against the COMPILED reference on 8 channels x 262 144 samples (SURVEY 8(d)) and every 32nd channel of the full-size bank;
   * a retune of the streaming DDC bank in the middle of an NCO chunk: the phase stays continuous (ADVICE r1).
 Every tolerance assert prints the value it achieved.
@@ -142,7 +142,7 @@ def test_fastddc_inverse_plan_equals_the_stateless_bank(gpu, oracle, channels, n
         plan.close()
 
 
-# ------------------------------------------------------------------------------------------ fastddc inverse: fold path vs round-1 kernels vs oracle
+# ------------------------------------------------------------------------------------------ fastddc inverse: fold path vs oracle
 @pytest.mark.parametrize("channels,nblocks", [(1, 1), (3, 5), (17, 33), (20, 130)])
 def test_fastddc_fold_path_ragged_banks(gpu, oracle, channels, nblocks):
     bw, dec = 0.002, 64

@@ -432,7 +432,10 @@ def test_k7_fft_every_size_both_directions(fft):
     for n in (2, 4, 8, 16, 32, 64, 128, 256, 512, 1024, 2048, 4096, 8192, 16384):
         x = _aligned((2, n), np.complex64); x[:] = _cplx(rng, 2, n); y = _aligned((2, n), np.complex64)
         for inv in (0, 1):
+            b0 = fft.emul_barriers()
             assert fft.emul_launch_fft_c2c_batch(P(x), n, P(y), n, n, 2, inv) >= 0, fft.emul_last_error()
+            if n == 4096:
+                assert (fft.emul_barriers() - b0) // 2 == 4                # radix-16 passes from 32 points on: three passes at 4096 (four barriers per row)
             want = np.fft.ifft(x.astype(np.complex128), axis=1) * n if inv else np.fft.fft(x.astype(np.complex128), axis=1)
             assert rel_rms(y, want) < 1e-6, (n, inv)                      # same bar as tests/test_gpu_parity2.py::test_fft_all_sizes_vs_float64_dft
         buf = _cplx(rng, n + 3); out = Z(n + 3, np.complex64)
@@ -442,45 +445,16 @@ def test_k7_fft_every_size_both_directions(fft):
     assert fft.emul_barriers() > 100                                       # the barriers were real
 
 
-def test_k7_radix8_kernels_behind_the_switch(fft, tmp_path_factory):
-    """radix-16 passes (fft16.cuh) are the default since round 2; CSDRB_FFT_RADIX16=0 selects the radix-8 kernels, which stay shipped (sizes without a
-    radix-16 plan, A/B runs) -- a private copy of the library reads the switch, so both generations run every size here.  Also covers the overlap-add
-    bank and the fastddc forward step of that generation."""
-    so, names, proto = _built["fft.cu"]
-    copy = so.with_name(f"{so.stem}_radix8.so")
-    if not copy.exists():
-        shutil.copy(so, copy)
-    z = _aligned((1, 32), np.complex64); z[:] = 1
-    assert fft.emul_launch_fft_c2c_batch(P(z), 32, P(z.copy()), 32, 32, 1, 0) >= 0      # the default library latches its (unset) switch now
-    os.environ["CSDRB_FFT_RADIX16"] = "0"
-    try:
-        lib = C.CDLL(str(copy))
-        f = lib.emul_launch_fft_c2c_batch; f.argtypes, f.restype = proto.emul_launch_fft_c2c_batch.argtypes, proto.emul_launch_fft_c2c_batch.restype
-        lib.emul_barriers.restype = C.c_long
-        rng = np.random.default_rng(16)
-        for n in (32, 64, 128, 256, 512, 1024, 2048, 4096, 8192, 16384):
-            x = _aligned((2, n), np.complex64); x[:] = _cplx(rng, 2, n); y = _aligned((2, n), np.complex64)
-            for inv in (0, 1):
-                b0 = lib.emul_barriers()                                # (the emulator's counters are one per process: inline-function statics are GNU-unique)
-                assert f(P(x), n, P(y), n, n, 2, inv) >= 0
-                passes8 = (lib.emul_barriers() - b0) // 2
-                want = np.fft.ifft(x.astype(np.complex128), axis=1) * n if inv else np.fft.fft(x.astype(np.complex128), axis=1)
-                assert rel_rms(y, want) < 1e-6, (n, inv)
-                y2 = _aligned((2, n), np.complex64); b1 = fft.emul_barriers()
-                assert fft.emul_launch_fft_c2c_batch(P(x), n, P(y2), n, n, 2, inv) >= 0 and rel_rms(y2, want) < 1e-6
-                passes16 = (fft.emul_barriers() - b1) // 2
-            if n == 4096:
-                assert passes16 == 4 and passes8 > 4                      # default library: three radix-16 passes; the copy: four radix-8 passes
-        g = lib.emul_launch_olafir_bank; g.argtypes, g.restype = proto.emul_launch_olafir_bank.argtypes, proto.emul_launch_olafir_bank.restype
-        N, isz, nb = 4096, 2098, 3
-        x = _aligned((1, nb * isz), np.complex64); x[:] = _cplx(rng, 1, nb * isz)
-        H = _aligned(N, np.complex64); H[:] = _cplx(rng, N)
-        tail = _aligned((1, N), np.complex64); tail[:] = 0; out = _aligned((1, nb * isz), np.complex64)
-        assert g(P(x), nb * isz, P(out), nb * isz, 1, N, isz, nb, P(H), 0, P(tail), 0) >= 0
-        want, _ = _overlap_add(x[0].astype(np.complex128), H.astype(np.complex128), N, isz)
-        assert rel_rms(out[0], want) < 5e-6
-    finally:
-        del os.environ["CSDRB_FFT_RADIX16"]
+def test_k7_apply_fir_fft_every_size(fft):
+    """apply_fir_fft_cc's one-block kernel runs the radix-8 block_fft passes at every size: forward FFT, product with taps_fft, inverse FFT, /N, + the
+    previous overlap, against float64"""
+    rng = np.random.default_rng(16)
+    for n in (2, 4, 8, 16, 32, 64, 128, 256, 512, 1024, 2048, 4096, 8192, 16384):
+        ov = n // 4
+        x = _cplx(rng, n); H = _cplx(rng, n); last = _cplx(rng, max(ov, 1)); out = Z(n, np.complex64)
+        assert fft.emul_launch_apply_fir_fft(P(x), P(H), P(last), ov, P(out), n) >= 0, fft.emul_last_error()
+        want = np.fft.ifft(np.fft.fft(x.astype(np.complex128)) * H.astype(np.complex128)); want[:ov] += last[:ov]
+        assert rel_rms(out, want) < 1e-6, n
 
 
 def _overlap_add(x, H, N, isz):
@@ -492,7 +466,7 @@ def _overlap_add(x, H, N, isz):
 
 
 @pytest.mark.parametrize("N,isz,nb,bpc", [(4096, 2098, 5, 2), (4096, 2098, 3, 0), (512, 300, 7, 3), (64, 40, 9, 4), (256, 178, 6, 6), (1024, 224, 12, 5),
-                                          (2048, 1500, 4, 2), (16, 9, 11, 3), (128, 128, 3, 2), (32, 1, 70, 16)])
+                                          (2048, 1500, 4, 2), (16, 9, 11, 3), (128, 128, 3, 2), (32, 1, 70, 16), (8192, 7000, 3, 2), (8, 5, 9, 4), (4, 3, 7, 2)])
 def test_k9_overlap_add_bank(fft, N, isz, nb, bpc):
     """bandpass_fir_fft_cc block loop: CTA runs of `bpc` blocks (lead-in recomputation), overlap > input_size, no overlap, streaming tails."""
     rng = np.random.default_rng(N + isz)
@@ -594,10 +568,12 @@ def test_k8_fastddc_inverse_plan_equals_the_stateless_bank(fft, oracle, nb, runs
         assert rel_rms(got[c, :gt[c]], ref[-gt[c]:]) < 5e-6, c
 
 
-@pytest.mark.parametrize("bw,dec,shift", [(0.05, 8, 0.123), (0.05, 3, -0.2), (0.01, 6, 0.25), (0.05, 4, 0.2), (0.02, 4, 0.05), (0.05, 16, -0.3), (0.05, 32, 0.4)])
+@pytest.mark.parametrize("bw,dec,shift", [(0.05, 8, 0.123), (0.05, 3, -0.2), (0.01, 6, 0.25), (0.05, 4, 0.2), (0.02, 4, 0.05), (0.05, 16, -0.3), (0.05, 32, 0.4),
+                                          (0.05, 64, -0.1)])
 def test_k8_fastddc_forward_and_inverse(fft, oracle, bw, dec, shift):
     """a12/a13 against the oracle (and, for the first geometry, the golden spectra / channel output of the compiled reference);
-    decimation 3 has pre_decimation 1 and takes the one-CTA-per-(block, channel) kernel, the others the tiled one."""
+    decimation 3 has pre_decimation 1 and takes the one-CTA-per-(block, channel) kernel, 6 has fft_inv_size 2048 and takes it too, decimation 64
+    (fft_inv_size 32) the tiled one, the others the fold path."""
     from oracle.pyoracle import _CF, _p, WINDOWS
     g, _ = oracle.fastddc_init(bw, dec, shift)
     rng = np.random.default_rng(dec)
@@ -626,3 +602,17 @@ def test_k8_fastddc_forward_and_inverse(fft, oracle, bw, dec, shift):
     assert total[0] == want.size and rel_rms(out[0, :want.size], want) < 5e-6
     if (bw, dec) == (0.05, 8):
         assert rel_rms(sp, GOLD["ddc_fwd_out"]) < 1e-6 and rel_rms(out[0, :total[0]], GOLD["ddc_inv_out"]) < 5e-6
+
+
+@pytest.mark.parametrize("N", [4, 8, 16, 32, 64, 128, 256, 512, 1024, 2048, 4096, 8192, 16384])
+def test_k8_fastddc_forward_every_size(fft, N):
+    """the forward step at every size (radix-8 passes below 32 points, radix-16 from 32 on): overlap-save blocks of the carried overlap followed by
+    the stream, against float64, and the overlap carried out"""
+    isz = N - max(1, N // 8)
+    rng = np.random.default_rng(N)
+    nb, ov = 5, N - isz
+    x = _cplx(rng, nb * isz); sp = Z((nb, N), np.complex64); carry = _cplx(rng, ov)
+    stream = np.concatenate([carry, x]).astype(np.complex128)
+    assert fft.emul_launch_fastddc_fwd(P(x), P(sp), P(carry), N, isz, nb) >= 0, fft.emul_last_error()
+    assert rel_rms(sp, np.stack([np.fft.fft(stream[b * isz:b * isz + N]) for b in range(nb)])) < 1e-6
+    assert np.array_equal(carry, x[nb * isz - ov:])
