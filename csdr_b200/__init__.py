@@ -44,6 +44,15 @@ class _FastAgc(C.Structure):            # fastagc_ff_t (= libcsdr.h:118-128)
                 ("peak_2", C.c_float), ("input_size", C.c_int), ("reference", C.c_float), ("last_gain", C.c_float)]
 
 
+class AgcParams(C.Structure):           # csdrb_agc_params_t; defaults = the agc_ff CLI's (csdr.c:1342-1361) with its 1024-sample calls
+    _fields_ = [("reference", C.c_float), ("attack_rate", C.c_float), ("decay_rate", C.c_float), ("max_gain", C.c_float),
+                ("hang_time", C.c_int), ("attack_wait_time", C.c_int), ("gain_filter_alpha", C.c_float), ("chunk", C.c_int)]
+
+    def __init__(self, reference=0.2, attack_rate=0.01, decay_rate=0.0001, max_gain=65536.0, hang_time=200, attack_wait_time=0,
+                 gain_filter_alpha=0.999, chunk=1024):
+        super().__init__(reference, attack_rate, decay_rate, max_gain, hang_time, attack_wait_time, gain_filter_alpha, chunk)
+
+
 class _Unroll(C.Structure):             # shift_unroll_data_t (= libcsdr.h:199-205)
     _fields_ = [("dsin", C.POINTER(C.c_float)), ("dcos", C.POINTER(C.c_float)), ("phase_increment", C.c_float), ("size", C.c_int)]
 
@@ -111,6 +120,13 @@ def lib() -> C.CDLL:
     L.csdrb_fastagc_bank_scratch_bytes.argtypes = [it, it]; L.csdrb_fastagc_bank_scratch_bytes.restype = sz
     L.csdrb_fastagc_bank_ff.argtypes = [vp, lg, vp, lg, it, it, it, C.c_float, vp, vp, vp, sz, vp]
     L.csdrb_fastagc_bank_f_s16.argtypes = [vp, lg, vp, lg, it, it, it, C.c_float, vp, vp, vp, sz, vp]
+    L.csdrb_amdemod_cf.argtypes = [vp, vp, lg, vp]
+    L.csdrb_fastdcblock_bank_ff.argtypes = [vp, lg, it, vp, lg, it, it, it, vp, vp]
+    L.csdrb_agc_bank_ff.argtypes = [vp, lg, it, vp, lg, it, it, it, C.POINTER(AgcParams), vp, C.c_float, vp]
+    L.amdemod_cf.argtypes = [vp, vp, it]
+    L.fastdcblock_ff.argtypes = [vp, vp, it, C.c_float]; L.fastdcblock_ff.restype = C.c_float
+    L.agc_ff.argtypes = [vp, vp, it, C.c_float, C.c_float, C.c_float, C.c_float, C.c_short, C.c_short, C.c_float, C.c_float]
+    L.agc_ff.restype = C.c_float
     L.csdrb_fft_c2c_batch.argtypes = [vp, lg, vp, lg, it, it, it, vp]
     L.csdrb_bandpass_fir_fft_bank_cc.argtypes = [vp, lg, vp, lg, it, it, it, it, vp, lg, vp, vp]
     L.csdrb_ddc_bank_scratch_bytes.argtypes = [it, it, it, it]; L.csdrb_ddc_bank_scratch_bytes.restype = sz
@@ -475,6 +491,26 @@ class libcsdr:
         return y
 
     @staticmethod
+    def amdemod_cf(x):
+        x = np.ascontiguousarray(x, np.complex64); y = np.empty(x.size, np.float32)
+        lib().amdemod_cf(x.ctypes.data, y.ctypes.data, x.size); return y
+
+    @staticmethod
+    def fastdcblock_ff(x, last_dc=0.0):
+        """one call on one block: (y, block average)"""
+        x = np.ascontiguousarray(x, np.float32); y = np.empty_like(x)
+        avg = lib().fastdcblock_ff(x.ctypes.data, y.ctypes.data, x.size, last_dc); return y, float(np.float32(avg))
+
+    @staticmethod
+    def agc_ff(x, reference=0.2, attack_rate=0.01, decay_rate=0.0001, max_gain=65536.0, hang_time=200, attack_wait_time=0,
+               gain_filter_alpha=0.999, last_gain=1.0):
+        """one agc_ff call: (y, last gain)"""
+        x = np.ascontiguousarray(x, np.float32); y = np.empty_like(x)
+        g = lib().agc_ff(x.ctypes.data, y.ctypes.data, x.size, reference, attack_rate, decay_rate, max_gain, hang_time, attack_wait_time,
+                         gain_filter_alpha, last_gain)
+        return y, float(np.float32(g))
+
+    @staticmethod
     def deemphasis_wfm_ff(x, tau, sample_rate, last=0.0, block=None):
         x = np.ascontiguousarray(x, np.float32); y = np.empty_like(x); block = block or max(x.size, 1)
         for s0 in range(0, x.size, block):
@@ -799,6 +835,51 @@ def fastagc_bank_f_s16(x, block: int = 1024, reference: float = 1.0, state=None,
     _check(lib().csdrb_fastagc_bank_f_s16(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, block, nblocks, reference,
                                           state.data_ptr(), hist.data_ptr(), scratch.data_ptr(), scratch.numel(), _stream()), "fastagc_bank_f_s16")
     return out, state, hist
+
+
+def amdemod_cf(x, out=None):
+    """|x| of a complex64 CUDA tensor (amdemod_cf, correctly rounded sqrt(i*i + q*q)) -> float32 of the same shape."""
+    import torch
+    assert x.dtype == torch.complex64 and x.is_cuda and x.is_contiguous()
+    out = torch.empty(x.shape, dtype=torch.float32, device=x.device) if out is None else out
+    _check(lib().csdrb_amdemod_cf(x.data_ptr(), out.data_ptr(), x.numel(), _stream()), "amdemod_cf")
+    return out
+
+
+def fastdcblock_bank_ff(x, block: int = 1024, last_dc=None):
+    """[amdemod_cf |] fastdcblock_ff over the whole blocks of each row: x [C, N] float32 (or complex64: its magnitude is taken first)
+    -> (y [C, (N // block) * block] float32, last_dc [C] float32).  The N % block samples left over are the caller's to carry."""
+    import torch
+    assert x.dtype in (torch.float32, torch.complex64) and x.is_cuda and x.dim() == 2 and x.stride(1) == 1
+    ch, n = x.shape
+    nblocks = n // block
+    out = torch.empty((ch, nblocks * block), dtype=torch.float32, device=x.device)
+    last_dc = torch.zeros(ch, dtype=torch.float32, device=x.device) if last_dc is None else last_dc
+    _check(lib().csdrb_fastdcblock_bank_ff(x.data_ptr(), x.stride(0), int(x.dtype == torch.complex64), out.data_ptr(), out.stride(0), ch, block,
+                                           nblocks, last_dc.data_ptr(), _stream()), "fastdcblock_bank_ff")
+    return out, last_dc
+
+
+def agc_state(channels: int, device="cuda"):
+    """csdrb_agc_state_t [C] at stream start (gain 1, offset 0), as a [C, 5] int32 tensor"""
+    import torch
+    st = torch.zeros((channels, 5), dtype=torch.int32)
+    st[:, 0] = int(np.array([1.0], np.float32).view(np.int32)[0])
+    return st.to(device)
+
+
+def agc_bank_ff(x, params: AgcParams | None = None, state=None, limit_max: float = 0.0, s16: bool = False):
+    """[realpart_cf |] agc_ff [| limit_ff limit_max] [| convert_f_s16] per row: x [C, N] float32 (or complex64: real part)
+    -> (y [C, N] float32 or int16, state).  Cutting a stream into calls of any sizes gives the bits of one call."""
+    import torch
+    assert x.dtype in (torch.float32, torch.complex64) and x.is_cuda and x.dim() == 2 and x.stride(1) == 1
+    ch, n = x.shape
+    params = AgcParams() if params is None else params
+    state = agc_state(ch, x.device) if state is None else state
+    out = torch.empty((ch, n), dtype=torch.int16 if s16 else torch.float32, device=x.device)
+    _check(lib().csdrb_agc_bank_ff(x.data_ptr(), x.stride(0), int(x.dtype == torch.complex64), out.data_ptr(), out.stride(0), int(s16), ch, n,
+                                   C.byref(params), state.data_ptr(), limit_max, _stream()), "agc_bank_ff")
+    return out, state
 
 
 def fft_c2c(x, inverse: bool = False):

@@ -501,6 +501,39 @@ int csdrb_fastagc_bank_f_s16(const float* d_in, long in_stride, short* d_out, lo
     return rc < 0 ? rc : counted(0, rc);
 }
 
+// amdemod_cf (libcsdr.c:861-873) over n samples
+int csdrb_amdemod_cf(const complexf* d_in, float* d_out, long n, void* stream)
+{
+    if (!d_in || !d_out) { set_error("amdemod_cf: null pointer"); return -1; }
+    int rc = launch_amdemod_cf(reinterpret_cast<const float2*>(d_in), d_out, n, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
+// [amdemod_cf |] fastdcblock_ff over whole blocks (libcsdr.c:861-873, 920-941; csdr.c:952-968)
+int csdrb_fastdcblock_bank_ff(const void* d_in, long in_stride, int cf32_in, float* d_out, long out_stride, int channels, int block, int nblocks,
+                              float* d_last_dc_io, void* stream)
+{
+    if (too_many_channels(channels, "fastdcblock bank")) return -1;
+    if (!d_in || !d_out || !d_last_dc_io) { set_error("fastdcblock bank: null pointer"); return -1; }
+    int rc = launch_fastdcblock_bank(d_in, in_stride, cf32_in, d_out, out_stride, channels, block, nblocks, d_last_dc_io, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
+// [realpart_cf |] agc_ff [| limit_ff] [| convert_f_s16] (csdr.c:634-645, 1337-1373; libcsdr_gpl.c:163-260; libcsdr.c:1130-1137, 2390-2398)
+int csdrb_agc_bank_ff(const void* d_in, long in_stride, int cf32_in, void* d_out, long out_stride, int s16_out, int channels, int n,
+                      const csdrb_agc_params_t* params, csdrb_agc_state_t* d_state, float limit_max, void* stream)
+{
+    static_assert(sizeof(csdrb_agc_params_t) == sizeof(AgcParams) && sizeof(csdrb_agc_state_t) == sizeof(AgcState), "AGC structs mirror kernels.h");
+    if (too_many_channels(channels, "agc bank")) return -1;
+    if (!d_in || !d_out || !params || !d_state) { set_error("agc bank: null pointer"); return -1; }
+    AgcParams p;
+    memcpy(&p, params, sizeof p);
+    p.hang_time = (short)p.hang_time;                                   // the reference's parameters are `short` (libcsdr_gpl.h:37)
+    p.attack_wait_time = (short)p.attack_wait_time;
+    int rc = launch_agc_bank(d_in, in_stride, cf32_in, d_out, out_stride, s16_out, channels, n, &p, d_state, limit_max, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
 int csdrb_fft_c2c_batch(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int size, int batch, int inverse, void* stream)
 {
     if (!d_in || !d_out) { set_error("fft: null pointer"); return -1; }
@@ -1208,6 +1241,54 @@ void limit_ff(float* input, float* output, int input_size, float max_amplitude)
     A_CHECK(csdrb_limit_ff((const float*)g_ctx.buf[0], (float*)g_ctx.buf[1], input_size, max_amplitude, g_ctx.stream), who);
     A_DOWN(output, 1, (size_t)input_size * 4, who);
     A_SYNC(who);
+}
+
+void amdemod_cf(complexf* input, float* output, int input_size)
+{
+    const char* who = "amdemod_cf";
+    if (input_size <= 0) return;
+    A_BEGIN(who);
+    A_UP(0, input, (size_t)input_size * 8, who);
+    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 4 + 16), who);
+    A_CHECK(csdrb_amdemod_cf((const complexf*)g_ctx.buf[0], (float*)g_ctx.buf[1], input_size, g_ctx.stream), who);
+    A_DOWN(output, 1, (size_t)input_size * 4, who);
+    A_SYNC(who);
+}
+
+// one call = one block; returns the block's average like libcsdr.c:940 (0 for input_size <= 0, as the reference build does).  input == output is allowed.
+float fastdcblock_ff(float* input, float* output, int input_size, float last_dc_level)
+{
+    const char* who = "fastdcblock_ff";
+    if (input_size <= 0) return 0.f;
+    A_BEGIN(who);
+    A_UP(0, input, (size_t)input_size * 4, who);
+    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 4 + 16), who);
+    A_UP(2, &last_dc_level, sizeof(float), who);
+    A_CHECK(csdrb_fastdcblock_bank_ff(g_ctx.buf[0], input_size, 0, (float*)g_ctx.buf[1], input_size, 1, input_size, 1, (float*)g_ctx.buf[2], g_ctx.stream), who);
+    A_DOWN(output, 1, (size_t)input_size * 4, who);
+    float avg = 0.f;
+    A_CUDA(cudaMemcpyAsync(&avg, g_ctx.buf[2], sizeof avg, cudaMemcpyDeviceToHost, g_ctx.stream), who);
+    A_SYNC(who);
+    return avg;
+}
+
+// one call = one agc_ff call of input_size samples; returns the last gain (libcsdr_gpl.c:259)
+float agc_ff(float* input, float* output, int input_size, float reference, float attack_rate, float decay_rate, float max_gain,
+             short hang_time, short attack_wait_time, float gain_filter_alpha, float last_gain)
+{
+    const char* who = "agc_ff";
+    if (input_size <= 0) return last_gain;
+    A_BEGIN(who);
+    A_UP(0, input, (size_t)input_size * 4, who);
+    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 4 + 16), who);
+    csdrb_agc_state_t st = {last_gain, 0.f, 0, 0, 0};
+    A_UP(2, &st, sizeof st, who);
+    const csdrb_agc_params_t p = {reference, attack_rate, decay_rate, max_gain, hang_time, attack_wait_time, gain_filter_alpha, input_size};
+    A_CHECK(csdrb_agc_bank_ff(g_ctx.buf[0], input_size, 0, g_ctx.buf[1], input_size, 0, 1, input_size, &p, (csdrb_agc_state_t*)g_ctx.buf[2], 0.f, g_ctx.stream), who);
+    A_DOWN(output, 1, (size_t)input_size * 4, who);
+    A_CUDA(cudaMemcpyAsync(&st, g_ctx.buf[2], sizeof st, cudaMemcpyDeviceToHost, g_ctx.stream), who);
+    A_SYNC(who);
+    return st.gain;
 }
 
 float deemphasis_wfm_ff(float* input, float* output, int input_size, float tau, int sample_rate, float last_output)

@@ -67,6 +67,15 @@ int launch_fastagc_bank_s16(const float* d_in, long in_stride, short* d_out, lon
 int launch_fastagc_bank(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int block, int nblocks,
                         float reference, void* d_state, float* d_hist, void* d_scratch, size_t scratch_bytes, cudaStream_t st);
 
+// AM / SSB receiver blocks, agc.cu.  AgcParams / AgcState have the layout of csdrb_agc_params_t / csdrb_agc_state_t (include/csdr_b200.h).
+struct AgcParams { float reference, attack_rate, decay_rate, max_gain; int hang_time, attack_wait_time; float gain_filter_alpha; int chunk; };
+struct AgcState { float gain, last_peak; int hang_counter, attack_wait_counter, offset; };
+int launch_amdemod_cf(const float2* d_in, float* d_out, long n, cudaStream_t st);
+int launch_fastdcblock_bank(const void* d_in, long in_stride, int cf32, float* d_out, long out_stride, int channels, int block, int nblocks,
+                            float* d_last_dc_io, cudaStream_t st);
+int launch_agc_bank(const void* d_in, long in_stride, int cf32, void* d_out, long out_stride, int s16, int channels, int n, const void* h_params_v,
+                    void* d_state_v, float limit_max, cudaStream_t st);   // AgcParams on the host, AgcState[channels] on the device
+
 // K7/K8/K9 fft.cu
 int launch_fft_c2c_batch(const float2* d_in, long in_stride, float2* d_out, long out_stride, int n, int batch, int inverse, cudaStream_t st);
 int launch_olafir_bank(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int fft_size, int input_size,

@@ -1,5 +1,5 @@
 /*
- * bankd.c -- csdr-bankd: a whole bank of FM receivers on ONE wideband IQ stream, in one process.
+ * bankd.c -- csdr-bankd: a whole bank of FM, AM or SSB receivers on ONE wideband IQ stream, in one process.
  *
  * SURVEY.md 8(f) rank 2.  What the reference does with processes -- `nmux` fanning the IQ stream out over TCP (nmux.cpp:246-353)
  * to one `csdr shift_addition_cc | csdr fir_decimate_cc | csdr fmdemod_quadri_cf | ...` chain per listener (ddcd_old.h:51-57,
@@ -13,11 +13,14 @@
  * first -- is process plumbing and is not reproduced; tests/test_gpu_zzz_bankd.py compares against the oracle run over the whole stream).
  *
  * usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]
- *                   [--tail nfm|none] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]  RATE:SINK [RATE:SINK ...]
+ *                   [--tail nfm|none|am|usb|lsb|iq] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]  RATE:SINK [RATE:SINK ...]
+ *   --tail: nfm (default) the README.md:87 tail, s16; none the raw discriminator output, f32; am / usb / lsb the AM and SSB graphs of README.md:95 and :110
+ *   behind the DDC's complex baseband (see bb_tail_t), s16; iq the complex baseband itself, cf32.  --limit is limit_ff's amplitude (default 1), --agc-ref
+ *   the AGC reference (default: fastagc_ff's 1.0 for nfm, agc_ff's 0.2 for am/usb/lsb).
  *   RATE  shift_addition_cc rate (fraction of the wideband sample rate), SINK a path (file or FIFO) or tcp:PORT (one listener).
  *   --devices: the channels are sliced over several GPUs of this node (csdrb_multi_bank_*: the block goes to the first device once and on to
- *   the others by NCCL broadcast), one block of latency more (two blocks are kept in flight); the NFM tail, audio-rate work, runs on the first
- *   device for all channels, through the same kernels as without --devices.
+ *   the others by NCCL broadcast), one block of latency more (two blocks are kept in flight); the audio tail (nfm, am, usb, lsb), audio-rate work, runs on
+ *   the first device for all channels, through the same kernels as without --devices.
  * Sinks never hold the stream up: a sink that cannot take a block within 200 ms loses the rest of that block (counted on stderr at exit), one
  * that fails is dropped -- nmux's policy for slow clients (tsmpool.cpp:101-117, nmux.cpp:339-346).
  */
@@ -216,33 +219,145 @@ static void nfm_tail_push(nfm_tail_t *t, channel_t *chan, int n_new, void *strea
     }
 }
 
-static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *chan, int C, const float *rates, int D, const float *taps, int T, int block,
-                     int nfm, float limit, float agc_ref)
+/* ---- the AM and SSB audio tails (README.md:95, :110) behind the DDC bank's complex baseband ------------------------------------------------------------------
+ *   am      : amdemod_cf | fastdcblock_ff 1024 | agc_ff | limit_ff L | convert_f_s16
+ *   usb/lsb : bandpass_fir_fft_cc 0 0.1 0.05 (or -0.1 0 0.05) | realpart_cf | agc_ff | limit_ff L | convert_f_s16
+ *   iq      : the baseband itself, cf32 (what either tail starts from)
+ * agc_ff runs with the CLI defaults (csdr.c:1342-1361) and its 1024-sample calls; --agc-ref overrides the reference.  Device buffers of ONE device:
+ *   bb   : [C][bs] complexf : [remainder (< unit samples) | new baseband]   unit = 1024 (am) or the overlap-add input size (usb/lsb)
+ *   mid  : [C][bs] float (am: DC-blocked envelope) or complexf (usb/lsb: filtered baseband) over the whole units
+ *   pcm  : [C][whole] s16 */
+#define SSB_BW 0.05f                                      /* bandpass_fir_fft_cc transition bandwidth of README.md:110 */
+enum { TAIL_NFM, TAIL_NONE, TAIL_IQ, TAIL_AM, TAIL_USB, TAIL_LSB };
+
+typedef struct {
+    int kind, C, unit, have, fft_size;
+    long bs;
+    float limit;
+    csdrb_agc_params_t agc;
+    complexf *d_bb, *d_carry, *d_taps_fft, *d_ola_tail;
+    void *d_mid;
+    short *d_pcm;
+    float *d_last_dc;
+    csdrb_agc_state_t *d_agc_state;
+    unsigned char *h_out;
+} bb_tail_t;
+
+static void bb_tail_init(bb_tail_t *t, int kind, int C, int out_cap, float limit, float agc_ref, void *stream)
 {
-    csdrb_multi_bank_t *mb = csdrb_multi_bank_create(ndev, dev, C, rates, D, taps, T, 1, 1024, block);
+    memset(t, 0, sizeof *t);
+    t->kind = kind; t->C = C; t->limit = limit;
+    csdrb_agc_params_t p = {0.2f, 0.01f, 0.0001f, 65536.0f, 200, 0, 0.999f, 1024};
+    if (agc_ref > 0.f) p.reference = agc_ref;
+    t->agc = p;
+    t->unit = 1024;
+    if (kind == TAIL_USB || kind == TAIL_LSB) {                  /* bandpass_fir_fft_cc geometry, csdr.c:1822-1831 */
+        const int T = firdes_filter_len(SSB_BW);
+        int N = next_pow2(T);
+        if (N - T < 200) N <<= 1;
+        t->fft_size = N; t->unit = N - T + 1;
+        complexf *h_taps = calloc((size_t)N, sizeof(complexf));
+        if (!h_taps) die("out of memory");
+        if (kind == TAIL_USB) firdes_bandpass_c(h_taps, T, 0.0f, 0.1f, WINDOW_HAMMING);
+        else firdes_bandpass_c(h_taps, T, -0.1f, 0.0f, WINDOW_HAMMING);
+        complexf *d_taps = csdrb_device_alloc(sizeof(complexf) * (size_t)N);
+        t->d_taps_fft = csdrb_device_alloc(sizeof(complexf) * (size_t)N);
+        t->d_ola_tail = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)N);
+        if (!d_taps || !t->d_taps_fft || !t->d_ola_tail) die("out of memory");
+        OK(csdrb_copy_h2d(d_taps, h_taps, sizeof(complexf) * (size_t)N, stream));
+        OK(csdrb_fft_c2c_batch(d_taps, N, t->d_taps_fft, N, N, 1, 0, stream));       /* the forward FFT of the zero-padded taps (csdr.c:1869) */
+        complexf *zeros = calloc((size_t)C * (size_t)N, sizeof(complexf));   /* the overlap tail is zero at stream start (csdr.c:1860) */
+        if (!zeros) die("out of memory");
+        OK(csdrb_copy_h2d(t->d_ola_tail, zeros, sizeof(complexf) * (size_t)C * (size_t)N, stream));
+        OK(csdrb_stream_synchronize(stream));
+        csdrb_device_free(d_taps); free(h_taps); free(zeros);
+    }
+    t->bs = ((long)t->unit + out_cap + 3) & ~3L;
+    t->d_bb = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->bs);
+    t->d_carry = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->unit);
+    t->d_mid = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->bs);
+    t->d_pcm = csdrb_device_alloc(sizeof(short) * (size_t)C * (size_t)t->bs + 16);
+    t->d_last_dc = csdrb_device_alloc(sizeof(float) * (size_t)C);
+    t->d_agc_state = csdrb_device_alloc(sizeof(csdrb_agc_state_t) * (size_t)C);
+    t->h_out = csdrb_host_alloc((size_t)C * (size_t)t->bs * sizeof(complexf));
+    if (!t->d_bb || !t->d_carry || !t->d_mid || !t->d_pcm || !t->d_last_dc || !t->d_agc_state || !t->h_out) die("out of memory");
+    csdrb_agc_state_t *h_st = calloc((size_t)C, sizeof *h_st);
+    if (!h_st) die("out of memory");
+    for (int c = 0; c < C; c++) h_st[c].gain = 1.0f;                 /* a stream starts at gain 1 (csdr.c:1363) */
+    OK(csdrb_copy_h2d(t->d_agc_state, h_st, sizeof *h_st * (size_t)C, stream));
+    float *h_dc = calloc((size_t)C, sizeof(float));                     /* last_dc_level starts at 0 (csdr.c:957) */
+    if (!h_dc) die("out of memory");
+    OK(csdrb_copy_h2d(t->d_last_dc, h_dc, sizeof(float) * (size_t)C, stream));
+    OK(csdrb_stream_synchronize(stream));
+    free(h_st); free(h_dc);
+}
+
+/* n_new fresh baseband samples per channel sit at d_bb + have: run the tail over the whole units, audio to the sinks, keep the remainder */
+static void bb_tail_push(bb_tail_t *t, channel_t *chan, int n_new, void *stream)
+{
+    const int C = t->C;
+    const long bs = t->bs;
+    const int n = t->have + n_new;
+    if (t->kind == TAIL_IQ) {                                    /* raw baseband: nothing is held back */
+        OK(csdrb_copy2d_d2h(t->h_out, sizeof(complexf) * (size_t)n, t->d_bb, sizeof(complexf) * (size_t)bs, sizeof(complexf) * (size_t)n, (size_t)C, stream));
+        OK(csdrb_stream_synchronize(stream));
+        for (int c = 0; c < C; c++) write_sink(&chan[c], t->h_out + sizeof(complexf) * (size_t)c * (size_t)n, sizeof(complexf) * (size_t)n);
+        return;
+    }
+    const int nb = n / t->unit, whole = nb * t->unit, rest = n - whole;
+    if (nb > 0) {
+        if (t->kind == TAIL_AM) {
+            OK(csdrb_fastdcblock_bank_ff(t->d_bb, bs, 1, (float *)t->d_mid, bs, C, t->unit, nb, t->d_last_dc, stream));
+            OK(csdrb_agc_bank_ff(t->d_mid, bs, 0, t->d_pcm, whole, 1, C, whole, &t->agc, t->d_agc_state, t->limit, stream));
+        } else {
+            OK(csdrb_bandpass_fir_fft_bank_cc(t->d_bb, bs, (complexf *)t->d_mid, bs, C, t->fft_size, t->unit, nb, t->d_taps_fft, 0, t->d_ola_tail, stream));
+            OK(csdrb_agc_bank_ff(t->d_mid, bs, 1, t->d_pcm, whole, 1, C, whole, &t->agc, t->d_agc_state, t->limit, stream));
+        }
+        OK(csdrb_copy_d2h(t->h_out, t->d_pcm, sizeof(short) * (size_t)C * (size_t)whole, stream));
+        if (rest > 0) {
+            OK(csdrb_copy2d_d2d(t->d_carry, sizeof(complexf) * (size_t)t->unit, t->d_bb + whole, sizeof(complexf) * (size_t)bs, sizeof(complexf) * (size_t)rest, (size_t)C, stream));
+            OK(csdrb_copy2d_d2d(t->d_bb, sizeof(complexf) * (size_t)bs, t->d_carry, sizeof(complexf) * (size_t)t->unit, sizeof(complexf) * (size_t)rest, (size_t)C, stream));
+        }
+        OK(csdrb_stream_synchronize(stream));
+        for (int c = 0; c < C; c++) write_sink(&chan[c], t->h_out + sizeof(short) * (size_t)c * (size_t)whole, sizeof(short) * (size_t)whole);
+    } else OK(csdrb_stream_synchronize(stream));
+    t->have = rest;
+}
+
+static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *chan, int C, const float *rates, int D, const float *taps, int T, int block,
+                     int kind, float limit, float agc_ref)
+{
+    const int nfm = kind == TAIL_NFM, demod = kind == TAIL_NFM || kind == TAIL_NONE;
+    const size_t osz = demod ? sizeof(float) : sizeof(complexf);
+    csdrb_multi_bank_t *mb = csdrb_multi_bank_create(ndev, dev, C, rates, D, taps, T, demod, 1024, block);
     if (!mb) die("cannot create the multi-GPU bank");
     const int n_out = (block - T) / D + 1, consumed = n_out * D, keep = block - consumed;
     float lut[256];
     for (int i = 0; i < 256; i++) lut[i] = (float)((float)i / (UCHAR_MAX / 2.0) - 1.0);      /* convert_u8_f, libcsdr.c:2365 */
     complexf *h_wide[2] = {csdrb_host_alloc(sizeof(complexf) * (size_t)block), csdrb_host_alloc(sizeof(complexf) * (size_t)block)};
-    float *h_out[2] = {csdrb_host_alloc(sizeof(float) * (size_t)C * (size_t)n_out), csdrb_host_alloc(sizeof(float) * (size_t)C * (size_t)n_out)};
+    unsigned char *h_out[2] = {csdrb_host_alloc(osz * (size_t)C * (size_t)n_out), csdrb_host_alloc(osz * (size_t)C * (size_t)n_out)};
     unsigned char *raw = malloc((size_t)block * 2);
     if (!h_wide[0] || !h_wide[1] || !h_out[0] || !h_out[1] || !raw) die("out of memory");
     /* --tail nfm: the audio tail is audio-rate work (C x 48 kHz): the discriminator rows every device returned go to the FIRST device once more and through
      * the same kernels as in the single-GPU path */
-    nfm_tail_t tail_state; void *tail_stream = NULL;
-    if (nfm) {
+    nfm_tail_t tail_state; bb_tail_t bb; void *tail_stream = NULL;
+    if (kind != TAIL_NONE) {
         OK(csdrb_set_device(dev[0]));
-        nfm_tail_init(&tail_state, C, n_out + 2, limit, agc_ref);
         tail_stream = csdrb_stream_create();
         if (!tail_stream) die("cannot create a stream");
+        if (nfm) nfm_tail_init(&tail_state, C, n_out + 2, limit, agc_ref);
+        else bb_tail_init(&bb, kind, C, n_out + 2, limit, agc_ref, tail_stream);
     }
 #define EMIT(slot_) do { \
         if (nfm) { \
             OK(csdrb_copy2d_h2d(tail_state.d_demod + tail_state.a_have, sizeof(float) * (size_t)tail_state.ds, h_out[slot_], sizeof(float) * (size_t)n_out, \
                                 sizeof(float) * (size_t)n_out, (size_t)C, tail_stream)); \
             nfm_tail_push(&tail_state, chan, n_out, tail_stream); \
-        } else for (int c = 0; c < C; c++) write_sink(&chan[c], h_out[slot_] + (size_t)c * (size_t)n_out, sizeof(float) * (size_t)n_out); \
+        } else if (!demod) { \
+            OK(csdrb_copy2d_h2d(bb.d_bb + bb.have, sizeof(complexf) * (size_t)bb.bs, h_out[slot_], sizeof(complexf) * (size_t)n_out, \
+                                sizeof(complexf) * (size_t)n_out, (size_t)C, tail_stream)); \
+            bb_tail_push(&bb, chan, n_out, tail_stream); \
+        } else for (int c = 0; c < C; c++) write_sink(&chan[c], h_out[slot_] + osz * (size_t)c * (size_t)n_out, osz * (size_t)n_out); \
     } while (0)
     long blocks = 0;
     int ticket[2] = {-1, -1};
@@ -283,7 +398,7 @@ int main(int argc, char **argv)
 {
     const char *in_spec = "-", *tail = "nfm";
     int u8 = 1, D = 50, block = 1 << 18, device = 0, ndev = 0, devs[64];
-    float bw = 0.005f, limit = 1.0f, agc_ref = 1.0f;
+    float bw = 0.005f, limit = 1.0f, agc_ref = 0.0f;                /* agc_ref 0: the tail's own default (fastagc_ff 1.0, agc_ff 0.2) */
     window_t window = WINDOW_HAMMING;
     channel_t *chan = calloc((size_t)argc, sizeof *chan);
     int C = 0;
@@ -314,13 +429,17 @@ int main(int argc, char **argv)
             chan[C].sink = end + 1; chan[C].fd = -1; chan[C].dropped = 0; C++;
         } else { fprintf(stderr, "csdr-bankd: unknown argument %s\n", o); return 2; }
     }
-    const int nfm = !strcmp(tail, "nfm");
-    if (!nfm && strcmp(tail, "none")) die("--tail is nfm or none");
+    static const char *kTails[] = {"nfm", "none", "iq", "am", "usb", "lsb"};
+    int kind = -1;
+    for (int k = 0; k < 6; k++) if (!strcmp(tail, kTails[k])) kind = k;
+    if (kind < 0) die("--tail is nfm, none, iq, am, usb or lsb");
+    const int nfm = kind == TAIL_NFM, demod = kind == TAIL_NFM || kind == TAIL_NONE;
+    if (nfm && agc_ref == 0.0f) agc_ref = 1.0f;                      /* fastagc_ff's default reference (csdr.c:1388) */
     if (C == 0) die("no channels (RATE:SINK ...)");
     if (block <= 0 || (block & 1)) die("--block must be a positive even number of samples");
     if (D <= 0 || (D & 1)) die("--decimation must be a positive even number (the fused kernels exist for 10 and 50)");
     if (!(bw > 0.f && bw < 0.5f)) die("--bw must be a transition bandwidth between 0 and 0.5");
-    if (!(limit > 0.f) || !(agc_ref > 0.f)) die("--limit and --agc-ref must be positive");
+    if (!(limit > 0.f) || !(agc_ref >= 0.f)) die("--limit and --agc-ref must be positive");
     signal(SIGPIPE, SIG_IGN);
 
     /* ---- filter and bank ---------------------------------------------------------------------------------------------------- */
@@ -335,12 +454,12 @@ int main(int argc, char **argv)
         for (int c = 0; c < C; c++) { chan[c].fd = open_sink(chan[c].sink); sink_nonblocking(chan[c].fd); }
         const int fd = open_input(in_spec);
         fprintf(stderr, "csdr-bankd: %d channels over %d devices, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, ndev, D, T, u8 ? "u8" : "f32", block, tail);
-        const int rc = run_multi(fd, u8, devs, ndev, chan, C, rates, D, taps, T, block, nfm, limit, agc_ref);
+        const int rc = run_multi(fd, u8, devs, ndev, chan, C, rates, D, taps, T, block, kind, limit, agc_ref);
         for (int c = 0; c < C; c++) { if (chan[c].dropped) fprintf(stderr, "csdr-bankd: sink %s lost %ld bytes (too slow)\n", chan[c].sink, chan[c].dropped); if (chan[c].fd >= 0) close(chan[c].fd); }
         return rc;
     }
     OK(csdrb_set_device(device));
-    csdrb_ddc_bank_t *bank = csdrb_ddc_bank_create(C, rates, D, taps, T, 1, 1024);   /* 1024 = the CLI's shift_addition_cc call size (csdr.c:911) */
+    csdrb_ddc_bank_t *bank = csdrb_ddc_bank_create(C, rates, D, taps, T, demod, 1024);   /* 1024 = the CLI's shift_addition_cc call size (csdr.c:911) */
     if (!bank) die("cannot create the bank");
     void *stream = csdrb_stream_create();
     if (!stream) die("cannot create a stream");
@@ -355,15 +474,17 @@ int main(int argc, char **argv)
     unsigned char *d_raw = u8 ? csdrb_device_alloc(in_bytes + 16) : NULL;
     const int out_cap = wide_cap / D + 2;                          /* discriminator samples one block can add */
     nfm_tail_t tl;
+    bb_tail_t bb;
     long ds = ((long)out_cap + 3) & ~3L;
     float *d_demod = NULL;
     unsigned char *h_out = NULL;
     if (nfm) { nfm_tail_init(&tl, C, out_cap, limit, agc_ref); ds = tl.ds; d_demod = tl.d_demod; }
+    else if (!demod) { bb_tail_init(&bb, kind, C, out_cap, limit, agc_ref, stream); ds = bb.bs; d_demod = (float *)bb.d_bb; }
     else {
         d_demod = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)ds);
         h_out = csdrb_host_alloc((size_t)C * (size_t)ds * sizeof(float));
     }
-    if (!h_in || !d_wide[0] || !d_wide[1] || (u8 && !d_raw) || !d_demod || (!nfm && !h_out)) die("out of memory");
+    if (!h_in || !d_wide[0] || !d_wide[1] || (u8 && !d_raw) || !d_demod || (kind == TAIL_NONE && !h_out)) die("out of memory");
 
     /* sinks last: tcp: sinks block until their listener arrives */
     for (int c = 0; c < C; c++) { chan[c].fd = open_sink(chan[c].sink); sink_nonblocking(chan[c].fd); }
@@ -388,15 +509,16 @@ int main(int argc, char **argv)
         const int n_in = block;
 
         /* 2. shift | fir_decimate | fmdemod for every channel, new discriminator samples behind the de-emphasis FIR's carried inputs */
-        const int a_have = nfm ? tl.a_have : 0;
-        const int n_out = csdrb_ddc_bank_process(bank, d_wide[cur], n_in, d_demod + a_have, ds, stream);
+        void *dst = nfm ? (void *)(d_demod + tl.a_have) : !demod ? (void *)(bb.d_bb + bb.have) : (void *)d_demod;
+        const int n_out = csdrb_ddc_bank_process(bank, d_wide[cur], n_in, dst, ds, stream);
         if (n_out < 0) die("csdrb_ddc_bank_process failed");
         const int consumed = n_out * D;
         keep = n_in - consumed;
         OK(csdrb_copy_d2d(d_wide[cur ^ 1], d_wide[cur] + consumed, sizeof(complexf) * (size_t)keep, stream));
         cur ^= 1;
 
-        if (!nfm) {                                                /* raw discriminator output, float */
+        if (!demod) bb_tail_push(&bb, chan, n_out, stream);         /* baseband tails: am / usb / lsb audio, or the raw baseband */
+        else if (!nfm) {                                           /* raw discriminator output, float */
             OK(csdrb_copy2d_d2h(h_out, sizeof(float) * (size_t)n_out, d_demod, sizeof(float) * (size_t)ds, sizeof(float) * (size_t)n_out, (size_t)C, stream));
             OK(csdrb_stream_synchronize(stream));
             for (int c = 0; c < C; c++) write_sink(&chan[c], h_out + sizeof(float) * (size_t)c * (size_t)n_out, sizeof(float) * (size_t)n_out);

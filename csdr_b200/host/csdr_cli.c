@@ -581,6 +581,72 @@ static int cmd_fastagc_ff(int argc, char **argv)
     }
 }
 
+static int cmd_amdemod_cf(int argc, char **argv)                            /* csdr.c:1088-1100 */
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    complexf *in = must_alloc(sizeof(complexf) * (size_t)block); float *out = must_alloc(sizeof(float) * (size_t)block);
+    for (;;) {
+        if (feof(stdin)) return 0;
+        fread(in, sizeof(complexf), (size_t)block, stdin);
+        amdemod_cf(in, out, block);
+        fwrite(out, sizeof(float), (size_t)block, stdout);
+        end_of_block();
+    }
+}
+
+static int cmd_realpart_cf(int argc, char **argv)                           /* csdr.c:634-645: pure I/O, the I of every sample */
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    float *in = must_alloc(sizeof(float) * 2 * (size_t)block), *out = must_alloc(sizeof(float) * (size_t)block);
+    for (;;) {
+        if (feof(stdin)) return 0;
+        fread(in, sizeof(float) * 2, (size_t)block, stdin);
+        for (int i = 0; i < block; i++) out[i] = in[2 * i];
+        fwrite(out, sizeof(float), (size_t)block, stdout);
+        end_of_block();
+    }
+}
+
+static int cmd_fastdcblock_ff(int argc, char **argv)                        /* csdr.c:952-968: its own block size, in place */
+{
+    int size = 1024; if (argc >= 3) sscanf(argv[2], "%d", &size);
+    if (size <= 0) return complain("block size must be positive");
+    incoming_block_size();                                              /* consumes the preamble if there is one (:959) */
+    announce_block(size);
+    float *buf = must_alloc(sizeof(float) * (size_t)size);
+    float last_dc = 0.0f;
+    for (;;) {
+        if (feof(stdin)) return 0;
+        fread(buf, sizeof(float), (size_t)size, stdin);
+        last_dc = fastdcblock_ff(buf, buf, size, last_dc);
+        fwrite(buf, sizeof(float), (size_t)size, stdout);
+        end_of_block();
+    }
+}
+
+static int cmd_agc_ff(int argc, char **argv)                                /* csdr.c:1337-1373: one agc_ff call per block */
+{
+    short hang_time = 200; if (argc >= 3) sscanf(argv[2], "%hd", &hang_time);
+    float reference = 0.2f; if (argc >= 4) sscanf(argv[3], "%g", &reference);
+    float attack_rate = 0.01f; if (argc >= 5) sscanf(argv[4], "%g", &attack_rate);
+    float decay_rate = 0.0001f; if (argc >= 6) sscanf(argv[5], "%g", &decay_rate);
+    float max_gain = 65536.0f; if (argc >= 7) sscanf(argv[6], "%g", &max_gain);
+    short attack_wait = 0; if (argc >= 8) sscanf(argv[7], "%hd", &attack_wait);
+    float filter_alpha = 0.999f; if (argc >= 9) sscanf(argv[8], "%g", &filter_alpha);
+    if (!announce_block(open_block())) return -2;
+    float *in = must_alloc(sizeof(float) * (size_t)block), *out = must_alloc(sizeof(float) * (size_t)block);
+    float last_gain = 1.0f;
+    for (;;) {
+        if (feof(stdin)) return 0;
+        fread(in, sizeof(float), (size_t)block, stdin);
+        last_gain = agc_ff(in, out, block, reference, attack_rate, decay_rate, max_gain, hang_time, attack_wait, filter_alpha, last_gain);
+        fwrite(out, sizeof(float), (size_t)block, stdout);
+        end_of_block();
+    }
+}
+
 static int cmd_bandpass_fir_fft_cc(int argc, char **argv)
 {
     float low_cut = 0, high_cut = 0, transition_bw = 0; window_t window = WINDOW_DEFAULT;
@@ -716,6 +782,10 @@ static const struct { const char *name; int (*run)(int, char **); const char *sy
     {"fractional_decimator_ff", cmd_fractional_decimator_ff, "fractional_decimator_ff <decimation_rate> [num_poly_points ( [transition_bw [window]] | --prefilter )]"},
     {"fastagc_ff", cmd_fastagc_ff, "fastagc_ff [block_size [reference]]"},
     {"limit_ff", cmd_limit_ff, "limit_ff [max_amplitude]"},
+    {"amdemod_cf", cmd_amdemod_cf, "amdemod_cf"},
+    {"realpart_cf", cmd_realpart_cf, "realpart_cf"},
+    {"fastdcblock_ff", cmd_fastdcblock_ff, "fastdcblock_ff [block_size (<= 49152)]"},
+    {"agc_ff", cmd_agc_ff, "agc_ff [hang_time [reference [attack_rate [decay_rate [max_gain [attack_wait [filter_alpha]]]]]]]"},
     {"fft_exchange_sides_ff", cmd_fft_exchange_sides_ff, "fft_exchange_sides_ff <fft_size>"},
     {"compress_fft_adpcm_f_u8", cmd_compress_fft_adpcm_f_u8, "compress_fft_adpcm_f_u8 <fft_size>"},
     {"encode_ima_adpcm_i16_u8", cmd_encode_ima_adpcm, "encode_ima_adpcm_i16_u8"},

@@ -84,6 +84,13 @@ typedef struct fastagc_ff_s {
 } fastagc_ff_t;
 void fastagc_ff(fastagc_ff_t *input, float *output);
 
+/* AM demodulator, DC block and AGC of the AM / SSB graphs (libcsdr.h:98, 116; libcsdr_gpl.h:37; libcsdr.c:861-873, 920-941;
+ * libcsdr_gpl.c:163-260) */
+void  amdemod_cf(complexf *input, float *output, int input_size);
+float fastdcblock_ff(float *input, float *output, int input_size, float last_dc_level);
+float agc_ff(float *input, float *output, int input_size, float reference, float attack_rate, float decay_rate, float max_gain,
+             short hang_time, short attack_wait_time, float gain_filter_alpha, float last_gain);
+
 /* audio tail of the WFM graph, SURVEY 8(f) rank 1 (libcsdr.h:100-105; libcsdr.c:1081-1097, 1130-1137) */
 float deemphasis_wfm_ff(float *input, float *output, int input_size, float tau, int sample_rate, float last_output);
 void  limit_ff(float *input, float *output, int input_size, float max_amplitude);
@@ -335,6 +342,33 @@ int csdrb_fastagc_bank_ff(const float *d_in, long in_stride, float *d_out, long 
 /* fastagc_ff | convert_f_s16 in one pass: d_out is short [channels][out_stride]; everything else as above */
 int csdrb_fastagc_bank_f_s16(const float *d_in, long in_stride, short *d_out, long out_stride, int channels, int block, int nblocks,
                              float reference, csdrb_fastagc_state_t *d_state, float *d_hist, void *d_scratch, size_t scratch_bytes, void *stream);
+
+/* AM / SSB receiver blocks (README.md:95, :110), computed as the reference's -O3 -ffast-math build computes them (DESIGN.md section 7).
+ *
+ * amdemod_cf over n samples (libcsdr.c:861-873): sqrt(i*i + q*q) with the correctly rounded square root. */
+int csdrb_amdemod_cf(const complexf *d_in, float *d_out, long n, void *stream);
+
+/* fastdcblock_ff bank (libcsdr.c:920-941, CLI loop csdr.c:952-968): nblocks whole blocks of `block` samples per channel (the caller
+ * holds any remainder).  cf32_in = 1: d_in is complexf rows and the bank runs amdemod_cf | fastdcblock_ff; 0: d_in is float rows.
+ * Strides count elements of the row's own type.  d_last_dc_io[c] is the reference's last_dc_level (0 at stream start).
+ * A block is staged whole in one CTA's shared memory: block <= 49152 samples (an error beyond; so for the drop-in fastdcblock_ff and the CLI). */
+int csdrb_fastdcblock_bank_ff(const void *d_in, long in_stride, int cf32_in, float *d_out, long out_stride, int channels, int block, int nblocks,
+                              float *d_last_dc_io, void *stream);
+
+/* agc_ff bank (libcsdr_gpl.c:163-260, CLI loop csdr.c:1337-1373): [realpart_cf |] agc_ff [| limit_ff] [| convert_f_s16] over n samples per
+ * channel.  agc_ff restarts every `chunk` samples counted from stream start (the CLI's the_bufsize), so a stream cut into bank calls of
+ * any sizes gives the bits of one long call.  hang_time and attack_wait_time are taken as the reference's `short`.
+ * cf32_in = 1: d_in is complexf rows of which only the real part is read (realpart_cf).  limit_max > 0 applies limit_ff limit_max.
+ * s16_out = 1: d_out is short rows (convert_f_s16), else float rows.  A stream starts at d_state[c] = {1.0f, 0, 0, 0, 0}. */
+typedef struct csdrb_agc_params_s {
+    float reference, attack_rate, decay_rate, max_gain;
+    int hang_time, attack_wait_time;
+    float gain_filter_alpha;
+    int chunk;
+} csdrb_agc_params_t;
+typedef struct csdrb_agc_state_s { float gain, last_peak; int hang_counter, attack_wait_counter, offset; } csdrb_agc_state_t;
+int csdrb_agc_bank_ff(const void *d_in, long in_stride, int cf32_in, void *d_out, long out_stride, int s16_out, int channels, int n,
+                      const csdrb_agc_params_t *params, csdrb_agc_state_t *d_state, float limit_max, void *stream);
 
 /* K7 batched unnormalised c2c DFT (power-of-two size 2..16384), sign -1 forward / +1 inverse */
 int csdrb_fft_c2c_batch(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int size, int batch, int inverse, void *stream);
