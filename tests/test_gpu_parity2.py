@@ -284,6 +284,10 @@ def test_fused_ddc_bank_streams_block_by_block(gpu, oracle):
     consumed = o1.shape[1] * D
     o2, ph2, last2 = gpu.ddc_bank(_dev(wide[consumed:]), rates, D, taps, demod=True, chunk=chunk, offset=consumed % chunk, phases=ph1, last=last1)
     got = np.concatenate([o1.cpu().numpy(), o2.cpu().numpy()], 1)
+    whole, ph_w, last_w = gpu.ddc_bank(_dev(wide), rates, D, taps, demod=True, chunk=chunk)
+    assert np.array_equal(got.view(np.uint32), whole.cpu().numpy().view(np.uint32))          # the split changes no bit (DESIGN.md 8b)
+    assert np.array_equal(ph2.cpu().numpy().view(np.uint32), ph_w.cpu().numpy().view(np.uint32))
+    assert np.array_equal(last2.cpu().numpy().view(np.uint32), last_w.cpu().numpy().view(np.uint32))
     for c, r in enumerate(rates):
         sh, _ = oracle.shift_addition_cc(wide, float(r), 0.0, chunk)
         want = oracle.fmdemod_quadri_cf(oracle.fir_decimate_cc(sh, D, taps))[0]
@@ -326,6 +330,8 @@ def test_ddc_bank_object_streams_with_lookahead(gpu, oracle):
         outs.append(o.cpu().numpy().copy())
         pos += o.shape[1] * D
     got = np.concatenate(outs, 1)
+    whole, _, _ = gpu.ddc_bank(dwide[:pos - D + T], rates, D, taps, demod=True, chunk=chunk)
+    assert np.array_equal(got.view(np.uint32), whole.cpu().numpy().view(np.uint32))          # block sizes and look-ahead change no bit (DESIGN.md 8b)
     for c, r in enumerate(rates):
         sh, _ = oracle.shift_addition_cc(wide[:pos + T], float(r), 0.0, chunk)
         want = oracle.fmdemod_quadri_cf(oracle.fir_decimate_cc(sh, D, taps))[0]
