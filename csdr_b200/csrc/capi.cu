@@ -1,8 +1,7 @@
 // capi.cu -- the C ABI of libcsdr_b200.so (see include/csdr_b200.h).
 //
 // Part B (csdrb_*) entry points are thin: validate, launch on the caller's stream, count the launch.
-// Part A (libcsdr names) wraps Part B for HOST buffers: grow-only device workspace, one private
-// stream, H2D -> kernel(s) -> D2H, synchronous per call -- what a drop-in for a CPU library has to be.
+// Part A (the libcsdr-named drop-ins on host buffers) lives in dropin.cu and calls these.
 #include "common.cuh"
 #include "kernels.h"
 #include "csdr_b200.h"
@@ -31,49 +30,7 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line)
     return -(1000 + (int)e);
 }
 static inline cudaStream_t S(void* s) { return reinterpret_cast<cudaStream_t>(s); }
-static inline int counted(int rc, int n = 1) { if (rc >= 0) g_launches += n; return rc; }
-
-// ---- host-pointer workspace for Part A -----------------------------------------------------------
-struct HostCtx {
-    std::mutex mu;
-    cudaStream_t stream = nullptr;
-    void* buf[4] = {nullptr, nullptr, nullptr, nullptr};
-    size_t cap[4] = {0, 0, 0, 0};
-    bool ready = false;
-    int init()
-    {
-        if (ready) return 0;
-        int n = 0;
-        CSDRB_CUDA(cudaGetDeviceCount(&n));
-        if (n <= 0) { set_error("no CUDA device visible"); return -1; }
-        CSDRB_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-        ready = true;
-        return 0;
-    }
-    int reserve(int slot, size_t bytes)
-    {
-        if (bytes <= cap[slot]) return 0;
-        if (buf[slot]) CSDRB_CUDA(cudaFree(buf[slot]));
-        size_t want = bytes + bytes / 2 + 4096;
-        CSDRB_CUDA(cudaMalloc(&buf[slot], want));
-        cap[slot] = want;
-        return 0;
-    }
-};
-// one workspace per device (a process may csdrb_set_device() between calls): the buffers, like the stream, belong to the device that was
-// current when they were made
-static HostCtx& host_ctx()
-{
-    static std::mutex mu;
-    static std::vector<HostCtx*> per_dev;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0) dev = 0;
-    std::lock_guard<std::mutex> lk(mu);
-    if ((size_t)dev >= per_dev.size()) per_dev.resize((size_t)dev + 1, nullptr);
-    if (!per_dev[(size_t)dev]) per_dev[(size_t)dev] = new HostCtx();
-    return *per_dev[(size_t)dev];
-}
-#define g_ctx (host_ctx())
+int counted(int rc, int n) { if (rc >= 0) g_launches += n; return rc; }
 
 // CSDRB_TRACE=1: report at exit how many kernels this process launched (lets a caller verify that a
 // preloaded/linked libcsdr_b200 really did the work instead of some other libcsdr).
@@ -85,14 +42,6 @@ struct ExitReport {
     }
 };
 static ExitReport g_exit_report;
-
-[[noreturn]] static void die(const char* who)
-{
-    fprintf(stderr, "libcsdr_b200: %s failed: %s\n", who, g_err[0] ? g_err : "(no detail)");
-    abort();
-}
-#define A_CHECK(expr, who) do { if ((expr) < 0) die(who); } while (0)
-#define A_CUDA(call, who) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { cuda_fail(e_, #call, __FILE__, __LINE__); die(who); } } while (0)
 
 }  // namespace csdrb
 
@@ -219,17 +168,6 @@ struct HostBank {
         return 0;
     }
 };
-static HostBank& host_bank()                                     // one per device, like the Part A workspace
-{
-    static std::mutex mu;
-    static std::vector<HostBank*> per_dev;
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0) dev = 0;
-    std::lock_guard<std::mutex> lk(mu);
-    if ((size_t)dev >= per_dev.size()) per_dev.resize((size_t)dev + 1, nullptr);
-    if (!per_dev[(size_t)dev]) per_dev[(size_t)dev] = new HostBank();
-    return *per_dev[(size_t)dev];
-}
 
 // Page-locked memory on the NUMA node the current device hangs off.  cudaHostAlloc places the pages where the calling thread runs; with one
 // process per GPU on a two-socket host half the ranks would otherwise stream their H2D traffic across the socket interconnect.
@@ -282,7 +220,7 @@ static int fir_bank_host(const void* h_in, int in_bytes, long in_stride, complex
     if (!h_in || !h_out || !h_taps || channels <= 0 || decimation <= 0 || taps_length <= 0) { set_error("fir_decimate host bank: bad argument"); return -1; }
     const int n_out = input_size >= taps_length ? (input_size - taps_length) / decimation + 1 : 0;
     if (n_out == 0) return 0;
-    HostBank& hb = host_bank();
+    HostBank& hb = per_device<HostBank>();
     std::lock_guard<std::mutex> lk(hb.mu);
     const long dstride_in = in_bytes == 2 ? (input_size + 7) & ~7L : (input_size + 1) & ~1L, dstride_out = (n_out + 1) & ~1L;
     if (chunk_channels <= 0) {                                 // ~192 MiB of cf32 input (48 MiB of u8) per chunk keeps all three stages busy
@@ -322,91 +260,8 @@ int csdrb_fir_decimate_bank_u8_host(const unsigned char* h_in, long in_stride, c
 }
 
 // =====================================================================================================
-// Part A -- host-pointer drop-ins
-// =====================================================================================================
-void convert_u8_f(unsigned char* input, float* output, int input_size)
-{
-    if (input_size <= 0) return;
-    std::lock_guard<std::mutex> lk(g_ctx.mu);
-    A_CHECK(g_ctx.init(), "convert_u8_f");
-    A_CHECK(g_ctx.reserve(0, (size_t)input_size), "convert_u8_f");
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 4), "convert_u8_f");
-    A_CUDA(cudaMemcpyAsync(g_ctx.buf[0], input, (size_t)input_size, cudaMemcpyHostToDevice, g_ctx.stream), "convert_u8_f");
-    A_CHECK(csdrb_convert_u8_f((const unsigned char*)g_ctx.buf[0], (float*)g_ctx.buf[1], input_size, g_ctx.stream), "convert_u8_f");
-    A_CUDA(cudaMemcpyAsync(output, g_ctx.buf[1], (size_t)input_size * 4, cudaMemcpyDeviceToHost, g_ctx.stream), "convert_u8_f");
-    A_CUDA(cudaStreamSynchronize(g_ctx.stream), "convert_u8_f");
-}
-
-void convert_s16_f(short* input, float* output, int input_size)
-{
-    if (input_size <= 0) return;
-    std::lock_guard<std::mutex> lk(g_ctx.mu);
-    A_CHECK(g_ctx.init(), "convert_s16_f");
-    A_CHECK(g_ctx.reserve(0, (size_t)input_size * 2), "convert_s16_f");
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 4), "convert_s16_f");
-    A_CUDA(cudaMemcpyAsync(g_ctx.buf[0], input, (size_t)input_size * 2, cudaMemcpyHostToDevice, g_ctx.stream), "convert_s16_f");
-    A_CHECK(csdrb_convert_s16_f((const short*)g_ctx.buf[0], (float*)g_ctx.buf[1], input_size, g_ctx.stream), "convert_s16_f");
-    A_CUDA(cudaMemcpyAsync(output, g_ctx.buf[1], (size_t)input_size * 4, cudaMemcpyDeviceToHost, g_ctx.stream), "convert_s16_f");
-    A_CUDA(cudaStreamSynchronize(g_ctx.stream), "convert_s16_f");
-}
-void convert_i16_f(short* input, float* output, int input_size) { convert_s16_f(input, output, input_size); }
-
-void convert_f_s16(float* input, short* output, int input_size)
-{
-    if (input_size <= 0) return;
-    std::lock_guard<std::mutex> lk(g_ctx.mu);
-    A_CHECK(g_ctx.init(), "convert_f_s16");
-    A_CHECK(g_ctx.reserve(0, (size_t)input_size * 4), "convert_f_s16");
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 2), "convert_f_s16");
-    A_CUDA(cudaMemcpyAsync(g_ctx.buf[0], input, (size_t)input_size * 4, cudaMemcpyHostToDevice, g_ctx.stream), "convert_f_s16");
-    A_CHECK(csdrb_convert_f_s16((const float*)g_ctx.buf[0], (short*)g_ctx.buf[1], input_size, g_ctx.stream), "convert_f_s16");
-    A_CUDA(cudaMemcpyAsync(output, g_ctx.buf[1], (size_t)input_size * 2, cudaMemcpyDeviceToHost, g_ctx.stream), "convert_f_s16");
-    A_CUDA(cudaStreamSynchronize(g_ctx.stream), "convert_f_s16");
-}
-void convert_f_i16(float* input, short* output, int input_size) { convert_f_s16(input, output, input_size); }
-
-int fir_decimate_cc(complexf* input, complexf* output, int input_size, int decimation, float* taps, int taps_length)
-{
-    if (input_size < taps_length || input_size <= 0) return 0;
-    std::lock_guard<std::mutex> lk(g_ctx.mu);
-    A_CHECK(g_ctx.init(), "fir_decimate_cc");
-    const int n_out = (input_size - taps_length) / decimation + 1;
-    A_CHECK(g_ctx.reserve(0, (size_t)input_size * 8 + 16), "fir_decimate_cc");
-    A_CHECK(g_ctx.reserve(1, (size_t)n_out * 8 + 16), "fir_decimate_cc");
-    A_CUDA(cudaMemcpyAsync(g_ctx.buf[0], input, (size_t)input_size * 8, cudaMemcpyHostToDevice, g_ctx.stream), "fir_decimate_cc");
-    int rc = csdrb_fir_decimate_bank_cc((const complexf*)g_ctx.buf[0], (input_size + 1) & ~1, (complexf*)g_ctx.buf[1], (n_out + 1) & ~1, 1,
-                                        input_size, decimation, taps, taps_length, -1, g_ctx.stream);
-    A_CHECK(rc, "fir_decimate_cc");
-    A_CUDA(cudaMemcpyAsync(output, g_ctx.buf[1], (size_t)rc * 8, cudaMemcpyDeviceToHost, g_ctx.stream), "fir_decimate_cc");
-    A_CUDA(cudaStreamSynchronize(g_ctx.stream), "fir_decimate_cc");
-    return rc;
-}
-
-complexf fmdemod_quadri_cf(complexf* input, float* output, int input_size, float* temp, complexf last_sample)
-{
-    (void)temp;
-    if (input_size <= 0) return last_sample;
-    std::lock_guard<std::mutex> lk(g_ctx.mu);
-    A_CHECK(g_ctx.init(), "fmdemod_quadri_cf");
-    A_CHECK(g_ctx.reserve(0, (size_t)input_size * 8 + 16), "fmdemod_quadri_cf");
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 4 + 16), "fmdemod_quadri_cf");
-    A_CHECK(g_ctx.reserve(2, 64), "fmdemod_quadri_cf");
-    A_CUDA(cudaMemcpyAsync(g_ctx.buf[0], input, (size_t)input_size * 8, cudaMemcpyHostToDevice, g_ctx.stream), "fmdemod_quadri_cf");
-    A_CUDA(cudaMemcpyAsync(g_ctx.buf[2], &last_sample, 8, cudaMemcpyHostToDevice, g_ctx.stream), "fmdemod_quadri_cf");
-    A_CHECK(csdrb_fmdemod_quadri_bank_cf((const complexf*)g_ctx.buf[0], (input_size + 1) & ~1, (float*)g_ctx.buf[1], (input_size + 1) & ~1, 1,
-                                         input_size, (const complexf*)g_ctx.buf[2], nullptr, g_ctx.stream), "fmdemod_quadri_cf");
-    A_CUDA(cudaMemcpyAsync(output, g_ctx.buf[1], (size_t)input_size * 4, cudaMemcpyDeviceToHost, g_ctx.stream), "fmdemod_quadri_cf");
-    A_CUDA(cudaStreamSynchronize(g_ctx.stream), "fmdemod_quadri_cf");
-    return input[input_size - 1];
-}
-
-}  // extern "C"
-
-// =====================================================================================================
 // Part B, continued: K2, K5-K9
 // =====================================================================================================
-extern "C" {
-
 size_t csdrb_shift_addition_bank_scratch_bytes(int channels, int input_size, int chunk) { return shift_bank_scratch_bytes(channels, input_size, chunk); }
 
 int csdrb_shift_addition_bank_cc(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int input_size,
@@ -940,473 +795,6 @@ int csdrb_ddc_bank_process(csdrb_ddc_bank_t* b, const complexf* d_wide, int inpu
     b->blocks++;
     g_launches += launches;
     return n_out;
-}
-
-// =====================================================================================================
-// Part A, continued: host-pointer drop-ins for shift / fractional decimator / fastagc / FFT / fastddc
-// =====================================================================================================
-#define A_BEGIN(who) std::lock_guard<std::mutex> lk(g_ctx.mu); A_CHECK(g_ctx.init(), who)
-#define A_UP(slot, ptr, bytes, who) do { A_CHECK(g_ctx.reserve(slot, (bytes) + 16), who); \
-    A_CUDA(cudaMemcpyAsync(g_ctx.buf[slot], ptr, bytes, cudaMemcpyHostToDevice, g_ctx.stream), who); } while (0)
-#define A_DOWN(ptr, slot, bytes, who) A_CUDA(cudaMemcpyAsync(ptr, g_ctx.buf[slot], bytes, cudaMemcpyDeviceToHost, g_ctx.stream), who)
-#define A_SYNC(who) A_CUDA(cudaStreamSynchronize(g_ctx.stream), who)
-
-float shift_addition_cc(complexf* input, complexf* output, int input_size, shift_addition_data_t d, float starting_phase)
-{
-    const char* who = "shift_addition_cc";
-    if (input_size <= 0) return starting_phase;      // the reference still wraps the phase; with n = 0 nothing changes unless |phase| > pi
-    A_BEGIN(who);
-    // slot 0: input, 1: output, 2: params(12 B) + phase(4 B) at +64, 3: scratch
-    A_UP(0, input, (size_t)input_size * 8, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 8 + 16), who);
-    struct { shift_addition_data_t p; float pad; float phase; } blob = {d, 0.f, starting_phase};
-    A_UP(2, &blob, sizeof blob, who);
-    const size_t sb = csdrb_shift_addition_bank_scratch_bytes(1, input_size, input_size);
-    A_CHECK(g_ctx.reserve(3, sb + 16), who);
-    float* d_phase = reinterpret_cast<float*>(static_cast<char*>(g_ctx.buf[2]) + offsetof(decltype(blob), phase));
-    A_CHECK(csdrb_shift_addition_bank_cc((const complexf*)g_ctx.buf[0], 0, (complexf*)g_ctx.buf[1], 0, 1, input_size,
-                                         (const shift_addition_data_t*)g_ctx.buf[2], d_phase, input_size, g_ctx.buf[3], g_ctx.cap[3], g_ctx.stream), who);
-    A_DOWN(output, 1, (size_t)input_size * 8, who);
-    float new_phase = 0.f;
-    A_CUDA(cudaMemcpyAsync(&new_phase, d_phase, 4, cudaMemcpyDeviceToHost, g_ctx.stream), who);
-    A_SYNC(who);
-    return new_phase;
-}
-
-float shift_table_cc(complexf* input, complexf* output, int input_size, float rate, shift_table_data_t table_data, float starting_phase)
-{
-    const char* who = "shift_table_cc";
-    if (input_size <= 0 || !table_data.table || table_data.table_size < 2) return starting_phase;
-    A_BEGIN(who);
-    // slot 0: input, 1: output, 2: rate at +0 and phase at +64, 3: scratch.  The table has its own device buffer and is sent with every call
-    // (256 KB for the default size: a host pointer is no proof that the contents are the ones sent last time).
-    static float* d_table = nullptr; static int d_table_cap = 0;
-    A_UP(0, input, (size_t)input_size * 8, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 8 + 16), who);
-    float blob[17] = {0};
-    blob[0] = rate; blob[16] = starting_phase;
-    A_UP(2, blob, sizeof blob, who);
-    float* d_rate = reinterpret_cast<float*>(g_ctx.buf[2]);
-    float* d_phase = d_rate + 16;
-    if (table_data.table_size > d_table_cap) {
-        if (d_table) A_CUDA(cudaFree(d_table), who);
-        d_table = nullptr; d_table_cap = 0;
-        A_CUDA(cudaMalloc(&d_table, (size_t)table_data.table_size * 4), who);
-        d_table_cap = table_data.table_size;
-    }
-    A_CUDA(cudaMemcpyAsync(d_table, table_data.table, (size_t)table_data.table_size * 4, cudaMemcpyHostToDevice, g_ctx.stream), who);
-    const size_t sb = csdrb_shift_math_bank_scratch_bytes(1, input_size);
-    A_CHECK(g_ctx.reserve(3, sb + 16), who);
-    A_CHECK(csdrb_shift_table_bank_cc((const complexf*)g_ctx.buf[0], 0, (complexf*)g_ctx.buf[1], 0, 1, input_size, d_rate, d_phase, d_table, table_data.table_size,
-                                      g_ctx.buf[3], g_ctx.cap[3], g_ctx.stream), who);
-    A_DOWN(output, 1, (size_t)input_size * 8, who);
-    float new_phase = 0.f;
-    A_CUDA(cudaMemcpyAsync(&new_phase, d_phase, 4, cudaMemcpyDeviceToHost, g_ctx.stream), who);
-    A_SYNC(who);
-    return new_phase;
-}
-
-float shift_math_cc(complexf* input, complexf* output, int input_size, float rate, float starting_phase)
-{
-    const char* who = "shift_math_cc";
-    if (input_size <= 0) return starting_phase;
-    A_BEGIN(who);
-    // slot 0: input, 1: output, 2: rate at +0 and phase at +64, 3: scratch
-    A_UP(0, input, (size_t)input_size * 8, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 8 + 16), who);
-    float blob[17] = {0};
-    blob[0] = rate; blob[16] = starting_phase;
-    A_UP(2, blob, sizeof blob, who);
-    const size_t sb = csdrb_shift_math_bank_scratch_bytes(1, input_size);
-    A_CHECK(g_ctx.reserve(3, sb + 16), who);
-    float* d_rate = reinterpret_cast<float*>(g_ctx.buf[2]);
-    float* d_phase = d_rate + 16;
-    A_CHECK(csdrb_shift_math_bank_cc((const complexf*)g_ctx.buf[0], 0, (complexf*)g_ctx.buf[1], 0, 1, input_size, d_rate, d_phase, g_ctx.buf[3], g_ctx.cap[3], g_ctx.stream), who);
-    A_DOWN(output, 1, (size_t)input_size * 8, who);
-    float new_phase = 0.f;
-    A_CUDA(cudaMemcpyAsync(&new_phase, d_phase, 4, cudaMemcpyDeviceToHost, g_ctx.stream), who);
-    A_SYNC(who);
-    return new_phase;
-}
-
-float shift_addfast_cc(complexf* input, complexf* output, int input_size, shift_addfast_data_t* d, float starting_phase)
-{
-    const char* who = "shift_addfast_cc";
-    if (input_size <= 0 || !d) return starting_phase;
-    A_BEGIN(who);
-    // slot 0: input, 1: output, 2: params (36 B) + phase at +64, 3: scratch
-    A_UP(0, input, (size_t)input_size * 8, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 8 + 16), who);
-    struct { shift_addfast_data_t p; float pad[7]; float phase; } blob;
-    blob.p = *d; blob.phase = starting_phase;
-    static_assert(offsetof(decltype(blob), phase) == 64, "phase sits at +64");
-    A_UP(2, &blob, sizeof blob, who);
-    const size_t sb = csdrb_shift_addition_bank_scratch_bytes(1, input_size, input_size);
-    A_CHECK(g_ctx.reserve(3, sb + 16), who);
-    float* d_phase = reinterpret_cast<float*>(static_cast<char*>(g_ctx.buf[2]) + 64);
-    A_CHECK(csdrb_shift_addfast_bank_cc((const complexf*)g_ctx.buf[0], 0, (complexf*)g_ctx.buf[1], 0, 1, input_size,
-                                        (const shift_addfast_data_t*)g_ctx.buf[2], d_phase, input_size, g_ctx.buf[3], g_ctx.cap[3], g_ctx.stream), who);
-    const int whole = input_size & ~3;                                  // the n%4 tail of `output` is left alone, like the reference
-    if (whole > 0) A_DOWN(output, 1, (size_t)whole * 8, who);
-    float new_phase = 0.f;
-    A_CUDA(cudaMemcpyAsync(&new_phase, d_phase, 4, cudaMemcpyDeviceToHost, g_ctx.stream), who);
-    A_SYNC(who);
-    return new_phase;
-}
-
-decimating_shift_addition_status_t decimating_shift_addition_cc(complexf* input, complexf* output, int input_size, shift_addition_data_t d,
-                                                                int decimation, decimating_shift_addition_status_t s)
-{
-    const char* who = "decimating_shift_addition_cc";
-    A_BEGIN(who);
-    if (input_size > 0) A_UP(0, input, (size_t)input_size * 8, who); else A_CHECK(g_ctx.reserve(0, 64), who);
-    const int cap = input_size / (decimation > 0 ? decimation : 1) + 2;
-    A_CHECK(g_ctx.reserve(1, (size_t)cap * 8 + 16), who);
-    struct { shift_addition_data_t p; int remain; float phase; int outsz; } blob = {d, s.decimation_remain, s.starting_phase, 0};
-    A_UP(2, &blob, sizeof blob, who);
-    char* b2 = static_cast<char*>(g_ctx.buf[2]);
-    A_CHECK(csdrb_decimating_shift_addition_bank_cc((const complexf*)g_ctx.buf[0], 0, (complexf*)g_ctx.buf[1], 0, 1, input_size,
-                                                    (const shift_addition_data_t*)b2, decimation, (int*)(b2 + offsetof(decltype(blob), remain)),
-                                                    (float*)(b2 + offsetof(decltype(blob), phase)), (int*)(b2 + offsetof(decltype(blob), outsz)), g_ctx.stream), who);
-    A_CUDA(cudaMemcpyAsync(&blob, b2, sizeof blob, cudaMemcpyDeviceToHost, g_ctx.stream), who);
-    A_SYNC(who);
-    if (blob.outsz > 0) { A_DOWN(output, 1, (size_t)blob.outsz * 8, who); A_SYNC(who); }
-    s.decimation_remain = blob.remain; s.starting_phase = blob.phase; s.output_size = blob.outsz;
-    return s;
-}
-
-fractional_decimator_ff_t fractional_decimator_ff_init(float rate, int num_poly_points, float* taps, int taps_length)
-{
-    // libcsdr.c:715-748 -- same field values; the three scratch arrays are kept so the struct stays layout- and
-    // ownership-compatible with callers that free them.
-    fractional_decimator_ff_t d;
-    d.num_poly_points = num_poly_points & ~1;
-    d.poly_precalc_denomiator = (float*)malloc(sizeof(float) * (size_t)(d.num_poly_points > 0 ? d.num_poly_points : 1));
-    d.xifirst = -(num_poly_points / 2) + 1;
-    d.xilast = num_poly_points / 2;
-    int slot = 0;
-    for (int xi = d.xifirst; xi <= d.xilast && slot < d.num_poly_points; xi++, slot++) {
-        float prod = 1;
-        for (int xj = d.xifirst; xj <= d.xilast; xj++) if (xi != xj) prod *= (float)(xi - xj);
-        d.poly_precalc_denomiator[slot] = prod;
-    }
-    d.where = (float)(-d.xifirst);
-    d.coeffs_buf = (float*)malloc(sizeof(float) * (size_t)(d.num_poly_points > 0 ? d.num_poly_points : 1));
-    d.filtered_buf = (float*)malloc(sizeof(float) * (size_t)(d.num_poly_points > 0 ? d.num_poly_points : 1));
-    d.rate = rate; d.taps = taps; d.taps_length = taps_length; d.input_processed = 0; d.output_size = 0;
-    return d;
-}
-
-void fractional_decimator_ff(float* input, float* output, int input_size, fractional_decimator_ff_t* d)
-{
-    const char* who = "fractional_decimator_ff";
-    if (input_size <= 0) { d->output_size = 0; return; }
-    A_BEGIN(who);
-    A_UP(0, input, (size_t)input_size * 4, who);
-    const int cap = (int)((double)input_size / (d->rate > 1.f ? d->rate : 1.0)) + 8;
-    A_CHECK(g_ctx.reserve(1, (size_t)cap * 4 + 16), who);
-    const int tl = d->taps ? d->taps_length : 0;
-    struct Blob { csdrb_fracdec_state_t st; int pad; } blob = {{d->where, 0, 0}, 0};
-    // slot 2: [state | taps]
-    const size_t tap_off = 64;
-    A_CHECK(g_ctx.reserve(2, tap_off + (size_t)tl * 4 + 16), who);
-    A_CUDA(cudaMemcpyAsync(g_ctx.buf[2], &blob, sizeof blob, cudaMemcpyHostToDevice, g_ctx.stream), who);
-    float* d_taps = nullptr;
-    if (tl > 0) {
-        d_taps = reinterpret_cast<float*>(static_cast<char*>(g_ctx.buf[2]) + tap_off);
-        A_CUDA(cudaMemcpyAsync(d_taps, d->taps, (size_t)tl * 4, cudaMemcpyHostToDevice, g_ctx.stream), who);
-    }
-    const size_t sb = csdrb_fractional_decimator_bank_scratch_bytes(1, input_size, d->rate);
-    A_CHECK(g_ctx.reserve(3, sb + 16), who);
-    A_CHECK(csdrb_fractional_decimator_bank_ff((const float*)g_ctx.buf[0], 0, (float*)g_ctx.buf[1], 0, 1, input_size, d->rate, d->num_poly_points,
-                                               d_taps, tl, (csdrb_fracdec_state_t*)g_ctx.buf[2], g_ctx.buf[3], g_ctx.cap[3], g_ctx.stream), who);
-    A_CUDA(cudaMemcpyAsync(&blob, g_ctx.buf[2], sizeof blob, cudaMemcpyDeviceToHost, g_ctx.stream), who);
-    A_SYNC(who);
-    if (blob.st.output_size > 0) { A_DOWN(output, 1, (size_t)blob.st.output_size * 4, who); A_SYNC(who); }
-    d->where = blob.st.where; d->input_processed = blob.st.input_processed; d->output_size = blob.st.output_size;
-}
-
-void fastagc_ff(fastagc_ff_t* a, float* output)
-{
-    const char* who = "fastagc_ff";
-    const int n = a->input_size;
-    if (n <= 0) return;
-    A_BEGIN(who);
-    A_UP(0, a->buffer_input, (size_t)n * 4, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)n * 4 + 16), who);
-    A_CHECK(g_ctx.reserve(2, (size_t)n * 8 + 64 + 16), who);            // [state 64 B | hist1 | hist2]
-    csdrb_fastagc_state_t st = {a->peak_1, a->peak_2, a->last_gain};
-    char* b2 = static_cast<char*>(g_ctx.buf[2]);
-    A_CUDA(cudaMemcpyAsync(b2, &st, sizeof st, cudaMemcpyHostToDevice, g_ctx.stream), who);
-    A_CUDA(cudaMemcpyAsync(b2 + 64, a->buffer_1, (size_t)n * 4, cudaMemcpyHostToDevice, g_ctx.stream), who);
-    A_CUDA(cudaMemcpyAsync(b2 + 64 + (size_t)n * 4, a->buffer_2, (size_t)n * 4, cudaMemcpyHostToDevice, g_ctx.stream), who);
-    A_CHECK(g_ctx.reserve(3, 256), who);
-    A_CHECK(csdrb_fastagc_bank_ff((const float*)g_ctx.buf[0], 0, (float*)g_ctx.buf[1], 0, 1, n, 1, a->reference, (csdrb_fastagc_state_t*)b2,
-                                  (float*)(b2 + 64), g_ctx.buf[3], g_ctx.cap[3], g_ctx.stream), who);
-    A_DOWN(output, 1, (size_t)n * 4, who);
-    A_CUDA(cudaMemcpyAsync(&st, b2, sizeof st, cudaMemcpyDeviceToHost, g_ctx.stream), who);
-    A_SYNC(who);
-    // rotate the three caller-owned buffers exactly like libcsdr.c:981-989
-    float* recycled = a->buffer_1;
-    a->buffer_1 = a->buffer_2; a->buffer_2 = a->buffer_input; a->buffer_input = recycled;
-    a->peak_1 = st.peak_1; a->peak_2 = st.peak_2; a->last_gain = st.last_gain;
-}
-
-void apply_precalculated_window_c(complexf* input, complexf* output, int size, float* windowt)
-{
-    const char* who = "apply_precalculated_window_c";
-    if (size <= 0) return;
-    A_BEGIN(who);
-    A_UP(0, input, (size_t)size * 8, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)size * 8 + 16), who);
-    A_UP(2, windowt, (size_t)size * 4, who);
-    A_CHECK(csdrb_apply_window_rows_c((const complexf*)g_ctx.buf[0], (complexf*)g_ctx.buf[1], (const float*)g_ctx.buf[2], size, 1, g_ctx.stream), who);
-    A_DOWN(output, 1, (size_t)size * 8, who);
-    A_SYNC(who);
-}
-
-void apply_window_c(complexf* input, complexf* output, int size, window_t window)
-{
-    float* table = precalculate_window(size, window);                    // the table itself is one-off host work, like every filter design step
-    apply_precalculated_window_c(input, output, size, table);
-    free(table);
-}
-
-static void power_dropin(const char* who, const void* in, size_t in_bytes, float* out, int n, float add_db, int mode)
-{
-    if (n <= 0) return;
-    A_BEGIN(who);
-    A_UP(0, in, in_bytes, who);
-    if (mode == 1) A_UP(1, out, (size_t)n * 4, who); else A_CHECK(g_ctx.reserve(1, (size_t)n * 4 + 16), who);
-    int rc = launch_power(mode == 2 ? nullptr : (const float2*)g_ctx.buf[0], mode == 2 ? (const float*)g_ctx.buf[0] : nullptr, (float*)g_ctx.buf[1], n, add_db, mode, g_ctx.stream);
-    A_CHECK(rc, who); counted(0, 1);
-    A_DOWN(out, 1, (size_t)n * 4, who);
-    A_SYNC(who);
-}
-void logpower_cf(complexf* input, float* output, int size, float add_db) { power_dropin("logpower_cf", input, (size_t)(size > 0 ? size : 0) * 8, output, size, add_db, 0); }
-void accumulate_power_cf(complexf* input, float* output, int size) { power_dropin("accumulate_power_cf", input, (size_t)(size > 0 ? size : 0) * 8, output, size, 0.f, 1); }
-void log_ff(float* input, float* output, int size, float add_db) { power_dropin("log_ff", input, (size_t)(size > 0 ? size : 0) * 4, output, size, add_db, 2); }
-
-float shift_unroll_cc(complexf* input, complexf* output, int input_size, shift_unroll_data_t* d, float starting_phase)
-{
-    const char* who = "shift_unroll_cc";
-    if (input_size <= 0) return starting_phase;
-    if (!d || input_size > d->size) { set_error("input_size %d exceeds the table size %d", input_size, d ? d->size : 0); die(who); }
-    A_BEGIN(who);
-    A_UP(0, input, (size_t)input_size * 8, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 8 + 16), who);
-    // slot 2: [starting phase at +16 | dsin at +64 | dcos after it]
-    const size_t tb = (size_t)d->size * 4;
-    A_CHECK(g_ctx.reserve(2, 64 + 2 * tb + 16), who);
-    char* b2 = static_cast<char*>(g_ctx.buf[2]);
-    // one call = one chunk: the phase carried to the next call is one float multiply-add and a wrap -- done right here on the host
-    float new_phase = starting_phase + input_size * d->phase_increment;
-    while (new_phase > 3.14159265358979323846f) new_phase -= 2 * 3.14159265358979323846f;
-    while (new_phase < -3.14159265358979323846f) new_phase += 2 * 3.14159265358979323846f;
-    A_CUDA(cudaMemcpyAsync(b2 + 16, &starting_phase, 4, cudaMemcpyHostToDevice, g_ctx.stream), who);
-    A_CUDA(cudaMemcpyAsync(b2 + 64, d->dsin, tb, cudaMemcpyHostToDevice, g_ctx.stream), who);
-    A_CUDA(cudaMemcpyAsync(b2 + 64 + tb, d->dcos, tb, cudaMemcpyHostToDevice, g_ctx.stream), who);
-    // single call = single chunk: chunk_phase[0] is the starting phase itself
-    shift_unroll_bank_single(reinterpret_cast<const float2*>(g_ctx.buf[0]), reinterpret_cast<float2*>(g_ctx.buf[1]), input_size,
-                             reinterpret_cast<const float*>(b2 + 64), reinterpret_cast<const float*>(b2 + 64 + tb), reinterpret_cast<const float*>(b2 + 16), g_ctx.stream);
-    counted(0, 1);
-    A_DOWN(output, 1, (size_t)input_size * 8, who);
-    A_SYNC(who);
-    return new_phase;
-}
-
-ima_adpcm_state_t encode_ima_adpcm_i16_u8(short* input, unsigned char* output, int input_length, ima_adpcm_state_t state)
-{
-    const char* who = "encode_ima_adpcm_i16_u8";
-    if (input_length < 2) return state;
-    A_BEGIN(who);
-    A_UP(0, input, (size_t)input_length * 2, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)input_length / 2 + 16), who);
-    A_UP(2, &state, sizeof state, who);
-    A_CHECK(csdrb_encode_ima_adpcm_rows_i16_u8((const short*)g_ctx.buf[0], input_length, (unsigned char*)g_ctx.buf[1], input_length / 2, 1, input_length,
-                                               (ima_adpcm_state_t*)g_ctx.buf[2], g_ctx.stream), who);
-    A_DOWN(output, 1, (size_t)(input_length / 2), who);
-    A_CUDA(cudaMemcpyAsync(&state, g_ctx.buf[2], sizeof state, cudaMemcpyDeviceToHost, g_ctx.stream), who);
-    A_SYNC(who);
-    return state;
-}
-
-void limit_ff(float* input, float* output, int input_size, float max_amplitude)
-{
-    const char* who = "limit_ff";
-    if (input_size <= 0) return;
-    A_BEGIN(who);
-    A_UP(0, input, (size_t)input_size * 4, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 4 + 16), who);
-    A_CHECK(csdrb_limit_ff((const float*)g_ctx.buf[0], (float*)g_ctx.buf[1], input_size, max_amplitude, g_ctx.stream), who);
-    A_DOWN(output, 1, (size_t)input_size * 4, who);
-    A_SYNC(who);
-}
-
-void amdemod_cf(complexf* input, float* output, int input_size)
-{
-    const char* who = "amdemod_cf";
-    if (input_size <= 0) return;
-    A_BEGIN(who);
-    A_UP(0, input, (size_t)input_size * 8, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 4 + 16), who);
-    A_CHECK(csdrb_amdemod_cf((const complexf*)g_ctx.buf[0], (float*)g_ctx.buf[1], input_size, g_ctx.stream), who);
-    A_DOWN(output, 1, (size_t)input_size * 4, who);
-    A_SYNC(who);
-}
-
-// one call = one block; returns the block's average like libcsdr.c:940 (0 for input_size <= 0, as the reference build does).  input == output is allowed.
-float fastdcblock_ff(float* input, float* output, int input_size, float last_dc_level)
-{
-    const char* who = "fastdcblock_ff";
-    if (input_size <= 0) return 0.f;
-    A_BEGIN(who);
-    A_UP(0, input, (size_t)input_size * 4, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 4 + 16), who);
-    A_UP(2, &last_dc_level, sizeof(float), who);
-    A_CHECK(csdrb_fastdcblock_bank_ff(g_ctx.buf[0], input_size, 0, (float*)g_ctx.buf[1], input_size, 1, input_size, 1, (float*)g_ctx.buf[2], g_ctx.stream), who);
-    A_DOWN(output, 1, (size_t)input_size * 4, who);
-    float avg = 0.f;
-    A_CUDA(cudaMemcpyAsync(&avg, g_ctx.buf[2], sizeof avg, cudaMemcpyDeviceToHost, g_ctx.stream), who);
-    A_SYNC(who);
-    return avg;
-}
-
-// one call = one agc_ff call of input_size samples; returns the last gain (libcsdr_gpl.c:259)
-float agc_ff(float* input, float* output, int input_size, float reference, float attack_rate, float decay_rate, float max_gain,
-             short hang_time, short attack_wait_time, float gain_filter_alpha, float last_gain)
-{
-    const char* who = "agc_ff";
-    if (input_size <= 0) return last_gain;
-    A_BEGIN(who);
-    A_UP(0, input, (size_t)input_size * 4, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 4 + 16), who);
-    csdrb_agc_state_t st = {last_gain, 0.f, 0, 0, 0};
-    A_UP(2, &st, sizeof st, who);
-    const csdrb_agc_params_t p = {reference, attack_rate, decay_rate, max_gain, hang_time, attack_wait_time, gain_filter_alpha, input_size};
-    A_CHECK(csdrb_agc_bank_ff(g_ctx.buf[0], input_size, 0, g_ctx.buf[1], input_size, 0, 1, input_size, &p, (csdrb_agc_state_t*)g_ctx.buf[2], 0.f, g_ctx.stream), who);
-    A_DOWN(output, 1, (size_t)input_size * 4, who);
-    A_CUDA(cudaMemcpyAsync(&st, g_ctx.buf[2], sizeof st, cudaMemcpyDeviceToHost, g_ctx.stream), who);
-    A_SYNC(who);
-    return st.gain;
-}
-
-float deemphasis_wfm_ff(float* input, float* output, int input_size, float tau, int sample_rate, float last_output)
-{
-    const char* who = "deemphasis_wfm_ff";
-    if (input_size <= 0) return last_output;
-    A_BEGIN(who);
-    A_UP(0, input, (size_t)input_size * 4, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 4 + 16), who);
-    A_UP(2, &last_output, 4, who);
-    A_CHECK(csdrb_deemphasis_wfm_bank_ff((const float*)g_ctx.buf[0], input_size, (float*)g_ctx.buf[1], input_size, 1, input_size, tau, sample_rate,
-                                         (float*)g_ctx.buf[2], g_ctx.stream), who);
-    A_DOWN(output, 1, (size_t)input_size * 4, who);
-    A_SYNC(who);
-    return output[input_size - 1];
-}
-
-int deemphasis_nfm_ff(float* input, float* output, int input_size, int sample_rate)
-{
-    const char* who = "deemphasis_nfm_ff";
-    int taps_length = 0;
-    if (!csdrb_deemphasis_nfm_taps(sample_rate, &taps_length)) return 0;          // libcsdr.c:1119: no table for this rate
-    if (input_size - taps_length <= 0) return 0;
-    A_BEGIN(who);
-    A_UP(0, input, (size_t)input_size * 4, who);
-    A_CHECK(g_ctx.reserve(1, (size_t)input_size * 4 + 16), who);
-    int produced = csdrb_deemphasis_nfm_bank_ff((const float*)g_ctx.buf[0], input_size, (float*)g_ctx.buf[1], input_size, 1, input_size, sample_rate, 0.f, g_ctx.stream);
-    A_CHECK(produced, who);
-    A_DOWN(output, 1, (size_t)produced * 4, who);
-    A_SYNC(who);
-    return produced;
-}
-
-// ---- FFT abstraction ---------------------------------------------------------------------------------
-struct csdrb_plan_impl { unsigned magic; int forward; };
-static const unsigned kPlanMagic = 0xC5D2B200u;
-
-FFT_PLAN_T* make_fft_c2c(int size, complexf* input, complexf* output, int forward, int benchmark)
-{
-    (void)benchmark;
-    if (size < 2 || size > 16384 || (size & (size - 1))) {
-        fprintf(stderr, "libcsdr_b200: make_fft_c2c: size %d unsupported (power of two, 2..16384)\n", size);
-        return nullptr;
-    }
-    FFT_PLAN_T* p = (FFT_PLAN_T*)malloc(sizeof(FFT_PLAN_T));
-    csdrb_plan_impl* impl = (csdrb_plan_impl*)malloc(sizeof(csdrb_plan_impl));
-    impl->magic = kPlanMagic; impl->forward = forward ? 1 : 0;
-    p->size = size; p->input = input; p->output = output; p->plan = impl;
-    return p;
-}
-
-void fft_execute(FFT_PLAN_T* plan)
-{
-    const char* who = "fft_execute";
-    if (!plan) return;
-    if (!plan->plan || ((csdrb_plan_impl*)plan->plan)->magic != kPlanMagic) {
-        set_error("plan was not created by libcsdr_b200's make_fft_c2c (r2c/c2r plans are outside the hot path)"); die(who);
-    }
-    A_BEGIN(who);
-    const size_t bytes = (size_t)plan->size * 8;
-    A_UP(0, plan->input, bytes, who);
-    A_CHECK(g_ctx.reserve(1, bytes + 16), who);
-    A_CHECK(csdrb_fft_c2c_batch((const complexf*)g_ctx.buf[0], plan->size, (complexf*)g_ctx.buf[1], plan->size, plan->size, 1,
-                                ((csdrb_plan_impl*)plan->plan)->forward ? 0 : 1, g_ctx.stream), who);
-    A_DOWN(plan->output, 1, bytes, who);
-    A_SYNC(who);
-}
-
-void fft_destroy(FFT_PLAN_T* plan) { if (plan) { free(plan->plan); free(plan); } }
-void* csdrb_fft_malloc(size_t bytes) { void* p = nullptr; return posix_memalign(&p, 64, bytes ? bytes : 64) ? nullptr : p; }
-void csdrb_fft_free(void* p) { free(p); }
-
-void apply_fir_fft_cc(FFT_PLAN_T* plan, FFT_PLAN_T* plan_inverse, complexf* taps_fft, complexf* last_overlap, int overlap_size)
-{
-    // libcsdr.c:814-849 in one fused kernel: the intermediate spectrum (plan->output) and product (plan_inverse->input)
-    // never leave the GPU, so those two caller buffers are NOT written (no caller in the reference reads them).
-    const char* who = "apply_fir_fft_cc";
-    A_BEGIN(who);
-    const int n = plan->size;
-    const size_t bytes = (size_t)n * 8;
-    A_UP(0, plan->input, bytes, who);
-    A_CHECK(g_ctx.reserve(1, bytes + 16), who);
-    A_UP(2, taps_fft, bytes, who);
-    if (overlap_size > 0) A_UP(3, last_overlap, (size_t)overlap_size * 8, who); else A_CHECK(g_ctx.reserve(3, 64), who);
-    int rc = launch_apply_fir_fft((const float2*)g_ctx.buf[0], (const float2*)g_ctx.buf[2], (const float2*)g_ctx.buf[3], overlap_size, (float2*)g_ctx.buf[1], n, g_ctx.stream);
-    A_CHECK(rc, who); counted(0, 1);
-    A_DOWN(plan_inverse->output, 1, bytes, who);
-    A_SYNC(who);
-}
-
-decimating_shift_addition_status_t fastddc_inv_cc(complexf* input, complexf* output, fastddc_t* ddc, FFT_PLAN_T* plan_inverse, complexf* taps_fft,
-                                                  decimating_shift_addition_status_t shift_stat)
-{
-    const char* who = "fastddc_inv_cc";
-    (void)plan_inverse;
-    {
-        A_BEGIN(who);
-        const size_t nb = (size_t)ddc->fft_size * 8;
-        A_UP(0, input, nb, who);
-        A_UP(2, taps_fft, nb, who);
-        A_CHECK(g_ctx.reserve(1, (size_t)ddc->post_input_size * 8 + 64), who);
-        struct { csdrb_fastddc_chan_t ch; int remain; float phase; int total; } blob =
-            {{ddc->offsetbin, ddc->dsadata.sindelta, ddc->dsadata.cosdelta, ddc->dsadata.rate}, shift_stat.decimation_remain, shift_stat.starting_phase, 0};
-        const size_t sb = csdrb_fastddc_inv_bank_scratch_bytes(1, 1);
-        A_CHECK(g_ctx.reserve(3, 256 + sb), who);
-        char* b3 = static_cast<char*>(g_ctx.buf[3]);
-        A_CUDA(cudaMemcpyAsync(b3, &blob, sizeof blob, cudaMemcpyHostToDevice, g_ctx.stream), who);
-        A_CHECK(csdrb_fastddc_inv_bank_cc((const complexf*)g_ctx.buf[0], 1, (const complexf*)g_ctx.buf[2], (const csdrb_fastddc_chan_t*)b3, 1, ddc,
-                                          (int*)(b3 + offsetof(decltype(blob), remain)), (float*)(b3 + offsetof(decltype(blob), phase)),
-                                          (complexf*)g_ctx.buf[1], ddc->post_input_size, (int*)(b3 + offsetof(decltype(blob), total)),
-                                          b3 + 256, sb, g_ctx.stream), who);
-        A_CUDA(cudaMemcpyAsync(&blob, b3, sizeof blob, cudaMemcpyDeviceToHost, g_ctx.stream), who);
-        A_SYNC(who);
-        if (blob.total > 0) { A_DOWN(output, 1, (size_t)blob.total * 8, who); A_SYNC(who); }
-        shift_stat.decimation_remain = blob.remain; shift_stat.starting_phase = blob.phase; shift_stat.output_size = blob.total;
-    }
-    fft_swap_sides(input, ddc->fft_size);            // the reference leaves its input swapped in place (fastddc.c:123)
-    return shift_stat;
 }
 
 }  // extern "C"

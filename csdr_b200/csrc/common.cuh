@@ -3,6 +3,9 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <mutex>
+#include <vector>
+
 #if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
 #error "csdr_b200 kernels are written for sm_90a (H100) only"
 #endif
@@ -27,6 +30,23 @@ int cuda_fail(cudaError_t e, const char* what, const char* file, int line);
         cudaError_t e_ = (call);                                                          \
         if (e_ != cudaSuccess) return ::csdrb::cuda_fail(e_, #call, __FILE__, __LINE__);  \
     } while (0)
+// adds n to the process's kernel-launch count (csdrb_kernel_launches, CSDRB_TRACE) when rc >= 0; returns rc
+int counted(int rc, int n = 1);
+
+// The T of the current device, created on first use: host-side state whose device buffers and streams belong to one device
+// (a process may csdrb_set_device() between calls).
+template <class T>
+T& per_device()
+{
+    static std::mutex mu;
+    static std::vector<T*> per_dev;
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0) dev = 0;
+    std::lock_guard<std::mutex> lk(mu);
+    if ((size_t)dev >= per_dev.size()) per_dev.resize((size_t)dev + 1, nullptr);
+    if (!per_dev[(size_t)dev]) per_dev[(size_t)dev] = new T();
+    return *per_dev[(size_t)dev];
+}
 
 // The inline-PTX helpers below have C++ models in tests/host_shim/cuda_emul.h (CPU test tier); the product never defines this macro.
 #ifndef CSDRB_HOST_EMULATION

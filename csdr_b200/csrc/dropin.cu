@@ -1,0 +1,528 @@
+// dropin.cu -- Part A of the C ABI of libcsdr_b200.so (see include/csdr_b200.h): the libcsdr-named drop-ins on HOST buffers.
+//
+// Each call stages its buffers through the current device's workspace (grow-only device buffers, one private stream), runs the
+// Part B entry point of capi.cu on them and waits for the result: synchronous per call, what a drop-in for a CPU library has to be.
+#include "common.cuh"
+#include "kernels.h"
+#include "csdr_b200.h"
+
+#include <cstdio>
+#include <cstdlib>
+#include <mutex>
+#include <vector>
+
+namespace csdrb {
+namespace {
+
+[[noreturn]] void die(const char* who)
+{
+    const char* e = csdrb_last_error();
+    fprintf(stderr, "libcsdr_b200: %s failed: %s\n", who, e[0] ? e : "(no detail)");
+    abort();
+}
+
+struct Workspace {
+    struct Buffer { void* p = nullptr; size_t cap = 0; };
+    std::mutex mu;
+    cudaStream_t stream = nullptr;
+    std::vector<Buffer> bufs;
+};
+
+// One drop-in call on the current device's workspace, whose mutex it holds for its lifetime.  The k-th alloc() of a call takes the
+// workspace's k-th buffer.  A drop-in has no error return (the reference's contract), so a failure prints
+// `libcsdr_b200: <who> failed: <detail>` and aborts.
+class Staging {
+public:
+    explicit Staging(const char* who) : who_(who), ws_(per_device<Workspace>()), lock_(ws_.mu)
+    {
+        if (ws_.stream) return;
+        int n = 0;
+        cuda(cudaGetDeviceCount(&n), "cudaGetDeviceCount");
+        if (n <= 0) { set_error("no CUDA device visible"); die(who_); }
+        cuda(cudaStreamCreateWithFlags(&ws_.stream, cudaStreamNonBlocking), "cudaStreamCreateWithFlags");
+    }
+    cudaStream_t stream() const { return ws_.stream; }
+
+    // room for n elements (none for n <= 0) and kSlack bytes more; a buffer that has to grow gets half as much again plus 4 KiB
+    template <class T>
+    T* alloc(long n)
+    {
+        const size_t bytes = (size_t)(n > 0 ? n : 0) * sizeof(T) + kSlack;
+        if (next_ == ws_.bufs.size()) ws_.bufs.emplace_back();
+        Workspace::Buffer& b = ws_.bufs[next_++];
+        if (bytes > b.cap) {
+            if (b.p) cuda(cudaFree(b.p), "cudaFree");
+            b = {};
+            cuda(cudaMalloc(&b.p, bytes + bytes / 2 + 4096), "cudaMalloc");
+            b.cap = bytes + bytes / 2 + 4096;
+        }
+        return static_cast<T*>(b.p);
+    }
+    // copies of n <= 0 elements are skipped
+    template <class T>
+    void put(T* dev, const T* host, long n)
+    {
+        if (n > 0) cuda(cudaMemcpyAsync(dev, host, (size_t)n * sizeof(T), cudaMemcpyHostToDevice, ws_.stream), "cudaMemcpyAsync to the device");
+    }
+    template <class T>
+    T* up(const T* host, long n)
+    {
+        T* dev = alloc<T>(n);
+        put(dev, host, n);
+        return dev;
+    }
+    template <class T>
+    void get(T* host, const T* dev, long n)
+    {
+        if (n > 0) cuda(cudaMemcpyAsync(host, dev, (size_t)n * sizeof(T), cudaMemcpyDeviceToHost, ws_.stream), "cudaMemcpyAsync to the host");
+    }
+    int check(int rc) const
+    {
+        if (rc < 0) die(who_);
+        return rc;
+    }
+    void sync() const { cuda(cudaStreamSynchronize(ws_.stream), "cudaStreamSynchronize"); }
+
+private:
+    static constexpr size_t kSlack = 64;            // kernels may read whole vectors past the last element
+    void cuda(cudaError_t e, const char* what) const
+    {
+        if (e == cudaSuccess) return;
+        cuda_fail(e, what, __FILE__, __LINE__);
+        die(who_);
+    }
+    const char* who_;
+    Workspace& ws_;
+    std::lock_guard<std::mutex> lock_;
+    size_t next_ = 0;
+};
+
+// the drop-ins that turn n input elements into n output elements with one Part B call f(d_in, d_out, n, stream)
+template <class In, class Out, class F>
+void elementwise(const char* who, const In* input, Out* output, int n, F f)
+{
+    if (n <= 0) return;
+    Staging st(who);
+    const In* d_in = st.up(input, n);
+    Out* d_out = st.alloc<Out>(n);
+    st.check(f(d_in, d_out, n, st.stream()));
+    st.get(output, d_out, n);
+    st.sync();
+}
+
+struct csdrb_plan_impl { unsigned magic; int forward; };
+const unsigned kPlanMagic = 0xC5D2B200u;
+
+}  // namespace
+}  // namespace csdrb
+
+using namespace csdrb;
+
+extern "C" {
+
+void convert_u8_f(unsigned char* input, float* output, int input_size) { elementwise("convert_u8_f", input, output, input_size, csdrb_convert_u8_f); }
+void convert_s16_f(short* input, float* output, int input_size) { elementwise("convert_s16_f", input, output, input_size, csdrb_convert_s16_f); }
+void convert_i16_f(short* input, float* output, int input_size) { convert_s16_f(input, output, input_size); }
+void convert_f_s16(float* input, short* output, int input_size) { elementwise("convert_f_s16", input, output, input_size, csdrb_convert_f_s16); }
+void convert_f_i16(float* input, short* output, int input_size) { convert_f_s16(input, output, input_size); }
+
+int fir_decimate_cc(complexf* input, complexf* output, int input_size, int decimation, float* taps, int taps_length)
+{
+    if (input_size < taps_length || input_size <= 0) return 0;
+    Staging st("fir_decimate_cc");
+    const int n_out = (input_size - taps_length) / decimation + 1;
+    const complexf* d_in = st.up(input, input_size);
+    complexf* d_out = st.alloc<complexf>(n_out);
+    const int rc = st.check(csdrb_fir_decimate_bank_cc(d_in, (input_size + 1) & ~1, d_out, (n_out + 1) & ~1, 1, input_size, decimation, taps, taps_length, -1,
+                                                       st.stream()));
+    st.get(output, d_out, rc);
+    st.sync();
+    return rc;
+}
+
+complexf fmdemod_quadri_cf(complexf* input, float* output, int input_size, float* temp, complexf last_sample)
+{
+    (void)temp;
+    if (input_size <= 0) return last_sample;
+    Staging st("fmdemod_quadri_cf");
+    const complexf* d_in = st.up(input, input_size);
+    const complexf* d_last = st.up(&last_sample, 1);
+    float* d_out = st.alloc<float>(input_size);
+    st.check(csdrb_fmdemod_quadri_bank_cf(d_in, (input_size + 1) & ~1, d_out, (input_size + 1) & ~1, 1, input_size, d_last, nullptr, st.stream()));
+    st.get(output, d_out, input_size);
+    st.sync();
+    return input[input_size - 1];
+}
+
+// ---- shift / fractional decimator / fastagc ----------------------------------------------------------
+float shift_addition_cc(complexf* input, complexf* output, int input_size, shift_addition_data_t d, float starting_phase)
+{
+    if (input_size <= 0) return starting_phase;      // the reference still wraps the phase; with n = 0 nothing changes unless |phase| > pi
+    Staging st("shift_addition_cc");
+    struct State { shift_addition_data_t params; float phase; } s = {d, starting_phase};
+    State* d_s = st.up(&s, 1);
+    const complexf* d_in = st.up(input, input_size);
+    complexf* d_out = st.alloc<complexf>(input_size);
+    const size_t sb = csdrb_shift_addition_bank_scratch_bytes(1, input_size, input_size);
+    void* scratch = st.alloc<char>(sb);
+    st.check(csdrb_shift_addition_bank_cc(d_in, 0, d_out, 0, 1, input_size, &d_s->params, &d_s->phase, input_size, scratch, sb, st.stream()));
+    st.get(output, d_out, input_size);
+    st.get(&s.phase, &d_s->phase, 1);
+    st.sync();
+    return s.phase;
+}
+
+float shift_table_cc(complexf* input, complexf* output, int input_size, float rate, shift_table_data_t table_data, float starting_phase)
+{
+    if (input_size <= 0 || !table_data.table || table_data.table_size < 2) return starting_phase;
+    Staging st("shift_table_cc");
+    struct State { float rate, phase; } s = {rate, starting_phase};
+    State* d_s = st.up(&s, 1);
+    const complexf* d_in = st.up(input, input_size);
+    complexf* d_out = st.alloc<complexf>(input_size);
+    // the table is sent with every call (256 KB for the default size): a host pointer is no proof that the contents are the ones sent last time
+    const float* d_table = st.up(table_data.table, table_data.table_size);
+    const size_t sb = csdrb_shift_math_bank_scratch_bytes(1, input_size);
+    void* scratch = st.alloc<char>(sb);
+    st.check(csdrb_shift_table_bank_cc(d_in, 0, d_out, 0, 1, input_size, &d_s->rate, &d_s->phase, d_table, table_data.table_size, scratch, sb, st.stream()));
+    st.get(output, d_out, input_size);
+    st.get(&s.phase, &d_s->phase, 1);
+    st.sync();
+    return s.phase;
+}
+
+float shift_math_cc(complexf* input, complexf* output, int input_size, float rate, float starting_phase)
+{
+    if (input_size <= 0) return starting_phase;
+    Staging st("shift_math_cc");
+    struct State { float rate, phase; } s = {rate, starting_phase};
+    State* d_s = st.up(&s, 1);
+    const complexf* d_in = st.up(input, input_size);
+    complexf* d_out = st.alloc<complexf>(input_size);
+    const size_t sb = csdrb_shift_math_bank_scratch_bytes(1, input_size);
+    void* scratch = st.alloc<char>(sb);
+    st.check(csdrb_shift_math_bank_cc(d_in, 0, d_out, 0, 1, input_size, &d_s->rate, &d_s->phase, scratch, sb, st.stream()));
+    st.get(output, d_out, input_size);
+    st.get(&s.phase, &d_s->phase, 1);
+    st.sync();
+    return s.phase;
+}
+
+float shift_addfast_cc(complexf* input, complexf* output, int input_size, shift_addfast_data_t* d, float starting_phase)
+{
+    if (input_size <= 0 || !d) return starting_phase;
+    Staging st("shift_addfast_cc");
+    struct State { shift_addfast_data_t params; float phase; } s = {*d, starting_phase};
+    State* d_s = st.up(&s, 1);
+    const complexf* d_in = st.up(input, input_size);
+    complexf* d_out = st.alloc<complexf>(input_size);
+    const size_t sb = csdrb_shift_addition_bank_scratch_bytes(1, input_size, input_size);
+    void* scratch = st.alloc<char>(sb);
+    st.check(csdrb_shift_addfast_bank_cc(d_in, 0, d_out, 0, 1, input_size, &d_s->params, &d_s->phase, input_size, scratch, sb, st.stream()));
+    st.get(output, d_out, input_size & ~3);                             // the n%4 tail of `output` is left alone, like the reference
+    st.get(&s.phase, &d_s->phase, 1);
+    st.sync();
+    return s.phase;
+}
+
+decimating_shift_addition_status_t decimating_shift_addition_cc(complexf* input, complexf* output, int input_size, shift_addition_data_t d,
+                                                                int decimation, decimating_shift_addition_status_t s)
+{
+    Staging st("decimating_shift_addition_cc");
+    struct State { shift_addition_data_t params; int remain; float phase; int output_size; } h = {d, s.decimation_remain, s.starting_phase, 0};
+    State* d_h = st.up(&h, 1);
+    const complexf* d_in = st.up(input, input_size);
+    complexf* d_out = st.alloc<complexf>(input_size / (decimation > 0 ? decimation : 1) + 2);
+    st.check(csdrb_decimating_shift_addition_bank_cc(d_in, 0, d_out, 0, 1, input_size, &d_h->params, decimation, &d_h->remain, &d_h->phase,
+                                                     &d_h->output_size, st.stream()));
+    st.get(&h, d_h, 1);
+    st.sync();
+    if (h.output_size > 0) { st.get(output, d_out, h.output_size); st.sync(); }
+    s.decimation_remain = h.remain; s.starting_phase = h.phase; s.output_size = h.output_size;
+    return s;
+}
+
+fractional_decimator_ff_t fractional_decimator_ff_init(float rate, int num_poly_points, float* taps, int taps_length)
+{
+    // libcsdr.c:715-748 -- same field values; the three scratch arrays are kept so the struct stays layout- and
+    // ownership-compatible with callers that free them.
+    fractional_decimator_ff_t d;
+    d.num_poly_points = num_poly_points & ~1;
+    d.poly_precalc_denomiator = (float*)malloc(sizeof(float) * (size_t)(d.num_poly_points > 0 ? d.num_poly_points : 1));
+    d.xifirst = -(num_poly_points / 2) + 1;
+    d.xilast = num_poly_points / 2;
+    int slot = 0;
+    for (int xi = d.xifirst; xi <= d.xilast && slot < d.num_poly_points; xi++, slot++) {
+        float prod = 1;
+        for (int xj = d.xifirst; xj <= d.xilast; xj++) if (xi != xj) prod *= (float)(xi - xj);
+        d.poly_precalc_denomiator[slot] = prod;
+    }
+    d.where = (float)(-d.xifirst);
+    d.coeffs_buf = (float*)malloc(sizeof(float) * (size_t)(d.num_poly_points > 0 ? d.num_poly_points : 1));
+    d.filtered_buf = (float*)malloc(sizeof(float) * (size_t)(d.num_poly_points > 0 ? d.num_poly_points : 1));
+    d.rate = rate; d.taps = taps; d.taps_length = taps_length; d.input_processed = 0; d.output_size = 0;
+    return d;
+}
+
+void fractional_decimator_ff(float* input, float* output, int input_size, fractional_decimator_ff_t* d)
+{
+    if (input_size <= 0) { d->output_size = 0; return; }
+    Staging st("fractional_decimator_ff");
+    csdrb_fracdec_state_t s = {d->where, 0, 0};
+    csdrb_fracdec_state_t* d_s = st.up(&s, 1);
+    const float* d_in = st.up(input, input_size);
+    float* d_out = st.alloc<float>((int)((double)input_size / (d->rate > 1.f ? d->rate : 1.0)) + 8);
+    const int tl = d->taps ? d->taps_length : 0;
+    const float* d_taps = tl > 0 ? st.up(d->taps, tl) : nullptr;
+    const size_t sb = csdrb_fractional_decimator_bank_scratch_bytes(1, input_size, d->rate);
+    void* scratch = st.alloc<char>(sb);
+    st.check(csdrb_fractional_decimator_bank_ff(d_in, 0, d_out, 0, 1, input_size, d->rate, d->num_poly_points, d_taps, tl, d_s, scratch, sb, st.stream()));
+    st.get(&s, d_s, 1);
+    st.sync();
+    if (s.output_size > 0) { st.get(output, d_out, s.output_size); st.sync(); }
+    d->where = s.where; d->input_processed = s.input_processed; d->output_size = s.output_size;
+}
+
+void fastagc_ff(fastagc_ff_t* a, float* output)
+{
+    const int n = a->input_size;
+    if (n <= 0) return;
+    Staging st("fastagc_ff");
+    csdrb_fastagc_state_t s = {a->peak_1, a->peak_2, a->last_gain};
+    csdrb_fastagc_state_t* d_s = st.up(&s, 1);
+    const float* d_in = st.up(a->buffer_input, n);
+    float* d_hist = st.alloc<float>(2L * n);                            // the two previous blocks, buffer_1 first
+    st.put(d_hist, a->buffer_1, n);
+    st.put(d_hist + n, a->buffer_2, n);
+    float* d_out = st.alloc<float>(n);
+    const size_t sb = csdrb_fastagc_bank_scratch_bytes(1, 1);
+    void* scratch = st.alloc<char>(sb);
+    st.check(csdrb_fastagc_bank_ff(d_in, 0, d_out, 0, 1, n, 1, a->reference, d_s, d_hist, scratch, sb, st.stream()));
+    st.get(output, d_out, n);
+    st.get(&s, d_s, 1);
+    st.sync();
+    // rotate the three caller-owned buffers exactly like libcsdr.c:981-989
+    float* recycled = a->buffer_1;
+    a->buffer_1 = a->buffer_2; a->buffer_2 = a->buffer_input; a->buffer_input = recycled;
+    a->peak_1 = s.peak_1; a->peak_2 = s.peak_2; a->last_gain = s.last_gain;
+}
+
+// ---- spectrum, shift_unroll, ADPCM ------------------------------------------------------------------
+void apply_precalculated_window_c(complexf* input, complexf* output, int size, float* windowt)
+{
+    if (size <= 0) return;
+    Staging st("apply_precalculated_window_c");
+    const complexf* d_in = st.up(input, size);
+    const float* d_window = st.up(windowt, size);
+    complexf* d_out = st.alloc<complexf>(size);
+    st.check(csdrb_apply_window_rows_c(d_in, d_out, d_window, size, 1, st.stream()));
+    st.get(output, d_out, size);
+    st.sync();
+}
+
+void apply_window_c(complexf* input, complexf* output, int size, window_t window)
+{
+    float* table = precalculate_window(size, window);                    // the table itself is one-off host work, like every filter design step
+    apply_precalculated_window_c(input, output, size, table);
+    free(table);
+}
+
+void logpower_cf(complexf* input, float* output, int size, float add_db)
+{
+    elementwise("logpower_cf", input, output, size, [=](const complexf* in, float* out, long n, void* s) { return csdrb_logpower_cf(in, out, n, add_db, s); });
+}
+
+void accumulate_power_cf(complexf* input, float* output, int size)
+{
+    if (size <= 0) return;
+    Staging st("accumulate_power_cf");
+    const complexf* d_in = st.up(input, size);
+    float* d_acc = st.up(output, size);
+    st.check(csdrb_accumulate_power_cf(d_in, d_acc, size, st.stream()));
+    st.get(output, d_acc, size);
+    st.sync();
+}
+
+void log_ff(float* input, float* output, int size, float add_db)
+{
+    elementwise("log_ff", input, output, size, [=](const float* in, float* out, long n, void* s) { return csdrb_log_ff(in, out, n, add_db, s); });
+}
+
+float shift_unroll_cc(complexf* input, complexf* output, int input_size, shift_unroll_data_t* d, float starting_phase)
+{
+    const char* who = "shift_unroll_cc";
+    if (input_size <= 0) return starting_phase;
+    if (!d || input_size > d->size) { set_error("input_size %d exceeds the table size %d", input_size, d ? d->size : 0); die(who); }
+    Staging st(who);
+    const complexf* d_in = st.up(input, input_size);
+    const float* d_phase = st.up(&starting_phase, 1);                    // single call = single chunk: chunk_phase[0] is the starting phase itself
+    const float* d_dsin = st.up(d->dsin, d->size);
+    const float* d_dcos = st.up(d->dcos, d->size);
+    complexf* d_out = st.alloc<complexf>(input_size);
+    shift_unroll_bank_single(reinterpret_cast<const float2*>(d_in), reinterpret_cast<float2*>(d_out), input_size, d_dsin, d_dcos, d_phase, st.stream());
+    counted(0, 1);
+    st.get(output, d_out, input_size);
+    st.sync();
+    // one call = one chunk: the phase carried to the next call is one float multiply-add and a wrap -- done right here on the host
+    float new_phase = starting_phase + input_size * d->phase_increment;
+    while (new_phase > 3.14159265358979323846f) new_phase -= 2 * 3.14159265358979323846f;
+    while (new_phase < -3.14159265358979323846f) new_phase += 2 * 3.14159265358979323846f;
+    return new_phase;
+}
+
+ima_adpcm_state_t encode_ima_adpcm_i16_u8(short* input, unsigned char* output, int input_length, ima_adpcm_state_t state)
+{
+    if (input_length < 2) return state;
+    Staging st("encode_ima_adpcm_i16_u8");
+    const short* d_in = st.up(input, input_length);
+    ima_adpcm_state_t* d_state = st.up(&state, 1);
+    unsigned char* d_out = st.alloc<unsigned char>(input_length / 2);
+    st.check(csdrb_encode_ima_adpcm_rows_i16_u8(d_in, input_length, d_out, input_length / 2, 1, input_length, d_state, st.stream()));
+    st.get(output, d_out, input_length / 2);
+    st.get(&state, d_state, 1);
+    st.sync();
+    return state;
+}
+
+// ---- audio tail, AM / SSB --------------------------------------------------------------------------
+void limit_ff(float* input, float* output, int input_size, float max_amplitude)
+{
+    elementwise("limit_ff", input, output, input_size, [=](const float* in, float* out, long n, void* s) { return csdrb_limit_ff(in, out, n, max_amplitude, s); });
+}
+
+void amdemod_cf(complexf* input, float* output, int input_size) { elementwise("amdemod_cf", input, output, input_size, csdrb_amdemod_cf); }
+
+// one call = one block; returns the block's average like libcsdr.c:940 (0 for input_size <= 0, as the reference build does).  input == output is allowed.
+float fastdcblock_ff(float* input, float* output, int input_size, float last_dc_level)
+{
+    if (input_size <= 0) return 0.f;
+    Staging st("fastdcblock_ff");
+    const float* d_in = st.up(input, input_size);
+    float* d_dc = st.up(&last_dc_level, 1);                              // in: the previous block's average; out: this block's
+    float* d_out = st.alloc<float>(input_size);
+    st.check(csdrb_fastdcblock_bank_ff(d_in, input_size, 0, d_out, input_size, 1, input_size, 1, d_dc, st.stream()));
+    st.get(output, d_out, input_size);
+    float avg = 0.f;
+    st.get(&avg, d_dc, 1);
+    st.sync();
+    return avg;
+}
+
+// one call = one agc_ff call of input_size samples; returns the last gain (libcsdr_gpl.c:259)
+float agc_ff(float* input, float* output, int input_size, float reference, float attack_rate, float decay_rate, float max_gain,
+             short hang_time, short attack_wait_time, float gain_filter_alpha, float last_gain)
+{
+    if (input_size <= 0) return last_gain;
+    Staging st("agc_ff");
+    const float* d_in = st.up(input, input_size);
+    csdrb_agc_state_t s = {last_gain, 0.f, 0, 0, 0};
+    csdrb_agc_state_t* d_s = st.up(&s, 1);
+    float* d_out = st.alloc<float>(input_size);
+    const csdrb_agc_params_t p = {reference, attack_rate, decay_rate, max_gain, hang_time, attack_wait_time, gain_filter_alpha, input_size};
+    st.check(csdrb_agc_bank_ff(d_in, input_size, 0, d_out, input_size, 0, 1, input_size, &p, d_s, 0.f, st.stream()));
+    st.get(output, d_out, input_size);
+    st.get(&s, d_s, 1);
+    st.sync();
+    return s.gain;
+}
+
+float deemphasis_wfm_ff(float* input, float* output, int input_size, float tau, int sample_rate, float last_output)
+{
+    if (input_size <= 0) return last_output;
+    Staging st("deemphasis_wfm_ff");
+    const float* d_in = st.up(input, input_size);
+    float* d_last = st.up(&last_output, 1);
+    float* d_out = st.alloc<float>(input_size);
+    st.check(csdrb_deemphasis_wfm_bank_ff(d_in, input_size, d_out, input_size, 1, input_size, tau, sample_rate, d_last, st.stream()));
+    st.get(output, d_out, input_size);
+    st.sync();
+    return output[input_size - 1];
+}
+
+int deemphasis_nfm_ff(float* input, float* output, int input_size, int sample_rate)
+{
+    int taps_length = 0;
+    if (!csdrb_deemphasis_nfm_taps(sample_rate, &taps_length)) return 0;          // libcsdr.c:1119: no table for this rate
+    if (input_size - taps_length <= 0) return 0;
+    Staging st("deemphasis_nfm_ff");
+    const float* d_in = st.up(input, input_size);
+    float* d_out = st.alloc<float>(input_size);
+    const int produced = st.check(csdrb_deemphasis_nfm_bank_ff(d_in, input_size, d_out, input_size, 1, input_size, sample_rate, 0.f, st.stream()));
+    st.get(output, d_out, produced);
+    st.sync();
+    return produced;
+}
+
+// ---- FFT abstraction, overlap-add step, fastddc ---------------------------------------------------------
+FFT_PLAN_T* make_fft_c2c(int size, complexf* input, complexf* output, int forward, int benchmark)
+{
+    (void)benchmark;
+    if (size < 2 || size > 16384 || (size & (size - 1))) {
+        fprintf(stderr, "libcsdr_b200: make_fft_c2c: size %d unsupported (power of two, 2..16384)\n", size);
+        return nullptr;
+    }
+    FFT_PLAN_T* p = (FFT_PLAN_T*)malloc(sizeof(FFT_PLAN_T));
+    csdrb_plan_impl* impl = (csdrb_plan_impl*)malloc(sizeof(csdrb_plan_impl));
+    impl->magic = kPlanMagic; impl->forward = forward ? 1 : 0;
+    p->size = size; p->input = input; p->output = output; p->plan = impl;
+    return p;
+}
+
+void fft_execute(FFT_PLAN_T* plan)
+{
+    const char* who = "fft_execute";
+    if (!plan) return;
+    if (!plan->plan || ((csdrb_plan_impl*)plan->plan)->magic != kPlanMagic) {
+        set_error("plan was not created by libcsdr_b200's make_fft_c2c (r2c/c2r plans are outside the hot path)"); die(who);
+    }
+    const int inverse = ((csdrb_plan_impl*)plan->plan)->forward ? 0 : 1;
+    elementwise(who, static_cast<const complexf*>(plan->input), static_cast<complexf*>(plan->output), plan->size,
+                [=](const complexf* in, complexf* out, long n, void* s) { return csdrb_fft_c2c_batch(in, n, out, n, (int)n, 1, inverse, s); });
+}
+
+void fft_destroy(FFT_PLAN_T* plan) { if (plan) { free(plan->plan); free(plan); } }
+void* csdrb_fft_malloc(size_t bytes) { void* p = nullptr; return posix_memalign(&p, 64, bytes ? bytes : 64) ? nullptr : p; }
+void csdrb_fft_free(void* p) { free(p); }
+
+void apply_fir_fft_cc(FFT_PLAN_T* plan, FFT_PLAN_T* plan_inverse, complexf* taps_fft, complexf* last_overlap, int overlap_size)
+{
+    // libcsdr.c:814-849 in one fused kernel: the intermediate spectrum (plan->output) and product (plan_inverse->input)
+    // never leave the GPU, so those two caller buffers are NOT written (no caller in the reference reads them).
+    Staging st("apply_fir_fft_cc");
+    const int n = plan->size;
+    const complexf* d_in = st.up(static_cast<const complexf*>(plan->input), n);
+    const complexf* d_taps = st.up(taps_fft, n);
+    const complexf* d_overlap = st.up(last_overlap, overlap_size);
+    complexf* d_out = st.alloc<complexf>(n);
+    st.check(counted(launch_apply_fir_fft(reinterpret_cast<const float2*>(d_in), reinterpret_cast<const float2*>(d_taps), reinterpret_cast<const float2*>(d_overlap),
+                                          overlap_size, reinterpret_cast<float2*>(d_out), n, st.stream())));
+    st.get(static_cast<complexf*>(plan_inverse->output), d_out, n);
+    st.sync();
+}
+
+decimating_shift_addition_status_t fastddc_inv_cc(complexf* input, complexf* output, fastddc_t* ddc, FFT_PLAN_T* plan_inverse, complexf* taps_fft,
+                                                  decimating_shift_addition_status_t shift_stat)
+{
+    (void)plan_inverse;
+    {
+        Staging st("fastddc_inv_cc");
+        struct State { csdrb_fastddc_chan_t chan; int remain; float phase; int total; } s =
+            {{ddc->offsetbin, ddc->dsadata.sindelta, ddc->dsadata.cosdelta, ddc->dsadata.rate}, shift_stat.decimation_remain, shift_stat.starting_phase, 0};
+        State* d_s = st.up(&s, 1);
+        const complexf* d_in = st.up(input, ddc->fft_size);
+        const complexf* d_taps = st.up(taps_fft, ddc->fft_size);
+        complexf* d_out = st.alloc<complexf>(ddc->post_input_size);
+        const size_t sb = csdrb_fastddc_inv_bank_scratch_bytes(1, 1);
+        void* scratch = st.alloc<char>(sb);
+        st.check(csdrb_fastddc_inv_bank_cc(d_in, 1, d_taps, &d_s->chan, 1, ddc, &d_s->remain, &d_s->phase, d_out, ddc->post_input_size, &d_s->total,
+                                           scratch, sb, st.stream()));
+        st.get(&s, d_s, 1);
+        st.sync();
+        if (s.total > 0) { st.get(output, d_out, s.total); st.sync(); }
+        shift_stat.decimation_remain = s.remain; shift_stat.starting_phase = s.phase; shift_stat.output_size = s.total;
+    }
+    fft_swap_sides(input, ddc->fft_size);            // the reference leaves its input swapped in place (fastddc.c:123), once the workspace is released
+    return shift_stat;
+}
+
+}  // extern "C"

@@ -137,8 +137,8 @@ using std::min;
 
 def build_full(out_dir: Path):
     """Every product translation unit (kernels, launchers, csrc/capi.cu, host C) compiled for the host under cuda_emul.h and linked into
-    ONE shared library that exports the product's C ABI, so host-side code on top of the ABI (the csdr CLI, Part A's workspace and
-    streaming logic in capi.cu) runs in the CPU tier.  Returns (library path, CLI path).  Test artefacts only -- built into a temporary
+    ONE shared library that exports the product's C ABI, so host-side code on top of the ABI (the csdr CLI, Part A's workspace in dropin.cu,
+    the streaming logic in capi.cu) runs in the CPU tier.  Returns (library path, CLI path).  Test artefacts only -- built into a temporary
     directory, never installed next to the product."""
     from concurrent.futures import ThreadPoolExecutor
     out_dir.mkdir(exist_ok=True)

@@ -1,4 +1,4 @@
-"""CPU tier: the product's C ABI layer (csrc/capi.cu) and its `csdr` CLI (host/csdr_cli.c) on top of the EMULATED kernels.
+"""CPU tier: the product's C ABI layer (csrc/capi.cu, csrc/dropin.cu) and its `csdr` CLI (host/csdr_cli.c) on top of the EMULATED kernels.
 
 tests/host_shim/emul_build.build_full() compiles every product translation unit for the host under tests/host_shim/cuda_emul.h into one
 library with the product's real C ABI and links the unmodified CLI source against it.  The pipe-graph tests of tests/test_gpu_cli.py

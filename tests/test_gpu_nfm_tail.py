@@ -45,11 +45,14 @@ def test_deemphasis_nfm_dropin_golden_and_oracle(gpu, oracle, rate):
             assert _rel(y, want) < 1e-6, n
 
 
-def test_deemphasis_nfm_degenerate_calls(gpu):
+def test_deemphasis_nfm_dropin_degenerate_calls(gpu):
     x = np.ones(4096, np.float32)
     assert gpu.libcsdr.deemphasis_nfm_ff(x, 12345).size == 0            # no table for this rate -> 0 samples processed (libcsdr.c:1119)
     assert gpu.libcsdr.deemphasis_nfm_ff(x[:201], 48000).size == 0      # input_size == taps_length -> the reference loop does not run
     assert gpu.libcsdr.deemphasis_nfm_ff(x[:100], 48000).size == 0
+
+
+def test_deemphasis_nfm_degenerate_calls(gpu):
     d = torch.ones((3, 4096), dtype=torch.float32, device="cuda")
     assert gpu.deemphasis_nfm_bank_ff(d, 22050).shape == (3, 0)
 

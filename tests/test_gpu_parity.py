@@ -46,6 +46,10 @@ def test_convert_u8_f_bit_exact(gpu, oracle):
     y = gpu.convert_u8_f(_dev(x)).cpu().numpy()
     assert np.array_equal(y, oracle.convert_u8_f(x))
     assert np.array_equal(y[:256], GOLD["u8_out"])
+
+
+def test_convert_u8_f_dropin_bit_exact(gpu, oracle):
+    x = np.concatenate([np.arange(256, dtype=np.uint8), np.random.default_rng(0).integers(0, 256, 2_000_003).astype(np.uint8)])
     # host-pointer drop-in, odd sizes
     for n in (1, 15, 16, 17, 1024, 4099):
         assert np.array_equal(gpu.libcsdr.convert_u8_f(x[:n]), oracle.convert_u8_f(x[:n]))
@@ -54,10 +58,13 @@ def test_convert_u8_f_bit_exact(gpu, oracle):
 def test_convert_s16_both_ways_bit_exact(gpu, oracle):
     s = np.arange(-32768, 32768).astype(np.int16)
     assert np.array_equal(gpu.convert_s16_f(_dev(s)).cpu().numpy(), oracle.convert_s16_f(s))
-    assert np.array_equal(gpu.libcsdr.convert_s16_f(GOLD["s16_in"]), GOLD["s16_out"])
     f = np.concatenate([GOLD["f_in"], np.random.default_rng(1).uniform(-1, 1, 1_000_001).astype(np.float32),
                         np.array([3e9, -3e9, np.nan, np.inf, -np.inf, 1.00001, -1.00001], np.float32)])
     assert np.array_equal(gpu.convert_f_s16(_dev(f)).cpu().numpy(), oracle.convert_f_s16(f))
+
+
+def test_convert_s16_dropin_both_ways_bit_exact(gpu, oracle):
+    assert np.array_equal(gpu.libcsdr.convert_s16_f(GOLD["s16_in"]), GOLD["s16_out"])
     assert np.array_equal(gpu.libcsdr.convert_f_s16(GOLD["f_in"]), GOLD["f_s16_out"])
 
 
@@ -75,28 +82,43 @@ def test_fir_bank_headline_shape_vs_oracle(gpu, oracle, variant):
         assert _rel(y[c], oracle.fir_decimate_cc(x[c], D, taps)) < 1e-6, c
 
 
-@pytest.mark.parametrize("T,D,N", [(79, 10, 16384), (199, 10, 16384), (199, 10, 199), (199, 10, 198), (199, 10, 208), (199, 10, 209),
-                                   (79, 7, 5000), (801, 50, 70000), (33, 3, 1001), (5, 1, 64), (200, 10, 30011), (123, 10, 9999)])
+FIR_EDGES = [(79, 10, 16384), (199, 10, 16384), (199, 10, 199), (199, 10, 198), (199, 10, 208), (199, 10, 209),
+             (79, 7, 5000), (801, 50, 70000), (33, 3, 1001), (5, 1, 64), (200, 10, 30011), (123, 10, 9999)]
+
+
+@pytest.mark.parametrize("T,D,N", FIR_EDGES)
 def test_fir_bank_edge_geometries(gpu, oracle, T, D, N):
     taps = np.random.default_rng(T).uniform(-1, 1, T).astype(np.float32) / T
     x = np.stack([_cplx(np.random.default_rng(100 + c), N) for c in range(3)])
     n_out = (N - T) // D + 1 if N >= T else 0
     if n_out == 0:
         assert gpu.fir_out_len(N, D, T) == 0
-        assert gpu.libcsdr.fir_decimate_cc(x[0], D, taps).size == 0
         return
     y = gpu.fir_decimate_bank_cc(_dev(x), D, taps).cpu().numpy()
     assert y.shape == (3, n_out)
     for c in range(3):
         assert _rel(y[c], oracle.fir_decimate_cc(x[c], D, taps)) < 2e-6
+
+
+@pytest.mark.parametrize("T,D,N", FIR_EDGES)
+def test_fir_dropin_edge_geometries(gpu, oracle, T, D, N):
+    taps = np.random.default_rng(T).uniform(-1, 1, T).astype(np.float32) / T
+    x = np.stack([_cplx(np.random.default_rng(100 + c), N) for c in range(3)])
+    n_out = (N - T) // D + 1 if N >= T else 0
+    if n_out == 0:
+        assert gpu.libcsdr.fir_decimate_cc(x[0], D, taps).size == 0
+        return
     # host-pointer drop-in on one channel
     assert _rel(gpu.libcsdr.fir_decimate_cc(x[1], D, taps), oracle.fir_decimate_cc(x[1], D, taps)) < 2e-6
 
 
-def test_fir_golden_and_reference(gpu, ref):
+def test_fir_dropin_golden(gpu, ref):
     for key, taps in (("fir_out_79_d10", "lowpass_79"), ("fir_out_199_d10", "lowpass_199")):
         y = gpu.libcsdr.fir_decimate_cc(GOLD["fir_in"], 10, GOLD[taps])
         assert y.size == GOLD[key].size and _rel(y, GOLD[key]) < NORTH_STAR_TOL / 5
+
+
+def test_fir_golden_and_reference(gpu, ref):
     x = _cplx(np.random.default_rng(5), 262144)
     taps = ref.firdes_lowpass_f(199, 0.05)
     y = gpu.fir_decimate_bank_cc(_dev(x[None, :]), 10, taps).cpu().numpy()[0]
@@ -145,5 +167,8 @@ def test_fmdemod_quadri(gpu, oracle):
         assert _rel(y[c], want) < 1e-6 and np.complex64(wl) == lo[c]
         assert np.abs(y[c] - want).max() <= 2e-7 * max(1.0, np.abs(want).max())
     assert not y[2, 101:110].any()
+
+
+def test_fmdemod_quadri_dropin(gpu, oracle):
     yg, lg = gpu.libcsdr.fmdemod_quadri_cf(GOLD["fm_in"], 0.25 - 0.5j)
     assert _rel(yg, GOLD["fm_out"]) < 1e-6 and np.complex64(lg) == GOLD["fm_last"]

@@ -83,12 +83,15 @@ def test_fractional_decimator_positions_are_exact(gpu, oracle, rate, pts, block)
     assert np.array_equal(got, want)                                                # same IEEE operation order -> bit exact vs the strict oracle
 
 
-def test_fractional_decimator_bank_prefilter_and_golden(gpu, oracle):
+def test_fractional_decimator_dropin_prefilter_and_golden(gpu, oracle):
     got = gpu.libcsdr.fractional_decimator_ff(GOLD["fd_in"], 5.0, 12, None, 1024)
     assert got.size == GOLD["fd_out_r5_blk1024"].size and _rel(got, GOLD["fd_out_r5_blk1024"]) < 1e-6
     taps = oracle.firdes_lowpass_f(31, 0.15)
     got = gpu.libcsdr.fractional_decimator_ff(GOLD["fd_in"][:3000], 3.0, 4, taps, None)
     assert got.size == GOLD["fd_out_r3_pts4_prefilter"].size and _rel(got, GOLD["fd_out_r3_pts4_prefilter"]) < 1e-6
+
+
+def test_fractional_decimator_bank_prefilter_and_golden(gpu, oracle):
     x = np.stack([np.random.default_rng(c).uniform(-1, 1, 30_000).astype(np.float32) for c in range(5)])
     y, state = gpu.fractional_decimator_bank_ff(_dev(x), 5.0, 12)
     y = y.cpu().numpy(); state = state.cpu().numpy()
@@ -98,9 +101,12 @@ def test_fractional_decimator_bank_prefilter_and_golden(gpu, oracle):
 
 
 # ------------------------------------------------------------------------------------------ K6
-def test_fastagc(gpu, oracle):
+def test_fastagc_dropin(gpu, oracle):
     assert _rel(gpu.libcsdr.fastagc_ff(GOLD["agc_in"], 256, 1.0), GOLD["agc_out_b256"]) < 1e-7
     assert _rel(gpu.libcsdr.fastagc_ff(GOLD["agc_in"], 512, 0.5), GOLD["agc_out_b512_ref0p5"]) < 1e-7
+
+
+def test_fastagc(gpu, oracle):
     rng = np.random.default_rng(4)
     env = np.repeat(rng.uniform(0.001, 1.0, 40).astype(np.float32), 1024)
     x = np.stack([rng.uniform(-1, 1, env.size).astype(np.float32) * env * s for s in (1.0, 0.01, 0.0, 30.0)])
@@ -122,7 +128,10 @@ def test_fastagc(gpu, oracle):
 
 
 # ------------------------------------------------------------------------------------------ K7
-@pytest.mark.parametrize("n", [2, 4, 8, 16, 32, 64, 128, 256, 512, 1024, 2048, 4096, 8192, 16384])
+FFT_SIZES = [2, 4, 8, 16, 32, 64, 128, 256, 512, 1024, 2048, 4096, 8192, 16384]
+
+
+@pytest.mark.parametrize("n", FFT_SIZES)
 def test_fft_all_sizes_vs_float64_dft(gpu, n):
     rng = np.random.default_rng(n)
     x = _cplx(rng, 3 * n).reshape(3, n)
@@ -130,6 +139,12 @@ def test_fft_all_sizes_vs_float64_dft(gpu, n):
         y = gpu.fft_c2c(_dev(x), inverse=inv).cpu().numpy()
         want = np.fft.ifft(x.astype(np.complex128), axis=1) * n if inv else np.fft.fft(x.astype(np.complex128), axis=1)
         assert _rel(y, want) < 1e-6, (n, inv)                                       # ~1e-7*log2(n) from the exact DFT
+
+
+@pytest.mark.parametrize("n", FFT_SIZES)
+def test_fft_dropin_all_sizes_vs_float64_dft(gpu, n):
+    rng = np.random.default_rng(n)
+    x = _cplx(rng, 3 * n).reshape(3, n)
     a = gpu.libcsdr.dft(x[0], True)
     assert _rel(a, np.fft.fft(x[0].astype(np.complex128))) < 1e-6
 
@@ -164,12 +179,15 @@ def test_bandpass_fir_fft_bank(gpu, oracle, bw, lo, hi, nblocks):
 
 
 # ------------------------------------------------------------------------------------------ K8
+def test_fastddc_dropin_golden(gpu):
+    y = gpu.libcsdr.fastddc_inv(list(GOLD["ddc_fwd_out"]), 0.05, 8, 0.123)
+    assert y.size == GOLD["ddc_inv_out"].size and _rel(y, GOLD["ddc_inv_out"]) < TOL / 2
+
+
 def test_fastddc_golden(gpu):
     ddc = gpu.fastddc_init(0.05, 8, 0.123)
     sp, _ = gpu.fastddc_fwd_cc(_dev(GOLD["ddc_in"]), ddc)
     assert _rel(sp.cpu().numpy(), GOLD["ddc_fwd_out"]) < 1e-6
-    y = gpu.libcsdr.fastddc_inv(list(GOLD["ddc_fwd_out"]), 0.05, 8, 0.123)
-    assert y.size == GOLD["ddc_inv_out"].size and _rel(y, GOLD["ddc_inv_out"]) < TOL / 2
     out, counts, _ = gpu.fastddc_inv_bank_cc(sp, [0.123], 8, 0.05)
     n = int(counts[0].item())
     assert n == GOLD["ddc_inv_out"].size and _rel(out[0, :n].cpu().numpy(), GOLD["ddc_inv_out"]) < TOL / 2
@@ -295,13 +313,16 @@ def test_fused_ddc_bank_streams_block_by_block(gpu, oracle):
 
 
 # ------------------------------------------------------------------------------------------ audio tail (8f rank 1)
+def test_audio_tail_dropin_limit_and_deemphasis(gpu, oracle):
+    assert np.array_equal(gpu.libcsdr.limit_ff(GOLD["deemph_in"], 1.0), GOLD["limit_out"])
+    y, last = gpu.libcsdr.deemphasis_wfm_ff(GOLD["deemph_in"], 50e-6, 48000, 0.0, 1024)
+    assert np.array_equal(y, GOLD["deemph_out_50us_48k"]) and np.float32(last) == GOLD["deemph_last"]     # same rounding sequence: bit exact
+
+
 def test_audio_tail_limit_and_deemphasis(gpu, oracle):
     x = np.random.default_rng(31).uniform(-2, 2, 200_003).astype(np.float32)
     x[7] = np.nan; x[9] = np.inf; x[11] = -np.inf
     assert np.array_equal(gpu.limit_ff(_dev(x), 0.7).cpu().numpy(), oracle.limit_ff(x, 0.7))
-    assert np.array_equal(gpu.libcsdr.limit_ff(GOLD["deemph_in"], 1.0), GOLD["limit_out"])
-    y, last = gpu.libcsdr.deemphasis_wfm_ff(GOLD["deemph_in"], 50e-6, 48000, 0.0, 1024)
-    assert np.array_equal(y, GOLD["deemph_out_50us_48k"]) and np.float32(last) == GOLD["deemph_last"]     # same rounding sequence: bit exact
     xb = np.stack([np.random.default_rng(c).uniform(-1, 1, 50_001).astype(np.float32) for c in range(37)])
     lasts = np.linspace(-0.5, 0.5, 37).astype(np.float32); lasts[3] = np.nan
     yb, lb = gpu.deemphasis_wfm_bank_ff(_dev(xb), 75e-6, 240000, last=_dev(lasts))
@@ -340,12 +361,17 @@ def test_ddc_bank_object_streams_with_lookahead(gpu, oracle):
 
 
 # ------------------------------------------------------------------------------------------ spectrum path + shift_unroll (8f ranks 3, 4)
-def test_spectrum_path_and_shift_unroll(gpu, oracle):
+def test_spectrum_path_and_shift_unroll_dropins(gpu, oracle):
     assert np.array_equal(gpu.libcsdr.precalculate_window(1024, "HAMMING"), oracle.precalculate_window(1024, "HAMMING"))
     x = GOLD["spec_in"]
     assert np.abs(gpu.libcsdr.logpower_cf(x, -70.0) - GOLD["logpower_out"]).max() < 2e-5
     assert np.abs(gpu.libcsdr.logaveragepower_cf(x, -70.0, 512, 4) - GOLD["logavg_out"]).max() < 2e-5
     assert np.array_equal(gpu.libcsdr.apply_window_c(x[:1024], "BLACKMAN"), oracle.apply_precalculated_window_c(x[:1024], oracle.precalculate_window(1024, "BLACKMAN")))
+    y, ph = gpu.libcsdr.shift_unroll_cc(GOLD["shift_in"], -0.085, 0.0, 1024)
+    assert _rel(y, GOLD["unroll_out"]) < 1e-7 and np.float32(ph) == GOLD["unroll_phase"]
+
+
+def test_spectrum_path_and_shift_unroll(gpu, oracle):
     # whole-stream spectrum on the device vs window -> float64 DFT -> logpower on the CPU
     big = _cplx(np.random.default_rng(41), 64 * 2048, 0.5)
     db = gpu.spectrum_logpower(_dev(big), 2048, "HAMMING", -30.0).cpu().numpy()
@@ -353,8 +379,6 @@ def test_spectrum_path_and_shift_unroll(gpu, oracle):
     for f in (0, 31, 63):
         want = oracle.logpower_cf(oracle.dft(oracle.apply_precalculated_window_c(big[f * 2048:(f + 1) * 2048], w)), -30.0)
         assert np.abs(db[f] - want).max() < 1e-3                                      # dB: FFT rounding (1e-7 relative) on bins far below the peak
-    y, ph = gpu.libcsdr.shift_unroll_cc(GOLD["shift_in"], -0.085, 0.0, 1024)
-    assert _rel(y, GOLD["unroll_out"]) < 1e-7 and np.float32(ph) == GOLD["unroll_phase"]
     xs = _cplx(np.random.default_rng(42), 20_000)
     rates = [0.2, -0.4999, 0.0123]
     yb, pb = gpu.shift_unroll_bank_cc(_dev(xs), rates)

@@ -36,6 +36,12 @@ def test_adpcm_rows_and_waterfall_lines_bit_exact(gpu, oracle):
         db = rng.uniform(-130, 10, (rows, fft_size)).astype(np.float32); db[0, :3] = [np.nan, 400.0, -400.0]
         got = gpu.compress_fft_adpcm_rows_f_u8(torch.from_numpy(db).cuda()).cpu().numpy()
         assert np.array_equal(got, oracle.compress_fft_adpcm_f_u8(db, fft_size)), fft_size
+
+
+def test_adpcm_dropin_bit_exact(gpu, oracle):
+    rng = np.random.default_rng(4)
+    rows, n = 300, 2050
+    x = (rng.standard_normal((rows, n)) * rng.choice([10, 300, 5000, 40000], (rows, 1))).clip(-32768, 32767).astype(np.int16)
     y, st = gpu.libcsdr.encode_ima_adpcm_i16_u8(x[0], 5, 1000)
     want, wst = oracle.encode_ima_adpcm_i16_u8(x[0], 5, 1000)
     assert np.array_equal(y, want) and st == wst

@@ -30,9 +30,12 @@ def _rel(y, ref):
     return rel_rms(y, ref)
 
 
-def test_shift_math_dropin_and_bank(gpu, oracle):
+def test_shift_math_dropin(gpu, oracle):
     y, ph = gpu.libcsdr.shift_math_cc(GOLD["shift_in"], -0.085, -7.5, 1024)
     assert np.float32(ph) == GOLD["math_phase"] and _rel(y, GOLD["math_out"]) < 1e-6
+
+
+def test_shift_math_bank(gpu, oracle):
     rng = np.random.default_rng(3)
     rates = np.array([-0.5, -0.31, -0.085, 0.0, 1e-4, 0.2, 0.4999, 0.5], np.float32)
     ph0 = np.array([0.0, 3.0, -7.5, 100.0, 6.2831855, 1.0, 2.0, -0.0], np.float32)

@@ -23,7 +23,7 @@ def gpu():
     return csdr_b200
 
 
-def test_shift_table_bank_and_dropin_bit_exact(gpu, oracle):
+def test_shift_table_bank_bit_exact(gpu, oracle):
     rng = np.random.default_rng(21)
     rates = np.array([-0.5, -0.31, -0.085, 0.0, 1e-4, 0.2, 0.4999, 0.5], np.float32)
     ph0 = np.array([0.0, 3.0, 1.5707964, 6.2831855, 0.5, 1.0, 2.0, 4.7], np.float32)
@@ -36,6 +36,10 @@ def test_shift_table_bank_and_dropin_bit_exact(gpu, oracle):
             want, wph, _bad = oracle.shift_table_cc(x, float(r), table, float(ph0[c]))
             assert np.float32(wph).view(np.uint32) == ph[c].view(np.uint32), (n, c)
             assert np.array_equal(out[c], want), (n, size, c, int(np.sum(out[c] != want)))
+
+
+def test_shift_table_dropin_bit_exact(gpu, oracle):
+    rng = np.random.default_rng(21)
     x = (rng.uniform(-1, 1, 40_000) + 1j * rng.uniform(-1, 1, 40_000)).astype(np.complex64)
     table = gpu.libcsdr.shift_table_init(65536)
     assert np.abs(table - oracle.shift_table_init(65536)).max() == 0                # host table: the same expression as the oracle's
