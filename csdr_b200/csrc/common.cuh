@@ -134,8 +134,19 @@ __device__ __forceinline__ unsigned f_to_s16_bits(float x)
     return (unsigned)w & 0xffffu;
 }
 
+// ---- the reference's complex rotation: two rounded products, then a rounded difference / sum ----------------------------
+//   (p.x*v.x - p.y*v.y, p.y*v.x + p.x*v.y)   e.g. libcsdr_gpl.c:39-45: the sample times the phasor, and the phasor recursion with v = (cosd, sind)
+__device__ __forceinline__ float2 rotate_rn(float2 p, float2 v)
+{
+    return make_float2(__fsub_rn(__fmul_rn(p.x, v.x), __fmul_rn(p.y, v.y)), __fadd_rn(__fmul_rn(p.y, v.x), __fmul_rn(p.x, v.y)));
+}
+
+// the reference's PI (libcsdr.h:65) as a float; 2*PI in float arithmetic is exactly twice it
+constexpr float kPiF = 3.14159265358979323846f;
+constexpr float kTwoPiF = 2.f * kPiF;
+
 // ---- exact fast-forward of the reference's phase wrap ----------------------------------------------
-//   while (ph >  PI) ph -= 2*PI;   while (ph < -PI) ph += 2*PI;        (libcsdr_gpl.c:49-50, PI = (float)3.14159...)
+//   while (ph >  PI) ph -= 2*PI;   while (ph < -PI) ph += 2*PI;        (libcsdr_gpl.c:49-50)
 // Every subtraction rounds, so the loop cannot be replaced by fmod.  But while |ph| stays in one binade
 // [2^E, 2^(E+1)), E >= 4, ph = M*u (u = 2^(E-23), M a 24-bit integer) and fl(ph - c) = (M - q)*u with
 // q = round(c/u) independent of M (c/u is never a tie for the float 2*pi = 0xC90FDB * 2^-21, checked for all E),
@@ -159,14 +170,13 @@ __device__ __forceinline__ float wrap_binade_step(float a)
     const float bulk = __uint_as_float(((unsigned)(E + 127) << 23) | ((M - k * q) & 0x7fffffu));
     a = a >= lo ? bulk : a;
     // after the bulk step a < 2^E + c + u, so at most two real (rounded) subtractions cross the boundary
-    a = a >= lo ? __fsub_rn(a, 6.28318530717958647692f) : a;
-    a = a >= lo ? __fsub_rn(a, 6.28318530717958647692f) : a;
+    a = a >= lo ? __fsub_rn(a, kTwoPiF) : a;
+    a = a >= lo ? __fsub_rn(a, kTwoPiF) : a;
     return a;
 }
 
 __device__ __forceinline__ float wrap_phase_pm_pi(float ph)
 {
-    const float PI_F32 = 3.14159265358979323846f, TWO_PI_F32 = 6.28318530717958647692f;   // float(2)*PI rounds to the same float
     const bool neg = (__float_as_uint(ph) >> 31) != 0u;   // sign bit, so that -0.0 stays -0.0 like the loop leaves it
     float a = fabsf(ph);
     if (!(a < 67108864.f)) return ph;                // |ph| >= 2^26 (or nan): subtracting 2*pi no longer changes it; the reference would spin
@@ -183,8 +193,13 @@ __device__ __forceinline__ float wrap_phase_pm_pi(float ph)
         a = wrap_binade_step<9>(a);  a = wrap_binade_step<8>(a);  a = wrap_binade_step<7>(a);
         a = wrap_binade_step<6>(a);  a = wrap_binade_step<5>(a);  a = wrap_binade_step<4>(a);
     }
-    while (a > PI_F32) a = __fsub_rn(a, TWO_PI_F32);                                       // below 16: at most three plain steps
+    while (a > kPiF) a = __fsub_rn(a, kTwoPiF);                                            // below 16: at most three plain steps
     return neg ? -a : a;
 }
+
+// The reference's phase advance over n samples, starting_phase += rate*PI*n (libcsdr_gpl.c:48, :154): fl(fl(rate*PI)*n) ...
+__device__ __forceinline__ float phase_increment(float rate, int n) { return __fmul_rn(__fmul_rn(rate, kPiF), (float)n); }
+// ... added to the phase and wrapped into [-PI, PI]: one step of the chain ph <- wrap(fl(ph + inc))
+__device__ __forceinline__ float phase_step(float ph, float inc) { return wrap_phase_pm_pi(__fadd_rn(ph, inc)); }
 
 }  // namespace csdrb

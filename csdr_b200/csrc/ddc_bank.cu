@@ -53,48 +53,37 @@ __global__ void ddc_seed_kernel(const float* __restrict__ chunk_phase, float2* _
 // chunk 0 on entry and, on return, the phase at the start of the chunk that contains sample `advance` (the next block's start).
 // Every step adds the same increment, so the wrap is a table lookup (phase_table.cuh): ~150 dependent cycles per chunk instead of ~1 200.
 // One WARP per channel: lane 0 builds the table (32 different control flows in one warp would serialise), the chain itself keeps the table in
-// registers across the lanes (wrap_after_add_warp) and stores 32 chunk phases at a time.
+// registers across the lanes (chain_walk_warp) and stores 32 chunk phases at a time.
 __global__ void __launch_bounds__(32)
 ddc_wrap_tables_kernel(const float3* __restrict__ params, int chunk, WrapTable* __restrict__ tables, int channels)
 {
     const int c = blockIdx.x;
-    if (c < channels && threadIdx.x == 0) wrap_table_build(__fmul_rn(__fmul_rn(params[c].z, 3.14159265358979323846f), (float)chunk), tables + c);
+    if (c < channels && threadIdx.x == 0) wrap_table_build(phase_increment(params[c].z, chunk), tables + c);
 }
 
-// One warp walks one channel (more than one per warp does not interleave -- the wrap's branches and votes keep the chains in program order,
-// as on the fastddc and shift chains).
-constexpr int DDC_CHAIN_WARPS = 1;                 // chains per CTA.  The pre-pass of block k+1 runs NEXT TO block k's main kernel, whose three CTAs leave ~10 K registers per SM: a one-warp
-                                                   // CTA slips in, an eight-warp CTA has to wait for an SM to drain and the pre-pass serialises behind the main kernel
+// Chains per CTA.  The pre-pass of block k+1 runs NEXT TO block k's main kernel, whose three CTAs leave ~10 K registers per SM: a one-warp
+// CTA slips in, an eight-warp CTA has to wait for an SM to drain and the pre-pass serialises behind the main kernel.
+constexpr int kDdcChainWarps = 1;
 
-__global__ void __launch_bounds__(32 * DDC_CHAIN_WARPS)
+__global__ void __launch_bounds__(32 * kDdcChainWarps)
 ddc_phase_chain_kernel(const float3* __restrict__ params, float* __restrict__ phase_io, float* __restrict__ chunk_phase,
                        int channels, int nchunks, int chunk, int next_chunk, const WrapTable* __restrict__ tables)
 {
-    const int c = blockIdx.x * DDC_CHAIN_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    const int c = blockIdx.x * kDdcChainWarps + (threadIdx.x >> 5);
     if (c >= channels) return;
-    const float inc = __fmul_rn(__fmul_rn(params[c].z, 3.14159265358979323846f), (float)chunk);
-    const WrapLanes w = wrap_lanes_load(tables + c, lane);
-    float ph = phase_io[c], keep = ph, mine = 0.f;
-    __syncwarp();                                      // every lane has read the carried phase before lane 0 overwrites it
-    for (int k = 0; k < nchunks; k++) {
-        if ((k & 31) == lane) mine = ph;
-        if (((k & 31) == 31 || k == nchunks - 1) && (k & ~31) + lane <= k)                               // one coalesced store per 32 steps
-            chunk_phase[(long)c * nchunks + (k & ~31) + lane] = mine;
-        if (k == next_chunk) keep = ph;
-        ph = wrap_after_add_warp(__fadd_rn(ph, inc), w);
-    }
-    if (next_chunk >= nchunks) {                       // the next block starts beyond the chunks this block touched
-        for (int k = nchunks; k < next_chunk; k++) ph = wrap_after_add_warp(__fadd_rn(ph, inc), w);
-        keep = ph;
-    }
-    if (lane == 0) phase_io[c] = keep;
+    const float inc = phase_increment(params[c].z, chunk);
+    const WrapLanes w = wrap_lanes_load(tables + c, threadIdx.x & 31);
+    float keep = 0.f;
+    const float ph = chain_walk_warp(phase_io[c], inc, &w, nchunks, chunk_phase + (long)c * nchunks, [&](int k, float p) { if (k == next_chunk) keep = p; });
+    if (next_chunk >= nchunks) keep = chain_walk_warp(ph, inc, &w, next_chunk - nchunks, nullptr);   // the next block starts beyond the chunks this block touched
+    if ((threadIdx.x & 31) == 0) phase_io[c] = keep;
 }
 
 // retune support: close the current chunk `n` samples in (every channel advances by n samples at its present rate), see csdrb_ddc_bank_process
 __global__ void ddc_rechunk_kernel(const float3* __restrict__ params, float* __restrict__ phase_io, int channels, int n)
 {
     const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c < channels) phase_io[c] = wrap_phase_pm_pi(__fadd_rn(phase_io[c], __fmul_rn(__fmul_rn(params[c].z, 3.14159265358979323846f), (float)n)));
+    if (c < channels) phase_io[c] = phase_step(phase_io[c], phase_increment(params[c].z, n));
 }
 
 // ---- the bank kernel: taps in shared memory, packed phasor arithmetic, ramp-aware tap ranges ---------------------------------------
@@ -361,7 +350,7 @@ int launch_ddc_prepass(int input_size, int channels, const float* d_params, floa
     }
     const long advance = (long)n_out * decimation;                      // the next block starts here (the caller re-presents the tail)
     const int next_chunk = (int)((offset + advance) / chunk);
-    ddc_phase_chain_kernel<<<(channels + DDC_CHAIN_WARPS - 1) / DDC_CHAIN_WARPS, 32 * DDC_CHAIN_WARPS, 0, st>>>(reinterpret_cast<const float3*>(d_params), d_phase_io, chunk_phase, channels, nchunks, chunk, next_chunk,
+    ddc_phase_chain_kernel<<<chain_ctas(channels, kDdcChainWarps), 32 * kDdcChainWarps, 0, st>>>(reinterpret_cast<const float3*>(d_params), d_phase_io, chunk_phase, channels, nchunks, chunk, next_chunk,
                                                              static_cast<const WrapTable*>(d_tables));
     CSDRB_CUDA(cudaGetLastError());
     const long total = (long)channels * nchunks;

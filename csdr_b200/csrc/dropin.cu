@@ -365,8 +365,8 @@ float shift_unroll_cc(complexf* input, complexf* output, int input_size, shift_u
     st.sync();
     // one call = one chunk: the phase carried to the next call is one float multiply-add and a wrap -- done right here on the host
     float new_phase = starting_phase + input_size * d->phase_increment;
-    while (new_phase > 3.14159265358979323846f) new_phase -= 2 * 3.14159265358979323846f;
-    while (new_phase < -3.14159265358979323846f) new_phase += 2 * 3.14159265358979323846f;
+    while (new_phase > kPiF) new_phase -= 2 * kPiF;
+    while (new_phase < -kPiF) new_phase += 2 * kPiF;
     return new_phase;
 }
 

@@ -260,7 +260,7 @@ bool fastddc_inv_fold_ok(int fft_size, int fft_inv_size)
 int launch_fastddc_inv_prepare(const void* d_chan, int channels, int nblocks, int post_input_size, int post_decimation, int* d_remain_io, float* d_phase_io,
                                int* d_out_total, const InvPrep& p, cudaStream_t s, bool build_tables = true)
 {
-    fastddc_state_chain_kernel<<<(channels + CHAIN_CPW * CHAIN_WARPS - 1) / (CHAIN_CPW * CHAIN_WARPS), 32 * CHAIN_WARPS, 0, s>>>(static_cast<const DdcChan*>(d_chan), d_remain_io, d_phase_io, p.blk_remain, p.blk_phase,
+    fastddc_state_chain_kernel<<<chain_ctas(channels, kFastddcChainWarps), 32 * kFastddcChainWarps, 0, s>>>(static_cast<const DdcChan*>(d_chan), d_remain_io, d_phase_io, p.blk_remain, p.blk_phase,
                                                        p.blk_offset, d_out_total, channels, nblocks, post_input_size, post_decimation, p.tables, build_tables ? 1 : 0);
     CSDRB_CUDA(cudaGetLastError());
     fastddc_phasor_kernel<<<(unsigned)(((long)channels * nblocks + 127) / 128), 128, 0, s>>>(static_cast<const DdcChan*>(d_chan), p.blk_phase, p.phasor, channels, nblocks, p.kmax);
@@ -303,7 +303,7 @@ int launch_fastddc_inv_apply(const float2* d_spectra, int nblocks, const float2*
 
 size_t fastddc_inv_scratch_bytes(int channels, int nblocks)
 {
-    return (((size_t)channels * nblocks * 12 + 64 + 15) & ~(size_t)15) + (nblocks > 96 ? (size_t)channels * sizeof(WrapTable) : 0);
+    return (((size_t)channels * nblocks * 12 + 64 + 15) & ~(size_t)15) + (nblocks > kWrapTableMinSteps ? (size_t)channels * sizeof(WrapTable) : 0);
 }
 
 int launch_fastddc_inv_bank(const float2* d_spectra, int nblocks, const float2* d_taps_fft, const void* d_chan, int channels,
@@ -321,7 +321,7 @@ int launch_fastddc_inv_bank(const float2* d_spectra, int nblocks, const float2* 
     int* blk_remain = static_cast<int*>(d_scratch);
     float* blk_phase = reinterpret_cast<float*>(blk_remain + (size_t)channels * nblocks);
     int* blk_offset = reinterpret_cast<int*>(blk_phase + (size_t)channels * nblocks);
-    WrapTable* tables = nblocks > 96 ? reinterpret_cast<WrapTable*>(static_cast<char*>(d_scratch) + (((size_t)channels * nblocks * 12 + 64 + 15) & ~(size_t)15)) : nullptr;
+    WrapTable* tables = nblocks > kWrapTableMinSteps ? reinterpret_cast<WrapTable*>(static_cast<char*>(d_scratch) + (((size_t)channels * nblocks * 12 + 64 + 15) & ~(size_t)15)) : nullptr;
     // Fold path: fold as a batched contraction (fastddc_fold_kernel), IFFT + post shift in a second kernel, and the data-independent
     // block-to-block state chain + phasor walk on a side stream meanwhile.  Anything fastddc_inv_fold_ok() refuses takes the single-kernel forms below.
     if (fastddc_inv_fold_ok(fft_size, fft_inv_size)) {
@@ -361,7 +361,7 @@ int launch_fastddc_inv_bank(const float2* d_spectra, int nblocks, const float2* 
         CSDRB_CUDA(cudaFreeAsync(folded, st));
         return 4;
     }
-    fastddc_state_chain_kernel<<<(channels + CHAIN_CPW * CHAIN_WARPS - 1) / (CHAIN_CPW * CHAIN_WARPS), 32 * CHAIN_WARPS, 0, st>>>(static_cast<const DdcChan*>(d_chan), d_remain_io, d_phase_io, blk_remain, blk_phase,
+    fastddc_state_chain_kernel<<<chain_ctas(channels, kFastddcChainWarps), 32 * kFastddcChainWarps, 0, st>>>(static_cast<const DdcChan*>(d_chan), d_remain_io, d_phase_io, blk_remain, blk_phase,
                                                                     blk_offset, d_out_total, channels, nblocks, post_input_size, post_decimation, tables, 1);
     CSDRB_CUDA(cudaGetLastError());
     if (fft_inv_size >= 8 && fft_inv_size <= 32 && (fft_size / fft_inv_size) % 2 == 0) {          // (64..1024 with an even P is the fold path's)
@@ -492,7 +492,7 @@ int fastddc_inv_plan_create(void** out_plan, const void* h_chan, int channels, i
         pr.blk_remain = reinterpret_cast<int*>(base);
         pr.blk_phase = reinterpret_cast<float*>(pr.blk_remain + (size_t)channels * nblocks);
         pr.blk_offset = reinterpret_cast<int*>(pr.blk_phase + (size_t)channels * nblocks);
-        pr.tables = nblocks > 96 ? pl->tables : nullptr;
+        pr.tables = nblocks > kWrapTableMinSteps ? pl->tables : nullptr;
         pr.phasor = reinterpret_cast<float2*>(base + ((state_part + 15) & ~(size_t)15));
         pr.kmax = pl->kmax;
         ok = cudaMemset(pl->d_remain[i], 0, sizeof(int) * channels) == cudaSuccess && cudaMemset(pl->d_phase[i], 0, sizeof(float) * channels) == cudaSuccess &&

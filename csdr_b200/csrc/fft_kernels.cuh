@@ -301,90 +301,61 @@ apply_fir_fft_kernel(const float2* __restrict__ in, const float2* __restrict__ H
 }
 
 struct DdcChan { int offsetbin; float sindelta, cosdelta, rate; };     // per channel: fastddc_t.offsetbin + dsadata
-#define PI_F 3.14159265358979323846f
-__device__ __forceinline__ float ddc_wrap(float ph) { return wrap_phase_pm_pi(ph); }
 
-// Walk the block-to-block state of decimating_shift_addition_cc (libcsdr_gpl.c:154-158), one WARP per CHAIN_CPW channels.  A chain is sequential and a step
-// is ~400 cycles of dependent latency; letting one warp carry four channels "side by side" did NOT interleave them -- the wrap's warp-uniform branches and
-// votes keep the steps of different chains in program order, so four chains per warp run four times as long on a quarter of the SMs.  The code stays
-// generic, the constant is 1.
-constexpr int CHAIN_CPW = 1;
-
-// CHAIN_WARPS chains per CTA: the chains run NEXT TO other kernels (the fold, the IFFT step), and a guest warp slows its host SM's CTAs down -- eight warps per CTA put the 64
+// Chains per CTA: the chains run NEXT TO other kernels (the fold, the IFFT step), and a guest warp slows its host SM's CTAs down -- eight warps per CTA put the 64
 // chains of config 3 on 8 SMs instead of 64 (the fold's one CTA per SM leaves room for a 256-thread guest, which
 // the fused NFM bank's three CTAs per SM do not: its chain kernel keeps one warp per CTA).
-constexpr int CHAIN_WARPS = 8;
+constexpr int kFastddcChainWarps = 8;
 
-__global__ void __launch_bounds__(32 * CHAIN_WARPS)
+// Walk the block-to-block state of decimating_shift_addition_cc (libcsdr_gpl.c:154-158), one WARP per channel (a step is ~400 cycles of dependent latency).
+__global__ void __launch_bounds__(32 * kFastddcChainWarps)
 fastddc_state_chain_kernel(const DdcChan* __restrict__ chan, int* __restrict__ remain_io, float* __restrict__ phase_io,
                            int* __restrict__ blk_remain, float* __restrict__ blk_phase, int* __restrict__ blk_offset,
                            int* __restrict__ out_total, int channels, int nblocks, int post_input_size, int post_decimation,
                            WrapTable* __restrict__ tables, int build_tables)
 {
-    const int c0 = (blockIdx.x * CHAIN_WARPS + (threadIdx.x >> 5)) * CHAIN_CPW, lane = threadIdx.x & 31;
-    if (c0 >= channels) return;
-    const int nc = min(CHAIN_CPW, channels - c0);
-    int remain[CHAIN_CPW], off[CHAIN_CPW];
-    float ph[CHAIN_CPW], adv_const[CHAIN_CPW], rate[CHAIN_CPW];
-    WrapLanes w[CHAIN_CPW];
+    const int c = blockIdx.x * kFastddcChainWarps + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (c >= channels) return;
     const int k_const = post_input_size / post_decimation;
-    bool all_tab = tables != nullptr && nblocks > 96 && (post_input_size % post_decimation == 0);
-#pragma unroll
-    for (int i = 0; i < CHAIN_CPW; i++) {
-        const int c = min(c0 + i, channels - 1);                        // slots past the bank shadow its last channel (they compute, they do not store)
-        remain[i] = remain_io[c]; ph[i] = phase_io[c]; off[i] = 0;
-        rate[i] = chan[c].rate;
-        adv_const[i] = __fmul_rn(__fmul_rn(rate[i], PI_F), (float)k_const);
-        // when post_decimation divides post_input_size (every fastddc geometry with an even scrap, e.g. 448/2) and the carried remainder is in range, both
-        // the per-block output count and the remainder are constants: no integer division in the loop, and the phase chain runs on its increment's wrap table
-        all_tab = all_tab && remain[i] >= 0 && remain[i] < post_decimation;
-    }
+    int remain = remain_io[c], off = 0;
+    float ph = phase_io[c];
+    const float rate = chan[c].rate;
+    const float adv_const = phase_increment(rate, k_const);
+    // when post_decimation divides post_input_size (every fastddc geometry with an even scrap, e.g. 448/2) and the carried remainder is in range, both
+    // the per-block output count and the remainder are constants: no integer division in the loop, and the phase chain runs on its increment's wrap table
+    const bool steady = (post_input_size % post_decimation == 0) && remain >= 0 && remain < post_decimation;
     __syncwarp();                                                       // every lane has read the carried state before lane 0 overwrites it
-    if (all_tab) {
-        // the tables depend on the channel's increment only: a caller that keeps them (the plan object) has them built once; lane i builds channel c0 + i's
-        if (build_tables && lane < nc) wrap_table_build(__fmul_rn(__fmul_rn(chan[c0 + lane].rate, PI_F), (float)k_const), tables + c0 + lane);
+    if (tables != nullptr && nblocks > kWrapTableMinSteps && steady) {
+        // the table depends on the channel's increment only: a caller that keeps it (the plan object) has it built once
+        if (build_tables && lane == 0) wrap_table_build(adv_const, tables + c);
         __syncwarp();
-#pragma unroll
-        for (int i = 0; i < CHAIN_CPW; i++) w[i] = wrap_lanes_load(tables + min(c0 + i, channels - 1), lane);
+        const WrapLanes w = wrap_lanes_load(tables + c, lane);
+        ph = chain_walk_warp(ph, adv_const, &w, nblocks, nullptr, [&](int b, float p) {
+            if (lane == 0) {                                            // [block][channel] like the consumers index it
+                const long at = (long)b * channels + c;
+                blk_remain[at] = remain; blk_phase[at] = p; blk_offset[at] = b * k_const;
+            }
+        });
+        off = nblocks * k_const;
+    } else {                                                            // general form
         for (int b = 0; b < nblocks; b++) {
-            if (lane < nc) {                                            // lane i stores channel c0 + i: [block][channel] like the consumers index it
-                float phs = ph[0]; int rm = remain[0];
-#pragma unroll
-                for (int i = 1; i < CHAIN_CPW; i++) if (lane == i) { phs = ph[i]; rm = remain[i]; }
-                const long at = (long)b * channels + c0 + lane;
-                blk_remain[at] = rm; blk_phase[at] = phs; blk_offset[at] = b * k_const;
+            if (lane == 0) {
+                const long at = (long)b * channels + c;
+                blk_remain[at] = remain; blk_phase[at] = ph; blk_offset[at] = off;
             }
-#pragma unroll
-            for (int i = 0; i < CHAIN_CPW; i++) ph[i] = wrap_after_add_warp(__fadd_rn(ph[i], adv_const[i]), w[i]);
-        }
-#pragma unroll
-        for (int i = 0; i < CHAIN_CPW; i++) off[i] = nblocks * k_const;
-    } else {
-        for (int i = 0; i < nc; i++) {                                  // general form, one channel after the other
-            const bool steady = (post_input_size % post_decimation == 0) && remain[i] >= 0 && remain[i] < post_decimation;
-            for (int b = 0; b < nblocks; b++) {
-                if (lane == 0) {
-                    const long at = (long)b * channels + c0 + i;
-                    blk_remain[at] = remain[i]; blk_phase[at] = ph[i]; blk_offset[at] = off[i];
-                }
-                if (steady) {
-                    ph[i] = ddc_wrap(__fadd_rn(ph[i], adv_const[i]));
-                    off[i] += k_const;
-                } else {
-                    int k = 0, pos = remain[i];
-                    if (pos < post_input_size) { k = (post_input_size - pos + post_decimation - 1) / post_decimation; pos += k * post_decimation; }
-                    remain[i] = pos - post_input_size;
-                    ph[i] = ddc_wrap(__fadd_rn(ph[i], __fmul_rn(__fmul_rn(rate[i], PI_F), (float)k)));
-                    off[i] += k;
-                }
+            if (steady) {
+                ph = phase_step(ph, adv_const);
+                off += k_const;
+            } else {
+                int k = 0, pos = remain;
+                if (pos < post_input_size) { k = (post_input_size - pos + post_decimation - 1) / post_decimation; pos += k * post_decimation; }
+                remain = pos - post_input_size;
+                ph = phase_step(ph, phase_increment(rate, k));
+                off += k;
             }
         }
     }
-    if (lane == 0) {
-#pragma unroll
-        for (int i = 0; i < CHAIN_CPW; i++)
-            if (i < nc) { remain_io[c0 + i] = remain[i]; phase_io[c0 + i] = ph[i]; out_total[c0 + i] = off[i]; }
-    }
+    if (lane == 0) { remain_io[c] = remain; phase_io[c] = ph; out_total[c] = off; }
 }
 
 template <int M>
@@ -426,16 +397,15 @@ fastddc_inv_kernel(const float2* __restrict__ spectra /*[nblocks][N]*/, const fl
         const float inv_m = 1.0f / (float)M;
         const long bi = (long)b * gridDim.y + c;
         const double ph = (double)blk_phase[bi];
-        float co = (float)cos(ph), si = (float)sin(ph);
+        float2 pc = make_float2((float)cos(ph), (float)sin(ph));
+        const float2 d = make_float2(cp.cosdelta, cp.sindelta);
         float2* y = out + (long)c * out_stride + blk_offset[bi];
         int k = 0;
         for (int pos = blk_remain[bi]; pos < post_input_size; pos += post_decimation) {
             const float2 raw = s[fft_pad(scrap + pos)];
             const float2 v = make_float2(raw.x * inv_m, raw.y * inv_m);
-            y[k++] = make_float2(__fsub_rn(__fmul_rn(co, v.x), __fmul_rn(si, v.y)), __fadd_rn(__fmul_rn(si, v.x), __fmul_rn(co, v.y)));
-            const float cn = __fsub_rn(__fmul_rn(co, cp.cosdelta), __fmul_rn(si, cp.sindelta));
-            const float sn = __fadd_rn(__fmul_rn(si, cp.cosdelta), __fmul_rn(co, cp.sindelta));
-            co = cn; si = sn;
+            y[k++] = rotate_rn(pc, v);
+            pc = rotate_rn(pc, d);
         }
     }
 }
@@ -518,16 +488,15 @@ fastddc_inv_tiled_kernel(const float2* __restrict__ spectra, const float2* __res
             const float inv_m = 1.0f / (float)M;
             const long bi = (long)(b0 + v) * channels + (c0 + u);
             const double ph = (double)blk_phase[bi];
-            float co = (float)cos(ph), si = (float)sin(ph);
+            float2 pc = make_float2((float)cos(ph), (float)sin(ph));
+            const float2 d = make_float2(cp.cosdelta, cp.sindelta);
             float2* y = out + (long)(c0 + u) * out_stride + blk_offset[bi];
             int k = 0;
             for (int pos = blk_remain[bi]; pos < post_input_size; pos += post_decimation) {
                 const float2 raw = src[fft_pad(scrap + pos)];
                 const float2 w = make_float2(raw.x * inv_m, raw.y * inv_m);
-                y[k++] = make_float2(__fsub_rn(__fmul_rn(co, w.x), __fmul_rn(si, w.y)), __fadd_rn(__fmul_rn(si, w.x), __fmul_rn(co, w.y)));
-                const float cn = __fsub_rn(__fmul_rn(co, cp.cosdelta), __fmul_rn(si, cp.sindelta));
-                const float sn = __fadd_rn(__fmul_rn(si, cp.cosdelta), __fmul_rn(co, cp.sindelta));
-                co = cn; si = sn;
+                y[k++] = rotate_rn(pc, w);
+                pc = rotate_rn(pc, d);
             }
         }
     }
@@ -640,15 +609,14 @@ fastddc_phasor_kernel(const DdcChan* __restrict__ chan, const float* __restrict_
     const int c = (int)(p / nblocks), b = (int)(p % nblocks);
     const DdcChan cp = chan[c];
     const double ph = (double)blk_phase[(long)b * channels + c];
-    float co = (float)cos(ph), si = (float)sin(ph);
+    float2 pc = make_float2((float)cos(ph), (float)sin(ph));
+    const float2 d = make_float2(cp.cosdelta, cp.sindelta);
     const int rows = (int)min((long)32, npairs - p_first);
     for (int k0 = 0; k0 < kmax; k0 += 32) {
 #pragma unroll 4
         for (int j = 0; j < 32; j++) {
-            tile[lane * 33 + j] = make_float2(co, si);
-            const float cn = __fsub_rn(__fmul_rn(co, cp.cosdelta), __fmul_rn(si, cp.sindelta));
-            const float sn = __fadd_rn(__fmul_rn(si, cp.cosdelta), __fmul_rn(co, cp.sindelta));
-            co = cn; si = sn;
+            tile[lane * 33 + j] = pc;
+            pc = rotate_rn(pc, d);
         }
         __syncwarp();
         for (int r = 0; r < rows; r++)
@@ -669,7 +637,7 @@ struct FastddcPostSink {
     {
         if (kk[r] < 0) return;
         const float2 w = make_float2(v.x * inv_m, v.y * inv_m);
-        y[kk[r]] = make_float2(__fsub_rn(__fmul_rn(ph[r].x, w.x), __fmul_rn(ph[r].y, w.y)), __fadd_rn(__fmul_rn(ph[r].y, w.x), __fmul_rn(ph[r].x, w.y)));
+        y[kk[r]] = rotate_rn(ph[r], w);
     }
 };
 

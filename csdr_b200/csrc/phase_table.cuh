@@ -19,7 +19,7 @@
 // below 2^32), the float tail loop.  ~150-200 cycles per step instead of ~1 200.  A window that needs more pieces than the table holds, or
 // a value outside the window (the caller's first phase may be anything), takes wrap_phase_pm_pi -- the table is an accelerator, never a
 // different answer.  Checked against the plain loop for every float in the window, for thousands of increments, on the CPU tier
-// (tests/test_phase_table_host.py), and on the GPU (tests/test_gpu_phase_table.py).
+// (tests/test_phase_table_host.py), and on the GPU (tests/test_gpu_round2.py::test_long_phase_chains_are_bit_exact).
 #pragma once
 #include "common.cuh"
 
@@ -33,6 +33,10 @@ struct WrapTable {
     float thr[kWrapPieces];             // thr[0] == lo, ascending; piece i = [thr[i], thr[i+1])
     double K[kWrapPieces];              // what the loop subtracts in total before the value falls below 16
 };
+
+// A chain of more than this many steps runs on its increment's wrap table (building one costs about as much as thirty direct steps).
+// The scratch-size functions reserve table space on the same condition.
+constexpr int kWrapTableMinSteps = 96;
 
 constexpr long long kWrapC = 0xC90FDBLL;                    // the float 2*pi in units of 2^-21
 constexpr long long kWrapV16 = 16LL << 21;
@@ -133,7 +137,6 @@ __host__ __device__ inline void wrap_table_build(float inc, WrapTable* t)
 // wrap_phase_pm_pi(x) for x = fl(ph + inc) of the chain the table was built for (any other x still gets the right answer, slowly)
 __device__ __forceinline__ float wrap_after_add(float x, const WrapTable* __restrict__ t)
 {
-    const float PI_F32 = 3.14159265358979323846f, TWO_PI_F32 = 6.28318530717958647692f;
     float a = fabsf(x);
     if (a >= 16.f) {
         const int n = t->n;
@@ -143,7 +146,7 @@ __device__ __forceinline__ float wrap_after_add(float x, const WrapTable* __rest
         for (int i = 0; i < n; i++) cnt += a >= t->thr[i] ? 1 : 0;
         a = (float)((double)a - t->K[cnt - 1]);             // exact; the result is the float the loop would hold at this point
     }
-    while (a > PI_F32) a = __fsub_rn(a, TWO_PI_F32);
+    while (a > kPiF) a = __fsub_rn(a, kTwoPiF);
     return (__float_as_uint(x) >> 31) ? -a : a;
 }
 
@@ -171,7 +174,6 @@ __device__ __forceinline__ WrapLanes wrap_lanes_load(const WrapTable* __restrict
 // Generic form: any table size, values outside the table's window (falls back to the exact loop fast-forward).
 static __device__ __noinline__ float wrap_after_add_warp_generic(float x, const WrapLanes& w)
 {
-    const float PI_F32 = 3.14159265358979323846f, TWO_PI_F32 = 6.28318530717958647692f;
     float a = fabsf(x);
     if (a >= 16.f) {                                                    // every branch here is warp-uniform (same x, same table in all lanes)
         if (w.n == 0 || !(a >= w.lo && a <= w.hi)) return wrap_phase_pm_pi(x);
@@ -184,7 +186,7 @@ static __device__ __noinline__ float wrap_after_add_warp_generic(float x, const 
         }
         a = (float)((double)a - K);                                     // exact; the float the loop would hold when it first drops below 16
     }
-    while (a > PI_F32) a = __fsub_rn(a, TWO_PI_F32);
+    while (a > kPiF) a = __fsub_rn(a, kTwoPiF);
     return (__float_as_uint(x) >> 31) ? -a : a;
 }
 
@@ -194,7 +196,6 @@ static __device__ __noinline__ float wrap_after_add_warp_generic(float x, const 
 // 16 - 3*2pi < pi).  Same operations in the same order as the generic form, which takes everything else.
 __device__ __forceinline__ float wrap_after_add_warp(float x, const WrapLanes& w)
 {
-    const float PI_F32 = 3.14159265358979323846f, TWO_PI_F32 = 6.28318530717958647692f;
     const float a = fabsf(x);
     const bool below = a < 16.f;
     const bool in = !below && w.n > 0 && a >= w.lo && a <= w.hi;
@@ -205,12 +206,41 @@ __device__ __forceinline__ float wrap_after_add_warp(float x, const WrapLanes& w
     const double K0 = __shfl_sync(0xffffffffu, w.K0, idx & 31), K1 = __shfl_sync(0xffffffffu, w.K1, (more - 1) & 31);
     const double K = more > 0 ? K1 : K0;
     float r = in ? (float)((double)a - K) : a;                          // exact; the float the loop would hold when it first drops below 16
-    r = r > PI_F32 ? __fsub_rn(r, TWO_PI_F32) : r;
-    r = r > PI_F32 ? __fsub_rn(r, TWO_PI_F32) : r;
-    r = r > PI_F32 ? __fsub_rn(r, TWO_PI_F32) : r;
+    r = r > kPiF ? __fsub_rn(r, kTwoPiF) : r;
+    r = r > kPiF ? __fsub_rn(r, kTwoPiF) : r;
+    r = r > kPiF ? __fsub_rn(r, kTwoPiF) : r;
     return (__float_as_uint(x) >> 31) ? -r : r;
 }
 
+struct NoChainSink { __device__ void operator()(int, float) const {} };
+
+// One warp walks `steps` steps of the chain ph <- wrap(fl(ph + inc)) from `ph` and returns the phase after them.  All 32 lanes pass the same
+// arguments and get the same phases.  A step goes through the wrap table `w`, or through wrap_phase_pm_pi without one (the same answer).
+// Before step k, `sink(k, ph)` runs in every lane and, given a `row`, ph goes to row[k]: lane i holds the phase of step i mod 32 and the warp
+// stores 32 of them at a time.  The walk starts with a __syncwarp: every lane has read the carried state it passed in before the caller's
+// lane 0 overwrites it.  (Several chains per warp do not interleave -- the wrap's branches and votes keep them in program order -- so a
+// warp walks one chain.)  Pass `w` as the address of a local or as nullptr, not as a pointer chosen at run time: the compiler then drops
+// the other step from the loop and keeps the table in registers (chosen at run time, the table goes to local memory and every step waits on it).
+template <class Sink = NoChainSink>
+__device__ __forceinline__ float chain_walk_warp(float ph, float inc, const WrapLanes* w, int steps, float* __restrict__ row, Sink sink = {})
+{
+    const int lane = threadIdx.x & 31;
+    float mine = 0.f;
+    __syncwarp();
+    for (int k = 0; k < steps; k++) {
+        sink(k, ph);
+        if (row) {
+            if ((k & 31) == lane) mine = ph;
+            if (((k & 31) == 31 || k == steps - 1) && (k & ~31) + lane <= k) row[(k & ~31) + lane] = mine;
+        }
+        ph = w ? wrap_after_add_warp(__fadd_rn(ph, inc), *w) : phase_step(ph, inc);
+    }
+    return ph;
+}
+
 #endif  // device (or emulated device) code
+
+// CTAs of a chain kernel with `warps` chains (one warp each) per CTA; every caller states its own `warps` at the launch
+inline unsigned chain_ctas(int channels, int warps) { return (unsigned)((channels + warps - 1) / warps); }
 
 }  // namespace csdrb

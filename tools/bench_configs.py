@@ -50,6 +50,10 @@ if "k" in which:
     xc = torch.view_as_complex(x)
     out = torch.empty((C, N), dtype=torch.complex64, device=dev)
     report("K2 shift_addition bank 64x2.4M chunk 1024", timed(lambda: cb.shift_addition_bank_cc(xc, rates, chunk=1024, out=out)), C * N, C * N * 16)
+    steps = np.stack([cb.shift_addfast_init(float(r)) for r in rates]); table = torch.from_numpy(cb.libcsdr.shift_table_init(65536)).to(dev)
+    report("K2 shift_addfast bank 64x2.4M chunk 1024", timed(lambda: cb.shift_addfast_bank_cc(xc, steps=steps, chunk=1024, out=out)), C * N, C * N * 16)
+    report("K2 shift_math bank 64x2.4M", timed(lambda: cb.shift_math_bank_cc(xc, rates, out=out)), C * N, C * N * 16)
+    report("K2 shift_table bank 64x2.4M (65536-entry table)", timed(lambda: cb.shift_table_bank_cc(xc, rates, table, out=out)), C * N, C * N * 16)
     a = y[:, :N // 10 * 10].contiguous()
     report("K5 fractional_decimator bank 64x2.4M rate 5", timed(lambda: cb.fractional_decimator_bank_ff(a, 5.0, 12)), C * a.shape[1], C * a.shape[1] * 4.8)
     a2 = a[:, :2343 * 1024].contiguous()
