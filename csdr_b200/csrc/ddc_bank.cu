@@ -128,8 +128,12 @@ struct DdcWalk {
     // one wideband sample against the taps of its phase p (tp = taps of phase p, MP/2 float2), accumulators JLO..JHI-1 only
     // The taps come as SCALARS (two per 64-bit shared load) and multiply the I and the Q lane of the shifted sample: the tap operand is one register
     // for both channels of the lane, and four taps come with one 128-bit shared load (a copy duplicated (h, h) in shared memory needs twice the loads).
-    template <int JLO, int JHI>
-    __device__ __forceinline__ void sample(float xi, float xq, const float2* __restrict__ tp)
+    // LIM >= 0 (the guarded form): only taps jD + p < T are applied, lim = T - p -- the zero-padded taps past T meet samples outside the
+    // output's window [oD, oD + T), and fma(sh, 0, acc) is NaN for a non-finite sh where the reference, which never reads them, stays finite.
+    // For a finite sh the skipped fma(sh, 0, acc) is acc, so both forms give the same bits; the walk takes the unguarded one only for samples
+    // it has checked to be small enough for sh to stay finite.
+    template <int JLO, int JHI, bool GUARD = false>
+    __device__ __forceinline__ void sample(float xi, float xq, const float2* __restrict__ tp, int lim = 0)
     {
         const float2 xi2 = make_float2(xi, xi), xq2 = make_float2(xq, xq);
         float2 sh[CPL];
@@ -141,10 +145,11 @@ struct DdcWalk {
 #pragma unroll
         for (int j = JLO; j < JHI; j += 2) {
             const float2 h2 = tp[j / 2];
+            const bool la = !GUARD || j * D < lim, lb = j + 1 < M && (!GUARD || (j + 1) * D < lim);
 #pragma unroll
             for (int u = 0; u < CPL; u++) {
-                acc[u][j] = ffma2(sh[u], make_float2(h2.x, h2.x), acc[u][j]);
-                if (j + 1 < M) acc[u][j + 1] = ffma2(sh[u], make_float2(h2.y, h2.y), acc[u][j + 1]);
+                if (la) acc[u][j] = ffma2(sh[u], make_float2(h2.x, h2.x), acc[u][j]);
+                if (lb) acc[u][j + 1] = ffma2(sh[u], make_float2(h2.y, h2.y), acc[u][j + 1]);
             }
         }
     }
@@ -155,7 +160,7 @@ __global__ void __launch_bounds__(128)
 ddc_bank_fused2_kernel(const float2* __restrict__ wide, int n_in, int offset, int chunk, int nchunks,
                        const float3* __restrict__ params, const float2* __restrict__ seeds, int channels, int sets,
                        void* __restrict__ out_v, long out_stride, int n_out, int seg_outputs, int nsegs,
-                       const float2* __restrict__ last_in, float2* __restrict__ last_out,
+                       const float2* __restrict__ last_in, float2* __restrict__ last_out, int T,
                        const __grid_constant__ DdcTaps<D * ((M + 1) & ~1)> taps)
 {
     constexpr int MP = (M + 1) & ~1;
@@ -207,7 +212,7 @@ ddc_bank_fused2_kernel(const float2* __restrict__ wide, int n_in, int offset, in
         }
         left--;
         const float2 x = idx < n_in ? __ldg(wide + idx) : make_float2(0.f, 0.f);   // samples past n_in only ever meet zero-padded taps
-        w.template sample<decltype(jlo)::value, decltype(jhi)::value>(x.x, x.y, staps + pidx * (MP / 2));
+        w.template sample<decltype(jlo)::value, decltype(jhi)::value, true>(x.x, x.y, staps + pidx * (MP / 2), T - pidx);
     };
     // one period (D samples) restricted to accumulators [JLO, JHI)
     auto period = [&](auto jlo, auto jhi, int q) {
@@ -222,19 +227,26 @@ ddc_bank_fused2_kernel(const float2* __restrict__ wide, int n_in, int offset, in
                 const float4* src = reinterpret_cast<const float4*>(wide + base + p0);     // D, UU even: 16-byte aligned
                 const float2* tp = staps + p0 * (MP / 2);
                 float4 cur[UU / 2];
+                float mag = 0.f;                                        // sum of |x.i| + |x.q| over the group: NaN, Inf or huge -> guarded path
 #pragma unroll
-                for (int e = 0; e < UU / 2; e++) cur[e] = __ldg(src + e);
-#pragma unroll
-                for (int e = 0; e < UU; e += 2) {
-                    const float4 xx = cur[e / 2];
-                    w.template sample<JLO, JHI>(xx.x, xx.y, tp + e * (MP / 2));
-                    w.template sample<JLO, JHI>(xx.z, xx.w, tp + (e + 1) * (MP / 2));
+                for (int e = 0; e < UU / 2; e++) {
+                    cur[e] = __ldg(src + e);
+                    mag += fabsf(cur[e].x) + fabsf(cur[e].y) + fabsf(cur[e].z) + fabsf(cur[e].w);
                 }
-                left -= UU;
-            } else {
-#pragma unroll 1
-                for (int e = 0; e < UU; e++) checked(jlo, jhi, base + p0 + e, p0 + e);
+                // |P|, |Q| stay near 1, so below 2^126 every shifted sample of the group is finite and the padded taps add exactly nothing
+                if (mag < 0x1p126f) {
+#pragma unroll
+                    for (int e = 0; e < UU; e += 2) {
+                        const float4 xx = cur[e / 2];
+                        w.template sample<JLO, JHI>(xx.x, xx.y, tp + e * (MP / 2));
+                        w.template sample<JLO, JHI>(xx.z, xx.w, tp + (e + 1) * (MP / 2));
+                    }
+                    left -= UU;
+                    continue;
+                }
             }
+#pragma unroll 1
+            for (int e = 0; e < UU; e++) checked(jlo, jhi, base + p0 + e, p0 + e);   // chunk boundary, block end or a group that failed the check
         }
     };
     // acc[.][j] collects output q-j while the walk is in period q (samples qD .. qD+D-1): sample qD+p meets tap p + jD.
@@ -320,7 +332,7 @@ static int launch_fused(const float2* wide, int n_in, int offset, int chunk, int
     const int nsegs = (n_out + seg - 1) / seg;
     const long warps = (long)nsegs * warps_per_seg;
     const unsigned ctas = (unsigned)((warps + 3) / 4);
-#define CSDRB_DDC_LAUNCH(CPLV, DM) ddc_bank_fused2_kernel<D, M, CPLV, DM><<<ctas, 128, 0, st>>>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, warps_per_seg, out, out_stride, n_out, seg, nsegs, last_in, last_out, tp)
+#define CSDRB_DDC_LAUNCH(CPLV, DM) ddc_bank_fused2_kernel<D, M, CPLV, DM><<<ctas, 128, 0, st>>>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, warps_per_seg, out, out_stride, n_out, seg, nsegs, last_in, last_out, T, tp)
     if (cpl == kDdcChannelsPerLane) { if (demod) CSDRB_DDC_LAUNCH(kDdcChannelsPerLane, true); else CSDRB_DDC_LAUNCH(kDdcChannelsPerLane, false); }
     else { if (demod) CSDRB_DDC_LAUNCH(1, true); else CSDRB_DDC_LAUNCH(1, false); }
 #undef CSDRB_DDC_LAUNCH

@@ -70,6 +70,32 @@ __device__ __forceinline__ void fir_accumulate(const float2* __restrict__ base, 
     }
 }
 
+// The zero-padded taps [T, D*M) meet samples past the output's window [oD, oD + T), and fma(x, 0, acc) is NaN when x is NaN or +-Inf, where the
+// reference, which never reads those samples, stays finite.  So an output that comes out non-finite is summed again from the tile with the padded
+// taps skipped, in fir_accumulate's order: per half, phase pairs, then sub-taps, then the two phases of the pair; the halves meet in one add.
+// For a finite sample the skipped fma(x, 0, acc) is acc, so this is the tile loop's value without padding, and the tile loop keeps its
+// branch-free padded form (taps in uniform registers); non-finite outputs are rare.
+template <int D, int MG>
+__device__ __noinline__ float2 fir_output_unpadded(const float2* __restrict__ x, const float2* __restrict__ hh, int T)
+{
+    float2 s[2];
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+        float2 acc = make_float2(0.f, 0.f);
+#pragma unroll 1
+        for (int pp = 0; pp < D / 2; pp++) {
+#pragma unroll 1
+            for (int m = 0; m < MG; m++) {
+                const int k = (h * MG + m) * D + 2 * pp;
+                if (k < T) acc = ffma2(x[k], hh[k], acc);
+                if (k + 1 < T) acc = ffma2(x[k + 1], hh[k + 1], acc);
+            }
+        }
+        s[h] = acc;
+    }
+    return fadd2(s[0], s[1]);
+}
+
 // U8 = true: the input is rtl_sdr-style unsigned 8-bit IQ (2 bytes per sample, what csdr-fm:41 feeds convert_u8_f) and the conversion of
 // libcsdr.c:2363-2366 happens on the way into the tile: the bytes arrive by the same bulk copy (a quarter of the HBM / PCIe traffic of cf32)
 // at the tail of the tile buffer, every thread pulls its share into registers, and after a barrier writes the floats over the whole buffer.
@@ -78,7 +104,7 @@ __device__ __forceinline__ void fir_accumulate(const float2* __restrict__ base, 
 template <int D, int M, int R, int NPAIR, int MINB, bool U8>
 __global__ void __launch_bounds__(NPAIR * 64, MINB)
 fir_bank_fast_kernel(const void* __restrict__ in_v, long in_stride, float2* __restrict__ out, long out_stride,
-                     int n_in, int n_out, const __grid_constant__ FirTaps<D * M> taps)
+                     int n_in, int n_out, int T, const __grid_constant__ FirTaps<D * M> taps)
 {
     using C = FirCfg<D, M, R, NPAIR>;
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -173,7 +199,13 @@ fir_bank_fast_kernel(const void* __restrict__ in_v, long in_stride, float2* __re
     named_bar_sync(1 + pair, 64);
     if (half == 0) {
 #pragma unroll
-        for (int r = 0; r < R; r++) myred[r] = fadd2(acc[r], myred[r]);
+        for (int r = 0; r < R; r++) {
+            float2 y = fadd2(acc[r], myred[r]);
+            constexpr unsigned EXP = 0x7f800000u;           // all exponent bits set: NaN or +-Inf
+            if (((__float_as_uint(y.x) & EXP) == EXP) || ((__float_as_uint(y.y) & EXP) == EXP))   // maybe a non-finite sample under a padded tap
+                y = fir_output_unpadded<D, C::MG>(xs + (pair * C::OUT_PAIR + lane * R + r) * D, taps.hh, T);
+            myred[r] = y;
+        }
     }
     named_bar_sync(1 + pair, 64);
     const int o0 = tile * C::OUT_TILE + pair * C::OUT_PAIR;  // first output of this pair (even)
@@ -229,7 +261,7 @@ static int launch_fast(const void* in, long in_stride, float2* out, long out_str
     FirTaps<D * M> tp;
     for (int k = 0; k < D * M; k++) { float h = k < T ? h_taps[k] : 0.f; tp.hh[k] = make_float2(h, h); }
     dim3 grid((n_out + C::OUT_TILE - 1) / C::OUT_TILE, channels);
-    kern<<<grid, C::THREADS, smem, st>>>(in, in_stride, out, out_stride, n_in, n_out, tp);
+    kern<<<grid, C::THREADS, smem, st>>>(in, in_stride, out, out_stride, n_in, n_out, T, tp);
     CSDRB_CUDA(cudaGetLastError());
     return 0;
 }

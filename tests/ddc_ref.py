@@ -11,7 +11,7 @@ sets, channel count or block split.  The helpers give
 """
 import numpy as np
 
-U = 2.0 ** -24                                                       # unit roundoff of binary32
+from bitcmp import U, assert_bits_equal, bits  # noqa: F401  (re-exported for the DDC bank test modules)
 
 KERNELS = [(50, 17), (10, 8), (10, 20)]                              # the compiled (D, M) instantiations of ddc_bank_fused2_kernel
 T_VALUES = {50: [1, 49, 50, 751, 800, 801, 850], 10: [1, 9, 10, 79, 80, 81, 199, 200]}
@@ -139,20 +139,6 @@ def bound(x, p, taps, D):
     return (T + 2) * U * (1 + 1e-3) * (_windows(a, T, D, n_out) @ np.abs(taps.astype(np.float64)))
 
 
-def bits(a):
-    """the bit patterns of a float32 / complex64 array (NaN-safe exact comparison)"""
-    a = np.ascontiguousarray(a)
-    return a.view(np.uint32) if a.dtype in (np.float32, np.complex64) else a
-
-
-def assert_bits_equal(a, b, what):
-    a, b = bits(a), bits(b)
-    assert a.shape == b.shape, (what, a.shape, b.shape)
-    if not np.array_equal(a, b):
-        bad = np.argwhere(a != b)
-        raise AssertionError(f"{what}: {len(bad)} of {a.size} words differ, first at {tuple(bad[0])}")
-
-
 def check_against_reference(oracle, case, x, rates, ph0, last, taps, base, phase, demod, demod_phase, last_out):
     """every assertion that needs only the oracle: the baseband (demod = 0 run) within bound() of the float64 reference at every output, the carried
     phases bit for bit, and the demod run = fmdemod_quadri_cf on the bank's own baseband, bit for bit, last_out included"""
@@ -173,3 +159,46 @@ def check_against_reference(oracle, case, x, rates, ph0, last, taps, base, phase
         wd, wl = oracle.fmdemod_quadri_cf(base[c], complex(last[c]))
         assert_bits_equal(demod[c], wd, f"demod of channel {c}")
         assert_bits_equal(np.complex64(last_out[c]), np.complex64(wl), f"last_out of channel {c}")
+
+
+NONFINITE = [(50, 801), (50, 51), (10, 79), (10, 9), (10, 199), (10, 81)]     # every (D, M) kernel, a full and a nearly empty last tap block
+
+
+def nonfinite_positions(D, T, n):
+    """wideband samples to poison: just past output 5's window, at its last zero-padded tap (D*M - 1), a sample in mid-window of a later output,
+    the first and the last sample of the block"""
+    M = kernel_for(D, T)[1]
+    pos = {5 * D + T, 5 * D + D * M - 1, 40 * D + T // 2 + 1, 0, n - 1}
+    return sorted(p for p in pos if 0 <= p < n)
+
+
+def check_nonfinite(run, case):
+    """NaN, +Inf and -Inf in the wideband block (in turn, on the I or the Q component): with demod off exactly the outputs whose window
+    [oD, oD + T) holds one are non-finite and every other output keeps the clean run's bits; with demod on every output whose own or previous
+    baseband sample is clean keeps its bits, last_out included.  run(x, rates, ph0, last, taps, demod) -> (out, last_out or None)."""
+    D, T = case["D"], case["T"]
+    x, rates, ph0, last, taps = make_inputs(case)
+    n = x.size
+    pos = nonfinite_positions(D, T, n)
+    xp = x.copy()
+    bad = [np.nan, np.inf, -np.inf]
+    for i, p in enumerate(pos):
+        xp[p] = complex(bad[i % 3], 0.5) if i % 2 == 0 else complex(-0.25, bad[i % 3])
+    n_out = n_out_of(n, D, T)
+    o = np.arange(n_out)
+    hit = np.zeros(n_out, bool)
+    for p in pos:
+        hit |= (o * D <= p) & (p < o * D + T)
+    what = f"D={D} T={T} chunk {case['chunk']}+{case['offset']}"
+    base0, _ = run(x, rates, ph0, last, taps, 0)
+    base1, _ = run(xp, rates, ph0, last, taps, 0)
+    for c in range(rates.size):
+        fin = np.isfinite(base1[c].real) & np.isfinite(base1[c].imag)
+        assert np.array_equal(~fin, hit), f"{what} channel {c}: non-finite outputs {np.flatnonzero(~fin)[:12]}, expected {np.flatnonzero(hit)[:12]}"
+    assert_bits_equal(base1[:, ~hit], base0[:, ~hit], f"{what}: baseband away from the poisoned samples")
+    dem0, lo0 = run(x, rates, ph0, last, taps, 1)
+    dem1, lo1 = run(xp, rates, ph0, last, taps, 1)
+    near = hit | np.concatenate([[False], hit[:-1]])
+    assert_bits_equal(dem1[:, ~near], dem0[:, ~near], f"{what}: discriminator away from the poisoned samples")
+    if not hit[-1]:
+        assert_bits_equal(lo1, lo0, f"{what}: last_out")

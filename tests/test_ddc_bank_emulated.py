@@ -22,7 +22,8 @@ ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT / "tests" / "host_shim"))
 sys.path.insert(0, str(ROOT / "tests"))
 import emul_build  # noqa: E402
-from ddc_ref import (assert_bits_equal, case_id, cases, check_against_reference, kernel_for, make_inputs, n_out_of, nco)  # noqa: E402
+from ddc_ref import (NONFINITE, assert_bits_equal, case_id, cases, check_against_reference, check_nonfinite, kernel_for, make_inputs, n_out_of,  # noqa: E402
+                     nco)
 
 ORDERS = ["alternate", "reverse", "random"]
 SM_COUNT, WARPS_PER_SM = 132, 12                                     # kSmCount (common.cuh), kDdcWarpsPerSm (ddc_bank.cu)
@@ -216,3 +217,25 @@ def test_fused_ddc_bank_unit_tap_is_the_reference_nco(banks, oracle, chunk, offs
                 out, _ = _main(lib, pre, chunk, offset, D, taps, 0, None)
                 for c in range(ch):
                     assert_bits_equal(out[c], refs[c][k::D][:out.shape[1]], f"D={D} T={T} k={k} CPL={lib.cpl} channel {c}")
+
+
+@pytest.mark.parametrize("D,T", NONFINITE)
+@pytest.mark.parametrize("chunk,offset", [(1024, 0), (13, 12)])
+def test_fused_ddc_bank_nonfinite_stays_in_its_windows(banks, D, T, chunk, offset):
+    """NaN / +-Inf wideband samples reach exactly the outputs whose window holds them (ddc_ref.check_nonfinite), both DEMOD kernels and both
+    channels-per-lane copies; the two copies give the same bits"""
+    case = dict(D=D, T=T, channels=33, chunk=chunk, offset=offset, n=T + 60 * D + 7, seed=D + T + chunk)
+    outs = []
+    for lib in banks:
+        got = {}
+
+        def run(x, rates, ph0, last, taps, demod):
+            out, _, lo = _run(lib, x, rates, ph0, chunk, offset, D, taps, demod, last if demod else None)
+            got[(x.tobytes(), demod)] = (out, lo)
+            return out, lo
+        check_nonfinite(run, case)
+        outs.append(got)
+    for k in outs[0]:
+        for a, b in zip(outs[0][k], outs[1][k]):
+            if a is not None:
+                assert_bits_equal(b, a, "CPL=1 against CPL=2")

@@ -20,7 +20,8 @@ import pytest
 
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT / "tests"))
-from ddc_ref import (KERNELS, assert_bits_equal, case_id, cases, check_against_reference, make_inputs, n_out_of, nco)  # noqa: E402
+from ddc_ref import (KERNELS, NONFINITE, assert_bits_equal, case_id, cases, check_against_reference, check_nonfinite, make_inputs, n_out_of,  # noqa: E402
+                     nco)
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -89,6 +90,22 @@ def run_matrix(gpu):
                 taps = np.zeros(T, np.float32); taps[k] = 1.0
                 res[f"probe_{chunk}+{offset}_D{D}T{T}_k{k}"], _, _ = _bank(gpu, x, PROBE_RATES, ph0, chunk, offset, D, taps, 0, None)
     res["probe_phase0"] = ph0
+    for D, T in NONFINITE:
+        for chunk, offset in ((1024, 0), (13, 12)):
+            key = f"nonfinite_D{D}T{T}_{chunk}+{offset}"
+            case = dict(D=D, T=T, channels=97, chunk=chunk, offset=offset, n=T + 300 * D + 7, seed=D + T + chunk)
+            runs = []
+
+            def run(x, rates, ph0, last, taps, demod):
+                out, _, lo = _bank(gpu, x, rates, ph0, chunk, offset, D, taps, demod, last if demod else None)
+                res[f"{key}__run{len(runs)}"] = out
+                runs.append(out)
+                return out, lo
+            try:
+                check_nonfinite(run, case)
+                res[key] = np.array("ok")
+            except AssertionError as e:
+                res[key] = np.array(str(e))
     return res
 
 
@@ -178,6 +195,15 @@ def test_gpu_one_channel_per_lane_gives_the_same_bits(cpl2, cpl1):
     assert sorted(res1) == sorted(res2)
     for k in res2:
         assert_bits_equal(res1[k], res2[k], f"CPL=1 against CPL=2: {k}")
+
+
+@pytest.mark.parametrize("D,T", NONFINITE)
+@pytest.mark.parametrize("chunk,offset", [(1024, 0), (13, 12)])
+def test_gpu_ddc_bank_nonfinite_stays_in_its_windows(cpl2, D, T, chunk, offset):
+    """NaN / +-Inf wideband samples reach exactly the outputs whose window holds them, both DEMOD kernels (ddc_ref.check_nonfinite); the
+    one-channel-per-lane child ran the same calls, and test_gpu_one_channel_per_lane_gives_the_same_bits compares its outputs"""
+    verdict = str(cpl2[0][f"nonfinite_D{D}T{T}_{chunk}+{offset}"])
+    assert verdict == "ok", verdict
 
 
 @pytest.mark.parametrize("D,T,demod", [(50, 801, True), (10, 199, False), (10, 79, True)])
