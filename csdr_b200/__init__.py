@@ -1040,6 +1040,8 @@ class FastddcInvPlan:
 def ddc_bank(wide, rates, decimation: int, taps: np.ndarray, demod: bool = True, chunk: int = 1024, offset: int = 0,
              phases=None, last=None, out=None):
     """Fused shared-input bank: one wideband block [N] complex64 -> per channel shift | fir_decimate | (fmdemod).
+    Any even decimation D whose filter has M = ceil(len(taps) / D) <= 24 and D * MP <= 8000 taps (MP = the smallest of 4, 8, 12, 18, 20, 24 >= M);
+    an odd D or a longer filter raises CsdrB200Error.
     Returns (out [C, n_out], new chunk-start phases [C], last baseband samples [C] or None)."""
     import torch
     assert wide.dtype == torch.complex64 and wide.is_cuda and wide.dim() == 1
@@ -1114,7 +1116,8 @@ def fir_valid_bank_ff(x, taps, limit_max: float = 0.0, out=None):
 
 class DdcBank:
     """Streaming shared-input DDC/NFM bank (csdrb_ddc_bank_*): shift | fir_decimate | [fmdemod] for C channels of one wideband stream,
-    one call per block, all per-channel state inside; the phase-chain pre-pass of the next block overlaps the current block."""
+    one call per block, all per-channel state inside; the phase-chain pre-pass of the next block overlaps the current block.
+    Serves the geometries ddc_bank() serves (any even decimation within the tap limits); the constructor raises CsdrB200Error for the others."""
 
     def __init__(self, rates, decimation: int, taps: np.ndarray, demod: bool = True, chunk: int = 1024):
         self.rates = np.ascontiguousarray(np.atleast_1d(rates), np.float32)

@@ -661,10 +661,7 @@ struct csdrb_ddc_bank_s {
 csdrb_ddc_bank_t* csdrb_ddc_bank_create(int channels, const float* h_rates, int decimation, const float* h_taps, int taps_length, int demod, int chunk)
 {
     if (channels <= 0 || !h_rates || !h_taps || decimation <= 0 || taps_length <= 0) { set_error("ddc bank create: bad argument"); return nullptr; }
-    if (!((decimation == 50 && taps_length <= 850) || (decimation == 10 && taps_length <= 200))) {     // the geometries launch_ddc_main has fused kernels for
-        set_error("ddc bank create: no fused kernel for decimation %d / %d taps (compiled: d=50 T<=850, d=10 T<=200); run the unfused bank calls", decimation, taps_length);
-        return nullptr;
-    }
+    if (ddc_bank_geometry(decimation, taps_length) < 0) return nullptr;
     auto* b = new csdrb_ddc_bank_s();
     b->channels = channels; b->decimation = decimation; b->taps_length = taps_length; b->demod = demod ? 1 : 0; b->chunk = chunk > 0 ? chunk : 1024;
     b->taps.assign(h_taps, h_taps + taps_length);

@@ -106,7 +106,22 @@ constexpr int kDdcChannelsPerLane = 2;
 // kernels.  Fewer, longer segments would leave SMs idle; more, shorter ones spend a larger share on the M-1 trailing periods of each.
 constexpr int kDdcWarpsPerSm = 12;
 
-template <int D, int M, int CPL, bool DEMOD>
+// Every other even decimation runs ddc_bank_generic_kernel<M, CPL, DEMOD>: D is a kernel argument and M a compile-time bucket, the smallest of
+// kDdcBuckets >= ceil(T/D) (the taps of the blocks past ceil(T/D) are zero).  17 is a bucket of its own because T = firdes_filter_len(0.25/D) =
+// 16D +- 1 -- a transition band of a quarter of the output rate, config 4's ratio -- has M = 16 or 17 at every D.
+constexpr int kDdcBuckets[] = {4, 8, 12, 17, 20, 24};
+constexpr int kDdcMaxM = 24;
+// The generic kernel takes its taps as one fixed-size kernel parameter (no device buffer: csdrb_ddc_bank takes host taps and its scratch size knows
+// neither D nor T).  All parameters together must stay within 32 764 bytes, so D * MP <= 8000 taps.
+constexpr int kDdcTapCapacity = 8000;
+// 4-warp CTAs per SM of each generic bucket (__launch_bounds__ caps the registers so that many fit; DESIGN.md 8b lists the registers): the
+// launcher sizes its segments for that many resident warps.
+__host__ __device__ constexpr int ddc_generic_ctas_per_sm(int M, int cpl)
+{
+    return cpl == 1 ? (M <= 8 ? 6 : M <= 12 ? 5 : M <= 20 ? 4 : 3) : (M <= 4 ? 5 : M <= 8 ? 4 : M <= 17 ? 3 : 2);
+}
+
+template <int M, int CPL>
 struct DdcWalk {
     static constexpr int MP = (M + 1) & ~1;
     float2 P[CPL], Q[CPL], cd2[CPL], sd2[CPL];
@@ -133,7 +148,7 @@ struct DdcWalk {
     // For a finite sh the skipped fma(sh, 0, acc) is acc, so both forms give the same bits; the walk takes the unguarded one only for samples
     // it has checked to be small enough for sh to stay finite.
     template <int JLO, int JHI, bool GUARD = false>
-    __device__ __forceinline__ void sample(float xi, float xq, const float2* __restrict__ tp, int lim = 0)
+    __device__ __forceinline__ void sample(float xi, float xq, const float2* __restrict__ tp, int lim = 0, int D = 0)
     {
         const float2 xi2 = make_float2(xi, xi), xq2 = make_float2(xq, xq);
         float2 sh[CPL];
@@ -155,19 +170,19 @@ struct DdcWalk {
     }
 };
 
-template <int D, int M, int CPL, bool DEMOD>
-__global__ void __launch_bounds__(128)
-ddc_bank_fused2_kernel(const float2* __restrict__ wide, int n_in, int offset, int chunk, int nchunks,
-                       const float3* __restrict__ params, const float2* __restrict__ seeds, int channels, int sets,
-                       void* __restrict__ out_v, long out_stride, int n_out, int seg_outputs, int nsegs,
-                       const float2* __restrict__ last_in, float2* __restrict__ last_out, int T,
-                       const __grid_constant__ DdcTaps<D * ((M + 1) & ~1)> taps)
+// The walk of one warp, shared by both bank kernels.  DC > 0: the decimation is the compile-time DC (ddc_bank_fused2_kernel); DC = 0: it is the
+// run-time d_rt (ddc_bank_generic_kernel).  U = samples per unchecked group of a full-width period: a period runs groups of U while U samples are
+// left and the rest in groups of 2 (DC is a multiple of U).  staps = the taps in shared memory, [p][j / 2] = taps (j, j+1) of phase p.
+template <int DC, int M, int CPL, bool DEMOD, int U>
+__device__ __forceinline__ void ddc_bank_walk(const float2* __restrict__ wide, int n_in, int offset, int chunk, int nchunks,
+                                              const float3* __restrict__ params, const float2* __restrict__ seeds, int channels, int sets,
+                                              void* __restrict__ out_v, long out_stride, int n_out, int seg_outputs, int nsegs,
+                                              const float2* __restrict__ last_in, float2* __restrict__ last_out, int T, int d_rt, const float2* staps)
 {
     constexpr int MP = (M + 1) & ~1;
-    constexpr int U = (D % 10 == 0) ? 10 : 2;                           // samples per unchecked group
-    __shared__ float2 staps[D * MP / 2];                               // [p][j / 2] = taps (j, j+1) of phase p
-    for (int i = threadIdx.x; i < D * MP / 2; i += 128) staps[i] = taps.h2[i];
-    __syncthreads();
+    static_assert(MP <= 24, "the head and tail ramps below step in fours up to 20");
+    static_assert(DC % U == 0 && U % 2 == 0, "groups of U samples tile a period");
+    const int D = DC > 0 ? DC : d_rt;
     const int lane = threadIdx.x & 31;
     const long wid = (long)blockIdx.x * 4 + (threadIdx.x >> 5);
     const int segi = (int)(wid / sets), set = (int)(wid % sets);
@@ -179,7 +194,7 @@ ddc_bank_fused2_kernel(const float2* __restrict__ wide, int n_in, int offset, in
     int o_start = o_first - (DEMOD ? 1 : 0);                            // the discriminator needs the previous baseband sample
     if (o_start < 0) o_start = 0;
 
-    DdcWalk<D, M, CPL, DEMOD> w;
+    DdcWalk<M, CPL> w;
     int chs[CPL]; bool live[CPL];
     float2 prev[CPL];
     const long n0 = (long)o_start * D;
@@ -212,41 +227,49 @@ ddc_bank_fused2_kernel(const float2* __restrict__ wide, int n_in, int offset, in
         }
         left--;
         const float2 x = idx < n_in ? __ldg(wide + idx) : make_float2(0.f, 0.f);   // samples past n_in only ever meet zero-padded taps
-        w.template sample<decltype(jlo)::value, decltype(jhi)::value, true>(x.x, x.y, staps + pidx * (MP / 2), T - pidx);
+        w.template sample<decltype(jlo)::value, decltype(jhi)::value, true>(x.x, x.y, staps + pidx * (MP / 2), T - pidx, D);
     };
     // one period (D samples) restricted to accumulators [JLO, JHI)
     auto period = [&](auto jlo, auto jhi, int q) {
         constexpr int JLO = decltype(jlo)::value, JHI = decltype(jhi)::value;
         constexpr int UU = (JLO == 0 && JHI == MP) ? U : 2;             // the steady-state body is unrolled deeper than the ramps
         const long base = (long)q * D;
-        // (fetching the next group's samples into registers while this one is multiplied was slower: the extra registers cost more
-        // than the exposed L1 round trip)
-#pragma unroll 1
-        for (int p0 = 0; p0 < D; p0 += UU) {
-            if (left >= UU && base + p0 + UU <= n_in) {
-                const float4* src = reinterpret_cast<const float4*>(wide + base + p0);     // D, UU even: 16-byte aligned
+        // samples p0 .. p0+G-1 of the period
+        auto group = [&](auto g, int p0) {
+            constexpr int G = decltype(g)::value;
+            // (fetching the next group's samples into registers while this one is multiplied was slower: the extra registers cost more
+            // than the exposed L1 round trip)
+            if (left >= G && base + p0 + G <= n_in) {
+                const float4* src = reinterpret_cast<const float4*>(wide + base + p0);     // D, p0 even: 16-byte aligned
                 const float2* tp = staps + p0 * (MP / 2);
-                float4 cur[UU / 2];
+                float4 cur[G / 2];
                 float mag = 0.f;                                        // sum of |x.i| + |x.q| over the group: NaN, Inf or huge -> guarded path
 #pragma unroll
-                for (int e = 0; e < UU / 2; e++) {
+                for (int e = 0; e < G / 2; e++) {
                     cur[e] = __ldg(src + e);
                     mag += fabsf(cur[e].x) + fabsf(cur[e].y) + fabsf(cur[e].z) + fabsf(cur[e].w);
                 }
                 // |P|, |Q| stay near 1, so below 2^126 every shifted sample of the group is finite and the padded taps add exactly nothing
                 if (mag < 0x1p126f) {
 #pragma unroll
-                    for (int e = 0; e < UU; e += 2) {
+                    for (int e = 0; e < G; e += 2) {
                         const float4 xx = cur[e / 2];
                         w.template sample<JLO, JHI>(xx.x, xx.y, tp + e * (MP / 2));
                         w.template sample<JLO, JHI>(xx.z, xx.w, tp + (e + 1) * (MP / 2));
                     }
-                    left -= UU;
-                    continue;
+                    left -= G;
+                    return;
                 }
             }
 #pragma unroll 1
-            for (int e = 0; e < UU; e++) checked(jlo, jhi, base + p0 + e, p0 + e);   // chunk boundary, block end or a group that failed the check
+            for (int e = 0; e < G; e++) checked(jlo, jhi, base + p0 + e, p0 + e);   // chunk boundary, block end or a group that failed the check
+        };
+        const int d_main = DC > 0 ? D : D - D % UU;
+#pragma unroll 1
+        for (int p0 = 0; p0 < d_main; p0 += UU) group(std::integral_constant<int, UU>{}, p0);
+        if constexpr (DC == 0 && UU > 2) {
+#pragma unroll 1
+            for (int p0 = d_main; p0 < D; p0 += 2) group(std::integral_constant<int, 2>{}, p0);
         }
     };
     // acc[.][j] collects output q-j while the walk is in period q (samples qD .. qD+D-1): sample qD+p meets tap p + jD.
@@ -260,6 +283,8 @@ ddc_bank_fused2_kernel(const float2* __restrict__ wide, int n_in, int offset, in
         else if (need_hi <= 8 && 8 < MP) period(I0{}, std::integral_constant<int, (8 < MP ? 8 : MP)>{}, q);
         else if (need_hi <= 12 && 12 < MP) period(I0{}, std::integral_constant<int, (12 < MP ? 12 : MP)>{}, q);
         else if (need_hi <= 16 && 16 < MP) period(I0{}, std::integral_constant<int, (16 < MP ? 16 : MP)>{}, q);
+        else if (need_hi <= 20 && 20 < MP) period(I0{}, std::integral_constant<int, (20 < MP ? 20 : MP)>{}, q);
+        else if (need_lo >= 20 && 20 < MP) period(std::integral_constant<int, (20 < MP ? 20 : 0)>{}, IM{}, q);
         else if (need_lo >= 16 && 16 < MP) period(std::integral_constant<int, (16 < MP ? 16 : 0)>{}, IM{}, q);
         else if (need_lo >= 12 && 12 < MP) period(std::integral_constant<int, (12 < MP ? 12 : 0)>{}, IM{}, q);
         else if (need_lo >= 8 && 8 < MP) period(std::integral_constant<int, (8 < MP ? 8 : 0)>{}, IM{}, q);
@@ -284,6 +309,43 @@ ddc_bank_fused2_kernel(const float2* __restrict__ wide, int n_in, int offset, in
             }
         }
     }
+}
+
+// D = 50 and D = 10: the taps in static shared memory, groups of 10 samples when D allows
+template <int D, int M, int CPL, bool DEMOD>
+__global__ void __launch_bounds__(128)
+ddc_bank_fused2_kernel(const float2* __restrict__ wide, int n_in, int offset, int chunk, int nchunks,
+                       const float3* __restrict__ params, const float2* __restrict__ seeds, int channels, int sets,
+                       void* __restrict__ out_v, long out_stride, int n_out, int seg_outputs, int nsegs,
+                       const float2* __restrict__ last_in, float2* __restrict__ last_out, int T,
+                       const __grid_constant__ DdcTaps<D * ((M + 1) & ~1)> taps)
+{
+    constexpr int MP = (M + 1) & ~1;
+    __shared__ float2 staps[D * MP / 2];
+    for (int i = threadIdx.x; i < D * MP / 2; i += 128) staps[i] = taps.h2[i];
+    __syncthreads();
+    ddc_bank_walk<D, M, CPL, DEMOD, (D % 10 == 0) ? 10 : 2>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, sets, out_v, out_stride, n_out,
+                                                            seg_outputs, nsegs, last_in, last_out, T, D, staps);
+}
+
+static_assert(sizeof(DdcTaps<kDdcTapCapacity>) + 160 <= 32764, "the generic kernel's parameters must fit the 32 764-byte parameter space");
+
+// any even D: D * MP floats of taps in dynamic shared memory (at most 32 000 bytes, no opt-in needed)
+template <int M, int CPL, bool DEMOD>
+__global__ void __launch_bounds__(128, ddc_generic_ctas_per_sm(M, CPL))
+ddc_bank_generic_kernel(const float2* __restrict__ wide, int n_in, int offset, int chunk, int nchunks,
+                        const float3* __restrict__ params, const float2* __restrict__ seeds, int channels, int sets,
+                        void* __restrict__ out_v, long out_stride, int n_out, int seg_outputs, int nsegs,
+                        const float2* __restrict__ last_in, float2* __restrict__ last_out, int T, int D,
+                        const __grid_constant__ DdcTaps<kDdcTapCapacity> taps)
+{
+    constexpr int MP = (M + 1) & ~1;
+    CSDRB_DYN_SMEM(smem);
+    float2* staps = reinterpret_cast<float2*>(smem);
+    for (int i = threadIdx.x; i < D * MP / 2; i += 128) staps[i] = taps.h2[i];
+    __syncthreads();
+    ddc_bank_walk<0, M, CPL, DEMOD, 8>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, sets, out_v, out_stride, n_out,
+                                       seg_outputs, nsegs, last_in, last_out, T, D, staps);
 }
 
 size_t ddc_bank_scratch_bytes(int channels, int input_size, int chunk, int offset)
@@ -311,33 +373,88 @@ int launch_ddc_tables(int channels, const float* d_params, int chunk, void* d_ta
     return 1;
 }
 
+// tap k = jD + p stored at [p][j], rows of MP = M rounded up to even; taps past T (and rows past M) are zero
+static void ddc_pack_taps(float2* h2, int D, int M, const float* h_taps, int T)
+{
+    const int MP = (M + 1) & ~1;
+    for (int p = 0; p < D; p++)
+        for (int j = 0; j < MP; j++) {
+            const int k = j * D + p; const float h = (j < M && k < T) ? h_taps[k] : 0.f;
+            float2& slot = h2[(p * MP + j) / 2];
+            if (j & 1) slot.y = h; else slot.x = h;
+        }
+}
+
+static int ddc_cpl_from_env() { return getenv("CSDRB_DDC_CPL") && atoi(getenv("CSDRB_DDC_CPL")) != kDdcChannelsPerLane ? 1 : kDdcChannelsPerLane; }
+
+// Grid of a bank launch: one warp per (segment, channel set).  Enough segments to fill warps_per_sm resident warps on every SM, while keeping the
+// M-1 trailing periods of every segment a small fraction (at least 2M outputs per segment).
+struct DdcGrid { int sets, seg, nsegs; unsigned ctas; };
+static DdcGrid ddc_grid(int channels, int n_out, int M, int cpl, int warps_per_sm)
+{
+    DdcGrid g;
+    g.sets = (channels + 32 * cpl - 1) / (32 * cpl);
+    const long want_segments = (kSmCount * warps_per_sm + g.sets - 1) / g.sets;
+    g.seg = (int)((n_out + want_segments - 1) / want_segments);
+    if (g.seg < 2 * M) g.seg = 2 * M;
+    g.nsegs = (n_out + g.seg - 1) / g.seg;
+    g.ctas = (unsigned)(((long)g.nsegs * g.sets + 3) / 4);
+    return g;
+}
+
 template <int D, int M>
 static int launch_fused(const float2* wide, int n_in, int offset, int chunk, int nchunks, const float3* params, const float2* seeds, int channels,
                         int demod, void* out, long out_stride, int n_out, const float2* last_in, float2* last_out, const float* h_taps, int T, cudaStream_t st)
 {
     constexpr int MP = (M + 1) & ~1;
-    DdcTaps<D * MP> tp;                                                 // tap k = jD + p stored at [p][j]
-    for (int p = 0; p < D; p++)
-        for (int j = 0; j < MP; j++) {
-            const int k = j * D + p; const float h = (j < M && k < T) ? h_taps[k] : 0.f;
-            float2& slot = tp.h2[(p * MP + j) / 2];
-            if (j & 1) slot.y = h; else slot.x = h;
-        }
-    static const int cpl = getenv("CSDRB_DDC_CPL") && atoi(getenv("CSDRB_DDC_CPL")) != kDdcChannelsPerLane ? 1 : kDdcChannelsPerLane;
-    const int warps_per_seg = (channels + 32 * cpl - 1) / (32 * cpl);
-    // enough warps to fill the machine while keeping the M-1 trailing periods of every segment a small fraction
-    long want_segments = (kSmCount * kDdcWarpsPerSm + warps_per_seg - 1) / warps_per_seg;
-    int seg = (int)((n_out + want_segments - 1) / want_segments);
-    if (seg < 2 * M) seg = 2 * M;
-    const int nsegs = (n_out + seg - 1) / seg;
-    const long warps = (long)nsegs * warps_per_seg;
-    const unsigned ctas = (unsigned)((warps + 3) / 4);
-#define CSDRB_DDC_LAUNCH(CPLV, DM) ddc_bank_fused2_kernel<D, M, CPLV, DM><<<ctas, 128, 0, st>>>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, warps_per_seg, out, out_stride, n_out, seg, nsegs, last_in, last_out, T, tp)
+    DdcTaps<D * MP> tp;
+    ddc_pack_taps(tp.h2, D, M, h_taps, T);
+    static const int cpl = ddc_cpl_from_env();
+    const DdcGrid g = ddc_grid(channels, n_out, M, cpl, kDdcWarpsPerSm);
+#define CSDRB_DDC_LAUNCH(CPLV, DM) ddc_bank_fused2_kernel<D, M, CPLV, DM><<<g.ctas, 128, 0, st>>>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, g.sets, out, out_stride, n_out, g.seg, g.nsegs, last_in, last_out, T, tp)
     if (cpl == kDdcChannelsPerLane) { if (demod) CSDRB_DDC_LAUNCH(kDdcChannelsPerLane, true); else CSDRB_DDC_LAUNCH(kDdcChannelsPerLane, false); }
     else { if (demod) CSDRB_DDC_LAUNCH(1, true); else CSDRB_DDC_LAUNCH(1, false); }
 #undef CSDRB_DDC_LAUNCH
     CSDRB_CUDA(cudaGetLastError());
     return 0;
+}
+
+// M = bucket; sized for the bucket's own resident warps (its registers allow fewer CTAs per SM than the D = 50 / 10 kernels' three at large M)
+template <int M>
+static int launch_generic(const float2* wide, int n_in, int offset, int chunk, int nchunks, const float3* params, const float2* seeds, int channels,
+                          int demod, void* out, long out_stride, int n_out, const float2* last_in, float2* last_out, const float* h_taps, int T, int D,
+                          cudaStream_t st)
+{
+    constexpr int MP = (M + 1) & ~1;
+    DdcTaps<kDdcTapCapacity> tp;
+    ddc_pack_taps(tp.h2, D, M, h_taps, T);
+    static const int cpl = ddc_cpl_from_env();
+    const DdcGrid g = ddc_grid(channels, n_out, M, cpl, 4 * ddc_generic_ctas_per_sm(M, cpl));
+    const size_t smem = (size_t)D * MP * sizeof(float);
+#define CSDRB_DDC_LAUNCH(CPLV, DM) ddc_bank_generic_kernel<M, CPLV, DM><<<g.ctas, 128, smem, st>>>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, g.sets, out, out_stride, n_out, g.seg, g.nsegs, last_in, last_out, T, D, tp)
+    if (cpl == kDdcChannelsPerLane) { if (demod) CSDRB_DDC_LAUNCH(kDdcChannelsPerLane, true); else CSDRB_DDC_LAUNCH(kDdcChannelsPerLane, false); }
+    else { if (demod) CSDRB_DDC_LAUNCH(1, true); else CSDRB_DDC_LAUNCH(1, false); }
+#undef CSDRB_DDC_LAUNCH
+    CSDRB_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// the generic bucket of a geometry: the smallest of kDdcBuckets >= ceil(T/D) whose D * MP taps fit the capacity, or 0
+static int ddc_bucket(int decimation, int taps_length)
+{
+    if (decimation <= 0 || (decimation & 1) || taps_length <= 0) return 0;
+    const long m = ((long)taps_length + decimation - 1) / decimation;
+    for (int b : kDdcBuckets)
+        if (m <= b) return (long)decimation * ((b + 1) & ~1) <= kDdcTapCapacity ? b : 0;
+    return 0;
+}
+
+int ddc_bank_geometry(int decimation, int taps_length)
+{
+    if (ddc_bucket(decimation, taps_length)) return 0;
+    set_error("ddc bank: no fused kernel for decimation %d / %d taps (served: even decimation D, M = ceil(taps / D) <= %d, and D * MP <= %d taps, "
+              "MP = the smallest of 4, 8, 12, 18, 20, 24 >= M); run the unfused bank calls", decimation, taps_length, kDdcMaxM, kDdcTapCapacity);
+    return -2;
 }
 
 // ---- the two halves of a block, exposed separately so a bank object can run the pre-pass of the NEXT block on a side stream ----
@@ -383,12 +500,22 @@ int launch_ddc_main(const float2* d_wide, int input_size, int channels, const fl
     if (reinterpret_cast<uintptr_t>(d_wide) & 15) { set_error("ddc bank: wideband input must be 16-byte aligned"); return -1; }
     const int nchunks = (int)(((long)offset + input_size + chunk - 1) / chunk) + 1;
     const float2* seeds = reinterpret_cast<const float2*>(static_cast<const char*>(d_scratch) + (((size_t)channels * nchunks * sizeof(float) + 15) & ~(size_t)15));
+    if (int rc = ddc_bank_geometry(decimation, taps_length); rc < 0) return rc;
     int rc = -1;
     const float3* P = reinterpret_cast<const float3*>(d_params);
-    if (decimation == 50 && taps_length <= 50 * 17) rc = launch_fused<50, 17>(d_wide, input_size, offset, chunk, nchunks, P, seeds, channels, demod, d_out, out_stride, n_out, d_last_in, d_last_out, h_taps, taps_length, st);
-    else if (decimation == 10 && taps_length <= 10 * 8) rc = launch_fused<10, 8>(d_wide, input_size, offset, chunk, nchunks, P, seeds, channels, demod, d_out, out_stride, n_out, d_last_in, d_last_out, h_taps, taps_length, st);
-    else if (decimation == 10 && taps_length <= 10 * 20) rc = launch_fused<10, 20>(d_wide, input_size, offset, chunk, nchunks, P, seeds, channels, demod, d_out, out_stride, n_out, d_last_in, d_last_out, h_taps, taps_length, st);
-    else { set_error("ddc bank: no fused kernel for decimation %d / %d taps (compiled: d=50 T<=850, d=10 T<=200); run the unfused bank calls", decimation, taps_length); return -2; }
+#define CSDRB_DDC_ARGS d_wide, input_size, offset, chunk, nchunks, P, seeds, channels, demod, d_out, out_stride, n_out, d_last_in, d_last_out, h_taps, taps_length
+    if (decimation == 50 && taps_length <= 50 * 17) rc = launch_fused<50, 17>(CSDRB_DDC_ARGS, st);
+    else if (decimation == 10 && taps_length <= 10 * 8) rc = launch_fused<10, 8>(CSDRB_DDC_ARGS, st);
+    else if (decimation == 10 && taps_length <= 10 * 20) rc = launch_fused<10, 20>(CSDRB_DDC_ARGS, st);
+    else switch (ddc_bucket(decimation, taps_length)) {
+        case 4: rc = launch_generic<4>(CSDRB_DDC_ARGS, decimation, st); break;
+        case 8: rc = launch_generic<8>(CSDRB_DDC_ARGS, decimation, st); break;
+        case 12: rc = launch_generic<12>(CSDRB_DDC_ARGS, decimation, st); break;
+        case 17: rc = launch_generic<17>(CSDRB_DDC_ARGS, decimation, st); break;
+        case 20: rc = launch_generic<20>(CSDRB_DDC_ARGS, decimation, st); break;
+        case 24: rc = launch_generic<24>(CSDRB_DDC_ARGS, decimation, st); break;
+    }
+#undef CSDRB_DDC_ARGS
     return rc < 0 ? rc : n_out;
 }
 
@@ -400,6 +527,9 @@ int launch_ddc_bank(const float2* d_wide, int input_size, int channels, const fl
     *launches = 0;
     if (channels <= 0 || decimation <= 0 || taps_length <= 0) { set_error("ddc bank: bad geometry"); return -1; }
     if (reinterpret_cast<uintptr_t>(d_wide) & 15) { set_error("ddc bank: wideband input must be 16-byte aligned"); return -1; }
+    if (input_size >= taps_length) {                                    // a refused geometry launches nothing (and leaves d_phase_io alone)
+        if (int rc = ddc_bank_geometry(decimation, taps_length); rc < 0) return rc;
+    }
     int rc = launch_ddc_prepass(input_size, channels, d_params, d_phase_io, chunk, offset, decimation, taps_length, d_scratch, scratch_bytes, nullptr, st);
     if (rc <= 0) return rc;
     const int pre = rc;

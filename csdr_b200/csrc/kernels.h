@@ -99,6 +99,7 @@ int fastddc_inv_plan_set_state(void* plan, const int* h_remain, const float* h_p
 void fastddc_inv_plan_destroy(void* plan);
 
 // fused shared-input DDC bank, ddc_bank.cu
+int ddc_bank_geometry(int decimation, int taps_length);               // 0 when the bank serves (decimation, taps_length); else -2 with the error set
 size_t ddc_bank_scratch_bytes(int channels, int input_size, int chunk, int offset);
 size_t ddc_bank_tables_bytes(int channels);                            // persistent phase-wrap tables of a bank (phase_table.cuh), one per channel
 int launch_ddc_rechunk(int channels, const float* d_params, float* d_phase_io, int n, cudaStream_t st);

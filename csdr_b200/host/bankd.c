@@ -17,6 +17,8 @@
  *   --tail: nfm (default) the README.md:87 tail, s16; none the raw discriminator output, f32; am / usb / lsb the AM and SSB graphs of README.md:95 and :110
  *   behind the DDC's complex baseband (see bb_tail_t), s16; iq the complex baseband itself, cf32.  --limit is limit_ff's amplitude (default 1), --agc-ref
  *   the AGC reference (default: fastagc_ff's 1.0 for nfm, agc_ff's 0.2 for am/usb/lsb).
+ *   --decimation: any even D (default 50) whose filter the fused bank serves: M = ceil(taps / D) <= 24 and D * M (rounded up to the kernel's
+ *   bucket) <= 8000 taps, see csdrb_ddc_bank in include/csdr_b200.h.  The NFM tail's deemphasis_nfm_ff stays at 48000 whatever D gives.
  *   RATE  shift_addition_cc rate (fraction of the wideband sample rate), SINK a path (file or FIFO) or tcp:PORT (one listener).
  *   --devices: the channels are sliced over several GPUs of this node (csdrb_multi_bank_*: the block goes to the first device once and on to
  *   the others by NCCL broadcast), one block of latency more (two blocks are kept in flight); the audio tail (nfm, am, usb, lsb), audio-rate work, runs on
@@ -437,7 +439,7 @@ int main(int argc, char **argv)
     if (nfm && agc_ref == 0.0f) agc_ref = 1.0f;                      /* fastagc_ff's default reference (csdr.c:1388) */
     if (C == 0) die("no channels (RATE:SINK ...)");
     if (block <= 0 || (block & 1)) die("--block must be a positive even number of samples");
-    if (D <= 0 || (D & 1)) die("--decimation must be a positive even number (the fused kernels exist for 10 and 50)");
+    if (D <= 0 || (D & 1)) die("--decimation must be a positive even number (the fused bank serves even decimations only)");
     if (!(bw > 0.f && bw < 0.5f)) die("--bw must be a transition bandwidth between 0 and 0.5");
     if (!(limit > 0.f) || !(agc_ref >= 0.f)) die("--limit and --agc-ref must be positive");
     signal(SIGPIPE, SIG_IGN);

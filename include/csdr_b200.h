@@ -235,7 +235,11 @@ int csdrb_decimating_shift_addition_bank_cc(const complexf *d_in, long in_stride
  * must start the next block (re-presenting the unconsumed tail exactly like fir_decimate_cc's callers do, csdr.c:1172-1174).
  * demod = 0: d_out is complexf [channels][out_stride] baseband; demod = 1: float [channels][out_stride] discriminator output,
  * d_last_in/d_last_out carry the previous baseband sample per channel (NULL = zeros / not wanted).
- * Returns outputs per channel, -2 when no fused kernel is compiled for (decimation, taps_length) -- use the unfused bank calls then. */
+ * Served geometries: any even decimation D with M = ceil(taps_length / D) <= 24 and D * MP <= 8000, MP being the smallest of 4, 8, 12, 18, 20, 24
+ * >= M (e.g. T = 16 D + 1 up to D = 444, D = 1000 up to M = 8, D = 2 up to 48 taps).  D = 50 up to 850 taps and D = 10 up to 200 taps run their own
+ * kernels, every other served geometry one kernel with D as an argument; the outputs follow the same contract either way.
+ * Returns outputs per channel, -2 for an odd decimation or a geometry beyond those limits (nothing is launched, d_phase_io is left as it was) -- use
+ * the unfused bank calls, or the fastddc overlap-save bank for very large decimations, then. */
 size_t csdrb_ddc_bank_scratch_bytes(int channels, int input_size, int chunk, int offset);
 int csdrb_ddc_bank(const complexf *d_wide, int input_size, int channels, const shift_addition_data_t *d_params, float *d_phase_io,
                    int chunk, int offset, int decimation, const float *h_taps, int taps_length, int demod, void *d_out, long out_stride,
@@ -245,7 +249,8 @@ int csdrb_ddc_bank(const complexf *d_wide, int input_size, int channels, const s
  * NCO chunk, so a wideband stream is processed with one call per block; internally the serial phase-chain pre-pass of block k+1 runs on
  * a private stream while the caller's stream executes block k.  Contract of process(): it consumes n_out*decimation samples (the return
  * value is n_out); the next block must start there, i.e. the caller re-presents the unconsumed tail exactly like fir_decimate_cc's
- * callers do (csdr.c:1172-1174).  d_out is float [channels][out_stride] when the bank was created with demod = 1, else complexf. */
+ * callers do (csdr.c:1172-1174).  d_out is float [channels][out_stride] when the bank was created with demod = 1, else complexf.
+ * create() serves the geometries csdrb_ddc_bank serves and returns NULL for the others (csdrb_last_error() names the served set). */
 typedef struct csdrb_ddc_bank_s csdrb_ddc_bank_t;
 csdrb_ddc_bank_t *csdrb_ddc_bank_create(int channels, const float *h_rates, int decimation, const float *h_taps, int taps_length, int demod, int chunk);
 void csdrb_ddc_bank_destroy(csdrb_ddc_bank_t *bank);
@@ -263,7 +268,8 @@ int  csdrb_ddc_bank_process(csdrb_ddc_bank_t *bank, const complexf *d_wide, int 
  * kernels, D2H of the results) and returns a ticket; collect(ticket) waits for that block.  Up to two blocks may be in flight, so a caller that submits
  * block k+1 before collecting block k has the broadcast of k+1 under the kernels of k.  h_wide / h_out of a submitted block belong to the library until
  * its collect returns (page-locked memory from csdrb_host_alloc for full PCIe rate).  h_out is [channels][out_stride] floats (demod = 1) or complexf.
- * Block contract as for csdrb_ddc_bank_process: a block consumes n_out*decimation samples, the caller re-presents the tail.  devices == NULL: 0..ndev-1. */
+ * Block contract as for csdrb_ddc_bank_process: a block consumes n_out*decimation samples, the caller re-presents the tail.  devices == NULL: 0..ndev-1.
+ * create() serves the (decimation, taps_length) geometries csdrb_ddc_bank serves and returns NULL for the others. */
 typedef struct csdrb_multi_bank_s csdrb_multi_bank_t;
 csdrb_multi_bank_t *csdrb_multi_bank_create(int ndev, const int *devices, int channels, const float *h_rates, int decimation, const float *h_taps,
                                             int taps_length, int demod, int chunk, int max_block);
