@@ -39,6 +39,10 @@ class _FracDec(C.Structure):            # include/csdr_b200.h fractional_decimat
                 ("xifirst", C.c_int), ("xilast", C.c_int), ("rate", C.c_float), ("taps", C.c_void_p), ("taps_length", C.c_int)]
 
 
+class _Resampler(C.Structure):          # rational_resampler_ff_t (= libcsdr.h:132-137)
+    _fields_ = [("input_processed", C.c_int), ("output_size", C.c_int), ("last_taps_delay", C.c_int)]
+
+
 class _FastAgc(C.Structure):            # fastagc_ff_t (= libcsdr.h:118-128)
     _fields_ = [("buffer_1", C.c_void_p), ("buffer_2", C.c_void_p), ("buffer_input", C.c_void_p), ("peak_1", C.c_float),
                 ("peak_2", C.c_float), ("input_size", C.c_int), ("reference", C.c_float), ("last_gain", C.c_float)]
@@ -195,6 +199,9 @@ def lib() -> C.CDLL:
     L.fractional_decimator_ff_init.argtypes = [C.c_float, it, vp, it]; L.fractional_decimator_ff_init.restype = _FracDec
     L.fractional_decimator_ff.argtypes = [vp, vp, it, C.POINTER(_FracDec)]
     L.fastagc_ff.argtypes = [C.POINTER(_FastAgc), vp]
+    L.rational_resampler_ff.argtypes = [vp, vp, it, it, it, C.POINTER(C.c_float), it, it]; L.rational_resampler_ff.restype = _Resampler
+    L.rational_resampler_get_lowpass_f.argtypes = [C.POINTER(C.c_float), it, it, it, it]
+    L.csdrb_rational_resampler_bank_ff.argtypes = [vp, lg, vp, lg, it, it, it, it, C.POINTER(C.c_float), it, it, C.POINTER(_Resampler), vp]
     L.make_fft_c2c.argtypes = [it, vp, vp, it, it]; L.make_fft_c2c.restype = C.POINTER(_Plan)
     L.fft_execute.argtypes = [C.POINTER(_Plan)]
     L.fft_destroy.argtypes = [C.POINTER(_Plan)]
@@ -246,6 +253,13 @@ def firdes_filter_len(transition_bw: float) -> int:
 def firdes_lowpass_f(length: int, cutoff_rate: float, window: str = "HAMMING") -> np.ndarray:
     t = np.empty(length, np.float32)
     lib().firdes_lowpass_f(_fp(t), length, cutoff_rate, WINDOWS[window])
+    return t
+
+
+def rational_resampler_get_lowpass_f(length: int, interpolation: int, decimation: int, window: str = "HAMMING") -> np.ndarray:
+    """the lowpass rational_resampler_ff's CLI designs (libcsdr.c:665-673): cutoff at half the lower of 1/I and 1/D"""
+    t = np.empty(length, np.float32)
+    lib().rational_resampler_get_lowpass_f(_fp(t), length, interpolation, decimation, WINDOWS[window])
     return t
 
 
@@ -475,6 +489,29 @@ class libcsdr:
             if d.input_processed == 0:
                 d.input_processed = block
             lib().fractional_decimator_ff(buf.ctypes.data, out.ctypes.data, block, C.byref(d))
+            outs.append(out[:d.output_size].copy())
+        return np.concatenate(outs) if outs else np.zeros(0, np.float32)
+
+    @staticmethod
+    def rational_resampler_ff(x, interpolation, decimation, taps, block=None, last_taps_delay=0):
+        """block=None: one call on all of x, returns (y, (input_processed, output_size, last_taps_delay)).
+        Else the CLI's block loop (csdr.c:1448-1461) over the complete reads of x: the first call takes `block` samples, each later one the
+        unconsumed tail plus input_processed new samples; returns the concatenated output."""
+        x = np.ascontiguousarray(x, np.float32); taps = np.ascontiguousarray(taps, np.float32)
+        if block is None:
+            y = np.empty(max(x.size * interpolation // decimation, 1), np.float32)
+            d = lib().rational_resampler_ff(x.ctypes.data, y.ctypes.data, x.size, interpolation, decimation, _fp(taps), taps.size, last_taps_delay)
+            return y[:d.output_size].copy(), (d.input_processed, d.output_size, d.last_taps_delay)
+        buf = np.zeros(block, np.float32); out = np.empty(max(block * interpolation // decimation, 1), np.float32)
+        d = _Resampler(0, 0, last_taps_delay); pos = 0; outs = []
+        while True:
+            need = block if d.input_processed == 0 else d.input_processed
+            if d.input_processed:
+                buf[:block - need] = buf[need:].copy()
+            if pos + need > x.size:
+                break
+            buf[block - need:] = x[pos:pos + need]; pos += need
+            d = lib().rational_resampler_ff(buf.ctypes.data, out.ctypes.data, block, interpolation, decimation, _fp(taps), taps.size, d.last_taps_delay)
             outs.append(out[:d.output_size].copy())
         return np.concatenate(outs) if outs else np.zeros(0, np.float32)
 
@@ -805,6 +842,23 @@ def fractional_decimator_bank_ff(x, rate: float, num_poly_points: int = 12, taps
                                                     d_taps.data_ptr() if d_taps is not None else None, d_taps.numel() if d_taps is not None else 0,
                                                     state.data_ptr(), scratch.data_ptr(), scratch.numel(), _stream()), "fractional_decimator_bank_ff")
     return out, state
+
+
+def rational_resampler_bank_ff(x, interpolation: int, decimation: int, taps, last_taps_delay: int = 0, out=None):
+    """x [C, N] float32 CUDA tensor -> (y [C, n_out], (input_processed, output_size, last_taps_delay)): every row through rational_resampler_ff
+    with the shared host ``taps`` and last_taps_delay.  The state is computed on the host; nothing waits for the device."""
+    import torch
+    assert x.dtype == torch.float32 and x.is_cuda and x.dim() == 2 and x.stride(1) == 1
+    taps = np.ascontiguousarray(taps, np.float32)
+    ch, n = x.shape
+    if out is None:
+        out = torch.empty((ch, max(n * interpolation // decimation, 1)), dtype=torch.float32, device=x.device)
+    assert out.dtype == torch.float32 and out.shape[0] == ch and out.stride(1) == 1
+    st = _Resampler()
+    rc = _check(lib().csdrb_rational_resampler_bank_ff(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, interpolation, decimation,
+                                                       _fp(taps), taps.size, last_taps_delay, C.byref(st), _stream()), "rational_resampler_bank_ff")
+    assert out.shape[1] >= rc
+    return out[:, :rc], (st.input_processed, st.output_size, st.last_taps_delay)
 
 
 def fastagc_bank_ff(x, block: int = 1024, reference: float = 1.0, state=None, hist=None):

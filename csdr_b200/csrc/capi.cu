@@ -328,6 +328,19 @@ int csdrb_fractional_decimator_bank_ff(const float* d_in, long in_stride, float*
     return rc < 0 ? rc : counted(0, rc);
 }
 
+int csdrb_rational_resampler_bank_ff(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int input_size, int interpolation,
+                                     int decimation, const float* h_taps, int taps_length, int last_taps_delay, rational_resampler_ff_t* h_state_out,
+                                     void* stream)
+{
+    if (too_many_channels(channels, "rational_resampler bank")) return -1;
+    if (!h_state_out) { set_error("rational_resampler bank: null state pointer"); return -1; }
+    static_assert(sizeof(rational_resampler_ff_t) == 3 * sizeof(int), "state layout");
+    int rc = launch_rational_resampler_bank(d_in, in_stride, d_out, out_stride, channels, input_size, interpolation, decimation, h_taps, taps_length,
+                                            last_taps_delay, reinterpret_cast<int*>(h_state_out), S(stream));
+    if (rc > 0 && channels > 0) counted(0, 1);
+    return rc;
+}
+
 size_t csdrb_fastagc_bank_scratch_bytes(int channels, int nblocks) { return fastagc_scratch_bytes(channels, nblocks); }
 
 int csdrb_fastagc_bank_ff(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int block, int nblocks, float reference,

@@ -283,6 +283,21 @@ void fractional_decimator_ff(float* input, float* output, int input_size, fracti
     d->where = s.where; d->input_processed = s.input_processed; d->output_size = s.output_size;
 }
 
+rational_resampler_ff_t rational_resampler_ff(float* input, float* output, int input_size, int interpolation, int decimation, float* taps,
+                                              int taps_length, int last_taps_delay)
+{
+    Staging st("rational_resampler_ff");
+    const long cap = interpolation > 0 && decimation > 0 && input_size > 0 ? (long)input_size * interpolation / decimation : 0;
+    const float* d_in = st.up(input, input_size);
+    float* d_out = st.alloc<float>(cap);
+    rational_resampler_ff_t s;
+    const int n = st.check(csdrb_rational_resampler_bank_ff(d_in, input_size, d_out, cap, 1, input_size, interpolation, decimation, taps, taps_length,
+                                                            last_taps_delay, &s, st.stream()));
+    st.get(output, d_out, n);
+    st.sync();
+    return s;
+}
+
 void fastagc_ff(fastagc_ff_t* a, float* output)
 {
     const int n = a->input_size;

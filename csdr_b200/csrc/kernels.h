@@ -67,6 +67,14 @@ int launch_fastagc_bank_s16(const float* d_in, long in_stride, short* d_out, lon
 int launch_fastagc_bank(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int block, int nblocks,
                         float reference, void* d_state, float* d_hist, void* d_scratch, size_t scratch_bytes, cudaStream_t st);
 
+// rational_resampler_ff, resample.cu.  The bank returns outputs per channel and writes the reference's state
+// {input_processed, output_size, last_taps_delay} to h_state (host memory) without waiting for the device.
+constexpr int kRsMaxTaps = 16384;
+int rational_resampler_state(int input_size, int interpolation, int decimation, int taps_length, int last_taps_delay, int* h_state);
+int launch_rational_resampler_bank(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int input_size,
+                                   int interpolation, int decimation, const float* h_taps, int taps_length, int last_taps_delay,
+                                   int* h_state, cudaStream_t st);
+
 // AM / SSB receiver blocks, agc.cu.  AgcParams / AgcState have the layout of csdrb_agc_params_t / csdrb_agc_state_t (include/csdr_b200.h).
 struct AgcParams { float reference, attack_rate, decay_rate, max_gain; int hang_time, attack_wait_time; float gain_filter_alpha; int chunk; };
 struct AgcState { float gain, last_peak; int hang_counter, attack_wait_counter, offset; };

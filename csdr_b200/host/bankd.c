@@ -13,12 +13,15 @@
  * first -- is process plumbing and is not reproduced; tests/test_gpu_zzz_bankd.py compares against the oracle run over the whole stream).
  *
  * usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]
- *                   [--tail nfm|none|am|usb|lsb|iq] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]  RATE:SINK [RATE:SINK ...]
+ *                   [--tail nfm|none|am|usb|lsb|iq] [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]
+ *                   RATE:SINK [RATE:SINK ...]
  *   --tail: nfm (default) the README.md:87 tail, s16; none the raw discriminator output, f32; am / usb / lsb the AM and SSB graphs of README.md:95 and :110
  *   behind the DDC's complex baseband (see bb_tail_t), s16; iq the complex baseband itself, cf32.  --limit is limit_ff's amplitude (default 1), --agc-ref
  *   the AGC reference (default: fastagc_ff's 1.0 for nfm, agc_ff's 0.2 for am/usb/lsb).
  *   --decimation: any even D (default 50) whose filter the fused bank serves: M = ceil(taps / D) <= 24 and D * M (rounded up to the kernel's
- *   bucket) <= 8000 taps, see csdrb_ddc_bank in include/csdr_b200.h.  The NFM tail's deemphasis_nfm_ff stays at 48000 whatever D gives.
+ *   bucket) <= 8000 taps, see csdrb_ddc_bank in include/csdr_b200.h.  The NFM tail's deemphasis_nfm_ff stays at 48000 whatever D gives: where
+ *   wideband rate / D is not 48 kHz, --resample I:D[:BW] puts rational_resampler_ff I D BW right behind the discriminator (tails nfm and none; see
+ *   --help for the geometries it serves), e.g. 2.048 Msps with --decimation 32 --resample 3:4, or 10 Msps with --decimation 200 --resample 24:25:0.02.
  *   RATE  shift_addition_cc rate (fraction of the wideband sample rate), SINK a path (file or FIFO) or tcp:PORT (one listener).
  *   --devices: the channels are sliced over several GPUs of this node (csdrb_multi_bank_*: the block goes to the first device once and on to
  *   the others by NCCL broadcast), one block of latency more (two blocks are kept in flight); the audio tail (nfm, am, usb, lsb), audio-rate work, runs on
@@ -221,6 +224,64 @@ static void nfm_tail_push(nfm_tail_t *t, channel_t *chan, int n_new, void *strea
     }
 }
 
+/* ---- --resample I:D[:BW]: rational_resampler_ff I D BW right behind the discriminator (tails nfm and none) ---------------------------------------------------
+ *   rs_in : [C][rs] float : [inputs the previous call left unconsumed (<= T/I) | new discriminator samples]
+ * Each call ends because its input runs out, never on the output cap (resample_geometry_ok), so the state carries over exactly and every
+ * channel's stream is the one a single rational_resampler_ff call over the whole discriminator stream gives. */
+typedef struct {
+    int C, I, D, T, ltd, have;
+    long rs;
+    float *taps, *d_in, *d_carry;
+} rs_stage_t;
+
+/* A call on n inputs computes outputs while the input lasts, floor((L*I + ltd) / D) + 1 of them with L = n - T/I - 1, and stops at the cap floor(n*I/D);
+ * ending on the cap repeats that call's last output in the next call.  The input always runs out first when (T/I + 1)*I >= 2*D + I - 1, whatever n and
+ * ltd < I (then (L*I + ltd)/D + 2 <= n*I/D); T >= 2*D + I - 2 is enough for that. */
+static int resample_geometry_ok(int I, int D, int T) { return (long)(T / I + 1) * I >= 2L * D + I - 1; }
+
+static void rs_init(rs_stage_t *r, int C, int I, int D, float bw, int in_cap)
+{
+    memset(r, 0, sizeof *r);
+    r->C = C; r->I = I; r->D = D; r->T = firdes_filter_len(bw);
+    r->taps = malloc(sizeof(float) * (size_t)r->T);
+    if (!r->taps) die("out of memory");
+    rational_resampler_get_lowpass_f(r->taps, r->T, I, D, WINDOW_HAMMING);
+    rational_resampler_ff_t st;                                      /* zero channels: the bank only checks the geometry */
+    if (csdrb_rational_resampler_bank_ff(NULL, 0, NULL, 0, 0, 0, I, D, r->taps, r->T, 0, &st, NULL) < 0) die("--resample: the resampler refuses this geometry");
+    r->rs = ((long)r->T / I + 2 + in_cap + 3) & ~3L;
+    r->d_in = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)r->rs);
+    r->d_carry = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)r->rs);
+    if (!r->d_in || !r->d_carry) die("out of memory");
+}
+
+static int rs_out_cap(const rs_stage_t *r) { return (int)(r->rs * r->I / r->D) + 1; }
+
+/* n_new fresh discriminator samples per channel sit at d_in + have: resample into dst (row pitch dst_pitch floats), keep what the call left unconsumed;
+ * returns the outputs per channel */
+static int rs_push(rs_stage_t *r, int n_new, float *dst, long dst_pitch, void *stream)
+{
+    const int n = r->have + n_new;
+    rational_resampler_ff_t st;
+    const int m = csdrb_rational_resampler_bank_ff(r->d_in, r->rs, dst, dst_pitch, r->C, n, r->I, r->D, r->taps, r->T, r->ltd, &st, stream);
+    if (m < 0) die("csdrb_rational_resampler_bank_ff failed");
+    const int keep = n - st.input_processed;
+    if (keep > 0 && st.input_processed > 0) {
+        const size_t row = sizeof(float) * (size_t)r->rs;
+        OK(csdrb_copy2d_d2d(r->d_carry, row, r->d_in + st.input_processed, row, sizeof(float) * (size_t)keep, (size_t)r->C, stream));
+        OK(csdrb_copy2d_d2d(r->d_in, row, r->d_carry, row, sizeof(float) * (size_t)keep, (size_t)r->C, stream));
+    }
+    r->have = keep; r->ltd = st.last_taps_delay;
+    return m;
+}
+
+/* --tail none: n float samples per channel (device rows, pitch `pitch`) to the sinks */
+static void raw_emit(const float *d_rows, long pitch, int n, unsigned char *h_out, channel_t *chan, int C, void *stream)
+{
+    OK(csdrb_copy2d_d2h(h_out, sizeof(float) * (size_t)n, d_rows, sizeof(float) * (size_t)pitch, sizeof(float) * (size_t)n, (size_t)C, stream));
+    OK(csdrb_stream_synchronize(stream));
+    for (int c = 0; c < C; c++) write_sink(&chan[c], h_out + sizeof(float) * (size_t)c * (size_t)n, sizeof(float) * (size_t)n);
+}
+
 /* ---- the AM and SSB audio tails (README.md:95, :110) behind the DDC bank's complex baseband ------------------------------------------------------------------
  *   am      : amdemod_cf | fastdcblock_ff 1024 | agc_ff | limit_ff L | convert_f_s16
  *   usb/lsb : bandpass_fir_fft_cc 0 0.1 0.05 (or -0.1 0 0.05) | realpart_cf | agc_ff | limit_ff L | convert_f_s16
@@ -327,7 +388,7 @@ static void bb_tail_push(bb_tail_t *t, channel_t *chan, int n_new, void *stream)
 }
 
 static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *chan, int C, const float *rates, int D, const float *taps, int T, int block,
-                     int kind, float limit, float agc_ref)
+                     int kind, float limit, float agc_ref, int rs_I, int rs_D, float rs_bw)
 {
     const int nfm = kind == TAIL_NFM, demod = kind == TAIL_NFM || kind == TAIL_NONE;
     const size_t osz = demod ? sizeof(float) : sizeof(complexf);
@@ -342,16 +403,31 @@ static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *cha
     if (!h_wide[0] || !h_wide[1] || !h_out[0] || !h_out[1] || !raw) die("out of memory");
     /* --tail nfm: the audio tail is audio-rate work (C x 48 kHz): the discriminator rows every device returned go to the FIRST device once more and through
      * the same kernels as in the single-GPU path */
-    nfm_tail_t tail_state; bb_tail_t bb; void *tail_stream = NULL;
-    if (kind != TAIL_NONE) {
+    nfm_tail_t tail_state; bb_tail_t bb; rs_stage_t rsm; void *tail_stream = NULL;
+    float *d_raw_out = NULL; unsigned char *h_raw_out = NULL;
+    const int resample = rs_I > 0;
+    if (kind != TAIL_NONE || resample) {
         OK(csdrb_set_device(dev[0]));
         tail_stream = csdrb_stream_create();
         if (!tail_stream) die("cannot create a stream");
-        if (nfm) nfm_tail_init(&tail_state, C, n_out + 2, limit, agc_ref);
-        else bb_tail_init(&bb, kind, C, n_out + 2, limit, agc_ref, tail_stream);
+        if (resample) rs_init(&rsm, C, rs_I, rs_D, rs_bw, n_out + 2);
+        const int tail_cap = resample ? rs_out_cap(&rsm) : n_out + 2;
+        if (nfm) nfm_tail_init(&tail_state, C, tail_cap, limit, agc_ref);
+        else if (!demod) bb_tail_init(&bb, kind, C, tail_cap, limit, agc_ref, tail_stream);
+        else {
+            d_raw_out = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)tail_cap);
+            h_raw_out = csdrb_host_alloc(sizeof(float) * (size_t)C * (size_t)tail_cap);
+            if (!d_raw_out || !h_raw_out) die("out of memory");
+        }
     }
+    /* --resample: the discriminator rows go to the first device's resampler, its output into the tail (or straight to the sinks for --tail none) */
 #define EMIT(slot_) do { \
-        if (nfm) { \
+        if (resample) { \
+            OK(csdrb_copy2d_h2d(rsm.d_in + rsm.have, sizeof(float) * (size_t)rsm.rs, h_out[slot_], sizeof(float) * (size_t)n_out, \
+                                sizeof(float) * (size_t)n_out, (size_t)C, tail_stream)); \
+            if (nfm) nfm_tail_push(&tail_state, chan, rs_push(&rsm, n_out, tail_state.d_demod + tail_state.a_have, tail_state.ds, tail_stream), tail_stream); \
+            else { const int m_ = rs_push(&rsm, n_out, d_raw_out, rs_out_cap(&rsm), tail_stream); raw_emit(d_raw_out, rs_out_cap(&rsm), m_, h_raw_out, chan, C, tail_stream); } \
+        } else if (nfm) { \
             OK(csdrb_copy2d_h2d(tail_state.d_demod + tail_state.a_have, sizeof(float) * (size_t)tail_state.ds, h_out[slot_], sizeof(float) * (size_t)n_out, \
                                 sizeof(float) * (size_t)n_out, (size_t)C, tail_stream)); \
             nfm_tail_push(&tail_state, chan, n_out, tail_stream); \
@@ -396,11 +472,27 @@ static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *cha
     return 0;
 }
 
+static int usage(void)
+{
+    fprintf(stderr,
+            "usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]\n"
+            "                  [--tail nfm|none|am|usb|lsb|iq] [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]\n"
+            "                  RATE:SINK [RATE:SINK ...]\n"
+            "  --resample I:D[:BW]  rational_resampler_ff I D BW (BW default 0.05) right behind the discriminator, for --tail nfm and none: brings\n"
+            "                       wideband/decimation to the 48 kHz the NFM de-emphasis is designed for (e.g. 2.048 Msps, --decimation 32,\n"
+            "                       --resample 3:4).  With T = taps of BW, the daemon needs (T/I + 1)*I >= 2*D + I - 1 (T >= 2*D + I - 2 suffices),\n"
+            "                       so that no resampler call ends on its output cap; other geometries are refused.\n"
+            "  see the head of csdr_b200/host/bankd.c for the other options\n");
+    return 2;
+}
+
 int main(int argc, char **argv)
 {
     const char *in_spec = "-", *tail = "nfm";
     int u8 = 1, D = 50, block = 1 << 18, device = 0, ndev = 0, devs[64];
     float bw = 0.005f, limit = 1.0f, agc_ref = 0.0f;                /* agc_ref 0: the tail's own default (fastagc_ff 1.0, agc_ff 0.2) */
+    int rs_I = 0, rs_D = 0;                                          /* --resample I:D[:BW]; 0: no resampler */
+    float rs_bw = 0.05f;                                             /* rational_resampler_ff's default transition bandwidth (csdr.c:1423) */
     window_t window = WINDOW_HAMMING;
     channel_t *chan = calloc((size_t)argc, sizeof *chan);
     int C = 0;
@@ -419,6 +511,11 @@ int main(int argc, char **argv)
         else if (!strcmp(o, "--agc-ref") && v) { agc_ref = (float)atof(v); a++; }
         else if (!strcmp(o, "--device") && v) { device = atoi(v); a++; }
         else if (!strcmp(o, "--devices") && v) { ndev = parse_devices(v, devs, 64); if (ndev <= 0) die("--devices wants N0,N1,..."); a++; }
+        else if (!strcmp(o, "--resample") && v) {
+            if (sscanf(v, "%d:%d:%f", &rs_I, &rs_D, &rs_bw) < 2 || rs_I < 1 || rs_D < 1) die("--resample wants I:D[:BW] with positive integers I and D");
+            a++;
+        }
+        else if (!strcmp(o, "--help")) return usage();
         else if (strchr(o, ':') && o[0] != '-' ) {
             char *end = NULL;
             chan[C].rate = strtof(o, &end);
@@ -442,6 +539,17 @@ int main(int argc, char **argv)
     if (D <= 0 || (D & 1)) die("--decimation must be a positive even number (the fused bank serves even decimations only)");
     if (!(bw > 0.f && bw < 0.5f)) die("--bw must be a transition bandwidth between 0 and 0.5");
     if (!(limit > 0.f) || !(agc_ref >= 0.f)) die("--limit and --agc-ref must be positive");
+    const int resample = rs_I > 0;
+    if (resample) {
+        if (!demod) die("--resample works with --tail nfm and --tail none only (the am, usb, lsb and iq tails are not resampled)");
+        if (!(rs_bw > 0.f && rs_bw < 0.5f)) die("--resample: the transition bandwidth must be between 0 and 0.5");
+        const int rs_T = firdes_filter_len(rs_bw);
+        if (!resample_geometry_ok(rs_I, rs_D, rs_T)) {
+            fprintf(stderr, "csdr-bankd: --resample %d:%d with %d taps: a resampler call could end on its output cap and repeat an output; "
+                            "the daemon needs (T/I + 1)*I >= 2*D + I - 1 (T >= 2*D + I - 2 suffices): lower the transition bandwidth\n", rs_I, rs_D, rs_T);
+            return 1;
+        }
+    }
     signal(SIGPIPE, SIG_IGN);
 
     /* ---- filter and bank ---------------------------------------------------------------------------------------------------- */
@@ -456,7 +564,7 @@ int main(int argc, char **argv)
         for (int c = 0; c < C; c++) { chan[c].fd = open_sink(chan[c].sink); sink_nonblocking(chan[c].fd); }
         const int fd = open_input(in_spec);
         fprintf(stderr, "csdr-bankd: %d channels over %d devices, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, ndev, D, T, u8 ? "u8" : "f32", block, tail);
-        const int rc = run_multi(fd, u8, devs, ndev, chan, C, rates, D, taps, T, block, kind, limit, agc_ref);
+        const int rc = run_multi(fd, u8, devs, ndev, chan, C, rates, D, taps, T, block, kind, limit, agc_ref, rs_I, rs_D, rs_bw);
         for (int c = 0; c < C; c++) { if (chan[c].dropped) fprintf(stderr, "csdr-bankd: sink %s lost %ld bytes (too slow)\n", chan[c].sink, chan[c].dropped); if (chan[c].fd >= 0) close(chan[c].fd); }
         return rc;
     }
@@ -477,10 +585,13 @@ int main(int argc, char **argv)
     const int out_cap = wide_cap / D + 2;                          /* discriminator samples one block can add */
     nfm_tail_t tl;
     bb_tail_t bb;
-    long ds = ((long)out_cap + 3) & ~3L;
+    rs_stage_t rsm;
+    if (resample) rs_init(&rsm, C, rs_I, rs_D, rs_bw, out_cap);
+    const int tail_cap = resample ? rs_out_cap(&rsm) : out_cap;   /* samples one block can add behind the discriminator (and resampler) */
+    long ds = ((long)tail_cap + 3) & ~3L;
     float *d_demod = NULL;
     unsigned char *h_out = NULL;
-    if (nfm) { nfm_tail_init(&tl, C, out_cap, limit, agc_ref); ds = tl.ds; d_demod = tl.d_demod; }
+    if (nfm) { nfm_tail_init(&tl, C, tail_cap, limit, agc_ref); ds = tl.ds; d_demod = tl.d_demod; }
     else if (!demod) { bb_tail_init(&bb, kind, C, out_cap, limit, agc_ref, stream); ds = bb.bs; d_demod = (float *)bb.d_bb; }
     else {
         d_demod = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)ds);
@@ -511,20 +622,19 @@ int main(int argc, char **argv)
         const int n_in = block;
 
         /* 2. shift | fir_decimate | fmdemod for every channel, new discriminator samples behind the de-emphasis FIR's carried inputs */
-        void *dst = nfm ? (void *)(d_demod + tl.a_have) : !demod ? (void *)(bb.d_bb + bb.have) : (void *)d_demod;
-        const int n_out = csdrb_ddc_bank_process(bank, d_wide[cur], n_in, dst, ds, stream);
+        void *dst = resample ? (void *)(rsm.d_in + rsm.have) : nfm ? (void *)(d_demod + tl.a_have) : !demod ? (void *)(bb.d_bb + bb.have) : (void *)d_demod;
+        const int n_out = csdrb_ddc_bank_process(bank, d_wide[cur], n_in, dst, resample ? rsm.rs : ds, stream);
         if (n_out < 0) die("csdrb_ddc_bank_process failed");
         const int consumed = n_out * D;
         keep = n_in - consumed;
         OK(csdrb_copy_d2d(d_wide[cur ^ 1], d_wide[cur] + consumed, sizeof(complexf) * (size_t)keep, stream));
         cur ^= 1;
 
+        /* 2b. --resample: the new discriminator samples through rational_resampler_ff, into the tail's rows */
+        const int n_tail = resample ? rs_push(&rsm, n_out, nfm ? d_demod + tl.a_have : d_demod, ds, stream) : n_out;
         if (!demod) bb_tail_push(&bb, chan, n_out, stream);         /* baseband tails: am / usb / lsb audio, or the raw baseband */
-        else if (!nfm) {                                           /* raw discriminator output, float */
-            OK(csdrb_copy2d_d2h(h_out, sizeof(float) * (size_t)n_out, d_demod, sizeof(float) * (size_t)ds, sizeof(float) * (size_t)n_out, (size_t)C, stream));
-            OK(csdrb_stream_synchronize(stream));
-            for (int c = 0; c < C; c++) write_sink(&chan[c], h_out + sizeof(float) * (size_t)c * (size_t)n_out, sizeof(float) * (size_t)n_out);
-        } else nfm_tail_push(&tl, chan, n_out, stream);           /* 3./4. limit | de-emphasis | AGC | s16, audio to the sinks */
+        else if (!nfm) raw_emit(d_demod, ds, n_tail, h_out, chan, C, stream);   /* raw discriminator output, float */
+        else nfm_tail_push(&tl, chan, n_tail, stream);             /* 3./4. limit | de-emphasis | AGC | s16, audio to the sinks */
         blocks++;
     }
     OK(csdrb_stream_synchronize(stream));

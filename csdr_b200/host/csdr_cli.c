@@ -561,6 +561,40 @@ static int cmd_fractional_decimator_ff(int argc, char **argv)
     }
 }
 
+static int cmd_rational_resampler_ff(int argc, char **argv)                 /* csdr.c:1409-1462 */
+{
+    if (argc <= 3) return complain("need required parameters (interpolation, decimation)");
+    int interpolation = 0, decimation = 0;
+    sscanf(argv[2], "%d", &interpolation); sscanf(argv[3], "%d", &decimation);
+    float transition_bw = 0.05f; if (argc >= 5) sscanf(argv[4], "%g", &transition_bw);
+    window_t window = WINDOW_DEFAULT;
+    if (argc >= 6) window = firdes_get_window_from_string(argv[5]);
+    else { who(); fprintf(stderr, "window = %s\n", firdes_get_string_from_window(window)); }
+    if (!open_block()) return -2;
+    float *in = must_alloc(sizeof(float) * (size_t)block);
+    if (interpolation == 1 && decimation == 1) {                        /* pass-through special case (:1438, clone_) */
+        announce_block(block);
+        for (;;) { fread(in, 1, (size_t)block, stdin); fwrite(in, 1, (size_t)block, stdout); end_of_block(); if (feof(stdin)) return 0; }
+    }
+    if (interpolation < 1 || decimation < 1) return complain("interpolation and decimation must be positive integers");
+    const int out_size = (int)((long)block * interpolation / decimation);
+    announce_block(out_size);
+    float *out = must_alloc(sizeof(float) * (size_t)(out_size > 0 ? out_size : 1));
+    const int taps_length = firdes_filter_len(transition_bw);
+    float *taps = must_alloc(sizeof(float) * (size_t)taps_length);
+    rational_resampler_get_lowpass_f(taps, taps_length, interpolation, decimation, window);
+    rational_resampler_ff_t d = {0, 0, 0};                              /* the reference's static (.bss) state */
+    for (;;) {
+        if (feof(stdin)) return 0;
+        if (d.input_processed == 0) d.input_processed = block;
+        else memmove(in, in + d.input_processed, sizeof(float) * (size_t)(block - d.input_processed));
+        fread(in + (block - d.input_processed), sizeof(float), (size_t)d.input_processed, stdin);
+        d = rational_resampler_ff(in, out, block, interpolation, decimation, taps, taps_length, d.last_taps_delay);
+        fwrite(out, sizeof(float), (size_t)d.output_size, stdout);
+        end_of_block();
+    }
+}
+
 static int cmd_fastagc_ff(int argc, char **argv)
 {
     static fastagc_ff_t agc;                                            /* zero-initialised like the reference's .bss copy */
@@ -780,6 +814,7 @@ static const struct { const char *name; int (*run)(int, char **); const char *sy
     {"fir_decimate_cc", cmd_fir_decimate_cc, "fir_decimate_cc <decimation_factor> [transition_bw [window]]"},
     {"fmdemod_quadri_cf", cmd_fmdemod_quadri_cf, "fmdemod_quadri_cf"},
     {"fractional_decimator_ff", cmd_fractional_decimator_ff, "fractional_decimator_ff <decimation_rate> [num_poly_points ( [transition_bw [window]] | --prefilter )]"},
+    {"rational_resampler_ff", cmd_rational_resampler_ff, "rational_resampler_ff <interpolation> <decimation> [transition_bw [window]]"},
     {"fastagc_ff", cmd_fastagc_ff, "fastagc_ff [block_size [reference]]"},
     {"limit_ff", cmd_limit_ff, "limit_ff [max_amplitude]"},
     {"amdemod_cf", cmd_amdemod_cf, "amdemod_cf"},

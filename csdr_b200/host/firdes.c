@@ -82,6 +82,14 @@ void firdes_lowpass_f(float *output, int length, float cutoff_rate, window_t win
     for (int k = 0; k < length; k++) output[k] = output[k] / dc_gain;
 }
 
+/* rational_resampler_ff's anti-imaging / anti-aliasing lowpass (libcsdr.c:665-673): cutoff at half the lower of 1/I and 1/D */
+void rational_resampler_get_lowpass_f(float *output, int output_size, int interpolation, int decimation, window_t window)
+{
+    const float for_interpolation = (float)(1.0 / interpolation), for_decimation = (float)(1.0 / decimation);
+    const float cutoff = for_interpolation < for_decimation ? for_interpolation : for_decimation;
+    firdes_lowpass_f(output, output_size, cutoff / 2, window);
+}
+
 void firdes_bandpass_c(complexf *output, int length, float lowcut, float highcut, window_t window)
 {
     float *prototype = (float *)malloc(sizeof(float) * (size_t)(length > 0 ? length : 1));

@@ -77,6 +77,15 @@ typedef struct fractional_decimator_ff_s {
 fractional_decimator_ff_t fractional_decimator_ff_init(float rate, int num_poly_points, float *taps, int taps_length);
 void fractional_decimator_ff(float *input, float *output, int input_size, fractional_decimator_ff_t *d);
 
+/* rational resampler (libcsdr.h:132-140; libcsdr.c:607-673).  The returned state is the reference's: when the input runs out, the index pair
+ * of the first output not produced; when the output cap input_size*interpolation/decimation ends the call, the pair of the last output
+ * produced (the next call computes it again).  With no output at all the reference leaves the fields uninitialised; here they are
+ * {0, 0, last_taps_delay}.  At most 16384 taps; input_size*interpolation must not exceed INT_MAX (the reference's int arithmetic). */
+typedef struct rational_resampler_ff_s { int input_processed; int output_size; int last_taps_delay; } rational_resampler_ff_t;
+rational_resampler_ff_t rational_resampler_ff(float *input, float *output, int input_size, int interpolation, int decimation, float *taps,
+                                              int taps_length, int last_taps_delay);
+void rational_resampler_get_lowpass_f(float *output, int output_size, int interpolation, int decimation, window_t window);
+
 /* block AGC (libcsdr.h:118-130; libcsdr.c:944-991) */
 typedef struct fastagc_ff_s {
     float *buffer_1; float *buffer_2; float *buffer_input;
@@ -337,6 +346,16 @@ size_t csdrb_fractional_decimator_bank_scratch_bytes(int channels, int input_siz
 int csdrb_fractional_decimator_bank_ff(const float *d_in, long in_stride, float *d_out, long out_stride, int channels, int input_size,
                                        float rate, int num_poly_points, const float *d_taps, int taps_length,
                                        csdrb_fracdec_state_t *d_state, void *d_scratch, size_t scratch_bytes, void *stream);
+
+/* rational_resampler_ff bank: every row resampled by interpolation/decimation with the shared h_taps (HOST pointer, copied on the stream) and
+ * one shared last_taps_delay, rows in lockstep.  Each output is summed in the reference's order, so a row equals rational_resampler_ff() on
+ * it bit for bit against a strict-IEEE build of the reference source.  Returns outputs per row and writes the reference's returned state
+ * (see rational_resampler_ff above) to *h_state_out on the host, computed from the sizes alone: the call stays asynchronous.
+ * -1 for invalid arguments (interpolation or decimation < 1, no taps, last_taps_delay outside 0..interpolation-1), -2 for more than
+ * 16384 taps or input_size*interpolation > INT_MAX. */
+int csdrb_rational_resampler_bank_ff(const float *d_in, long in_stride, float *d_out, long out_stride, int channels, int input_size,
+                                     int interpolation, int decimation, const float *h_taps, int taps_length, int last_taps_delay,
+                                     rational_resampler_ff_t *h_state_out, void *stream);
 
 /* K6 fastagc_ff bank: nblocks consecutive blocks of `block` samples per channel; d_hist is [channels][2][block]
  * (the reference's buffer_1, buffer_2; zero it at stream start), d_state[c] = {peak_1, peak_2, last_gain}. */
