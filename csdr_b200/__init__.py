@@ -57,6 +57,16 @@ class AgcParams(C.Structure):           # csdrb_agc_params_t; defaults = the agc
         super().__init__(reference, attack_rate, decay_rate, max_gain, hang_time, attack_wait_time, gain_filter_alpha, chunk)
 
 
+class TimingRecoveryParams(C.Structure):    # csdrb_timing_recovery_params_t; algorithm 0 = GARDNER, 1 = EARLYLATE
+    _fields_ = [("algorithm", C.c_int), ("decimation", C.c_int), ("use_q", C.c_int), ("loop_gain", C.c_float), ("max_error", C.c_float)]
+
+
+class _TimingRecovery(C.Structure):     # timing_recovery_state_t (= libcsdr.h:322-336)
+    _fields_ = [("algorithm", C.c_int), ("decimation_rate", C.c_int), ("output_size", C.c_int), ("input_processed", C.c_int),
+                ("use_q", C.c_int), ("debug_phase", C.c_int), ("debug_every_nth", C.c_int), ("debug_writefiles_path", C.c_char_p),
+                ("last_correction_offset", C.c_int), ("earlylate_ratio", C.c_float), ("loop_gain", C.c_float), ("max_error", C.c_float)]
+
+
 class _Unroll(C.Structure):             # shift_unroll_data_t (= libcsdr.h:199-205)
     _fields_ = [("dsin", C.POINTER(C.c_float)), ("dcos", C.POINTER(C.c_float)), ("phase_increment", C.c_float), ("size", C.c_int)]
 
@@ -220,6 +230,14 @@ def lib() -> C.CDLL:
     L.convert_f_s16.argtypes = [vp, vp, it]
     L.fir_decimate_cc.argtypes = [vp, vp, it, it, C.POINTER(C.c_float), it]
     L.fmdemod_quadri_cf.argtypes = [vp, vp, it, vp, _CF]; L.fmdemod_quadri_cf.restype = _CF
+    L.csdrb_simple_agc_bank_cc.argtypes = [vp, lg, vp, lg, it, it, C.c_float, C.c_float, C.c_float, vp, vp]
+    L.csdrb_timing_recovery_bank_cc.argtypes = [vp, lg, vp, vp, it, vp, lg, vp, vp, it, C.POINTER(TimingRecoveryParams), vp, vp]
+    L.csdrb_dbpsk_decoder_bank_c_u8.argtypes = [vp, lg, vp, lg, it, it, vp, vp, vp, vp]
+    L.csdrb_psk31_varicode_decoder_bank_u8_u8.argtypes = [vp, lg, vp, lg, it, it, vp, vp, vp, vp]
+    L.simple_agc_cc.argtypes = [vp, vp, it, C.c_float, C.c_float, C.c_float, vp]
+    L.dbpsk_decoder_c_u8.argtypes = [vp, vp, it]
+    L.timing_recovery_init.argtypes = [it, it, it, C.c_float, C.c_float, it, C.c_char_p]; L.timing_recovery_init.restype = _TimingRecovery
+    L.timing_recovery_cc.argtypes = [vp, vp, it, vp, vp, C.POINTER(_TimingRecovery)]
     _lib = L
     return L
 
@@ -432,6 +450,29 @@ class libcsdr:
     def convert_u8_f(x):
         x = np.ascontiguousarray(x, np.uint8); y = np.empty(x.size, np.float32)
         lib().convert_u8_f(x.ctypes.data, y.ctypes.data, x.size); return y
+
+    @staticmethod
+    def simple_agc_cc(x, rate, reference=1.0, max_gain=65535.0, gain=1.0):
+        """-> (y, gain)"""
+        x = np.ascontiguousarray(x, np.complex64); y = np.empty_like(x); g = np.array([gain], np.float32)
+        lib().simple_agc_cc(x.ctypes.data, y.ctypes.data, x.size, rate, reference, max_gain, g.ctypes.data); return y, float(g[0])
+
+    @staticmethod
+    def dbpsk_decoder_c_u8(x):
+        """the previous sample of the last call is library state, as in the reference"""
+        x = np.ascontiguousarray(x, np.complex64); y = np.empty(x.size, np.uint8)
+        lib().dbpsk_decoder_c_u8(x.ctypes.data, y.ctypes.data, x.size); return y
+
+    @staticmethod
+    def timing_recovery_cc(x, algorithm, decimation, use_q=True, loop_gain=0.5, max_error=2.0, last_correction_offset=0):
+        """-> (symbols, error, indexes, (last_correction_offset, input_processed, output_size))"""
+        x = np.ascontiguousarray(x, np.complex64); cap = max(x.size, 1)
+        y = np.empty(cap, np.complex64); e = np.empty(cap, np.float32); ix = np.empty(cap, np.int32)
+        st = lib().timing_recovery_init(algorithm, decimation, int(use_q), loop_gain, max_error, -1, None)
+        st.last_correction_offset = last_correction_offset
+        lib().timing_recovery_cc(x.ctypes.data, y.ctypes.data, x.size, e.ctypes.data, ix.ctypes.data, C.byref(st))
+        m = st.output_size
+        return y[:m].copy(), e[:m].copy(), ix[:m].copy(), (st.last_correction_offset, st.input_processed, m)
 
     @staticmethod
     def convert_s16_f(x):
@@ -934,6 +975,69 @@ def agc_bank_ff(x, params: AgcParams | None = None, state=None, limit_max: float
     _check(lib().csdrb_agc_bank_ff(x.data_ptr(), x.stride(0), int(x.dtype == torch.complex64), out.data_ptr(), out.stride(0), int(s16), ch, n,
                                    C.byref(params), state.data_ptr(), limit_max, _stream()), "agc_bank_ff")
     return out, state
+
+
+def simple_agc_bank_cc(x, rate: float = 0.001, reference: float = 1.0, max_gain: float = 65535.0, gain=None):
+    """simple_agc_cc per row: x [C, N] complex64 -> (y [C, N], gain [C] float32, carried between calls; 1.0 at stream start)"""
+    import torch
+    assert x.dtype == torch.complex64 and x.is_cuda and x.dim() == 2 and x.stride(1) == 1
+    ch, n = x.shape
+    gain = torch.ones(ch, dtype=torch.float32, device=x.device) if gain is None else gain
+    out = torch.empty((ch, n), dtype=torch.complex64, device=x.device)
+    _check(lib().csdrb_simple_agc_bank_cc(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, rate, reference, max_gain, gain.data_ptr(),
+                                          _stream()), "simple_agc_bank_cc")
+    return out, gain
+
+
+def timing_recovery_bank_cc(x, algorithm: int, decimation: int, use_q: bool = True, loop_gain: float = 0.5, max_error: float = 2.0,
+                            start=None, size=None, state=None, outputs: str = "symbols"):
+    """one timing_recovery_cc call per row over x[c, start[c]:start[c] + size[c]] (start 0 and size N by default): returns
+    (symbols [C, cap] complex64, error [C, cap] float32 or None, indexes [C, cap] int32 or None, state [C, 3] int32 =
+    {last_correction_offset, input_processed, output_size}).  Pass `state` back to continue a stream; its counts are data-dependent."""
+    import torch
+    assert x.dtype == torch.complex64 and x.is_cuda and x.dim() == 2 and x.stride(1) == 1
+    ch, n = x.shape
+    start = torch.zeros(ch, dtype=torch.int32, device=x.device) if start is None else start
+    size = torch.full((ch,), n, dtype=torch.int32, device=x.device) if size is None else size
+    state = torch.zeros((ch, 3), dtype=torch.int32, device=x.device) if state is None else state
+    # room for every symbol one call can make: n/(decimation/2) + 1 while |loop_gain*max_error| <= 1, n above (a symbol may not advance)
+    cap = (n // (decimation // 2) + 1 if abs(loop_gain * max_error) <= 1 else max(n, 1)) if decimation >= 2 else 1
+    out = torch.empty((ch, cap), dtype=torch.complex64, device=x.device)
+    err = torch.empty((ch, cap), dtype=torch.float32, device=x.device)
+    idx = torch.empty((ch, cap), dtype=torch.int32, device=x.device)
+    p = TimingRecoveryParams(algorithm, decimation, int(use_q), loop_gain, max_error)
+    _check(lib().csdrb_timing_recovery_bank_cc(x.data_ptr(), x.stride(0), start.data_ptr(), size.data_ptr(), n, out.data_ptr(), cap, err.data_ptr(),
+                                               idx.data_ptr(), ch, C.byref(p), state.data_ptr(), _stream()), "timing_recovery_bank_cc")
+    return out, err, idx, state
+
+
+def dbpsk_decoder_bank_c_u8(x, lengths=None, last=None):
+    """dbpsk_decoder_c_u8 per row: x [C, N] complex64 (row c holds lengths[c] samples) -> (bits [C, N] uint8, last sample [C] complex64)"""
+    import torch
+    assert x.dtype == torch.complex64 and x.is_cuda and x.dim() == 2 and x.stride(1) == 1
+    ch, n = x.shape
+    last = torch.zeros(ch, dtype=torch.complex64, device=x.device) if last is None else last
+    new_last = torch.empty_like(last)
+    out = torch.zeros((ch, n), dtype=torch.uint8, device=x.device)
+    _check(lib().csdrb_dbpsk_decoder_bank_c_u8(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n,
+                                               lengths.data_ptr() if lengths is not None else None, last.data_ptr(), new_last.data_ptr(), _stream()),
+           "dbpsk_decoder_bank_c_u8")
+    return out, new_last
+
+
+def psk31_varicode_decoder_bank_u8_u8(bits, lengths=None, hist=None):
+    """the varicode decoder per row: bits [C, N] uint8 (row c holds lengths[c] bits) -> (chars [C, N] uint8, count [C] int32, hist [C] int64,
+    the decoder's shift register carried between calls)"""
+    import torch
+    assert bits.dtype == torch.uint8 and bits.is_cuda and bits.dim() == 2 and bits.stride(1) == 1
+    ch, n = bits.shape
+    hist = torch.zeros(ch, dtype=torch.int64, device=bits.device) if hist is None else hist
+    out = torch.zeros((ch, max(n, 1)), dtype=torch.uint8, device=bits.device)
+    count = torch.zeros(ch, dtype=torch.int32, device=bits.device)
+    _check(lib().csdrb_psk31_varicode_decoder_bank_u8_u8(bits.data_ptr(), bits.stride(0), out.data_ptr(), out.stride(0), ch, n,
+                                                         lengths.data_ptr() if lengths is not None else None, hist.data_ptr(), count.data_ptr(),
+                                                         _stream()), "psk31_varicode_decoder_bank_u8_u8")
+    return out, count, hist
 
 
 def fft_c2c(x, inverse: bool = False):

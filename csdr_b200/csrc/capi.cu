@@ -402,6 +402,48 @@ int csdrb_agc_bank_ff(const void* d_in, long in_stride, int cf32_in, void* d_out
     return rc < 0 ? rc : counted(0, rc);
 }
 
+// BPSK31 receive chain (psk31.cu; libcsdr.c:2201-2217, 1977-2072, 2319-2333, 1536-1549)
+int csdrb_simple_agc_bank_cc(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int input_size, float rate,
+                             float reference, float max_gain, float* d_gain_io, void* stream)
+{
+    if (too_many_channels(channels, "simple_agc bank")) return -1;
+    if (!d_in || !d_out || !d_gain_io) { set_error("simple_agc bank: null pointer"); return -1; }
+    int rc = launch_simple_agc_bank(reinterpret_cast<const float2*>(d_in), in_stride, reinterpret_cast<float2*>(d_out), out_stride, channels, input_size,
+                                    rate, reference, max_gain, d_gain_io, S(stream));
+    return rc < 0 ? rc : counted(input_size > 0 ? input_size : 0, rc);
+}
+
+int csdrb_timing_recovery_bank_cc(const complexf* d_in, long in_stride, const int* d_start, const int* d_size, int max_size, complexf* d_out,
+                                  long out_stride, float* d_error, int* d_indexes, int channels, const csdrb_timing_recovery_params_t* params,
+                                  csdrb_timing_recovery_state_t* d_state, void* stream)
+{
+    static_assert(sizeof(csdrb_timing_recovery_params_t) == sizeof(TrParams) && sizeof(csdrb_timing_recovery_state_t) == sizeof(TrState),
+                  "timing recovery structs mirror kernels.h");
+    if (too_many_channels(channels, "timing_recovery bank")) return -1;
+    if (!d_in || !d_start || !d_size || !d_out || !params || !d_state) { set_error("timing_recovery bank: null pointer"); return -1; }
+    int rc = launch_timing_recovery_bank(reinterpret_cast<const float2*>(d_in), in_stride, d_start, d_size, reinterpret_cast<float2*>(d_out), out_stride,
+                                         d_error, d_indexes, channels, params, d_state, max_size, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
+int csdrb_dbpsk_decoder_bank_c_u8(const complexf* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels, int input_size,
+                                  const int* d_lengths, const complexf* d_last_in, complexf* d_last_out, void* stream)
+{
+    if (null_io(d_in, d_out, "dbpsk bank")) return -1;
+    int rc = launch_dbpsk_bank(reinterpret_cast<const float2*>(d_in), in_stride, d_out, out_stride, channels, input_size, d_lengths,
+                               reinterpret_cast<const float2*>(d_last_in), reinterpret_cast<float2*>(d_last_out), S(stream));
+    return rc < 0 ? rc : counted(input_size > 0 ? input_size : 0, rc);
+}
+
+int csdrb_psk31_varicode_decoder_bank_u8_u8(const unsigned char* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels,
+                                            int input_size, const int* d_lengths, unsigned long long* d_hist_io, int* d_count, void* stream)
+{
+    if (null_io(d_in, d_out, "varicode bank")) return -1;
+    if (!d_hist_io || !d_count) { set_error("varicode bank: null pointer"); return -1; }
+    int rc = launch_varicode_bank(d_in, in_stride, d_out, out_stride, channels, input_size, d_lengths, d_hist_io, d_count, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
 int csdrb_fft_c2c_batch(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int size, int batch, int inverse, void* stream)
 {
     if (!d_in || !d_out) { set_error("fft: null pointer"); return -1; }

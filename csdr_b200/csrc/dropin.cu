@@ -540,4 +540,74 @@ decimating_shift_addition_status_t fastddc_inv_cc(complexf* input, complexf* out
     return shift_stat;
 }
 
+// ---- BPSK31 receive chain ---------------------------------------------------------------------------------
+void simple_agc_cc(complexf* input, complexf* output, int input_size, float rate, float reference, float max_gain, float* current_gain)
+{
+    if (input_size <= 0) return;
+    Staging st("simple_agc_cc");
+    const complexf* d_in = st.up(input, input_size);
+    float* d_gain = st.up(current_gain, 1);
+    complexf* d_out = st.alloc<complexf>(input_size);
+    st.check(csdrb_simple_agc_bank_cc(d_in, input_size, d_out, input_size, 1, input_size, rate, reference, max_gain, d_gain, st.stream()));
+    st.get(output, d_out, input_size);
+    st.get(current_gain, d_gain, 1);
+    st.sync();
+}
+
+// the reference's `static complexf last_input` (libcsdr.c:2321), zero at process start
+static std::mutex g_dbpsk_mu;
+static complexf g_dbpsk_last = {0.f, 0.f};
+
+void dbpsk_decoder_c_u8(complexf* input, unsigned char* output, int input_size)
+{
+    if (input_size <= 0) return;
+    std::lock_guard<std::mutex> lk(g_dbpsk_mu);
+    Staging st("dbpsk_decoder_c_u8");
+    const complexf* d_in = st.up(input, input_size);
+    const complexf* d_last_in = st.up(&g_dbpsk_last, 1);
+    unsigned char* d_out = st.alloc<unsigned char>(input_size);
+    st.check(csdrb_dbpsk_decoder_bank_c_u8(d_in, input_size, d_out, input_size, 1, input_size, nullptr, d_last_in, nullptr, st.stream()));
+    st.get(output, d_out, input_size);
+    st.sync();
+    g_dbpsk_last = input[input_size - 1];
+}
+
+timing_recovery_state_t timing_recovery_init(timing_recovery_algorithm_t algorithm, int decimation_rate, int use_q, float loop_gain, float max_error,
+                                             int debug_every_nth, char* debug_writefiles_path)
+{
+    timing_recovery_state_t s = {};                                        // libcsdr.c:1960-1973
+    s.algorithm = algorithm; s.decimation_rate = decimation_rate; s.loop_gain = loop_gain; s.max_error = max_error; s.use_q = use_q;
+    s.debug_phase = s.debug_every_nth = debug_every_nth; s.last_correction_offset = 0; s.earlylate_ratio = 0.25f;
+    s.debug_writefiles_path = debug_writefiles_path;
+    return s;
+}
+
+void timing_recovery_cc(complexf* input, complexf* output, int input_size, float* timing_error, int* sampled_indexes, timing_recovery_state_t* state)
+{
+    if (state->debug_every_nth >= 0) { set_error("the octave debug output (debug_every_nth >= 0) is not part of this build"); die("timing_recovery_cc"); }
+    if (state->earlylate_ratio != 0.25f) { set_error("earlylate_ratio other than timing_recovery_init's 0.25 is not served"); die("timing_recovery_cc"); }
+    const csdrb_timing_recovery_params_t p = {(int)state->algorithm, state->decimation_rate, state->use_q, state->loop_gain, state->max_error};
+    csdrb_timing_recovery_state_t s = {state->last_correction_offset, 0, 0};
+    const int n = input_size > 0 ? input_size : 0;
+    const int cap = p.decimation >= 2 ? timing_recovery_max_outputs(p.decimation, n, p.loop_gain, p.max_error) : 1;
+    Staging st("timing_recovery_cc");
+    const complexf* d_in = st.up(input, n);
+    struct Call { int start, size; csdrb_timing_recovery_state_t state; } call = {0, n, s};
+    Call* d_call = st.up(&call, 1);
+    complexf* d_out = st.alloc<complexf>(cap);
+    float* d_err = timing_error ? st.alloc<float>(cap) : nullptr;
+    int* d_idx = sampled_indexes ? st.alloc<int>(cap) : nullptr;
+    st.check(csdrb_timing_recovery_bank_cc(d_in, n, &d_call->start, &d_call->size, n, d_out, cap, d_err, d_idx, 1, &p, &d_call->state, st.stream()));
+    st.get(&call, d_call, 1);
+    st.sync();
+    const int m = call.state.output_size;
+    st.get(output, d_out, m);
+    if (timing_error) st.get(timing_error, d_err, m);
+    if (sampled_indexes) st.get(sampled_indexes, d_idx, m);
+    st.sync();
+    state->input_processed = call.state.input_processed;
+    state->output_size = m;
+    state->last_correction_offset = call.state.last_correction_offset;
+}
+
 }  // extern "C"

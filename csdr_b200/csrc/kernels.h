@@ -84,6 +84,19 @@ int launch_fastdcblock_bank(const void* d_in, long in_stride, int cf32, float* d
 int launch_agc_bank(const void* d_in, long in_stride, int cf32, void* d_out, long out_stride, int s16, int channels, int n, const void* h_params_v,
                     void* d_state_v, float limit_max, cudaStream_t st);   // AgcParams on the host, AgcState[channels] on the device
 
+// BPSK31 receive chain, psk31.cu.  TrParams / TrState have the layout of csdrb_timing_recovery_params_t / csdrb_timing_recovery_state_t.
+struct TrParams { int algorithm, decimation, use_q; float loop_gain, max_error; };
+struct TrState { int last_correction_offset, input_processed, output_size; };
+int launch_simple_agc_bank(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n, float rate, float reference,
+                           float max_gain, float* d_gain_io, cudaStream_t st);
+int timing_recovery_max_outputs(int decimation, int input_size, float loop_gain, float max_error);   // symbols one call on input_size samples can make
+int launch_timing_recovery_bank(const float2* d_in, long in_stride, const int* d_start, const int* d_size, float2* d_out, long out_stride, float* d_err,
+                                int* d_idx, int channels, const void* h_params_v, void* d_state_v, int max_size, cudaStream_t st);   // TrParams on the host, TrState[channels] on the device
+int launch_dbpsk_bank(const float2* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels, int n, const int* d_lengths,
+                      const float2* d_last_in, float2* d_last_out, cudaStream_t st);
+int launch_varicode_bank(const unsigned char* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels, int n, const int* d_lengths,
+                         unsigned long long* d_hist_io, int* d_count, cudaStream_t st);
+
 // K7/K8/K9 fft.cu
 int launch_fft_c2c_batch(const float2* d_in, long in_stride, float2* d_out, long out_stride, int n, int batch, int inverse, cudaStream_t st);
 int launch_olafir_bank(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int fft_size, int input_size,

@@ -1,5 +1,5 @@
 /*
- * bankd.c -- csdr-bankd: a whole bank of FM, AM or SSB receivers on ONE wideband IQ stream, in one process.
+ * bankd.c -- csdr-bankd: a whole bank of FM, AM, SSB or BPSK31 receivers on ONE wideband IQ stream, in one process.
  *
  * SURVEY.md 8(f) rank 2.  What the reference does with processes -- `nmux` fanning the IQ stream out over TCP (nmux.cpp:246-353)
  * to one `csdr shift_addition_cc | csdr fir_decimate_cc | csdr fmdemod_quadri_cf | ...` chain per listener (ddcd_old.h:51-57,
@@ -13,11 +13,16 @@
  * first -- is process plumbing and is not reproduced; tests/test_gpu_zzz_bankd.py compares against the oracle run over the whole stream).
  *
  * usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]
- *                   [--tail nfm|none|am|usb|lsb|iq] [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]
+ *                   [--tail nfm|none|am|usb|lsb|iq|bpsk31] [--sps N] [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]
  *                   RATE:SINK [RATE:SINK ...]
  *   --tail: nfm (default) the README.md:87 tail, s16; none the raw discriminator output, f32; am / usb / lsb the AM and SSB graphs of README.md:95 and :110
- *   behind the DDC's complex baseband (see bb_tail_t), s16; iq the complex baseband itself, cf32.  --limit is limit_ff's amplitude (default 1), --agc-ref
- *   the AGC reference (default: fastagc_ff's 1.0 for nfm, agc_ff's 0.2 for am/usb/lsb).
+ *   behind the DDC's complex baseband (see bb_tail_t), s16; iq the complex baseband itself, cf32; bpsk31 the BPSK31 receive chain
+ *   simple_agc_cc 0.001 R | timing_recovery_cc GARDNER N 0.5 2 --add_q | dbpsk_decoder_c_u8 | psk31_varicode_decoder_u8_u8 behind the baseband, the
+ *   decoded text per channel (--sps N: samples per symbol at the baseband rate, > 4 and divisible by 4).  --limit is limit_ff's amplitude (default 1),
+ *   --agc-ref the AGC reference (default: fastagc_ff's 1.0 for nfm, agc_ff's 0.2 for am/usb/lsb, simple_agc_cc's 0.5 for bpsk31).
+ *   A PSK31 skimmer at 2.4 Msps: --decimation 300 --bw 0.001 gives 8 kHz baseband (4001 taps, M = 14 taps per output period: the fused bank serves it),
+ *   and --sps 256 is 31.25 Bd:
+ *     rtl_sdr -s 2400000 -f 14070000 - | csdr-bankd --decimation 300 --bw 0.001 --tail bpsk31 --sps 256 -0.1:ch1.txt 0.05:ch2.txt 0.2:ch3.txt
  *   --decimation: any even D (default 50) whose filter the fused bank serves: M = ceil(taps / D) <= 24 and D * M (rounded up to the kernel's
  *   bucket) <= 8000 taps, see csdrb_ddc_bank in include/csdr_b200.h.  The NFM tail's deemphasis_nfm_ff stays at 48000 whatever D gives: where
  *   wideband rate / D is not 48 kHz, --resample I:D[:BW] puts rational_resampler_ff I D BW right behind the discriminator (tails nfm and none; see
@@ -291,7 +296,101 @@ static void raw_emit(const float *d_rows, long pitch, int n, unsigned char *h_ou
  *   mid  : [C][bs] float (am: DC-blocked envelope) or complexf (usb/lsb: filtered baseband) over the whole units
  *   pcm  : [C][whole] s16 */
 #define SSB_BW 0.05f                                      /* bandpass_fir_fft_cc transition bandwidth of README.md:110 */
-enum { TAIL_NFM, TAIL_NONE, TAIL_IQ, TAIL_AM, TAIL_USB, TAIL_LSB };
+enum { TAIL_NFM, TAIL_NONE, TAIL_IQ, TAIL_AM, TAIL_USB, TAIL_LSB, TAIL_BPSK31 };
+
+/* ---- the BPSK31 tail: simple_agc_cc 0.001 R | timing_recovery_cc GARDNER N 0.5 2 --add_q | dbpsk_decoder_c_u8 | psk31_varicode_decoder_u8_u8 --------
+ * Channels consume different amounts of baseband, so the timing recovery bank gets a start offset per channel.  Device buffers of ONE device:
+ *   tr   : [C][ts] complexf : AGC output; row c's unconsumed samples are [start[c], end) (end is the same for every row), new samples go to end
+ *   sym  : [C][cap] complexf symbols, bits : [C][cap] dbpsk bits, chars : [C][cap] decoded text
+ * Carried per channel: the AGC gain, the timing loop's correction offset and unconsumed baseband, the last dbpsk input, the varicode register.
+ * The timing recovery leaves at most 3N/2 samples unconsumed, so every push first moves [min start, end) to the front of the rows. */
+typedef struct {
+    int C, sps, end, cap, last_cur;
+    long ts;
+    float agc_ref;
+    complexf *d_tr, *d_carry, *d_sym, *d_last[2];
+    unsigned char *d_bits, *d_chars;
+    float *d_gain;
+    int *d_start, *d_size, *d_counts, *d_char_count, *h_start, *h_size, *h_char_count;
+    csdrb_timing_recovery_state_t *d_state, *h_state;
+    unsigned long long *d_hist;
+    unsigned char *h_chars;
+} bpsk_tail_t;
+
+static void bpsk_tail_init(bpsk_tail_t *t, int C, int sps, int in_cap, float agc_ref, void *stream)
+{
+    memset(t, 0, sizeof *t);
+    t->C = C; t->sps = sps; t->agc_ref = agc_ref;
+    t->ts = ((long)in_cap + 2L * sps + 3) & ~3L;
+    t->cap = (int)(t->ts / (sps / 2) + 1);
+    t->d_tr = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->ts);
+    t->d_carry = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->ts);
+    t->d_sym = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->cap);
+    t->d_last[0] = csdrb_device_alloc(sizeof(complexf) * (size_t)C);          /* zero-filled: dbpsk's previous sample starts at 0 */
+    t->d_last[1] = csdrb_device_alloc(sizeof(complexf) * (size_t)C);
+    t->d_bits = csdrb_device_alloc((size_t)C * (size_t)t->cap);
+    t->d_chars = csdrb_device_alloc((size_t)C * (size_t)t->cap);
+    t->d_gain = csdrb_device_alloc(sizeof(float) * (size_t)C);
+    t->d_start = csdrb_device_alloc(sizeof(int) * (size_t)C * 2);            /* start[C] then size[C], one copy for both */
+    t->d_size = t->d_start ? t->d_start + C : NULL;
+    t->d_counts = csdrb_device_alloc(sizeof(int) * (size_t)C);
+    t->d_char_count = csdrb_device_alloc(sizeof(int) * (size_t)C);
+    t->d_state = csdrb_device_alloc(sizeof(csdrb_timing_recovery_state_t) * (size_t)C);   /* zero-filled: correction offset 0 */
+    t->d_hist = csdrb_device_alloc(sizeof(unsigned long long) * (size_t)C);              /* zero-filled: status_shr = 0 */
+    t->h_start = csdrb_host_alloc(sizeof(int) * (size_t)C * 3);
+    t->h_state = csdrb_host_alloc(sizeof(csdrb_timing_recovery_state_t) * (size_t)C);
+    t->h_chars = csdrb_host_alloc((size_t)C * (size_t)t->cap);
+    if (!t->d_tr || !t->d_carry || !t->d_sym || !t->d_last[0] || !t->d_last[1] || !t->d_bits || !t->d_chars || !t->d_gain || !t->d_start || !t->d_size ||
+        !t->d_counts || !t->d_char_count || !t->d_state || !t->d_hist || !t->h_start || !t->h_state || !t->h_chars) die("out of memory");
+    t->h_size = t->h_start + C; t->h_char_count = t->h_start + 2 * C;
+    float *g = malloc(sizeof(float) * (size_t)C);
+    if (!g) die("out of memory");
+    for (int c = 0; c < C; c++) g[c] = 1.0f;                               /* simple_agc_cc's current_gain starts at 1 (csdr.c:2917) */
+    OK(csdrb_copy_h2d(t->d_gain, g, sizeof(float) * (size_t)C, stream));
+    OK(csdrb_stream_synchronize(stream));
+    free(g);
+}
+
+/* n new baseband samples per channel at d_bb (row pitch bs): the chain over them, the decoded text to the sinks */
+static void bpsk_tail_push(bpsk_tail_t *t, channel_t *chan, const complexf *d_bb, long bs, int n, void *stream)
+{
+    const int C = t->C;
+    const size_t row = sizeof(complexf) * (size_t)t->ts;
+    int lo = t->end;
+    for (int c = 0; c < C; c++) lo = t->h_start[c] < lo ? t->h_start[c] : lo;
+    if (lo > 0 && t->end > lo) {                                            /* the unconsumed samples to the front of the rows */
+        OK(csdrb_copy2d_d2d(t->d_carry, row, t->d_tr + lo, row, sizeof(complexf) * (size_t)(t->end - lo), (size_t)C, stream));
+        OK(csdrb_copy2d_d2d(t->d_tr, row, t->d_carry, row, sizeof(complexf) * (size_t)(t->end - lo), (size_t)C, stream));
+    }
+    for (int c = 0; c < C; c++) t->h_start[c] -= lo;
+    t->end -= lo;
+    if (t->end + n > t->ts) die("bpsk31 tail: baseband buffer overflow");
+    OK(csdrb_simple_agc_bank_cc(d_bb, bs, t->d_tr + t->end, t->ts, C, n, 0.001f, t->agc_ref, 65535.0f, t->d_gain, stream));
+    t->end += n;
+    for (int c = 0; c < C; c++) t->h_size[c] = t->end - t->h_start[c];
+    OK(csdrb_copy_h2d(t->d_start, t->h_start, sizeof(int) * (size_t)C * 2, stream));      /* h_start and h_size are adjacent */
+    const csdrb_timing_recovery_params_t p = {0, t->sps, 1, 0.5f, 2.0f};  /* GARDNER <sps> 0.5 2 --add_q */
+    OK(csdrb_timing_recovery_bank_cc(t->d_tr, t->ts, t->d_start, t->d_size, t->end, t->d_sym, t->cap, NULL, NULL, C, &p, t->d_state, stream));
+    OK(csdrb_copy_d2h(t->h_state, t->d_state, sizeof(csdrb_timing_recovery_state_t) * (size_t)C, stream));
+    OK(csdrb_stream_synchronize(stream));
+    int *h_counts = t->h_size;                                              /* reused: the symbols each channel produced */
+    int m = 0;
+    for (int c = 0; c < C; c++) {
+        t->h_start[c] += t->h_state[c].input_processed;
+        h_counts[c] = t->h_state[c].output_size;
+        m = h_counts[c] > m ? h_counts[c] : m;
+    }
+    if (m > 0) {
+        OK(csdrb_copy_h2d(t->d_counts, h_counts, sizeof(int) * (size_t)C, stream));
+        OK(csdrb_dbpsk_decoder_bank_c_u8(t->d_sym, t->cap, t->d_bits, t->cap, C, m, t->d_counts, t->d_last[t->last_cur], t->d_last[t->last_cur ^ 1], stream));
+        t->last_cur ^= 1;
+        OK(csdrb_psk31_varicode_decoder_bank_u8_u8(t->d_bits, t->cap, t->d_chars, t->cap, C, m, t->d_counts, t->d_hist, t->d_char_count, stream));
+        OK(csdrb_copy_d2h(t->h_char_count, t->d_char_count, sizeof(int) * (size_t)C, stream));
+        OK(csdrb_copy2d_d2h(t->h_chars, (size_t)m, t->d_chars, (size_t)t->cap, (size_t)m, (size_t)C, stream));
+        OK(csdrb_stream_synchronize(stream));
+        for (int c = 0; c < C; c++) if (t->h_char_count[c] > 0) write_sink(&chan[c], t->h_chars + (size_t)c * (size_t)m, (size_t)t->h_char_count[c]);
+    }
+}
 
 typedef struct {
     int kind, C, unit, have, fft_size;
@@ -304,12 +403,21 @@ typedef struct {
     float *d_last_dc;
     csdrb_agc_state_t *d_agc_state;
     unsigned char *h_out;
+    bpsk_tail_t bpsk;
 } bb_tail_t;
 
-static void bb_tail_init(bb_tail_t *t, int kind, int C, int out_cap, float limit, float agc_ref, void *stream)
+static void bb_tail_init(bb_tail_t *t, int kind, int C, int out_cap, float limit, float agc_ref, int sps, void *stream)
 {
     memset(t, 0, sizeof *t);
     t->kind = kind; t->C = C; t->limit = limit;
+    if (kind == TAIL_BPSK31) {                                       /* the baseband rows only pass the new samples on */
+        t->unit = 1;
+        t->bs = ((long)out_cap + 3) & ~3L;
+        t->d_bb = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->bs);
+        if (!t->d_bb) die("out of memory");
+        bpsk_tail_init(&t->bpsk, C, sps, out_cap, agc_ref, stream);
+        return;
+    }
     csdrb_agc_params_t p = {0.2f, 0.01f, 0.0001f, 65536.0f, 200, 0, 0.999f, 1024};
     if (agc_ref > 0.f) p.reference = agc_ref;
     t->agc = p;
@@ -361,6 +469,7 @@ static void bb_tail_push(bb_tail_t *t, channel_t *chan, int n_new, void *stream)
     const int C = t->C;
     const long bs = t->bs;
     const int n = t->have + n_new;
+    if (t->kind == TAIL_BPSK31) { bpsk_tail_push(&t->bpsk, chan, t->d_bb, bs, n, stream); t->have = 0; return; }
     if (t->kind == TAIL_IQ) {                                    /* raw baseband: nothing is held back */
         OK(csdrb_copy2d_d2h(t->h_out, sizeof(complexf) * (size_t)n, t->d_bb, sizeof(complexf) * (size_t)bs, sizeof(complexf) * (size_t)n, (size_t)C, stream));
         OK(csdrb_stream_synchronize(stream));
@@ -388,7 +497,7 @@ static void bb_tail_push(bb_tail_t *t, channel_t *chan, int n_new, void *stream)
 }
 
 static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *chan, int C, const float *rates, int D, const float *taps, int T, int block,
-                     int kind, float limit, float agc_ref, int rs_I, int rs_D, float rs_bw)
+                     int kind, float limit, float agc_ref, int rs_I, int rs_D, float rs_bw, int sps)
 {
     const int nfm = kind == TAIL_NFM, demod = kind == TAIL_NFM || kind == TAIL_NONE;
     const size_t osz = demod ? sizeof(float) : sizeof(complexf);
@@ -413,7 +522,7 @@ static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *cha
         if (resample) rs_init(&rsm, C, rs_I, rs_D, rs_bw, n_out + 2);
         const int tail_cap = resample ? rs_out_cap(&rsm) : n_out + 2;
         if (nfm) nfm_tail_init(&tail_state, C, tail_cap, limit, agc_ref);
-        else if (!demod) bb_tail_init(&bb, kind, C, tail_cap, limit, agc_ref, tail_stream);
+        else if (!demod) bb_tail_init(&bb, kind, C, tail_cap, limit, agc_ref, sps, tail_stream);
         else {
             d_raw_out = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)tail_cap);
             h_raw_out = csdrb_host_alloc(sizeof(float) * (size_t)C * (size_t)tail_cap);
@@ -476,8 +585,13 @@ static int usage(void)
 {
     fprintf(stderr,
             "usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]\n"
-            "                  [--tail nfm|none|am|usb|lsb|iq] [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]\n"
+            "                  [--tail nfm|none|am|usb|lsb|iq|bpsk31] [--sps N] [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]\n"
             "                  RATE:SINK [RATE:SINK ...]\n"
+            "  --tail bpsk31 --sps N  per channel simple_agc_cc 0.001 R | timing_recovery_cc GARDNER N 0.5 2 --add_q | dbpsk_decoder_c_u8 |\n"
+            "                       psk31_varicode_decoder_u8_u8 (R = --agc-ref, default 0.5) behind the baseband; the sinks get the decoded text.\n"
+            "                       N is samples per symbol at the baseband rate, > 4 and divisible by 4.  A PSK31 skimmer at 2.4 Msps:\n"
+            "                       csdr-bankd --decimation 300 --bw 0.001 --tail bpsk31 --sps 256 -0.1:ch1.txt 0.05:ch2.txt 0.2:ch3.txt\n"
+            "                       (8 kHz baseband, 4001 taps = 14 per output period, which the fused bank serves; 31.25 Bd)\n"
             "  --resample I:D[:BW]  rational_resampler_ff I D BW (BW default 0.05) right behind the discriminator, for --tail nfm and none: brings\n"
             "                       wideband/decimation to the 48 kHz the NFM de-emphasis is designed for (e.g. 2.048 Msps, --decimation 32,\n"
             "                       --resample 3:4).  With T = taps of BW, the daemon needs (T/I + 1)*I >= 2*D + I - 1 (T >= 2*D + I - 2 suffices),\n"
@@ -492,6 +606,7 @@ int main(int argc, char **argv)
     int u8 = 1, D = 50, block = 1 << 18, device = 0, ndev = 0, devs[64];
     float bw = 0.005f, limit = 1.0f, agc_ref = 0.0f;                /* agc_ref 0: the tail's own default (fastagc_ff 1.0, agc_ff 0.2) */
     int rs_I = 0, rs_D = 0;                                          /* --resample I:D[:BW]; 0: no resampler */
+    int sps = 0;                                                     /* --sps N of --tail bpsk31 */
     float rs_bw = 0.05f;                                             /* rational_resampler_ff's default transition bandwidth (csdr.c:1423) */
     window_t window = WINDOW_HAMMING;
     channel_t *chan = calloc((size_t)argc, sizeof *chan);
@@ -509,6 +624,7 @@ int main(int argc, char **argv)
         else if (!strcmp(o, "--tail") && v) { tail = v; a++; }
         else if (!strcmp(o, "--limit") && v) { limit = (float)atof(v); a++; }
         else if (!strcmp(o, "--agc-ref") && v) { agc_ref = (float)atof(v); a++; }
+        else if (!strcmp(o, "--sps") && v) { sps = atoi(v); a++; }
         else if (!strcmp(o, "--device") && v) { device = atoi(v); a++; }
         else if (!strcmp(o, "--devices") && v) { ndev = parse_devices(v, devs, 64); if (ndev <= 0) die("--devices wants N0,N1,..."); a++; }
         else if (!strcmp(o, "--resample") && v) {
@@ -528,10 +644,14 @@ int main(int argc, char **argv)
             chan[C].sink = end + 1; chan[C].fd = -1; chan[C].dropped = 0; C++;
         } else { fprintf(stderr, "csdr-bankd: unknown argument %s\n", o); return 2; }
     }
-    static const char *kTails[] = {"nfm", "none", "iq", "am", "usb", "lsb"};
+    static const char *kTails[] = {"nfm", "none", "iq", "am", "usb", "lsb", "bpsk31"};
     int kind = -1;
-    for (int k = 0; k < 6; k++) if (!strcmp(tail, kTails[k])) kind = k;
-    if (kind < 0) die("--tail is nfm, none, iq, am, usb or lsb");
+    for (int k = 0; k < 7; k++) if (!strcmp(tail, kTails[k])) kind = k;
+    if (kind < 0) die("--tail is nfm, none, iq, am, usb, lsb or bpsk31");
+    if (kind == TAIL_BPSK31) {
+        if (sps <= 4 || (sps & 3)) die("--tail bpsk31 needs --sps N with N > 4 and divisible by 4 (timing_recovery_cc's decimation)");
+        if (agc_ref == 0.0f) agc_ref = 0.5f;                         /* simple_agc_cc's reference in the OpenWebRX chain */
+    } else if (sps) die("--sps belongs to --tail bpsk31");
     const int nfm = kind == TAIL_NFM, demod = kind == TAIL_NFM || kind == TAIL_NONE;
     if (nfm && agc_ref == 0.0f) agc_ref = 1.0f;                      /* fastagc_ff's default reference (csdr.c:1388) */
     if (C == 0) die("no channels (RATE:SINK ...)");
@@ -541,7 +661,7 @@ int main(int argc, char **argv)
     if (!(limit > 0.f) || !(agc_ref >= 0.f)) die("--limit and --agc-ref must be positive");
     const int resample = rs_I > 0;
     if (resample) {
-        if (!demod) die("--resample works with --tail nfm and --tail none only (the am, usb, lsb and iq tails are not resampled)");
+        if (!demod) die("--resample works with --tail nfm and --tail none only (the am, usb, lsb, iq and bpsk31 tails are not resampled)");
         if (!(rs_bw > 0.f && rs_bw < 0.5f)) die("--resample: the transition bandwidth must be between 0 and 0.5");
         const int rs_T = firdes_filter_len(rs_bw);
         if (!resample_geometry_ok(rs_I, rs_D, rs_T)) {
@@ -564,7 +684,7 @@ int main(int argc, char **argv)
         for (int c = 0; c < C; c++) { chan[c].fd = open_sink(chan[c].sink); sink_nonblocking(chan[c].fd); }
         const int fd = open_input(in_spec);
         fprintf(stderr, "csdr-bankd: %d channels over %d devices, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, ndev, D, T, u8 ? "u8" : "f32", block, tail);
-        const int rc = run_multi(fd, u8, devs, ndev, chan, C, rates, D, taps, T, block, kind, limit, agc_ref, rs_I, rs_D, rs_bw);
+        const int rc = run_multi(fd, u8, devs, ndev, chan, C, rates, D, taps, T, block, kind, limit, agc_ref, rs_I, rs_D, rs_bw, sps);
         for (int c = 0; c < C; c++) { if (chan[c].dropped) fprintf(stderr, "csdr-bankd: sink %s lost %ld bytes (too slow)\n", chan[c].sink, chan[c].dropped); if (chan[c].fd >= 0) close(chan[c].fd); }
         return rc;
     }
@@ -592,7 +712,7 @@ int main(int argc, char **argv)
     float *d_demod = NULL;
     unsigned char *h_out = NULL;
     if (nfm) { nfm_tail_init(&tl, C, tail_cap, limit, agc_ref); ds = tl.ds; d_demod = tl.d_demod; }
-    else if (!demod) { bb_tail_init(&bb, kind, C, out_cap, limit, agc_ref, stream); ds = bb.bs; d_demod = (float *)bb.d_bb; }
+    else if (!demod) { bb_tail_init(&bb, kind, C, out_cap, limit, agc_ref, sps, stream); ds = bb.bs; d_demod = (float *)bb.d_bb; }
     else {
         d_demod = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)ds);
         h_out = csdrb_host_alloc((size_t)C * (size_t)ds * sizeof(float));

@@ -803,6 +803,111 @@ static int cmd_fastddc_inv_cc(int argc, char **argv)
     }
 }
 
+static int cmd_simple_agc_cc(int argc, char **argv)                          /* csdr.c:2902-2931 */
+{
+    float rate = 0.f;
+    if (argc <= 2) return complain("need required parameter (rate)");
+    sscanf(argv[2], "%f", &rate);
+    if (rate <= 0) return complain("rate should be > 0");
+    float reference = 1.f; if (argc > 3) sscanf(argv[3], "%f", &reference);
+    if (reference <= 0) return complain("reference should be > 0");
+    float max_gain = 65535.f; if (argc > 4) sscanf(argv[4], "%f", &max_gain);
+    if (max_gain <= 0) return complain("max_gain should be > 0");
+    if (!announce_block(open_block())) return -2;
+    complexf *in = must_alloc(sizeof(complexf) * (size_t)block), *out = must_alloc(sizeof(complexf) * (size_t)block);
+    float gain = 1.f;
+    for (;;) {
+        if (feof(stdin)) return 0;
+        fread(in, sizeof(complexf), (size_t)block, stdin);
+        simple_agc_cc(in, out, block, rate, reference, max_gain, &gain);
+        fwrite(out, sizeof(complexf), (size_t)block, stdout);
+        end_of_block();
+    }
+}
+
+static int cmd_timing_recovery_cc(int argc, char **argv)                     /* csdr.c:2573-2637 */
+{
+    if (argc <= 2) return complain("need required parameter (algorithm)");
+    timing_recovery_algorithm_t algorithm = !strcmp(argv[2], "EARLYLATE") ? TIMING_RECOVERY_ALGORITHM_EARLYLATE : TIMING_RECOVERY_ALGORITHM_GARDNER;
+    if (argc <= 3) return complain("need required parameter (decimation factor)");
+    int decimation = 0; sscanf(argv[3], "%d", &decimation);
+    if (decimation <= 4 || decimation & 3) return complain("decimation factor should be a positive integer divisible by 4");
+    float loop_gain = 0.5f; if (argc > 4) sscanf(argv[4], "%f", &loop_gain);
+    float max_error = 2.f; if (argc > 5) sscanf(argv[5], "%f", &max_error);
+    const int add_q = argc >= 7 && !strcmp(argv[6], "--add_q");
+    /* like the reference, --octave / --octave_save select a debug mode only when their count follows (csdr.c:2600) */
+    if (argc >= 8 + add_q && (!strcmp(argv[6 + add_q], "--octave") || !strcmp(argv[6 + add_q], "--octave_save")))
+        return complain("the --octave and --octave_save debug outputs are not part of this build");
+    if (!(fabs((double)loop_gain * (double)max_error) <= 2.0))
+        return complain("|mu * max_error| must be at most 2: a larger correction can move a symbol back, before the start of its input");
+    who(); fprintf(stderr, "--add_q mode on\n");                        /* printed whatever add_q is, like the reference */
+    const int output_error = argc >= 7 + add_q && !strcmp(argv[6 + add_q], "--output_error");
+    if (output_error) { who(); fprintf(stderr, "--output_error mode\n"); }
+    const int output_indexes = argc >= 7 + add_q && !strcmp(argv[6 + add_q], "--output_indexes");
+    if (output_indexes) { who(); fprintf(stderr, "--output_indexes mode\n"); }
+    if (!open_block()) return -2;
+    announce_block(block / decimation);
+    complexf *in = must_alloc(sizeof(complexf) * (size_t)block), *out = must_alloc(sizeof(complexf) * (size_t)block);
+    float *error = output_error ? must_alloc(sizeof(float) * (size_t)block) : NULL;
+    unsigned *indexes = output_indexes ? must_alloc(sizeof(unsigned) * (size_t)block) : NULL;
+    timing_recovery_state_t state = timing_recovery_init(algorithm, decimation, add_q, loop_gain, max_error, -1, NULL);
+    fread(in, sizeof(complexf), (size_t)block, stdin);
+    unsigned buffer_start_counter = 0;
+    for (;;) {
+        if (feof(stdin)) return 0;
+        timing_recovery_cc(in, out, block, error, (int *)indexes, &state);
+        if (error) fwrite(error, sizeof(float), (size_t)state.output_size, stdout);
+        else if (indexes) {
+            for (int i = 0; i < state.output_size; i++) indexes[i] += buffer_start_counter;
+            fwrite(indexes, sizeof(unsigned), (size_t)state.output_size, stdout);
+        } else fwrite(out, sizeof(complexf), (size_t)state.output_size, stdout);
+        end_of_block();
+        buffer_start_counter += (unsigned)state.input_processed;          /* keep the unconsumed tail, refill behind it */
+        memmove(in, in + state.input_processed, sizeof(complexf) * (size_t)(block - state.input_processed));
+        fread(in + (block - state.input_processed), sizeof(complexf), (size_t)state.input_processed, stdin);
+    }
+}
+
+static int cmd_dbpsk_decoder_c_u8(int argc, char **argv)                     /* csdr.c:3256-3268 */
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    complexf *in = must_alloc(sizeof(complexf) * (size_t)block);
+    unsigned char *out = must_alloc((size_t)block);
+    for (;;) {
+        if (feof(stdin)) return 0;
+        fread(in, sizeof(complexf), (size_t)block, stdin);
+        dbpsk_decoder_c_u8(in, out, block);
+        fwrite(out, 1, (size_t)block, stdout);
+        end_of_block();
+    }
+}
+
+/* csdr.c:2418-2430 pushes one getchar() at a time through psk31_varicode_decoder_push and flushes every character.  Here every read()
+ * (whatever the pipe holds, up to one block) goes through the varicode bank, and the characters it decoded are written and flushed at once. */
+static int cmd_psk31_varicode_decoder_u8_u8(int argc, char **argv)
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    unsigned char *in = must_alloc((size_t)block), *out = must_alloc((size_t)block);
+    unsigned char *d_in = csdrb_device_alloc((size_t)block), *d_out = csdrb_device_alloc((size_t)block);
+    unsigned long long *d_hist = csdrb_device_alloc(sizeof(unsigned long long));      /* zero-filled: the reference's status_shr = 0 */
+    int *d_count = csdrb_device_alloc(sizeof(int));
+    if (!d_in || !d_out || !d_hist || !d_count) { who(); fprintf(stderr, "%s\n", csdrb_last_error()); return -2; }
+    for (;;) {
+        const ssize_t got = read(STDIN_FILENO, in, (size_t)block);
+        if (got <= 0) return 0;
+        int count = 0;
+        if (csdrb_copy_h2d(d_in, in, (size_t)got, NULL) < 0 ||
+            csdrb_psk31_varicode_decoder_bank_u8_u8(d_in, got, d_out, got, 1, (int)got, NULL, d_hist, d_count, NULL) < 0 ||
+            csdrb_copy_d2h(&count, d_count, sizeof count, NULL) < 0 || csdrb_stream_synchronize(NULL) < 0 ||
+            (count > 0 && (csdrb_copy_d2h(out, d_out, (size_t)count, NULL) < 0 || csdrb_stream_synchronize(NULL) < 0))) {
+            who(); fprintf(stderr, "%s\n", csdrb_last_error()); return -2;
+        }
+        if (count > 0) { fwrite(out, 1, (size_t)count, stdout); fflush(stdout); }
+    }
+}
+
 /* ---- dispatch ------------------------------------------------------------------------------------ */
 static const struct { const char *name; int (*run)(int, char **); const char *syntax; } kCommands[] = {
     {"convert_u8_f", cmd_convert_u8_f, "convert_u8_f"},
@@ -837,6 +942,10 @@ static const struct { const char *name; int (*run)(int, char **); const char *sy
     {"deemphasis_nfm_ff", cmd_deemphasis_nfm_ff, "deemphasis_nfm_ff <one_of_the_predefined_sample_rates>"},
     {"bandpass_fir_fft_cc", cmd_bandpass_fir_fft_cc, "bandpass_fir_fft_cc <low_cut> <high_cut> <transition_bw> [window] | --fifo <fifo_path> <transition_bw> [window]"},
     {"fastddc_fwd_cc", cmd_fastddc_fwd_cc, "fastddc_fwd_cc <decimation> [transition_bw [window]]"},
+    {"simple_agc_cc", cmd_simple_agc_cc, "simple_agc_cc <rate> [reference [max_gain]]"},
+    {"timing_recovery_cc", cmd_timing_recovery_cc, "timing_recovery_cc <algorithm> <decimation> [mu [max_error [--add_q [--output_error | --output_indexes]]]]"},
+    {"dbpsk_decoder_c_u8", cmd_dbpsk_decoder_c_u8, "dbpsk_decoder_c_u8"},
+    {"psk31_varicode_decoder_u8_u8", cmd_psk31_varicode_decoder_u8_u8, "psk31_varicode_decoder_u8_u8"},
     {"fastddc_inv_cc", cmd_fastddc_inv_cc, "fastddc_inv_cc <shift_rate> <decimation> [transition_bw [window]] | --fifo <fifo_path> ... | --fd <fd> ..."},
 };
 

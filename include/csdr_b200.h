@@ -100,6 +100,23 @@ float fastdcblock_ff(float *input, float *output, int input_size, float last_dc_
 float agc_ff(float *input, float *output, int input_size, float reference, float attack_rate, float decay_rate, float max_gain,
              short hang_time, short attack_wait_time, float gain_filter_alpha, float last_gain);
 
+/* BPSK31 receive chain (libcsdr.h:314-336, 340-345; libcsdr.c:1960-2072, 2201-2217, 2319-2333), computed as the reference's -O3 -ffast-math build
+ * computes it (DESIGN.md section 7).  simple_agc_cc: *current_gain carries the gain between calls (1.0 at stream start).  dbpsk_decoder_c_u8 keeps
+ * the reference's static previous sample as library state (zero at process start).  timing_recovery_cc serves GARDNER and EARLYLATE with
+ * |loop_gain * max_error| <= 2; the octave debug output (debug_every_nth >= 0) is not part of this build: such a call prints
+ * `libcsdr_b200: timing_recovery_cc failed: ...` and aborts, like any other failing drop-in.  psk31_varicode_decoder_push, one bit per call,
+ * is not offered here: the bank csdrb_psk31_varicode_decoder_bank_u8_u8 decodes whole streams. */
+void simple_agc_cc(complexf *input, complexf *output, int input_size, float rate, float reference, float max_gain, float *current_gain);
+void dbpsk_decoder_c_u8(complexf *input, unsigned char *output, int input_size);
+typedef enum timing_recovery_algorithm_e { TIMING_RECOVERY_ALGORITHM_GARDNER, TIMING_RECOVERY_ALGORITHM_EARLYLATE } timing_recovery_algorithm_t;
+typedef struct timing_recovery_state_s {
+    timing_recovery_algorithm_t algorithm; int decimation_rate; int output_size; int input_processed; int use_q; int debug_phase; int debug_every_nth;
+    char *debug_writefiles_path; int last_correction_offset; float earlylate_ratio; float loop_gain; float max_error;
+} timing_recovery_state_t;
+timing_recovery_state_t timing_recovery_init(timing_recovery_algorithm_t algorithm, int decimation_rate, int use_q, float loop_gain, float max_error,
+                                             int debug_every_nth, char *debug_writefiles_path);
+void timing_recovery_cc(complexf *input, complexf *output, int input_size, float *timing_error, int *sampled_indexes, timing_recovery_state_t *state);
+
 /* audio tail of the WFM graph, SURVEY 8(f) rank 1 (libcsdr.h:100-105; libcsdr.c:1081-1097, 1130-1137) */
 float deemphasis_wfm_ff(float *input, float *output, int input_size, float tau, int sample_rate, float last_output);
 void  limit_ff(float *input, float *output, int input_size, float max_amplitude);
@@ -394,6 +411,38 @@ typedef struct csdrb_agc_params_s {
 typedef struct csdrb_agc_state_s { float gain, last_peak; int hang_counter, attack_wait_counter, offset; } csdrb_agc_state_t;
 int csdrb_agc_bank_ff(const void *d_in, long in_stride, int cf32_in, void *d_out, long out_stride, int s16_out, int channels, int n,
                       const csdrb_agc_params_t *params, csdrb_agc_state_t *d_state, float limit_max, void *stream);
+
+/* BPSK31 receive chain banks (psk31.cu), one row per channel.
+ *
+ * simple_agc_cc bank: input_size samples per row; d_gain_io[c] is the reference's current_gain (1.0f at stream start).  Each sample's
+ * reference/sqrt(i*i + q*q) is correctly rounded where the reference build uses a vendor-dependent rsqrtss approximation; everything else is the
+ * build's arithmetic.  Returns input_size. */
+int csdrb_simple_agc_bank_cc(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int input_size, float rate,
+                             float reference, float max_gain, float *d_gain_io, void *stream);
+/* timing_recovery_cc bank: channel c runs one timing_recovery_cc call over the d_size[c] samples at d_in + c*in_stride + d_start[c] (every
+ * d_size[c] <= max_size), bit for bit with the reference build.  d_state[c].last_correction_offset carries the loop between calls (0 at stream
+ * start); on return d_state[c] = {last_correction_offset, input_processed, output_size} as the reference fills them.  The next call re-presents
+ * the input from input_processed on, like the reference CLI (csdr.c:2621-2636); positions are absolute, so any split of a stream into calls gives
+ * the same symbols.  d_out (and d_error, d_indexes when not NULL) are rows of out_stride elements, at least max_size/(decimation/2) + 1 when
+ * |loop_gain * max_error| <= 1 (every symbol then advances by decimation/2 or more) and max_size above that (a symbol may not advance); the indexes
+ * count from the call's first sample.  Serves algorithm 0 (GARDNER) and 1 (EARLYLATE), decimation > 4 and divisible by 4, -1 otherwise;
+ * -2 when |loop_gain * max_error| > 2 (a correction can then move a symbol back, and the reference reads before its input).
+ * The output counts are data-dependent: read d_state back to use them.  Returns 0. */
+typedef struct csdrb_timing_recovery_params_s { int algorithm, decimation, use_q; float loop_gain, max_error; } csdrb_timing_recovery_params_t;
+typedef struct csdrb_timing_recovery_state_s { int last_correction_offset, input_processed, output_size; } csdrb_timing_recovery_state_t;
+int csdrb_timing_recovery_bank_cc(const complexf *d_in, long in_stride, const int *d_start, const int *d_size, int max_size, complexf *d_out,
+                                  long out_stride, float *d_error, int *d_indexes, int channels, const csdrb_timing_recovery_params_t *params,
+                                  csdrb_timing_recovery_state_t *d_state, void *stream);
+/* dbpsk_decoder_c_u8 bank: row c holds d_lengths[c] <= input_size samples (d_lengths NULL: input_size each); one output bit per sample.
+ * d_last_in[c] is the sample before the row (NULL = zeros), d_last_out[c] receives the row's last sample (d_last_in[c] for an empty row;
+ * may be NULL; must not alias d_last_in).  Returns input_size. */
+int csdrb_dbpsk_decoder_bank_c_u8(const complexf *d_in, long in_stride, unsigned char *d_out, long out_stride, int channels, int input_size,
+                                  const int *d_lengths, const complexf *d_last_in, complexf *d_last_out, void *stream);
+/* psk31_varicode_decoder bank: row c holds d_lengths[c] <= input_size bits (bytes, non-zero = 1; d_lengths NULL: input_size each) and is pushed
+ * through psk31_varicode_decoder_push (libcsdr.c:1536-1549) bit by bit; the non-zero characters go to the row of d_out in order and their count
+ * to d_count[c].  d_hist_io[c] is the decoder's shift register (0 at stream start).  out_stride >= input_size.  Returns 0. */
+int csdrb_psk31_varicode_decoder_bank_u8_u8(const unsigned char *d_in, long in_stride, unsigned char *d_out, long out_stride, int channels,
+                                            int input_size, const int *d_lengths, unsigned long long *d_hist_io, int *d_count, void *stream);
 
 /* K7 batched unnormalised c2c DFT (power-of-two size 2..16384), sign -1 forward / +1 inverse */
 int csdrb_fft_c2c_batch(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int size, int batch, int inverse, void *stream);
