@@ -67,6 +67,15 @@ class _TimingRecovery(C.Structure):     # timing_recovery_state_t (= libcsdr.h:3
                 ("last_correction_offset", C.c_int), ("earlylate_ratio", C.c_float), ("loop_gain", C.c_float), ("max_error", C.c_float)]
 
 
+class SerialLineParams(C.Structure):    # csdrb_serial_line_params_t
+    _fields_ = [("samples_per_bits", C.c_float), ("databits", C.c_int), ("stopbits", C.c_float), ("bit_sampling_width_ratio", C.c_float)]
+
+
+class _SerialLine(C.Structure):         # serial_line_t (= libcsdr.h:278-286)
+    _fields_ = [("samples_per_bits", C.c_float), ("databits", C.c_int), ("stopbits", C.c_float), ("output_size", C.c_int),
+                ("input_used", C.c_int), ("bit_sampling_width_ratio", C.c_float)]
+
+
 class _Unroll(C.Structure):             # shift_unroll_data_t (= libcsdr.h:199-205)
     _fields_ = [("dsin", C.POINTER(C.c_float)), ("dcos", C.POINTER(C.c_float)), ("phase_increment", C.c_float), ("size", C.c_int)]
 
@@ -238,6 +247,9 @@ def lib() -> C.CDLL:
     L.dbpsk_decoder_c_u8.argtypes = [vp, vp, it]
     L.timing_recovery_init.argtypes = [it, it, it, C.c_float, C.c_float, it, C.c_char_p]; L.timing_recovery_init.restype = _TimingRecovery
     L.timing_recovery_cc.argtypes = [vp, vp, it, vp, vp, C.POINTER(_TimingRecovery)]
+    L.csdrb_serial_line_decoder_bank_f_u8.argtypes = [vp, lg, it, vp, vp, lg, vp, vp, it, C.POINTER(SerialLineParams), it, vp]
+    L.csdrb_rtty_baudot2ascii_bank_u8_u8.argtypes = [vp, lg, vp, lg, it, it, vp, vp, vp, vp]
+    L.serial_line_decoder_f_u8.argtypes = [C.POINTER(_SerialLine), vp, vp, it]
     _lib = L
     return L
 
@@ -473,6 +485,14 @@ class libcsdr:
         lib().timing_recovery_cc(x.ctypes.data, y.ctypes.data, x.size, e.ctypes.data, ix.ctypes.data, C.byref(st))
         m = st.output_size
         return y[:m].copy(), e[:m].copy(), ix[:m].copy(), (st.last_correction_offset, st.input_processed, m)
+
+    @staticmethod
+    def serial_line_decoder_f_u8(x, samples_per_bits, databits=8, stopbits=1.0, bit_sampling_width_ratio=0.4):
+        """one call -> (characters as bytes, input_used)"""
+        x = np.ascontiguousarray(x, np.float32); y = np.empty(max(x.size, 1), np.uint8)
+        s = _SerialLine(samples_per_bits, databits, stopbits, 0, 0, bit_sampling_width_ratio)
+        lib().serial_line_decoder_f_u8(C.byref(s), x.ctypes.data, y.ctypes.data, x.size)
+        return y[:s.output_size].tobytes(), s.input_used
 
     @staticmethod
     def convert_s16_f(x):
@@ -1038,6 +1058,43 @@ def psk31_varicode_decoder_bank_u8_u8(bits, lengths=None, hist=None):
                                                          lengths.data_ptr() if lengths is not None else None, hist.data_ptr(), count.data_ptr(),
                                                          _stream()), "psk31_varicode_decoder_bank_u8_u8")
     return out, count, hist
+
+
+def serial_line_decoder_bank_f_u8(x, samples_per_bits: float, databits: int = 8, stopbits: float = 1.0, bit_sampling_width_ratio: float = 0.4,
+                                  bufsize: int | None = None, start=None, end: int | None = None):
+    """serial_line_decoder_f_u8 per row, framed like the CLI: while at least bufsize samples of x[c, start[c]:end] remain, one call on exactly
+    bufsize of them (bufsize and end default to N: one call per row).  x [C, N] float32 -> (characters [C, cap] uint8, count [C] int32,
+    start [C] int32 advanced past what the calls consumed, stuck [C] int32: 1 where a call consumed nothing)"""
+    import torch
+    assert x.dtype == torch.float32 and x.is_cuda and x.dim() == 2 and x.stride(1) == 1
+    ch, n = x.shape
+    end = n if end is None else end
+    bufsize = n if bufsize is None else bufsize
+    start = torch.zeros(ch, dtype=torch.int32, device=x.device) if start is None else start
+    p = SerialLineParams(samples_per_bits, databits, stopbits, bit_sampling_width_ratio)
+    span = np.float32(samples_per_bits) * (np.float32(1 + databits) + np.float32(stopbits))
+    cap = end // max(int(span), 1) + 1
+    out = torch.zeros((ch, cap), dtype=torch.uint8, device=x.device)
+    count = torch.zeros(ch, dtype=torch.int32, device=x.device)
+    stuck = torch.zeros(ch, dtype=torch.int32, device=x.device)
+    _check(lib().csdrb_serial_line_decoder_bank_f_u8(x.data_ptr(), x.stride(0), end, start.data_ptr(), out.data_ptr(), cap, count.data_ptr(),
+                                                     stuck.data_ptr(), ch, C.byref(p), bufsize, _stream()), "serial_line_decoder_bank_f_u8")
+    return out, count, start, stuck
+
+
+def rtty_baudot2ascii_bank_u8_u8(codes, lengths=None, fig_mode=None):
+    """rtty_baudot_decoder_lookup per row: codes [C, N] uint8 (row c holds lengths[c] codes) -> (chars [C, N] uint8, count [C] int32,
+    fig_mode [C] uint8, the letters/figures mode carried between calls)"""
+    import torch
+    assert codes.dtype == torch.uint8 and codes.is_cuda and codes.dim() == 2 and codes.stride(1) == 1
+    ch, n = codes.shape
+    fig_mode = torch.zeros(ch, dtype=torch.uint8, device=codes.device) if fig_mode is None else fig_mode
+    out = torch.zeros((ch, max(n, 1)), dtype=torch.uint8, device=codes.device)
+    count = torch.zeros(ch, dtype=torch.int32, device=codes.device)
+    _check(lib().csdrb_rtty_baudot2ascii_bank_u8_u8(codes.data_ptr(), codes.stride(0), out.data_ptr(), out.stride(0), ch, n,
+                                                    lengths.data_ptr() if lengths is not None else None, fig_mode.data_ptr(), count.data_ptr(),
+                                                    _stream()), "rtty_baudot2ascii_bank_u8_u8")
+    return out, count, fig_mode
 
 
 def fft_c2c(x, inverse: bool = False):

@@ -444,6 +444,26 @@ int csdrb_psk31_varicode_decoder_bank_u8_u8(const unsigned char* d_in, long in_s
     return rc < 0 ? rc : counted(0, rc);
 }
 
+// RTTY receive chain (rtty.cu; libcsdr.c:1662-1729, 1608-1616)
+int csdrb_serial_line_decoder_bank_f_u8(const float* d_in, long in_stride, int end, int* d_start_io, unsigned char* d_out, long out_stride, int* d_count,
+                                        int* d_stuck, int channels, const csdrb_serial_line_params_t* params, int bufsize, void* stream)
+{
+    static_assert(sizeof(csdrb_serial_line_params_t) == sizeof(SerialLineParams), "serial line params mirror kernels.h");
+    if (too_many_channels(channels, "serial_line bank")) return -1;
+    if (!d_in || !d_start_io || !d_out || !d_count || !d_stuck || !params) { set_error("serial_line bank: null pointer"); return -1; }
+    int rc = launch_serial_line_bank(d_in, in_stride, end, d_start_io, d_out, out_stride, d_count, d_stuck, channels, params, bufsize, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
+int csdrb_rtty_baudot2ascii_bank_u8_u8(const unsigned char* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels, int input_size,
+                                       const int* d_lengths, unsigned char* d_fig_mode_io, int* d_count, void* stream)
+{
+    if (null_io(d_in, d_out, "baudot bank")) return -1;
+    if (!d_fig_mode_io || !d_count) { set_error("baudot bank: null pointer"); return -1; }
+    int rc = launch_baudot_bank(d_in, in_stride, d_out, out_stride, channels, input_size, d_lengths, d_fig_mode_io, d_count, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
 int csdrb_fft_c2c_batch(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int size, int batch, int inverse, void* stream)
 {
     if (!d_in || !d_out) { set_error("fft: null pointer"); return -1; }

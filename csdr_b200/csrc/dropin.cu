@@ -610,4 +610,30 @@ void timing_recovery_cc(complexf* input, complexf* output, int input_size, float
     state->last_correction_offset = call.state.last_correction_offset;
 }
 
+// ---- RTTY receive chain -----------------------------------------------------------------------------------
+void serial_line_decoder_f_u8(serial_line_t* s, float* input, unsigned char* output, int input_size)
+{
+    const SerialLineParams p = {s->samples_per_bits, s->databits, s->stopbits, s->bit_sampling_width_ratio};
+    if (p.databits < 1 || p.databits > 8) {
+        set_error("databits %d: 1..8 are served (the CLI's range; wider characters are written as 16 or 32 bits)", p.databits);
+        die("serial_line_decoder_f_u8");
+    }
+    s->output_size = 0;
+    if (input_size <= 0) { s->input_used = 1; return; }                  // the edge search's i = 1 with nothing to read (libcsdr.c:1676-1678)
+    Staging st("serial_line_decoder_f_u8");
+    const float* d_in = st.up(input, input_size);
+    struct Row { int start, count, stuck; } row = {0, 0, 0};
+    Row* d_row = st.up(&row, 1);
+    const int cap = serial_line_max_outputs(p.samples_per_bits, p.databits, p.stopbits, input_size);
+    unsigned char* d_out = st.alloc<unsigned char>(cap);
+    st.check(csdrb_serial_line_decoder_bank_f_u8(d_in, input_size, input_size, &d_row->start, d_out, cap, &d_row->count, &d_row->stuck, 1,
+                                                 reinterpret_cast<const csdrb_serial_line_params_t*>(&p), input_size, st.stream()));
+    st.get(&row, d_row, 1);
+    st.sync();
+    st.get(output, d_out, row.count);
+    st.sync();
+    s->output_size = row.count;
+    s->input_used = row.start;
+}
+
 }  // extern "C"

@@ -97,6 +97,14 @@ int launch_dbpsk_bank(const float2* d_in, long in_stride, unsigned char* d_out, 
 int launch_varicode_bank(const unsigned char* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels, int n, const int* d_lengths,
                          unsigned long long* d_hist_io, int* d_count, cudaStream_t st);
 
+// RTTY receive chain, rtty.cu.  SerialLineParams has the layout of csdrb_serial_line_params_t.
+struct SerialLineParams { float samples_per_bits; int databits; float stopbits, bit_sampling_width_ratio; };
+int serial_line_max_outputs(float samples_per_bits, int databits, float stopbits, int input_size);   // characters input_size samples can hold at most
+int launch_serial_line_bank(const float* d_in, long in_stride, int end, int* d_start_io, unsigned char* d_out, long out_stride, int* d_count,
+                            int* d_stuck, int channels, const void* h_params_v, int bufsize, cudaStream_t st);   // SerialLineParams on the host
+int launch_baudot_bank(const unsigned char* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels, int n, const int* d_lengths,
+                       unsigned char* d_mode_io, int* d_count, cudaStream_t st);
+
 // K7/K8/K9 fft.cu
 int launch_fft_c2c_batch(const float2* d_in, long in_stride, float2* d_out, long out_stride, int n, int batch, int inverse, cudaStream_t st);
 int launch_olafir_bank(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int fft_size, int input_size,

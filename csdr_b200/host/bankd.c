@@ -1,5 +1,5 @@
 /*
- * bankd.c -- csdr-bankd: a whole bank of FM, AM, SSB or BPSK31 receivers on ONE wideband IQ stream, in one process.
+ * bankd.c -- csdr-bankd: a whole bank of FM, AM, SSB, BPSK31 or RTTY receivers on ONE wideband IQ stream, in one process.
  *
  * SURVEY.md 8(f) rank 2.  What the reference does with processes -- `nmux` fanning the IQ stream out over TCP (nmux.cpp:246-353)
  * to one `csdr shift_addition_cc | csdr fir_decimate_cc | csdr fmdemod_quadri_cf | ...` chain per listener (ddcd_old.h:51-57,
@@ -13,8 +13,8 @@
  * first -- is process plumbing and is not reproduced; tests/test_gpu_zzz_bankd.py compares against the oracle run over the whole stream).
  *
  * usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]
- *                   [--tail nfm|none|am|usb|lsb|iq|bpsk31] [--sps N] [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]
- *                   RATE:SINK [RATE:SINK ...]
+ *                   [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B] [--resample I:D[:BW]]
+ *                   [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...] RATE:SINK [RATE:SINK ...]
  *   --tail: nfm (default) the README.md:87 tail, s16; none the raw discriminator output, f32; am / usb / lsb the AM and SSB graphs of README.md:95 and :110
  *   behind the DDC's complex baseband (see bb_tail_t), s16; iq the complex baseband itself, cf32; bpsk31 the BPSK31 receive chain
  *   simple_agc_cc 0.001 R | timing_recovery_cc GARDNER N 0.5 2 --add_q | dbpsk_decoder_c_u8 | psk31_varicode_decoder_u8_u8 behind the baseband, the
@@ -23,6 +23,13 @@
  *   A PSK31 skimmer at 2.4 Msps: --decimation 300 --bw 0.001 gives 8 kHz baseband (4001 taps, M = 14 taps per output period: the fused bank serves it),
  *   and --sps 256 is 31.25 Bd:
  *     rtl_sdr -s 2400000 -f 14070000 - | csdr-bankd --decimation 300 --bw 0.001 --tail bpsk31 --sps 256 -0.1:ch1.txt 0.05:ch2.txt 0.2:ch3.txt
+ *   rtty: the RTTY receive chain serial_line_decoder_f_u8 F N S | rtty_baudot2ascii_u8_u8 behind the discriminator (the bank runs with fmdemod),
+ *   the decoded text per channel (--sps F: samples per bit at the baseband rate, a float; --databits N default 5, --stopbits S default 1.5).  The
+ *   decoder runs in calls of exactly --rtty-bufsize B samples (default the CLI's 16384), so the text lags the signal by up to B baseband samples
+ *   (about 8 s at 2 kHz); B must exceed F*(1 + N + S) + 2, or a call could not hold a character and the CLI would get stuck.  An RTTY skimmer
+ *   at 2.4 Msps: --decimation 1200 --bw 0.001 gives 2 kHz baseband (4001 taps, M = 4 per output period, D*MP = 4800 <= 8000: the fused bank
+ *   serves it), and --sps 44 is 45.45 Bd:
+ *     rtl_sdr -s 2400000 -f 14080000 - | csdr-bankd --decimation 1200 --bw 0.001 --tail rtty --sps 44 -0.1:ch1.txt 0.05:ch2.txt 0.2:ch3.txt
  *   --decimation: any even D (default 50) whose filter the fused bank serves: M = ceil(taps / D) <= 24 and D * M (rounded up to the kernel's
  *   bucket) <= 8000 taps, see csdrb_ddc_bank in include/csdr_b200.h.  The NFM tail's deemphasis_nfm_ff stays at 48000 whatever D gives: where
  *   wideband rate / D is not 48 kHz, --resample I:D[:BW] puts rational_resampler_ff I D BW right behind the discriminator (tails nfm and none; see
@@ -30,7 +37,7 @@
  *   RATE  shift_addition_cc rate (fraction of the wideband sample rate), SINK a path (file or FIFO) or tcp:PORT (one listener).
  *   --devices: the channels are sliced over several GPUs of this node (csdrb_multi_bank_*: the block goes to the first device once and on to
  *   the others by NCCL broadcast), one block of latency more (two blocks are kept in flight); the audio tail (nfm, am, usb, lsb), audio-rate work, runs on
- *   the first device for all channels, through the same kernels as without --devices.
+ *   the first device for all channels, through the same kernels as without --devices; so do the bpsk31 and rtty decoders.
  * Sinks never hold the stream up: a sink that cannot take a block within 200 ms loses the rest of that block (counted on stderr at exit), one
  * that fails is dropped -- nmux's policy for slow clients (tsmpool.cpp:101-117, nmux.cpp:339-346).
  */
@@ -296,7 +303,7 @@ static void raw_emit(const float *d_rows, long pitch, int n, unsigned char *h_ou
  *   mid  : [C][bs] float (am: DC-blocked envelope) or complexf (usb/lsb: filtered baseband) over the whole units
  *   pcm  : [C][whole] s16 */
 #define SSB_BW 0.05f                                      /* bandpass_fir_fft_cc transition bandwidth of README.md:110 */
-enum { TAIL_NFM, TAIL_NONE, TAIL_IQ, TAIL_AM, TAIL_USB, TAIL_LSB, TAIL_BPSK31 };
+enum { TAIL_NFM, TAIL_NONE, TAIL_IQ, TAIL_AM, TAIL_USB, TAIL_LSB, TAIL_BPSK31, TAIL_RTTY };
 
 /* ---- the BPSK31 tail: simple_agc_cc 0.001 R | timing_recovery_cc GARDNER N 0.5 2 --add_q | dbpsk_decoder_c_u8 | psk31_varicode_decoder_u8_u8 --------
  * Channels consume different amounts of baseband, so the timing recovery bank gets a start offset per channel.  Device buffers of ONE device:
@@ -389,6 +396,73 @@ static void bpsk_tail_push(bpsk_tail_t *t, channel_t *chan, const complexf *d_bb
         OK(csdrb_copy2d_d2h(t->h_chars, (size_t)m, t->d_chars, (size_t)t->cap, (size_t)m, (size_t)C, stream));
         OK(csdrb_stream_synchronize(stream));
         for (int c = 0; c < C; c++) if (t->h_char_count[c] > 0) write_sink(&chan[c], t->h_chars + (size_t)c * (size_t)m, (size_t)t->h_char_count[c]);
+    }
+}
+
+/* ---- the RTTY tail: serial_line_decoder_f_u8 F N S | rtty_baudot2ascii_u8_u8 behind the discriminator ---------------------------------------------
+ * Channels consume different amounts of signal, so each row has its own start.  Device buffers of ONE device:
+ *   rows  : [C][rs] float : discriminator output; row c's unconsumed samples are [start[c], end) (end is the same for every row), new ones go to end
+ *   codes : [C][cap] ITA2 codes, chars : [C][cap] decoded text
+ * The decoder bank runs calls of exactly B samples while B remain (the CLI's framing), so each row keeps fewer than B samples; after every push
+ * [min start, end) moves to the front of the rows.  Carried per channel: the start, the FIGS/LTRS mode. */
+typedef struct {
+    int C, B, end, cap;
+    long rs;
+    csdrb_serial_line_params_t p;
+    float *d_rows, *d_carry;
+    unsigned char *d_codes, *d_chars, *d_mode, *h_chars;
+    int *d_start, *d_count, *d_stuck, *d_char_count, *h_start;                 /* h_start: start[C], stuck[C], char_count[C] */
+} rtty_tail_t;
+
+static void rtty_tail_init(rtty_tail_t *t, int C, const csdrb_serial_line_params_t *p, int bufsize, int in_cap)
+{
+    memset(t, 0, sizeof *t);
+    t->C = C; t->B = bufsize; t->p = *p;
+    t->rs = ((long)bufsize + in_cap + 3) & ~3L;
+    t->cap = (int)(t->rs / (long)(p->samples_per_bits * ((float)(1 + p->databits) + p->stopbits)) + 1);   /* the bank's output bound */
+    t->d_rows = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)t->rs);
+    t->d_carry = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)bufsize);
+    t->d_codes = csdrb_device_alloc((size_t)C * (size_t)t->cap);
+    t->d_chars = csdrb_device_alloc((size_t)C * (size_t)t->cap);
+    t->d_mode = csdrb_device_alloc((size_t)C);                               /* zero-filled: letters mode */
+    t->d_start = csdrb_device_alloc(sizeof(int) * (size_t)C * 3);            /* start[C], stuck[C], char_count[C]: one copy back for all three */
+    t->d_stuck = t->d_start ? t->d_start + C : NULL;
+    t->d_char_count = t->d_start ? t->d_start + 2 * C : NULL;
+    t->d_count = csdrb_device_alloc(sizeof(int) * (size_t)C);
+    t->h_start = csdrb_host_alloc(sizeof(int) * (size_t)C * 3);
+    t->h_chars = csdrb_host_alloc((size_t)C * (size_t)t->cap);
+    if (!t->d_rows || !t->d_carry || !t->d_codes || !t->d_chars || !t->d_mode || !t->d_start || !t->d_count || !t->h_start || !t->h_chars)
+        die("out of memory");
+}
+
+/* n new discriminator samples per channel sit at d_rows + end: decode what fills whole calls, the text to the sinks, keep the rest */
+static void rtty_tail_push(rtty_tail_t *t, channel_t *chan, int n, void *stream)
+{
+    const int C = t->C;
+    t->end += n;
+    if (t->end > t->rs) die("rtty tail: signal buffer overflow");
+    OK(csdrb_serial_line_decoder_bank_f_u8(t->d_rows, t->rs, t->end, t->d_start, t->d_codes, t->cap, t->d_count, t->d_stuck, C, &t->p, t->B, stream));
+    OK(csdrb_rtty_baudot2ascii_bank_u8_u8(t->d_codes, t->cap, t->d_chars, t->cap, C, t->cap, t->d_count, t->d_mode, t->d_char_count, stream));
+    OK(csdrb_copy_d2h(t->h_start, t->d_start, sizeof(int) * (size_t)C * 3, stream));
+    OK(csdrb_copy_d2h(t->h_chars, t->d_chars, (size_t)C * (size_t)t->cap, stream));
+    OK(csdrb_stream_synchronize(stream));
+    const int *stuck = t->h_start + C, *chars = t->h_start + 2 * C;
+    int lo = t->end;
+    for (int c = 0; c < C; c++) {
+        if (stuck[c]) die("rtty tail: serial_line_decoder_f_u8 got stuck");   /* main() refuses the parameters that allow it */
+        if (chars[c] > 0) write_sink(&chan[c], t->h_chars + (size_t)c * (size_t)t->cap, (size_t)chars[c]);
+        lo = t->h_start[c] < lo ? t->h_start[c] : lo;
+    }
+    if (lo > 0) {                                                           /* the unconsumed samples (fewer than B per row) to the front */
+        const size_t row = sizeof(float) * (size_t)t->rs, keep = sizeof(float) * (size_t)(t->end - lo);
+        if (keep) {
+            OK(csdrb_copy2d_d2d(t->d_carry, sizeof(float) * (size_t)t->B, t->d_rows + lo, row, keep, (size_t)C, stream));
+            OK(csdrb_copy2d_d2d(t->d_rows, row, t->d_carry, sizeof(float) * (size_t)t->B, keep, (size_t)C, stream));
+        }
+        for (int c = 0; c < C; c++) t->h_start[c] -= lo;
+        t->end -= lo;
+        OK(csdrb_copy_h2d(t->d_start, t->h_start, sizeof(int) * (size_t)C, stream));
+        OK(csdrb_stream_synchronize(stream));
     }
 }
 
@@ -497,9 +571,9 @@ static void bb_tail_push(bb_tail_t *t, channel_t *chan, int n_new, void *stream)
 }
 
 static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *chan, int C, const float *rates, int D, const float *taps, int T, int block,
-                     int kind, float limit, float agc_ref, int rs_I, int rs_D, float rs_bw, int sps)
+                     int kind, float limit, float agc_ref, int rs_I, int rs_D, float rs_bw, int sps, const csdrb_serial_line_params_t *rtty_p, int rtty_B)
 {
-    const int nfm = kind == TAIL_NFM, demod = kind == TAIL_NFM || kind == TAIL_NONE;
+    const int nfm = kind == TAIL_NFM, rtty = kind == TAIL_RTTY, demod = nfm || rtty || kind == TAIL_NONE;
     const size_t osz = demod ? sizeof(float) : sizeof(complexf);
     csdrb_multi_bank_t *mb = csdrb_multi_bank_create(ndev, dev, C, rates, D, taps, T, demod, 1024, block);
     if (!mb) die("cannot create the multi-GPU bank");
@@ -512,7 +586,7 @@ static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *cha
     if (!h_wide[0] || !h_wide[1] || !h_out[0] || !h_out[1] || !raw) die("out of memory");
     /* --tail nfm: the audio tail is audio-rate work (C x 48 kHz): the discriminator rows every device returned go to the FIRST device once more and through
      * the same kernels as in the single-GPU path */
-    nfm_tail_t tail_state; bb_tail_t bb; rs_stage_t rsm; void *tail_stream = NULL;
+    nfm_tail_t tail_state; bb_tail_t bb; rs_stage_t rsm; rtty_tail_t rt; void *tail_stream = NULL;
     float *d_raw_out = NULL; unsigned char *h_raw_out = NULL;
     const int resample = rs_I > 0;
     if (kind != TAIL_NONE || resample) {
@@ -522,6 +596,7 @@ static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *cha
         if (resample) rs_init(&rsm, C, rs_I, rs_D, rs_bw, n_out + 2);
         const int tail_cap = resample ? rs_out_cap(&rsm) : n_out + 2;
         if (nfm) nfm_tail_init(&tail_state, C, tail_cap, limit, agc_ref);
+        else if (rtty) rtty_tail_init(&rt, C, rtty_p, rtty_B, tail_cap);
         else if (!demod) bb_tail_init(&bb, kind, C, tail_cap, limit, agc_ref, sps, tail_stream);
         else {
             d_raw_out = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)tail_cap);
@@ -540,6 +615,10 @@ static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *cha
             OK(csdrb_copy2d_h2d(tail_state.d_demod + tail_state.a_have, sizeof(float) * (size_t)tail_state.ds, h_out[slot_], sizeof(float) * (size_t)n_out, \
                                 sizeof(float) * (size_t)n_out, (size_t)C, tail_stream)); \
             nfm_tail_push(&tail_state, chan, n_out, tail_stream); \
+        } else if (rtty) { \
+            OK(csdrb_copy2d_h2d(rt.d_rows + rt.end, sizeof(float) * (size_t)rt.rs, h_out[slot_], sizeof(float) * (size_t)n_out, \
+                                sizeof(float) * (size_t)n_out, (size_t)C, tail_stream)); \
+            rtty_tail_push(&rt, chan, n_out, tail_stream); \
         } else if (!demod) { \
             OK(csdrb_copy2d_h2d(bb.d_bb + bb.have, sizeof(complexf) * (size_t)bb.bs, h_out[slot_], sizeof(complexf) * (size_t)n_out, \
                                 sizeof(complexf) * (size_t)n_out, (size_t)C, tail_stream)); \
@@ -585,13 +664,19 @@ static int usage(void)
 {
     fprintf(stderr,
             "usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]\n"
-            "                  [--tail nfm|none|am|usb|lsb|iq|bpsk31] [--sps N] [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]\n"
-            "                  RATE:SINK [RATE:SINK ...]\n"
+            "                  [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B]\n"
+            "                  [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...] RATE:SINK [RATE:SINK ...]\n"
             "  --tail bpsk31 --sps N  per channel simple_agc_cc 0.001 R | timing_recovery_cc GARDNER N 0.5 2 --add_q | dbpsk_decoder_c_u8 |\n"
             "                       psk31_varicode_decoder_u8_u8 (R = --agc-ref, default 0.5) behind the baseband; the sinks get the decoded text.\n"
             "                       N is samples per symbol at the baseband rate, > 4 and divisible by 4.  A PSK31 skimmer at 2.4 Msps:\n"
             "                       csdr-bankd --decimation 300 --bw 0.001 --tail bpsk31 --sps 256 -0.1:ch1.txt 0.05:ch2.txt 0.2:ch3.txt\n"
             "                       (8 kHz baseband, 4001 taps = 14 per output period, which the fused bank serves; 31.25 Bd)\n"
+            "  --tail rtty --sps F    per channel fmdemod_quadri_cf | serial_line_decoder_f_u8 F N S | rtty_baudot2ascii_u8_u8 (--databits N, default 5;\n"
+            "                       --stopbits S, default 1.5); the sinks get the decoded text.  F is samples per bit at the baseband rate (a float).\n"
+            "                       The decoder runs in calls of --rtty-bufsize B samples (default 16384, the CLI's), so the text lags the signal\n"
+            "                       by up to B samples; B must exceed F*(1 + N + S) + 2.  An RTTY skimmer at 2.4 Msps:\n"
+            "                       csdr-bankd --decimation 1200 --bw 0.001 --tail rtty --sps 44 -0.1:ch1.txt 0.05:ch2.txt 0.2:ch3.txt\n"
+            "                       (2 kHz baseband, 4001 taps = 4 per output period, which the fused bank serves; 45.45 Bd; about 8 s of lag)\n"
             "  --resample I:D[:BW]  rational_resampler_ff I D BW (BW default 0.05) right behind the discriminator, for --tail nfm and none: brings\n"
             "                       wideband/decimation to the 48 kHz the NFM de-emphasis is designed for (e.g. 2.048 Msps, --decimation 32,\n"
             "                       --resample 3:4).  With T = taps of BW, the daemon needs (T/I + 1)*I >= 2*D + I - 1 (T >= 2*D + I - 2 suffices),\n"
@@ -607,6 +692,9 @@ int main(int argc, char **argv)
     float bw = 0.005f, limit = 1.0f, agc_ref = 0.0f;                /* agc_ref 0: the tail's own default (fastagc_ff 1.0, agc_ff 0.2) */
     int rs_I = 0, rs_D = 0;                                          /* --resample I:D[:BW]; 0: no resampler */
     int sps = 0;                                                     /* --sps N of --tail bpsk31 */
+    float spb = 0.f;                                                 /* --sps F of --tail rtty */
+    int databits = 5, rtty_B = 16384, rtty_opts = 0;                 /* --databits, --rtty-bufsize (the CLI's big buffer, csdr.c:190) */
+    float stopbits = 1.5f;                                           /* --stopbits */
     float rs_bw = 0.05f;                                             /* rational_resampler_ff's default transition bandwidth (csdr.c:1423) */
     window_t window = WINDOW_HAMMING;
     channel_t *chan = calloc((size_t)argc, sizeof *chan);
@@ -624,7 +712,10 @@ int main(int argc, char **argv)
         else if (!strcmp(o, "--tail") && v) { tail = v; a++; }
         else if (!strcmp(o, "--limit") && v) { limit = (float)atof(v); a++; }
         else if (!strcmp(o, "--agc-ref") && v) { agc_ref = (float)atof(v); a++; }
-        else if (!strcmp(o, "--sps") && v) { sps = atoi(v); a++; }
+        else if (!strcmp(o, "--sps") && v) { sps = atoi(v); spb = (float)atof(v); a++; }
+        else if (!strcmp(o, "--databits") && v) { databits = atoi(v); rtty_opts = 1; a++; }
+        else if (!strcmp(o, "--stopbits") && v) { stopbits = (float)atof(v); rtty_opts = 1; a++; }
+        else if (!strcmp(o, "--rtty-bufsize") && v) { rtty_B = atoi(v); rtty_opts = 1; a++; }
         else if (!strcmp(o, "--device") && v) { device = atoi(v); a++; }
         else if (!strcmp(o, "--devices") && v) { ndev = parse_devices(v, devs, 64); if (ndev <= 0) die("--devices wants N0,N1,..."); a++; }
         else if (!strcmp(o, "--resample") && v) {
@@ -644,15 +735,26 @@ int main(int argc, char **argv)
             chan[C].sink = end + 1; chan[C].fd = -1; chan[C].dropped = 0; C++;
         } else { fprintf(stderr, "csdr-bankd: unknown argument %s\n", o); return 2; }
     }
-    static const char *kTails[] = {"nfm", "none", "iq", "am", "usb", "lsb", "bpsk31"};
+    static const char *kTails[] = {"nfm", "none", "iq", "am", "usb", "lsb", "bpsk31", "rtty"};
     int kind = -1;
-    for (int k = 0; k < 7; k++) if (!strcmp(tail, kTails[k])) kind = k;
-    if (kind < 0) die("--tail is nfm, none, iq, am, usb, lsb or bpsk31");
+    for (int k = 0; k < 8; k++) if (!strcmp(tail, kTails[k])) kind = k;
+    if (kind < 0) die("--tail is nfm, none, iq, am, usb, lsb, bpsk31 or rtty");
+    const csdrb_serial_line_params_t rtty_p = {spb, databits, stopbits, 0.4f};   /* serial_line_decoder_f_u8's bit_sampling_width_ratio (csdr.c:2510) */
     if (kind == TAIL_BPSK31) {
         if (sps <= 4 || (sps & 3)) die("--tail bpsk31 needs --sps N with N > 4 and divisible by 4 (timing_recovery_cc's decimation)");
         if (agc_ref == 0.0f) agc_ref = 0.5f;                         /* simple_agc_cc's reference in the OpenWebRX chain */
-    } else if (sps) die("--sps belongs to --tail bpsk31");
-    const int nfm = kind == TAIL_NFM, demod = kind == TAIL_NFM || kind == TAIL_NONE;
+    } else if (kind == TAIL_RTTY) {
+        if (!(spb >= 1.f && spb <= 1e6f)) die("--tail rtty needs --sps F, samples per bit at the baseband rate, at least 1 (serial_line_decoder_f_u8's range)");
+        if (spb < 5.f) fprintf(stderr, "csdr-bankd: warning: serial_line_decoder_f_u8 does not work well below 5 samples per bit\n");
+        if (databits < 1 || databits > 8) die("--databits must be between 1 and 8");
+        if (!(stopbits >= 1.f && stopbits <= 1000.f)) die("--stopbits must be at least 1");
+        if (rtty_B < 1 || rtty_B > (1 << 22)) die("--rtty-bufsize must be between 1 and 4194304 samples");
+        /* a character that starts at the third sample of a call and does not fit makes the call consume nothing: the CLI exits "stuck" */
+        if (spb * ((float)(1 + databits) + stopbits) + 2.0f >= (float)rtty_B)
+            die("--rtty-bufsize must exceed sps*(1 + databits + stopbits) + 2: a call could not hold one character and would get stuck");
+    } else if (sps) die("--sps belongs to --tail bpsk31 and --tail rtty");
+    if (kind != TAIL_RTTY && rtty_opts) die("--databits, --stopbits and --rtty-bufsize belong to --tail rtty");
+    const int nfm = kind == TAIL_NFM, rtty = kind == TAIL_RTTY, demod = nfm || rtty || kind == TAIL_NONE;
     if (nfm && agc_ref == 0.0f) agc_ref = 1.0f;                      /* fastagc_ff's default reference (csdr.c:1388) */
     if (C == 0) die("no channels (RATE:SINK ...)");
     if (block <= 0 || (block & 1)) die("--block must be a positive even number of samples");
@@ -661,7 +763,7 @@ int main(int argc, char **argv)
     if (!(limit > 0.f) || !(agc_ref >= 0.f)) die("--limit and --agc-ref must be positive");
     const int resample = rs_I > 0;
     if (resample) {
-        if (!demod) die("--resample works with --tail nfm and --tail none only (the am, usb, lsb, iq and bpsk31 tails are not resampled)");
+        if (!demod || rtty) die("--resample works with --tail nfm and --tail none only (the am, usb, lsb, iq, bpsk31 and rtty tails are not resampled)");
         if (!(rs_bw > 0.f && rs_bw < 0.5f)) die("--resample: the transition bandwidth must be between 0 and 0.5");
         const int rs_T = firdes_filter_len(rs_bw);
         if (!resample_geometry_ok(rs_I, rs_D, rs_T)) {
@@ -684,7 +786,7 @@ int main(int argc, char **argv)
         for (int c = 0; c < C; c++) { chan[c].fd = open_sink(chan[c].sink); sink_nonblocking(chan[c].fd); }
         const int fd = open_input(in_spec);
         fprintf(stderr, "csdr-bankd: %d channels over %d devices, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, ndev, D, T, u8 ? "u8" : "f32", block, tail);
-        const int rc = run_multi(fd, u8, devs, ndev, chan, C, rates, D, taps, T, block, kind, limit, agc_ref, rs_I, rs_D, rs_bw, sps);
+        const int rc = run_multi(fd, u8, devs, ndev, chan, C, rates, D, taps, T, block, kind, limit, agc_ref, rs_I, rs_D, rs_bw, sps, &rtty_p, rtty_B);
         for (int c = 0; c < C; c++) { if (chan[c].dropped) fprintf(stderr, "csdr-bankd: sink %s lost %ld bytes (too slow)\n", chan[c].sink, chan[c].dropped); if (chan[c].fd >= 0) close(chan[c].fd); }
         return rc;
     }
@@ -706,12 +808,14 @@ int main(int argc, char **argv)
     nfm_tail_t tl;
     bb_tail_t bb;
     rs_stage_t rsm;
+    rtty_tail_t rt;
     if (resample) rs_init(&rsm, C, rs_I, rs_D, rs_bw, out_cap);
     const int tail_cap = resample ? rs_out_cap(&rsm) : out_cap;   /* samples one block can add behind the discriminator (and resampler) */
     long ds = ((long)tail_cap + 3) & ~3L;
     float *d_demod = NULL;
     unsigned char *h_out = NULL;
     if (nfm) { nfm_tail_init(&tl, C, tail_cap, limit, agc_ref); ds = tl.ds; d_demod = tl.d_demod; }
+    else if (rtty) { rtty_tail_init(&rt, C, &rtty_p, rtty_B, out_cap); ds = rt.rs; d_demod = rt.d_rows; }
     else if (!demod) { bb_tail_init(&bb, kind, C, out_cap, limit, agc_ref, sps, stream); ds = bb.bs; d_demod = (float *)bb.d_bb; }
     else {
         d_demod = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)ds);
@@ -742,7 +846,8 @@ int main(int argc, char **argv)
         const int n_in = block;
 
         /* 2. shift | fir_decimate | fmdemod for every channel, new discriminator samples behind the de-emphasis FIR's carried inputs */
-        void *dst = resample ? (void *)(rsm.d_in + rsm.have) : nfm ? (void *)(d_demod + tl.a_have) : !demod ? (void *)(bb.d_bb + bb.have) : (void *)d_demod;
+        void *dst = resample ? (void *)(rsm.d_in + rsm.have) : nfm ? (void *)(d_demod + tl.a_have) : rtty ? (void *)(rt.d_rows + rt.end)
+                  : !demod ? (void *)(bb.d_bb + bb.have) : (void *)d_demod;
         const int n_out = csdrb_ddc_bank_process(bank, d_wide[cur], n_in, dst, resample ? rsm.rs : ds, stream);
         if (n_out < 0) die("csdrb_ddc_bank_process failed");
         const int consumed = n_out * D;
@@ -753,6 +858,7 @@ int main(int argc, char **argv)
         /* 2b. --resample: the new discriminator samples through rational_resampler_ff, into the tail's rows */
         const int n_tail = resample ? rs_push(&rsm, n_out, nfm ? d_demod + tl.a_have : d_demod, ds, stream) : n_out;
         if (!demod) bb_tail_push(&bb, chan, n_out, stream);         /* baseband tails: am / usb / lsb audio, or the raw baseband */
+        else if (rtty) rtty_tail_push(&rt, chan, n_out, stream);    /* serial_line_decoder_f_u8 | rtty_baudot2ascii_u8_u8, text to the sinks */
         else if (!nfm) raw_emit(d_demod, ds, n_tail, h_out, chan, C, stream);   /* raw discriminator output, float */
         else nfm_tail_push(&tl, chan, n_tail, stream);             /* 3./4. limit | de-emphasis | AGC | s16, audio to the sinks */
         blocks++;

@@ -908,6 +908,66 @@ static int cmd_psk31_varicode_decoder_u8_u8(int argc, char **argv)
     }
 }
 
+static int cmd_serial_line_decoder_f_u8(int argc, char **argv)               /* csdr.c:2490-2530 */
+{
+    G.wideband = 1;
+    serial_line_t serial = {0};
+    if (argc <= 2) return complain("need required parameter (samples_per_bits)");
+    sscanf(argv[2], "%f", &serial.samples_per_bits);
+    if (serial.samples_per_bits < 1) return complain("samples_per_bits should be at least 1.");
+    if (serial.samples_per_bits < 5)
+        fprintf(stderr, "%s: warning: this algorithm does not work well if samples_per_bits is too low. It should be at least 5.\n", argv[1]);
+    serial.databits = 8;
+    if (argc > 3) sscanf(argv[3], "%d", &serial.databits);
+    if (serial.databits > 8 || serial.databits < 1) return complain("databits should be between 1 and 8.");
+    serial.stopbits = 1;
+    if (argc > 4) sscanf(argv[4], "%f", &serial.stopbits);
+    if (serial.stopbits < 1) return complain("stopbits should be equal or above 1.");
+    serial.bit_sampling_width_ratio = 0.4f;
+    if (!announce_block(open_block())) return -2;
+    float *in = must_alloc(sizeof(float) * (size_t)block);
+    unsigned char *out = must_alloc((size_t)block);
+    /* the reference keeps what a call left unconsumed at the front and refills behind it; after a short final read the buffer's tail still
+     * holds the samples of the call before, and that last call is decoded and written like any other */
+    for (;;) {
+        if (feof(stdin)) return 0;
+        if (serial.input_used) {
+            memmove(in, in + serial.input_used, sizeof(float) * (size_t)(block - serial.input_used));
+            fread(in + (block - serial.input_used), sizeof(float), (size_t)serial.input_used, stdin);
+        } else fread(in, sizeof(float), (size_t)block, stdin);
+        serial_line_decoder_f_u8(&serial, in, out, block);
+        if (serial.input_used == 0) { who(); fprintf(stderr, "error: serial_line_decoder_f_u8() got stuck.\n"); return -3; }
+        fwrite(out, 1, (size_t)serial.output_size, stdout);
+        end_of_block();
+    }
+}
+
+/* csdr.c:2461-2474 pushes one getchar() at a time through rtty_baudot_decoder_lookup and flushes every character; after the end of the input
+ * it pushes up to 255 EOF values (0xFF), which give nothing.  Here every read() (whatever the pipe holds, up to one block) goes through the
+ * baudot bank, and the characters it decoded are written and flushed at once. */
+static int cmd_rtty_baudot2ascii_u8_u8(int argc, char **argv)
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    unsigned char *in = must_alloc((size_t)block), *out = must_alloc((size_t)block);
+    unsigned char *d_in = csdrb_device_alloc((size_t)block), *d_out = csdrb_device_alloc((size_t)block);
+    unsigned char *d_mode = csdrb_device_alloc(1);                             /* zero-filled: letters mode, as fig_mode = 0 */
+    int *d_count = csdrb_device_alloc(sizeof(int));
+    if (!d_in || !d_out || !d_mode || !d_count) { who(); fprintf(stderr, "%s\n", csdrb_last_error()); return -2; }
+    for (;;) {
+        const ssize_t got = read(STDIN_FILENO, in, (size_t)block);
+        if (got <= 0) return 0;
+        int count = 0;
+        if (csdrb_copy_h2d(d_in, in, (size_t)got, NULL) < 0 ||
+            csdrb_rtty_baudot2ascii_bank_u8_u8(d_in, got, d_out, got, 1, (int)got, NULL, d_mode, d_count, NULL) < 0 ||
+            csdrb_copy_d2h(&count, d_count, sizeof count, NULL) < 0 || csdrb_stream_synchronize(NULL) < 0 ||
+            (count > 0 && (csdrb_copy_d2h(out, d_out, (size_t)count, NULL) < 0 || csdrb_stream_synchronize(NULL) < 0))) {
+            who(); fprintf(stderr, "%s\n", csdrb_last_error()); return -2;
+        }
+        if (count > 0) { fwrite(out, 1, (size_t)count, stdout); fflush(stdout); }
+    }
+}
+
 /* ---- dispatch ------------------------------------------------------------------------------------ */
 static const struct { const char *name; int (*run)(int, char **); const char *syntax; } kCommands[] = {
     {"convert_u8_f", cmd_convert_u8_f, "convert_u8_f"},
@@ -946,6 +1006,8 @@ static const struct { const char *name; int (*run)(int, char **); const char *sy
     {"timing_recovery_cc", cmd_timing_recovery_cc, "timing_recovery_cc <algorithm> <decimation> [mu [max_error [--add_q [--output_error | --output_indexes]]]]"},
     {"dbpsk_decoder_c_u8", cmd_dbpsk_decoder_c_u8, "dbpsk_decoder_c_u8"},
     {"psk31_varicode_decoder_u8_u8", cmd_psk31_varicode_decoder_u8_u8, "psk31_varicode_decoder_u8_u8"},
+    {"serial_line_decoder_f_u8", cmd_serial_line_decoder_f_u8, "serial_line_decoder_f_u8 <samples_per_bits> [databits [stopbits]]"},
+    {"rtty_baudot2ascii_u8_u8", cmd_rtty_baudot2ascii_u8_u8, "rtty_baudot2ascii_u8_u8"},
     {"fastddc_inv_cc", cmd_fastddc_inv_cc, "fastddc_inv_cc <shift_rate> <decimation> [transition_bw [window]] | --fifo <fifo_path> ... | --fd <fd> ..."},
 };
 

@@ -117,6 +117,16 @@ timing_recovery_state_t timing_recovery_init(timing_recovery_algorithm_t algorit
                                              int debug_every_nth, char *debug_writefiles_path);
 void timing_recovery_cc(complexf *input, complexf *output, int input_size, float *timing_error, int *sampled_indexes, timing_recovery_state_t *state);
 
+/* RTTY receive chain (libcsdr.h:278-287; libcsdr.c:1662-1729), computed as the reference's -O3 -ffast-math build computes it (DESIGN.md
+ * section 7).  serial_line_decoder_f_u8 serves what the CLI accepts -- databits 1..8, samples_per_bits and stopbits >= 1 -- with
+ * 0 <= bit_sampling_width_ratio <= 1 and input_size <= 2^22; other values print `libcsdr_b200: serial_line_decoder_f_u8 failed: ...` and
+ * abort, like any other failing drop-in.  rtty_baudot_decoder_lookup and _push, one symbol per call, are not offered here: the bank
+ * csdrb_rtty_baudot2ascii_bank_u8_u8 decodes whole streams. */
+typedef struct serial_line_s {
+    float samples_per_bits; int databits; float stopbits; int output_size; int input_used; float bit_sampling_width_ratio;
+} serial_line_t;
+void serial_line_decoder_f_u8(serial_line_t *s, float *input, unsigned char *output, int input_size);
+
 /* audio tail of the WFM graph, SURVEY 8(f) rank 1 (libcsdr.h:100-105; libcsdr.c:1081-1097, 1130-1137) */
 float deemphasis_wfm_ff(float *input, float *output, int input_size, float tau, int sample_rate, float last_output);
 void  limit_ff(float *input, float *output, int input_size, float max_amplitude);
@@ -443,6 +453,27 @@ int csdrb_dbpsk_decoder_bank_c_u8(const complexf *d_in, long in_stride, unsigned
  * to d_count[c].  d_hist_io[c] is the decoder's shift register (0 at stream start).  out_stride >= input_size.  Returns 0. */
 int csdrb_psk31_varicode_decoder_bank_u8_u8(const unsigned char *d_in, long in_stride, unsigned char *d_out, long out_stride, int channels,
                                             int input_size, const int *d_lengths, unsigned long long *d_hist_io, int *d_count, void *stream);
+
+/* RTTY receive chain banks (rtty.cu), one row per channel.
+ *
+ * serial_line_decoder_f_u8 bank: channel c's unconsumed discriminator samples are d_in[c*in_stride + d_start_io[c] .. end) (0 <= d_start_io[c]
+ * <= end, one end for all rows).  While at least bufsize of them remain, one serial_line_decoder_f_u8 call (libcsdr.c:1662-1729) runs on
+ * exactly bufsize samples from d_start_io[c], bit for bit with the reference build, and d_start_io[c] advances by its input_used: the CLI's
+ * memmove-and-refill framing (csdr.c:2517-2527), so a row gives the bytes the CLI gives with the same buffer size, and bufsize = n on rows of
+ * n samples is exactly one call.  A call that consumes nothing is where the CLI exits with "got stuck": the row stops there and d_stuck[c] = 1
+ * (else 0).  The characters (one byte each) go to row c of d_out in order and their count to d_count[c]; out_stride must hold the most a row
+ * can give, end / floor(all_bits * samples_per_bits) + 1 with all_bits = 1 + databits + stopbits (float).  Serves databits 1..8,
+ * samples_per_bits in [1, 1e6], stopbits in [1, 1000], 0 <= bit_sampling_width_ratio <= 1 (the CLI uses 0.4) and 1 <= bufsize <= 2^22; -1
+ * otherwise.  The counts and positions are data-dependent: read them back to use them.  Returns 0. */
+typedef struct csdrb_serial_line_params_s { float samples_per_bits; int databits; float stopbits, bit_sampling_width_ratio; } csdrb_serial_line_params_t;
+int csdrb_serial_line_decoder_bank_f_u8(const float *d_in, long in_stride, int end, int *d_start_io, unsigned char *d_out, long out_stride, int *d_count,
+                                        int *d_stuck, int channels, const csdrb_serial_line_params_t *params, int bufsize, void *stream);
+/* rtty_baudot2ascii bank: row c holds d_lengths[c] <= input_size ITA2 codes (d_lengths NULL: input_size each) and goes through
+ * rtty_baudot_decoder_lookup (libcsdr.c:1608-1616) code by code; the non-zero characters go to the row of d_out in order and their count to
+ * d_count[c].  d_fig_mode_io[c] is the letters (0) / figures (1) mode, carried between calls (0 at stream start).  out_stride >= input_size.
+ * Returns 0. */
+int csdrb_rtty_baudot2ascii_bank_u8_u8(const unsigned char *d_in, long in_stride, unsigned char *d_out, long out_stride, int channels, int input_size,
+                                       const int *d_lengths, unsigned char *d_fig_mode_io, int *d_count, void *stream);
 
 /* K7 batched unnormalised c2c DFT (power-of-two size 2..16384), sign -1 forward / +1 inverse */
 int csdrb_fft_c2c_batch(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int size, int batch, int inverse, void *stream);
