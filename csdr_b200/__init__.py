@@ -71,6 +71,14 @@ class SerialLineParams(C.Structure):    # csdrb_serial_line_params_t
     _fields_ = [("samples_per_bits", C.c_float), ("databits", C.c_int), ("stopbits", C.c_float), ("bit_sampling_width_ratio", C.c_float)]
 
 
+class SpectrumParams(C.Structure):      # csdrb_spectrum_params_t
+    _fields_ = [("fft_size", C.c_int), ("every", C.c_int), ("averages", C.c_int), ("compress", C.c_int), ("add_db", C.c_float)]
+
+
+class SpectrumState(C.Structure):       # csdrb_spectrum_state_t; {0, 0} at stream start
+    _fields_ = [("consumed", C.c_longlong), ("frames", C.c_longlong)]
+
+
 class _SerialLine(C.Structure):         # serial_line_t (= libcsdr.h:278-286)
     _fields_ = [("samples_per_bits", C.c_float), ("databits", C.c_int), ("stopbits", C.c_float), ("output_size", C.c_int),
                 ("input_used", C.c_int), ("bit_sampling_width_ratio", C.c_float)]
@@ -250,6 +258,9 @@ def lib() -> C.CDLL:
     L.csdrb_serial_line_decoder_bank_f_u8.argtypes = [vp, lg, it, vp, vp, lg, vp, vp, it, C.POINTER(SerialLineParams), it, vp]
     L.csdrb_rtty_baudot2ascii_bank_u8_u8.argtypes = [vp, lg, vp, lg, it, it, vp, vp, vp, vp]
     L.serial_line_decoder_f_u8.argtypes = [C.POINTER(_SerialLine), vp, vp, it]
+    L.csdrb_spectrum_bank_lines.argtypes = [C.POINTER(SpectrumParams), C.POINTER(SpectrumState), lg]; L.csdrb_spectrum_bank_lines.restype = lg
+    L.csdrb_spectrum_bank_scratch_bytes.argtypes = [it, lg, C.POINTER(SpectrumParams)]; L.csdrb_spectrum_bank_scratch_bytes.restype = sz
+    L.csdrb_spectrum_bank_cf.argtypes = [vp, lg, it, lg, vp, C.POINTER(SpectrumParams), vp, vp, C.POINTER(SpectrumState), vp, lg, vp, sz, vp]
     _lib = L
     return L
 
@@ -1438,6 +1449,49 @@ def shift_unroll_bank_cc(x, rates, phases=None, table_size: int = 1024, out=None
     _check(lib().csdrb_shift_unroll_bank_cc(ptr, stride, out.data_ptr(), out.stride(0), ch, n, params.data_ptr(), d_ds.data_ptr(), d_dc.data_ptr(), table_size,
                                             table_size, d_phase.data_ptr(), scratch.data_ptr(), scratch.numel(), _stream()), "shift_unroll_bank_cc")
     return out, d_phase
+
+
+class SpectrumBank:
+    """The OpenWebRX waterfall chain `fft_cc N E W | logaveragepower_cf ADD_DB N A | fft_exchange_sides_ff N [| compress_fft_adpcm_f_u8 N]` on
+    `rows` streams at once (csdrb_spectrum_bank_cf).  Owns the window table, the carried history and partial line, and the host state;
+    process(x) takes the next n samples of every row ([rows, n] complex64 CUDA tensor, or [n] for one row) and returns the lines they complete:
+    [rows, lines, N] float32 dB, or [rows, lines, (N + 10) // 2] uint8 with compress=True."""
+
+    def __init__(self, rows: int, fft_size: int, every: int, averages: int, add_db: float, window: str = "HAMMING", compress: bool = False,
+                 device="cuda"):
+        import torch
+        self.rows, self.device = rows, torch.device(device)
+        self.params = SpectrumParams(fft_size, every, averages, 1 if compress else 0, add_db)
+        self.state = SpectrumState(0, 0)
+        self.window = torch.from_numpy(libcsdr.precalculate_window(fft_size, window)).to(self.device)
+        self.hist = torch.zeros((rows, fft_size), dtype=torch.complex64, device=self.device)
+        self.acc = torch.zeros((rows, fft_size), dtype=torch.float32, device=self.device)
+        self.line_bytes = (fft_size + 10) // 2 if compress else 4 * fft_size
+
+    def lines(self, n: int) -> int:
+        return _check(lib().csdrb_spectrum_bank_lines(C.byref(self.params), C.byref(self.state), n), "spectrum_bank_lines")
+
+    def process(self, x, scratch_bytes: int | None = None):
+        import torch
+        if x.dtype == torch.complex64 and x.dim() == 1:
+            x = x.unsqueeze(0)
+        xr, ptr, stride, rows, n = _as_cf32_rows(x)
+        if rows != self.rows:
+            raise ValueError(f"expected {self.rows} rows, got {rows}")
+        N, L = self.params.fft_size, self.lines(n)
+        if self.params.compress:
+            out = torch.empty((rows, L, self.line_bytes), dtype=torch.uint8, device=self.device)
+        else:
+            out = torch.empty((rows, L, N), dtype=torch.float32, device=self.device)
+        if scratch_bytes is None:
+            scratch_bytes = lib().csdrb_spectrum_bank_scratch_bytes(rows, n, C.byref(self.params))
+        scratch = _scratch(scratch_bytes + 16, self.device)
+        got = _check(lib().csdrb_spectrum_bank_cf(ptr if n else self.hist.data_ptr(), stride, rows, n, self.window.data_ptr(), C.byref(self.params),
+                                                  self.hist.data_ptr(), self.acc.data_ptr(), C.byref(self.state),
+                                                  out.data_ptr() if out.numel() else self.acc.data_ptr(),
+                                                  out.stride(0) * out.element_size(), scratch.data_ptr(), scratch_bytes, _stream()), "spectrum_bank_cf")
+        assert got == L
+        return out
 
 
 def spectrum_logpower(x, fft_size: int, window: str = "HAMMING", add_db: float = 0.0):

@@ -573,6 +573,20 @@ int csdrb_log_ff(const float* d_in, float* d_out, long n, float add_db, void* st
     int rc = launch_power(nullptr, d_in, d_out, n, add_db, 2, S(stream));
     return rc < 0 ? rc : counted(0, rc);
 }
+// waterfall bank (spectrum.cu): fft_cc | logaveragepower_cf | fft_exchange_sides_ff [| compress_fft_adpcm_f_u8] per row
+long csdrb_spectrum_bank_lines(const csdrb_spectrum_params_t* p, const csdrb_spectrum_state_t* s, long n) { return spectrum_lines(p, s, n); }
+size_t csdrb_spectrum_bank_scratch_bytes(int rows, long n, const csdrb_spectrum_params_t* p) { return spectrum_scratch_bytes(rows, n, p); }
+int csdrb_spectrum_bank_cf(const complexf* d_in, long in_stride, int rows, long n, const float* d_window, const csdrb_spectrum_params_t* p,
+                           complexf* d_hist_io, float* d_acc_io, csdrb_spectrum_state_t* state_io, void* d_out, long out_stride_bytes,
+                           void* d_scratch, size_t scratch_bytes, void* stream)
+{
+    static_assert(sizeof(csdrb_spectrum_params_t) == sizeof(SpectrumParams) && sizeof(csdrb_spectrum_state_t) == sizeof(SpectrumState),
+                  "spectrum structs mirror kernels.h");
+    int launches = 0;
+    int rc = launch_spectrum_bank(reinterpret_cast<const float2*>(d_in), in_stride, rows, n, d_window, p, reinterpret_cast<float2*>(d_hist_io), d_acc_io,
+                                  state_io, d_out, out_stride_bytes, d_scratch, scratch_bytes, &launches, S(stream));
+    return rc < 0 ? rc : counted(rc, launches);
+}
 int csdrb_shift_unroll_bank_cc(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int input_size,
                                const shift_addition_data_t* d_params, const float* d_dsin, const float* d_dcos, long table_stride, int table_size,
                                float* d_phase_io, void* d_scratch, size_t scratch_bytes, void* stream)

@@ -105,7 +105,9 @@ int launch_serial_line_bank(const float* d_in, long in_stride, int end, int* d_s
 int launch_baudot_bank(const unsigned char* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels, int n, const int* d_lengths,
                        unsigned char* d_mode_io, int* d_count, cudaStream_t st);
 
-// K7/K8/K9 fft.cu
+// K7/K8/K9 fft.cu.  get_twiddles / get_twiddles16: the per-size device tables of the radix-8 and radix-16 passes (cached per process).
+int get_twiddles(int n, const float2** out, cudaStream_t st);
+int get_twiddles16(int n, const float2** out, cudaStream_t st);
 int launch_fft_c2c_batch(const float2* d_in, long in_stride, float2* d_out, long out_stride, int n, int batch, int inverse, cudaStream_t st);
 int launch_olafir_bank(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int fft_size, int input_size,
                        int nblocks, const float2* d_taps_fft, long taps_stride, float2* d_tail_io, int blocks_per_cta, cudaStream_t st);
@@ -126,6 +128,16 @@ int fastddc_inv_plan_set_channel(void* plan, int c, const void* h_chan_one);
 int fastddc_inv_plan_get_state(void* plan, int* h_remain, float* h_phase);
 int fastddc_inv_plan_set_state(void* plan, const int* h_remain, const float* h_phase);
 void fastddc_inv_plan_destroy(void* plan);
+
+// waterfall spectrum bank, spectrum.cu.  SpectrumParams / SpectrumState have the layout of csdrb_spectrum_params_t / csdrb_spectrum_state_t.
+struct SpectrumParams { int fft_size, every, averages, compress; float add_db; };
+struct SpectrumState { long long consumed, frames; };
+long long spectrum_frames_at(int fft_size, int every, long long total);        // frames fft_cc completes on the first `total` samples of a stream
+long spectrum_lines(const void* h_params_v, const void* h_state_v, long n);      // lines a call on n samples completes; < 0 for bad arguments
+size_t spectrum_scratch_bytes(int rows, long n, const void* h_params_v);         // one launch for a whole call; 0 for bad arguments
+int launch_spectrum_bank(const float2* d_in, long in_stride, int rows, long n, const float* d_window, const void* h_params_v, float2* d_hist_io,
+                         float* d_acc_io, void* h_state_io, void* d_out, long out_stride_bytes, void* d_scratch, size_t scratch_bytes, int* launches,
+                         cudaStream_t st);   // SpectrumParams and SpectrumState on the host; returns lines written per row
 
 // fused shared-input DDC bank, ddc_bank.cu
 int ddc_bank_geometry(int decimation, int taps_length);               // 0 when the bank serves (decimation, taps_length); else -2 with the error set

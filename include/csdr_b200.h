@@ -345,6 +345,28 @@ int csdrb_apply_window_rows_c(const complexf *d_in, complexf *d_out, const float
 int csdrb_logpower_cf(const complexf *d_in, float *d_out, long n, float add_db, void *stream);
 int csdrb_accumulate_power_cf(const complexf *d_in, float *d_acc, long n, void *stream);
 int csdrb_log_ff(const float *d_in, float *d_out, long n, float add_db, void *stream);
+/* Waterfall bank: `fft_cc N E W | logaveragepower_cf ADD_DB N A | fft_exchange_sides_ff N [| compress_fft_adpcm_f_u8 N]` (csdr.c:1569-1715,
+ * 1745-1767) on `rows` independent streams in lockstep, any cut of a stream into calls giving the bytes of one call.
+ *   framing : with s counted from stream start, frame k is [(k+1)E - N, (k+1)E) for E <= N and [kE, kE + N) for E > N; samples before the
+ *             stream are 0.  d_window is precalculate_window(N, W) (device, N floats).
+ *   line j  : the bin powers of frames jA .. jA+A-1 summed in frame order from 0.0f, 10*log10 + (float)(add_db - 10*log10(A)), halves swapped;
+ *             with compress = 1 each line is then (N + 10) / 2 bytes of compress_fft_adpcm_f_u8 (fresh encoder per line), else N floats.
+ * The FFT, power, dB and ADPCM arithmetic are those of csdrb_apply_window_rows_c, csdrb_fft_c2c_batch, csdrb_accumulate_power_cf, csdrb_log_ff and
+ * csdrb_compress_fft_adpcm_rows_f_u8, so the bank gives their composition's bytes.  The caller owns the carried state: d_hist_io [rows][N]
+ * complexf (the last N samples so far) and d_acc_io [rows][N] floats (the partial line), both zero at stream start, and *state_io (host,
+ * {0, 0} at stream start), which the call advances.  Row r's input is n samples at d_in + r*in_stride; its line j of the call lands at
+ * (char *)d_out + r*out_stride_bytes + j*line_bytes.  csdrb_spectrum_bank_lines gives the lines a call completes (the same for every row);
+ * csdrb_spectrum_bank_scratch_bytes the scratch for one launch of the whole call.  Less scratch is served in several launches, down to one
+ * frame per row; the bytes do not change.  Returns the lines written per row; -1 for bad arguments (rows < 1, n < 0, every < 1,
+ * averages < 1, a state that does not belong to the parameters, a null or misaligned pointer: input and history 8 bytes, accumulator and
+ * window 4, float output and its stride 4, scratch 16; scratch below one frame per row), -2 for fft_size other than a power of two in 2..16384. */
+typedef struct csdrb_spectrum_params_s { int fft_size, every, averages, compress; float add_db; } csdrb_spectrum_params_t;
+typedef struct csdrb_spectrum_state_s { long long consumed, frames; } csdrb_spectrum_state_t;
+long csdrb_spectrum_bank_lines(const csdrb_spectrum_params_t *p, const csdrb_spectrum_state_t *s, long n);
+size_t csdrb_spectrum_bank_scratch_bytes(int rows, long n, const csdrb_spectrum_params_t *p);
+int csdrb_spectrum_bank_cf(const complexf *d_in, long in_stride, int rows, long n, const float *d_window, const csdrb_spectrum_params_t *p,
+                           complexf *d_hist_io, float *d_acc_io, csdrb_spectrum_state_t *state_io, void *d_out, long out_stride_bytes,
+                           void *d_scratch, size_t scratch_bytes, void *stream);
 /* shift_math_cc bank: d_rates[c] is the plain rate argument; d_phase_io[c] the carried float phase.  The phase chain is sequential over the
  * whole block (one thread per channel walks it), the rotation itself runs fully parallel. */
 size_t csdrb_shift_math_bank_scratch_bytes(int channels, int input_size);
