@@ -79,6 +79,14 @@ class SpectrumState(C.Structure):       # csdrb_spectrum_state_t; {0, 0} at stre
     _fields_ = [("consumed", C.c_longlong), ("frames", C.c_longlong)]
 
 
+class WfmAudioParams(C.Structure):     # csdrb_wfm_audio_params_t
+    _fields_ = [("rate", C.c_float), ("bufsize", C.c_int), ("tau", C.c_float), ("sample_rate", C.c_int)]
+
+
+class WfmAudioState(C.Structure):      # csdrb_wfm_audio_state_t; zeroed at stream start
+    _fields_ = [("where", C.c_float), ("audio", C.c_longlong)]
+
+
 class _SerialLine(C.Structure):         # serial_line_t (= libcsdr.h:278-286)
     _fields_ = [("samples_per_bits", C.c_float), ("databits", C.c_int), ("stopbits", C.c_float), ("output_size", C.c_int),
                 ("input_used", C.c_int), ("bit_sampling_width_ratio", C.c_float)]
@@ -261,6 +269,8 @@ def lib() -> C.CDLL:
     L.csdrb_spectrum_bank_lines.argtypes = [C.POINTER(SpectrumParams), C.POINTER(SpectrumState), lg]; L.csdrb_spectrum_bank_lines.restype = lg
     L.csdrb_spectrum_bank_scratch_bytes.argtypes = [it, lg, C.POINTER(SpectrumParams)]; L.csdrb_spectrum_bank_scratch_bytes.restype = sz
     L.csdrb_spectrum_bank_cf.argtypes = [vp, lg, it, lg, vp, C.POINTER(SpectrumParams), vp, vp, C.POINTER(SpectrumState), vp, lg, vp, sz, vp]
+    L.csdrb_wfm_audio_bank_outputs.argtypes = [C.POINTER(WfmAudioParams), C.POINTER(WfmAudioState), it, C.POINTER(it)]
+    L.csdrb_wfm_audio_bank_f_s16.argtypes = [vp, lg, it, it, C.POINTER(WfmAudioParams), C.POINTER(WfmAudioState), vp, vp, lg, C.POINTER(it), vp]
     _lib = L
     return L
 
@@ -1491,6 +1501,45 @@ class SpectrumBank:
                                                   out.data_ptr() if out.numel() else self.acc.data_ptr(),
                                                   out.stride(0) * out.element_size(), scratch.data_ptr(), scratch_bytes, _stream()), "spectrum_bank_cf")
         assert got == L
+        return out
+
+
+class WfmAudioBank:
+    """The WFM audio tail `fractional_decimator_ff rate 12 | deemphasis_wfm_ff sample_rate tau | convert_f_s16` on `channels` streams at once,
+    in the CLI's calls of `bufsize` samples (csdrb_wfm_audio_bank_f_s16).  Owns the unconsumed rest of every row, the de-emphasis carry and the
+    host state; process(x) takes the next samples of every row ([channels, n] float32 CUDA tensor) and returns the audio they complete as
+    [channels, m] int16."""
+
+    def __init__(self, channels: int, rate: float = 5.0, tau: float = 50e-6, sample_rate: int = 48000, bufsize: int = 1024, device="cuda"):
+        import torch
+        self.channels, self.device = channels, torch.device(device)
+        self.params = WfmAudioParams(rate, bufsize, tau, sample_rate)
+        self.state = WfmAudioState(0.0, 0)
+        self.last = torch.zeros(channels, dtype=torch.float32, device=self.device)
+        self.rest = torch.zeros((channels, 0), dtype=torch.float32, device=self.device)
+        _check(self.outputs(0)[0], "wfm_audio_bank_outputs")               # refuses bad parameters here rather than at the first call
+
+    def outputs(self, n: int):
+        """(s16 samples per row, samples consumed per row) of a call on n samples, from the host state alone"""
+        consumed = C.c_int(0)
+        m = lib().csdrb_wfm_audio_bank_outputs(C.byref(self.params), C.byref(self.state), n, C.byref(consumed))
+        return m, consumed.value
+
+    def process(self, x):
+        import torch
+        if x.dim() != 2 or x.shape[0] != self.channels or x.dtype != torch.float32 or not x.is_cuda:
+            raise ValueError(f"expected a [{self.channels}, n] float32 CUDA tensor")
+        x = torch.cat([self.rest, x], dim=1) if self.rest.shape[1] else x.contiguous()
+        n = x.shape[1]
+        m, _ = self.outputs(n)
+        _check(m, "wfm_audio_bank_outputs")
+        out = torch.empty((self.channels, m), dtype=torch.int16, device=self.device)
+        consumed = C.c_int(0)
+        got = _check(lib().csdrb_wfm_audio_bank_f_s16(x.data_ptr() if n else self.last.data_ptr(), max(n, 1), self.channels, n, C.byref(self.params),
+                                                      C.byref(self.state), self.last.data_ptr(), out.data_ptr() if m else self.last.data_ptr(),
+                                                      max(m, 1), C.byref(consumed), _stream()), "wfm_audio_bank_f_s16")
+        assert got == m
+        self.rest = x[:, consumed.value:].clone()
         return out
 
 

@@ -13,6 +13,9 @@
 #include "common.cuh"
 #include "kernels.h"
 
+#include <cmath>
+#include <new>
+
 namespace csdrb {
 
 // ---------------------------------------------------------------------------------------------- K5
@@ -303,6 +306,185 @@ int launch_deemphasis_wfm_bank(const float* d_in, long in_stride, float* d_out, 
     deemphasis_wfm_bank_kernel<<<(channels + 127) / 128, 128, 0, st>>>(d_in, in_stride, d_out, out_stride, channels, n, alpha, keep, d_last_io);
     CSDRB_CUDA(cudaGetLastError());
     return 1;
+}
+
+// ---------------------------------------------------------------------------------------------- WFM audio tail
+// `fractional_decimator_ff R 12 | deemphasis_wfm_ff SR TAU | convert_f_s16` (README.md:66) per row, as the CLI runs it: the decimator in calls of
+// exactly B samples (csdr.c:1510-1522: memmove of the unconsumed rest, `where -= input_processed` in float), the de-emphasis restarting a NaN carry
+// at every B-th audio sample (libcsdr.c:1092, one call per B samples).  Every row shares the rate, the start and the framing, so the `where` chain,
+// the sample positions and the 12 Lagrange weights of every output are the same for all rows: the host replays the chain (wfm_audio_replay, the
+// reference's own float adds and ceilf) into a position table, and the kernel computes each output's weights once for all the rows of a warp.
+struct WfmParams { float rate; int bufsize; float tau; int sample_rate; };   // layout of csdrb_wfm_audio_params_t
+struct WfmState { float where; long long audio; };                           // layout of csdrb_wfm_audio_state_t; zeroed = stream start
+struct WfmPos { int low; float xw; };                                         // first of the 12 input samples (row-relative), xwhere
+
+constexpr int kWfmPoints = 12;
+constexpr int kWfmXiFirst = 1 - kWfmPoints / 2;                               // -5: the reference starts at where = -xifirst (libcsdr.c:728)
+
+// One warp per 32 rows (the deemphasis_wfm_bank_kernel scheme).  Per tile of 32 outputs: lane j forms the weights of output j once; for each of
+// the warp's rows lane j sums w_i * x[low_j + i] into the padded tile; lane r then walks row r's recursion over the tile; the warp writes s16 rows.
+__global__ void __launch_bounds__(128)
+wfm_audio_bank_kernel(const float* __restrict__ in, long in_stride, short* __restrict__ out, long out_stride, int channels, int m,
+                      const WfmPos* __restrict__ pos, float alpha, float keep, int bufsize, int phase0, float* __restrict__ last_io)
+{
+    __shared__ float tile_all[4][32 * 33];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    float* tile = tile_all[warp];
+    const int c0 = (blockIdx.x * 4 + warp) * 32;
+    if (c0 >= channels) return;
+    const int rows = min(32, channels - c0);
+    const bool live = lane < rows;
+    float y = live ? last_io[c0 + lane] : 0.f;
+    int phase = phase0;                                                // audio index of the tile's first output, mod bufsize
+    for (int t0 = 0; t0 < m; t0 += 32) {
+        const int len = min(32, m - t0);
+        const bool have = lane < len;
+        float w[kWfmPoints];
+        int low = 0;
+        if (have) {
+            const WfmPos p = pos[t0 + lane];
+            low = p.low;
+            float dxj[kWfmPoints];
+#pragma unroll
+            for (int k = 0; k < kWfmPoints; k++) dxj[k] = __fsub_rn(p.xw, (float)(kWfmXiFirst + k));
+#pragma unroll
+            for (int wi = 0; wi < kWfmPoints; wi++) {
+                float coef = 1.f, den = 1.f;
+#pragma unroll
+                for (int wj = 0; wj < kWfmPoints; wj++)
+                    if (wj != wi) { coef = __fmul_rn(coef, dxj[wj]); den = __fmul_rn(den, (float)(wi - wj)); }   // den folds to a constant
+                w[wi] = __fdiv_rn(coef, den);
+            }
+        }
+        for (int r0 = 0; r0 < rows; r0 += 8) {                          // eight rows' points in flight before the first sum
+            float v[8][kWfmPoints];
+#pragma unroll
+            for (int u = 0; u < 8; u++) {
+                const bool ok = have && r0 + u < rows;
+                const float* x = in + (long)(c0 + (ok ? r0 + u : 0)) * in_stride + low;
+#pragma unroll
+                for (int k = 0; k < kWfmPoints; k++) v[u][k] = ok ? x[k] : 0.f;
+            }
+#pragma unroll
+            for (int u = 0; u < 8; u++) {
+                if (have && r0 + u < rows) {
+                    float acc = 0.f;
+#pragma unroll
+                    for (int k = 0; k < kWfmPoints; k++) acc = __fadd_rn(acc, __fmul_rn(w[k], v[u][k]));
+                    tile[(r0 + u) * 33 + lane] = acc;
+                }
+            }
+        }
+        __syncwarp();
+        if (live) {
+            float* row = tile + lane * 33;
+            int q = phase;
+            for (int j = 0; j < len; j++) {
+                if (q == 0 && y != y) y = 0.f;                            // a new deemphasis_wfm_ff call: NaN carry restarts from 0
+                y = __fadd_rn(__fmul_rn(alpha, row[j]), __fmul_rn(keep, y));
+                row[j] = y;
+                if (++q == bufsize) q = 0;
+            }
+        }
+        phase = (phase + len) % bufsize;
+        __syncwarp();
+        for (int r = 0; r < rows; r++) if (have) out[(long)(c0 + r) * out_stride + t0 + lane] = (short)f_to_s16_bits(tile[r * 33 + lane]);
+        __syncwarp();
+    }
+    if (live) last_io[c0 + lane] = y;
+}
+
+// Replays the reference's decimator calls over n samples from *s: returns the outputs and sets *consumed and *where_out; appends each output's
+// position to `table` when given.  -1 for bad parameters or state, -2 for a call the CLI cannot run (it would consume nothing, or more than B).
+int wfm_audio_replay(const void* h_params, const void* h_state, int n, int* consumed, float* where_out, std::vector<WfmPos>* table)
+{
+    const WfmParams* p = static_cast<const WfmParams*>(h_params);
+    const WfmState* s = static_cast<const WfmState*>(h_state);
+    if (!p || !s) { set_error("wfm_audio: null parameters or state"); return -1; }
+    if (n < 0) { set_error("wfm_audio: negative sample count"); return -1; }
+    if (!(p->rate > 1.0f)) { set_error("wfm_audio: rate must be > 1.0 (reference asserts it, libcsdr.c:756)"); return -1; }
+    if (!std::isfinite(p->rate)) { set_error("wfm_audio: rate must be finite"); return -1; }
+    if (!(p->tau > 0.0f)) { set_error("wfm_audio: tau must be positive"); return -1; }
+    if (p->sample_rate <= 0) { set_error("wfm_audio: sample_rate must be positive"); return -1; }
+    const bool start = s->where == 0.0f && s->audio == 0;
+    if (!start && !(s->where >= 5.0f && s->where <= 6.0f && s->audio >= 0)) {
+        set_error("wfm_audio: state {where %g, audio %lld} is neither a stream start nor one a call leaves (where in (5, 6])", (double)s->where, s->audio);
+        return -1;
+    }
+    const int B = p->bufsize;
+    if (B <= kWfmPoints) { set_error("wfm_audio: bufsize %d: a call needs more than %d samples", B, kWfmPoints); return -2; }
+    float where = start ? (float)-kWfmXiFirst : s->where;
+    const float rate = p->rate;
+    int at = 0, m = 0;
+    while (n - at >= B) {                                                 // one fractional_decimator_ff call on [at, at + B)
+        double high;                                                      // ceilf(where) in double: exact, and no int overflow at huge rates
+        for (; (high = (double)ceilf(where)) + kWfmPoints < (double)B; where += rate) {
+            const int h = (int)high;                                      // < B here
+            if (table) table->push_back(WfmPos{at + h - 1, where - (float)(h - 1)});
+            m++;
+        }
+        const double processed = (high - 1) + kWfmXiFirst;
+        if (!(processed >= 1 && processed <= (double)B)) {
+            set_error("wfm_audio: a call at rate %g would consume %.0f of its %d samples, which the CLI cannot run", (double)rate, processed, B);
+            return -2;
+        }
+        where -= (float)processed;
+        at += (int)processed;
+    }
+    *consumed = at;
+    *where_out = at > 0 ? where : s->where;                              // no call: the state stays as it was
+    return m;
+}
+
+int wfm_audio_outputs(const void* h_params, const void* h_state, int n, int* consumed_out)
+{
+    int consumed = 0;
+    float where = 0.f;
+    const int m = wfm_audio_replay(h_params, h_state, n, &consumed, &where, nullptr);
+    if (m >= 0 && consumed_out) *consumed_out = consumed;
+    return m;
+}
+
+int launch_wfm_audio_bank(const float* d_in, long in_stride, int channels, int n, const void* h_params, void* h_state_io, float* d_last_io,
+                          short* d_out, long out_stride, int* consumed_out, int* launches, cudaStream_t st)
+{
+    *launches = 0;
+    if (channels < 1) { set_error("wfm_audio: channels must be at least 1"); return -1; }
+    if (!d_in || !d_last_io || !d_out || !consumed_out) { set_error("wfm_audio: null pointer"); return -1; }
+    if ((reinterpret_cast<uintptr_t>(d_in) & 3) || (reinterpret_cast<uintptr_t>(d_last_io) & 3) || (reinterpret_cast<uintptr_t>(d_out) & 1)) {
+        set_error("wfm_audio: misaligned pointer (input and carry 4 bytes, output 2)"); return -1;
+    }
+    if (in_stride < n) { set_error("wfm_audio: input stride %ld below %d samples", in_stride, n); return -1; }
+    std::vector<WfmPos> table;
+    int consumed = 0;
+    float where = 0.f;
+    int m;
+    try {
+        m = wfm_audio_replay(h_params, h_state_io, n, &consumed, &where, &table);
+    } catch (const std::bad_alloc&) {
+        set_error("wfm_audio: no host memory for the position table of %d samples", n); return -1;
+    }
+    if (m < 0) return m;
+    if (out_stride < m) { set_error("wfm_audio: output stride %ld below %d samples", out_stride, m); return -1; }
+    WfmState* s = static_cast<WfmState*>(h_state_io);
+    const WfmParams* p = static_cast<const WfmParams*>(h_params);
+    if (m > 0) {
+        const float dt = (float)(1.0 / p->sample_rate);                  // as launch_deemphasis_wfm_bank (libcsdr.c:1090-1091)
+        const float alpha = dt / (p->tau + dt);
+        const float keep = 1 - alpha;
+        WfmPos* d_pos = nullptr;                                          // stream-ordered copy of the host table: the call never waits for the device
+        CSDRB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&d_pos), sizeof(WfmPos) * (size_t)m, st));
+        CSDRB_CUDA(cudaMemcpyAsync(d_pos, table.data(), sizeof(WfmPos) * (size_t)m, cudaMemcpyHostToDevice, st));
+        wfm_audio_bank_kernel<<<(channels + 127) / 128, 128, 0, st>>>(d_in, in_stride, d_out, out_stride, channels, m, d_pos, alpha, keep, p->bufsize,
+                                                                      (int)(s->audio % p->bufsize), d_last_io);
+        CSDRB_CUDA(cudaGetLastError());
+        CSDRB_CUDA(cudaFreeAsync(d_pos, st));
+        *launches = 1;
+    }
+    s->where = where;
+    s->audio += m;
+    *consumed_out = consumed;
+    return m;
 }
 
 // deemphasis_nfm_ff (libcsdr.c:1101-1128): a plain "valid" FIR over a real row, out[i] = sum_t taps[t] * in[i+t] for i < n - T

@@ -688,6 +688,20 @@ int csdrb_deemphasis_wfm_bank_ff(const float* d_in, long in_stride, float* d_out
     int rc = launch_deemphasis_wfm_bank(d_in, in_stride, d_out, out_stride, channels, input_size, tau, sample_rate, d_last_io, S(stream));
     return rc < 0 ? rc : counted(0, rc);
 }
+// WFM audio tail (audio.cu): fractional_decimator_ff R 12 | deemphasis_wfm_ff SR TAU | convert_f_s16 per row, in the CLI's B-sample calls
+int csdrb_wfm_audio_bank_outputs(const csdrb_wfm_audio_params_t* params, const csdrb_wfm_audio_state_t* state, int n, int* consumed_out)
+{
+    return wfm_audio_outputs(params, state, n, consumed_out);
+}
+int csdrb_wfm_audio_bank_f_s16(const float* d_in, long in_stride, int channels, int n, const csdrb_wfm_audio_params_t* params,
+                               csdrb_wfm_audio_state_t* state_io, float* d_last_io, short* d_out, long out_stride, int* consumed_out, void* stream)
+{
+    static_assert(sizeof(csdrb_wfm_audio_params_t) == 16 && sizeof(csdrb_wfm_audio_state_t) == 16, "wfm structs mirror audio.cu");
+    if (too_many_channels(channels, "wfm_audio bank")) return -1;
+    int launches = 0;
+    int rc = launch_wfm_audio_bank(d_in, in_stride, channels, n, params, state_io, d_last_io, d_out, out_stride, consumed_out, &launches, S(stream));
+    return rc < 0 ? rc : counted(rc, launches);
+}
 
 int csdrb_fir_valid_bank_ff(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int input_size, const float* taps,
                             int taps_length, float limit_max, void* stream)

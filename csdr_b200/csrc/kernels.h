@@ -25,6 +25,11 @@ int launch_compress_fft_adpcm_rows(const float* d_in, long in_stride, unsigned c
 int launch_limit_ff(const float* d_in, float* d_out, long n, float max_amplitude, cudaStream_t st);
 int launch_deemphasis_wfm_bank(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int n, float tau, int sample_rate,
                                float* d_last_io, cudaStream_t st);
+// WFM audio tail `fractional_decimator_ff R 12 | deemphasis_wfm_ff SR TAU | convert_f_s16`, audio.cu.  Parameters and state are the host
+// csdrb_wfm_audio_params_t / csdrb_wfm_audio_state_t; both return the s16 samples per row (< 0 refused).
+int wfm_audio_outputs(const void* h_params, const void* h_state, int n, int* consumed_out);
+int launch_wfm_audio_bank(const float* d_in, long in_stride, int channels, int n, const void* h_params, void* h_state_io, float* d_last_io,
+                          short* d_out, long out_stride, int* consumed_out, int* launches, cudaStream_t st);
 
 // deemphasis_nfm_ff: the tap tables live in host/firdes.c (public accessor, see include/csdr_b200.h)
 constexpr int kNfmMaxTaps = 208;

@@ -1,5 +1,5 @@
 /*
- * bankd.c -- csdr-bankd: a whole bank of FM, AM, SSB, BPSK31 or RTTY receivers on ONE wideband IQ stream, in one process.
+ * bankd.c -- csdr-bankd: a whole bank of NFM, WFM, AM, SSB, BPSK31 or RTTY receivers on ONE wideband IQ stream, in one process.
  *
  * SURVEY.md 8(f) rank 2.  What the reference does with processes -- `nmux` fanning the IQ stream out over TCP (nmux.cpp:246-353)
  * to one `csdr shift_addition_cc | csdr fir_decimate_cc | csdr fmdemod_quadri_cf | ...` chain per listener (ddcd_old.h:51-57,
@@ -13,7 +13,8 @@
  * first -- is process plumbing and is not reproduced; tests/test_gpu_zzz_bankd.py compares against the oracle run over the whole stream).
  *
  * usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]
- *                   [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B] [--resample I:D[:BW]]
+ *                   [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty|wfm] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B] [--resample I:D[:BW]]
+ *                   [--wfm-rate R] [--tau T]
  *                   [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]
  *                   [--waterfall SINK [--fft-size N] [--fft-every E] [--fft-averages A] [--fft-add-db X] [--fft-window W] [--fft-compression adpcm|none]]
  *                   RATE:SINK [RATE:SINK ...]
@@ -32,6 +33,14 @@
  *   at 2.4 Msps: --decimation 1200 --bw 0.001 gives 2 kHz baseband (4001 taps, M = 4 per output period, D*MP = 4800 <= 8000: the fused bank
  *   serves it), and --sps 44 is 45.45 Bd:
  *     rtl_sdr -s 2400000 -f 14080000 - | csdr-bankd --decimation 1200 --bw 0.001 --tail rtty --sps 44 -0.1:ch1.txt 0.05:ch2.txt 0.2:ch3.txt
+ *   wfm: broadcast FM, the README.md:66 graph's fractional_decimator_ff R | deemphasis_wfm_ff 48000 T | convert_f_s16 behind the discriminator (the bank
+ *   runs with fmdemod), s16 audio per channel.  --wfm-rate R (default 5, above 1 and at most 16) brings wideband / D to 48 kHz, the de-emphasis rate;
+ *   --tau T (default 50e-6; 75e-6 in the Americas).  Both run in the CLI's calls of 1024 samples (csdrb_wfm_audio_bank_f_s16), so every channel
+ *   gets the bytes of that CLI pipe on the daemon's discriminator output.  No --resample: the fractional decimator is the rate converter.
+ *   Three stations of a 2.4 Msps capture (240 kHz channels, 79 taps = 8 per output period, which the fused bank serves):
+ *     rtl_sdr -s 2400000 -f 89300000 - | csdr-bankd --decimation 10 --bw 0.05 --tail wfm -0.085:a.s16 0.0:b.s16 0.2:c.s16
+ *   and the whole 88-108 MHz band from a 20 Msps receiver, about 100 stations (250 kHz channels, 999 taps = 13 per output period):
+ *     ... | csdr-bankd --decimation 80 --bw 0.004 --tail wfm --wfm-rate 5.2083333 -0.45:s1.s16 -0.44:s2.s16 ...
  *   --decimation: any even D (default 50) whose filter the fused bank serves: M = ceil(taps / D) <= 24 and D * M (rounded up to the kernel's
  *   bucket) <= 8000 taps, see csdrb_ddc_bank in include/csdr_b200.h.  The NFM tail's deemphasis_nfm_ff stays at 48000 whatever D gives: where
  *   wideband rate / D is not 48 kHz, --resample I:D[:BW] puts rational_resampler_ff I D BW right behind the discriminator (tails nfm and none; see
@@ -39,7 +48,7 @@
  *   RATE  shift_addition_cc rate (fraction of the wideband sample rate), SINK a path (file or FIFO) or tcp:PORT (one listener).
  *   --devices: the channels are sliced over several GPUs of this node (csdrb_multi_bank_*: the block goes to the first device once and on to
  *   the others by NCCL broadcast), one block of latency more (two blocks are kept in flight); the audio tail (nfm, am, usb, lsb), audio-rate work, runs on
- *   the first device for all channels, through the same kernels as without --devices; so do the bpsk31 and rtty decoders.
+ *   the first device for all channels, through the same kernels as without --devices; so do the bpsk31 and rtty decoders and the wfm tail.
  *   --waterfall SINK: the receiver server's other consumer of the wideband stream, OpenWebRX's waterfall
  *     fft_cc N E W | logaveragepower_cf X N A | fft_exchange_sides_ff N [| compress_fft_adpcm_f_u8 N]
  *   on every input sample (csdrb_spectrum_bank_cf on the block's cf32 samples, already on the device: no extra transfer; with --devices on the
@@ -314,7 +323,7 @@ static void raw_emit(const float *d_rows, long pitch, int n, unsigned char *h_ou
  *   mid  : [C][bs] float (am: DC-blocked envelope) or complexf (usb/lsb: filtered baseband) over the whole units
  *   pcm  : [C][whole] s16 */
 #define SSB_BW 0.05f                                      /* bandpass_fir_fft_cc transition bandwidth of README.md:110 */
-enum { TAIL_NFM, TAIL_NONE, TAIL_IQ, TAIL_AM, TAIL_USB, TAIL_LSB, TAIL_BPSK31, TAIL_RTTY };
+enum { TAIL_NFM, TAIL_NONE, TAIL_IQ, TAIL_AM, TAIL_USB, TAIL_LSB, TAIL_BPSK31, TAIL_RTTY, TAIL_WFM };
 
 /* ---- the BPSK31 tail: simple_agc_cc 0.001 R | timing_recovery_cc GARDNER N 0.5 2 --add_q | dbpsk_decoder_c_u8 | psk31_varicode_decoder_u8_u8 --------
  * Channels consume different amounts of baseband, so the timing recovery bank gets a start offset per channel.  Device buffers of ONE device:
@@ -475,6 +484,60 @@ static void rtty_tail_push(rtty_tail_t *t, channel_t *chan, int n, void *stream)
         OK(csdrb_copy_h2d(t->d_start, t->h_start, sizeof(int) * (size_t)C, stream));
         OK(csdrb_stream_synchronize(stream));
     }
+}
+
+/* ---- the WFM tail: fractional_decimator_ff R | deemphasis_wfm_ff 48000 TAU | convert_f_s16 behind the discriminator (README.md:66) --------------
+ * The bank runs the decimator in the CLI's calls of WFM_BUFSIZE samples and consumes the same samples of every row.  Device buffers of ONE device:
+ *   rows : [C][rs] float : [the unconsumed rest (< WFM_BUFSIZE) | new discriminator samples]
+ *   pcm  : [C][cap] s16
+ * Carried: the rest of every row, the host state {where, audio} and the de-emphasis carry of every channel. */
+#define WFM_BUFSIZE 1024                                 /* the CLI's the_bufsize: the decimator's call size and the de-emphasis NaN-reset period */
+
+typedef struct {
+    int C, have, cap;
+    long rs;
+    csdrb_wfm_audio_params_t p;
+    csdrb_wfm_audio_state_t s;
+    float *d_rows, *d_carry, *d_last;
+    short *d_pcm;
+    unsigned char *h_pcm;
+} wfm_tail_t;
+
+static void wfm_tail_init(wfm_tail_t *t, int C, float rate, float tau, int in_cap)
+{
+    memset(t, 0, sizeof *t);
+    const csdrb_wfm_audio_params_t p = {rate, WFM_BUFSIZE, tau, NFM_RATE};
+    t->C = C; t->p = p;
+    t->rs = ((long)WFM_BUFSIZE + in_cap + 3) & ~3L;
+    t->cap = (int)((double)t->rs / rate) + 2;                         /* every output advances the position by rate (> 1) */
+    t->d_rows = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)t->rs);
+    t->d_carry = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)WFM_BUFSIZE);
+    t->d_last = csdrb_device_alloc(sizeof(float) * (size_t)C);           /* zero-filled: the de-emphasis starts from 0 */
+    t->d_pcm = csdrb_device_alloc(sizeof(short) * (size_t)C * (size_t)t->cap);
+    t->h_pcm = csdrb_host_alloc(sizeof(short) * (size_t)C * (size_t)t->cap);
+    if (!t->d_rows || !t->d_carry || !t->d_last || !t->d_pcm || !t->h_pcm) die("out of memory");
+}
+
+/* n new discriminator samples per channel sit at d_rows + have: the audio of the whole decimator calls to the sinks, the rest to the front */
+static void wfm_tail_push(wfm_tail_t *t, channel_t *chan, int n, void *stream)
+{
+    const int C = t->C, total = t->have + n;
+    int consumed = 0;
+    const int m = csdrb_wfm_audio_bank_outputs(&t->p, &t->s, total, &consumed);
+    if (m < 0) die("csdrb_wfm_audio_bank_outputs failed");
+    if (m > t->cap) die("wfm tail: more audio than the buffer holds");
+    if (csdrb_wfm_audio_bank_f_s16(t->d_rows, t->rs, C, total, &t->p, &t->s, t->d_last, t->d_pcm, t->cap, &consumed, stream) != m)
+        die("csdrb_wfm_audio_bank_f_s16 failed");
+    const int rest = total - consumed;
+    if (rest > 0 && consumed > 0) {
+        const size_t row = sizeof(float) * (size_t)t->rs;
+        OK(csdrb_copy2d_d2d(t->d_carry, sizeof(float) * WFM_BUFSIZE, t->d_rows + consumed, row, sizeof(float) * (size_t)rest, (size_t)C, stream));
+        OK(csdrb_copy2d_d2d(t->d_rows, row, t->d_carry, sizeof(float) * WFM_BUFSIZE, sizeof(float) * (size_t)rest, (size_t)C, stream));
+    }
+    t->have = rest;
+    if (m > 0) OK(csdrb_copy2d_d2h(t->h_pcm, sizeof(short) * (size_t)m, t->d_pcm, sizeof(short) * (size_t)t->cap, sizeof(short) * (size_t)m, (size_t)C, stream));
+    OK(csdrb_stream_synchronize(stream));
+    if (m > 0) for (int c = 0; c < C; c++) write_sink(&chan[c], t->h_pcm + sizeof(short) * (size_t)c * (size_t)m, sizeof(short) * (size_t)m);
 }
 
 /* ---- --waterfall SINK: fft_cc N E W | logaveragepower_cf X N A | fft_exchange_sides_ff N [| compress_fft_adpcm_f_u8 N] on the wideband stream ---
@@ -671,9 +734,9 @@ static void bb_tail_push(bb_tail_t *t, channel_t *chan, int n_new, void *stream)
 
 static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *chan, int C, const float *rates, int D, const float *taps, int T, int block,
                      int kind, float limit, float agc_ref, int rs_I, int rs_D, float rs_bw, int sps, const csdrb_serial_line_params_t *rtty_p, int rtty_B,
-                     waterfall_t *wf, const waterfall_opts_t *wo)
+                     float wfm_rate, float tau, waterfall_t *wf, const waterfall_opts_t *wo)
 {
-    const int nfm = kind == TAIL_NFM, rtty = kind == TAIL_RTTY, demod = nfm || rtty || kind == TAIL_NONE;
+    const int nfm = kind == TAIL_NFM, rtty = kind == TAIL_RTTY, wfm = kind == TAIL_WFM, demod = nfm || rtty || wfm || kind == TAIL_NONE;
     const size_t osz = demod ? sizeof(float) : sizeof(complexf);
     csdrb_multi_bank_t *mb = csdrb_multi_bank_create(ndev, dev, C, rates, D, taps, T, demod, 1024, block);
     if (!mb) die("cannot create the multi-GPU bank");
@@ -686,7 +749,7 @@ static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *cha
     if (!h_wide[0] || !h_wide[1] || !h_out[0] || !h_out[1] || !raw) die("out of memory");
     /* --tail nfm: the audio tail is audio-rate work (C x 48 kHz): the discriminator rows every device returned go to the FIRST device once more and through
      * the same kernels as in the single-GPU path */
-    nfm_tail_t tail_state; bb_tail_t bb; rs_stage_t rsm; rtty_tail_t rt; void *tail_stream = NULL;
+    nfm_tail_t tail_state; bb_tail_t bb; rs_stage_t rsm; rtty_tail_t rt; wfm_tail_t wt; void *tail_stream = NULL;
     float *d_raw_out = NULL; unsigned char *h_raw_out = NULL;
     const int resample = rs_I > 0;
     if (kind != TAIL_NONE || resample) {
@@ -697,6 +760,7 @@ static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *cha
         const int tail_cap = resample ? rs_out_cap(&rsm) : n_out + 2;
         if (nfm) nfm_tail_init(&tail_state, C, tail_cap, limit, agc_ref);
         else if (rtty) rtty_tail_init(&rt, C, rtty_p, rtty_B, tail_cap);
+        else if (wfm) wfm_tail_init(&wt, C, wfm_rate, tau, tail_cap);
         else if (!demod) bb_tail_init(&bb, kind, C, tail_cap, limit, agc_ref, sps, tail_stream);
         else {
             d_raw_out = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)tail_cap);
@@ -727,6 +791,10 @@ static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *cha
             OK(csdrb_copy2d_h2d(rt.d_rows + rt.end, sizeof(float) * (size_t)rt.rs, h_out[slot_], sizeof(float) * (size_t)n_out, \
                                 sizeof(float) * (size_t)n_out, (size_t)C, tail_stream)); \
             rtty_tail_push(&rt, chan, n_out, tail_stream); \
+        } else if (wfm) { \
+            OK(csdrb_copy2d_h2d(wt.d_rows + wt.have, sizeof(float) * (size_t)wt.rs, h_out[slot_], sizeof(float) * (size_t)n_out, \
+                                sizeof(float) * (size_t)n_out, (size_t)C, tail_stream)); \
+            wfm_tail_push(&wt, chan, n_out, tail_stream); \
         } else if (!demod) { \
             OK(csdrb_copy2d_h2d(bb.d_bb + bb.have, sizeof(complexf) * (size_t)bb.bs, h_out[slot_], sizeof(complexf) * (size_t)n_out, \
                                 sizeof(complexf) * (size_t)n_out, (size_t)C, tail_stream)); \
@@ -777,8 +845,16 @@ static int usage(void)
 {
     fprintf(stderr,
             "usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]\n"
-            "                  [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B]\n"
-            "                  [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...] RATE:SINK [RATE:SINK ...]\n"
+            "                  [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty|wfm] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B]\n"
+            "                  [--wfm-rate R] [--tau T] [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]\n"
+            "                  RATE:SINK [RATE:SINK ...]\n"
+            "  --tail wfm           broadcast FM: per channel fmdemod_quadri_cf | fractional_decimator_ff R | deemphasis_wfm_ff 48000 T | convert_f_s16,\n"
+            "                       in the CLI's calls of 1024 samples; the sinks get s16 audio.  --wfm-rate R (default 5, above 1 and at most 16)\n"
+            "                       takes wideband/decimation to 48 kHz; --tau T (default 50e-6; 75e-6 in the Americas).  Not with --resample.\n"
+            "                       Three stations at 2.4 Msps (240 kHz channels, 79 taps = 8 per output period, which the fused bank serves):\n"
+            "                       rtl_sdr -s 2400000 -f 89300000 - | csdr-bankd --decimation 10 --bw 0.05 --tail wfm -0.085:a.s16 0.0:b.s16 0.2:c.s16\n"
+            "                       The whole 88-108 MHz band at 20 Msps, about 100 stations (250 kHz channels, 999 taps = 13 per output period):\n"
+            "                       ... | csdr-bankd --decimation 80 --bw 0.004 --tail wfm --wfm-rate 5.2083333 -0.45:s1.s16 -0.44:s2.s16 ...\n"
             "  --tail bpsk31 --sps N  per channel simple_agc_cc 0.001 R | timing_recovery_cc GARDNER N 0.5 2 --add_q | dbpsk_decoder_c_u8 |\n"
             "                       psk31_varicode_decoder_u8_u8 (R = --agc-ref, default 0.5) behind the baseband; the sinks get the decoded text.\n"
             "                       N is samples per symbol at the baseband rate, > 4 and divisible by 4.  A PSK31 skimmer at 2.4 Msps:\n"
@@ -820,6 +896,8 @@ int main(int argc, char **argv)
     const char *wf_sink = NULL;                                      /* --waterfall SINK */
     waterfall_opts_t wo = {2048, 0, 1, 1, -70.0f, WINDOW_DEFAULT};   /* --fft-every 0 stands for N */
     int wf_opts = 0;
+    float wfm_rate = 5.0f, tau = 50e-6f;                             /* --wfm-rate, --tau: the README.md:66 graph (75e-6 in the Americas) */
+    int wfm_opts = 0;
     channel_t *chan = calloc((size_t)argc, sizeof *chan);
     int C = 0;
     for (int a = 1; a < argc; a++) {
@@ -839,6 +917,8 @@ int main(int argc, char **argv)
         else if (!strcmp(o, "--databits") && v) { databits = atoi(v); rtty_opts = 1; a++; }
         else if (!strcmp(o, "--stopbits") && v) { stopbits = (float)atof(v); rtty_opts = 1; a++; }
         else if (!strcmp(o, "--rtty-bufsize") && v) { rtty_B = atoi(v); rtty_opts = 1; a++; }
+        else if (!strcmp(o, "--wfm-rate") && v) { wfm_rate = (float)atof(v); wfm_opts = 1; a++; }
+        else if (!strcmp(o, "--tau") && v) { tau = (float)atof(v); wfm_opts = 1; a++; }
         else if (!strcmp(o, "--waterfall") && v) { wf_sink = v; a++; }
         else if (!strcmp(o, "--fft-size") && v) { wo.fft_size = atoi(v); wf_opts = 1; a++; }
         else if (!strcmp(o, "--fft-every") && v) { wo.every = atoi(v); wf_opts = 1; if (wo.every < 1) die("--fft-every must be at least 1"); a++; }
@@ -870,10 +950,10 @@ int main(int argc, char **argv)
             chan[C].sink = end + 1; chan[C].fd = -1; chan[C].dropped = 0; C++;
         } else { fprintf(stderr, "csdr-bankd: unknown argument %s\n", o); return 2; }
     }
-    static const char *kTails[] = {"nfm", "none", "iq", "am", "usb", "lsb", "bpsk31", "rtty"};
+    static const char *kTails[] = {"nfm", "none", "iq", "am", "usb", "lsb", "bpsk31", "rtty", "wfm"};
     int kind = -1;
-    for (int k = 0; k < 8; k++) if (!strcmp(tail, kTails[k])) kind = k;
-    if (kind < 0) die("--tail is nfm, none, iq, am, usb, lsb, bpsk31 or rtty");
+    for (int k = 0; k < 9; k++) if (!strcmp(tail, kTails[k])) kind = k;
+    if (kind < 0) die("--tail is nfm, none, iq, am, usb, lsb, bpsk31, rtty or wfm");
     const csdrb_serial_line_params_t rtty_p = {spb, databits, stopbits, 0.4f};   /* serial_line_decoder_f_u8's bit_sampling_width_ratio (csdr.c:2510) */
     if (kind == TAIL_BPSK31) {
         if (sps <= 4 || (sps & 3)) die("--tail bpsk31 needs --sps N with N > 4 and divisible by 4 (timing_recovery_cc's decimation)");
@@ -889,7 +969,12 @@ int main(int argc, char **argv)
             die("--rtty-bufsize must exceed sps*(1 + databits + stopbits) + 2: a call could not hold one character and would get stuck");
     } else if (sps) die("--sps belongs to --tail bpsk31 and --tail rtty");
     if (kind != TAIL_RTTY && rtty_opts) die("--databits, --stopbits and --rtty-bufsize belong to --tail rtty");
-    const int nfm = kind == TAIL_NFM, rtty = kind == TAIL_RTTY, demod = nfm || rtty || kind == TAIL_NONE;
+    if (kind == TAIL_WFM) {
+        /* above 16 a decimator call could consume more than its 1024 samples (the reference then memmoves a negative length): WFM needs about 5 */
+        if (!(wfm_rate > 1.0f && wfm_rate <= 16.0f)) die("--wfm-rate must be above 1 and at most 16 (wideband rate / decimation / 48 kHz)");
+        if (!(tau > 0.0f)) die("--tau must be positive (50e-6 in Europe, 75e-6 in the Americas)");
+    } else if (wfm_opts) die("--wfm-rate and --tau belong to --tail wfm");
+    const int nfm = kind == TAIL_NFM, rtty = kind == TAIL_RTTY, wfm = kind == TAIL_WFM, demod = nfm || rtty || wfm || kind == TAIL_NONE;
     if (nfm && agc_ref == 0.0f) agc_ref = 1.0f;                      /* fastagc_ff's default reference (csdr.c:1388) */
     if (C == 0) die("no channels (RATE:SINK ...)");
     if (block <= 0 || (block & 1)) die("--block must be a positive even number of samples");
@@ -898,7 +983,7 @@ int main(int argc, char **argv)
     if (!(limit > 0.f) || !(agc_ref >= 0.f)) die("--limit and --agc-ref must be positive");
     const int resample = rs_I > 0;
     if (resample) {
-        if (!demod || rtty) die("--resample works with --tail nfm and --tail none only (the am, usb, lsb, iq, bpsk31 and rtty tails are not resampled)");
+        if (!demod || rtty || wfm) die("--resample works with --tail nfm and --tail none only (the am, usb, lsb, iq, bpsk31, rtty and wfm tails are not resampled)");
         if (!(rs_bw > 0.f && rs_bw < 0.5f)) die("--resample: the transition bandwidth must be between 0 and 0.5");
         const int rs_T = firdes_filter_len(rs_bw);
         if (!resample_geometry_ok(rs_I, rs_D, rs_T)) {
@@ -934,7 +1019,7 @@ int main(int argc, char **argv)
         const int fd = open_input(in_spec);
         fprintf(stderr, "csdr-bankd: %d channels over %d devices, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, ndev, D, T, u8 ? "u8" : "f32", block, tail);
         const int rc = run_multi(fd, u8, devs, ndev, chan, C, rates, D, taps, T, block, kind, limit, agc_ref, rs_I, rs_D, rs_bw, sps, &rtty_p, rtty_B,
-                                 wf_sink ? &wf : NULL, &wo);
+                                 wfm_rate, tau, wf_sink ? &wf : NULL, &wo);
         for (int c = 0; c < C; c++) { if (chan[c].dropped) fprintf(stderr, "csdr-bankd: sink %s lost %ld bytes (too slow)\n", chan[c].sink, chan[c].dropped); if (chan[c].fd >= 0) close(chan[c].fd); }
         if (wf_sink) waterfall_report(&wf);
         return rc;
@@ -958,6 +1043,7 @@ int main(int argc, char **argv)
     bb_tail_t bb;
     rs_stage_t rsm;
     rtty_tail_t rt;
+    wfm_tail_t wt;
     if (resample) rs_init(&rsm, C, rs_I, rs_D, rs_bw, out_cap);
     const int tail_cap = resample ? rs_out_cap(&rsm) : out_cap;   /* samples one block can add behind the discriminator (and resampler) */
     long ds = ((long)tail_cap + 3) & ~3L;
@@ -965,6 +1051,7 @@ int main(int argc, char **argv)
     unsigned char *h_out = NULL;
     if (nfm) { nfm_tail_init(&tl, C, tail_cap, limit, agc_ref); ds = tl.ds; d_demod = tl.d_demod; }
     else if (rtty) { rtty_tail_init(&rt, C, &rtty_p, rtty_B, out_cap); ds = rt.rs; d_demod = rt.d_rows; }
+    else if (wfm) { wfm_tail_init(&wt, C, wfm_rate, tau, out_cap); ds = wt.rs; d_demod = wt.d_rows; }
     else if (!demod) { bb_tail_init(&bb, kind, C, out_cap, limit, agc_ref, sps, stream); ds = bb.bs; d_demod = (float *)bb.d_bb; }
     else {
         d_demod = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)ds);
@@ -1001,7 +1088,7 @@ int main(int argc, char **argv)
 
         /* 2. shift | fir_decimate | fmdemod for every channel, new discriminator samples behind the de-emphasis FIR's carried inputs */
         void *dst = resample ? (void *)(rsm.d_in + rsm.have) : nfm ? (void *)(d_demod + tl.a_have) : rtty ? (void *)(rt.d_rows + rt.end)
-                  : !demod ? (void *)(bb.d_bb + bb.have) : (void *)d_demod;
+                  : wfm ? (void *)(wt.d_rows + wt.have) : !demod ? (void *)(bb.d_bb + bb.have) : (void *)d_demod;
         const int n_out = csdrb_ddc_bank_process(bank, d_wide[cur], n_in, dst, resample ? rsm.rs : ds, stream);
         if (n_out < 0) die("csdrb_ddc_bank_process failed");
         const int consumed = n_out * D;
@@ -1013,6 +1100,7 @@ int main(int argc, char **argv)
         const int n_tail = resample ? rs_push(&rsm, n_out, nfm ? d_demod + tl.a_have : d_demod, ds, stream) : n_out;
         if (!demod) bb_tail_push(&bb, chan, n_out, stream);         /* baseband tails: am / usb / lsb audio, or the raw baseband */
         else if (rtty) rtty_tail_push(&rt, chan, n_out, stream);    /* serial_line_decoder_f_u8 | rtty_baudot2ascii_u8_u8, text to the sinks */
+        else if (wfm) wfm_tail_push(&wt, chan, n_out, stream);      /* fractional_decimator_ff | deemphasis_wfm_ff | convert_f_s16, audio to the sinks */
         else if (!nfm) raw_emit(d_demod, ds, n_tail, h_out, chan, C, stream);   /* raw discriminator output, float */
         else nfm_tail_push(&tl, chan, n_tail, stream);             /* 3./4. limit | de-emphasis | AGC | s16, audio to the sinks */
         blocks++;

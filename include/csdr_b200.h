@@ -321,6 +321,25 @@ int  csdrb_multi_bank_process_host(csdrb_multi_bank_t *bank, const complexf *h_w
 int csdrb_limit_ff(const float *d_in, float *d_out, long n, float max_amplitude, void *stream);
 int csdrb_deemphasis_wfm_bank_ff(const float *d_in, long in_stride, float *d_out, long out_stride, int channels, int input_size,
                                  float tau, int sample_rate, float *d_last_io, void *stream);
+/* WFM audio tail: `fractional_decimator_ff rate 12 | deemphasis_wfm_ff sample_rate tau | convert_f_s16` (README.md:66) per row, run the way the CLI
+ * runs it with buffer size B = bufsize:
+ *   - the decimator runs calls on exactly B samples from the row's start while B samples remain; each call is the reference loop (12 points,
+ *     no prefilter), `where` carried and reduced by input_processed after each call (csdr.c:1510-1522, libcsdr.c:751-793);
+ *   - the de-emphasis carry is kept, and a NaN carry restarts from 0 where the audio sample index, counted from stream start, is a multiple of B
+ *     (libcsdr.c:1092; Inf is kept); alpha and 1 - alpha as csdrb_deemphasis_wfm_bank_ff computes them;
+ *   - s16 as csdrb_convert_f_s16.
+ * All rows run in lockstep.  Carried state: *state_io on the host (zeroed at stream start; the call advances it) and d_last_io[c] on the device
+ * (0 at stream start).  A call reads n samples of each row at d_in + c*in_stride and consumes the same *consumed_out samples of every row; the
+ * caller presents the unconsumed rest (fewer than B) again at the start of each row next time.  Row c's audio goes to d_out + c*out_stride.
+ * Returns the s16 samples written per row; csdrb_wfm_audio_bank_outputs gives that count and the consumed samples on the host alone.
+ * -1 for bad arguments (channels < 1, n < 0, rate <= 1 or not finite, tau <= 0, sample_rate <= 0, strides below n or the output count, a null or misaligned
+ * pointer, a state that is not a stream start and has `where` outside [5, 6]), -2 for a call the CLI cannot run: bufsize <= 12, or a call that
+ * would consume no sample or more than bufsize samples (the reference would memmove a negative length); the state is then unchanged. */
+typedef struct csdrb_wfm_audio_params_s { float rate; int bufsize; float tau; int sample_rate; } csdrb_wfm_audio_params_t;
+typedef struct csdrb_wfm_audio_state_s { float where; long long audio; } csdrb_wfm_audio_state_t;
+int csdrb_wfm_audio_bank_outputs(const csdrb_wfm_audio_params_t *params, const csdrb_wfm_audio_state_t *state, int n, int *consumed_out);
+int csdrb_wfm_audio_bank_f_s16(const float *d_in, long in_stride, int channels, int n, const csdrb_wfm_audio_params_t *params,
+                               csdrb_wfm_audio_state_t *state_io, float *d_last_io, short *d_out, long out_stride, int *consumed_out, void *stream);
 
 /* NFM de-emphasis bank: every row through the fixed FIR of `sample_rate`; returns outputs per row (input_size - taps_length),
  * 0 when the rate has no table.  limit_max > 0 fuses the preceding `limit_ff limit_max` of the NFM graph (README.md:87) into the load.
