@@ -167,6 +167,7 @@ def lib() -> C.CDLL:
     L.agc_ff.argtypes = [vp, vp, it, C.c_float, C.c_float, C.c_float, C.c_float, C.c_short, C.c_short, C.c_float, C.c_float]
     L.agc_ff.restype = C.c_float
     L.csdrb_fft_c2c_batch.argtypes = [vp, lg, vp, lg, it, it, it, vp]
+    L.csdrb_fft_c2c_large_batch.argtypes = [vp, lg, vp, lg, it, it, it, vp]
     L.csdrb_bandpass_fir_fft_bank_cc.argtypes = [vp, lg, vp, lg, it, it, it, it, vp, lg, vp, vp]
     L.csdrb_ddc_bank_scratch_bytes.argtypes = [it, it, it, it]; L.csdrb_ddc_bank_scratch_bytes.restype = sz
     L.csdrb_ddc_bank.argtypes = [vp, it, it, vp, vp, it, it, it, C.POINTER(C.c_float), it, it, vp, lg, vp, vp, vp, sz, vp]
@@ -1119,11 +1120,13 @@ def rtty_baudot2ascii_bank_u8_u8(codes, lengths=None, fig_mode=None):
 
 
 def fft_c2c(x, inverse: bool = False):
-    """Batched unnormalised DFT along the last axis of a [B, N] (or [N]) complex64 CUDA tensor."""
+    """Batched unnormalised DFT along the last axis of a [B, N] (or [N]) complex64 CUDA tensor; N a power of two from 2 to 2^20
+    (csdrb_fft_c2c_batch up to 16384 points, csdrb_fft_c2c_large_batch above)."""
     import torch
     xr, ptr, stride, b, n = _as_cf32_rows(x)
     out = torch.empty((b, n), dtype=torch.complex64, device=xr.device)
-    _check(lib().csdrb_fft_c2c_batch(ptr, stride, out.data_ptr(), out.stride(0), n, b, 1 if inverse else 0, _stream()), "fft_c2c")
+    call = lib().csdrb_fft_c2c_batch if n <= 16384 else lib().csdrb_fft_c2c_large_batch
+    _check(call(ptr, stride, out.data_ptr(), out.stride(0), n, b, 1 if inverse else 0, _stream()), "fft_c2c")
     return out if x.dim() > 1 or x.dtype != torch.complex64 else out[0]
 
 

@@ -471,6 +471,13 @@ int csdrb_fft_c2c_batch(const complexf* d_in, long in_stride, complexf* d_out, l
     return rc < 0 ? rc : counted(0, rc);
 }
 
+int csdrb_fft_c2c_large_batch(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int size, int batch, int inverse, void* stream)
+{
+    if (!d_in || !d_out) { set_error("fft (large): null pointer"); return -1; }
+    int rc = launch_fft_c2c_large_batch(reinterpret_cast<const float2*>(d_in), in_stride, reinterpret_cast<float2*>(d_out), out_stride, size, batch, inverse, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
 int csdrb_bandpass_fir_fft_bank_cc(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int fft_size, int input_size,
                                    int nblocks, const complexf* d_taps_fft, long taps_stride, complexf* d_tail_io, void* stream)
 {

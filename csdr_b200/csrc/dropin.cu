@@ -472,8 +472,8 @@ int deemphasis_nfm_ff(float* input, float* output, int input_size, int sample_ra
 FFT_PLAN_T* make_fft_c2c(int size, complexf* input, complexf* output, int forward, int benchmark)
 {
     (void)benchmark;
-    if (size < 2 || size > 16384 || (size & (size - 1))) {
-        fprintf(stderr, "libcsdr_b200: make_fft_c2c: size %d unsupported (power of two, 2..16384)\n", size);
+    if (size < 2 || size > kFftLargeMaxN || (size & (size - 1))) {
+        fprintf(stderr, "libcsdr_b200: make_fft_c2c: size %d unsupported (power of two, 2..%d)\n", size, kFftLargeMaxN);
         return nullptr;
     }
     FFT_PLAN_T* p = (FFT_PLAN_T*)malloc(sizeof(FFT_PLAN_T));
@@ -492,7 +492,9 @@ void fft_execute(FFT_PLAN_T* plan)
     }
     const int inverse = ((csdrb_plan_impl*)plan->plan)->forward ? 0 : 1;
     elementwise(who, static_cast<const complexf*>(plan->input), static_cast<complexf*>(plan->output), plan->size,
-                [=](const complexf* in, complexf* out, long n, void* s) { return csdrb_fft_c2c_batch(in, n, out, n, (int)n, 1, inverse, s); });
+                [=](const complexf* in, complexf* out, long n, void* s) {
+                    return n < kFftLargeMinN ? csdrb_fft_c2c_batch(in, n, out, n, (int)n, 1, inverse, s) : csdrb_fft_c2c_large_batch(in, n, out, n, (int)n, 1, inverse, s);
+                });
 }
 
 void fft_destroy(FFT_PLAN_T* plan) { if (plan) { free(plan->plan); free(plan); } }
@@ -501,16 +503,18 @@ void csdrb_fft_free(void* p) { free(p); }
 
 void apply_fir_fft_cc(FFT_PLAN_T* plan, FFT_PLAN_T* plan_inverse, complexf* taps_fft, complexf* last_overlap, int overlap_size)
 {
-    // libcsdr.c:814-849 in one fused kernel: the intermediate spectrum (plan->output) and product (plan_inverse->input)
-    // never leave the GPU, so those two caller buffers are NOT written (no caller in the reference reads them).
+    // libcsdr.c:814-849 in one fused kernel (above 16384 points: transform, product, transform, overlap add as separate launches): the intermediate
+    // spectrum (plan->output) and product (plan_inverse->input) never leave the GPU, so those two caller buffers are NOT written (no caller in the
+    // reference reads them).
     Staging st("apply_fir_fft_cc");
     const int n = plan->size;
     const complexf* d_in = st.up(static_cast<const complexf*>(plan->input), n);
     const complexf* d_taps = st.up(taps_fft, n);
     const complexf* d_overlap = st.up(last_overlap, overlap_size);
     complexf* d_out = st.alloc<complexf>(n);
-    st.check(counted(launch_apply_fir_fft(reinterpret_cast<const float2*>(d_in), reinterpret_cast<const float2*>(d_taps), reinterpret_cast<const float2*>(d_overlap),
-                                          overlap_size, reinterpret_cast<float2*>(d_out), n, st.stream())));
+    const int launches = st.check(launch_apply_fir_fft(reinterpret_cast<const float2*>(d_in), reinterpret_cast<const float2*>(d_taps), reinterpret_cast<const float2*>(d_overlap),
+                                                       overlap_size, reinterpret_cast<float2*>(d_out), n, st.stream()));
+    counted(0, launches);
     st.get(static_cast<complexf*>(plan_inverse->output), d_out, n);
     st.sync();
 }

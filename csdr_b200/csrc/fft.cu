@@ -1,4 +1,4 @@
-// fft.cu -- K7 batched c2c FFT, K9 overlap-add FFT filter bank, a12 fastddc forward step, K8 fastddc inverse bank.
+// fft.cu -- K7 batched c2c FFT (and its four-step form above 16384 points), K9 overlap-add FFT filter bank, a12 fastddc forward step, K8 fastddc inverse bank.
 //
 //   fft_c2c_batch_kernel  : fft_execute() of a make_fft_c2c plan (fft_fftw.c:6-41), one CTA per transform.
 //   olafir_bank_kernel    : apply_fir_fft_cc (libcsdr.c:814-849) + the block loop of bandpass_fir_fft_cc
@@ -12,6 +12,7 @@
 //                           (same summation order as the reference: ascending bin index per destination),
 //                           /pre_decimation, swap, IFFT_M, /M, drop `scrap`, post shift + decimate.
 #include "fft_kernels.cuh"
+#include "fft_large.cuh"
 #include "kernels.h"
 #include "side_stream.cuh"
 
@@ -182,7 +183,8 @@ int launch_olafir_bank(const float2* d_in, long in_stride, float2* d_out, long o
 int launch_fastddc_fwd(const float2* d_in, float2* d_spectra, float2* d_overlap_io, int fft_size, int input_size, int nblocks, cudaStream_t st)
 {
     if (nblocks <= 0) return 0;
-    if (fft_size < 4 || fft_size > FFT_MAX_N || (fft_size & (fft_size - 1))) { set_error("fastddc_fwd: fft_size %d unsupported", fft_size); return -1; }
+    if (fft_size > FFT_MAX_N) return launch_fastddc_fwd_large(d_in, d_spectra, d_overlap_io, fft_size, input_size, nblocks, st);
+    if (fft_size < 4 || (fft_size & (fft_size - 1))) { set_error("fastddc_fwd: fft_size %d unsupported (power of two, 4..%d)", fft_size, kFftLargeMaxN); return -1; }
     if (fft_size >= 32) {                                               // radix-16 passes, as in launch_fft_c2c_batch
         const float2* tw16 = nullptr;
         if (int rc = get_twiddles16(fft_size, &tw16, st)) return rc;
@@ -227,7 +229,8 @@ int launch_fastddc_fwd(const float2* d_in, float2* d_spectra, float2* d_overlap_
 int launch_apply_fir_fft(const float2* d_in, const float2* d_taps_fft, const float2* d_last_overlap, int overlap_size, float2* d_out,
                          int fft_size, cudaStream_t st)
 {
-    if (fft_size < 2 || fft_size > FFT_MAX_N || (fft_size & (fft_size - 1))) { set_error("apply_fir_fft: fft_size %d unsupported", fft_size); return -1; }
+    if (fft_size > FFT_MAX_N) return launch_apply_fir_fft_large(d_in, d_taps_fft, d_last_overlap, overlap_size, d_out, fft_size, st);
+    if (fft_size < 2 || (fft_size & (fft_size - 1))) { set_error("apply_fir_fft: fft_size %d unsupported (power of two, 2..%d)", fft_size, kFftLargeMaxN); return -1; }
     const float2* tw = nullptr;
     if (int rc = get_twiddles(fft_size, &tw, st)) return rc;
     const size_t smem = sizeof(float2) * (size_t)fft_smem_elems(fft_size);
@@ -587,6 +590,138 @@ int fastddc_inv_plan_set_state(void* plan, const int* h_remain, const float* h_p
     CSDRB_CUDA(cudaMemcpy(pl->d_phase[dst], h_phase, sizeof(float) * pl->channels, cudaMemcpyHostToDevice));
     pl->ahead = false;
     return 0;
+}
+
+// ==== four-step transforms above FFT_MAX_N points (kernels: fft_large.cuh) ==========================================================================
+// ---- inter-step twiddles, cached per device and size ------------------------------------------------------------------------------------------
+struct LargeTwiddles { std::mutex mu; std::map<int, float2*> by_n; };
+
+static int get_large_twiddles(int n, const float2** lo, const float2** hi, cudaStream_t st)
+{
+    LargeTwiddles& c = per_device<LargeTwiddles>();
+    std::lock_guard<std::mutex> lk(c.mu);
+    auto it = c.by_n.find(n);
+    if (it == c.by_n.end()) {
+        const int nhi = n / kFftLargeSplit;
+        std::vector<float2> h((size_t)kFftLargeSplit + nhi);
+        for (int m = 0; m < kFftLargeSplit + nhi; m++) {
+            const double a = -2.0 * 3.14159265358979323846 * (m < kFftLargeSplit ? (double)m : (double)kFftLargeSplit * (m - kFftLargeSplit)) / (double)n;
+            h[(size_t)m] = make_float2((float)cos(a), (float)sin(a));
+        }
+        float2* d = nullptr;
+        CSDRB_CUDA(cudaMalloc(&d, sizeof(float2) * h.size()));
+        CSDRB_CUDA(cudaMemcpyAsync(d, h.data(), sizeof(float2) * h.size(), cudaMemcpyHostToDevice, st));
+        CSDRB_CUDA(cudaStreamSynchronize(st));                           // h leaves scope; once per device and size
+        it = c.by_n.emplace(n, d).first;
+    }
+    *lo = it->second; *hi = it->second + kFftLargeSplit;
+    return 0;
+}
+
+// ---- launchers -------------------------------------------------------------------------------------------------------------------------------------
+template <int F, bool FIRST, typename In>
+static int launch_step(In in, int in_b0, float2* out, long out_stride, int out_b0, int S, int count, bool inverse, const float2* lo, const float2* hi, cudaStream_t st)
+{
+    constexpr int W = kFftLargeTile;
+    const float2* tw16 = nullptr;
+    if (int rc = get_twiddles16(F, &tw16, st)) return rc;
+    const size_t smem = sizeof(float2) * (size_t)W * fft_large_seg(F);
+    const dim3 grid(S / W, count);
+    if (inverse) {
+        auto k = fft_large_step_kernel<F, true, FIRST, In>;
+        if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k<<<grid, W * (F / 16), smem, st>>>(in, in_b0, out, out_stride, out_b0, S, tw16, lo, hi);
+    } else {
+        auto k = fft_large_step_kernel<F, false, FIRST, In>;
+        if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k<<<grid, W * (F / 16), smem, st>>>(in, in_b0, out, out_stride, out_b0, S, tw16, lo, hi);
+    }
+    CSDRB_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// N = 2^LG = N1 * N2; the longer factor goes first
+#define CSDRB_FFT_LARGE_SIZES(X) X(15, 256, 128) X(16, 256, 256) X(17, 512, 256) X(18, 512, 512) X(19, 1024, 512) X(20, 1024, 1024)
+
+static bool fft_large_size_ok(int n) { return n >= kFftLargeMinN && n <= kFftLargeMaxN && (n & (n - 1)) == 0; }
+
+// `batch` transforms in.at(b, .) -> d_out + b*out_stride, in chunks that keep the intermediate within kFftLargeScratchBytes; returns the launches
+template <typename In>
+static int fft_large_run(In in, float2* d_out, long out_stride, int n, int batch, bool inverse, cudaStream_t st)
+{
+    const float2 *lo = nullptr, *hi = nullptr;
+    if (int rc = get_large_twiddles(n, &lo, &hi, st)) return rc;
+    const int chunk = (int)(kFftLargeScratchBytes / (sizeof(float2) * (size_t)n));
+    float2* t = nullptr;
+    CSDRB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&t), sizeof(float2) * (size_t)n * (size_t)(batch < chunk ? batch : chunk), st));
+    int launches = 0, rc = 0;
+    for (int b0 = 0; b0 < batch && rc == 0; b0 += chunk) {
+        const int count = batch - b0 < chunk ? batch - b0 : chunk;
+        switch (n) {
+#define X(LG, N1, N2) case 1 << LG: \
+            rc = launch_step<N1, true>(in, b0, t, (long)n, 0, N2, count, inverse, lo, hi, st); \
+            if (rc == 0) rc = launch_step<N2, false>(LargeRowsIn{t, (long)n}, 0, d_out, out_stride, b0, N1, count, inverse, lo, hi, st); \
+            break;
+            CSDRB_FFT_LARGE_SIZES(X)
+#undef X
+        }
+        launches += 2;
+    }
+    const cudaError_t freed = cudaFreeAsync(t, st);
+    if (rc) return rc;
+    CSDRB_CUDA(freed);
+    return launches;
+}
+
+int launch_fft_c2c_large_batch(const float2* d_in, long in_stride, float2* d_out, long out_stride, int n, int batch, int inverse, cudaStream_t st)
+{
+    if (!fft_large_size_ok(n)) { set_error("fft (large): size %d unsupported (power of two, %d..%d)", n, kFftLargeMinN, kFftLargeMaxN); return -1; }
+    if (batch <= 0) return 0;
+    return fft_large_run(LargeRowsIn{d_in, in_stride}, d_out, out_stride, n, batch, inverse != 0, st);
+}
+
+int launch_fastddc_fwd_large(const float2* d_in, float2* d_spectra, float2* d_overlap_io, int fft_size, int input_size, int nblocks, cudaStream_t st)
+{
+    if (!fft_large_size_ok(fft_size)) { set_error("fastddc_fwd: fft_size %d unsupported (power of two, 4..%d)", fft_size, kFftLargeMaxN); return -1; }
+    if (input_size <= 0 || input_size > fft_size) { set_error("fastddc_fwd: bad input_size %d for fft_size %d", input_size, fft_size); return -1; }
+    const int overlap = fft_size - input_size;
+    int launches = fft_large_run(LargeSlideIn{d_in, d_overlap_io, input_size, overlap}, d_spectra, (long)fft_size, fft_size, nblocks, false, st);
+    if (launches < 0 || overlap == 0) return launches;
+    // carry: the last `overlap` samples of (old overlap ++ new input).  A call shorter than the overlap shifts the old overlap, which a
+    // many-CTA copy cannot do in place: it goes through a stream-ordered buffer.
+    const long total = (long)nblocks * input_size;
+    const unsigned ctas = (unsigned)((overlap + 255) / 256 < 1024 ? (overlap + 255) / 256 : 1024);
+    if (total >= overlap) {
+        fft_large_gather_overlap_kernel<<<ctas, 256, 0, st>>>(d_in, d_overlap_io, d_overlap_io, overlap, total);
+        CSDRB_CUDA(cudaGetLastError());
+    } else {
+        float2* tmp = nullptr;
+        CSDRB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&tmp), sizeof(float2) * (size_t)overlap, st));
+        fft_large_gather_overlap_kernel<<<ctas, 256, 0, st>>>(d_in, d_overlap_io, tmp, overlap, total);
+        CSDRB_CUDA(cudaGetLastError());
+        CSDRB_CUDA(cudaMemcpyAsync(d_overlap_io, tmp, sizeof(float2) * (size_t)overlap, cudaMemcpyDeviceToDevice, st));
+        CSDRB_CUDA(cudaFreeAsync(tmp, st));
+    }
+    return launches + 1;
+}
+
+int launch_apply_fir_fft_large(const float2* d_in, const float2* d_taps_fft, const float2* d_last_overlap, int overlap_size, float2* d_out,
+                               int fft_size, cudaStream_t st)
+{
+    if (!fft_large_size_ok(fft_size)) { set_error("apply_fir_fft: fft_size %d unsupported (power of two, 2..%d)", fft_size, kFftLargeMaxN); return -1; }
+    float2* spec = nullptr;
+    CSDRB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&spec), sizeof(float2) * (size_t)fft_size, st));
+    int rc = fft_large_run(LargeRowsIn{d_in, (long)fft_size}, spec, (long)fft_size, fft_size, 1, false, st);
+    if (rc >= 0) {
+        fft_large_times_taps_kernel<<<(fft_size + 255) / 256, 256, 0, st>>>(spec, d_taps_fft, fft_size);
+        rc = fft_large_run(LargeRowsIn{spec, (long)fft_size}, d_out, (long)fft_size, fft_size, 1, true, st);
+    }
+    const cudaError_t freed = cudaFreeAsync(spec, st);
+    if (rc < 0) return rc;
+    CSDRB_CUDA(freed);
+    fft_large_scale_overlap_kernel<<<(fft_size + 255) / 256, 256, 0, st>>>(d_out, d_last_overlap, overlap_size, 1.0f / (float)fft_size, fft_size);
+    CSDRB_CUDA(cudaGetLastError());
+    return 6;
 }
 
 }  // namespace csdrb

@@ -119,6 +119,13 @@ int launch_olafir_bank(const float2* d_in, long in_stride, float2* d_out, long o
 int launch_apply_fir_fft(const float2* d_in, const float2* d_taps_fft, const float2* d_last_overlap, int overlap_size, float2* d_out,
                          int fft_size, cudaStream_t st);
 int launch_fastddc_fwd(const float2* d_in, float2* d_spectra, float2* d_overlap_io, int fft_size, int input_size, int nblocks, cudaStream_t st);
+// four-step transforms above the single-CTA range, fft.cu: the batched c2c call, and the forms launch_fastddc_fwd and launch_apply_fir_fft hand
+// their sizes above 16384 to (same contracts)
+constexpr int kFftLargeMinN = 1 << 15, kFftLargeMaxN = 1 << 20;
+int launch_fft_c2c_large_batch(const float2* d_in, long in_stride, float2* d_out, long out_stride, int n, int batch, int inverse, cudaStream_t st);
+int launch_fastddc_fwd_large(const float2* d_in, float2* d_spectra, float2* d_overlap_io, int fft_size, int input_size, int nblocks, cudaStream_t st);
+int launch_apply_fir_fft_large(const float2* d_in, const float2* d_taps_fft, const float2* d_last_overlap, int overlap_size, float2* d_out,
+                               int fft_size, cudaStream_t st);
 size_t fastddc_inv_scratch_bytes(int channels, int nblocks);
 int launch_fastddc_inv_bank(const float2* d_spectra, int nblocks, const float2* d_taps_fft, const void* d_chan, int channels,
                             int fft_size, int fft_inv_size, int pre_decimation, int scrap, int post_input_size, int post_decimation,

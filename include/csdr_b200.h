@@ -275,7 +275,8 @@ int csdrb_decimating_shift_addition_bank_cc(const complexf *d_in, long in_stride
  * >= M (e.g. T = 16 D + 1 up to D = 444, D = 1000 up to M = 8, D = 2 up to 48 taps).  D = 50 up to 850 taps and D = 10 up to 200 taps run their own
  * kernels, every other served geometry one kernel with D as an argument; the outputs follow the same contract either way.
  * Returns outputs per channel, -2 for an odd decimation or a geometry beyond those limits (nothing is launched, d_phase_io is left as it was) -- use
- * the unfused bank calls, or the fastddc overlap-save bank for very large decimations, then. */
+ * the unfused bank calls, or the fastddc overlap-save bank (csdrb_fastddc_fwd_cc with fft_size up to 2^20, csdrb_fastddc_inv_bank_cc with
+ * fft_inv_size up to 4096) for very large decimations and long filters, then. */
 size_t csdrb_ddc_bank_scratch_bytes(int channels, int input_size, int chunk, int offset);
 int csdrb_ddc_bank(const complexf *d_wide, int input_size, int channels, const shift_addition_data_t *d_params, float *d_phase_io,
                    int chunk, int offset, int decimation, const float *h_taps, int taps_length, int demod, void *d_out, long out_stride,
@@ -518,6 +519,10 @@ int csdrb_rtty_baudot2ascii_bank_u8_u8(const unsigned char *d_in, long in_stride
 
 /* K7 batched unnormalised c2c DFT (power-of-two size 2..16384), sign -1 forward / +1 inverse */
 int csdrb_fft_c2c_batch(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int size, int batch, int inverse, void *stream);
+/* The same transform for the sizes above one CTA's shared memory: power-of-two size 32768..1048576 (2^15..2^20), two launches per chunk of
+ * 2^21/size transforms (four-step algorithm, csrc/fft_large.cuh), the intermediate in stream-ordered scratch of at most 16 MiB; out of place
+ * (d_out must not overlap d_in); the call does not wait for the device.  -1 for any other size (nothing is launched). */
+int csdrb_fft_c2c_large_batch(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int size, int batch, int inverse, void *stream);
 
 /* K9 overlap-add FFT filter bank = bandpass_fir_fft_cc block loop (csdr.c:1872-1883) for many channels.
  * d_taps_fft: FFT of the zero-padded taps (taps_stride 0 = shared); d_tail_io [channels][fft_size] carries the
@@ -526,7 +531,9 @@ int csdrb_bandpass_fir_fft_bank_cc(const complexf *d_in, long in_stride, complex
                                    int input_size, int nblocks, const complexf *d_taps_fft, long taps_stride, complexf *d_tail_io, void *stream);
 
 /* fastddc forward step (csdr.c:2288-2299): nblocks x input_size new samples -> nblocks x fft_size bins;
- * d_overlap_io [fft_size - input_size] carries the overlap between calls (zero at stream start). */
+ * d_overlap_io [fft_size - input_size] carries the overlap between calls (zero at stream start).  fft_size is a power of two from 4 to
+ * 1048576 (2^20); above 16384 the transform is the four-step one of csdrb_fft_c2c_large_batch (stream-ordered scratch, at most 16 MiB), so
+ * fastddc_init geometries up to 131073 taps are served. */
 int csdrb_fastddc_fwd_cc(const complexf *d_in, complexf *d_spectra, complexf *d_overlap_io, int fft_size, int input_size, int nblocks, void *stream);
 
 /* K8 fastddc_inv_cc bank: every channel c (its own d_taps_fft + c*fft_size, offsetbin and post-shift NCO) consumes the
