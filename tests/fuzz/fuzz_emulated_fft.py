@@ -1,10 +1,11 @@
 """Fuzz the SHIPPED FFT-family kernels on the CPU (tests/host_shim/cuda_emul.h): random overlap-add geometries against numpy, random fastddc
-geometries against the oracle.  usage: python tests/fuzz/fuzz_emulated_fft.py [seed] [seconds]   -- test infrastructure."""
+geometries against the oracle, each also within the per-output bounds of tests/test_fft_bound_emulated.py.  usage: python tests/fuzz/fuzz_emulated_fft.py [seed] [seconds]   -- test infrastructure."""
 import sys, time, tempfile, ctypes as C, numpy as np
 from pathlib import Path
 _ROOT = str(Path(__file__).resolve().parents[2])
-sys.path.insert(0, _ROOT); sys.path.insert(0, _ROOT + '/tests/host_shim')
+sys.path.insert(0, _ROOT); sys.path.insert(0, _ROOT + '/tests/host_shim'); sys.path.insert(0, _ROOT + '/tests')
 import emul_build as eb
+import test_fft_bound_emulated as B
 from oracle.pyoracle import Oracle, rel_rms, _CF, _p, WINDOWS
 o = Oracle()
 fft, _ = eb.build_file(Path(tempfile.mkdtemp(prefix='fuzz_fft_')), 'fft.cu')
@@ -25,6 +26,8 @@ while time.time() < t_end:
                 blk = np.zeros(N, np.complex128); blk[:isz] = x[c, b * isz:(b + 1) * isz]
                 out[b * isz:b * isz + N] += np.fft.ifft(np.fft.fft(blk) * H[c].astype(np.complex128))
             e = rel_rms(y[c], out[:nb * isz]); worst['ola'] = max(worst.get('ola', 0), e); assert e < 3e-6, ('ola', N, isz, nb, bpc, e)
+            want, bound = B.ola_model(x[c], H[c], N, isz, B.ola_form(N), tail=tail0[c])
+            r = float(np.max(np.abs(y[c] - want) / bound)); worst['ola bound'] = max(worst.get('ola bound', 0), r); assert r <= 1, ('ola bound', N, isz, nb, bpc, r)
             if N > isz:
                 scale = np.sqrt(np.mean(np.abs(out) ** 2))                         # a one-sample tail is all cancellation: normalise by the stream's level
                 e = float(np.abs(tail[c, :N - isz] - out[nb * isz:]).max() / scale); assert e < 1e-5, ('ola tail', N, isz, nb, bpc, e)
@@ -54,4 +57,6 @@ while time.time() < t_end:
             assert total[k] == w.size, ('inv count', bw, dec, s, total[k], w.size)
             if w.size:
                 e = rel_rms(out[k, :w.size], w); worst['inv'] = max(worst.get('inv', 0), e); assert e < 1e-5, ('inv', bw, dec, s, e)
+                m, bound, _, _, _ = B.fastddc_inv_model(o, want_sp, tf[k], chan[k], gs[k], B.inv_path(g, nb, chn))
+                r = float(np.max(np.abs(out[k, :w.size] - m) / bound)); worst['inv bound'] = max(worst.get('inv bound', 0), r); assert r <= 1, ('inv bound', bw, dec, s, r)
 print("iterations", it, "worst", worst)
