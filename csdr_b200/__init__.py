@@ -153,6 +153,7 @@ def lib() -> C.CDLL:
     sz = C.c_size_t
     L.csdrb_shift_addition_bank_scratch_bytes.argtypes = [it, it, it]; L.csdrb_shift_addition_bank_scratch_bytes.restype = sz
     L.csdrb_shift_addition_bank_cc.argtypes = [vp, lg, vp, lg, it, it, vp, vp, it, vp, sz, vp]
+    L.csdrb_shift_addition_bank_fc.argtypes = [vp, lg, vp, lg, it, it, vp, vp, it, vp, sz, vp]
     L.csdrb_decimating_shift_addition_bank_cc.argtypes = [vp, lg, vp, lg, it, it, vp, it, vp, vp, vp, vp]
     L.csdrb_fractional_decimator_bank_scratch_bytes.argtypes = [it, it, C.c_float]; L.csdrb_fractional_decimator_bank_scratch_bytes.restype = sz
     L.csdrb_fractional_decimator_bank_ff.argtypes = [vp, lg, vp, lg, it, it, C.c_float, it, vp, it, vp, vp, sz, vp]
@@ -171,11 +172,13 @@ def lib() -> C.CDLL:
     L.csdrb_bandpass_fir_fft_bank_cc.argtypes = [vp, lg, vp, lg, it, it, it, it, vp, lg, vp, vp]
     L.csdrb_ddc_bank_scratch_bytes.argtypes = [it, it, it, it]; L.csdrb_ddc_bank_scratch_bytes.restype = sz
     L.csdrb_ddc_bank.argtypes = [vp, it, it, vp, vp, it, it, it, C.POINTER(C.c_float), it, it, vp, lg, vp, vp, vp, sz, vp]
+    L.csdrb_ddc_bank_f.argtypes = [vp, it, it, vp, vp, it, it, it, C.POINTER(C.c_float), it, it, vp, lg, vp, vp, vp, sz, vp]
     L.csdrb_ddc_bank_create.argtypes = [it, C.POINTER(C.c_float), it, C.POINTER(C.c_float), it, it, it]; L.csdrb_ddc_bank_create.restype = vp
     L.csdrb_ddc_bank_destroy.argtypes = [vp]
     L.csdrb_ddc_bank_set_rate.argtypes = [vp, it, C.c_float]
     L.csdrb_ddc_bank_offset.argtypes = [vp]
     L.csdrb_ddc_bank_process.argtypes = [vp, vp, it, vp, lg, vp]
+    L.csdrb_ddc_bank_process_f.argtypes = [vp, vp, it, vp, lg, vp]
     L.csdrb_ddc_bank_rechunk.argtypes = [vp]
     L.csdrb_fastddc_inv_plan_create.argtypes = [vp, it, vp, it]; L.csdrb_fastddc_inv_plan_create.restype = vp
     L.csdrb_fastddc_inv_plan_run.argtypes = [vp, vp, vp, vp, lg, vp, vp]
@@ -231,6 +234,7 @@ def lib() -> C.CDLL:
     L.fastddc_init.argtypes = [C.POINTER(FastDDC), C.c_float, it, C.c_float]
     L.decimating_shift_addition_init.argtypes = [C.c_float, it]; L.decimating_shift_addition_init.restype = _Shift
     L.shift_addition_cc.argtypes = [vp, vp, it, _Shift, C.c_float]; L.shift_addition_cc.restype = C.c_float
+    L.shift_addition_fc.argtypes = [vp, vp, it, _Shift, C.c_float]; L.shift_addition_fc.restype = C.c_float
     L.decimating_shift_addition_cc.argtypes = [vp, vp, it, _Shift, it, _DShiftStatus]; L.decimating_shift_addition_cc.restype = _DShiftStatus
     L.fractional_decimator_ff_init.argtypes = [C.c_float, it, vp, it]; L.fractional_decimator_ff_init.restype = _FracDec
     L.fractional_decimator_ff.argtypes = [vp, vp, it, C.POINTER(_FracDec)]
@@ -543,6 +547,16 @@ class libcsdr:
         return y, float(np.float32(phase))
 
     @staticmethod
+    def shift_addition_fc(x, rate, phase=0.0, chunk=None):
+        """real x -> (complex64 y, phase): one shift_addition_fc call per `chunk` samples"""
+        x = np.ascontiguousarray(x, np.float32); y = np.empty(x.size, np.complex64); d = lib().shift_addition_init(rate)
+        chunk = chunk or max(x.size, 1)
+        for s in range(0, x.size, chunk):
+            n = min(chunk, x.size - s)
+            phase = lib().shift_addition_fc(x[s:].ctypes.data, y[s:].ctypes.data, n, d, phase)
+        return y, float(np.float32(phase))
+
+    @staticmethod
     def decimating_shift_addition_cc(x, rate, decimation, remain=0, phase=0.0):
         x = np.ascontiguousarray(x, np.complex64); y = np.empty(x.size // decimation + 2, np.complex64)
         d = lib().decimating_shift_addition_init(rate, decimation)
@@ -811,6 +825,29 @@ def shift_addition_bank_cc(x, rates, phases=None, chunk: int = 1024, out=None):
     scratch = _scratch(sb, xr.device)
     _check(lib().csdrb_shift_addition_bank_cc(ptr, stride, out.data_ptr(), out.stride(0), ch, n, d_params.data_ptr(), d_phase.data_ptr(), chunk,
                                               scratch.data_ptr(), scratch.numel(), _stream()), "shift_addition_bank_cc")
+    return out, d_phase
+
+
+def shift_addition_bank_fc(x, rates, phases=None, chunk: int = 1024, out=None):
+    """x: [N] (one shared real wideband stream) or [C, N] float32 CUDA tensor; rates: C floats.  Returns (y [C, N] complex64, new phases [C]):
+    shift_addition_fc called once per `chunk` samples, bit for bit."""
+    import torch
+    assert x.dtype == torch.float32 and x.is_cuda and x.dim() in (1, 2) and x.stride(-1) == 1
+    rates = np.atleast_1d(np.asarray(rates, np.float32))
+    ch = rates.size
+    n = x.shape[-1]
+    if x.dim() == 1:
+        stride = 0
+    else:
+        assert x.shape[0] == ch
+        stride = x.stride(0)
+    d_params = torch.from_numpy(np.array([shift_addition_init(float(r)) for r in rates], np.float32)).to(x.device)
+    d_phase = torch.zeros(ch, dtype=torch.float32, device=x.device) if phases is None else phases.clone()
+    if out is None:
+        out = torch.empty((ch, n), dtype=torch.complex64, device=x.device)
+    scratch = _scratch(lib().csdrb_shift_addition_bank_scratch_bytes(ch, n, chunk), x.device)
+    _check(lib().csdrb_shift_addition_bank_fc(x.data_ptr(), stride, out.data_ptr(), out.stride(0), ch, n, d_params.data_ptr(), d_phase.data_ptr(), chunk,
+                                              scratch.data_ptr(), scratch.numel(), _stream()), "shift_addition_bank_fc")
     return out, d_phase
 
 
@@ -1278,12 +1315,14 @@ class FastddcInvPlan:
 
 def ddc_bank(wide, rates, decimation: int, taps: np.ndarray, demod: bool = True, chunk: int = 1024, offset: int = 0,
              phases=None, last=None, out=None):
-    """Fused shared-input bank: one wideband block [N] complex64 -> per channel shift | fir_decimate | (fmdemod).
+    """Fused shared-input bank: one wideband block [N] complex64 -> per channel shift | fir_decimate | (fmdemod).  A float32 block is a REAL
+    stream (shift_addition_fc in front, csdrb_ddc_bank_f): tune a station at f Hz of a stream sampled at fs with rate -f/fs.
     Any even decimation D whose filter has M = ceil(len(taps) / D) <= 24 and D * MP <= 8000 taps (MP = the smallest of 4, 8, 12, 18, 20, 24 >= M);
     an odd D or a longer filter raises CsdrB200Error.
     Returns (out [C, n_out], new chunk-start phases [C], last baseband samples [C] or None)."""
     import torch
-    assert wide.dtype == torch.complex64 and wide.is_cuda and wide.dim() == 1
+    assert wide.dtype in (torch.complex64, torch.float32) and wide.is_cuda and wide.dim() == 1
+    entry = lib().csdrb_ddc_bank_f if wide.dtype == torch.float32 else lib().csdrb_ddc_bank
     rates = np.atleast_1d(np.asarray(rates, np.float32)); ch = rates.size
     taps = np.ascontiguousarray(taps, np.float32)
     n = wide.numel()
@@ -1296,7 +1335,7 @@ def ddc_bank(wide, rates, decimation: int, taps: np.ndarray, demod: bool = True,
         out = torch.empty((ch, stride), dtype=torch.float32 if demod else torch.complex64, device=dev)
     last_out = torch.empty(ch, dtype=torch.complex64, device=dev) if demod else None
     scratch = _scratch(lib().csdrb_ddc_bank_scratch_bytes(ch, n, chunk, offset), dev)
-    rc = _check(lib().csdrb_ddc_bank(wide.data_ptr(), n, ch, params.data_ptr(), d_phase.data_ptr(), chunk, offset, decimation, _fp(taps), taps.size,
+    rc = _check(entry(wide.data_ptr(), n, ch, params.data_ptr(), d_phase.data_ptr(), chunk, offset, decimation, _fp(taps), taps.size,
                                      1 if demod else 0, out.data_ptr(), out.stride(0), last.data_ptr() if last is not None else None,
                                      last_out.data_ptr() if last_out is not None else None, scratch.data_ptr(), scratch.numel(), _stream()), "ddc_bank")
     assert rc == n_out
@@ -1367,13 +1406,15 @@ class DdcBank:
             raise CsdrB200Error(f"csdrb_ddc_bank_create: {lib().csdrb_last_error().decode()}")
 
     def process(self, wide, out=None):
-        """wide: [N] complex64 CUDA tensor starting where the previous call stopped consuming (n_out*decimation samples in)."""
+        """wide: [N] complex64 CUDA tensor starting where the previous call stopped consuming (n_out*decimation samples in); a float32 tensor is
+        a block of a real stream (csdrb_ddc_bank_process_f)."""
         import torch
-        assert wide.dtype == torch.complex64 and wide.is_cuda and wide.dim() == 1
+        assert wide.dtype in (torch.complex64, torch.float32) and wide.is_cuda and wide.dim() == 1
+        entry = lib().csdrb_ddc_bank_process_f if wide.dtype == torch.float32 else lib().csdrb_ddc_bank_process
         n_out = fir_out_len(wide.numel(), self.decimation, self.taps.size)
         if out is None:
             out = torch.empty((self.channels, n_out + (n_out & 1)), dtype=torch.float32 if self.demod else torch.complex64, device=wide.device)
-        rc = _check(lib().csdrb_ddc_bank_process(self.h, wide.data_ptr(), wide.numel(), out.data_ptr(), out.stride(0), _stream()), "ddc_bank_process")
+        rc = _check(entry(self.h, wide.data_ptr(), wide.numel(), out.data_ptr(), out.stride(0), _stream()), "ddc_bank_process")
         return out[:, :rc]
 
     def set_rate(self, channel: int, rate: float):

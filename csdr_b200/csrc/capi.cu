@@ -274,6 +274,16 @@ int csdrb_shift_addition_bank_cc(const complexf* d_in, long in_stride, complexf*
     return rc < 0 ? rc : counted(0, rc);
 }
 
+int csdrb_shift_addition_bank_fc(const float* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int input_size,
+                                 const shift_addition_data_t* d_params, float* d_phase_io, int chunk, void* d_scratch, size_t scratch_bytes, void* stream)
+{
+    if (too_many_channels(channels, "shift_addition_fc bank")) return -1;
+    if (!d_in || !d_out || !d_params || !d_phase_io) { set_error("shift_addition_fc bank: null pointer"); return -1; }
+    int rc = launch_shift_addition_bank_fc(d_in, in_stride, reinterpret_cast<float2*>(d_out), out_stride, channels, input_size,
+                                           reinterpret_cast<const float*>(d_params), d_phase_io, chunk, d_scratch, scratch_bytes, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
 size_t csdrb_shift_math_bank_scratch_bytes(int channels, int input_size) { return shift_math_scratch_bytes(channels, input_size); }
 
 int csdrb_shift_math_bank_cc(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int input_size,
@@ -743,6 +753,19 @@ int csdrb_ddc_bank(const complexf* d_wide, int input_size, int channels, const s
     return rc;
 }
 
+int csdrb_ddc_bank_f(const float* d_wide, int input_size, int channels, const shift_addition_data_t* d_params, float* d_phase_io, int chunk, int offset,
+                     int decimation, const float* h_taps, int taps_length, int demod, void* d_out, long out_stride,
+                     const complexf* d_last_in, complexf* d_last_out, void* d_scratch, size_t scratch_bytes, void* stream)
+{
+    if (!d_wide || !d_params || !d_phase_io || !h_taps || !d_out) { set_error("ddc bank: null pointer"); return -1; }
+    int launches = 0;
+    int rc = launch_ddc_bank_f(d_wide, input_size, channels, reinterpret_cast<const float*>(d_params), d_phase_io, chunk, offset,
+                               decimation, h_taps, taps_length, demod, d_out, out_stride, reinterpret_cast<const float2*>(d_last_in),
+                               reinterpret_cast<float2*>(d_last_out), d_scratch, scratch_bytes, &launches, S(stream));
+    if (rc >= 0) g_launches += launches;
+    return rc;
+}
+
 // ---- streaming DDC/NFM bank object ---------------------------------------------------------------------
 // Owns every piece of per-channel state (NCO parameters, chunk-start phases, discriminator history, position inside the current
 // chunk) so that a stream is processed block by block with one call per block, and hides the serial float phase chain: while the
@@ -825,7 +848,8 @@ int csdrb_ddc_bank_rechunk(csdrb_ddc_bank_t* b)
 
 int csdrb_ddc_bank_offset(const csdrb_ddc_bank_t* b) { return b ? b->offset : -1; }
 
-int csdrb_ddc_bank_process(csdrb_ddc_bank_t* b, const complexf* d_wide, int input_size, void* d_out, long out_stride, void* stream)
+// one block of complex (real = false) or real (real = true) wideband samples; the bank's state does not depend on which, so a stream may even switch
+static int ddc_bank_process(csdrb_ddc_bank_t* b, const void* d_wide, bool real, int input_size, void* d_out, long out_stride, void* stream)
 {
     if (!b || !d_wide || !d_out) { set_error("ddc bank process: null pointer"); return -1; }
     cudaStream_t st = S(stream);
@@ -876,8 +900,10 @@ int csdrb_ddc_bank_process(csdrb_ddc_bank_t* b, const complexf* d_wide, int inpu
     }
     b->ahead_valid = false;
     // main kernel of this block: discriminator history ping-pongs last[last_sel] -> last[last_sel^1]
-    int rc = launch_ddc_main(reinterpret_cast<const float2*>(d_wide), input_size, b->channels, b->d_params, b->chunk, b->offset, b->decimation, b->taps.data(),
-                             b->taps_length, b->demod, d_out, out_stride, b->d_last[b->last_sel], b->d_last[b->last_sel ^ 1], b->d_scratch[sel], st);
+    int rc = real ? launch_ddc_main_f(static_cast<const float*>(d_wide), input_size, b->channels, b->d_params, b->chunk, b->offset, b->decimation, b->taps.data(),
+                                      b->taps_length, b->demod, d_out, out_stride, b->d_last[b->last_sel], b->d_last[b->last_sel ^ 1], b->d_scratch[sel], st)
+                  : launch_ddc_main(static_cast<const float2*>(d_wide), input_size, b->channels, b->d_params, b->chunk, b->offset, b->decimation, b->taps.data(),
+                                    b->taps_length, b->demod, d_out, out_stride, b->d_last[b->last_sel], b->d_last[b->last_sel ^ 1], b->d_scratch[sel], st);
     if (rc < 0) return rc;
     launches += 1;
     b->last_sel ^= 1;
@@ -902,6 +928,16 @@ int csdrb_ddc_bank_process(csdrb_ddc_bank_t* b, const complexf* d_wide, int inpu
     b->blocks++;
     g_launches += launches;
     return n_out;
+}
+
+int csdrb_ddc_bank_process(csdrb_ddc_bank_t* b, const complexf* d_wide, int input_size, void* d_out, long out_stride, void* stream)
+{
+    return ddc_bank_process(b, d_wide, false, input_size, d_out, out_stride, stream);
+}
+
+int csdrb_ddc_bank_process_f(csdrb_ddc_bank_t* b, const float* d_wide, int input_size, void* d_out, long out_stride, void* stream)
+{
+    return ddc_bank_process(b, d_wide, true, input_size, d_out, out_stride, stream);
 }
 
 }  // extern "C"

@@ -147,14 +147,22 @@ struct DdcWalk {
     // output's window [oD, oD + T), and fma(sh, 0, acc) is NaN for a non-finite sh where the reference, which never reads them, stays finite.
     // For a finite sh the skipped fma(sh, 0, acc) is acc, so both forms give the same bits; the walk takes the unguarded one only for samples
     // it has checked to be small enough for sh to stay finite.
-    template <int JLO, int JHI, bool GUARD = false>
-    __device__ __forceinline__ void sample(float xi, float xq, const float2* __restrict__ tp, int lim = 0, int D = 0)
+    // The shifted sample: complex x is one product rounded and the other fused (the data path has 1e-5 to spend; the phasor state has none);
+    // real x (shift_addition_fc, libcsdr_gpl.c:66-67) is P * x, one rounded product per component -- the value ffma2(P, x, Q * 0) would give up to
+    // the sign of a zero, without its extra multiply.
+    __device__ __forceinline__ float2 shifted(int u, float2 x) const
     {
-        const float2 xi2 = make_float2(xi, xi), xq2 = make_float2(xq, xq);
+        return ffma2(P[u], make_float2(x.x, x.x), fmul2(Q[u], make_float2(x.y, x.y)));
+    }
+    __device__ __forceinline__ float2 shifted(int u, float x) const { return fmul2(P[u], make_float2(x, x)); }
+
+    template <int JLO, int JHI, bool GUARD = false, class X>
+    __device__ __forceinline__ void sample(X x, const float2* __restrict__ tp, int lim = 0, int D = 0)
+    {
         float2 sh[CPL];
 #pragma unroll
         for (int u = 0; u < CPL; u++) {
-            sh[u] = ffma2(P[u], xi2, fmul2(Q[u], xq2));             // one product rounded, the other fused (the data path has 1e-5 to spend; the phasor state has none)
+            sh[u] = shifted(u, x);
             advance(u);
         }
 #pragma unroll
@@ -173,8 +181,9 @@ struct DdcWalk {
 // The walk of one warp, shared by both bank kernels.  DC > 0: the decimation is the compile-time DC (ddc_bank_fused2_kernel); DC = 0: it is the
 // run-time d_rt (ddc_bank_generic_kernel).  U = samples per unchecked group of a full-width period: a period runs groups of U while U samples are
 // left and the rest in groups of 2 (DC is a multiple of U).  staps = the taps in shared memory, [p][j / 2] = taps (j, j+1) of phase p.
-template <int DC, int M, int CPL, bool DEMOD, int U>
-__device__ __forceinline__ void ddc_bank_walk(const float2* __restrict__ wide, int n_in, int offset, int chunk, int nchunks,
+// TIn = float2: complex wideband samples (shift_addition_cc); TIn = float: real ones (shift_addition_fc), read two per 8-byte load.
+template <int DC, int M, int CPL, bool DEMOD, int U, class TIn = float2>
+__device__ __forceinline__ void ddc_bank_walk(const TIn* __restrict__ wide, int n_in, int offset, int chunk, int nchunks,
                                               const float3* __restrict__ params, const float2* __restrict__ seeds, int channels, int sets,
                                               void* __restrict__ out_v, long out_stride, int n_out, int seg_outputs, int nsegs,
                                               const float2* __restrict__ last_in, float2* __restrict__ last_out, int T, int d_rt, const float2* staps)
@@ -226,8 +235,8 @@ __device__ __forceinline__ void ddc_bank_walk(const float2* __restrict__ wide, i
             left = chunk;
         }
         left--;
-        const float2 x = idx < n_in ? __ldg(wide + idx) : make_float2(0.f, 0.f);   // samples past n_in only ever meet zero-padded taps
-        w.template sample<decltype(jlo)::value, decltype(jhi)::value, true>(x.x, x.y, staps + pidx * (MP / 2), T - pidx, D);
+        const TIn x = idx < n_in ? __ldg(wide + idx) : TIn{};       // samples past n_in only ever meet zero-padded taps
+        w.template sample<decltype(jlo)::value, decltype(jhi)::value, true>(x, staps + pidx * (MP / 2), T - pidx, D);
     };
     // one period (D samples) restricted to accumulators [JLO, JHI)
     auto period = [&](auto jlo, auto jhi, int q) {
@@ -240,22 +249,30 @@ __device__ __forceinline__ void ddc_bank_walk(const float2* __restrict__ wide, i
             // (fetching the next group's samples into registers while this one is multiplied was slower: the extra registers cost more
             // than the exposed L1 round trip)
             if (left >= G && base + p0 + G <= n_in) {
-                const float4* src = reinterpret_cast<const float4*>(wide + base + p0);     // D, p0 even: 16-byte aligned
+                // two samples per load: D, p0 even, so 16-byte aligned for complex samples and 8-byte aligned for real ones
+                using Pair = std::conditional_t<std::is_same_v<TIn, float>, float2, float4>;
+                const Pair* src = reinterpret_cast<const Pair*>(wide + base + p0);
                 const float2* tp = staps + p0 * (MP / 2);
-                float4 cur[G / 2];
+                Pair cur[G / 2];
                 float mag = 0.f;                                        // sum of |x.i| + |x.q| over the group: NaN, Inf or huge -> guarded path
 #pragma unroll
                 for (int e = 0; e < G / 2; e++) {
                     cur[e] = __ldg(src + e);
-                    mag += fabsf(cur[e].x) + fabsf(cur[e].y) + fabsf(cur[e].z) + fabsf(cur[e].w);
+                    if constexpr (std::is_same_v<TIn, float>) mag += fabsf(cur[e].x) + fabsf(cur[e].y);
+                    else mag += fabsf(cur[e].x) + fabsf(cur[e].y) + fabsf(cur[e].z) + fabsf(cur[e].w);
                 }
                 // |P|, |Q| stay near 1, so below 2^126 every shifted sample of the group is finite and the padded taps add exactly nothing
                 if (mag < 0x1p126f) {
 #pragma unroll
                     for (int e = 0; e < G; e += 2) {
-                        const float4 xx = cur[e / 2];
-                        w.template sample<JLO, JHI>(xx.x, xx.y, tp + e * (MP / 2));
-                        w.template sample<JLO, JHI>(xx.z, xx.w, tp + (e + 1) * (MP / 2));
+                        const Pair xx = cur[e / 2];
+                        if constexpr (std::is_same_v<TIn, float>) {
+                            w.template sample<JLO, JHI>(xx.x, tp + e * (MP / 2));
+                            w.template sample<JLO, JHI>(xx.y, tp + (e + 1) * (MP / 2));
+                        } else {
+                            w.template sample<JLO, JHI>(make_float2(xx.x, xx.y), tp + e * (MP / 2));
+                            w.template sample<JLO, JHI>(make_float2(xx.z, xx.w), tp + (e + 1) * (MP / 2));
+                        }
                     }
                     left -= G;
                     return;
@@ -330,6 +347,21 @@ ddc_bank_fused2_kernel(const float2* __restrict__ wide, int n_in, int offset, in
 
 static_assert(sizeof(DdcTaps<kDdcTapCapacity>) + 160 <= 32764, "the generic kernel's parameters must fit the 32 764-byte parameter space");
 
+// the generic kernels' body: the taps into `staps` (D * MP floats of dynamic shared memory), then the walk with D a run-time argument
+template <int M, int CPL, bool DEMOD, class TIn>
+__device__ __forceinline__ void ddc_generic_body(const TIn* __restrict__ wide, int n_in, int offset, int chunk, int nchunks,
+                                                 const float3* __restrict__ params, const float2* __restrict__ seeds, int channels, int sets,
+                                                 void* __restrict__ out_v, long out_stride, int n_out, int seg_outputs, int nsegs,
+                                                 const float2* __restrict__ last_in, float2* __restrict__ last_out, int T, int D,
+                                                 const DdcTaps<kDdcTapCapacity>& taps, float2* staps)
+{
+    constexpr int MP = (M + 1) & ~1;
+    for (int i = threadIdx.x; i < D * MP / 2; i += 128) staps[i] = taps.h2[i];
+    __syncthreads();
+    ddc_bank_walk<0, M, CPL, DEMOD, 8, TIn>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, sets, out_v, out_stride, n_out,
+                                            seg_outputs, nsegs, last_in, last_out, T, D, staps);
+}
+
 // any even D: D * MP floats of taps in dynamic shared memory (at most 32 000 bytes, no opt-in needed)
 template <int M, int CPL, bool DEMOD>
 __global__ void __launch_bounds__(128, ddc_generic_ctas_per_sm(M, CPL))
@@ -339,13 +371,23 @@ ddc_bank_generic_kernel(const float2* __restrict__ wide, int n_in, int offset, i
                         const float2* __restrict__ last_in, float2* __restrict__ last_out, int T, int D,
                         const __grid_constant__ DdcTaps<kDdcTapCapacity> taps)
 {
-    constexpr int MP = (M + 1) & ~1;
     CSDRB_DYN_SMEM(smem);
-    float2* staps = reinterpret_cast<float2*>(smem);
-    for (int i = threadIdx.x; i < D * MP / 2; i += 128) staps[i] = taps.h2[i];
-    __syncthreads();
-    ddc_bank_walk<0, M, CPL, DEMOD, 8>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, sets, out_v, out_stride, n_out,
-                                       seg_outputs, nsegs, last_in, last_out, T, D, staps);
+    ddc_generic_body<M, CPL, DEMOD, float2>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, sets, out_v, out_stride, n_out, seg_outputs, nsegs,
+                                            last_in, last_out, T, D, taps, reinterpret_cast<float2*>(smem));
+}
+
+// the same on real wideband samples (csdrb_ddc_bank_f), at every served geometry -- D = 50 and 10 too -- and kDdcChannelsPerLane channels per lane
+template <int M, bool DEMOD>
+__global__ void __launch_bounds__(128, ddc_generic_ctas_per_sm(M, kDdcChannelsPerLane))
+ddc_bank_generic_real_kernel(const float* __restrict__ wide, int n_in, int offset, int chunk, int nchunks,
+                             const float3* __restrict__ params, const float2* __restrict__ seeds, int channels, int sets,
+                             void* __restrict__ out_v, long out_stride, int n_out, int seg_outputs, int nsegs,
+                             const float2* __restrict__ last_in, float2* __restrict__ last_out, int T, int D,
+                             const __grid_constant__ DdcTaps<kDdcTapCapacity> taps)
+{
+    CSDRB_DYN_SMEM(smem);
+    ddc_generic_body<M, kDdcChannelsPerLane, DEMOD, float>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, sets, out_v, out_stride, n_out,
+                                                           seg_outputs, nsegs, last_in, last_out, T, D, taps, reinterpret_cast<float2*>(smem));
 }
 
 size_t ddc_bank_scratch_bytes(int channels, int input_size, int chunk, int offset)
@@ -419,22 +461,32 @@ static int launch_fused(const float2* wide, int n_in, int offset, int chunk, int
     return 0;
 }
 
-// M = bucket; sized for the bucket's own resident warps (its registers allow fewer CTAs per SM than the D = 50 / 10 kernels' three at large M)
-template <int M>
-static int launch_generic(const float2* wide, int n_in, int offset, int chunk, int nchunks, const float3* params, const float2* seeds, int channels,
+// M = bucket; sized for the bucket's own resident warps (its registers allow fewer CTAs per SM than the D = 50 / 10 kernels' three at large M).
+// Real input (TIn = float) runs at kDdcChannelsPerLane whatever CSDRB_DDC_CPL says: one instantiation per bucket and DEMOD.
+template <int M, class TIn = float2>
+static int launch_generic(const TIn* wide, int n_in, int offset, int chunk, int nchunks, const float3* params, const float2* seeds, int channels,
                           int demod, void* out, long out_stride, int n_out, const float2* last_in, float2* last_out, const float* h_taps, int T, int D,
                           cudaStream_t st)
 {
     constexpr int MP = (M + 1) & ~1;
     DdcTaps<kDdcTapCapacity> tp;
     ddc_pack_taps(tp.h2, D, M, h_taps, T);
-    static const int cpl = ddc_cpl_from_env();
+    static const int env_cpl = ddc_cpl_from_env();
+    constexpr bool real = std::is_same_v<TIn, float>;
+    const int cpl = real ? kDdcChannelsPerLane : env_cpl;
     const DdcGrid g = ddc_grid(channels, n_out, M, cpl, 4 * ddc_generic_ctas_per_sm(M, cpl));
     const size_t smem = (size_t)D * MP * sizeof(float);
-#define CSDRB_DDC_LAUNCH(CPLV, DM) ddc_bank_generic_kernel<M, CPLV, DM><<<g.ctas, 128, smem, st>>>(wide, n_in, offset, chunk, nchunks, params, seeds, channels, g.sets, out, out_stride, n_out, g.seg, g.nsegs, last_in, last_out, T, D, tp)
-    if (cpl == kDdcChannelsPerLane) { if (demod) CSDRB_DDC_LAUNCH(kDdcChannelsPerLane, true); else CSDRB_DDC_LAUNCH(kDdcChannelsPerLane, false); }
-    else { if (demod) CSDRB_DDC_LAUNCH(1, true); else CSDRB_DDC_LAUNCH(1, false); }
+#define CSDRB_DDC_ARGS wide, n_in, offset, chunk, nchunks, params, seeds, channels, g.sets, out, out_stride, n_out, g.seg, g.nsegs, last_in, last_out, T, D, tp
+    if constexpr (real) {
+        if (demod) ddc_bank_generic_real_kernel<M, true><<<g.ctas, 128, smem, st>>>(CSDRB_DDC_ARGS);
+        else ddc_bank_generic_real_kernel<M, false><<<g.ctas, 128, smem, st>>>(CSDRB_DDC_ARGS);
+    } else {
+#define CSDRB_DDC_LAUNCH(CPLV, DM) ddc_bank_generic_kernel<M, CPLV, DM><<<g.ctas, 128, smem, st>>>(CSDRB_DDC_ARGS)
+        if (cpl == kDdcChannelsPerLane) { if (demod) CSDRB_DDC_LAUNCH(kDdcChannelsPerLane, true); else CSDRB_DDC_LAUNCH(kDdcChannelsPerLane, false); }
+        else { if (demod) CSDRB_DDC_LAUNCH(1, true); else CSDRB_DDC_LAUNCH(1, false); }
 #undef CSDRB_DDC_LAUNCH
+    }
+#undef CSDRB_DDC_ARGS
     CSDRB_CUDA(cudaGetLastError());
     return 0;
 }
@@ -488,8 +540,21 @@ int launch_ddc_prepass(int input_size, int channels, const float* d_params, floa
     return launches;
 }
 
-// main kernel: needs the seeds a matching launch_ddc_prepass() left in d_scratch
-int launch_ddc_main(const float2* d_wide, int input_size, int channels, const float* d_params, int chunk, int offset, int decimation,
+// the alignment the group loads need: two samples per load, 16 bytes for complex input, 8 for real
+template <class TIn>
+static bool ddc_wide_aligned(const TIn* d_wide)
+{
+    constexpr bool real = std::is_same_v<TIn, float>;
+    if (!(reinterpret_cast<uintptr_t>(d_wide) & (real ? 7 : 15))) return true;
+    set_error(real ? "ddc bank: real wideband input must be 8-byte aligned (an even sample of a 16-byte aligned buffer)"
+                   : "ddc bank: wideband input must be 16-byte aligned");
+    return false;
+}
+
+// main kernel: needs the seeds a matching launch_ddc_prepass() left in d_scratch.  Complex input: D = 50 and 10 run their own kernels; real input
+// runs the generic kernel at every served geometry.
+template <class TIn>
+static int ddc_main(const TIn* d_wide, int input_size, int channels, const float* d_params, int chunk, int offset, int decimation,
                     const float* h_taps, int taps_length, int demod, void* d_out, long out_stride, const float2* d_last_in, float2* d_last_out,
                     const void* d_scratch, cudaStream_t st)
 {
@@ -497,46 +562,84 @@ int launch_ddc_main(const float2* d_wide, int input_size, int channels, const fl
     const int n_out = input_size >= taps_length ? (input_size - taps_length) / decimation + 1 : 0;
     if (n_out == 0) return 0;
     if (chunk <= 0) chunk = input_size;
-    if (reinterpret_cast<uintptr_t>(d_wide) & 15) { set_error("ddc bank: wideband input must be 16-byte aligned"); return -1; }
+    if (!ddc_wide_aligned(d_wide)) return -1;
     const int nchunks = (int)(((long)offset + input_size + chunk - 1) / chunk) + 1;
     const float2* seeds = reinterpret_cast<const float2*>(static_cast<const char*>(d_scratch) + (((size_t)channels * nchunks * sizeof(float) + 15) & ~(size_t)15));
     if (int rc = ddc_bank_geometry(decimation, taps_length); rc < 0) return rc;
     int rc = -1;
     const float3* P = reinterpret_cast<const float3*>(d_params);
 #define CSDRB_DDC_ARGS d_wide, input_size, offset, chunk, nchunks, P, seeds, channels, demod, d_out, out_stride, n_out, d_last_in, d_last_out, h_taps, taps_length
-    if (decimation == 50 && taps_length <= 50 * 17) rc = launch_fused<50, 17>(CSDRB_DDC_ARGS, st);
-    else if (decimation == 10 && taps_length <= 10 * 8) rc = launch_fused<10, 8>(CSDRB_DDC_ARGS, st);
-    else if (decimation == 10 && taps_length <= 10 * 20) rc = launch_fused<10, 20>(CSDRB_DDC_ARGS, st);
-    else switch (ddc_bucket(decimation, taps_length)) {
-        case 4: rc = launch_generic<4>(CSDRB_DDC_ARGS, decimation, st); break;
-        case 8: rc = launch_generic<8>(CSDRB_DDC_ARGS, decimation, st); break;
-        case 12: rc = launch_generic<12>(CSDRB_DDC_ARGS, decimation, st); break;
-        case 17: rc = launch_generic<17>(CSDRB_DDC_ARGS, decimation, st); break;
-        case 20: rc = launch_generic<20>(CSDRB_DDC_ARGS, decimation, st); break;
-        case 24: rc = launch_generic<24>(CSDRB_DDC_ARGS, decimation, st); break;
+    bool done = false;
+    if constexpr (std::is_same_v<TIn, float2>) {
+        done = true;
+        if (decimation == 50 && taps_length <= 50 * 17) rc = launch_fused<50, 17>(CSDRB_DDC_ARGS, st);
+        else if (decimation == 10 && taps_length <= 10 * 8) rc = launch_fused<10, 8>(CSDRB_DDC_ARGS, st);
+        else if (decimation == 10 && taps_length <= 10 * 20) rc = launch_fused<10, 20>(CSDRB_DDC_ARGS, st);
+        else done = false;
+    }
+    if (!done) switch (ddc_bucket(decimation, taps_length)) {
+        case 4: rc = launch_generic<4, TIn>(CSDRB_DDC_ARGS, decimation, st); break;
+        case 8: rc = launch_generic<8, TIn>(CSDRB_DDC_ARGS, decimation, st); break;
+        case 12: rc = launch_generic<12, TIn>(CSDRB_DDC_ARGS, decimation, st); break;
+        case 17: rc = launch_generic<17, TIn>(CSDRB_DDC_ARGS, decimation, st); break;
+        case 20: rc = launch_generic<20, TIn>(CSDRB_DDC_ARGS, decimation, st); break;
+        case 24: rc = launch_generic<24, TIn>(CSDRB_DDC_ARGS, decimation, st); break;
     }
 #undef CSDRB_DDC_ARGS
     return rc < 0 ? rc : n_out;
 }
 
+int launch_ddc_main(const float2* d_wide, int input_size, int channels, const float* d_params, int chunk, int offset, int decimation,
+                    const float* h_taps, int taps_length, int demod, void* d_out, long out_stride, const float2* d_last_in, float2* d_last_out,
+                    const void* d_scratch, cudaStream_t st)
+{
+    return ddc_main(d_wide, input_size, channels, d_params, chunk, offset, decimation, h_taps, taps_length, demod, d_out, out_stride, d_last_in, d_last_out,
+                    d_scratch, st);
+}
+
+int launch_ddc_main_f(const float* d_wide, int input_size, int channels, const float* d_params, int chunk, int offset, int decimation,
+                      const float* h_taps, int taps_length, int demod, void* d_out, long out_stride, const float2* d_last_in, float2* d_last_out,
+                      const void* d_scratch, cudaStream_t st)
+{
+    return ddc_main(d_wide, input_size, channels, d_params, chunk, offset, decimation, h_taps, taps_length, demod, d_out, out_stride, d_last_in, d_last_out,
+                    d_scratch, st);
+}
+
 // one-shot: pre-pass and main kernel back to back on the caller's stream
-int launch_ddc_bank(const float2* d_wide, int input_size, int channels, const float* d_params, float* d_phase_io, int chunk, int offset,
+template <class TIn>
+static int ddc_bank(const TIn* d_wide, int input_size, int channels, const float* d_params, float* d_phase_io, int chunk, int offset,
                     int decimation, const float* h_taps, int taps_length, int demod, void* d_out, long out_stride,
                     const float2* d_last_in, float2* d_last_out, void* d_scratch, size_t scratch_bytes, int* launches, cudaStream_t st)
 {
     *launches = 0;
     if (channels <= 0 || decimation <= 0 || taps_length <= 0) { set_error("ddc bank: bad geometry"); return -1; }
-    if (reinterpret_cast<uintptr_t>(d_wide) & 15) { set_error("ddc bank: wideband input must be 16-byte aligned"); return -1; }
+    if (!ddc_wide_aligned(d_wide)) return -1;
     if (input_size >= taps_length) {                                    // a refused geometry launches nothing (and leaves d_phase_io alone)
         if (int rc = ddc_bank_geometry(decimation, taps_length); rc < 0) return rc;
     }
     int rc = launch_ddc_prepass(input_size, channels, d_params, d_phase_io, chunk, offset, decimation, taps_length, d_scratch, scratch_bytes, nullptr, st);
     if (rc <= 0) return rc;
     const int pre = rc;
-    rc = launch_ddc_main(d_wide, input_size, channels, d_params, chunk, offset, decimation, h_taps, taps_length, demod, d_out, out_stride, d_last_in, d_last_out, d_scratch, st);
+    rc = ddc_main(d_wide, input_size, channels, d_params, chunk, offset, decimation, h_taps, taps_length, demod, d_out, out_stride, d_last_in, d_last_out, d_scratch, st);
     if (rc < 0) return rc;
     *launches = pre + 1;
     return rc;
+}
+
+int launch_ddc_bank(const float2* d_wide, int input_size, int channels, const float* d_params, float* d_phase_io, int chunk, int offset,
+                    int decimation, const float* h_taps, int taps_length, int demod, void* d_out, long out_stride,
+                    const float2* d_last_in, float2* d_last_out, void* d_scratch, size_t scratch_bytes, int* launches, cudaStream_t st)
+{
+    return ddc_bank(d_wide, input_size, channels, d_params, d_phase_io, chunk, offset, decimation, h_taps, taps_length, demod, d_out, out_stride,
+                    d_last_in, d_last_out, d_scratch, scratch_bytes, launches, st);
+}
+
+int launch_ddc_bank_f(const float* d_wide, int input_size, int channels, const float* d_params, float* d_phase_io, int chunk, int offset,
+                      int decimation, const float* h_taps, int taps_length, int demod, void* d_out, long out_stride,
+                      const float2* d_last_in, float2* d_last_out, void* d_scratch, size_t scratch_bytes, int* launches, cudaStream_t st)
+{
+    return ddc_bank(d_wide, input_size, channels, d_params, d_phase_io, chunk, offset, decimation, h_taps, taps_length, demod, d_out, out_stride,
+                    d_last_in, d_last_out, d_scratch, scratch_bytes, launches, st);
 }
 
 }  // namespace csdrb

@@ -6,6 +6,7 @@
 #include "kernels.h"
 #include "csdr_b200.h"
 
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <mutex>
@@ -166,6 +167,30 @@ float shift_addition_cc(complexf* input, complexf* output, int input_size, shift
     const size_t sb = csdrb_shift_addition_bank_scratch_bytes(1, input_size, input_size);
     void* scratch = st.alloc<char>(sb);
     st.check(csdrb_shift_addition_bank_cc(d_in, 0, d_out, 0, 1, input_size, &d_s->params, &d_s->phase, input_size, scratch, sb, st.stream()));
+    st.get(output, d_out, input_size);
+    st.get(&s.phase, &d_s->phase, 1);
+    st.sync();
+    return s.phase;
+}
+
+// The reference BUILD seeds shift_addition_fc's phasor with one sincosf() of the float phase (-ffast-math narrows the source's cos/sin pair of
+// libcsdr_gpl.c:64-65 to it; objdump of the built libcsdr: `call sincosf@plt`), not with the double evaluation its shift_addition_cc keeps.  The
+// two differ by an ulp for a few per cent of phases, and the recursion carries that through the call, so the drop-in seeds the call on the host
+// with the same sincosf and gives the reference's bytes; the rest of the call is the bank kernel's.
+float shift_addition_fc(float* input, complexf* output, int input_size, shift_addition_data_t d, float starting_phase)
+{
+    if (input_size <= 0) return starting_phase;      // as shift_addition_cc above
+    Staging st("shift_addition_fc");
+    struct State { shift_addition_data_t params; float phase; float2 seed; } s = {d, starting_phase, {0.f, 0.f}};
+    sincosf(starting_phase, &s.seed.y, &s.seed.x);
+    State* d_s = st.up(&s, 1);
+    const float* d_in = st.up(input, input_size);
+    complexf* d_out = st.alloc<complexf>(input_size);
+    const size_t sb = csdrb_shift_addition_bank_scratch_bytes(1, input_size, input_size);
+    void* scratch = st.alloc<char>(sb);
+    const int rc = launch_shift_addition_fc_seeded(d_in, reinterpret_cast<float2*>(d_out), input_size, reinterpret_cast<const float*>(&d_s->params),
+                                                   &d_s->phase, &d_s->seed, scratch, sb, st.stream());
+    st.check(rc < 0 ? rc : counted(0, rc));
     st.get(output, d_out, input_size);
     st.get(&s.phase, &d_s->phase, 1);
     st.sync();

@@ -51,6 +51,12 @@ void shift_unroll_bank_single(const float2* d_in, float2* d_out, int n, const fl
 size_t shift_bank_scratch_bytes(int channels, int n, int chunk);
 int launch_shift_addition_bank(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n,
                                const float* d_params, float* d_phase_io, int chunk, void* d_scratch, size_t scratch_bytes, cudaStream_t st);
+// shift_addition_fc: real rows in (in_stride 0: every channel shifts the same row), complex rows out; the phase chain and scratch of the _cc bank
+int launch_shift_addition_bank_fc(const float* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n,
+                                  const float* d_params, float* d_phase_io, int chunk, void* d_scratch, size_t scratch_bytes, cudaStream_t st);
+// one shift_addition_fc call (n samples, one channel) whose phasor starts at *d_seed instead of (cos, sin) of *d_phase_io evaluated in double
+int launch_shift_addition_fc_seeded(const float* d_in, float2* d_out, int n, const float* d_params, float* d_phase_io, const float2* d_seed,
+                                    void* d_scratch, size_t scratch_bytes, cudaStream_t st);
 int launch_shift_addfast_bank(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n,
                               const float* d_params, float* d_phase_io, int chunk, void* d_scratch, size_t scratch_bytes, cudaStream_t st);
 size_t shift_math_scratch_bytes(int channels, int n);
@@ -165,5 +171,12 @@ int launch_ddc_main(const float2* d_wide, int input_size, int channels, const fl
 int launch_ddc_bank(const float2* d_wide, int input_size, int channels, const float* d_params, float* d_phase_io, int chunk, int offset,
                     int decimation, const float* h_taps, int taps_length, int demod, void* d_out, long out_stride,
                     const float2* d_last_in, float2* d_last_out, void* d_scratch, size_t scratch_bytes, int* launches, cudaStream_t st);
+// the same bank on real wideband samples (shift_addition_fc | fir_decimate_cc [| fmdemod_quadri_cf]): d_wide 8-byte aligned, same geometries and contract
+int launch_ddc_main_f(const float* d_wide, int input_size, int channels, const float* d_params, int chunk, int offset, int decimation,
+                      const float* h_taps, int taps_length, int demod, void* d_out, long out_stride, const float2* d_last_in, float2* d_last_out,
+                      const void* d_scratch, cudaStream_t st);
+int launch_ddc_bank_f(const float* d_wide, int input_size, int channels, const float* d_params, float* d_phase_io, int chunk, int offset,
+                      int decimation, const float* h_taps, int taps_length, int demod, void* d_out, long out_stride,
+                      const float2* d_last_in, float2* d_last_out, void* d_scratch, size_t scratch_bytes, int* launches, cudaStream_t st);
 
 }  // namespace csdrb

@@ -1,6 +1,7 @@
 // shift.cu -- K2: NCO frequency shift by phasor recursion, faithful to the reference's float arithmetic.
 //
-// Replaces shift_addition_cc (libcsdr_gpl.c:27-52) and decimating_shift_addition_cc (libcsdr_gpl.c:131-160).
+// Replaces shift_addition_cc (libcsdr_gpl.c:27-52), its real-input form shift_addition_fc (libcsdr_gpl.c:54-77) and decimating_shift_addition_cc
+// (libcsdr_gpl.c:131-160).
 //
 // The reference's result IS its rounding sequence (SURVEY.md section 7, hard part 2): inside one call the
 // phasor (cos phi, sin phi) is advanced by   c' = c*cosd - s*sind ;  s' = s*cosd + c*sind   in fp32 with
@@ -12,7 +13,7 @@
 // Kernels:
 //   shift_phase_chain_kernel : one warp per channel walks the chunk-to-chunk float phase chain
 //                              (sequential by definition, a few thousand steps) and stores each chunk's seed phase.
-//   shift_bank_kernel        : one lane per (channel, chunk) runs the <=chunk-step recursion; a warp owns 32
+//   shift_bank_kernel<TIn>   : one lane per (channel, chunk) runs the <=chunk-step recursion (complex or real input); a warp owns 32
 //                              consecutive chunks and moves data through a padded shared tile so that every
 //                              global access is a coalesced 256-byte row while each lane walks its own row.
 //   dshift_kernel            : decimating variant, one thread per channel (chains of a few hundred outputs).
@@ -23,6 +24,7 @@
 #include "kernels.h"
 #include "side_stream.cuh"
 #include <cstdlib>
+#include <type_traits>
 
 namespace csdrb {
 
@@ -73,20 +75,25 @@ shift_phase_chain_kernel(const float3* __restrict__ params, float* __restrict__ 
 
 constexpr int SH_TILE = 32;                       // samples per lane per sub-step
 
+// a wideband sample as the tile holds it: complex as it is, real x as (x, 0)
+__device__ __forceinline__ float2 tile_sample(float2 v) { return v; }
+__device__ __forceinline__ float2 tile_sample(float v) { return make_float2(v, 0.f); }
+
 // Load `rows` rows of 32 consecutive samples into the padded tile: row r covers stream positions (k0 + r)*seg + t0 .. +31 (zeros past the row's
 // length).  Eight rows' loads are issued before the first shared store -- a load-then-store loop serialises one DRAM/L2 round trip per row.
-__device__ __forceinline__ void tile_load_rows(float2* __restrict__ tile, const float2* __restrict__ x, int rows, int k0, int seg, int n, int t0, int lane, int pitch)
+template <class TIn>
+__device__ __forceinline__ void tile_load_rows(float2* __restrict__ tile, const TIn* __restrict__ x, int rows, int k0, int seg, int n, int t0, int lane, int pitch)
 {
     for (int r0 = 0; r0 < rows; r0 += 8) {
-        float2 v[8];
+        TIn v[8];
 #pragma unroll
         for (int u = 0; u < 8; u++) {
             const int r = r0 + u;
             const int len_r = r < rows ? min(seg, n - (k0 + r) * seg) : 0;
-            v[u] = (t0 + lane < len_r) ? x[(long)(k0 + r) * seg + t0 + lane] : make_float2(0.f, 0.f);
+            v[u] = (t0 + lane < len_r) ? x[(long)(k0 + r) * seg + t0 + lane] : TIn{};
         }
 #pragma unroll
-        for (int u = 0; u < 8; u++) if (r0 + u < rows) tile[(r0 + u) * pitch + lane] = v[u];
+        for (int u = 0; u < 8; u++) if (r0 + u < rows) tile[(r0 + u) * pitch + lane] = tile_sample(v[u]);
     }
 }
 constexpr int SH_PITCH = SH_TILE + 1;             // odd pitch in 8-byte units: row-wise walks are conflict-free
@@ -99,8 +106,9 @@ constexpr int SH_PITCH = SH_TILE + 1;             // odd pitch in 8-byte units: 
 // (Two double-buffered forms were slower than this one -- the tile of step t+1 arriving by 8-byte cp.async while step t is rotated: 32 x 32
 // tiles, 67 KB per CTA; 32 x 16 tiles in the same shared memory as here with the rotation in registers -- against this
 // plain load / rotate / store form with its 24 resident warps per SM.)
-template <int STEP, class MakeMixer>
-__device__ __forceinline__ void shift_tiled(const float2* __restrict__ in, long in_stride, float2* __restrict__ out, long out_stride,
+// `in` holds complex (float2) or real (float) samples; a real row lands in the tile as (x, 0), rows of 32 floats = 128-byte loads.
+template <int STEP, class TIn, class MakeMixer>
+__device__ __forceinline__ void shift_tiled(const TIn* __restrict__ in, long in_stride, float2* __restrict__ out, long out_stride,
                                             int n, int seg, int k_first, int k_end, int len_mask, MakeMixer make_mixer)
 {
     __shared__ float2 tile_all[4][32 * SH_PITCH];
@@ -109,7 +117,7 @@ __device__ __forceinline__ void shift_tiled(const float2* __restrict__ in, long 
     const int ch = blockIdx.y;
     const int k0 = k_first + (blockIdx.x * 4 + warp) * 32;    // first row of this warp
     if (k0 >= k_end) return;
-    const float2* x = in + (long)ch * in_stride;
+    const TIn* x = in + (long)ch * in_stride;
     float2* y = out + (long)ch * out_stride;
     const int k = k0 + lane;
     const bool live = k < k_end;
@@ -138,16 +146,26 @@ __device__ __forceinline__ void shift_tiled(const float2* __restrict__ in, long 
 // (cos, sin) of a float phase evaluated in double, as the reference seeds its phasor at each call
 __device__ __forceinline__ float2 seed_phasor(float ph) { return make_float2((float)cos((double)ph), (float)sin((double)ph)); }
 
+// TIn = float2: shift_addition_cc.  TIn = float: shift_addition_fc (libcsdr_gpl.c:54-77), the same recursion with the sample (cos phi * x, sin phi * x):
+// one rounded product per component.  `seeds` (may be null) overrides the phasor of each chunk: the shift_addition_fc drop-in hands in the
+// reference build's own seed, see dropin.cu.
+template <class TIn>
 __global__ void __launch_bounds__(128)
-shift_bank_kernel(const float2* __restrict__ in, long in_stride, float2* __restrict__ out, long out_stride,
-                  const float3* __restrict__ params, const float* __restrict__ chunk_phase, int n, int chunk, int nchunks, int k_first, int k_end)
+shift_bank_kernel(const TIn* __restrict__ in, long in_stride, float2* __restrict__ out, long out_stride,
+                  const float3* __restrict__ params, const float* __restrict__ chunk_phase, int n, int chunk, int nchunks, int k_first, int k_end,
+                  const float2* __restrict__ seeds)
 {
     // [k_first, k_end) is the launcher's slice of the chunk range
     shift_tiled<1>(in, in_stride, out, out_stride, n, chunk, k_first, k_end, ~0, [&](int ch, int k, bool live) {
         const float3 p = params[ch];
         const float2 d = make_float2(p.y, p.x);                         // (cosd, sind)
-        float2 ph = live ? seed_phasor(chunk_phase[(long)ch * nchunks + k]) : make_float2(0.f, 0.f);
-        return [=](float2* v) mutable { *v = rotate_rn(ph, *v); ph = rotate_rn(ph, d); };
+        const long i = (long)ch * nchunks + k;
+        float2 ph = !live ? make_float2(0.f, 0.f) : seeds ? seeds[i] : seed_phasor(chunk_phase[i]);
+        return [=](float2* v) mutable {
+            if constexpr (std::is_same_v<TIn, float>) *v = make_float2(__fmul_rn(ph.x, v->x), __fmul_rn(ph.y, v->x));
+            else *v = rotate_rn(ph, *v);
+            ph = rotate_rn(ph, d);
+        };
     });
 }
 
@@ -352,9 +370,11 @@ static inline WrapTable* chain_tables(void* d_scratch, size_t scratch_bytes, int
     return reinterpret_cast<WrapTable*>(static_cast<char*>(d_scratch) + phases);
 }
 
-int launch_shift_addition_bank(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n,
-                               const float* d_params /*[C][3] sindelta,cosdelta,rate*/, float* d_phase_io, int chunk,
-                               void* d_scratch, size_t scratch_bytes, cudaStream_t st)
+// shift_addition_cc (TIn = float2) and shift_addition_fc (TIn = float): the same phase chain, the same slices
+template <class TIn>
+static int launch_shift_bank(const TIn* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n,
+                             const float* d_params /*[C][3] sindelta,cosdelta,rate*/, float* d_phase_io, int chunk,
+                             void* d_scratch, size_t scratch_bytes, cudaStream_t st, const float2* d_seeds = nullptr)
 {
     if (channels <= 0 || n <= 0) return 0;
     if (chunk <= 0 || chunk > n) chunk = n;
@@ -377,7 +397,7 @@ int launch_shift_addition_bank(const float2* d_in, long in_stride, float2* d_out
     if (slices < 2) {
         shift_phase_chain_kernel<<<chain_ctas(channels, kShiftChainWarps), 32 * kShiftChainWarps, 0, st>>>(prm, d_phase_io, chunk_phase, channels, n, chunk, nchunks, tables, 0, nchunks);
         CSDRB_CUDA(cudaGetLastError());
-        shift_bank_kernel<<<dim3((nchunks + 127) / 128, channels), 128, smem, st>>>(d_in, in_stride, d_out, out_stride, prm, chunk_phase, n, chunk, nchunks, 0, nchunks);
+        shift_bank_kernel<TIn><<<dim3((nchunks + 127) / 128, channels), 128, smem, st>>>(d_in, in_stride, d_out, out_stride, prm, chunk_phase, n, chunk, nchunks, 0, nchunks, d_seeds);
         CSDRB_CUDA(cudaGetLastError());
         return 2;
     }
@@ -396,11 +416,29 @@ int launch_shift_addition_bank(const float2* d_in, long in_stride, float2* d_out
         CSDRB_CUDA(cudaGetLastError());
         CSDRB_CUDA(cudaEventRecord(ss->slice[i], ss->stream));
         CSDRB_CUDA(cudaStreamWaitEvent(st, ss->slice[i], 0));
-        shift_bank_kernel<<<dim3((k_end - k_first + 127) / 128, channels), 128, smem, st>>>(d_in, in_stride, d_out, out_stride, prm, chunk_phase, n, chunk, nchunks, k_first, k_end);
+        shift_bank_kernel<TIn><<<dim3((k_end - k_first + 127) / 128, channels), 128, smem, st>>>(d_in, in_stride, d_out, out_stride, prm, chunk_phase, n, chunk, nchunks, k_first, k_end, d_seeds);
         CSDRB_CUDA(cudaGetLastError());
         launches += 2;
     }
     return launches;
+}
+
+int launch_shift_addition_bank(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n,
+                               const float* d_params, float* d_phase_io, int chunk, void* d_scratch, size_t scratch_bytes, cudaStream_t st)
+{
+    return launch_shift_bank(d_in, in_stride, d_out, out_stride, channels, n, d_params, d_phase_io, chunk, d_scratch, scratch_bytes, st);
+}
+
+int launch_shift_addition_bank_fc(const float* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n,
+                                  const float* d_params, float* d_phase_io, int chunk, void* d_scratch, size_t scratch_bytes, cudaStream_t st)
+{
+    return launch_shift_bank(d_in, in_stride, d_out, out_stride, channels, n, d_params, d_phase_io, chunk, d_scratch, scratch_bytes, st);
+}
+
+int launch_shift_addition_fc_seeded(const float* d_in, float2* d_out, int n, const float* d_params, float* d_phase_io, const float2* d_seed,
+                                    void* d_scratch, size_t scratch_bytes, cudaStream_t st)
+{
+    return launch_shift_bank(d_in, 0, d_out, 0, 1, n, d_params, d_phase_io, n, d_scratch, scratch_bytes, st, d_seed);
 }
 
 int launch_shift_addfast_bank(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n,

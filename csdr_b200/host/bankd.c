@@ -12,7 +12,7 @@
  * as ONE continuous stream (the CLI's per-process block framing -- stale tail blocks at EOF, the zero block deemphasis_nfm_ff emits
  * first -- is process plumbing and is not reproduced; tests/test_gpu_zzz_bankd.py compares against the oracle run over the whole stream).
  *
- * usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]
+ * usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32|--s16|--real-s16|--real-f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]
  *                   [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty|wfm] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B] [--resample I:D[:BW]]
  *                   [--wfm-rate R] [--tau T]
  *                   [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]
@@ -46,6 +46,15 @@
  *   wideband rate / D is not 48 kHz, --resample I:D[:BW] puts rational_resampler_ff I D BW right behind the discriminator (tails nfm and none; see
  *   --help for the geometries it serves), e.g. 2.048 Msps with --decimation 32 --resample 3:4, or 10 Msps with --decimation 200 --resample 24:25:0.02.
  *   RATE  shift_addition_cc rate (fraction of the wideband sample rate), SINK a path (file or FIFO) or tcp:PORT (one listener).
+ *   Input formats: --u8 (default) rtl_sdr's unsigned 8-bit IQ, --f32 complex float, --s16 complex signed 16-bit (Airspy INT16_IQ, SDRplay, LimeSDR,
+ *   PlutoSDR; convert_s16_f in front of the complex bank), and REAL streams as direct-sampling receivers (RX888 / SDDC, Airspy real modes, ADC
+ *   boards) deliver them: --real-s16 (convert_s16_f) and --real-f32.  A real stream runs csdrb_ddc_bank_process_f, per channel
+ *     convert_s16_f | shift_addition_fc r | fir_decimate_cc D bw W | <tail>
+ *   and every tail works behind it.  A station at frequency f of a real stream sampled at fs is tuned with RATE = -f/fs (shift_addition_fc moves
+ *   it to 0 Hz); +f/fs selects its mirror image, the conjugate: sidebands swapped and the discriminator negated.  E.g. 7.074 MHz FT8 from an RX888 at
+ *   64.8 Msps, 48 kHz baseband: --real-s16 --decimation 1350 --bw 0.0008 --tail usb -0.10916667:ft8.s16.  --devices expands a real block to
+ *   x + 0j on the host and runs the complex multi-GPU bank (the same outputs); --waterfall needs complex input (a real stream's waterfall is
+ *   fft_fc, a real-to-complex transform this build does not have).
  *   --devices: the channels are sliced over several GPUs of this node (csdrb_multi_bank_*: the block goes to the first device once and on to
  *   the others by NCCL broadcast), one block of latency more (two blocks are kept in flight); the audio tail (nfm, am, usb, lsb), audio-rate work, runs on
  *   the first device for all channels, through the same kernels as without --devices; so do the bpsk31 and rtty decoders and the wfm tail.
@@ -732,7 +741,14 @@ static void bb_tail_push(bb_tail_t *t, channel_t *chan, int n_new, void *stream)
     t->have = rest;
 }
 
-static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *chan, int C, const float *rates, int D, const float *taps, int T, int block,
+/* wideband input formats (--u8 ...), their bytes per sample on the wire, whether the stream is real, and their names */
+enum { IN_U8, IN_F32, IN_S16, IN_REAL_S16, IN_REAL_F32 };
+static const int kWireBytes[] = {2, 8, 4, 2, 4};
+static const char *kFormatNames[] = {"u8", "f32", "s16", "real s16", "real f32"};
+static int format_is_real(int fmt) { return fmt == IN_REAL_S16 || fmt == IN_REAL_F32; }
+#define S16_RECIP (1.0f / 32767.0f)                       /* convert_s16_f: the reference build multiplies by the float reciprocal (csdrb_convert_s16_f) */
+
+static int run_multi(int in_fd, int fmt, const int *dev, int ndev, channel_t *chan, int C, const float *rates, int D, const float *taps, int T, int block,
                      int kind, float limit, float agc_ref, int rs_I, int rs_D, float rs_bw, int sps, const csdrb_serial_line_params_t *rtty_p, int rtty_B,
                      float wfm_rate, float tau, waterfall_t *wf, const waterfall_opts_t *wo)
 {
@@ -745,7 +761,7 @@ static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *cha
     for (int i = 0; i < 256; i++) lut[i] = (float)((float)i / (UCHAR_MAX / 2.0) - 1.0);      /* convert_u8_f, libcsdr.c:2365 */
     complexf *h_wide[2] = {csdrb_host_alloc(sizeof(complexf) * (size_t)block), csdrb_host_alloc(sizeof(complexf) * (size_t)block)};
     unsigned char *h_out[2] = {csdrb_host_alloc(osz * (size_t)C * (size_t)n_out), csdrb_host_alloc(osz * (size_t)C * (size_t)n_out)};
-    unsigned char *raw = malloc((size_t)block * 2);
+    unsigned char *raw = malloc((size_t)block * (size_t)kWireBytes[fmt]);
     if (!h_wide[0] || !h_wide[1] || !h_out[0] || !h_out[1] || !raw) die("out of memory");
     /* --tail nfm: the audio tail is audio-rate work (C x 48 kHz): the discriminator rows every device returned go to the FIRST device once more and through
      * the same kernels as in the single-GPU path */
@@ -815,10 +831,18 @@ static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *cha
         if (!first) memcpy(w, h_wide[slot ^ 1] + consumed, sizeof(complexf) * (size_t)keep);   /* the unconsumed tail (csdr.c:1172-1174) */
         complexf *dst = w + (first ? 0 : keep);
         int ok;
-        if (u8) {
-            ok = read_block(in_fd, raw, (size_t)fresh * 2);
-            if (ok) for (int i = 0; i < fresh; i++) { dst[i].i = lut[raw[2 * i]]; dst[i].q = lut[raw[2 * i + 1]]; }
-        } else ok = read_block(in_fd, (unsigned char *)dst, sizeof(complexf) * (size_t)fresh);
+        if (fmt == IN_F32) ok = read_block(in_fd, (unsigned char *)dst, sizeof(complexf) * (size_t)fresh);
+        else {                                                     /* converted on the host: real samples become x + 0j */
+            ok = read_block(in_fd, raw, (size_t)fresh * (size_t)kWireBytes[fmt]);
+            const short *s16 = (const short *)raw;
+            const float *f32 = (const float *)raw;
+            if (ok) for (int i = 0; i < fresh; i++) {
+                if (fmt == IN_U8) { dst[i].i = lut[raw[2 * i]]; dst[i].q = lut[raw[2 * i + 1]]; }
+                else if (fmt == IN_S16) { dst[i].i = (float)s16[2 * i] * S16_RECIP; dst[i].q = (float)s16[2 * i + 1] * S16_RECIP; }
+                else if (fmt == IN_REAL_S16) { dst[i].i = (float)s16[i] * S16_RECIP; dst[i].q = 0.0f; }
+                else { dst[i].i = f32[i]; dst[i].q = 0.0f; }
+            }
+        }
         if (!ok) break;
         if (wf) {
             OK(csdrb_copy_h2d(wf->d_in, dst, sizeof(complexf) * (size_t)fresh, wf_stream));
@@ -844,10 +868,18 @@ static int run_multi(int in_fd, int u8, const int *dev, int ndev, channel_t *cha
 static int usage(void)
 {
     fprintf(stderr,
-            "usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]\n"
+            "usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32|--s16|--real-s16|--real-f32] [--decimation D] [--bw TRANSITION_BW] [--window W]\n"
+            "                  [--block SAMPLES]\n"
             "                  [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty|wfm] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B]\n"
             "                  [--wfm-rate R] [--tau T] [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]\n"
             "                  RATE:SINK [RATE:SINK ...]\n"
+            "  --u8 | --f32 | --s16 the complex input: rtl_sdr's u8 IQ (default), complex float, or complex s16 (Airspy INT16_IQ, SDRplay, ...)\n"
+            "  --real-s16 | --real-f32  a REAL stream from a direct-sampling receiver (RX888 / SDDC, Airspy real modes, ADC boards): per channel\n"
+            "                       convert_s16_f | shift_addition_fc RATE | fir_decimate_cc D bw | <tail>.  A station at f Hz of a real stream\n"
+            "                       sampled at fs is tuned with RATE = -f/fs; +f/fs gives it conjugated (sidebands swapped, discriminator negated).\n"
+            "                       FT8 at 7.074 MHz from an RX888 at 64.8 Msps, 48 kHz baseband:\n"
+            "                       csdr-bankd --real-s16 --decimation 1350 --bw 0.0008 --tail usb -0.10916667:ft8.s16\n"
+            "                       Not with --waterfall (the waterfall of a real stream is fft_fc, which this build does not have).\n"
             "  --tail wfm           broadcast FM: per channel fmdemod_quadri_cf | fractional_decimator_ff R | deemphasis_wfm_ff 48000 T | convert_f_s16,\n"
             "                       in the CLI's calls of 1024 samples; the sinks get s16 audio.  --wfm-rate R (default 5, above 1 and at most 16)\n"
             "                       takes wideband/decimation to 48 kHz; --tau T (default 50e-6; 75e-6 in the Americas).  Not with --resample.\n"
@@ -884,7 +916,7 @@ static int usage(void)
 int main(int argc, char **argv)
 {
     const char *in_spec = "-", *tail = "nfm";
-    int u8 = 1, D = 50, block = 1 << 18, device = 0, ndev = 0, devs[64];
+    int fmt = IN_U8, D = 50, block = 1 << 18, device = 0, ndev = 0, devs[64];
     float bw = 0.005f, limit = 1.0f, agc_ref = 0.0f;                /* agc_ref 0: the tail's own default (fastagc_ff 1.0, agc_ff 0.2) */
     int rs_I = 0, rs_D = 0;                                          /* --resample I:D[:BW]; 0: no resampler */
     int sps = 0;                                                     /* --sps N of --tail bpsk31 */
@@ -903,8 +935,11 @@ int main(int argc, char **argv)
     for (int a = 1; a < argc; a++) {
         const char *o = argv[a];
         const char *v = a + 1 < argc ? argv[a + 1] : NULL;
-        if (!strcmp(o, "--u8")) u8 = 1;
-        else if (!strcmp(o, "--f32")) u8 = 0;
+        if (!strcmp(o, "--u8")) fmt = IN_U8;
+        else if (!strcmp(o, "--f32")) fmt = IN_F32;
+        else if (!strcmp(o, "--s16")) fmt = IN_S16;
+        else if (!strcmp(o, "--real-s16")) fmt = IN_REAL_S16;
+        else if (!strcmp(o, "--real-f32")) fmt = IN_REAL_F32;
         else if (!strcmp(o, "--in") && v) { in_spec = v; a++; }
         else if (!strcmp(o, "--decimation") && v) { D = atoi(v); a++; }
         else if (!strcmp(o, "--bw") && v) { bw = (float)atof(v); a++; }
@@ -992,6 +1027,8 @@ int main(int argc, char **argv)
             return 1;
         }
     }
+    const int real = format_is_real(fmt);
+    if (real && wf_sink) die("--waterfall needs a complex input: the waterfall of a real stream is fft_fc, a real-to-complex transform this build does not have");
     if (wf_opts && !wf_sink) die("--fft-size, --fft-every, --fft-averages, --fft-add-db, --fft-window and --fft-compression belong to --waterfall");
     waterfall_t wf;
     memset(&wf, 0, sizeof wf);
@@ -1017,8 +1054,8 @@ int main(int argc, char **argv)
         for (int c = 0; c < C; c++) { chan[c].fd = open_sink(chan[c].sink); sink_nonblocking(chan[c].fd); }
         if (wf_sink) { wf.sink.fd = open_sink(wf_sink); sink_nonblocking(wf.sink.fd); }
         const int fd = open_input(in_spec);
-        fprintf(stderr, "csdr-bankd: %d channels over %d devices, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, ndev, D, T, u8 ? "u8" : "f32", block, tail);
-        const int rc = run_multi(fd, u8, devs, ndev, chan, C, rates, D, taps, T, block, kind, limit, agc_ref, rs_I, rs_D, rs_bw, sps, &rtty_p, rtty_B,
+        fprintf(stderr, "csdr-bankd: %d channels over %d devices, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, ndev, D, T, kFormatNames[fmt], block, tail);
+        const int rc = run_multi(fd, fmt, devs, ndev, chan, C, rates, D, taps, T, block, kind, limit, agc_ref, rs_I, rs_D, rs_bw, sps, &rtty_p, rtty_B,
                                  wfm_rate, tau, wf_sink ? &wf : NULL, &wo);
         for (int c = 0; c < C; c++) { if (chan[c].dropped) fprintf(stderr, "csdr-bankd: sink %s lost %ld bytes (too slow)\n", chan[c].sink, chan[c].dropped); if (chan[c].fd >= 0) close(chan[c].fd); }
         if (wf_sink) waterfall_report(&wf);
@@ -1031,13 +1068,17 @@ int main(int argc, char **argv)
     if (!stream) die("cannot create a stream");
 
     /* ---- buffers ----------------------------------------------------------------------------------------------------------------
-     * wide[2]  : [tail of the previous block | new block] cf32, ping-pong so the tail copy never overlaps
+     * wide[2]  : [tail of the previous block | new block] cf32 (f32 for a real input), ping-pong so the tail copy never overlaps
+     * raw      : the block as it arrived, for the formats converted on the device; stage: real s16 converted where the block lands unaligned
      * with the NFM tail the discriminator output goes straight into nfm_tail_t's demod rows; without it into a plain [C][ds] array */
-    const size_t in_bytes = (size_t)block * (u8 ? 2 : 8);
+    const size_t in_bytes = (size_t)block * (size_t)kWireBytes[fmt];
+    const size_t ssz = real ? sizeof(float) : sizeof(complexf);   /* one wideband sample on the device */
     unsigned char *h_in = csdrb_host_alloc(in_bytes);
     const int wide_cap = block + T + D + 16;
-    complexf *d_wide[2] = {csdrb_device_alloc(sizeof(complexf) * (size_t)wide_cap), csdrb_device_alloc(sizeof(complexf) * (size_t)wide_cap)};
-    unsigned char *d_raw = u8 ? csdrb_device_alloc(in_bytes + 16) : NULL;
+    unsigned char *d_wide[2] = {csdrb_device_alloc(ssz * (size_t)wide_cap), csdrb_device_alloc(ssz * (size_t)wide_cap)};
+    const int raw_in = fmt == IN_U8 || fmt == IN_S16 || fmt == IN_REAL_S16;
+    unsigned char *d_raw = raw_in ? csdrb_device_alloc(in_bytes + 16) : NULL;
+    float *d_stage = fmt == IN_REAL_S16 ? csdrb_device_alloc(sizeof(float) * (size_t)block + 16) : NULL;
     const int out_cap = wide_cap / D + 2;                          /* discriminator samples one block can add */
     nfm_tail_t tl;
     bb_tail_t bb;
@@ -1057,7 +1098,7 @@ int main(int argc, char **argv)
         d_demod = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)ds);
         h_out = csdrb_host_alloc((size_t)C * (size_t)ds * sizeof(float));
     }
-    if (!h_in || !d_wide[0] || !d_wide[1] || (u8 && !d_raw) || !d_demod || (kind == TAIL_NONE && !h_out)) die("out of memory");
+    if (!h_in || !d_wide[0] || !d_wide[1] || (raw_in && !d_raw) || (fmt == IN_REAL_S16 && !d_stage) || !d_demod || (kind == TAIL_NONE && !h_out)) die("out of memory");
 
     /* sinks last: tcp: sinks block until their listener arrives */
     for (int c = 0; c < C; c++) { chan[c].fd = open_sink(chan[c].sink); sink_nonblocking(chan[c].fd); }
@@ -1066,7 +1107,7 @@ int main(int argc, char **argv)
         wf.sink.fd = open_sink(wf_sink); sink_nonblocking(wf.sink.fd);
     }
     const int in_fd = open_input(in_spec);
-    fprintf(stderr, "csdr-bankd: %d channels, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, D, T, u8 ? "u8" : "f32", block, tail);
+    fprintf(stderr, "csdr-bankd: %d channels, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, D, T, kFormatNames[fmt], block, tail);
 
     int cur = 0, keep = 0;
     long blocks = 0;
@@ -1075,25 +1116,31 @@ int main(int argc, char **argv)
      * block % D made it miss, and re-run inline, on most blocks). */
     for (;;) {
         const int fresh_n = block - keep;                            /* first block: everything; later: what the last call consumed (even) */
-        const size_t fresh_bytes = (size_t)fresh_n * (u8 ? 2 : 8);
+        const size_t fresh_bytes = (size_t)fresh_n * (size_t)kWireBytes[fmt];
         if (!read_block(in_fd, h_in, fresh_bytes)) break;
-        /* 1. the new samples land behind the unconsumed tail (keep is even because block and D are: 16-byte alignment holds) */
-        complexf *fresh = d_wide[cur] + keep;
-        if (u8) {
-            OK(csdrb_copy_h2d(d_raw, h_in, fresh_bytes, stream));
-            OK(csdrb_convert_u8_f(d_raw, (float *)fresh, 2L * fresh_n, stream));
+        /* 1. the new samples land behind the unconsumed tail.  keep is even because block and D are: 16-byte alignment holds for complex samples,
+         *    but a real block can land 8 bytes off, where convert_s16_f (16-byte aligned buffers) converts into the stage and the block is copied */
+        float *fresh = (float *)(d_wide[cur] + ssz * (size_t)keep);
+        if (raw_in) OK(csdrb_copy_h2d(d_raw, h_in, fresh_bytes, stream));
+        if (fmt == IN_U8) OK(csdrb_convert_u8_f(d_raw, fresh, 2L * fresh_n, stream));
+        else if (fmt == IN_S16) OK(csdrb_convert_s16_f((const short *)d_raw, fresh, 2L * fresh_n, stream));
+        else if (fmt == IN_REAL_S16 && !((size_t)fresh & 15)) OK(csdrb_convert_s16_f((const short *)d_raw, fresh, fresh_n, stream));
+        else if (fmt == IN_REAL_S16) {
+            OK(csdrb_convert_s16_f((const short *)d_raw, d_stage, fresh_n, stream));
+            OK(csdrb_copy_d2d(fresh, d_stage, sizeof(float) * (size_t)fresh_n, stream));
         } else OK(csdrb_copy_h2d(fresh, h_in, fresh_bytes, stream));
-        if (wf_sink) waterfall_push(&wf, fresh, fresh_n, stream);   /* the waterfall of the same samples, lines to its sink */
+        if (wf_sink) waterfall_push(&wf, (const complexf *)fresh, fresh_n, stream);   /* the waterfall of the same samples, lines to its sink */
         const int n_in = block;
 
         /* 2. shift | fir_decimate | fmdemod for every channel, new discriminator samples behind the de-emphasis FIR's carried inputs */
         void *dst = resample ? (void *)(rsm.d_in + rsm.have) : nfm ? (void *)(d_demod + tl.a_have) : rtty ? (void *)(rt.d_rows + rt.end)
                   : wfm ? (void *)(wt.d_rows + wt.have) : !demod ? (void *)(bb.d_bb + bb.have) : (void *)d_demod;
-        const int n_out = csdrb_ddc_bank_process(bank, d_wide[cur], n_in, dst, resample ? rsm.rs : ds, stream);
+        const int n_out = real ? csdrb_ddc_bank_process_f(bank, (const float *)d_wide[cur], n_in, dst, resample ? rsm.rs : ds, stream)
+                               : csdrb_ddc_bank_process(bank, (const complexf *)d_wide[cur], n_in, dst, resample ? rsm.rs : ds, stream);
         if (n_out < 0) die("csdrb_ddc_bank_process failed");
         const int consumed = n_out * D;
         keep = n_in - consumed;
-        OK(csdrb_copy_d2d(d_wide[cur ^ 1], d_wide[cur] + consumed, sizeof(complexf) * (size_t)keep, stream));
+        OK(csdrb_copy_d2d(d_wide[cur ^ 1], d_wide[cur] + ssz * (size_t)consumed, ssz * (size_t)keep, stream));
         cur ^= 1;
 
         /* 2b. --resample: the new discriminator samples through rational_resampler_ff, into the tail's rows */

@@ -192,6 +192,36 @@ static int cmd_shift_addition_cc(int argc, char **argv)
     }
 }
 
+/* csdr.c:3365-3410: cmd_shift_addition_cc with real input -- the big buffer, 1024-sample calls, the stop on an empty read and the retune
+ * between buffers are the same; only the input is one float per sample */
+static int cmd_shift_addition_fc(int argc, char **argv)
+{
+    G.wideband = 1;
+    float phase = 0, rate = 0;
+    int ctl = open_control(argc, argv);
+    if (ctl) { while (!poll_control(ctl, "%g\n", &rate)) usleep(10000); }
+    else { if (argc <= 2) return complain("need required parameter (rate)"); sscanf(argv[2], "%g", &rate); }
+    if (!announce_block(open_block())) return -2;
+    float *in = must_alloc(sizeof(float) * (size_t)block);
+    complexf *out = must_alloc(sizeof(complexf) * (size_t)block);
+    for (;;) {
+        shift_addition_data_t nco = shift_addition_init(rate);
+        who(); fprintf(stderr, "reinitialized to %g\n", rate);
+        for (;;) {
+            if (feof(stdin)) return 0;
+            if (!fread(in, sizeof(float), (size_t)block, stdin)) break;
+            for (int done = 0; done < block;) {
+                int n = block - done > 1024 ? 1024 : block - done;
+                phase = shift_addition_fc(in + done, out + done, n, nco, phase);
+                done += n;
+            }
+            fwrite(out, sizeof(complexf), (size_t)block, stdout);
+            if (poll_control(ctl, "%g\n", &rate)) break;
+            end_of_block();
+        }
+    }
+}
+
 static int cmd_fir_decimate_cc(int argc, char **argv)
 {
     G.wideband = 1;
@@ -976,6 +1006,7 @@ static const struct { const char *name; int (*run)(int, char **); const char *sy
     {"convert_f_s16", cmd_convert_f_s16, "convert_f_s16"},
     {"convert_f_i16", cmd_convert_f_s16, "convert_f_i16"},
     {"shift_addition_cc", cmd_shift_addition_cc, "shift_addition_cc <rate> | --fifo <fifo_path> | --fd <fd>"},
+    {"shift_addition_fc", cmd_shift_addition_fc, "shift_addition_fc <rate> | --fifo <fifo_path> | --fd <fd>"},
     {"fir_decimate_cc", cmd_fir_decimate_cc, "fir_decimate_cc <decimation_factor> [transition_bw [window]]"},
     {"fmdemod_quadri_cf", cmd_fmdemod_quadri_cf, "fmdemod_quadri_cf"},
     {"fractional_decimator_ff", cmd_fractional_decimator_ff, "fractional_decimator_ff <decimation_rate> [num_poly_points ( [transition_bw [window]] | --prefilter )]"},

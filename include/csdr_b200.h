@@ -57,6 +57,8 @@ void convert_f_i16(float *input, short *output, int input_size);
 typedef struct shift_addition_data_s { float sindelta; float cosdelta; float rate; } shift_addition_data_t;
 shift_addition_data_t shift_addition_init(float rate);
 float shift_addition_cc(complexf *input, complexf *output, int input_size, shift_addition_data_t d, float starting_phase);
+/* real input (libcsdr_gpl.h; libcsdr_gpl.c:54-77): output[i] = (cos phi * input[i], sin phi * input[i]), the same phasor recursion and returned phase */
+float shift_addition_fc(float *input, complexf *output, int input_size, shift_addition_data_t d, float starting_phase);
 typedef struct decimating_shift_addition_status_s { int decimation_remain; float starting_phase; int output_size; } decimating_shift_addition_status_t;
 shift_addition_data_t decimating_shift_addition_init(float rate, int decimation);
 decimating_shift_addition_status_t decimating_shift_addition_cc(complexf *input, complexf *output, int input_size,
@@ -260,6 +262,12 @@ size_t csdrb_shift_addition_bank_scratch_bytes(int channels, int input_size, int
 int csdrb_shift_addition_bank_cc(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int input_size,
                                  const shift_addition_data_t *d_params, float *d_phase_io, int chunk,
                                  void *d_scratch, size_t scratch_bytes, void *stream);
+/* shift_addition_fc bank: real rows in (d_in + c*in_stride floats; in_stride == 0: every channel shifts the SAME real wideband row, e.g. a
+ * direct-sampling receiver's stream), complexf rows out; d_params, d_phase_io, chunk and scratch (csdrb_shift_addition_bank_scratch_bytes) as above.
+ * Output and returned phase equal the reference's shift_addition_fc called once per chunk, bit for bit. */
+int csdrb_shift_addition_bank_fc(const float *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int input_size,
+                                 const shift_addition_data_t *d_params, float *d_phase_io, int chunk,
+                                 void *d_scratch, size_t scratch_bytes, void *stream);
 int csdrb_decimating_shift_addition_bank_cc(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int channels,
                                             int input_size, const shift_addition_data_t *d_params, int decimation,
                                             int *d_remain_io, float *d_phase_io, int *d_out_size, void *stream);
@@ -281,6 +289,13 @@ size_t csdrb_ddc_bank_scratch_bytes(int channels, int input_size, int chunk, int
 int csdrb_ddc_bank(const complexf *d_wide, int input_size, int channels, const shift_addition_data_t *d_params, float *d_phase_io,
                    int chunk, int offset, int decimation, const float *h_taps, int taps_length, int demod, void *d_out, long out_stride,
                    const complexf *d_last_in, complexf *d_last_out, void *d_scratch, size_t scratch_bytes, void *stream);
+/* The same bank on a REAL wideband stream = shift_addition_fc(rate_c) | fir_decimate_cc(D, taps) [| fmdemod_quadri_cf]: same arguments, served
+ * geometries, return codes and scratch size; d_wide is 8-byte aligned (any even sample of a 16-byte aligned buffer; otherwise -1 and a message).
+ * On x it gives the complex bank's outputs on x + 0j (equal float values: a zero may differ in sign) and the same carried phases, bit for bit.
+ * A station at frequency f of a real stream sampled at fs is tuned with rate -f/fs; +f/fs gives its conjugate (sidebands swapped). */
+int csdrb_ddc_bank_f(const float *d_wide, int input_size, int channels, const shift_addition_data_t *d_params, float *d_phase_io,
+                     int chunk, int offset, int decimation, const float *h_taps, int taps_length, int demod, void *d_out, long out_stride,
+                     const complexf *d_last_in, complexf *d_last_out, void *d_scratch, size_t scratch_bytes, void *stream);
 
 /* Streaming bank object over the fused kernel: owns rates, chunk phases, discriminator history and the position inside the current
  * NCO chunk, so a wideband stream is processed with one call per block; internally the serial phase-chain pre-pass of block k+1 runs on
@@ -298,6 +313,8 @@ int  csdrb_ddc_bank_set_rate(csdrb_ddc_bank_t *bank, int channel, float rate);
 int  csdrb_ddc_bank_rechunk(csdrb_ddc_bank_t *bank);                               /* close the NCO chunk at the next block's first sample, rates unchanged */
 int  csdrb_ddc_bank_offset(const csdrb_ddc_bank_t *bank);                          /* samples of the current NCO chunk already consumed */
 int  csdrb_ddc_bank_process(csdrb_ddc_bank_t *bank, const complexf *d_wide, int input_size, void *d_out, long out_stride, void *stream);
+/* the same with a block of real samples (csdrb_ddc_bank_f's kernel and alignment); block contract, set_rate, rechunk and offset as above */
+int  csdrb_ddc_bank_process_f(csdrb_ddc_bank_t *bank, const float *d_wide, int input_size, void *d_out, long out_stride, void *stream);
 
 /* The same bank sliced over several GPUs of one node, driven from ONE process (what nmux + one process chain per channel do in the reference,
  * nmux.cpp:246-353, ddcd_old.h:51-57): contiguous channel slices per device, the wideband block goes host -> devices[0] once and on to the other
