@@ -180,6 +180,31 @@ static void write_sink(channel_t *ch, const void *data, size_t bytes)
     }
 }
 
+/* row c of the host rows at h (pitch bytes apart) to sink c: the whole row, or its first counts[c] bytes when counts is given */
+static void write_rows(channel_t *chan, int C, const unsigned char *h, size_t pitch, const int *counts)
+{
+    for (int c = 0; c < C; c++) write_sink(&chan[c], h + pitch * (size_t)c, counts ? (size_t)(counts[c] > 0 ? counts[c] : 0) : pitch);
+}
+
+/* each of the C device rows at d_rows (pitch samples of esz bytes) keeps its n samples from `from` on, moved to the front through d_carry
+ * (at least C x n samples): two copies on the stream, no synchronisation */
+static void rows_to_front(void *d_rows, long pitch, int from, int n, size_t esz, void *d_carry, int C, void *stream)
+{
+    unsigned char *rows = d_rows;
+    const size_t width = esz * (size_t)n;
+    OK(csdrb_copy2d_d2d(d_carry, width, rows + esz * (size_t)from, esz * (size_t)pitch, width, (size_t)C, stream));
+    OK(csdrb_copy2d_d2d(rows, esz * (size_t)pitch, d_carry, width, width, (size_t)C, stream));
+}
+
+/* a new stream on device dev, which stays the current device */
+static void *device_stream(int dev)
+{
+    OK(csdrb_set_device(dev));
+    void *stream = csdrb_stream_create();
+    if (!stream) die("cannot create a stream");
+    return stream;
+}
+
 /* ---- several GPUs: csdrb_multi_bank, raw discriminator output ------------------------------------------------------------------------ */
 static int parse_devices(const char *list, int *dev, int max)
 {
@@ -193,7 +218,6 @@ static int parse_devices(const char *list, int *dev, int max)
     }
     return n;
 }
-
 
 /* ---- the NFM audio tail of README.md:87 behind the discriminator: limit_ff | deemphasis_nfm_ff 48000 | fastagc_ff | convert_f_s16 ------------------------
  * Device buffers of ONE device (the single-GPU path's own, the first device of --devices):
@@ -216,7 +240,6 @@ typedef struct {
 
 static void nfm_tail_init(nfm_tail_t *t, int C, int out_cap, float limit, float agc_ref)
 {
-    memset(t, 0, sizeof *t);
     t->C = C; t->limit = limit; t->agc_ref = agc_ref;
     if (!csdrb_deemphasis_nfm_taps(NFM_RATE, &t->Tn)) die("no de-emphasis table");
     t->ds = ((long)t->Tn + out_cap + 3) & ~3L;
@@ -244,8 +267,7 @@ static void nfm_tail_push(nfm_tail_t *t, channel_t *chan, int n_new, void *strea
     if (a_n > Tn) {
         m = csdrb_deemphasis_nfm_bank_ff(t->d_demod, ds, t->d_agc_in + t->g_have, gs, C, a_n, NFM_RATE, t->limit, stream);
         if (m < 0) die("csdrb_deemphasis_nfm_bank_ff failed");
-        OK(csdrb_copy2d_d2d(t->d_carry, sizeof(float) * (size_t)Tn, t->d_demod + m, sizeof(float) * (size_t)ds, sizeof(float) * (size_t)Tn, (size_t)C, stream));
-        OK(csdrb_copy2d_d2d(t->d_demod, sizeof(float) * (size_t)ds, t->d_carry, sizeof(float) * (size_t)Tn, sizeof(float) * (size_t)Tn, (size_t)C, stream));
+        rows_to_front(t->d_demod, ds, m, Tn, sizeof(float), t->d_carry, C, stream);
         t->a_have = Tn;
     } else t->a_have = a_n;
     /* fastagc_ff over the whole AGC blocks available, then convert_f_s16 (one pass); the remainder waits for the next block */
@@ -254,11 +276,10 @@ static void nfm_tail_push(nfm_tail_t *t, channel_t *chan, int n_new, void *strea
         OK(csdrb_fastagc_bank_f_s16(t->d_agc_in, gs, t->d_pcm, whole, C, AGC_BLOCK, nb, t->agc_ref, t->d_agc_state, t->d_agc_hist, t->d_agc_scratch, t->agc_sb + 16, stream));
         OK(csdrb_copy_d2h(t->h_out, t->d_pcm, sizeof(short) * (size_t)C * (size_t)whole, stream));
         const int rest = g_n - whole;
-        OK(csdrb_copy2d_d2d(t->d_carry, sizeof(float) * (size_t)AGC_BLOCK, t->d_agc_in + whole, sizeof(float) * (size_t)gs, sizeof(float) * (size_t)rest, (size_t)C, stream));
-        OK(csdrb_copy2d_d2d(t->d_agc_in, sizeof(float) * (size_t)gs, t->d_carry, sizeof(float) * (size_t)AGC_BLOCK, sizeof(float) * (size_t)rest, (size_t)C, stream));
+        rows_to_front(t->d_agc_in, gs, whole, rest, sizeof(float), t->d_carry, C, stream);
         t->g_have = rest;
         OK(csdrb_stream_synchronize(stream));
-        for (int c = 0; c < C; c++) write_sink(&chan[c], t->h_out + sizeof(short) * (size_t)c * (size_t)whole, sizeof(short) * (size_t)whole);
+        write_rows(chan, C, t->h_out, sizeof(short) * (size_t)whole, NULL);
     } else {
         t->g_have = g_n;
         OK(csdrb_stream_synchronize(stream));
@@ -282,7 +303,6 @@ static int resample_geometry_ok(int I, int D, int T) { return (long)(T / I + 1) 
 
 static void rs_init(rs_stage_t *r, int C, int I, int D, float bw, int in_cap)
 {
-    memset(r, 0, sizeof *r);
     r->C = C; r->I = I; r->D = D; r->T = firdes_filter_len(bw);
     r->taps = malloc(sizeof(float) * (size_t)r->T);
     if (!r->taps) die("out of memory");
@@ -306,45 +326,130 @@ static int rs_push(rs_stage_t *r, int n_new, float *dst, long dst_pitch, void *s
     const int m = csdrb_rational_resampler_bank_ff(r->d_in, r->rs, dst, dst_pitch, r->C, n, r->I, r->D, r->taps, r->T, r->ltd, &st, stream);
     if (m < 0) die("csdrb_rational_resampler_bank_ff failed");
     const int keep = n - st.input_processed;
-    if (keep > 0 && st.input_processed > 0) {
-        const size_t row = sizeof(float) * (size_t)r->rs;
-        OK(csdrb_copy2d_d2d(r->d_carry, row, r->d_in + st.input_processed, row, sizeof(float) * (size_t)keep, (size_t)r->C, stream));
-        OK(csdrb_copy2d_d2d(r->d_in, row, r->d_carry, row, sizeof(float) * (size_t)keep, (size_t)r->C, stream));
-    }
+    if (keep > 0 && st.input_processed > 0) rows_to_front(r->d_in, r->rs, st.input_processed, keep, sizeof(float), r->d_carry, r->C, stream);
     r->have = keep; r->ltd = st.last_taps_delay;
     return m;
 }
 
-/* --tail none: n float samples per channel (device rows, pitch `pitch`) to the sinks */
-static void raw_emit(const float *d_rows, long pitch, int n, unsigned char *h_out, channel_t *chan, int C, void *stream)
+/* ---- --tail none and --tail iq: the bank's output itself, the discriminator (float) or the complex baseband (cf32) -----------------------------
+ *   rows : [C][pitch] samples of esz bytes, the new ones from the front of every row; nothing is held back */
+typedef struct { int C; size_t esz; long pitch; unsigned char *d_rows, *h_out; } raw_tail_t;
+
+static void raw_tail_init(raw_tail_t *t, int C, int in_cap, size_t esz)
 {
-    OK(csdrb_copy2d_d2h(h_out, sizeof(float) * (size_t)n, d_rows, sizeof(float) * (size_t)pitch, sizeof(float) * (size_t)n, (size_t)C, stream));
+    t->C = C; t->esz = esz; t->pitch = ((long)in_cap + 3) & ~3L;
+    t->d_rows = csdrb_device_alloc(esz * (size_t)C * (size_t)t->pitch);
+    t->h_out = csdrb_host_alloc(esz * (size_t)C * (size_t)t->pitch);
+    if (!t->d_rows || !t->h_out) die("out of memory");
+}
+
+/* n new samples per channel at the front of d_rows to the sinks */
+static void raw_tail_push(raw_tail_t *t, channel_t *chan, int n, void *stream)
+{
+    const size_t width = t->esz * (size_t)n;
+    OK(csdrb_copy2d_d2h(t->h_out, width, t->d_rows, t->esz * (size_t)t->pitch, width, (size_t)t->C, stream));
     OK(csdrb_stream_synchronize(stream));
-    for (int c = 0; c < C; c++) write_sink(&chan[c], h_out + sizeof(float) * (size_t)c * (size_t)n, sizeof(float) * (size_t)n);
+    write_rows(chan, t->C, t->h_out, width, NULL);
 }
 
 /* ---- the AM and SSB audio tails (README.md:95, :110) behind the DDC bank's complex baseband ------------------------------------------------------------------
  *   am      : amdemod_cf | fastdcblock_ff 1024 | agc_ff | limit_ff L | convert_f_s16
  *   usb/lsb : bandpass_fir_fft_cc 0 0.1 0.05 (or -0.1 0 0.05) | realpart_cf | agc_ff | limit_ff L | convert_f_s16
- *   iq      : the baseband itself, cf32 (what either tail starts from)
  * agc_ff runs with the CLI defaults (csdr.c:1342-1361) and its 1024-sample calls; --agc-ref overrides the reference.  Device buffers of ONE device:
  *   bb   : [C][bs] complexf : [remainder (< unit samples) | new baseband]   unit = 1024 (am) or the overlap-add input size (usb/lsb)
  *   mid  : [C][bs] float (am: DC-blocked envelope) or complexf (usb/lsb: filtered baseband) over the whole units
  *   pcm  : [C][whole] s16 */
 #define SSB_BW 0.05f                                      /* bandpass_fir_fft_cc transition bandwidth of README.md:110 */
-enum { TAIL_NFM, TAIL_NONE, TAIL_IQ, TAIL_AM, TAIL_USB, TAIL_LSB, TAIL_BPSK31, TAIL_RTTY, TAIL_WFM };
+
+typedef struct {
+    int C, unit, have, fft_size;                                  /* fft_size 0: am, else the usb/lsb bandpass */
+    long bs;
+    float limit;
+    csdrb_agc_params_t agc;
+    complexf *d_bb, *d_carry, *d_taps_fft, *d_ola_tail;
+    void *d_mid;
+    short *d_pcm;
+    float *d_last_dc;
+    csdrb_agc_state_t *d_agc_state;
+    unsigned char *h_out;
+} bb_tail_t;
+
+/* band: the usb or lsb bandpass edges {lo, hi}; NULL for am */
+static void bb_tail_init(bb_tail_t *t, int C, int out_cap, float limit, float agc_ref, const float *band, void *stream)
+{
+    t->C = C; t->limit = limit;
+    const csdrb_agc_params_t p = {agc_ref, 0.01f, 0.0001f, 65536.0f, 200, 0, 0.999f, 1024};
+    t->agc = p;
+    t->unit = 1024;
+    if (band) {                                                      /* bandpass_fir_fft_cc geometry, csdr.c:1822-1831 */
+        const int T = firdes_filter_len(SSB_BW);
+        int N = next_pow2(T);
+        if (N - T < 200) N <<= 1;
+        t->fft_size = N; t->unit = N - T + 1;
+        complexf *h_taps = calloc((size_t)N, sizeof(complexf));
+        if (!h_taps) die("out of memory");
+        firdes_bandpass_c(h_taps, T, band[0], band[1], WINDOW_HAMMING);
+        complexf *d_taps = csdrb_device_alloc(sizeof(complexf) * (size_t)N);
+        t->d_taps_fft = csdrb_device_alloc(sizeof(complexf) * (size_t)N);
+        t->d_ola_tail = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)N);   /* zero-filled: the overlap tail is zero at stream start (csdr.c:1860) */
+        if (!d_taps || !t->d_taps_fft || !t->d_ola_tail) die("out of memory");
+        OK(csdrb_copy_h2d(d_taps, h_taps, sizeof(complexf) * (size_t)N, stream));
+        OK(csdrb_fft_c2c_batch(d_taps, N, t->d_taps_fft, N, N, 1, 0, stream));       /* the forward FFT of the zero-padded taps (csdr.c:1869) */
+        OK(csdrb_stream_synchronize(stream));
+        csdrb_device_free(d_taps); free(h_taps);
+    }
+    t->bs = ((long)t->unit + out_cap + 3) & ~3L;
+    t->d_bb = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->bs);
+    t->d_carry = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->unit);
+    t->d_mid = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->bs);
+    t->d_pcm = csdrb_device_alloc(sizeof(short) * (size_t)C * (size_t)t->bs + 16);
+    t->d_last_dc = csdrb_device_alloc(sizeof(float) * (size_t)C);                  /* zero-filled: last_dc_level starts at 0 (csdr.c:957) */
+    t->d_agc_state = csdrb_device_alloc(sizeof(csdrb_agc_state_t) * (size_t)C);
+    t->h_out = csdrb_host_alloc((size_t)C * (size_t)t->bs * sizeof(complexf));
+    if (!t->d_bb || !t->d_carry || !t->d_mid || !t->d_pcm || !t->d_last_dc || !t->d_agc_state || !t->h_out) die("out of memory");
+    csdrb_agc_state_t *h_st = calloc((size_t)C, sizeof *h_st);
+    if (!h_st) die("out of memory");
+    for (int c = 0; c < C; c++) h_st[c].gain = 1.0f;                 /* a stream starts at gain 1 (csdr.c:1363) */
+    OK(csdrb_copy_h2d(t->d_agc_state, h_st, sizeof *h_st * (size_t)C, stream));
+    OK(csdrb_stream_synchronize(stream));
+    free(h_st);
+}
+
+/* n_new fresh baseband samples per channel sit at d_bb + have: run the tail over the whole units, audio to the sinks, keep the remainder */
+static void bb_tail_push(bb_tail_t *t, channel_t *chan, int n_new, void *stream)
+{
+    const int C = t->C;
+    const long bs = t->bs;
+    const int n = t->have + n_new;
+    const int nb = n / t->unit, whole = nb * t->unit, rest = n - whole;
+    if (nb > 0) {
+        if (!t->fft_size) {
+            OK(csdrb_fastdcblock_bank_ff(t->d_bb, bs, 1, (float *)t->d_mid, bs, C, t->unit, nb, t->d_last_dc, stream));
+            OK(csdrb_agc_bank_ff(t->d_mid, bs, 0, t->d_pcm, whole, 1, C, whole, &t->agc, t->d_agc_state, t->limit, stream));
+        } else {
+            OK(csdrb_bandpass_fir_fft_bank_cc(t->d_bb, bs, (complexf *)t->d_mid, bs, C, t->fft_size, t->unit, nb, t->d_taps_fft, 0, t->d_ola_tail, stream));
+            OK(csdrb_agc_bank_ff(t->d_mid, bs, 1, t->d_pcm, whole, 1, C, whole, &t->agc, t->d_agc_state, t->limit, stream));
+        }
+        OK(csdrb_copy_d2h(t->h_out, t->d_pcm, sizeof(short) * (size_t)C * (size_t)whole, stream));
+        if (rest > 0) rows_to_front(t->d_bb, bs, whole, rest, sizeof(complexf), t->d_carry, C, stream);
+        OK(csdrb_stream_synchronize(stream));
+        write_rows(chan, C, t->h_out, sizeof(short) * (size_t)whole, NULL);
+    } else OK(csdrb_stream_synchronize(stream));
+    t->have = rest;
+}
 
 /* ---- the BPSK31 tail: simple_agc_cc 0.001 R | timing_recovery_cc GARDNER N 0.5 2 --add_q | dbpsk_decoder_c_u8 | psk31_varicode_decoder_u8_u8 --------
  * Channels consume different amounts of baseband, so the timing recovery bank gets a start offset per channel.  Device buffers of ONE device:
+ *   in   : [C][bs] complexf : the new baseband, from the front of every row
  *   tr   : [C][ts] complexf : AGC output; row c's unconsumed samples are [start[c], end) (end is the same for every row), new samples go to end
  *   sym  : [C][cap] complexf symbols, bits : [C][cap] dbpsk bits, chars : [C][cap] decoded text
  * Carried per channel: the AGC gain, the timing loop's correction offset and unconsumed baseband, the last dbpsk input, the varicode register.
  * The timing recovery leaves at most 3N/2 samples unconsumed, so every push first moves [min start, end) to the front of the rows. */
 typedef struct {
     int C, sps, end, cap, last_cur;
-    long ts;
+    long bs, ts;
     float agc_ref;
-    complexf *d_tr, *d_carry, *d_sym, *d_last[2];
+    complexf *d_in, *d_tr, *d_carry, *d_sym, *d_last[2];
     unsigned char *d_bits, *d_chars;
     float *d_gain;
     int *d_start, *d_size, *d_counts, *d_char_count, *h_start, *h_size, *h_char_count;
@@ -355,10 +460,11 @@ typedef struct {
 
 static void bpsk_tail_init(bpsk_tail_t *t, int C, int sps, int in_cap, float agc_ref, void *stream)
 {
-    memset(t, 0, sizeof *t);
     t->C = C; t->sps = sps; t->agc_ref = agc_ref;
+    t->bs = ((long)in_cap + 3) & ~3L;
     t->ts = ((long)in_cap + 2L * sps + 3) & ~3L;
     t->cap = (int)(t->ts / (sps / 2) + 1);
+    t->d_in = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->bs);
     t->d_tr = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->ts);
     t->d_carry = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->ts);
     t->d_sym = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->cap);
@@ -376,7 +482,7 @@ static void bpsk_tail_init(bpsk_tail_t *t, int C, int sps, int in_cap, float agc
     t->h_start = csdrb_host_alloc(sizeof(int) * (size_t)C * 3);
     t->h_state = csdrb_host_alloc(sizeof(csdrb_timing_recovery_state_t) * (size_t)C);
     t->h_chars = csdrb_host_alloc((size_t)C * (size_t)t->cap);
-    if (!t->d_tr || !t->d_carry || !t->d_sym || !t->d_last[0] || !t->d_last[1] || !t->d_bits || !t->d_chars || !t->d_gain || !t->d_start || !t->d_size ||
+    if (!t->d_in || !t->d_tr || !t->d_carry || !t->d_sym || !t->d_last[0] || !t->d_last[1] || !t->d_bits || !t->d_chars || !t->d_gain || !t->d_start || !t->d_size ||
         !t->d_counts || !t->d_char_count || !t->d_state || !t->d_hist || !t->h_start || !t->h_state || !t->h_chars) die("out of memory");
     t->h_size = t->h_start + C; t->h_char_count = t->h_start + 2 * C;
     float *g = malloc(sizeof(float) * (size_t)C);
@@ -387,21 +493,17 @@ static void bpsk_tail_init(bpsk_tail_t *t, int C, int sps, int in_cap, float agc
     free(g);
 }
 
-/* n new baseband samples per channel at d_bb (row pitch bs): the chain over them, the decoded text to the sinks */
-static void bpsk_tail_push(bpsk_tail_t *t, channel_t *chan, const complexf *d_bb, long bs, int n, void *stream)
+/* n new baseband samples per channel at the front of d_in: the chain over them, the decoded text to the sinks */
+static void bpsk_tail_push(bpsk_tail_t *t, channel_t *chan, int n, void *stream)
 {
     const int C = t->C;
-    const size_t row = sizeof(complexf) * (size_t)t->ts;
     int lo = t->end;
     for (int c = 0; c < C; c++) lo = t->h_start[c] < lo ? t->h_start[c] : lo;
-    if (lo > 0 && t->end > lo) {                                            /* the unconsumed samples to the front of the rows */
-        OK(csdrb_copy2d_d2d(t->d_carry, row, t->d_tr + lo, row, sizeof(complexf) * (size_t)(t->end - lo), (size_t)C, stream));
-        OK(csdrb_copy2d_d2d(t->d_tr, row, t->d_carry, row, sizeof(complexf) * (size_t)(t->end - lo), (size_t)C, stream));
-    }
+    if (lo > 0 && t->end > lo) rows_to_front(t->d_tr, t->ts, lo, t->end - lo, sizeof(complexf), t->d_carry, C, stream);   /* the unconsumed samples */
     for (int c = 0; c < C; c++) t->h_start[c] -= lo;
     t->end -= lo;
     if (t->end + n > t->ts) die("bpsk31 tail: baseband buffer overflow");
-    OK(csdrb_simple_agc_bank_cc(d_bb, bs, t->d_tr + t->end, t->ts, C, n, 0.001f, t->agc_ref, 65535.0f, t->d_gain, stream));
+    OK(csdrb_simple_agc_bank_cc(t->d_in, t->bs, t->d_tr + t->end, t->ts, C, n, 0.001f, t->agc_ref, 65535.0f, t->d_gain, stream));
     t->end += n;
     for (int c = 0; c < C; c++) t->h_size[c] = t->end - t->h_start[c];
     OK(csdrb_copy_h2d(t->d_start, t->h_start, sizeof(int) * (size_t)C * 2, stream));      /* h_start and h_size are adjacent */
@@ -424,7 +526,7 @@ static void bpsk_tail_push(bpsk_tail_t *t, channel_t *chan, const complexf *d_bb
         OK(csdrb_copy_d2h(t->h_char_count, t->d_char_count, sizeof(int) * (size_t)C, stream));
         OK(csdrb_copy2d_d2h(t->h_chars, (size_t)m, t->d_chars, (size_t)t->cap, (size_t)m, (size_t)C, stream));
         OK(csdrb_stream_synchronize(stream));
-        for (int c = 0; c < C; c++) if (t->h_char_count[c] > 0) write_sink(&chan[c], t->h_chars + (size_t)c * (size_t)m, (size_t)t->h_char_count[c]);
+        write_rows(chan, C, t->h_chars, (size_t)m, t->h_char_count);
     }
 }
 
@@ -445,7 +547,6 @@ typedef struct {
 
 static void rtty_tail_init(rtty_tail_t *t, int C, const csdrb_serial_line_params_t *p, int bufsize, int in_cap)
 {
-    memset(t, 0, sizeof *t);
     t->C = C; t->B = bufsize; t->p = *p;
     t->rs = ((long)bufsize + in_cap + 3) & ~3L;
     t->cap = (int)(t->rs / (long)(p->samples_per_bits * ((float)(1 + p->databits) + p->stopbits)) + 1);   /* the bank's output bound */
@@ -479,15 +580,11 @@ static void rtty_tail_push(rtty_tail_t *t, channel_t *chan, int n, void *stream)
     int lo = t->end;
     for (int c = 0; c < C; c++) {
         if (stuck[c]) die("rtty tail: serial_line_decoder_f_u8 got stuck");   /* main() refuses the parameters that allow it */
-        if (chars[c] > 0) write_sink(&chan[c], t->h_chars + (size_t)c * (size_t)t->cap, (size_t)chars[c]);
         lo = t->h_start[c] < lo ? t->h_start[c] : lo;
     }
+    write_rows(chan, C, t->h_chars, (size_t)t->cap, chars);
     if (lo > 0) {                                                           /* the unconsumed samples (fewer than B per row) to the front */
-        const size_t row = sizeof(float) * (size_t)t->rs, keep = sizeof(float) * (size_t)(t->end - lo);
-        if (keep) {
-            OK(csdrb_copy2d_d2d(t->d_carry, sizeof(float) * (size_t)t->B, t->d_rows + lo, row, keep, (size_t)C, stream));
-            OK(csdrb_copy2d_d2d(t->d_rows, row, t->d_carry, sizeof(float) * (size_t)t->B, keep, (size_t)C, stream));
-        }
+        if (t->end > lo) rows_to_front(t->d_rows, t->rs, lo, t->end - lo, sizeof(float), t->d_carry, C, stream);
         for (int c = 0; c < C; c++) t->h_start[c] -= lo;
         t->end -= lo;
         OK(csdrb_copy_h2d(t->d_start, t->h_start, sizeof(int) * (size_t)C, stream));
@@ -514,7 +611,6 @@ typedef struct {
 
 static void wfm_tail_init(wfm_tail_t *t, int C, float rate, float tau, int in_cap)
 {
-    memset(t, 0, sizeof *t);
     const csdrb_wfm_audio_params_t p = {rate, WFM_BUFSIZE, tau, NFM_RATE};
     t->C = C; t->p = p;
     t->rs = ((long)WFM_BUFSIZE + in_cap + 3) & ~3L;
@@ -538,15 +634,11 @@ static void wfm_tail_push(wfm_tail_t *t, channel_t *chan, int n, void *stream)
     if (csdrb_wfm_audio_bank_f_s16(t->d_rows, t->rs, C, total, &t->p, &t->s, t->d_last, t->d_pcm, t->cap, &consumed, stream) != m)
         die("csdrb_wfm_audio_bank_f_s16 failed");
     const int rest = total - consumed;
-    if (rest > 0 && consumed > 0) {
-        const size_t row = sizeof(float) * (size_t)t->rs;
-        OK(csdrb_copy2d_d2d(t->d_carry, sizeof(float) * WFM_BUFSIZE, t->d_rows + consumed, row, sizeof(float) * (size_t)rest, (size_t)C, stream));
-        OK(csdrb_copy2d_d2d(t->d_rows, row, t->d_carry, sizeof(float) * WFM_BUFSIZE, sizeof(float) * (size_t)rest, (size_t)C, stream));
-    }
+    if (rest > 0 && consumed > 0) rows_to_front(t->d_rows, t->rs, consumed, rest, sizeof(float), t->d_carry, C, stream);
     t->have = rest;
     if (m > 0) OK(csdrb_copy2d_d2h(t->h_pcm, sizeof(short) * (size_t)m, t->d_pcm, sizeof(short) * (size_t)t->cap, sizeof(short) * (size_t)m, (size_t)C, stream));
     OK(csdrb_stream_synchronize(stream));
-    if (m > 0) for (int c = 0; c < C; c++) write_sink(&chan[c], t->h_pcm + sizeof(short) * (size_t)c * (size_t)m, sizeof(short) * (size_t)m);
+    write_rows(chan, C, t->h_pcm, sizeof(short) * (size_t)m, NULL);
 }
 
 /* ---- --waterfall SINK: fft_cc N E W | logaveragepower_cf X N A | fft_exchange_sides_ff N [| compress_fft_adpcm_f_u8 N] on the wideband stream ---
@@ -631,192 +723,152 @@ static void waterfall_push(waterfall_t *w, const complexf *d_fresh, int n, void 
     write_lines(w, lines);
 }
 
-static void waterfall_report(waterfall_t *w)
+/* ---- sinks of both loops: opened last (a tcp: sink blocks until its listener arrives), losses reported at the end ------------------------------ */
+static void open_sinks(channel_t *chan, int C, waterfall_t *wf)
 {
-    if (w->lines_dropped) fprintf(stderr, "csdr-bankd: waterfall sink %s lost %ld lines (too slow)\n", w->sink.sink, w->lines_dropped);
-    if (w->sink.fd >= 0) close(w->sink.fd);
+    for (int c = 0; c < C; c++) { chan[c].fd = open_sink(chan[c].sink); sink_nonblocking(chan[c].fd); }
+    if (wf) { wf->sink.fd = open_sink(wf->sink.sink); sink_nonblocking(wf->sink.fd); }
 }
 
-typedef struct {
-    int kind, C, unit, have, fft_size;
-    long bs;
-    float limit;
-    csdrb_agc_params_t agc;
-    complexf *d_bb, *d_carry, *d_taps_fft, *d_ola_tail;
-    void *d_mid;
-    short *d_pcm;
-    float *d_last_dc;
-    csdrb_agc_state_t *d_agc_state;
-    unsigned char *h_out;
-    bpsk_tail_t bpsk;
-} bb_tail_t;
-
-static void bb_tail_init(bb_tail_t *t, int kind, int C, int out_cap, float limit, float agc_ref, int sps, void *stream)
+static void close_sinks(channel_t *chan, int C, waterfall_t *wf)
 {
-    memset(t, 0, sizeof *t);
-    t->kind = kind; t->C = C; t->limit = limit;
-    if (kind == TAIL_BPSK31) {                                       /* the baseband rows only pass the new samples on */
-        t->unit = 1;
-        t->bs = ((long)out_cap + 3) & ~3L;
-        t->d_bb = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->bs);
-        if (!t->d_bb) die("out of memory");
-        bpsk_tail_init(&t->bpsk, C, sps, out_cap, agc_ref, stream);
-        return;
+    for (int c = 0; c < C; c++) { if (chan[c].dropped) fprintf(stderr, "csdr-bankd: sink %s lost %ld bytes (too slow)\n", chan[c].sink, chan[c].dropped); if (chan[c].fd >= 0) close(chan[c].fd); }
+    if (wf) {
+        if (wf->lines_dropped) fprintf(stderr, "csdr-bankd: waterfall sink %s lost %ld lines (too slow)\n", wf->sink.sink, wf->lines_dropped);
+        if (wf->sink.fd >= 0) close(wf->sink.fd);
     }
-    csdrb_agc_params_t p = {0.2f, 0.01f, 0.0001f, 65536.0f, 200, 0, 0.999f, 1024};
-    if (agc_ref > 0.f) p.reference = agc_ref;
-    t->agc = p;
-    t->unit = 1024;
-    if (kind == TAIL_USB || kind == TAIL_LSB) {                  /* bandpass_fir_fft_cc geometry, csdr.c:1822-1831 */
-        const int T = firdes_filter_len(SSB_BW);
-        int N = next_pow2(T);
-        if (N - T < 200) N <<= 1;
-        t->fft_size = N; t->unit = N - T + 1;
-        complexf *h_taps = calloc((size_t)N, sizeof(complexf));
-        if (!h_taps) die("out of memory");
-        if (kind == TAIL_USB) firdes_bandpass_c(h_taps, T, 0.0f, 0.1f, WINDOW_HAMMING);
-        else firdes_bandpass_c(h_taps, T, -0.1f, 0.0f, WINDOW_HAMMING);
-        complexf *d_taps = csdrb_device_alloc(sizeof(complexf) * (size_t)N);
-        t->d_taps_fft = csdrb_device_alloc(sizeof(complexf) * (size_t)N);
-        t->d_ola_tail = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)N);
-        if (!d_taps || !t->d_taps_fft || !t->d_ola_tail) die("out of memory");
-        OK(csdrb_copy_h2d(d_taps, h_taps, sizeof(complexf) * (size_t)N, stream));
-        OK(csdrb_fft_c2c_batch(d_taps, N, t->d_taps_fft, N, N, 1, 0, stream));       /* the forward FFT of the zero-padded taps (csdr.c:1869) */
-        complexf *zeros = calloc((size_t)C * (size_t)N, sizeof(complexf));   /* the overlap tail is zero at stream start (csdr.c:1860) */
-        if (!zeros) die("out of memory");
-        OK(csdrb_copy_h2d(t->d_ola_tail, zeros, sizeof(complexf) * (size_t)C * (size_t)N, stream));
-        OK(csdrb_stream_synchronize(stream));
-        csdrb_device_free(d_taps); free(h_taps); free(zeros);
-    }
-    t->bs = ((long)t->unit + out_cap + 3) & ~3L;
-    t->d_bb = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->bs);
-    t->d_carry = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->unit);
-    t->d_mid = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->bs);
-    t->d_pcm = csdrb_device_alloc(sizeof(short) * (size_t)C * (size_t)t->bs + 16);
-    t->d_last_dc = csdrb_device_alloc(sizeof(float) * (size_t)C);
-    t->d_agc_state = csdrb_device_alloc(sizeof(csdrb_agc_state_t) * (size_t)C);
-    t->h_out = csdrb_host_alloc((size_t)C * (size_t)t->bs * sizeof(complexf));
-    if (!t->d_bb || !t->d_carry || !t->d_mid || !t->d_pcm || !t->d_last_dc || !t->d_agc_state || !t->h_out) die("out of memory");
-    csdrb_agc_state_t *h_st = calloc((size_t)C, sizeof *h_st);
-    if (!h_st) die("out of memory");
-    for (int c = 0; c < C; c++) h_st[c].gain = 1.0f;                 /* a stream starts at gain 1 (csdr.c:1363) */
-    OK(csdrb_copy_h2d(t->d_agc_state, h_st, sizeof *h_st * (size_t)C, stream));
-    float *h_dc = calloc((size_t)C, sizeof(float));                     /* last_dc_level starts at 0 (csdr.c:957) */
-    if (!h_dc) die("out of memory");
-    OK(csdrb_copy_h2d(t->d_last_dc, h_dc, sizeof(float) * (size_t)C, stream));
-    OK(csdrb_stream_synchronize(stream));
-    free(h_st); free(h_dc);
 }
 
-/* n_new fresh baseband samples per channel sit at d_bb + have: run the tail over the whole units, audio to the sinks, keep the remainder */
-static void bb_tail_push(bb_tail_t *t, channel_t *chan, int n_new, void *stream)
-{
-    const int C = t->C;
-    const long bs = t->bs;
-    const int n = t->have + n_new;
-    if (t->kind == TAIL_BPSK31) { bpsk_tail_push(&t->bpsk, chan, t->d_bb, bs, n, stream); t->have = 0; return; }
-    if (t->kind == TAIL_IQ) {                                    /* raw baseband: nothing is held back */
-        OK(csdrb_copy2d_d2h(t->h_out, sizeof(complexf) * (size_t)n, t->d_bb, sizeof(complexf) * (size_t)bs, sizeof(complexf) * (size_t)n, (size_t)C, stream));
-        OK(csdrb_stream_synchronize(stream));
-        for (int c = 0; c < C; c++) write_sink(&chan[c], t->h_out + sizeof(complexf) * (size_t)c * (size_t)n, sizeof(complexf) * (size_t)n);
-        return;
-    }
-    const int nb = n / t->unit, whole = nb * t->unit, rest = n - whole;
-    if (nb > 0) {
-        if (t->kind == TAIL_AM) {
-            OK(csdrb_fastdcblock_bank_ff(t->d_bb, bs, 1, (float *)t->d_mid, bs, C, t->unit, nb, t->d_last_dc, stream));
-            OK(csdrb_agc_bank_ff(t->d_mid, bs, 0, t->d_pcm, whole, 1, C, whole, &t->agc, t->d_agc_state, t->limit, stream));
-        } else {
-            OK(csdrb_bandpass_fir_fft_bank_cc(t->d_bb, bs, (complexf *)t->d_mid, bs, C, t->fft_size, t->unit, nb, t->d_taps_fft, 0, t->d_ola_tail, stream));
-            OK(csdrb_agc_bank_ff(t->d_mid, bs, 1, t->d_pcm, whole, 1, C, whole, &t->agc, t->d_agc_state, t->limit, stream));
-        }
-        OK(csdrb_copy_d2h(t->h_out, t->d_pcm, sizeof(short) * (size_t)C * (size_t)whole, stream));
-        if (rest > 0) {
-            OK(csdrb_copy2d_d2d(t->d_carry, sizeof(complexf) * (size_t)t->unit, t->d_bb + whole, sizeof(complexf) * (size_t)bs, sizeof(complexf) * (size_t)rest, (size_t)C, stream));
-            OK(csdrb_copy2d_d2d(t->d_bb, sizeof(complexf) * (size_t)bs, t->d_carry, sizeof(complexf) * (size_t)t->unit, sizeof(complexf) * (size_t)rest, (size_t)C, stream));
-        }
-        OK(csdrb_stream_synchronize(stream));
-        for (int c = 0; c < C; c++) write_sink(&chan[c], t->h_out + sizeof(short) * (size_t)c * (size_t)whole, sizeof(short) * (size_t)whole);
-    } else OK(csdrb_stream_synchronize(stream));
-    t->have = rest;
-}
-
-/* wideband input formats (--u8 ...), their bytes per sample on the wire, whether the stream is real, and their names */
+/* ---- options: main() parses and validates them, both loops read them ------------------------------------------------------------------------ */
+/* wideband input formats (--u8 ...), their bytes per sample on the wire and their names */
 enum { IN_U8, IN_F32, IN_S16, IN_REAL_S16, IN_REAL_F32 };
 static const int kWireBytes[] = {2, 8, 4, 2, 4};
 static const char *kFormatNames[] = {"u8", "f32", "s16", "real s16", "real f32"};
-static int format_is_real(int fmt) { return fmt == IN_REAL_S16 || fmt == IN_REAL_F32; }
 #define S16_RECIP (1.0f / 32767.0f)                       /* convert_s16_f: the reference build multiplies by the float reciprocal (csdrb_convert_s16_f) */
 
-static int run_multi(int in_fd, int fmt, const int *dev, int ndev, channel_t *chan, int C, const float *rates, int D, const float *taps, int T, int block,
-                     int kind, float limit, float agc_ref, int rs_I, int rs_D, float rs_bw, int sps, const csdrb_serial_line_params_t *rtty_p, int rtty_B,
-                     float wfm_rate, float tau, waterfall_t *wf, const waterfall_opts_t *wo)
+/* the tails (--tail NAME): whether the bank demodulates for them (float discriminator rows, else cf32 baseband rows), whether --resample
+ * may run in front of them, and their AGC reference when --agc-ref is not given: fastagc_ff's default (csdr.c:1388), agc_ff's (csdr.c:1342),
+ * simple_agc_cc's in the OpenWebRX chain */
+enum { TAIL_NFM, TAIL_NONE, TAIL_IQ, TAIL_AM, TAIL_USB, TAIL_LSB, TAIL_BPSK31, TAIL_RTTY, TAIL_WFM };
+static const struct { const char *name; int demod, resample; float agc_ref; } kTails[] = {
+    [TAIL_NFM] = {"nfm", 1, 1, 1.0f}, [TAIL_NONE] = {"none", 1, 1, 0.f}, [TAIL_IQ] = {"iq", 0, 0, 0.f}, [TAIL_AM] = {"am", 0, 0, 0.2f},
+    [TAIL_USB] = {"usb", 0, 0, 0.2f}, [TAIL_LSB] = {"lsb", 0, 0, 0.2f}, [TAIL_BPSK31] = {"bpsk31", 0, 0, 0.5f}, [TAIL_RTTY] = {"rtty", 1, 0, 0.f},
+    [TAIL_WFM] = {"wfm", 1, 0, 0.f},
+};
+
+typedef struct {
+    const char *in_spec, *wf_sink;                                   /* --in; --waterfall SINK, NULL without a waterfall */
+    int fmt, D, block, tail, device, ndev, devs[64];
+    float bw, limit, agc_ref;                                        /* agc_ref 0: the tail's own default (kTails) */
+    window_t window;
+    int rs_I, rs_D, sps, rtty_B;                                     /* --resample I:D (rs_I 0: no resampler), --sps N of bpsk31, --rtty-bufsize */
+    float rs_bw, wfm_rate, tau;                                      /* --resample's BW, --wfm-rate, --tau */
+    csdrb_serial_line_params_t rtty;                                 /* --sps F, --databits, --stopbits of --tail rtty */
+    waterfall_opts_t wf;
+} opts_t;
+
+/* ---- the tail interface: the only code past option validation that knows which tail runs ----------------------------------------------------
+ * tail_in gives the device rows where the next bank outputs land (the resampler's input with --resample); tail_push runs the resampler if on
+ * and the tail over the n samples per channel put there and writes the sinks; tail_push_host does both for rows in host memory (--devices).
+ * All buffers are on ONE device: the single-GPU path's own, the first device of --devices. */
+typedef struct {
+    int kind, C, resample;
+    size_t esz;                                                      /* one bank output sample: float (demodulated) or complexf */
+    rs_stage_t rs;
+    union { nfm_tail_t nfm; raw_tail_t raw; bb_tail_t bb; bpsk_tail_t bpsk; rtty_tail_t rtty; wfm_tail_t wfm; } u;
+} tail_t;
+
+/* --devices --tail none without --resample: the rows collected on the host are the output, so that tail needs no device, stream or buffer */
+static int tail_host_fed(int kind, int resample) { return kind == TAIL_NONE && !resample; }
+
+/* in_cap: the most samples per channel one block adds; stream NULL for a host-fed tail, which allocates nothing.  The per-tail inits fill the
+ * state zeroed here. */
+static void tail_init(tail_t *t, const opts_t *o, int C, int in_cap, void *stream)
 {
-    const int nfm = kind == TAIL_NFM, rtty = kind == TAIL_RTTY, wfm = kind == TAIL_WFM, demod = nfm || rtty || wfm || kind == TAIL_NONE;
-    const size_t osz = demod ? sizeof(float) : sizeof(complexf);
-    csdrb_multi_bank_t *mb = csdrb_multi_bank_create(ndev, dev, C, rates, D, taps, T, demod, 1024, block);
+    memset(t, 0, sizeof *t);
+    t->kind = o->tail; t->C = C; t->resample = o->rs_I > 0;
+    t->esz = kTails[o->tail].demod ? sizeof(float) : sizeof(complexf);
+    if (!stream) return;
+    if (t->resample) { rs_init(&t->rs, C, o->rs_I, o->rs_D, o->rs_bw, in_cap); in_cap = rs_out_cap(&t->rs); }
+    switch (t->kind) {
+    case TAIL_NFM: nfm_tail_init(&t->u.nfm, C, in_cap, o->limit, o->agc_ref); break;
+    case TAIL_NONE: case TAIL_IQ: raw_tail_init(&t->u.raw, C, in_cap, t->esz); break;
+    case TAIL_AM: bb_tail_init(&t->u.bb, C, in_cap, o->limit, o->agc_ref, NULL, stream); break;
+    case TAIL_USB: bb_tail_init(&t->u.bb, C, in_cap, o->limit, o->agc_ref, (const float[2]){0.0f, 0.1f}, stream); break;
+    case TAIL_LSB: bb_tail_init(&t->u.bb, C, in_cap, o->limit, o->agc_ref, (const float[2]){-0.1f, 0.0f}, stream); break;
+    case TAIL_BPSK31: bpsk_tail_init(&t->u.bpsk, C, o->sps, in_cap, o->agc_ref, stream); break;
+    case TAIL_RTTY: rtty_tail_init(&t->u.rtty, C, &o->rtty, o->rtty_B, in_cap); break;
+    case TAIL_WFM: wfm_tail_init(&t->u.wfm, C, o->wfm_rate, o->tau, in_cap); break;
+    }
+}
+
+static void *tail_in(tail_t *t, long *pitch)
+{
+    if (t->resample) { *pitch = t->rs.rs; return t->rs.d_in + t->rs.have; }
+    switch (t->kind) {
+    case TAIL_NFM: *pitch = t->u.nfm.ds; return t->u.nfm.d_demod + t->u.nfm.a_have;
+    case TAIL_NONE: case TAIL_IQ: *pitch = t->u.raw.pitch; return t->u.raw.d_rows;
+    case TAIL_AM: case TAIL_USB: case TAIL_LSB: *pitch = t->u.bb.bs; return t->u.bb.d_bb + t->u.bb.have;
+    case TAIL_BPSK31: *pitch = t->u.bpsk.bs; return t->u.bpsk.d_in;
+    case TAIL_RTTY: *pitch = t->u.rtty.rs; return t->u.rtty.d_rows + t->u.rtty.end;
+    case TAIL_WFM: default: *pitch = t->u.wfm.rs; return t->u.wfm.d_rows + t->u.wfm.have;
+    }
+}
+
+/* n new bank outputs per channel sit at tail_in: through the resampler if on, then the tail, output to the sinks */
+static void tail_push(tail_t *t, channel_t *chan, int n, void *stream)
+{
+    switch (t->kind) {
+    case TAIL_NFM:
+        if (t->resample) n = rs_push(&t->rs, n, t->u.nfm.d_demod + t->u.nfm.a_have, t->u.nfm.ds, stream);
+        nfm_tail_push(&t->u.nfm, chan, n, stream);
+        break;
+    case TAIL_NONE: case TAIL_IQ:
+        if (t->resample) n = rs_push(&t->rs, n, (float *)t->u.raw.d_rows, t->u.raw.pitch, stream);
+        raw_tail_push(&t->u.raw, chan, n, stream);
+        break;
+    case TAIL_AM: case TAIL_USB: case TAIL_LSB: bb_tail_push(&t->u.bb, chan, n, stream); break;
+    case TAIL_BPSK31: bpsk_tail_push(&t->u.bpsk, chan, n, stream); break;
+    case TAIL_RTTY: rtty_tail_push(&t->u.rtty, chan, n, stream); break;
+    case TAIL_WFM: wfm_tail_push(&t->u.wfm, chan, n, stream); break;
+    }
+}
+
+/* n bank outputs per channel in host rows of n samples: straight to the sinks for a host-fed tail, else to tail_in and tail_push */
+static void tail_push_host(tail_t *t, channel_t *chan, const unsigned char *h_rows, int n, void *stream)
+{
+    const size_t width = t->esz * (size_t)n;
+    if (tail_host_fed(t->kind, t->resample)) { write_rows(chan, t->C, h_rows, width, NULL); return; }
+    long pitch;
+    void *d_in = tail_in(t, &pitch);
+    OK(csdrb_copy2d_h2d(d_in, t->esz * (size_t)pitch, h_rows, width, width, (size_t)t->C, stream));
+    tail_push(t, chan, n, stream);
+}
+
+static int run_multi(const opts_t *o, channel_t *chan, int C, const float *rates, const float *taps, int T, waterfall_t *wf)
+{
+    const int fmt = o->fmt, D = o->D, block = o->block;
+    open_sinks(chan, C, wf);
+    const int in_fd = open_input(o->in_spec);
+    fprintf(stderr, "csdr-bankd: %d channels over %d devices, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, o->ndev, D, T,
+            kFormatNames[fmt], block, kTails[o->tail].name);
+    csdrb_multi_bank_t *mb = csdrb_multi_bank_create(o->ndev, o->devs, C, rates, D, taps, T, kTails[o->tail].demod, 1024, block);
     if (!mb) die("cannot create the multi-GPU bank");
     const int n_out = (block - T) / D + 1, consumed = n_out * D, keep = block - consumed;
+    /* the tail (and the resampler) is audio-rate work (C x the channel rate): the rows every device returned go to the FIRST device once more and
+     * through the same tail as in the single-GPU path */
+    tail_t tail;
+    void *tail_stream = tail_host_fed(o->tail, o->rs_I > 0) ? NULL : device_stream(o->devs[0]);
+    tail_init(&tail, o, C, n_out + 2, tail_stream);
     float lut[256];
     for (int i = 0; i < 256; i++) lut[i] = (float)((float)i / (UCHAR_MAX / 2.0) - 1.0);      /* convert_u8_f, libcsdr.c:2365 */
     complexf *h_wide[2] = {csdrb_host_alloc(sizeof(complexf) * (size_t)block), csdrb_host_alloc(sizeof(complexf) * (size_t)block)};
-    unsigned char *h_out[2] = {csdrb_host_alloc(osz * (size_t)C * (size_t)n_out), csdrb_host_alloc(osz * (size_t)C * (size_t)n_out)};
+    unsigned char *h_out[2] = {csdrb_host_alloc(tail.esz * (size_t)C * (size_t)n_out), csdrb_host_alloc(tail.esz * (size_t)C * (size_t)n_out)};
     unsigned char *raw = malloc((size_t)block * (size_t)kWireBytes[fmt]);
     if (!h_wide[0] || !h_wide[1] || !h_out[0] || !h_out[1] || !raw) die("out of memory");
-    /* --tail nfm: the audio tail is audio-rate work (C x 48 kHz): the discriminator rows every device returned go to the FIRST device once more and through
-     * the same kernels as in the single-GPU path */
-    nfm_tail_t tail_state; bb_tail_t bb; rs_stage_t rsm; rtty_tail_t rt; wfm_tail_t wt; void *tail_stream = NULL;
-    float *d_raw_out = NULL; unsigned char *h_raw_out = NULL;
-    const int resample = rs_I > 0;
-    if (kind != TAIL_NONE || resample) {
-        OK(csdrb_set_device(dev[0]));
-        tail_stream = csdrb_stream_create();
-        if (!tail_stream) die("cannot create a stream");
-        if (resample) rs_init(&rsm, C, rs_I, rs_D, rs_bw, n_out + 2);
-        const int tail_cap = resample ? rs_out_cap(&rsm) : n_out + 2;
-        if (nfm) nfm_tail_init(&tail_state, C, tail_cap, limit, agc_ref);
-        else if (rtty) rtty_tail_init(&rt, C, rtty_p, rtty_B, tail_cap);
-        else if (wfm) wfm_tail_init(&wt, C, wfm_rate, tau, tail_cap);
-        else if (!demod) bb_tail_init(&bb, kind, C, tail_cap, limit, agc_ref, sps, tail_stream);
-        else {
-            d_raw_out = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)tail_cap);
-            h_raw_out = csdrb_host_alloc(sizeof(float) * (size_t)C * (size_t)tail_cap);
-            if (!d_raw_out || !h_raw_out) die("out of memory");
-        }
-    }
     /* --waterfall: the block's fresh samples go to the first device once more, through the same bank as in the single-GPU path */
-    void *wf_stream = NULL;
-    if (wf) {
-        OK(csdrb_set_device(dev[0]));
-        wf_stream = csdrb_stream_create();
-        if (!wf_stream) die("cannot create a stream");
-        waterfall_init(wf, wo, block, 1, wf_stream);
-    }
-    /* --resample: the discriminator rows go to the first device's resampler, its output into the tail (or straight to the sinks for --tail none) */
-#define EMIT(slot_) do { \
-        if (resample) { \
-            OK(csdrb_copy2d_h2d(rsm.d_in + rsm.have, sizeof(float) * (size_t)rsm.rs, h_out[slot_], sizeof(float) * (size_t)n_out, \
-                                sizeof(float) * (size_t)n_out, (size_t)C, tail_stream)); \
-            if (nfm) nfm_tail_push(&tail_state, chan, rs_push(&rsm, n_out, tail_state.d_demod + tail_state.a_have, tail_state.ds, tail_stream), tail_stream); \
-            else { const int m_ = rs_push(&rsm, n_out, d_raw_out, rs_out_cap(&rsm), tail_stream); raw_emit(d_raw_out, rs_out_cap(&rsm), m_, h_raw_out, chan, C, tail_stream); } \
-        } else if (nfm) { \
-            OK(csdrb_copy2d_h2d(tail_state.d_demod + tail_state.a_have, sizeof(float) * (size_t)tail_state.ds, h_out[slot_], sizeof(float) * (size_t)n_out, \
-                                sizeof(float) * (size_t)n_out, (size_t)C, tail_stream)); \
-            nfm_tail_push(&tail_state, chan, n_out, tail_stream); \
-        } else if (rtty) { \
-            OK(csdrb_copy2d_h2d(rt.d_rows + rt.end, sizeof(float) * (size_t)rt.rs, h_out[slot_], sizeof(float) * (size_t)n_out, \
-                                sizeof(float) * (size_t)n_out, (size_t)C, tail_stream)); \
-            rtty_tail_push(&rt, chan, n_out, tail_stream); \
-        } else if (wfm) { \
-            OK(csdrb_copy2d_h2d(wt.d_rows + wt.have, sizeof(float) * (size_t)wt.rs, h_out[slot_], sizeof(float) * (size_t)n_out, \
-                                sizeof(float) * (size_t)n_out, (size_t)C, tail_stream)); \
-            wfm_tail_push(&wt, chan, n_out, tail_stream); \
-        } else if (!demod) { \
-            OK(csdrb_copy2d_h2d(bb.d_bb + bb.have, sizeof(complexf) * (size_t)bb.bs, h_out[slot_], sizeof(complexf) * (size_t)n_out, \
-                                sizeof(complexf) * (size_t)n_out, (size_t)C, tail_stream)); \
-            bb_tail_push(&bb, chan, n_out, tail_stream); \
-        } else for (int c = 0; c < C; c++) write_sink(&chan[c], h_out[slot_] + osz * (size_t)c * (size_t)n_out, osz * (size_t)n_out); \
-    } while (0)
+    void *wf_stream = wf ? device_stream(o->devs[0]) : NULL;
+    if (wf) waterfall_init(wf, &o->wf, block, 1, wf_stream);
     long blocks = 0;
     int ticket[2] = {-1, -1};
     for (int first = 1;; first = 0) {
@@ -825,7 +877,7 @@ static int run_multi(int in_fd, int fmt, const int *dev, int ndev, channel_t *ch
         /* this buffer's previous block (two submits ago) must be done before it is overwritten; its results go out meanwhile */
         if (ticket[slot] >= 0) {
             if (csdrb_multi_bank_collect(mb, ticket[slot]) < 0) die("csdrb_multi_bank_collect failed");
-            EMIT(slot);
+            tail_push_host(&tail, chan, h_out[slot], n_out, tail_stream);
             ticket[slot] = -1;
         }
         if (!first) memcpy(w, h_wide[slot ^ 1] + consumed, sizeof(complexf) * (size_t)keep);   /* the unconsumed tail (csdr.c:1172-1174) */
@@ -856,12 +908,12 @@ static int run_multi(int in_fd, int fmt, const int *dev, int ndev, channel_t *ch
         const int slot = (int)((blocks + k) & 1);
         if (ticket[slot] < 0) continue;
         if (csdrb_multi_bank_collect(mb, ticket[slot]) < 0) die("csdrb_multi_bank_collect failed");
-        EMIT(slot);
+        tail_push_host(&tail, chan, h_out[slot], n_out, tail_stream);
     }
-#undef EMIT
-    fprintf(stderr, "csdr-bankd: end of input after %ld blocks on %d devices, %ld kernel launches\n", blocks, ndev, csdrb_kernel_launches());
+    fprintf(stderr, "csdr-bankd: end of input after %ld blocks on %d devices, %ld kernel launches\n", blocks, o->ndev, csdrb_kernel_launches());
     if (wf_stream) csdrb_stream_destroy(wf_stream);
     csdrb_multi_bank_destroy(mb);
+    close_sinks(chan, C, wf);
     return 0;
 }
 
@@ -915,162 +967,134 @@ static int usage(void)
 
 int main(int argc, char **argv)
 {
-    const char *in_spec = "-", *tail = "nfm";
-    int fmt = IN_U8, D = 50, block = 1 << 18, device = 0, ndev = 0, devs[64];
-    float bw = 0.005f, limit = 1.0f, agc_ref = 0.0f;                /* agc_ref 0: the tail's own default (fastagc_ff 1.0, agc_ff 0.2) */
-    int rs_I = 0, rs_D = 0;                                          /* --resample I:D[:BW]; 0: no resampler */
-    int sps = 0;                                                     /* --sps N of --tail bpsk31 */
-    float spb = 0.f;                                                 /* --sps F of --tail rtty */
-    int databits = 5, rtty_B = 16384, rtty_opts = 0;                 /* --databits, --rtty-bufsize (the CLI's big buffer, csdr.c:190) */
-    float stopbits = 1.5f;                                           /* --stopbits */
-    float rs_bw = 0.05f;                                             /* rational_resampler_ff's default transition bandwidth (csdr.c:1423) */
-    window_t window = WINDOW_HAMMING;
-    const char *wf_sink = NULL;                                      /* --waterfall SINK */
-    waterfall_opts_t wo = {2048, 0, 1, 1, -70.0f, WINDOW_DEFAULT};   /* --fft-every 0 stands for N */
-    int wf_opts = 0;
-    float wfm_rate = 5.0f, tau = 50e-6f;                             /* --wfm-rate, --tau: the README.md:66 graph (75e-6 in the Americas) */
-    int wfm_opts = 0;
+    const char *tail = "nfm";
+    opts_t o = {.in_spec = "-", .fmt = IN_U8, .D = 50, .block = 1 << 18, .bw = 0.005f, .limit = 1.0f, .window = WINDOW_HAMMING,
+                .rs_bw = 0.05f,                                      /* rational_resampler_ff's default transition bandwidth (csdr.c:1423) */
+                .rtty = {0.f, 5, 1.5f, 0.4f}, .rtty_B = 16384,       /* bit_sampling_width_ratio (csdr.c:2510), the CLI's big buffer (csdr.c:190) */
+                .wfm_rate = 5.0f, .tau = 50e-6f,                     /* the README.md:66 graph (75e-6 in the Americas) */
+                .wf = {2048, 0, 1, 1, -70.0f, WINDOW_DEFAULT}};      /* --fft-every 0 stands for N */
+    int rtty_opts = 0, wfm_opts = 0, wf_opts = 0;
     channel_t *chan = calloc((size_t)argc, sizeof *chan);
     int C = 0;
     for (int a = 1; a < argc; a++) {
-        const char *o = argv[a];
+        const char *arg = argv[a];
         const char *v = a + 1 < argc ? argv[a + 1] : NULL;
-        if (!strcmp(o, "--u8")) fmt = IN_U8;
-        else if (!strcmp(o, "--f32")) fmt = IN_F32;
-        else if (!strcmp(o, "--s16")) fmt = IN_S16;
-        else if (!strcmp(o, "--real-s16")) fmt = IN_REAL_S16;
-        else if (!strcmp(o, "--real-f32")) fmt = IN_REAL_F32;
-        else if (!strcmp(o, "--in") && v) { in_spec = v; a++; }
-        else if (!strcmp(o, "--decimation") && v) { D = atoi(v); a++; }
-        else if (!strcmp(o, "--bw") && v) { bw = (float)atof(v); a++; }
-        else if (!strcmp(o, "--window") && v) { window = firdes_get_window_from_string((char *)v); a++; }
-        else if (!strcmp(o, "--block") && v) { block = atoi(v); a++; }
-        else if (!strcmp(o, "--tail") && v) { tail = v; a++; }
-        else if (!strcmp(o, "--limit") && v) { limit = (float)atof(v); a++; }
-        else if (!strcmp(o, "--agc-ref") && v) { agc_ref = (float)atof(v); a++; }
-        else if (!strcmp(o, "--sps") && v) { sps = atoi(v); spb = (float)atof(v); a++; }
-        else if (!strcmp(o, "--databits") && v) { databits = atoi(v); rtty_opts = 1; a++; }
-        else if (!strcmp(o, "--stopbits") && v) { stopbits = (float)atof(v); rtty_opts = 1; a++; }
-        else if (!strcmp(o, "--rtty-bufsize") && v) { rtty_B = atoi(v); rtty_opts = 1; a++; }
-        else if (!strcmp(o, "--wfm-rate") && v) { wfm_rate = (float)atof(v); wfm_opts = 1; a++; }
-        else if (!strcmp(o, "--tau") && v) { tau = (float)atof(v); wfm_opts = 1; a++; }
-        else if (!strcmp(o, "--waterfall") && v) { wf_sink = v; a++; }
-        else if (!strcmp(o, "--fft-size") && v) { wo.fft_size = atoi(v); wf_opts = 1; a++; }
-        else if (!strcmp(o, "--fft-every") && v) { wo.every = atoi(v); wf_opts = 1; if (wo.every < 1) die("--fft-every must be at least 1"); a++; }
-        else if (!strcmp(o, "--fft-averages") && v) { wo.averages = atoi(v); wf_opts = 1; a++; }
-        else if (!strcmp(o, "--fft-add-db") && v) { wo.add_db = (float)atof(v); wf_opts = 1; a++; }
-        else if (!strcmp(o, "--fft-window") && v) { wo.window = firdes_get_window_from_string((char *)v); wf_opts = 1; a++; }
-        else if (!strcmp(o, "--fft-compression") && v) {
-            if (!strcmp(v, "adpcm")) wo.compress = 1;
-            else if (!strcmp(v, "none")) wo.compress = 0;
+        if (!strcmp(arg, "--u8")) o.fmt = IN_U8;
+        else if (!strcmp(arg, "--f32")) o.fmt = IN_F32;
+        else if (!strcmp(arg, "--s16")) o.fmt = IN_S16;
+        else if (!strcmp(arg, "--real-s16")) o.fmt = IN_REAL_S16;
+        else if (!strcmp(arg, "--real-f32")) o.fmt = IN_REAL_F32;
+        else if (!strcmp(arg, "--in") && v) { o.in_spec = v; a++; }
+        else if (!strcmp(arg, "--decimation") && v) { o.D = atoi(v); a++; }
+        else if (!strcmp(arg, "--bw") && v) { o.bw = (float)atof(v); a++; }
+        else if (!strcmp(arg, "--window") && v) { o.window = firdes_get_window_from_string((char *)v); a++; }
+        else if (!strcmp(arg, "--block") && v) { o.block = atoi(v); a++; }
+        else if (!strcmp(arg, "--tail") && v) { tail = v; a++; }
+        else if (!strcmp(arg, "--limit") && v) { o.limit = (float)atof(v); a++; }
+        else if (!strcmp(arg, "--agc-ref") && v) { o.agc_ref = (float)atof(v); a++; }
+        else if (!strcmp(arg, "--sps") && v) { o.sps = atoi(v); o.rtty.samples_per_bits = (float)atof(v); a++; }
+        else if (!strcmp(arg, "--databits") && v) { o.rtty.databits = atoi(v); rtty_opts = 1; a++; }
+        else if (!strcmp(arg, "--stopbits") && v) { o.rtty.stopbits = (float)atof(v); rtty_opts = 1; a++; }
+        else if (!strcmp(arg, "--rtty-bufsize") && v) { o.rtty_B = atoi(v); rtty_opts = 1; a++; }
+        else if (!strcmp(arg, "--wfm-rate") && v) { o.wfm_rate = (float)atof(v); wfm_opts = 1; a++; }
+        else if (!strcmp(arg, "--tau") && v) { o.tau = (float)atof(v); wfm_opts = 1; a++; }
+        else if (!strcmp(arg, "--waterfall") && v) { o.wf_sink = v; a++; }
+        else if (!strcmp(arg, "--fft-size") && v) { o.wf.fft_size = atoi(v); wf_opts = 1; a++; }
+        else if (!strcmp(arg, "--fft-every") && v) { o.wf.every = atoi(v); wf_opts = 1; if (o.wf.every < 1) die("--fft-every must be at least 1"); a++; }
+        else if (!strcmp(arg, "--fft-averages") && v) { o.wf.averages = atoi(v); wf_opts = 1; a++; }
+        else if (!strcmp(arg, "--fft-add-db") && v) { o.wf.add_db = (float)atof(v); wf_opts = 1; a++; }
+        else if (!strcmp(arg, "--fft-window") && v) { o.wf.window = firdes_get_window_from_string((char *)v); wf_opts = 1; a++; }
+        else if (!strcmp(arg, "--fft-compression") && v) {
+            if (!strcmp(v, "adpcm")) o.wf.compress = 1;
+            else if (!strcmp(v, "none")) o.wf.compress = 0;
             else die("--fft-compression is adpcm or none");
             wf_opts = 1; a++;
         }
-        else if (!strcmp(o, "--device") && v) { device = atoi(v); a++; }
-        else if (!strcmp(o, "--devices") && v) { ndev = parse_devices(v, devs, 64); if (ndev <= 0) die("--devices wants N0,N1,..."); a++; }
-        else if (!strcmp(o, "--resample") && v) {
-            if (sscanf(v, "%d:%d:%f", &rs_I, &rs_D, &rs_bw) < 2 || rs_I < 1 || rs_D < 1) die("--resample wants I:D[:BW] with positive integers I and D");
+        else if (!strcmp(arg, "--device") && v) { o.device = atoi(v); a++; }
+        else if (!strcmp(arg, "--devices") && v) { o.ndev = parse_devices(v, o.devs, 64); if (o.ndev <= 0) die("--devices wants N0,N1,..."); a++; }
+        else if (!strcmp(arg, "--resample") && v) {
+            if (sscanf(v, "%d:%d:%f", &o.rs_I, &o.rs_D, &o.rs_bw) < 2 || o.rs_I < 1 || o.rs_D < 1) die("--resample wants I:D[:BW] with positive integers I and D");
             a++;
         }
-        else if (!strcmp(o, "--help")) return usage();
-        else if (strchr(o, ':') && o[0] != '-' ) {
+        else if (!strcmp(arg, "--help")) return usage();
+        else if (strchr(arg, ':') && (arg[0] != '-' || arg[1] == '.' || (arg[1] >= '0' && arg[1] <= '9'))) {      /* RATE:SINK, RATE may be negative */
             char *end = NULL;
-            chan[C].rate = strtof(o, &end);
+            chan[C].rate = strtof(arg, &end);
             if (!end || *end != ':') die("channels are RATE:SINK");
             chan[C].sink = end + 1; chan[C].fd = -1; chan[C].dropped = 0; C++;
-        } else if (o[0] == '-' && strchr(o + 1, ':') && (o[1] == '.' || (o[1] >= '0' && o[1] <= '9'))) {      /* negative rate */
-            char *end = NULL;
-            chan[C].rate = strtof(o, &end);
-            if (!end || *end != ':') die("channels are RATE:SINK");
-            chan[C].sink = end + 1; chan[C].fd = -1; chan[C].dropped = 0; C++;
-        } else { fprintf(stderr, "csdr-bankd: unknown argument %s\n", o); return 2; }
+        } else { fprintf(stderr, "csdr-bankd: unknown argument %s\n", arg); return 2; }
     }
-    static const char *kTails[] = {"nfm", "none", "iq", "am", "usb", "lsb", "bpsk31", "rtty", "wfm"};
-    int kind = -1;
-    for (int k = 0; k < 9; k++) if (!strcmp(tail, kTails[k])) kind = k;
-    if (kind < 0) die("--tail is nfm, none, iq, am, usb, lsb, bpsk31, rtty or wfm");
-    const csdrb_serial_line_params_t rtty_p = {spb, databits, stopbits, 0.4f};   /* serial_line_decoder_f_u8's bit_sampling_width_ratio (csdr.c:2510) */
-    if (kind == TAIL_BPSK31) {
-        if (sps <= 4 || (sps & 3)) die("--tail bpsk31 needs --sps N with N > 4 and divisible by 4 (timing_recovery_cc's decimation)");
-        if (agc_ref == 0.0f) agc_ref = 0.5f;                         /* simple_agc_cc's reference in the OpenWebRX chain */
-    } else if (kind == TAIL_RTTY) {
+    o.tail = -1;
+    for (int k = 0; k < (int)(sizeof kTails / sizeof *kTails); k++) if (!strcmp(tail, kTails[k].name)) o.tail = k;
+    if (o.tail < 0) die("--tail is nfm, none, iq, am, usb, lsb, bpsk31, rtty or wfm");
+    if (o.tail == TAIL_BPSK31) {
+        if (o.sps <= 4 || (o.sps & 3)) die("--tail bpsk31 needs --sps N with N > 4 and divisible by 4 (timing_recovery_cc's decimation)");
+    } else if (o.tail == TAIL_RTTY) {
+        const float spb = o.rtty.samples_per_bits;
         if (!(spb >= 1.f && spb <= 1e6f)) die("--tail rtty needs --sps F, samples per bit at the baseband rate, at least 1 (serial_line_decoder_f_u8's range)");
         if (spb < 5.f) fprintf(stderr, "csdr-bankd: warning: serial_line_decoder_f_u8 does not work well below 5 samples per bit\n");
-        if (databits < 1 || databits > 8) die("--databits must be between 1 and 8");
-        if (!(stopbits >= 1.f && stopbits <= 1000.f)) die("--stopbits must be at least 1");
-        if (rtty_B < 1 || rtty_B > (1 << 22)) die("--rtty-bufsize must be between 1 and 4194304 samples");
+        if (o.rtty.databits < 1 || o.rtty.databits > 8) die("--databits must be between 1 and 8");
+        if (!(o.rtty.stopbits >= 1.f && o.rtty.stopbits <= 1000.f)) die("--stopbits must be at least 1");
+        if (o.rtty_B < 1 || o.rtty_B > (1 << 22)) die("--rtty-bufsize must be between 1 and 4194304 samples");
         /* a character that starts at the third sample of a call and does not fit makes the call consume nothing: the CLI exits "stuck" */
-        if (spb * ((float)(1 + databits) + stopbits) + 2.0f >= (float)rtty_B)
+        if (spb * ((float)(1 + o.rtty.databits) + o.rtty.stopbits) + 2.0f >= (float)o.rtty_B)
             die("--rtty-bufsize must exceed sps*(1 + databits + stopbits) + 2: a call could not hold one character and would get stuck");
-    } else if (sps) die("--sps belongs to --tail bpsk31 and --tail rtty");
-    if (kind != TAIL_RTTY && rtty_opts) die("--databits, --stopbits and --rtty-bufsize belong to --tail rtty");
-    if (kind == TAIL_WFM) {
+    } else if (o.sps) die("--sps belongs to --tail bpsk31 and --tail rtty");
+    if (o.tail != TAIL_RTTY && rtty_opts) die("--databits, --stopbits and --rtty-bufsize belong to --tail rtty");
+    if (o.tail == TAIL_WFM) {
         /* above 16 a decimator call could consume more than its 1024 samples (the reference then memmoves a negative length): WFM needs about 5 */
-        if (!(wfm_rate > 1.0f && wfm_rate <= 16.0f)) die("--wfm-rate must be above 1 and at most 16 (wideband rate / decimation / 48 kHz)");
-        if (!(tau > 0.0f)) die("--tau must be positive (50e-6 in Europe, 75e-6 in the Americas)");
+        if (!(o.wfm_rate > 1.0f && o.wfm_rate <= 16.0f)) die("--wfm-rate must be above 1 and at most 16 (wideband rate / decimation / 48 kHz)");
+        if (!(o.tau > 0.0f)) die("--tau must be positive (50e-6 in Europe, 75e-6 in the Americas)");
     } else if (wfm_opts) die("--wfm-rate and --tau belong to --tail wfm");
-    const int nfm = kind == TAIL_NFM, rtty = kind == TAIL_RTTY, wfm = kind == TAIL_WFM, demod = nfm || rtty || wfm || kind == TAIL_NONE;
-    if (nfm && agc_ref == 0.0f) agc_ref = 1.0f;                      /* fastagc_ff's default reference (csdr.c:1388) */
+    if (o.agc_ref == 0.0f) o.agc_ref = kTails[o.tail].agc_ref;
     if (C == 0) die("no channels (RATE:SINK ...)");
-    if (block <= 0 || (block & 1)) die("--block must be a positive even number of samples");
-    if (D <= 0 || (D & 1)) die("--decimation must be a positive even number (the fused bank serves even decimations only)");
-    if (!(bw > 0.f && bw < 0.5f)) die("--bw must be a transition bandwidth between 0 and 0.5");
-    if (!(limit > 0.f) || !(agc_ref >= 0.f)) die("--limit and --agc-ref must be positive");
-    const int resample = rs_I > 0;
-    if (resample) {
-        if (!demod || rtty || wfm) die("--resample works with --tail nfm and --tail none only (the am, usb, lsb, iq, bpsk31, rtty and wfm tails are not resampled)");
-        if (!(rs_bw > 0.f && rs_bw < 0.5f)) die("--resample: the transition bandwidth must be between 0 and 0.5");
-        const int rs_T = firdes_filter_len(rs_bw);
-        if (!resample_geometry_ok(rs_I, rs_D, rs_T)) {
+    if (o.block <= 0 || (o.block & 1)) die("--block must be a positive even number of samples");
+    if (o.D <= 0 || (o.D & 1)) die("--decimation must be a positive even number (the fused bank serves even decimations only)");
+    if (!(o.bw > 0.f && o.bw < 0.5f)) die("--bw must be a transition bandwidth between 0 and 0.5");
+    if (!(o.limit > 0.f) || !(o.agc_ref >= 0.f)) die("--limit and --agc-ref must be positive");
+    if (o.rs_I > 0) {
+        if (!kTails[o.tail].resample) die("--resample works with --tail nfm and --tail none only (the am, usb, lsb, iq, bpsk31, rtty and wfm tails are not resampled)");
+        if (!(o.rs_bw > 0.f && o.rs_bw < 0.5f)) die("--resample: the transition bandwidth must be between 0 and 0.5");
+        const int rs_T = firdes_filter_len(o.rs_bw);
+        if (!resample_geometry_ok(o.rs_I, o.rs_D, rs_T)) {
             fprintf(stderr, "csdr-bankd: --resample %d:%d with %d taps: a resampler call could end on its output cap and repeat an output; "
-                            "the daemon needs (T/I + 1)*I >= 2*D + I - 1 (T >= 2*D + I - 2 suffices): lower the transition bandwidth\n", rs_I, rs_D, rs_T);
+                            "the daemon needs (T/I + 1)*I >= 2*D + I - 1 (T >= 2*D + I - 2 suffices): lower the transition bandwidth\n", o.rs_I, o.rs_D, rs_T);
             return 1;
         }
     }
-    const int real = format_is_real(fmt);
-    if (real && wf_sink) die("--waterfall needs a complex input: the waterfall of a real stream is fft_fc, a real-to-complex transform this build does not have");
-    if (wf_opts && !wf_sink) die("--fft-size, --fft-every, --fft-averages, --fft-add-db, --fft-window and --fft-compression belong to --waterfall");
-    waterfall_t wf;
+    const int fmt = o.fmt, D = o.D, block = o.block, real = fmt == IN_REAL_S16 || fmt == IN_REAL_F32;
+    if (real && o.wf_sink) die("--waterfall needs a complex input: the waterfall of a real stream is fft_fc, a real-to-complex transform this build does not have");
+    if (wf_opts && !o.wf_sink) die("--fft-size, --fft-every, --fft-averages, --fft-add-db, --fft-window and --fft-compression belong to --waterfall");
+    waterfall_t wf, *wfp = NULL;
     memset(&wf, 0, sizeof wf);
-    if (wf_sink) {
-        if (wo.every == 0) wo.every = wo.fft_size;
-        if (wo.averages < 1) die("--fft-averages must be at least 1");
-        const csdrb_spectrum_params_t p = {wo.fft_size, wo.every, wo.averages, wo.compress, wo.add_db};
+    if (o.wf_sink) {
+        if (o.wf.every == 0) o.wf.every = o.wf.fft_size;
+        if (o.wf.averages < 1) die("--fft-averages must be at least 1");
+        const csdrb_spectrum_params_t p = {o.wf.fft_size, o.wf.every, o.wf.averages, o.wf.compress, o.wf.add_db};
         const csdrb_spectrum_state_t s0 = {0, 0};
         if (csdrb_spectrum_bank_lines(&p, &s0, 0) < 0) die("--fft-size must be a power of two from 2 to 16384");
-        wf.sink.rate = 0.f; wf.sink.sink = wf_sink; wf.sink.fd = -1;
+        wf.sink.rate = 0.f; wf.sink.sink = o.wf_sink; wf.sink.fd = -1;
+        wfp = &wf;
     }
     signal(SIGPIPE, SIG_IGN);
 
     /* ---- filter and bank ---------------------------------------------------------------------------------------------------- */
-    const int T = firdes_filter_len(bw);
+    const int T = firdes_filter_len(o.bw);
     float *taps = malloc(sizeof(float) * (size_t)T);
-    firdes_lowpass_f(taps, T, 0.5f / (float)D, window);
+    firdes_lowpass_f(taps, T, 0.5f / (float)D, o.window);
     if (block < 2 * T) die("--block is shorter than two filter lengths");
     float *rates = malloc(sizeof(float) * (size_t)C);
     for (int c = 0; c < C; c++) rates[c] = chan[c].rate;
-    if (ndev > 0) {
-        if (ndev > C) die("more devices than channels");
-        for (int c = 0; c < C; c++) { chan[c].fd = open_sink(chan[c].sink); sink_nonblocking(chan[c].fd); }
-        if (wf_sink) { wf.sink.fd = open_sink(wf_sink); sink_nonblocking(wf.sink.fd); }
-        const int fd = open_input(in_spec);
-        fprintf(stderr, "csdr-bankd: %d channels over %d devices, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, ndev, D, T, kFormatNames[fmt], block, tail);
-        const int rc = run_multi(fd, fmt, devs, ndev, chan, C, rates, D, taps, T, block, kind, limit, agc_ref, rs_I, rs_D, rs_bw, sps, &rtty_p, rtty_B,
-                                 wfm_rate, tau, wf_sink ? &wf : NULL, &wo);
-        for (int c = 0; c < C; c++) { if (chan[c].dropped) fprintf(stderr, "csdr-bankd: sink %s lost %ld bytes (too slow)\n", chan[c].sink, chan[c].dropped); if (chan[c].fd >= 0) close(chan[c].fd); }
-        if (wf_sink) waterfall_report(&wf);
-        return rc;
-    }
-    OK(csdrb_set_device(device));
-    csdrb_ddc_bank_t *bank = csdrb_ddc_bank_create(C, rates, D, taps, T, demod, 1024);   /* 1024 = the CLI's shift_addition_cc call size (csdr.c:911) */
+    if (o.ndev > C) die("more devices than channels");
+    if (o.ndev > 0) return run_multi(&o, chan, C, rates, taps, T, wfp);
+    void *stream = device_stream(o.device);
+    csdrb_ddc_bank_t *bank = csdrb_ddc_bank_create(C, rates, D, taps, T, kTails[o.tail].demod, 1024);   /* 1024 = the CLI's shift_addition_cc call size (csdr.c:911) */
     if (!bank) die("cannot create the bank");
-    void *stream = csdrb_stream_create();
-    if (!stream) die("cannot create a stream");
 
     /* ---- buffers ----------------------------------------------------------------------------------------------------------------
      * wide[2]  : [tail of the previous block | new block] cf32 (f32 for a real input), ping-pong so the tail copy never overlaps
      * raw      : the block as it arrived, for the formats converted on the device; stage: real s16 converted where the block lands unaligned
-     * with the NFM tail the discriminator output goes straight into nfm_tail_t's demod rows; without it into a plain [C][ds] array */
+     * the bank writes straight into the tail's input rows (tail_in) */
     const size_t in_bytes = (size_t)block * (size_t)kWireBytes[fmt];
     const size_t ssz = real ? sizeof(float) : sizeof(complexf);   /* one wideband sample on the device */
     unsigned char *h_in = csdrb_host_alloc(in_bytes);
@@ -1079,35 +1103,16 @@ int main(int argc, char **argv)
     const int raw_in = fmt == IN_U8 || fmt == IN_S16 || fmt == IN_REAL_S16;
     unsigned char *d_raw = raw_in ? csdrb_device_alloc(in_bytes + 16) : NULL;
     float *d_stage = fmt == IN_REAL_S16 ? csdrb_device_alloc(sizeof(float) * (size_t)block + 16) : NULL;
-    const int out_cap = wide_cap / D + 2;                          /* discriminator samples one block can add */
-    nfm_tail_t tl;
-    bb_tail_t bb;
-    rs_stage_t rsm;
-    rtty_tail_t rt;
-    wfm_tail_t wt;
-    if (resample) rs_init(&rsm, C, rs_I, rs_D, rs_bw, out_cap);
-    const int tail_cap = resample ? rs_out_cap(&rsm) : out_cap;   /* samples one block can add behind the discriminator (and resampler) */
-    long ds = ((long)tail_cap + 3) & ~3L;
-    float *d_demod = NULL;
-    unsigned char *h_out = NULL;
-    if (nfm) { nfm_tail_init(&tl, C, tail_cap, limit, agc_ref); ds = tl.ds; d_demod = tl.d_demod; }
-    else if (rtty) { rtty_tail_init(&rt, C, &rtty_p, rtty_B, out_cap); ds = rt.rs; d_demod = rt.d_rows; }
-    else if (wfm) { wfm_tail_init(&wt, C, wfm_rate, tau, out_cap); ds = wt.rs; d_demod = wt.d_rows; }
-    else if (!demod) { bb_tail_init(&bb, kind, C, out_cap, limit, agc_ref, sps, stream); ds = bb.bs; d_demod = (float *)bb.d_bb; }
-    else {
-        d_demod = csdrb_device_alloc(sizeof(float) * (size_t)C * (size_t)ds);
-        h_out = csdrb_host_alloc((size_t)C * (size_t)ds * sizeof(float));
-    }
-    if (!h_in || !d_wide[0] || !d_wide[1] || (raw_in && !d_raw) || (fmt == IN_REAL_S16 && !d_stage) || !d_demod || (kind == TAIL_NONE && !h_out)) die("out of memory");
+    const int out_cap = wide_cap / D + 2;                          /* bank outputs one block can add */
+    tail_t tl;
+    tail_init(&tl, &o, C, out_cap, stream);
+    if (!h_in || !d_wide[0] || !d_wide[1] || (raw_in && !d_raw) || (fmt == IN_REAL_S16 && !d_stage)) die("out of memory");
+    if (wfp) waterfall_init(wfp, &o.wf, block, 0, stream);
 
-    /* sinks last: tcp: sinks block until their listener arrives */
-    for (int c = 0; c < C; c++) { chan[c].fd = open_sink(chan[c].sink); sink_nonblocking(chan[c].fd); }
-    if (wf_sink) {
-        waterfall_init(&wf, &wo, block, 0, stream);
-        wf.sink.fd = open_sink(wf_sink); sink_nonblocking(wf.sink.fd);
-    }
-    const int in_fd = open_input(in_spec);
-    fprintf(stderr, "csdr-bankd: %d channels, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, D, T, kFormatNames[fmt], block, tail);
+    open_sinks(chan, C, wfp);
+    const int in_fd = open_input(o.in_spec);
+    fprintf(stderr, "csdr-bankd: %d channels, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, D, T, kFormatNames[fmt], block,
+            kTails[o.tail].name);
 
     int cur = 0, keep = 0;
     long blocks = 0;
@@ -1129,33 +1134,27 @@ int main(int argc, char **argv)
             OK(csdrb_convert_s16_f((const short *)d_raw, d_stage, fresh_n, stream));
             OK(csdrb_copy_d2d(fresh, d_stage, sizeof(float) * (size_t)fresh_n, stream));
         } else OK(csdrb_copy_h2d(fresh, h_in, fresh_bytes, stream));
-        if (wf_sink) waterfall_push(&wf, (const complexf *)fresh, fresh_n, stream);   /* the waterfall of the same samples, lines to its sink */
+        if (wfp) waterfall_push(wfp, (const complexf *)fresh, fresh_n, stream);   /* the waterfall of the same samples, lines to its sink */
         const int n_in = block;
 
-        /* 2. shift | fir_decimate | fmdemod for every channel, new discriminator samples behind the de-emphasis FIR's carried inputs */
-        void *dst = resample ? (void *)(rsm.d_in + rsm.have) : nfm ? (void *)(d_demod + tl.a_have) : rtty ? (void *)(rt.d_rows + rt.end)
-                  : wfm ? (void *)(wt.d_rows + wt.have) : !demod ? (void *)(bb.d_bb + bb.have) : (void *)d_demod;
-        const int n_out = real ? csdrb_ddc_bank_process_f(bank, (const float *)d_wide[cur], n_in, dst, resample ? rsm.rs : ds, stream)
-                               : csdrb_ddc_bank_process(bank, (const complexf *)d_wide[cur], n_in, dst, resample ? rsm.rs : ds, stream);
+        /* 2. shift | fir_decimate | fmdemod for every channel, the new outputs straight into the tail's input rows */
+        long pitch;
+        void *dst = tail_in(&tl, &pitch);
+        const int n_out = real ? csdrb_ddc_bank_process_f(bank, (const float *)d_wide[cur], n_in, dst, pitch, stream)
+                               : csdrb_ddc_bank_process(bank, (const complexf *)d_wide[cur], n_in, dst, pitch, stream);
         if (n_out < 0) die("csdrb_ddc_bank_process failed");
         const int consumed = n_out * D;
         keep = n_in - consumed;
         OK(csdrb_copy_d2d(d_wide[cur ^ 1], d_wide[cur] + ssz * (size_t)consumed, ssz * (size_t)keep, stream));
         cur ^= 1;
 
-        /* 2b. --resample: the new discriminator samples through rational_resampler_ff, into the tail's rows */
-        const int n_tail = resample ? rs_push(&rsm, n_out, nfm ? d_demod + tl.a_have : d_demod, ds, stream) : n_out;
-        if (!demod) bb_tail_push(&bb, chan, n_out, stream);         /* baseband tails: am / usb / lsb audio, or the raw baseband */
-        else if (rtty) rtty_tail_push(&rt, chan, n_out, stream);    /* serial_line_decoder_f_u8 | rtty_baudot2ascii_u8_u8, text to the sinks */
-        else if (wfm) wfm_tail_push(&wt, chan, n_out, stream);      /* fractional_decimator_ff | deemphasis_wfm_ff | convert_f_s16, audio to the sinks */
-        else if (!nfm) raw_emit(d_demod, ds, n_tail, h_out, chan, C, stream);   /* raw discriminator output, float */
-        else nfm_tail_push(&tl, chan, n_tail, stream);             /* 3./4. limit | de-emphasis | AGC | s16, audio to the sinks */
+        /* 3. the resampler if on, the tail, its output to the sinks */
+        tail_push(&tl, chan, n_out, stream);
         blocks++;
     }
     OK(csdrb_stream_synchronize(stream));
     fprintf(stderr, "csdr-bankd: end of input after %ld blocks, %ld kernel launches\n", blocks, csdrb_kernel_launches());
-    for (int c = 0; c < C; c++) { if (chan[c].dropped) fprintf(stderr, "csdr-bankd: sink %s lost %ld bytes (too slow)\n", chan[c].sink, chan[c].dropped); if (chan[c].fd >= 0) close(chan[c].fd); }
-    if (wf_sink) waterfall_report(&wf);
+    close_sinks(chan, C, wfp);
     csdrb_ddc_bank_destroy(bank);
     csdrb_stream_destroy(stream);
     return 0;

@@ -192,3 +192,46 @@ def build_full_once(tmp_path_factory):
     if _full is None:
         _full = build_full(tmp_path_factory.mktemp("emul_full"))
     return _full
+
+
+_ABSENT = object()
+
+
+def _swap(obj, key, value):
+    """set obj.key (a module) or obj[key] (a list or dict) to value, or delete it for _ABSENT; returns what was there"""
+    if isinstance(obj, (list, dict)):
+        old = obj[key] if isinstance(obj, list) or key in obj else _ABSENT
+        if value is _ABSENT:
+            del obj[key]
+        else:
+            obj[key] = value
+    else:
+        old = getattr(obj, key, _ABSENT)
+        if value is _ABSENT:
+            delattr(obj, key)
+        else:
+            setattr(obj, key, value)
+    return old
+
+
+def emulated_bankd(tmp_path_factory, patches=lambda lib, cli: ()):
+    """Generator behind the module fixtures of tests/test_bankd_*_emulated.py: csdr-bankd linked against the emulated library, with two pretend
+    devices for --devices (CUDA_EMUL_DEVICES=2) and a memcpy stand-in for NCCL (fake_nccl.c), both inherited by the daemon.  patches(lib, cli)
+    lists (module or container, name or key, value) to set while the module's tests run, e.g. its MULTI_DEVICES.  Yields the daemon's path;
+    afterwards every patched attribute is restored and the environment variables are cleared."""
+    import os
+    import pytest
+    if not available():
+        pytest.skip("needs g++ and the CUDA toolkit headers")
+    lib, cli = build_full_once(tmp_path_factory)
+    fake = tmp_path_factory.mktemp("fake_nccl") / "libfake_nccl.so"
+    subprocess.run(["gcc", "-O1", "-fPIC", "-shared", str(SHIM / "fake_nccl.c"), "-o", str(fake)], check=True)
+    saved = [(obj, key, _swap(obj, key, value)) for obj, key, value in patches(lib, cli)]
+    os.environ["CUDA_EMUL_DEVICES"] = "2"
+    os.environ["CSDRB_NCCL_LIB"] = str(fake)
+    try:
+        yield str(lib.parent / "csdr-bankd_emul")
+    finally:
+        for obj, key, old in reversed(saved):
+            _swap(obj, key, old)
+        del os.environ["CUDA_EMUL_DEVICES"], os.environ["CSDRB_NCCL_LIB"]

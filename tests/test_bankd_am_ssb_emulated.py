@@ -42,20 +42,8 @@ def emul_bandpass(bb, lo, hi):
 
 @pytest.fixture(scope="module")
 def bankd(tmp_path_factory):
-    if not emul_build.available():
-        pytest.skip("needs g++ and the CUDA toolkit headers")
-    lib, _cli = emul_build.build_full_once(tmp_path_factory)
-    import os, subprocess
-    fake = tmp_path_factory.mktemp("fake_nccl_am") / "libfake_nccl.so"
-    subprocess.run(["gcc", "-O1", "-fPIC", "-shared", str(ROOT / "tests" / "host_shim" / "fake_nccl.c"), "-o", str(fake)], check=True)
-    os.environ["CUDA_EMUL_DEVICES"] = "2"; os.environ["CSDRB_NCCL_LIB"] = str(fake)
-    saved = base.MULTI_DEVICES, g.BANDPASS
-    base.MULTI_DEVICES = lambda: ["0", "0,1"]
-    _emul["lib"] = C.CDLL(str(lib))
-    g.BANDPASS = emul_bandpass
-    yield str(lib.parent / "csdr-bankd_emul")
-    base.MULTI_DEVICES, g.BANDPASS = saved
-    del os.environ["CUDA_EMUL_DEVICES"], os.environ["CSDRB_NCCL_LIB"]
+    yield from emul_build.emulated_bankd(tmp_path_factory, lambda lib, cli: [(base, "MULTI_DEVICES", lambda: ["0", "0,1"]), (_emul, "lib", C.CDLL(str(lib))),
+                                                                             (g, "BANDPASS", emul_bandpass)])
 
 
 test_am_ssb_tails_equal_the_oracle_on_the_banks_baseband = g.test_am_ssb_tails_equal_the_oracle_on_the_banks_baseband

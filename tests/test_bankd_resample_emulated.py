@@ -19,19 +19,7 @@ import test_gpu_zzz_bankd_resample as gr  # noqa: E402
 
 @pytest.fixture(scope="module")
 def bankd(tmp_path_factory):
-    if not emul_build.available():
-        pytest.skip("needs g++ and the CUDA toolkit headers")
-    lib, _cli = emul_build.build_full_once(tmp_path_factory)
-    # --devices 0,1: two pretend devices and a memcpy stand-in for NCCL (tests/host_shim/fake_nccl.c), as in tests/test_bankd_emulated.py
-    import os, subprocess
-    fake = tmp_path_factory.mktemp("fake_nccl_r") / "libfake_nccl.so"
-    subprocess.run(["gcc", "-O1", "-fPIC", "-shared", str(ROOT / "tests" / "host_shim" / "fake_nccl.c"), "-o", str(fake)], check=True)
-    os.environ["CUDA_EMUL_DEVICES"] = "2"; os.environ["CSDRB_NCCL_LIB"] = str(fake)
-    saved = g.MULTI_DEVICES
-    g.MULTI_DEVICES = lambda: ["0", "0,1"]
-    yield str(lib.parent / "csdr-bankd_emul")
-    g.MULTI_DEVICES = saved
-    del os.environ["CUDA_EMUL_DEVICES"], os.environ["CSDRB_NCCL_LIB"]
+    yield from emul_build.emulated_bankd(tmp_path_factory, lambda lib, cli: [(g, "MULTI_DEVICES", lambda: ["0", "0,1"])])
 
 
 test_nfm_resampled_to_48k_equals_the_oracle_graph = gr.test_nfm_resampled_to_48k_equals_the_oracle_graph

@@ -1,7 +1,5 @@
 """CPU tier: csdr-bankd's RTTY tail on the emulated library, with two pretend devices for --devices -- the test bodies of
 tests/test_gpu_zzz_bankd_rtty.py except the 2.4 Msps skimmer geometry, which is too large for the emulator."""
-import os
-import subprocess
 import sys
 from pathlib import Path
 
@@ -19,17 +17,7 @@ import test_gpu_zzz_bankd_rtty as g  # noqa: E402
 
 @pytest.fixture(scope="module")
 def bankd(tmp_path_factory):
-    if not emul_build.available():
-        pytest.skip("needs g++ and the CUDA toolkit headers")
-    lib, _cli = emul_build.build_full_once(tmp_path_factory)
-    fake = tmp_path_factory.mktemp("fake_nccl_rtty") / "libfake_nccl.so"
-    subprocess.run(["gcc", "-O1", "-fPIC", "-shared", str(ROOT / "tests" / "host_shim" / "fake_nccl.c"), "-o", str(fake)], check=True)
-    os.environ["CUDA_EMUL_DEVICES"] = "2"; os.environ["CSDRB_NCCL_LIB"] = str(fake)
-    saved = base.MULTI_DEVICES
-    base.MULTI_DEVICES = lambda: ["0", "0,1"]
-    yield str(lib.parent / "csdr-bankd_emul")
-    base.MULTI_DEVICES = saved
-    del os.environ["CUDA_EMUL_DEVICES"], os.environ["CSDRB_NCCL_LIB"]
+    yield from emul_build.emulated_bankd(tmp_path_factory, lambda lib, cli: [(base, "MULTI_DEVICES", lambda: ["0", "0,1"])])
 
 
 test_rtty_tail_equals_the_checker_on_the_banks_discriminator = g.test_rtty_tail_equals_the_checker_on_the_banks_discriminator

@@ -1,7 +1,5 @@
 """CPU tier: csdr-bankd --waterfall on the emulated library, with two pretend devices for --devices -- the test bodies of
 tests/test_gpu_zzz_bankd_waterfall.py except the comparison with the compiled reference CLI, which needs the real library."""
-import os
-import subprocess
 import sys
 from pathlib import Path
 
@@ -19,18 +17,8 @@ import test_gpu_zzz_bankd_waterfall as g  # noqa: E402
 
 @pytest.fixture(scope="module")
 def bankd(tmp_path_factory):
-    if not emul_build.available():
-        pytest.skip("needs g++ and the CUDA toolkit headers")
-    lib, cli = emul_build.build_full_once(tmp_path_factory)
-    fake = tmp_path_factory.mktemp("fake_nccl_wf") / "libfake_nccl.so"
-    subprocess.run(["gcc", "-O1", "-fPIC", "-shared", str(ROOT / "tests" / "host_shim" / "fake_nccl.c"), "-o", str(fake)], check=True)
-    os.environ["CUDA_EMUL_DEVICES"] = "2"; os.environ["CSDRB_NCCL_LIB"] = str(fake)
-    saved, saved_cli = base.MULTI_DEVICES, g.CLI[0]
-    base.MULTI_DEVICES = lambda: ["0", "0,1"]
-    g.CLI[0] = cli                                                      # the product CLI on the same emulated library
-    yield str(lib.parent / "csdr-bankd_emul")
-    base.MULTI_DEVICES, g.CLI[0] = saved, saved_cli
-    del os.environ["CUDA_EMUL_DEVICES"], os.environ["CSDRB_NCCL_LIB"]
+    yield from emul_build.emulated_bankd(tmp_path_factory, lambda lib, cli: [(base, "MULTI_DEVICES", lambda: ["0", "0,1"]),
+                                                                             (g.CLI, 0, cli)])   # the product CLI on the same emulated library
 
 
 test_waterfall_equals_the_cli_pipe = g.test_waterfall_equals_the_cli_pipe
