@@ -169,6 +169,7 @@ def lib() -> C.CDLL:
     L.agc_ff.restype = C.c_float
     L.csdrb_fft_c2c_batch.argtypes = [vp, lg, vp, lg, it, it, it, vp]
     L.csdrb_fft_c2c_large_batch.argtypes = [vp, lg, vp, lg, it, it, it, vp]
+    L.csdrb_fft_r2c_batch.argtypes = [vp, lg, vp, lg, it, it, vp]
     L.csdrb_bandpass_fir_fft_bank_cc.argtypes = [vp, lg, vp, lg, it, it, it, it, vp, lg, vp, vp]
     L.csdrb_ddc_bank_scratch_bytes.argtypes = [it, it, it, it]; L.csdrb_ddc_bank_scratch_bytes.restype = sz
     L.csdrb_ddc_bank.argtypes = [vp, it, it, vp, vp, it, it, it, C.POINTER(C.c_float), it, it, vp, lg, vp, vp, vp, sz, vp]
@@ -243,6 +244,8 @@ def lib() -> C.CDLL:
     L.rational_resampler_get_lowpass_f.argtypes = [C.POINTER(C.c_float), it, it, it, it]
     L.csdrb_rational_resampler_bank_ff.argtypes = [vp, lg, vp, lg, it, it, it, it, C.POINTER(C.c_float), it, it, C.POINTER(_Resampler), vp]
     L.make_fft_c2c.argtypes = [it, vp, vp, it, it]; L.make_fft_c2c.restype = C.POINTER(_Plan)
+    L.make_fft_r2c.argtypes = [it, vp, vp, it]; L.make_fft_r2c.restype = C.POINTER(_Plan)
+    L.apply_precalculated_window_f.argtypes = [vp, vp, it, vp]
     L.fft_execute.argtypes = [C.POINTER(_Plan)]
     L.fft_destroy.argtypes = [C.POINTER(_Plan)]
     L.apply_fir_fft_cc.argtypes = [C.POINTER(_Plan), C.POINTER(_Plan), vp, vp, it]
@@ -274,6 +277,9 @@ def lib() -> C.CDLL:
     L.csdrb_spectrum_bank_lines.argtypes = [C.POINTER(SpectrumParams), C.POINTER(SpectrumState), lg]; L.csdrb_spectrum_bank_lines.restype = lg
     L.csdrb_spectrum_bank_scratch_bytes.argtypes = [it, lg, C.POINTER(SpectrumParams)]; L.csdrb_spectrum_bank_scratch_bytes.restype = sz
     L.csdrb_spectrum_bank_cf.argtypes = [vp, lg, it, lg, vp, C.POINTER(SpectrumParams), vp, vp, C.POINTER(SpectrumState), vp, lg, vp, sz, vp]
+    L.csdrb_spectrum_bank_lines_f.argtypes = [C.POINTER(SpectrumParams), C.POINTER(SpectrumState), lg]; L.csdrb_spectrum_bank_lines_f.restype = lg
+    L.csdrb_spectrum_bank_scratch_bytes_f.argtypes = [it, lg, C.POINTER(SpectrumParams)]; L.csdrb_spectrum_bank_scratch_bytes_f.restype = sz
+    L.csdrb_spectrum_bank_f.argtypes = [vp, lg, it, lg, vp, C.POINTER(SpectrumParams), vp, vp, C.POINTER(SpectrumState), vp, lg, vp, sz, vp]
     L.csdrb_wfm_audio_bank_outputs.argtypes = [C.POINTER(WfmAudioParams), C.POINTER(WfmAudioState), it, C.POINTER(it)]
     L.csdrb_wfm_audio_bank_f_s16.argtypes = [vp, lg, it, it, C.POINTER(WfmAudioParams), C.POINTER(WfmAudioState), vp, vp, lg, C.POINTER(it), vp]
     _lib = L
@@ -743,6 +749,13 @@ class libcsdr:
         lib().fft_execute(pl); lib().fft_destroy(pl); return y
 
     @staticmethod
+    def rdft(x):
+        """make_fft_r2c + fft_execute: x.size real points -> x.size // 2 + 1 bins"""
+        x = np.ascontiguousarray(x, np.float32).copy(); y = np.empty(x.size // 2 + 1, np.complex64)
+        pl = lib().make_fft_r2c(x.size, x.ctypes.data, y.ctypes.data, 0)
+        lib().fft_execute(pl); lib().fft_destroy(pl); return y
+
+    @staticmethod
     def bandpass_fir_fft_cc(x, lo, hi, bw, window="HAMMING"):
         """The CLI block loop of csdr.c:1833-1883 over the libcsdr-named entry points (complete blocks only)."""
         x = np.ascontiguousarray(x, np.complex64)
@@ -1167,6 +1180,29 @@ def fft_c2c(x, inverse: bool = False):
     return out if x.dim() > 1 or x.dtype != torch.complex64 else out[0]
 
 
+def _as_f32_rows(x):
+    """Accept [C, N] (or [N]) float32 CUDA tensors whose rows are contiguous; return (tensor, data_ptr, row stride in floats, C, N)."""
+    import torch
+    if x.dtype != torch.float32:
+        raise TypeError("expected float32 [C,N]")
+    xr = x.unsqueeze(0) if x.dim() == 1 else x
+    if not xr.is_cuda:
+        raise CsdrB200Error("bank API needs CUDA tensors (no CPU fallback)")
+    if xr.dim() != 2 or xr.stride(1) != 1:
+        raise ValueError("samples must be contiguous within a row")
+    return xr, xr.data_ptr(), xr.stride(0), xr.shape[0], xr.shape[1]
+
+
+def fft_r2c(x):
+    """Forward real-to-complex DFT along the last axis of a [B, N] (or [N]) float32 CUDA tensor: N a power of two from 4 to 2^21 real points,
+    N // 2 + 1 complex64 bins per row as FFTW's r2c gives them (csdrb_fft_r2c_batch)."""
+    import torch
+    xr, ptr, stride, b, n = _as_f32_rows(x)
+    out = torch.empty((b, n // 2 + 1), dtype=torch.complex64, device=xr.device)
+    _check(lib().csdrb_fft_r2c_batch(ptr, stride, out.data_ptr(), out.stride(0), n, b, _stream()), "fft_r2c")
+    return out if x.dim() > 1 else out[0]
+
+
 def bandpass_geometry(transition_bw: float):
     """(taps_length, fft_size, input_size, overlap) exactly as csdr.c:1833-1838 sizes them."""
     T = firdes_filter_len(transition_bw)
@@ -1509,27 +1545,35 @@ class SpectrumBank:
     """The OpenWebRX waterfall chain `fft_cc N E W | logaveragepower_cf ADD_DB N A | fft_exchange_sides_ff N [| compress_fft_adpcm_f_u8 N]` on
     `rows` streams at once (csdrb_spectrum_bank_cf).  Owns the window table, the carried history and partial line, and the host state;
     process(x) takes the next n samples of every row ([rows, n] complex64 CUDA tensor, or [n] for one row) and returns the lines they complete:
-    [rows, lines, N] float32 dB, or [rows, lines, (N + 10) // 2] uint8 with compress=True."""
+    [rows, lines, N] float32 dB, or [rows, lines, (N + 10) // 2] uint8 with compress=True.
+    real=True: the chain of a real stream, `fft_fc N E W | logaveragepower_cf ADD_DB N A [| compress_fft_adpcm_f_u8 N]` (csdrb_spectrum_bank_f):
+    process(x) takes [rows, n] (or [n]) float32 real samples, `every` counts real samples, a frame is 2N of them and the lines are N bins in
+    bin order (DC first)."""
 
     def __init__(self, rows: int, fft_size: int, every: int, averages: int, add_db: float, window: str = "HAMMING", compress: bool = False,
-                 device="cuda"):
+                 device="cuda", real: bool = False):
         import torch
-        self.rows, self.device = rows, torch.device(device)
+        self.rows, self.device, self.real = rows, torch.device(device), real
         self.params = SpectrumParams(fft_size, every, averages, 1 if compress else 0, add_db)
         self.state = SpectrumState(0, 0)
-        self.window = torch.from_numpy(libcsdr.precalculate_window(fft_size, window)).to(self.device)
-        self.hist = torch.zeros((rows, fft_size), dtype=torch.complex64, device=self.device)
+        frame = 2 * fft_size if real else fft_size
+        self.window = torch.from_numpy(libcsdr.precalculate_window(frame, window)).to(self.device)
+        self.hist = torch.zeros((rows, frame), dtype=torch.float32 if real else torch.complex64, device=self.device)
         self.acc = torch.zeros((rows, fft_size), dtype=torch.float32, device=self.device)
         self.line_bytes = (fft_size + 10) // 2 if compress else 4 * fft_size
 
     def lines(self, n: int) -> int:
-        return _check(lib().csdrb_spectrum_bank_lines(C.byref(self.params), C.byref(self.state), n), "spectrum_bank_lines")
+        f = lib().csdrb_spectrum_bank_lines_f if self.real else lib().csdrb_spectrum_bank_lines
+        return _check(f(C.byref(self.params), C.byref(self.state), n), "spectrum_bank_lines")
 
     def process(self, x, scratch_bytes: int | None = None):
         import torch
-        if x.dtype == torch.complex64 and x.dim() == 1:
-            x = x.unsqueeze(0)
-        xr, ptr, stride, rows, n = _as_cf32_rows(x)
+        if self.real:
+            xr, ptr, stride, rows, n = _as_f32_rows(x)
+        else:
+            if x.dtype == torch.complex64 and x.dim() == 1:
+                x = x.unsqueeze(0)
+            xr, ptr, stride, rows, n = _as_cf32_rows(x)
         if rows != self.rows:
             raise ValueError(f"expected {self.rows} rows, got {rows}")
         N, L = self.params.fft_size, self.lines(n)
@@ -1538,12 +1582,14 @@ class SpectrumBank:
         else:
             out = torch.empty((rows, L, N), dtype=torch.float32, device=self.device)
         if scratch_bytes is None:
-            scratch_bytes = lib().csdrb_spectrum_bank_scratch_bytes(rows, n, C.byref(self.params))
+            scratch_bytes = (lib().csdrb_spectrum_bank_scratch_bytes_f if self.real else lib().csdrb_spectrum_bank_scratch_bytes)(rows, n, C.byref(self.params))
         scratch = _scratch(scratch_bytes + 16, self.device)
-        got = _check(lib().csdrb_spectrum_bank_cf(ptr if n else self.hist.data_ptr(), stride, rows, n, self.window.data_ptr(), C.byref(self.params),
-                                                  self.hist.data_ptr(), self.acc.data_ptr(), C.byref(self.state),
-                                                  out.data_ptr() if out.numel() else self.acc.data_ptr(),
-                                                  out.stride(0) * out.element_size(), scratch.data_ptr(), scratch_bytes, _stream()), "spectrum_bank_cf")
+        bank = lib().csdrb_spectrum_bank_f if self.real else lib().csdrb_spectrum_bank_cf
+        got = _check(bank(ptr if n else self.hist.data_ptr(), stride, rows, n, self.window.data_ptr(), C.byref(self.params),
+                          self.hist.data_ptr(), self.acc.data_ptr(), C.byref(self.state),
+                          out.data_ptr() if out.numel() else self.acc.data_ptr(),
+                          out.stride(0) * out.element_size(), scratch.data_ptr(), scratch_bytes, _stream()),
+                     "spectrum_bank_f" if self.real else "spectrum_bank_cf")
         assert got == L
         return out
 

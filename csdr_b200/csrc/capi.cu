@@ -488,6 +488,13 @@ int csdrb_fft_c2c_large_batch(const complexf* d_in, long in_stride, complexf* d_
     return rc < 0 ? rc : counted(0, rc);
 }
 
+int csdrb_fft_r2c_batch(const float* d_in, long in_stride, complexf* d_out, long out_stride, int size, int batch, void* stream)
+{
+    if (!d_in || !d_out) { set_error("fft r2c: null pointer"); return -1; }
+    int rc = launch_fft_r2c_batch(d_in, in_stride, reinterpret_cast<float2*>(d_out), out_stride, size, batch, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
 int csdrb_bandpass_fir_fft_bank_cc(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int fft_size, int input_size,
                                    int nblocks, const complexf* d_taps_fft, long taps_stride, complexf* d_tail_io, void* stream)
 {
@@ -591,7 +598,7 @@ int csdrb_log_ff(const float* d_in, float* d_out, long n, float add_db, void* st
     return rc < 0 ? rc : counted(0, rc);
 }
 // waterfall bank (spectrum.cu): fft_cc | logaveragepower_cf | fft_exchange_sides_ff [| compress_fft_adpcm_f_u8] per row
-long csdrb_spectrum_bank_lines(const csdrb_spectrum_params_t* p, const csdrb_spectrum_state_t* s, long n) { return spectrum_lines(p, s, n); }
+long csdrb_spectrum_bank_lines(const csdrb_spectrum_params_t* p, const csdrb_spectrum_state_t* s, long n) { return spectrum_lines(p, s, n, 0); }
 size_t csdrb_spectrum_bank_scratch_bytes(int rows, long n, const csdrb_spectrum_params_t* p) { return spectrum_scratch_bytes(rows, n, p); }
 int csdrb_spectrum_bank_cf(const complexf* d_in, long in_stride, int rows, long n, const float* d_window, const csdrb_spectrum_params_t* p,
                            complexf* d_hist_io, float* d_acc_io, csdrb_spectrum_state_t* state_io, void* d_out, long out_stride_bytes,
@@ -602,6 +609,18 @@ int csdrb_spectrum_bank_cf(const complexf* d_in, long in_stride, int rows, long 
     int launches = 0;
     int rc = launch_spectrum_bank(reinterpret_cast<const float2*>(d_in), in_stride, rows, n, d_window, p, reinterpret_cast<float2*>(d_hist_io), d_acc_io,
                                   state_io, d_out, out_stride_bytes, d_scratch, scratch_bytes, &launches, S(stream));
+    return rc < 0 ? rc : counted(rc, launches);
+}
+// real-input waterfall bank (spectrum.cu): fft_fc | logaveragepower_cf [| compress_fft_adpcm_f_u8] per row
+long csdrb_spectrum_bank_lines_f(const csdrb_spectrum_params_t* p, const csdrb_spectrum_state_t* s, long n) { return spectrum_lines(p, s, n, 1); }
+size_t csdrb_spectrum_bank_scratch_bytes_f(int rows, long n, const csdrb_spectrum_params_t* p) { return spectrum_scratch_bytes(rows, n, p); }
+int csdrb_spectrum_bank_f(const float* d_in, long in_stride, int rows, long n, const float* d_window, const csdrb_spectrum_params_t* p,
+                          float* d_hist_io, float* d_acc_io, csdrb_spectrum_state_t* state_io, void* d_out, long out_stride_bytes,
+                          void* d_scratch, size_t scratch_bytes, void* stream)
+{
+    int launches = 0;
+    int rc = launch_spectrum_bank_f(d_in, in_stride, rows, n, d_window, p, d_hist_io, d_acc_io, state_io, d_out, out_stride_bytes, d_scratch, scratch_bytes,
+                                    &launches, S(stream));
     return rc < 0 ? rc : counted(rc, launches);
 }
 int csdrb_shift_unroll_bank_cc(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int input_size,

@@ -113,6 +113,7 @@ void elementwise(const char* who, const In* input, Out* output, int n, F f)
 
 struct csdrb_plan_impl { unsigned magic; int forward; };
 const unsigned kPlanMagic = 0xC5D2B200u;
+const unsigned kPlanMagicR2C = 0xC5D2B2F1u;                                // make_fft_r2c's plans (always forward)
 
 }  // namespace
 }  // namespace csdrb
@@ -360,6 +361,13 @@ void apply_precalculated_window_c(complexf* input, complexf* output, int size, f
     st.sync();
 }
 
+// fft_fc windows its frames on the host (csdr.c:3478) right before fft_execute stages them: an O(n) multiply that a device round trip would only
+// slow down.  The float product is the one the real waterfall bank computes on the device (__fmul_rn).
+void apply_precalculated_window_f(float* input, float* output, int size, float* windowt)
+{
+    for (int i = 0; i < size; i++) output[i] = input[i] * windowt[i];
+}
+
 void apply_window_c(complexf* input, complexf* output, int size, window_t window)
 {
     float* table = precalculate_window(size, window);                    // the table itself is one-off host work, like every filter design step
@@ -508,12 +516,39 @@ FFT_PLAN_T* make_fft_c2c(int size, complexf* input, complexf* output, int forwar
     return p;
 }
 
+FFT_PLAN_T* make_fft_r2c(int size, float* input, complexf* output, int benchmark)
+{
+    (void)benchmark;
+    if (size < 4 || size > 2 * kFftLargeMaxN || (size & (size - 1))) {
+        fprintf(stderr, "libcsdr_b200: make_fft_r2c: size %d unsupported (power of two, 4..%d)\n", size, 2 * kFftLargeMaxN);
+        return nullptr;
+    }
+    FFT_PLAN_T* p = (FFT_PLAN_T*)malloc(sizeof(FFT_PLAN_T));
+    csdrb_plan_impl* impl = (csdrb_plan_impl*)malloc(sizeof(csdrb_plan_impl));
+    impl->magic = kPlanMagicR2C; impl->forward = 1;
+    p->size = size; p->input = input; p->output = output; p->plan = impl;
+    return p;
+}
+
+// size real points in, size/2 + 1 bins out, like FFTW's r2c
+static void fft_execute_r2c(FFT_PLAN_T* plan)
+{
+    Staging st("fft_execute");
+    const int n = plan->size;
+    const float* d_in = st.up(static_cast<const float*>(plan->input), n);
+    complexf* d_out = st.alloc<complexf>(n / 2 + 1);
+    st.check(csdrb_fft_r2c_batch(d_in, n, d_out, n / 2 + 1, n, 1, st.stream()));
+    st.get(static_cast<complexf*>(plan->output), d_out, n / 2 + 1);
+    st.sync();
+}
+
 void fft_execute(FFT_PLAN_T* plan)
 {
     const char* who = "fft_execute";
     if (!plan) return;
+    if (plan->plan && ((csdrb_plan_impl*)plan->plan)->magic == kPlanMagicR2C) { fft_execute_r2c(plan); return; }
     if (!plan->plan || ((csdrb_plan_impl*)plan->plan)->magic != kPlanMagic) {
-        set_error("plan was not created by libcsdr_b200's make_fft_c2c (r2c/c2r plans are outside the hot path)"); die(who);
+        set_error("plan was not created by libcsdr_b200's make_fft_c2c or make_fft_r2c (c2r plans are outside the hot path)"); die(who);
     }
     const int inverse = ((csdrb_plan_impl*)plan->plan)->forward ? 0 : 1;
     elementwise(who, static_cast<const complexf*>(plan->input), static_cast<complexf*>(plan->output), plan->size,

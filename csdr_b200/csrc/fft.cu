@@ -11,8 +11,11 @@
 //   fastddc_inv_kernel    : fastddc_inv_cc (fastddc.c:106-166) -- fold N bins x taps into M aliasing bins
 //                           (same summation order as the reference: ascending bin index per destination),
 //                           /pre_decimation, swap, IFFT_M, /M, drop `scrap`, post shift + decimate.
+//   fft_r2c_batch_kernel  : fft_execute() of a make_fft_r2c plan (fft_fftw.c:16-24) up to 32768 real points, one CTA per row (fft_real.cuh);
+//   fft_r2c_split_kernel    above that, the four-step transform of the packed rows and this split in place.
 #include "fft_kernels.cuh"
 #include "fft_large.cuh"
+#include "fft_real.cuh"
 #include "kernels.h"
 #include "side_stream.cuh"
 
@@ -703,6 +706,80 @@ int launch_fastddc_fwd_large(const float2* d_in, float2* d_spectra, float2* d_ov
         CSDRB_CUDA(cudaFreeAsync(tmp, st));
     }
     return launches + 1;
+}
+
+// ==== real-to-complex transforms (kernels: fft_real.cuh) ===========================================================================================
+struct RfftTwiddles { std::mutex mu; std::map<int, float2*> by_m; };
+
+int get_rfft_twiddles(int m, const float2** out, cudaStream_t st)
+{
+    RfftTwiddles& c = per_device<RfftTwiddles>();
+    std::lock_guard<std::mutex> lk(c.mu);
+    auto it = c.by_m.find(m);
+    if (it == c.by_m.end()) {
+        std::vector<float2> h((size_t)m / 2 + 1);
+        rfft_fill_twiddles(m, h.data());
+        float2* d = nullptr;
+        CSDRB_CUDA(cudaMalloc(&d, sizeof(float2) * h.size()));
+        CSDRB_CUDA(cudaMemcpyAsync(d, h.data(), sizeof(float2) * h.size(), cudaMemcpyHostToDevice, st));
+        CSDRB_CUDA(cudaStreamSynchronize(st));                           // h leaves scope; once per device and size
+        it = c.by_m.emplace(m, d).first;
+    }
+    *out = it->second;
+    return 0;
+}
+
+// the split behind the four-step transform, in place: row r holds Z[0..M) and gets X[0..M]; thread k reads and writes only bins k and M - k
+// (and M for k = 0, which no thread reads)
+__global__ void __launch_bounds__(256)
+fft_r2c_split_kernel(float2* __restrict__ y, long stride, int M, int rows, const float2* __restrict__ rtw)
+{
+    const int k = blockIdx.x * 256 + threadIdx.x;
+    if (k > M / 2) return;
+    for (int r = blockIdx.y; r < rows; r += gridDim.y) {
+        RfftRowOut dst{y + (long)r * stride};
+        rfft_split_pair(k, M, dst.y[k], dst.y[(M - k) & (M - 1)], rtw, dst);
+    }
+}
+
+template <int M>
+static int launch_r2c_n(const float* in, long is, float2* out, long os, int batch, const float2* tw, const float2* rtw, cudaStream_t st)
+{
+    const size_t smem = sizeof(float2) * fft_smem_elems(M);
+    auto k = fft_r2c_batch_kernel<M>;
+    if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    k<<<batch, rfft_threads(M), smem, st>>>(in, is, out, os, tw, rtw);
+    CSDRB_CUDA(cudaGetLastError());
+    return 1;
+}
+
+int launch_fft_r2c_batch(const float* d_in, long in_stride, float2* d_out, long out_stride, int n, int batch, cudaStream_t st)
+{
+    if (n < 4 || n > 2 * kFftLargeMaxN || (n & (n - 1))) { set_error("fft r2c: size %d unsupported (power of two, 4..%d)", n, 2 * kFftLargeMaxN); return -1; }
+    if (batch <= 0) return 0;
+    const int m = n / 2;
+    if (batch > 1 && (in_stride < n || out_stride < m + 1)) {
+        set_error("fft r2c: rows overlap (in_stride %ld < %d real points or out_stride %ld < %d bins)", in_stride, n, out_stride, m + 1); return -1;
+    }
+    const float2* rtw = nullptr;
+    if (int rc = get_rfft_twiddles(m, &rtw, st)) return rc;
+    if (m >= kFftLargeMinN) {
+        // Z of the packed rows straight into the output rows (m of their m + 1 bins), then the split in place
+        const int launches = fft_large_run(RfftLargeRowsIn{d_in, in_stride}, d_out, out_stride, m, batch, false, st);
+        if (launches < 0) return launches;
+        fft_r2c_split_kernel<<<dim3((unsigned)((m / 2 + 256) / 256), (unsigned)(batch < 65535 ? batch : 65535)), 256, 0, st>>>(d_out, out_stride, m, batch, rtw);
+        CSDRB_CUDA(cudaGetLastError());
+        return launches + 1;
+    }
+    const float2* tw = nullptr;
+    if (m >= 32) { if (int rc = get_twiddles16(m, &tw, st)) return rc; }
+    else if (int rc = get_twiddles(m, &tw, st)) return rc;
+    switch (m) {
+#define X(M) case M: return launch_r2c_n<M>(d_in, in_stride, d_out, out_stride, batch, tw, rtw, st);
+        CSDRB_FFT_SIZES(X)
+#undef X
+    }
+    return -1;
 }
 
 int launch_apply_fir_fft_large(const float2* d_in, const float2* d_taps_fft, const float2* d_last_overlap, int overlap_size, float2* d_out,

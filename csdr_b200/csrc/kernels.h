@@ -132,6 +132,10 @@ int launch_fft_c2c_large_batch(const float2* d_in, long in_stride, float2* d_out
 int launch_fastddc_fwd_large(const float2* d_in, float2* d_spectra, float2* d_overlap_io, int fft_size, int input_size, int nblocks, cudaStream_t st);
 int launch_apply_fir_fft_large(const float2* d_in, const float2* d_taps_fft, const float2* d_last_overlap, int overlap_size, float2* d_out,
                                int fft_size, cudaStream_t st);
+// real-to-complex transforms (fft.cu, kernels fft_real.cuh): n real points (power of two, 4..2*kFftLargeMaxN) -> n/2 + 1 bins per row; the split
+// table W_n^k, k = 0..n/4, of the n/2-point packed transform (cached per device and size)
+int get_rfft_twiddles(int m, const float2** out, cudaStream_t st);
+int launch_fft_r2c_batch(const float* d_in, long in_stride, float2* d_out, long out_stride, int n, int batch, cudaStream_t st);
 size_t fastddc_inv_scratch_bytes(int channels, int nblocks);
 int launch_fastddc_inv_bank(const float2* d_spectra, int nblocks, const float2* d_taps_fft, const void* d_chan, int channels,
                             int fft_size, int fft_inv_size, int pre_decimation, int scrap, int post_input_size, int post_decimation,
@@ -150,12 +154,17 @@ void fastddc_inv_plan_destroy(void* plan);
 // waterfall spectrum bank, spectrum.cu.  SpectrumParams / SpectrumState have the layout of csdrb_spectrum_params_t / csdrb_spectrum_state_t.
 struct SpectrumParams { int fft_size, every, averages, compress; float add_db; };
 struct SpectrumState { long long consumed, frames; };
+// real = 1: the real-input bank (fft_fc N E W | logaveragepower_cf X N A [| compress_fft_adpcm_f_u8 N]): n, every and the history count real samples.
 long long spectrum_frames_at(int fft_size, int every, long long total);        // frames fft_cc completes on the first `total` samples of a stream
-long spectrum_lines(const void* h_params_v, const void* h_state_v, long n);      // lines a call on n samples completes; < 0 for bad arguments
+long long spectrum_frames_at_f(int fft_size, int every, long long total);      // frames fft_fc completes (fft_size bins, 2*fft_size real points)
+long spectrum_lines(const void* h_params_v, const void* h_state_v, long n, int real);   // lines a call on n samples completes; < 0 for bad arguments
 size_t spectrum_scratch_bytes(int rows, long n, const void* h_params_v);         // one launch for a whole call; 0 for bad arguments
 int launch_spectrum_bank(const float2* d_in, long in_stride, int rows, long n, const float* d_window, const void* h_params_v, float2* d_hist_io,
                          float* d_acc_io, void* h_state_io, void* d_out, long out_stride_bytes, void* d_scratch, size_t scratch_bytes, int* launches,
                          cudaStream_t st);   // SpectrumParams and SpectrumState on the host; returns lines written per row
+int launch_spectrum_bank_f(const float* d_in, long in_stride, int rows, long n, const float* d_window, const void* h_params_v, float* d_hist_io,
+                           float* d_acc_io, void* h_state_io, void* d_out, long out_stride_bytes, void* d_scratch, size_t scratch_bytes, int* launches,
+                           cudaStream_t st);   // the real-input bank: d_window 2N floats, d_hist_io [rows][2N] floats
 
 // fused shared-input DDC bank, ddc_bank.cu
 int ddc_bank_geometry(int decimation, int taps_length);               // 0 when the bank serves (decimation, taps_length); else -2 with the error set

@@ -16,7 +16,8 @@
  *                   [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty|wfm] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B] [--resample I:D[:BW]]
  *                   [--wfm-rate R] [--tau T]
  *                   [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]
- *                   [--waterfall SINK [--fft-size N] [--fft-every E] [--fft-averages A] [--fft-add-db X] [--fft-window W] [--fft-compression adpcm|none]]
+ *                   [--waterfall SINK [--fft-size N] [--fft-every E] [--fft-averages A] [--fft-add-db X] [--fft-window W] [--fft-compression adpcm|none]
+ *                    [--fft-real]]
  *                   RATE:SINK [RATE:SINK ...]
  *   --tail: nfm (default) the README.md:87 tail, s16; none the raw discriminator output, f32; am / usb / lsb the AM and SSB graphs of README.md:95 and :110
  *   behind the DDC's complex baseband (see bb_tail_t), s16; iq the complex baseband itself, cf32; bpsk31 the BPSK31 receive chain
@@ -53,8 +54,8 @@
  *   and every tail works behind it.  A station at frequency f of a real stream sampled at fs is tuned with RATE = -f/fs (shift_addition_fc moves
  *   it to 0 Hz); +f/fs selects its mirror image, the conjugate: sidebands swapped and the discriminator negated.  E.g. 7.074 MHz FT8 from an RX888 at
  *   64.8 Msps, 48 kHz baseband: --real-s16 --decimation 1350 --bw 0.0008 --tail usb -0.10916667:ft8.s16.  --devices expands a real block to
- *   x + 0j on the host and runs the complex multi-GPU bank (the same outputs); --waterfall needs complex input (a real stream's waterfall is
- *   fft_fc, a real-to-complex transform this build does not have).
+ *   x + 0j on the host and runs the complex multi-GPU bank (the same outputs).  A real stream's waterfall is fft_fc's one-sided spectrum:
+ *   --waterfall SINK --fft-real (below).
  *   --devices: the channels are sliced over several GPUs of this node (csdrb_multi_bank_*: the block goes to the first device once and on to
  *   the others by NCCL broadcast), one block of latency more (two blocks are kept in flight); the audio tail (nfm, am, usb, lsb), audio-rate work, runs on
  *   the first device for all channels, through the same kernels as without --devices; so do the bpsk31 and rtty decoders and the wfm tail.
@@ -66,6 +67,11 @@
  *   writes N floats of dB per line).  The sink gets the CLI pipe's lines on the whole stream, byte for byte.  At 2.4 Msps,
  *     rtl_sdr -s 2400000 - | csdr-bankd --waterfall wf.fifo --fft-size 4096 --fft-every 4096 --fft-averages 64 -0.1:ch1.s16 0.2:ch2.s16
  *   gives about 9 lines/s (2.4e6 / 4096 / 64).
+ *   --fft-real (with --real-s16 | --real-f32): the waterfall of a real stream, fft_fc N E W | logaveragepower_cf X N A [| compress_fft_adpcm_f_u8 N]
+ *   (csdrb_spectrum_bank_f on the block's real floats, where they already are on the device; with --devices the real floats of the host
+ *   conversion go to the first device).  N counts bins (2N real samples per frame), --fft-every counts real samples and defaults to 2N, the lines
+ *   run from DC up without a swap.  FT8 at 64.8 Msps with the whole HF waterfall beside it:
+ *     csdr-bankd --real-s16 --decimation 1350 --bw 0.0008 --tail usb --waterfall wf.bin --fft-real --fft-size 16384 -0.10916667:ft8.s16
  * Sinks never hold the stream up: a sink that cannot take a block within 200 ms loses the rest of that block (counted on stderr at exit), one
  * that fails is dropped -- nmux's policy for slow clients (tsmpool.cpp:101-117, nmux.cpp:339-346).  The waterfall sink loses whole lines only
  * (a partial line would shift every later line): a line that cannot start within the block's 200 ms is dropped, one that started is finished.
@@ -645,15 +651,16 @@ static void wfm_tail_push(wfm_tail_t *t, channel_t *chan, int n, void *stream)
  * One row of csdrb_spectrum_bank_cf over the block's fresh cf32 samples: the bank carries the framing and the partial line from block to block, so
  * the sink gets the bytes of the CLI pipe on the whole stream.  Device buffers of ONE device (the single-GPU path's own, the first device of --devices);
  * d_in holds the block for --devices, whose samples arrive in host memory. */
-typedef struct { int fft_size, every, averages, compress; float add_db; window_t window; } waterfall_opts_t;
+typedef struct { int fft_size, every, averages, compress; float add_db; window_t window; int real; } waterfall_opts_t;   /* real: --fft-real */
 
 typedef struct {
     csdrb_spectrum_params_t p;
     csdrb_spectrum_state_t s;
     size_t line_bytes, sb;
     long cap;                                                   /* lines one block can complete */
+    int real;                                                   /* --fft-real: csdrb_spectrum_bank_f on real samples, d_hist / d_in hold floats */
     float *d_window, *d_acc;
-    complexf *d_hist, *d_in;
+    void *d_hist, *d_in;
     unsigned char *d_lines, *h_lines;
     void *d_scratch;
     channel_t sink;
@@ -662,26 +669,29 @@ typedef struct {
 
 static void waterfall_init(waterfall_t *w, const waterfall_opts_t *o, int block, int need_in, void *stream)
 {
-    const int fft_size = o->fft_size;
+    const int fft_size = o->fft_size, frame = o->real ? 2 * fft_size : fft_size;       /* fft_fc's frame is 2N real samples */
+    const size_t ssz = o->real ? sizeof(float) : sizeof(complexf);
     const csdrb_spectrum_params_t p = {fft_size, o->every, o->averages, o->compress, o->add_db};
     w->p = p;
+    w->real = o->real;
     w->s.consumed = 0; w->s.frames = 0;
     w->lines_dropped = 0;
     w->line_bytes = o->compress ? (size_t)(fft_size + 10) / 2 : sizeof(float) * (size_t)fft_size;
     w->cap = ((long)block + o->every - 1) / o->every / o->averages + 1;
     /* one launch per block when that takes at most 64 MB of scratch, else chunks of frames (same bytes) */
-    const size_t full = csdrb_spectrum_bank_scratch_bytes(1, block, &w->p), one = csdrb_spectrum_bank_scratch_bytes(1, 1, &w->p), cap = (size_t)64 << 20;
+    size_t (*scratch_bytes)(int, long, const csdrb_spectrum_params_t *) = o->real ? csdrb_spectrum_bank_scratch_bytes_f : csdrb_spectrum_bank_scratch_bytes;
+    const size_t full = scratch_bytes(1, block, &w->p), one = scratch_bytes(1, 1, &w->p), cap = (size_t)64 << 20;
     w->sb = full <= cap ? full : (one > cap ? one : cap);
-    float *h_window = precalculate_window(fft_size, o->window);
-    w->d_window = csdrb_device_alloc(sizeof(float) * (size_t)fft_size);
+    float *h_window = precalculate_window(frame, o->window);
+    w->d_window = csdrb_device_alloc(sizeof(float) * (size_t)frame);
     w->d_acc = csdrb_device_alloc(sizeof(float) * (size_t)fft_size);            /* zero-filled: the first line starts from 0 */
-    w->d_hist = csdrb_device_alloc(sizeof(complexf) * (size_t)fft_size);        /* zero-filled: samples before the stream are 0 */
-    w->d_in = need_in ? csdrb_device_alloc(sizeof(complexf) * (size_t)block) : NULL;
+    w->d_hist = csdrb_device_alloc(ssz * (size_t)frame);                        /* zero-filled: samples before the stream are 0 */
+    w->d_in = need_in ? csdrb_device_alloc(ssz * (size_t)block) : NULL;
     w->d_lines = csdrb_device_alloc(w->line_bytes * (size_t)w->cap);
     w->h_lines = csdrb_host_alloc(w->line_bytes * (size_t)w->cap);
     w->d_scratch = csdrb_device_alloc(w->sb);
     if (!h_window || !w->d_window || !w->d_acc || !w->d_hist || (need_in && !w->d_in) || !w->d_lines || !w->h_lines || !w->d_scratch) die("out of memory");
-    OK(csdrb_copy_h2d(w->d_window, h_window, sizeof(float) * (size_t)fft_size, stream));
+    OK(csdrb_copy_h2d(w->d_window, h_window, sizeof(float) * (size_t)frame, stream));
     OK(csdrb_stream_synchronize(stream));
     free(h_window);
 }
@@ -711,12 +721,15 @@ static void write_lines(waterfall_t *w, long lines)
     }
 }
 
-/* n fresh wideband samples at d_fresh (on the stream's device): the lines they complete to the waterfall sink */
-static void waterfall_push(waterfall_t *w, const complexf *d_fresh, int n, void *stream)
+/* n fresh wideband samples at d_fresh (on the stream's device; cf32, or f32 with --fft-real): the lines they complete to the waterfall sink */
+static void waterfall_push(waterfall_t *w, const void *d_fresh, int n, void *stream)
 {
-    const int lines = csdrb_spectrum_bank_cf(d_fresh, n, 1, n, w->d_window, &w->p, w->d_hist, w->d_acc, &w->s, w->d_lines, (long)(w->line_bytes * (size_t)w->cap),
-                                             w->d_scratch, w->sb, stream);
-    if (lines < 0) die("csdrb_spectrum_bank_cf failed");
+    const long pitch = (long)(w->line_bytes * (size_t)w->cap);
+    const int lines = w->real ? csdrb_spectrum_bank_f((const float *)d_fresh, n, 1, n, w->d_window, &w->p, (float *)w->d_hist, w->d_acc, &w->s, w->d_lines, pitch,
+                                                      w->d_scratch, w->sb, stream)
+                              : csdrb_spectrum_bank_cf((const complexf *)d_fresh, n, 1, n, w->d_window, &w->p, (complexf *)w->d_hist, w->d_acc, &w->s, w->d_lines,
+                                                       pitch, w->d_scratch, w->sb, stream);
+    if (lines < 0) die(w->real ? "csdrb_spectrum_bank_f failed" : "csdrb_spectrum_bank_cf failed");
     if (lines > w->cap) die("waterfall: more lines than the buffer holds");
     OK(csdrb_copy_d2h(w->h_lines, w->d_lines, w->line_bytes * (size_t)lines, stream));
     OK(csdrb_stream_synchronize(stream));
@@ -865,7 +878,8 @@ static int run_multi(const opts_t *o, channel_t *chan, int C, const float *rates
     complexf *h_wide[2] = {csdrb_host_alloc(sizeof(complexf) * (size_t)block), csdrb_host_alloc(sizeof(complexf) * (size_t)block)};
     unsigned char *h_out[2] = {csdrb_host_alloc(tail.esz * (size_t)C * (size_t)n_out), csdrb_host_alloc(tail.esz * (size_t)C * (size_t)n_out)};
     unsigned char *raw = malloc((size_t)block * (size_t)kWireBytes[fmt]);
-    if (!h_wide[0] || !h_wide[1] || !h_out[0] || !h_out[1] || !raw) die("out of memory");
+    float *h_real = wf && o->wf.real ? csdrb_host_alloc(sizeof(float) * (size_t)block) : NULL;  /* --fft-real: the block's real samples */
+    if (!h_wide[0] || !h_wide[1] || !h_out[0] || !h_out[1] || !raw || (wf && o->wf.real && !h_real)) die("out of memory");
     /* --waterfall: the block's fresh samples go to the first device once more, through the same bank as in the single-GPU path */
     void *wf_stream = wf ? device_stream(o->devs[0]) : NULL;
     if (wf) waterfall_init(wf, &o->wf, block, 1, wf_stream);
@@ -896,7 +910,11 @@ static int run_multi(const opts_t *o, channel_t *chan, int C, const float *rates
             }
         }
         if (!ok) break;
-        if (wf) {
+        if (wf && wf->real) {                                      /* the real floats the conversion produced, without the + 0j */
+            for (int i = 0; i < fresh; i++) h_real[i] = dst[i].i;
+            OK(csdrb_copy_h2d(wf->d_in, h_real, sizeof(float) * (size_t)fresh, wf_stream));
+            waterfall_push(wf, wf->d_in, fresh, wf_stream);
+        } else if (wf) {
             OK(csdrb_copy_h2d(wf->d_in, dst, sizeof(complexf) * (size_t)fresh, wf_stream));
             waterfall_push(wf, wf->d_in, fresh, wf_stream);
         }
@@ -931,7 +949,7 @@ static int usage(void)
             "                       sampled at fs is tuned with RATE = -f/fs; +f/fs gives it conjugated (sidebands swapped, discriminator negated).\n"
             "                       FT8 at 7.074 MHz from an RX888 at 64.8 Msps, 48 kHz baseband:\n"
             "                       csdr-bankd --real-s16 --decimation 1350 --bw 0.0008 --tail usb -0.10916667:ft8.s16\n"
-            "                       Not with --waterfall (the waterfall of a real stream is fft_fc, which this build does not have).\n"
+            "                       Its waterfall is fft_fc's one-sided spectrum: --waterfall SINK --fft-real (below).\n"
             "  --tail wfm           broadcast FM: per channel fmdemod_quadri_cf | fractional_decimator_ff R | deemphasis_wfm_ff 48000 T | convert_f_s16,\n"
             "                       in the CLI's calls of 1024 samples; the sinks get s16 audio.  --wfm-rate R (default 5, above 1 and at most 16)\n"
             "                       takes wideband/decimation to 48 kHz; --tau T (default 50e-6; 75e-6 in the Americas).  Not with --resample.\n"
@@ -961,6 +979,11 @@ static int usage(void)
             "                       adpcm|none (default adpcm: (N + 10) / 2 bytes per line; none: N floats of dB).  A slow sink loses whole\n"
             "                       lines only.  At 2.4 Msps, about 9 lines/s of 4096 bins:\n"
             "                       csdr-bankd --waterfall wf.fifo --fft-size 4096 --fft-every 4096 --fft-averages 64 -0.1:ch1.s16 0.2:ch2.s16\n"
+            "  --fft-real           with --real-s16 | --real-f32: the real stream's waterfall fft_fc N E W | logaveragepower_cf X N A\n"
+            "                       [| compress_fft_adpcm_f_u8 N] instead: N bins (2N real samples per frame) from DC up, --fft-every E in\n"
+            "                       real samples (default 2N).  The whole HF band from an RX888 beside an FT8 channel:\n"
+            "                       csdr-bankd --real-s16 --decimation 1350 --bw 0.0008 --tail usb --waterfall wf.bin --fft-real --fft-size 16384\n"
+            "                       -0.10916667:ft8.s16\n"
             "  see the head of csdr_b200/host/bankd.c for the other options\n");
     return 2;
 }
@@ -1003,6 +1026,7 @@ int main(int argc, char **argv)
         else if (!strcmp(arg, "--fft-every") && v) { o.wf.every = atoi(v); wf_opts = 1; if (o.wf.every < 1) die("--fft-every must be at least 1"); a++; }
         else if (!strcmp(arg, "--fft-averages") && v) { o.wf.averages = atoi(v); wf_opts = 1; a++; }
         else if (!strcmp(arg, "--fft-add-db") && v) { o.wf.add_db = (float)atof(v); wf_opts = 1; a++; }
+        else if (!strcmp(arg, "--fft-real")) { o.wf.real = 1; wf_opts = 1; }
         else if (!strcmp(arg, "--fft-window") && v) { o.wf.window = firdes_get_window_from_string((char *)v); wf_opts = 1; a++; }
         else if (!strcmp(arg, "--fft-compression") && v) {
             if (!strcmp(v, "adpcm")) o.wf.compress = 1;
@@ -1063,16 +1087,18 @@ int main(int argc, char **argv)
         }
     }
     const int fmt = o.fmt, D = o.D, block = o.block, real = fmt == IN_REAL_S16 || fmt == IN_REAL_F32;
-    if (real && o.wf_sink) die("--waterfall needs a complex input: the waterfall of a real stream is fft_fc, a real-to-complex transform this build does not have");
-    if (wf_opts && !o.wf_sink) die("--fft-size, --fft-every, --fft-averages, --fft-add-db, --fft-window and --fft-compression belong to --waterfall");
+    if (real && o.wf_sink && !o.wf.real)
+        die("--waterfall needs a complex input; the waterfall of a real stream is fft_fc's one-sided spectrum: add --fft-real");
+    if (o.wf.real && !real) die("--fft-real takes a real input (--real-s16 or --real-f32)");
+    if (wf_opts && !o.wf_sink) die("--fft-size, --fft-every, --fft-averages, --fft-add-db, --fft-window, --fft-compression and --fft-real belong to --waterfall");
     waterfall_t wf, *wfp = NULL;
     memset(&wf, 0, sizeof wf);
     if (o.wf_sink) {
-        if (o.wf.every == 0) o.wf.every = o.wf.fft_size;
+        if (o.wf.every == 0) o.wf.every = o.wf.real ? 2 * o.wf.fft_size : o.wf.fft_size;      /* fft_fc's frame is 2N real samples */
         if (o.wf.averages < 1) die("--fft-averages must be at least 1");
         const csdrb_spectrum_params_t p = {o.wf.fft_size, o.wf.every, o.wf.averages, o.wf.compress, o.wf.add_db};
         const csdrb_spectrum_state_t s0 = {0, 0};
-        if (csdrb_spectrum_bank_lines(&p, &s0, 0) < 0) die("--fft-size must be a power of two from 2 to 16384");
+        if (csdrb_spectrum_bank_lines(&p, &s0, 0) < 0) die(o.wf.real ? "--fft-size must be a power of two from 2 to 16384 (bins)" : "--fft-size must be a power of two from 2 to 16384");
         wf.sink.rate = 0.f; wf.sink.sink = o.wf_sink; wf.sink.fd = -1;
         wfp = &wf;
     }
@@ -1134,7 +1160,7 @@ int main(int argc, char **argv)
             OK(csdrb_convert_s16_f((const short *)d_raw, d_stage, fresh_n, stream));
             OK(csdrb_copy_d2d(fresh, d_stage, sizeof(float) * (size_t)fresh_n, stream));
         } else OK(csdrb_copy_h2d(fresh, h_in, fresh_bytes, stream));
-        if (wfp) waterfall_push(wfp, (const complexf *)fresh, fresh_n, stream);   /* the waterfall of the same samples, lines to its sink */
+        if (wfp) waterfall_push(wfp, fresh, fresh_n, stream);       /* the waterfall of the same samples (cf32, or f32 with --fft-real), lines to its sink */
         const int n_in = block;
 
         /* 2. shift | fir_decimate | fmdemod for every channel, the new outputs straight into the tail's input rows */

@@ -408,6 +408,45 @@ static int cmd_fft_cc(int argc, char **argv)                               /* cs
     }
 }
 
+/* csdr.c:3414-3498: the spectrum of a real stream, N bins of a 2N-point r2c transform per frame (no Nyquist bin, no half swap).  Frames overlap
+ * like fft_cc's for E <= 2N; for E > 2N the reference reads 2N floats and then skips E - 2N COMPLEX samples (its skip counts floats but freads
+ * sizeof(complexf) items), so frames start 2E - 2N samples apart -- reproduced here, as the pipes downstream expect.  The first frames of an
+ * overlapped stream see zeros before the stream (the reference reads an uninitialised buffer there). */
+static int cmd_fft_fc(int argc, char **argv)
+{
+    if (argc <= 3) return complain("need required parameters (fft_out_size, out_of_every_n_samples)");
+    int out_size = 0; sscanf(argv[2], "%d", &out_size);
+    if (log2n(out_size) == -1) return complain("fft_out_size should be power of 2");
+    if (out_size < 2 || out_size > (1 << 20)) return complain("fft_out_size must be from 2 to 1048576 bins (a real transform of 4 to 2097152 points)");
+    const int in_size = 2 * out_size;
+    int every = 0; sscanf(argv[3], "%d", &every);
+    if (every < 1) return complain("out_of_every_n_samples must be at least 1");
+    window_t window = WINDOW_DEFAULT;
+    if (argc >= 5) window = firdes_get_window_from_string(argv[4]);
+    if (!open_block()) return -2;
+    announce_block(out_size);
+    float *in = fft_malloc(sizeof(float) * (size_t)in_size), *win = fft_malloc(sizeof(float) * (size_t)in_size);
+    complexf *out = fft_malloc(sizeof(complexf) * (size_t)(out_size + 1)), *skip = must_alloc(sizeof(complexf) * (size_t)block);   /* r2c: N + 1 bins */
+    FFT_PLAN_T *plan = make_fft_r2c(in_size, win, out, 0);
+    if (!plan) return complain("FFT size error.");
+    float *table = precalculate_window(in_size, window);
+    memset(in, 0, sizeof(float) * (size_t)in_size);
+    for (;;) {
+        if (feof(stdin)) return 0;
+        if (every > in_size) {
+            fread(in, sizeof(float), (size_t)in_size, stdin);
+            for (int remain = every - in_size; remain > 0; remain -= block) fread(skip, sizeof(complexf), (size_t)(remain < block ? remain : block), stdin);
+        } else {
+            memmove(in, in + every, sizeof(float) * (size_t)(in_size - every));
+            fread(in + in_size - every, sizeof(float), (size_t)every, stdin);
+        }
+        apply_precalculated_window_f(in, win, in_size, table);
+        fft_execute(plan);
+        fwrite(out, sizeof(complexf), (size_t)out_size, stdout);
+        end_of_block();
+    }
+}
+
 static int cmd_logpower_cf(int argc, char **argv)                          /* csdr.c:1645-1661 */
 {
     float add_db = 0; if (argc >= 3) sscanf(argv[2], "%g", &add_db);
@@ -1027,6 +1066,7 @@ static const struct { const char *name; int (*run)(int, char **); const char *sy
     {"shift_addfast_cc", cmd_shift_addfast_cc, "shift_addfast_cc <rate> | --fifo <fifo_path> | --fd <fd>"},
     {"decimating_shift_addition_cc", cmd_decimating_shift_addition_cc, "decimating_shift_addition_cc <rate> [decimation]"},
     {"fft_cc", cmd_fft_cc, "fft_cc <fft_size> <out_of_every_n_samples> [window]"},
+    {"fft_fc", cmd_fft_fc, "fft_fc <fft_out_size> <out_of_every_n_samples> [window]"},
     {"logpower_cf", cmd_logpower_cf, "logpower_cf [add_db]"},
     {"logaveragepower_cf", cmd_logaveragepower_cf, "logaveragepower_cf <add_db> <fft_size> <avgnumber>"},
     {"deemphasis_wfm_ff", cmd_deemphasis_wfm_ff, "deemphasis_wfm_ff <sample_rate> <tau>"},

@@ -144,6 +144,7 @@ ima_adpcm_state_t encode_ima_adpcm_i16_u8(short *input, unsigned char *output, i
 float *precalculate_window(int size, window_t window);                                   /* host table, malloc'ed like the reference's */
 void  apply_window_c(complexf *input, complexf *output, int size, window_t window);
 void  apply_precalculated_window_c(complexf *input, complexf *output, int size, float *windowt);
+void  apply_precalculated_window_f(float *input, float *output, int size, float *windowt);                 /* host loop, libcsdr.c:1278-1282 */
 void  logpower_cf(complexf *input, float *output, int size, float add_db);
 void  accumulate_power_cf(complexf *input, float *output, int size);
 void  log_ff(float *input, float *output, int size, float add_db);
@@ -169,6 +170,8 @@ float shift_addfast_cc(complexf *input, complexf *output, int input_size, shift_
 struct fft_plan_s { int size; void *input; void *output; void *plan; };
 #define FFT_PLAN_T struct fft_plan_s
 FFT_PLAN_T *make_fft_c2c(int size, complexf *input, complexf *output, int forward, int benchmark);
+/* fft_fftw.c:16-24: a forward r2c plan of `size` real points (a power of two, 4..2097152); fft_execute writes size/2 + 1 bins to output */
+FFT_PLAN_T *make_fft_r2c(int size, float *input, complexf *output, int benchmark);
 void  fft_execute(FFT_PLAN_T *plan);
 void  fft_destroy(FFT_PLAN_T *plan);
 void *csdrb_fft_malloc(size_t bytes);            /* stands in for the fft_malloc macro (fft_fftw.h:11) */
@@ -404,6 +407,23 @@ size_t csdrb_spectrum_bank_scratch_bytes(int rows, long n, const csdrb_spectrum_
 int csdrb_spectrum_bank_cf(const complexf *d_in, long in_stride, int rows, long n, const float *d_window, const csdrb_spectrum_params_t *p,
                            complexf *d_hist_io, float *d_acc_io, csdrb_spectrum_state_t *state_io, void *d_out, long out_stride_bytes,
                            void *d_scratch, size_t scratch_bytes, void *stream);
+/* Real-input waterfall bank: `fft_fc N E W | logaveragepower_cf ADD_DB N A [| compress_fft_adpcm_f_u8 N]` (csdr.c:3414-3498) on `rows` real
+ * streams, with the parameters and state structs of the complex bank.  fft_size = N is the number of bins (fft_fc's argument, a power of two in
+ * 2..16384); a frame is 2N real samples and n, every and the state count real samples.
+ *   framing : frame k is [(k+1)E - 2N, (k+1)E) for E <= 2N; for E > 2N fft_fc skips E - 2N complex samples after each frame (its skip counts
+ *             floats but reads complexf items), so frame k is [k(2E - 2N), k(2E - 2N) + 2N).  Samples before the stream are 0.  d_window is
+ *             precalculate_window(2N, W) (device, 2N floats).
+ *   line j  : bins 0..N-1 of frames jA .. jA+A-1 (no half swap, no Nyquist bin), power summed and converted as in the complex bank; N floats or
+ *             (N + 10) / 2 ADPCM bytes.
+ * Bits: those of apply_precalculated_window_f -> csdrb_fft_r2c_batch -> csdrb_accumulate_power_cf (A frames) -> csdrb_log_ff
+ * [-> csdrb_compress_fft_adpcm_rows_f_u8].  d_hist_io is [rows][2N] floats (zero at stream start), d_acc_io [rows][N] floats.  Any cut into
+ * calls and any scratch down to one frame per row give the same bytes.  Returns the lines written per row; -1 for bad arguments (as the complex
+ * bank; input, history, accumulator, window and float output 4-byte aligned, scratch 16), -2 for an unsupported fft_size. */
+long csdrb_spectrum_bank_lines_f(const csdrb_spectrum_params_t *p, const csdrb_spectrum_state_t *s, long n);
+size_t csdrb_spectrum_bank_scratch_bytes_f(int rows, long n, const csdrb_spectrum_params_t *p);
+int csdrb_spectrum_bank_f(const float *d_in, long in_stride, int rows, long n, const float *d_window, const csdrb_spectrum_params_t *p,
+                          float *d_hist_io, float *d_acc_io, csdrb_spectrum_state_t *state_io, void *d_out, long out_stride_bytes,
+                          void *d_scratch, size_t scratch_bytes, void *stream);
 /* shift_math_cc bank: d_rates[c] is the plain rate argument; d_phase_io[c] the carried float phase.  The phase chain is sequential over the
  * whole block (one thread per channel walks it), the rotation itself runs fully parallel. */
 size_t csdrb_shift_math_bank_scratch_bytes(int channels, int input_size);
@@ -540,6 +560,13 @@ int csdrb_fft_c2c_batch(const complexf *d_in, long in_stride, complexf *d_out, l
  * 2^21/size transforms (four-step algorithm, csrc/fft_large.cuh), the intermediate in stream-ordered scratch of at most 16 MiB; out of place
  * (d_out must not overlap d_in); the call does not wait for the device.  -1 for any other size (nothing is launched). */
 int csdrb_fft_c2c_large_batch(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int size, int batch, int inverse, void *stream);
+/* Forward real-to-complex DFT (FFTW's r2c, sign -1): `size` real points per row (a power of two, 4..2097152 = 2^21) -> size/2 + 1 bins, the
+ * imaginary parts of bins 0 and size/2 exactly 0.  Rows may start at any float (in_stride in floats, out_stride in complexf); with batch > 1 they
+ * must not overlap (in_stride >= size, out_stride >= size/2 + 1).  The size/2-point c2c of the packed pairs x[2n] + i x[2n+1] (single CTA up to
+ * 32768 real points, above that the four-step transform of csdrb_fft_c2c_large_batch written into d_out) and a split with a per-size table;
+ * out of place; the call does not wait for the device.  -1 for a null pointer, another size or overlapping rows (nothing is launched); 0 for
+ * batch <= 0. */
+int csdrb_fft_r2c_batch(const float *d_in, long in_stride, complexf *d_out, long out_stride, int size, int batch, void *stream);
 
 /* K9 overlap-add FFT filter bank = bandpass_fir_fft_cc block loop (csdr.c:1872-1883) for many channels.
  * d_taps_fft: FFT of the zero-padded taps (taps_stride 0 = shared); d_tail_io [channels][fft_size] carries the
