@@ -127,20 +127,10 @@ int launch_fastdcblock_bank(const void* d_in, long in_stride, int cf32, float* d
     if (in_stride < (long)block * nblocks || out_stride < (long)block * nblocks) { set_error("fastdcblock bank: row stride shorter than the row"); return -1; }
     const size_t smem = (size_t)block * sizeof(float);
     const dim3 grid((unsigned)((nblocks + DC_RUN - 1) / DC_RUN), (unsigned)channels);
-    if (cf32) {
-        CSDRB_CUDA(cudaFuncSetAttribute(am_front_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CSDRB_CUDA(cudaFuncSetAttribute(am_front_carry_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        am_front_kernel<true><<<grid, DC_THREADS, smem, st>>>(d_in, in_stride, d_out, out_stride, block, nblocks, d_last_dc_io);
-        CSDRB_CUDA(cudaGetLastError());
-        am_front_carry_kernel<true><<<channels, DC_THREADS, smem, st>>>(d_in, in_stride, block, nblocks, d_last_dc_io);
-    } else {
-        CSDRB_CUDA(cudaFuncSetAttribute(am_front_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        CSDRB_CUDA(cudaFuncSetAttribute(am_front_carry_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        am_front_kernel<false><<<grid, DC_THREADS, smem, st>>>(d_in, in_stride, d_out, out_stride, block, nblocks, d_last_dc_io);
-        CSDRB_CUDA(cudaGetLastError());
-        am_front_carry_kernel<false><<<channels, DC_THREADS, smem, st>>>(d_in, in_stride, block, nblocks, d_last_dc_io);
-    }
-    CSDRB_CUDA(cudaGetLastError());
+    CSDRB_CUDA(launch_kernel(cf32 ? am_front_kernel<true> : am_front_kernel<false>, grid, DC_THREADS, smem, st, d_in, in_stride, d_out, out_stride, block, nblocks,
+                             d_last_dc_io));
+    CSDRB_CUDA(launch_kernel(cf32 ? am_front_carry_kernel<true> : am_front_carry_kernel<false>, channels, DC_THREADS, smem, st, d_in, in_stride, block, nblocks,
+                             d_last_dc_io));
     return 2;
 }
 

@@ -48,6 +48,24 @@ T& per_device()
     return *per_dev[(size_t)dev];
 }
 
+// k<<<grid, block, smem, st>>>(args...), returning the launch's error.  Above 47 KB of dynamic shared memory the kernel's limit is raised first, on
+// every call: the attribute belongs to the current device's context, and the 48 KB default also has to hold the kernel's static shared memory.
+#if defined(__CUDACC__) || defined(CSDRB_HOST_EMULATION)
+template <typename K, typename... A>
+cudaError_t launch_kernel(K k, dim3 grid, dim3 block, size_t smem, cudaStream_t st, A... args)
+{
+    if (smem > 47 * 1024) {
+        if (cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) return e;
+    }
+#ifdef CSDRB_HOST_EMULATION
+    ::cuda_emul::cfg(grid, block, smem, st).run(k, args...);         // what tests/host_shim/emul_build.py makes of a launch in a .cu file
+#else
+    k<<<grid, block, smem, st>>>(args...);
+#endif
+    return cudaGetLastError();
+}
+#endif
+
 // The inline-PTX helpers below have C++ models in tests/host_shim/cuda_emul.h (CPU test tier); the product never defines this macro.
 #ifndef CSDRB_HOST_EMULATION
 // ---- complex-lane FP32 pairs ------------------------------------------------------------------

@@ -28,98 +28,55 @@
 
 namespace csdrb {
 
-// ---- twiddle tables ------------------------------------------------------------------------------
-static std::map<int, float2*> g_tw;
-static std::mutex g_tw_mu;
+// ---- device tables -------------------------------------------------------------------------------
+// Every twiddle table the FFT kernels read, per device (a process may csdrb_set_device() between calls), kind and size: filled on the host in
+// double and rounded once, uploaded on first use.
+enum FftTableKind { kTwRadix8, kTwRadix16, kTwLargeStep, kTwRfftSplit };
 
-int get_twiddles(int n, const float2** out, cudaStream_t st)
-{
-    std::lock_guard<std::mutex> lk(g_tw_mu);
-    auto it = g_tw.find(n);
-    if (it != g_tw.end()) { *out = it->second; return 0; }
-    std::vector<float2> h((size_t)3 * n);
-    fft_fill_twiddles(n, h.data());
-    float2* d = nullptr;
-    CSDRB_CUDA(cudaMalloc(&d, sizeof(float2) * h.size()));
-    CSDRB_CUDA(cudaMemcpyAsync(d, h.data(), sizeof(float2) * h.size(), cudaMemcpyHostToDevice, st));
-    CSDRB_CUDA(cudaStreamSynchronize(st));
-    g_tw[n] = d;
-    *out = d;
-    return 0;
-}
+struct FftTables { std::mutex mu; std::map<std::pair<int, int>, float2*> by_kind_n; };
 
-static std::map<int, float2*> g_tw16;
-int get_twiddles16(int n, const float2** out, cudaStream_t st)
+static int fft_table(FftTableKind kind, int n, const float2** out, cudaStream_t st)
 {
-    std::lock_guard<std::mutex> lk(g_tw_mu);
-    auto it = g_tw16.find(n);
-    if (it != g_tw16.end()) { *out = it->second; return 0; }
-    std::vector<float2> h((size_t)4 * n);
-    fft16_fill_twiddles(n, h.data());
-    float2* d = nullptr;
-    CSDRB_CUDA(cudaMalloc(&d, sizeof(float2) * h.size()));
-    CSDRB_CUDA(cudaMemcpyAsync(d, h.data(), sizeof(float2) * h.size(), cudaMemcpyHostToDevice, st));
-    CSDRB_CUDA(cudaStreamSynchronize(st));
-    g_tw16[n] = d;
-    *out = d;
-    return 0;
-}
-
-template <int N>
-static int launch_c2c16_n(const float2* in, long is, float2* out, long os, int batch, bool inverse, const float2* tw16, cudaStream_t st)
-{
-    const size_t smem = sizeof(float2) * fft_smem_elems(N);
-    if (inverse) {
-        auto k = fft_c2c_batch16_kernel<N, true>;
-        if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k<<<batch, fft16_threads(N), smem, st>>>(in, is, out, os, tw16);
-    } else {
-        auto k = fft_c2c_batch16_kernel<N, false>;
-        if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k<<<batch, fft16_threads(N), smem, st>>>(in, is, out, os, tw16);
+    FftTables& c = per_device<FftTables>();
+    std::lock_guard<std::mutex> lk(c.mu);
+    auto it = c.by_kind_n.find({kind, n});
+    if (it == c.by_kind_n.end()) {
+        std::vector<float2> h;
+        switch (kind) {
+        case kTwRadix8: h.resize((size_t)3 * n); fft_fill_twiddles(n, h.data()); break;
+        case kTwRadix16: h.resize((size_t)4 * n); fft16_fill_twiddles(n, h.data()); break;
+        case kTwLargeStep:                                              // four-step inter-step twiddles: kFftLargeSplit low powers, then n / kFftLargeSplit high ones
+            h.resize((size_t)kFftLargeSplit + n / kFftLargeSplit);
+            for (int m = 0; m < (int)h.size(); m++) {
+                const double a = -2.0 * 3.14159265358979323846 * (m < kFftLargeSplit ? (double)m : (double)kFftLargeSplit * (m - kFftLargeSplit)) / (double)n;
+                h[(size_t)m] = make_float2((float)cos(a), (float)sin(a));
+            }
+            break;
+        case kTwRfftSplit: h.resize((size_t)n / 2 + 1); rfft_fill_twiddles(n, h.data()); break;
+        }
+        float2* d = nullptr;
+        CSDRB_CUDA(cudaMalloc(&d, sizeof(float2) * h.size()));
+        CSDRB_CUDA(cudaMemcpyAsync(d, h.data(), sizeof(float2) * h.size(), cudaMemcpyHostToDevice, st));
+        CSDRB_CUDA(cudaStreamSynchronize(st));                           // h leaves scope; once per device, kind and size
+        it = c.by_kind_n.emplace(std::make_pair((int)kind, n), d).first;
     }
-    CSDRB_CUDA(cudaGetLastError());
-    return 1;
+    *out = it->second;
+    return 0;
 }
+
+int row_fft_twiddles(int n, const float2** out, cudaStream_t st) { return fft_table(n >= 32 ? kTwRadix16 : kTwRadix8, n, out, st); }
+int get_rfft_twiddles(int m, const float2** out, cudaStream_t st) { return fft_table(kTwRfftSplit, m, out, st); }
 
 // ---- K7: batched c2c -------------------------------------------------------------------------------
-template <int N>
-static int launch_c2c_n(const float2* in, long is, float2* out, long os, int batch, bool inverse, const float2* tw, cudaStream_t st)
-{
-    const size_t smem = sizeof(float2) * fft_smem_elems(N);
-    if (inverse) {
-        auto k = fft_c2c_batch_kernel<N, true>;
-        if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k<<<batch, fft_threads(N), smem, st>>>(in, is, out, os, tw);
-    } else {
-        auto k = fft_c2c_batch_kernel<N, false>;
-        if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k<<<batch, fft_threads(N), smem, st>>>(in, is, out, os, tw);
-    }
-    CSDRB_CUDA(cudaGetLastError());
-    return 1;
-}
-
-#define CSDRB_FFT_SIZES(X) X(2) X(4) X(8) X(16) X(32) X(64) X(128) X(256) X(512) X(1024) X(2048) X(4096) X(8192) X(16384)
-
 int launch_fft_c2c_batch(const float2* d_in, long in_stride, float2* d_out, long out_stride, int n, int batch, int inverse, cudaStream_t st)
 {
     if (batch <= 0) return 0;
     if (n < 2 || n > FFT_MAX_N || (n & (n - 1))) { set_error("fft: size %d unsupported (power of two, 2..%d)", n, FFT_MAX_N); return -1; }
-    // radix-16 passes (fft16.cuh) from 32 points on: fewer passes over shared memory than radix 8 (4096: three instead of four, 16384: four instead of five)
-    if (n >= 32) {
-        const float2* tw16 = nullptr;
-        if (int rc = get_twiddles16(n, &tw16, st)) return rc;
-        switch (n) {
-#define X(N) case N: if constexpr (N >= 32) return launch_c2c16_n<N>(d_in, in_stride, d_out, out_stride, batch, inverse != 0, tw16, st); break;
-            CSDRB_FFT_SIZES(X)
-#undef X
-        }
-    }
     const float2* tw = nullptr;
-    if (int rc = get_twiddles(n, &tw, st)) return rc;
+    if (int rc = row_fft_twiddles(n, &tw, st)) return rc;
     switch (n) {
-#define X(N) case N: if constexpr (N < 32) return launch_c2c_n<N>(d_in, in_stride, d_out, out_stride, batch, inverse != 0, tw, st); break;
+#define X(N) case N: CSDRB_CUDA(launch_kernel(inverse ? fft_c2c_batch_kernel<N, true> : fft_c2c_batch_kernel<N, false>, batch, fft_threads(N), \
+                                              sizeof(float2) * fft_smem_elems(N), st, d_in, in_stride, d_out, out_stride, tw)); return 1;
         CSDRB_FFT_SIZES(X)
 #undef X
     }
@@ -133,8 +90,6 @@ int launch_olafir_bank(const float2* d_in, long in_stride, float2* d_out, long o
     if (channels <= 0 || nblocks <= 0) return 0;
     if (fft_size < 4 || fft_size > 8192 || (fft_size & (fft_size - 1))) { set_error("overlap-add FIR: fft_size %d unsupported (power of two, 4..8192)", fft_size); return -1; }
     if (input_size <= 0 || input_size > fft_size) { set_error("overlap-add FIR: bad input_size %d for fft_size %d", input_size, fft_size); return -1; }
-    const float2* tw = nullptr;
-    if (int rc = get_twiddles(fft_size, &tw, st)) return rc;
     if (blocks_per_cta <= 0) {
         // enough CTAs to fill the machine a few times over, but runs long enough that the recomputed lead-in block stays cheap
         long want = (kSmCount * 8 + channels - 1) / channels;
@@ -142,43 +97,23 @@ int launch_olafir_bank(const float2* d_in, long in_stride, float2* d_out, long o
         if (blocks_per_cta < 16) blocks_per_cta = nblocks < 16 ? nblocks : 16;
     }
     const dim3 grid((nblocks + blocks_per_cta - 1) / blocks_per_cta, channels);
+    const size_t fsmem = sizeof(float2) * ((size_t)fft_smem_elems(fft_size) + 2 * (size_t)(fft_size - input_size));
     // fused kernels: radix-16 passes at 256 and 4096 points, radix-8 passes at the other sizes from 16 on; 4 and 8 points take the staged kernel
-    if (fft_size == 256 || fft_size == 4096) {
-        const float2* tw16 = nullptr;
-        if (int rc = get_twiddles16(fft_size, &tw16, st)) return rc;
-        const size_t fsmem = sizeof(float2) * ((size_t)fft_smem_elems(fft_size) + 2 * (size_t)(fft_size - input_size));
-        if (fft_size == 256) {
-            auto k = olafir_bank_fused16_kernel<256>;
-            k<<<grid, fft16_threads(256), fsmem, st>>>(d_in, in_stride, d_out, out_stride, d_taps_fft, taps_stride, d_tail_io, input_size, nblocks, blocks_per_cta, tw16);
-        } else {
-            auto k = olafir_bank_fused16_kernel<4096>;
-            if (fsmem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
-            k<<<grid, fft16_threads(4096), fsmem, st>>>(d_in, in_stride, d_out, out_stride, d_taps_fft, taps_stride, d_tail_io, input_size, nblocks, blocks_per_cta, tw16);
-        }
-        CSDRB_CUDA(cudaGetLastError());
-        return 1;
-    }
-    if (fft_size >= 16) {
-        const size_t fsmem = sizeof(float2) * ((size_t)fft_smem_elems(fft_size) + 2 * (size_t)(fft_size - input_size));
-        switch (fft_size) {
-#define X(N) case N: if constexpr (N >= 16 && N <= 8192 && N != 256 && N != 4096) { auto k = olafir_bank_fused_kernel<N>; \
-            if (fsmem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem)); \
-            k<<<grid, fft_threads(N), fsmem, st>>>(d_in, in_stride, d_out, out_stride, d_taps_fft, taps_stride, d_tail_io, input_size, nblocks, blocks_per_cta, tw); } break;
-            CSDRB_FFT_SIZES(X)
-#undef X
-        }
-        CSDRB_CUDA(cudaGetLastError());
-        return 1;
-    }
-    const size_t smem = sizeof(float2) * ((size_t)fft_smem_elems(fft_size) + (size_t)fft_size);
+    const bool r16 = fft_size == 256 || fft_size == 4096;
+    const float2* tw = nullptr;
+    if (int rc = fft_table(r16 ? kTwRadix16 : kTwRadix8, fft_size, &tw, st)) return rc;
     switch (fft_size) {
-#define X(N) case N: if constexpr (N == 4 || N == 8) { auto k = olafir_bank_kernel<N>; \
-        if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        k<<<grid, fft_threads(N), smem, st>>>(d_in, in_stride, d_out, out_stride, d_taps_fft, taps_stride, d_tail_io, input_size, nblocks, blocks_per_cta, tw); } break;
+#define X(N) case N: \
+        if constexpr (N == 256 || N == 4096) CSDRB_CUDA(launch_kernel(olafir_bank_fused16_kernel<N>, grid, fft_threads(N), fsmem, st, d_in, in_stride, d_out, out_stride, \
+                                                                      d_taps_fft, taps_stride, d_tail_io, input_size, nblocks, blocks_per_cta, tw)); \
+        else if constexpr (N >= 16 && N <= 8192) CSDRB_CUDA(launch_kernel(olafir_bank_fused_kernel<N>, grid, fft_threads(N), fsmem, st, d_in, in_stride, d_out, out_stride, \
+                                                                           d_taps_fft, taps_stride, d_tail_io, input_size, nblocks, blocks_per_cta, tw)); \
+        else if constexpr (N == 4 || N == 8) CSDRB_CUDA(launch_kernel(olafir_bank_kernel<N>, grid, fft_threads(N), sizeof(float2) * (size_t)(fft_smem_elems(N) + N), st, \
+                                                                      d_in, in_stride, d_out, out_stride, d_taps_fft, taps_stride, d_tail_io, input_size, nblocks, blocks_per_cta, tw)); \
+        break;
         CSDRB_FFT_SIZES(X)
 #undef X
     }
-    CSDRB_CUDA(cudaGetLastError());
     return 1;
 }
 
@@ -188,37 +123,14 @@ int launch_fastddc_fwd(const float2* d_in, float2* d_spectra, float2* d_overlap_
     if (nblocks <= 0) return 0;
     if (fft_size > FFT_MAX_N) return launch_fastddc_fwd_large(d_in, d_spectra, d_overlap_io, fft_size, input_size, nblocks, st);
     if (fft_size < 4 || (fft_size & (fft_size - 1))) { set_error("fastddc_fwd: fft_size %d unsupported (power of two, 4..%d)", fft_size, kFftLargeMaxN); return -1; }
-    if (fft_size >= 32) {                                               // radix-16 passes, as in launch_fft_c2c_batch
-        const float2* tw16 = nullptr;
-        if (int rc = get_twiddles16(fft_size, &tw16, st)) return rc;
-        const size_t smem16 = sizeof(float2) * (size_t)fft_smem_elems(fft_size);
-        switch (fft_size) {
-#define X(N) case N: if constexpr (N >= 32) { auto k = fastddc_fwd16_kernel<N>; \
-            if (smem16 > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem16)); \
-            k<<<nblocks, fft16_threads(N), smem16, st>>>(d_in, d_spectra, d_overlap_io, input_size, tw16); } break;
-            CSDRB_FFT_SIZES(X)
-#undef X
-        }
-        CSDRB_CUDA(cudaGetLastError());
-        const int ov16 = fft_size - input_size;
-        if (ov16 > 0) {
-            fastddc_carry_overlap_kernel<<<1, 1024, 0, st>>>(d_in, d_overlap_io, ov16, (long)nblocks * input_size);
-            CSDRB_CUDA(cudaGetLastError());
-            return 2;
-        }
-        return 1;
-    }
     const float2* tw = nullptr;
-    if (int rc = get_twiddles(fft_size, &tw, st)) return rc;
-    const size_t smem = sizeof(float2) * (size_t)fft_smem_elems(fft_size);
+    if (int rc = row_fft_twiddles(fft_size, &tw, st)) return rc;
     switch (fft_size) {
-#define X(N) case N: if constexpr (N >= 4 && N < 32) { auto k = fastddc_fwd_kernel<N>; \
-        if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        k<<<nblocks, fft_threads(N), smem, st>>>(d_in, d_spectra, d_overlap_io, input_size, tw); } break;
+#define X(N) case N: if constexpr (N >= 4) CSDRB_CUDA(launch_kernel(fastddc_fwd_kernel<N>, nblocks, fft_threads(N), sizeof(float2) * fft_smem_elems(N), st, \
+                                                                d_in, d_spectra, d_overlap_io, input_size, tw)); break;
         CSDRB_FFT_SIZES(X)
 #undef X
     }
-    CSDRB_CUDA(cudaGetLastError());
     const int overlap = fft_size - input_size;
     if (overlap > 0) {
         fastddc_carry_overlap_kernel<<<1, 1024, 0, st>>>(d_in, d_overlap_io, overlap, (long)nblocks * input_size);
@@ -235,16 +147,13 @@ int launch_apply_fir_fft(const float2* d_in, const float2* d_taps_fft, const flo
     if (fft_size > FFT_MAX_N) return launch_apply_fir_fft_large(d_in, d_taps_fft, d_last_overlap, overlap_size, d_out, fft_size, st);
     if (fft_size < 2 || (fft_size & (fft_size - 1))) { set_error("apply_fir_fft: fft_size %d unsupported (power of two, 2..%d)", fft_size, kFftLargeMaxN); return -1; }
     const float2* tw = nullptr;
-    if (int rc = get_twiddles(fft_size, &tw, st)) return rc;
-    const size_t smem = sizeof(float2) * (size_t)fft_smem_elems(fft_size);
+    if (int rc = fft_table(kTwRadix8, fft_size, &tw, st)) return rc;
     switch (fft_size) {
-#define X(N) case N: { auto k = apply_fir_fft_kernel<N>; \
-        if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-        k<<<1, fft_threads(N), smem, st>>>(d_in, d_taps_fft, d_last_overlap, overlap_size, d_out, tw); } break;
+#define X(N) case N: CSDRB_CUDA(launch_kernel(apply_fir_fft_kernel<N>, 1, fft_threads(N), sizeof(float2) * fft_smem_elems(N), st, \
+                                              d_in, d_taps_fft, d_last_overlap, overlap_size, d_out, tw)); break;
         CSDRB_FFT_SIZES(X)
 #undef X
     }
-    CSDRB_CUDA(cudaGetLastError());
     return 1;
 }
 
@@ -280,16 +189,13 @@ int launch_fastddc_inv_apply(const float2* d_spectra, int nblocks, const float2*
                              long out_stride, cudaEvent_t prepared, cudaEvent_t after_fold, cudaStream_t st)
 {
     const float2* tw = nullptr;
-    if (int rc = get_twiddles(fft_inv_size, &tw, st)) return rc;
+    if (int rc = fft_table(kTwRadix8, fft_inv_size, &tw, st)) return rc;
     const size_t fsmem = sizeof(float2) * (size_t)FOLD_ST * 2 * (2 * FOLD_BT) * FOLD_R;
     const dim3 fgrid(fft_inv_size / FOLD_R, (channels + 2 * FOLD_CT - 1) / (2 * FOLD_CT), (nblocks + 2 * FOLD_BT - 1) / (2 * FOLD_BT));
     if (fgrid.y > 65535u || fgrid.z > 65535u) { set_error("fastddc_inv: bank too large for one call"); return -1; }
     const float inv_pre = 1.0f / (float)pre_decimation;
     const DdcChan* dc = static_cast<const DdcChan*>(d_chan);
-    // (the attribute belongs to the current device's context: set per call, not latched per process)
-    CSDRB_CUDA(cudaFuncSetAttribute(fastddc_fold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fsmem));
-    fastddc_fold_kernel<<<fgrid, FOLD_NT, fsmem, st>>>(d_spectra, d_taps_fft, dc, folded, fft_size, fft_inv_size, nblocks, channels, inv_pre);
-    CSDRB_CUDA(cudaGetLastError());
+    CSDRB_CUDA(launch_kernel(fastddc_fold_kernel, fgrid, FOLD_NT, fsmem, st, d_spectra, d_taps_fft, dc, folded, fft_size, fft_inv_size, nblocks, channels, inv_pre));
     if (after_fold) CSDRB_CUDA(cudaEventRecord(after_fold, st));
     if (prepared) CSDRB_CUDA(cudaStreamWaitEvent(st, prepared, 0));
     const long npairs = (long)channels * nblocks;
@@ -323,7 +229,7 @@ int launch_fastddc_inv_bank(const float2* d_spectra, int nblocks, const float2* 
     }
     if (!d_scratch || scratch_bytes < fastddc_inv_scratch_bytes(channels, nblocks)) { set_error("fastddc_inv: scratch too small"); return -1; }
     const float2* tw = nullptr;
-    if (int rc = get_twiddles(fft_inv_size, &tw, st)) return rc;
+    if (int rc = fft_table(kTwRadix8, fft_inv_size, &tw, st)) return rc;
     int* blk_remain = static_cast<int*>(d_scratch);
     float* blk_phase = reinterpret_cast<float*>(blk_remain + (size_t)channels * nblocks);
     int* blk_offset = reinterpret_cast<int*>(blk_phase + (size_t)channels * nblocks);
@@ -380,19 +286,13 @@ int launch_fastddc_inv_bank(const float2* d_spectra, int nblocks, const float2* 
         const dim3 tgrid((nblocks + BTv - 1) / BTv, (channels + CTv - 1) / CTv);
         const size_t smem = sizeof(float2) * (size_t)CTv * BTv * fft_smem_elems(fft_inv_size);
         switch (fft_inv_size) {
-#define X(M) case M: if constexpr (M >= 8 && M <= 32) { \
-            if (small_tile) { auto k = fastddc_inv_tiled_kernel<M, 2, 2>; \
-                if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-                k<<<tgrid, 256, smem, st>>>(d_spectra, d_taps_fft, static_cast<const DdcChan*>(d_chan), blk_remain, blk_phase, blk_offset, d_out, out_stride, \
-                                           fft_size, pre_decimation, scrap, post_input_size, post_decimation, nblocks, channels, tw); } \
-            else { auto k = fastddc_inv_tiled_kernel<M, 4, 4>; \
-                if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-                k<<<tgrid, 256, smem, st>>>(d_spectra, d_taps_fft, static_cast<const DdcChan*>(d_chan), blk_remain, blk_phase, blk_offset, d_out, out_stride, \
-                                           fft_size, pre_decimation, scrap, post_input_size, post_decimation, nblocks, channels, tw); } } break;
+#define X(M) case M: if constexpr (M >= 8 && M <= 32) \
+            CSDRB_CUDA(launch_kernel(small_tile ? fastddc_inv_tiled_kernel<M, 2, 2> : fastddc_inv_tiled_kernel<M, 4, 4>, tgrid, 256, smem, st, d_spectra, d_taps_fft, \
+                                     static_cast<const DdcChan*>(d_chan), blk_remain, blk_phase, blk_offset, d_out, out_stride, fft_size, pre_decimation, scrap, \
+                                     post_input_size, post_decimation, nblocks, channels, tw)); break;
             CSDRB_FFT_SIZES(X)
 #undef X
         }
-        CSDRB_CUDA(cudaGetLastError());
         return 2;
     }
     const dim3 grid(nblocks, channels);
@@ -596,50 +496,15 @@ int fastddc_inv_plan_set_state(void* plan, const int* h_remain, const float* h_p
 }
 
 // ==== four-step transforms above FFT_MAX_N points (kernels: fft_large.cuh) ==========================================================================
-// ---- inter-step twiddles, cached per device and size ------------------------------------------------------------------------------------------
-struct LargeTwiddles { std::mutex mu; std::map<int, float2*> by_n; };
-
-static int get_large_twiddles(int n, const float2** lo, const float2** hi, cudaStream_t st)
-{
-    LargeTwiddles& c = per_device<LargeTwiddles>();
-    std::lock_guard<std::mutex> lk(c.mu);
-    auto it = c.by_n.find(n);
-    if (it == c.by_n.end()) {
-        const int nhi = n / kFftLargeSplit;
-        std::vector<float2> h((size_t)kFftLargeSplit + nhi);
-        for (int m = 0; m < kFftLargeSplit + nhi; m++) {
-            const double a = -2.0 * 3.14159265358979323846 * (m < kFftLargeSplit ? (double)m : (double)kFftLargeSplit * (m - kFftLargeSplit)) / (double)n;
-            h[(size_t)m] = make_float2((float)cos(a), (float)sin(a));
-        }
-        float2* d = nullptr;
-        CSDRB_CUDA(cudaMalloc(&d, sizeof(float2) * h.size()));
-        CSDRB_CUDA(cudaMemcpyAsync(d, h.data(), sizeof(float2) * h.size(), cudaMemcpyHostToDevice, st));
-        CSDRB_CUDA(cudaStreamSynchronize(st));                           // h leaves scope; once per device and size
-        it = c.by_n.emplace(n, d).first;
-    }
-    *lo = it->second; *hi = it->second + kFftLargeSplit;
-    return 0;
-}
-
 // ---- launchers -------------------------------------------------------------------------------------------------------------------------------------
 template <int F, bool FIRST, typename In>
 static int launch_step(In in, int in_b0, float2* out, long out_stride, int out_b0, int S, int count, bool inverse, const float2* lo, const float2* hi, cudaStream_t st)
 {
     constexpr int W = kFftLargeTile;
     const float2* tw16 = nullptr;
-    if (int rc = get_twiddles16(F, &tw16, st)) return rc;
-    const size_t smem = sizeof(float2) * (size_t)W * fft_large_seg(F);
-    const dim3 grid(S / W, count);
-    if (inverse) {
-        auto k = fft_large_step_kernel<F, true, FIRST, In>;
-        if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k<<<grid, W * (F / 16), smem, st>>>(in, in_b0, out, out_stride, out_b0, S, tw16, lo, hi);
-    } else {
-        auto k = fft_large_step_kernel<F, false, FIRST, In>;
-        if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k<<<grid, W * (F / 16), smem, st>>>(in, in_b0, out, out_stride, out_b0, S, tw16, lo, hi);
-    }
-    CSDRB_CUDA(cudaGetLastError());
+    if (int rc = fft_table(kTwRadix16, F, &tw16, st)) return rc;
+    CSDRB_CUDA(launch_kernel(inverse ? fft_large_step_kernel<F, true, FIRST, In> : fft_large_step_kernel<F, false, FIRST, In>, dim3(S / W, count), W * (F / 16),
+                             sizeof(float2) * (size_t)W * fft_large_seg(F), st, in, in_b0, out, out_stride, out_b0, S, tw16, lo, hi));
     return 0;
 }
 
@@ -652,8 +517,9 @@ static bool fft_large_size_ok(int n) { return n >= kFftLargeMinN && n <= kFftLar
 template <typename In>
 static int fft_large_run(In in, float2* d_out, long out_stride, int n, int batch, bool inverse, cudaStream_t st)
 {
-    const float2 *lo = nullptr, *hi = nullptr;
-    if (int rc = get_large_twiddles(n, &lo, &hi, st)) return rc;
+    const float2* lo = nullptr;
+    if (int rc = fft_table(kTwLargeStep, n, &lo, st)) return rc;
+    const float2* hi = lo + kFftLargeSplit;
     const int chunk = (int)(kFftLargeScratchBytes / (sizeof(float2) * (size_t)n));
     float2* t = nullptr;
     CSDRB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&t), sizeof(float2) * (size_t)n * (size_t)(batch < chunk ? batch : chunk), st));
@@ -709,26 +575,6 @@ int launch_fastddc_fwd_large(const float2* d_in, float2* d_spectra, float2* d_ov
 }
 
 // ==== real-to-complex transforms (kernels: fft_real.cuh) ===========================================================================================
-struct RfftTwiddles { std::mutex mu; std::map<int, float2*> by_m; };
-
-int get_rfft_twiddles(int m, const float2** out, cudaStream_t st)
-{
-    RfftTwiddles& c = per_device<RfftTwiddles>();
-    std::lock_guard<std::mutex> lk(c.mu);
-    auto it = c.by_m.find(m);
-    if (it == c.by_m.end()) {
-        std::vector<float2> h((size_t)m / 2 + 1);
-        rfft_fill_twiddles(m, h.data());
-        float2* d = nullptr;
-        CSDRB_CUDA(cudaMalloc(&d, sizeof(float2) * h.size()));
-        CSDRB_CUDA(cudaMemcpyAsync(d, h.data(), sizeof(float2) * h.size(), cudaMemcpyHostToDevice, st));
-        CSDRB_CUDA(cudaStreamSynchronize(st));                           // h leaves scope; once per device and size
-        it = c.by_m.emplace(m, d).first;
-    }
-    *out = it->second;
-    return 0;
-}
-
 // the split behind the four-step transform, in place: row r holds Z[0..M) and gets X[0..M]; thread k reads and writes only bins k and M - k
 // (and M for k = 0, which no thread reads)
 __global__ void __launch_bounds__(256)
@@ -740,17 +586,6 @@ fft_r2c_split_kernel(float2* __restrict__ y, long stride, int M, int rows, const
         RfftRowOut dst{y + (long)r * stride};
         rfft_split_pair(k, M, dst.y[k], dst.y[(M - k) & (M - 1)], rtw, dst);
     }
-}
-
-template <int M>
-static int launch_r2c_n(const float* in, long is, float2* out, long os, int batch, const float2* tw, const float2* rtw, cudaStream_t st)
-{
-    const size_t smem = sizeof(float2) * fft_smem_elems(M);
-    auto k = fft_r2c_batch_kernel<M>;
-    if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k<<<batch, rfft_threads(M), smem, st>>>(in, is, out, os, tw, rtw);
-    CSDRB_CUDA(cudaGetLastError());
-    return 1;
 }
 
 int launch_fft_r2c_batch(const float* d_in, long in_stride, float2* d_out, long out_stride, int n, int batch, cudaStream_t st)
@@ -772,10 +607,10 @@ int launch_fft_r2c_batch(const float* d_in, long in_stride, float2* d_out, long 
         return launches + 1;
     }
     const float2* tw = nullptr;
-    if (m >= 32) { if (int rc = get_twiddles16(m, &tw, st)) return rc; }
-    else if (int rc = get_twiddles(m, &tw, st)) return rc;
+    if (int rc = row_fft_twiddles(m, &tw, st)) return rc;
     switch (m) {
-#define X(M) case M: return launch_r2c_n<M>(d_in, in_stride, d_out, out_stride, batch, tw, rtw, st);
+#define X(M) case M: CSDRB_CUDA(launch_kernel(fft_r2c_batch_kernel<M>, batch, fft_threads(M), sizeof(float2) * fft_smem_elems(M), st, \
+                                              d_in, in_stride, d_out, out_stride, tw, rtw)); return 1;
         CSDRB_FFT_SIZES(X)
 #undef X
     }

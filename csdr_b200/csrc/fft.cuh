@@ -533,5 +533,7 @@ inline void fft_fill_twiddles(int n, float2* h)
 
 constexpr int fft_threads(int n) { return n / 16 < 32 ? 32 : n / 16; }
 constexpr int FFT_MAX_N = 16384;
+// every size of the single-CTA transforms, for the launchers' switches
+#define CSDRB_FFT_SIZES(X) X(2) X(4) X(8) X(16) X(32) X(64) X(128) X(256) X(512) X(1024) X(2048) X(4096) X(8192) X(16384)
 
 }  // namespace csdrb

@@ -13,7 +13,6 @@
 namespace csdrb {
 
 constexpr int fft16_first_radix(int n) { return ilog2_c(n) % 4 == 1 ? 2 : (ilog2_c(n) % 4 == 2 ? 4 : (ilog2_c(n) % 4 == 3 ? 8 : 16)); }
-constexpr int fft16_threads(int n) { return n / 16 < 32 ? 32 : n / 16; }
 
 // host: four planes (w^1, w^2, w^4, w^8) of n entries each; a radix-16 pass over sub-size NS reads index NS + k, k < NS
 inline void fft16_fill_twiddles(int n, float2* h)
@@ -159,7 +158,7 @@ __device__ __forceinline__ void fft16_rest_but_last(float2* __restrict__ s, cons
     }
 }
 
-// N-point transform in.load(i) -> out.store(i), N >= 32 (smaller sizes stay on block_fft_io); `s` is scratch; NT = fft16_threads(N)
+// N-point transform in.load(i) -> out.store(i), N >= 32 (smaller sizes stay on block_fft_io); `s` is scratch; NT = fft_threads(N)
 template <int N, int NT, bool INV, typename In, typename Out>
 __device__ __forceinline__ void block_fft16_io(float2* __restrict__ s, const float2* __restrict__ tw, int tid, In& in, Out& out)
 {
@@ -168,6 +167,16 @@ __device__ __forceinline__ void block_fft16_io(float2* __restrict__ s, const flo
     static_assert(R0 < N, "at least one radix-16 pass follows the first pass");
     fft16_pass_first<N, NT, R0, INV>(s, tid, in);
     fft16_rest<N, NT, R0, INV>(s, tw, tid, out);
+}
+
+// The one-CTA row transform of the batched c2c, r2c, fastddc forward and waterfall kernels: radix-16 passes from 32 points on (fewer passes over
+// shared memory than radix 8: 4096 points take three instead of four, 16384 four instead of five), radix 8 below.  tw is the matching table
+// (fft.cu: row_fft_twiddles); all fft_threads(N) threads must call.
+template <int N, bool INV, typename In, typename Out>
+__device__ __forceinline__ void block_row_fft_io(float2* __restrict__ s, const float2* __restrict__ tw, int tid, In& in, Out& out)
+{
+    if constexpr (N >= 32) block_fft16_io<N, fft_threads(N), INV>(s, tw, tid, in, out);
+    else block_fft_io<N, fft_threads(N), INV>(s, tw, tid, in, out);
 }
 
 // FFT_N(in) -> map -> IFFT_N -> out for N = 16^k (256, 4096): the forward transform's last radix-16 pass leaves elements j + r*N/16 in the

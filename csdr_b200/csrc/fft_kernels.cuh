@@ -8,18 +8,15 @@
 
 namespace csdrb {
 
+// tw: row_fft_twiddles(N)
 template <int N, bool INV>
 __global__ void __launch_bounds__(fft_threads(N))
 fft_c2c_batch_kernel(const float2* __restrict__ in, long in_stride, float2* __restrict__ out, long out_stride, const float2* __restrict__ tw)
 {
     CSDRB_DYN_SMEM(smem_raw);
     float2* s = reinterpret_cast<float2*>(smem_raw);
-    constexpr int NT = fft_threads(N);
-    const int tid = threadIdx.x;
-    const float2* x = in + (long)blockIdx.x * in_stride;
-    float2* y = out + (long)blockIdx.x * out_stride;
-    FftRowIn src(x); FftRowOut dst(y);
-    block_fft_io<N, NT, INV>(s, tw, tid, src, dst);                    // first pass reads the row, last pass writes it: no staging copies
+    FftRowIn src(in + (long)blockIdx.x * in_stride); FftRowOut dst(out + (long)blockIdx.x * out_stride);
+    block_row_fft_io<N, INV>(s, tw, threadIdx.x, src, dst);           // first pass reads the row, last pass writes it: no staging copies
 }
 
 template <int N>
@@ -87,14 +84,14 @@ olafir_bank_kernel(const float2* __restrict__ in, long in_stride, float2* __rest
 
 // The fused overlap-add kernel on radix-16 passes, sizes 16^k (config 5's 4096): 4R+4W shared accesses per point and block
 template <int N>
-__global__ void __launch_bounds__(fft16_threads(N), (N <= 4096 ? 2 : 1))
+__global__ void __launch_bounds__(fft_threads(N), (N <= 4096 ? 2 : 1))
 olafir_bank_fused16_kernel(const float2* __restrict__ in, long in_stride, float2* __restrict__ out, long out_stride,
                            const float2* __restrict__ taps_fft, long taps_stride, float2* __restrict__ tail_io /*[C][N]*/,
                            int input_size, int nblocks, int blocks_per_cta, const float2* __restrict__ tw16)
 {
     CSDRB_DYN_SMEM(smem_raw);
     float2* s = reinterpret_cast<float2*>(smem_raw);
-    constexpr int NT = fft16_threads(N);
+    constexpr int NT = fft_threads(N);
     const int tid = threadIdx.x, ch = blockIdx.y;
     const int overlap = N - input_size;
     float2* tail_cur = s + fft_smem_elems(N);
@@ -139,17 +136,6 @@ olafir_bank_fused16_kernel(const float2* __restrict__ in, long in_stride, float2
     }
     __syncthreads();
     if (b_last == nblocks) for (int i = tid; i < overlap; i += NT) tail_io[(long)ch * N + i] = tail_cur[i];
-}
-
-// The batched transform with radix-16 passes (fft16.cuh); tw16 = the four-plane table of fft16_fill_twiddles
-template <int N, bool INV>
-__global__ void __launch_bounds__(fft16_threads(N))
-fft_c2c_batch16_kernel(const float2* __restrict__ in, long in_stride, float2* __restrict__ out, long out_stride, const float2* __restrict__ tw16)
-{
-    CSDRB_DYN_SMEM(smem_raw);
-    float2* s = reinterpret_cast<float2*>(smem_raw);
-    FftRowIn src(in + (long)blockIdx.x * in_stride); FftRowOut dst(out + (long)blockIdx.x * out_stride);
-    block_fft16_io<N, fft16_threads(N), INV>(s, tw16, threadIdx.x, src, dst);
 }
 
 // Same operation with the transforms' ends fused: the forward FFT's first pass reads the zero-padded block straight from global
@@ -216,6 +202,7 @@ olafir_bank_fused_kernel(const float2* __restrict__ in, long in_stride, float2* 
     if (b_last == nblocks) for (int i = tid; i < overlap; i += NT) tail_io[(long)ch * N + i] = tail_cur[i];
 }
 
+// tw: row_fft_twiddles(N)
 template <int N>
 __global__ void __launch_bounds__(fft_threads(N))
 fastddc_fwd_kernel(const float2* __restrict__ in, float2* __restrict__ spectra, const float2* __restrict__ overlap_in,
@@ -223,8 +210,7 @@ fastddc_fwd_kernel(const float2* __restrict__ in, float2* __restrict__ spectra, 
 {
     CSDRB_DYN_SMEM(smem_raw);
     float2* s = reinterpret_cast<float2*>(smem_raw);
-    constexpr int NT = fft_threads(N);
-    const int tid = threadIdx.x, b = blockIdx.x;
+    const int b = blockIdx.x;
     const int overlap = N - input_size;
     // block b transforms stream samples [b*input_size - overlap, (b+1)*input_size); negative positions come from the carried overlap
     const long start = (long)b * input_size - overlap;
@@ -234,26 +220,7 @@ fastddc_fwd_kernel(const float2* __restrict__ in, float2* __restrict__ spectra, 
         __device__ __forceinline__ float4 load2(int i) const { const float2 a = load(i), b = load(i + 1); return make_float4(a.x, a.y, b.x, b.y); }
     } src{in, overlap_in, start, overlap};
     FftRowOut dst(spectra + (long)b * N);
-    block_fft_io<N, NT, false>(s, tw, tid, src, dst);
-}
-
-// The same forward step on radix-16 passes (16384 = 4*16^3: four passes instead of five)
-template <int N>
-__global__ void __launch_bounds__(fft16_threads(N))
-fastddc_fwd16_kernel(const float2* __restrict__ in, float2* __restrict__ spectra, const float2* __restrict__ overlap_in,
-                     int input_size, const float2* __restrict__ tw16)
-{
-    CSDRB_DYN_SMEM(smem_raw);
-    float2* s = reinterpret_cast<float2*>(smem_raw);
-    const int b = blockIdx.x;
-    const int overlap = N - input_size;
-    const long start = (long)b * input_size - overlap;
-    struct SlideIn {
-        const float2* in; const float2* ov; long start; int overlap;
-        __device__ __forceinline__ float2 load(int i) const { const long p = start + i; return p >= 0 ? __ldg(in + p) : ov[overlap + p]; }
-    } src{in, overlap_in, start, overlap};
-    FftRowOut dst(spectra + (long)b * N);
-    block_fft16_io<N, fft16_threads(N), false>(s, tw16, threadIdx.x, src, dst);
+    block_row_fft_io<N, false>(s, tw, threadIdx.x, src, dst);
 }
 
 __global__ void __launch_bounds__(1024)

@@ -37,22 +37,18 @@ __device__ __forceinline__ void rfft_split_pair(int k, int M, float2 zk, float2 
     if (2 * k != M) out.store(M - k, rfft_split(zmk, zk, make_float2(-w.x, w.y)));
 }
 
-constexpr int rfft_threads(int M) { return M >= 32 ? fft16_threads(M) : fft_threads(M); }
-
 // 2M-point real transform: in.load(i) / in.load2(i) give packed elements (x[2i], x[2i+1]); out.store(k, X[k]) for k = 0..M.  `s` holds
-// fft_smem_elems(M) slots; tw is the c2c table of M points (get_twiddles16 from 32 on, get_twiddles below), rtw the split table.  All
-// rfft_threads(M) threads must call.
+// fft_smem_elems(M) slots; tw is the c2c table of M points (row_fft_twiddles), rtw the split table.  All fft_threads(M) threads must call.
 template <int M, typename In, typename Out>
 __device__ __forceinline__ void block_rfft_io(float2* __restrict__ s, const float2* __restrict__ tw, const float2* __restrict__ rtw, int tid, In& in, Out& out)
 {
-    constexpr int NT = rfft_threads(M);
+    constexpr int NT = fft_threads(M);
     struct ToShared {                                                   // Z back into the transform's buffer (the last pass has read all of it)
         float2* s;
         __device__ __forceinline__ void store(int i, float2 v) const { s[fft_pad(i)] = v; }
         __device__ __forceinline__ void store2(int i, float2 a, float2 b) const { *reinterpret_cast<float4*>(s + fft_pad(i)) = make_float4(a.x, a.y, b.x, b.y); }
     } z{s};
-    if constexpr (M >= 32) block_fft16_io<M, NT, false>(s, tw, tid, in, z);
-    else block_fft_io<M, NT, false>(s, tw, tid, in, z);
+    block_row_fft_io<M, false>(s, tw, tid, in, z);
     __syncthreads();
     for (int k = tid; k <= M / 2; k += NT) rfft_split_pair(k, M, s[fft_pad(k)], s[fft_pad((M - k) & (M - 1))], rtw, out);
 }
@@ -75,7 +71,7 @@ struct RfftRowOut {
 
 // csdrb_fft_r2c_batch up to 2*FFT_MAX_N real points: one CTA per row, M + 1 bins out
 template <int M>
-__global__ void __launch_bounds__(rfft_threads(M))
+__global__ void __launch_bounds__(fft_threads(M))
 fft_r2c_batch_kernel(const float* __restrict__ in, long in_stride, float2* __restrict__ out, long out_stride, const float2* __restrict__ tw,
                      const float2* __restrict__ rtw)
 {

@@ -116,9 +116,8 @@ int launch_serial_line_bank(const float* d_in, long in_stride, int end, int* d_s
 int launch_baudot_bank(const unsigned char* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels, int n, const int* d_lengths,
                        unsigned char* d_mode_io, int* d_count, cudaStream_t st);
 
-// K7/K8/K9 fft.cu.  get_twiddles / get_twiddles16: the per-size device tables of the radix-8 and radix-16 passes (cached per process).
-int get_twiddles(int n, const float2** out, cudaStream_t st);
-int get_twiddles16(int n, const float2** out, cudaStream_t st);
+// K7/K8/K9 fft.cu.  row_fft_twiddles: the device table of block_row_fft_io<n> (fft16.cuh), cached per device and size.
+int row_fft_twiddles(int n, const float2** out, cudaStream_t st);
 int launch_fft_c2c_batch(const float2* d_in, long in_stride, float2* d_out, long out_stride, int n, int batch, int inverse, cudaStream_t st);
 int launch_olafir_bank(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int fft_size, int input_size,
                        int nblocks, const float2* d_taps_fft, long taps_stride, float2* d_tail_io, int blocks_per_cta, cudaStream_t st);

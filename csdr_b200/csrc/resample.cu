@@ -100,11 +100,9 @@ int launch_rational_resampler_bank(const float* d_in, long in_stride, float* d_o
     float* d_taps = nullptr;                                            // stream-ordered copy of the host taps: the call never blocks
     CSDRB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&d_taps), sizeof(float) * (size_t)T, st));
     CSDRB_CUDA(cudaMemcpyAsync(d_taps, h_taps, sizeof(float) * (size_t)T, cudaMemcpyHostToDevice, st));
-    if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(rational_resampler_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const dim3 grid((unsigned)((n_out + tile - 1) / tile), (unsigned)channels);
-    rational_resampler_kernel<<<grid, kRsThreads, smem, st>>>(d_in, in_stride, d_out, out_stride, n_out, I, D, d_taps, T, taps_pad,
-                                                              last_taps_delay, tile);
-    CSDRB_CUDA(cudaGetLastError());
+    CSDRB_CUDA(launch_kernel(rational_resampler_kernel, grid, kRsThreads, smem, st, d_in, in_stride, d_out, out_stride, n_out, I, D, d_taps, T, taps_pad,
+                             last_taps_delay, tile));
     CSDRB_CUDA(cudaFreeAsync(d_taps, st));
     return n_out;
 }

@@ -3,8 +3,8 @@
 //     fft_cc N E [window] | logaveragepower_cf ADD_DB N A | fft_exchange_sides_ff N [| compress_fft_adpcm_f_u8 N]
 //
 // on many independent streams (rows) at once, carrying fft_cc's framing and logaveragepower_cf's partial line between calls.
-//   spectrum_frames_kernel<N> : one CTA per (row, frame): window -> N-point forward FFT -> bin power, the FFT being the device functions of
-//                               csdrb_fft_c2c_batch (block_fft16_io from 32 points on, block_fft_io below) with the window in the first pass's
+//   spectrum_frames_kernel<N> : one CTA per (row, frame): window -> N-point forward FFT -> bin power, the FFT being the device function of
+//                               csdrb_fft_c2c_batch (block_row_fft_io) with the window in the first pass's
 //                               loads and the power in the last pass's stores, so a frame's power has the bits of the composition
 //                               apply_window_rows -> fft_c2c_batch -> accumulate_power.
 //   spectrum_lines_kernel     : one thread per (row, bin pair b, b + N/2): sums the call's frames in frame order onto the carried accumulator,
@@ -15,8 +15,6 @@
 //   spectrum_frames_real_kernel<N> : one CTA per (row, frame) of 2N real samples: the window in the loads of the packed N-point transform, the
 //                               r2c split of fft_real.cuh (block_rfft_io, the device function of csdrb_fft_r2c_batch) and the power of bins 0..N-1.
 // Frames are independent, so a single wideband row still spreads over the whole GPU; only the A-frame sums run in frame order, one thread per bin.
-#include "fft.cuh"
-#include "fft16.cuh"
 #include "fft_real.cuh"
 #include "kernels.h"
 
@@ -69,9 +67,9 @@ struct SpectrumPowerOut {                                               // accum
     __device__ __forceinline__ void store2(int i, float2 a, float2 b) const { *reinterpret_cast<float2*>(p + i) = make_float2(power(a), power(b)); }
 };
 
-// tw: the twiddle table csdrb_fft_c2c_batch uses at this size (get_twiddles16 from 32 points on, get_twiddles below)
+// tw: row_fft_twiddles(N), the table csdrb_fft_c2c_batch uses at this size
 template <int N>
-__global__ void __launch_bounds__(N >= 32 ? fft16_threads(N) : fft_threads(N))
+__global__ void __launch_bounds__(fft_threads(N))
 spectrum_frames_kernel(const float2* __restrict__ in, long in_stride, const float2* __restrict__ hist /*[rows][N]*/, const float* __restrict__ window,
                        float* __restrict__ power /*[rows][frames][N]*/, long long consumed, int every, long long first_frame, int frames,
                        const float2* __restrict__ tw)
@@ -82,8 +80,7 @@ spectrum_frames_kernel(const float2* __restrict__ in, long in_stride, const floa
     const long long s0 = spectrum_frame_start(first_frame + f, N, every);
     SpectrumFrameIn src{in + (long)r * in_stride, hist + (long)r * N, window, s0 - consumed, s0, N};
     SpectrumPowerOut dst{power + ((long)r * frames + f) * N};
-    if constexpr (N >= 32) block_fft16_io<N, fft16_threads(N), false>(s, tw, threadIdx.x, src, dst);
-    else block_fft_io<N, fft_threads(N), false>(s, tw, threadIdx.x, src, dst);
+    block_row_fft_io<N, false>(s, tw, threadIdx.x, src, dst);
 }
 
 // bins 0..N-1 of a real frame (fft_fc writes no Nyquist bin)
@@ -94,7 +91,7 @@ struct SpectrumRealPowerOut {
 
 // rtw: the split table of get_rfft_twiddles(N); tw as for spectrum_frames_kernel<N>
 template <int N>
-__global__ void __launch_bounds__(rfft_threads(N))
+__global__ void __launch_bounds__(fft_threads(N))
 spectrum_frames_real_kernel(const float* __restrict__ in, long in_stride, const float* __restrict__ hist /*[rows][2N]*/, const float* __restrict__ window,
                             float* __restrict__ power /*[rows][frames][N]*/, long long consumed, int every, long long first_frame, int frames,
                             const float2* __restrict__ tw, const float2* __restrict__ rtw)
@@ -223,33 +220,6 @@ size_t spectrum_scratch_bytes(int rows, long n, const void* h_params_v)
     return spectrum_chunk_bytes(rows, F > 1 ? F : 1, p);
 }
 
-template <int N>
-static int launch_frames_n(const float2* in, long in_stride, const float2* hist, const float* window, float* power, long long consumed, int every,
-                           long long first_frame, int frames, int rows, const float2* tw, cudaStream_t st)
-{
-    const size_t smem = sizeof(float2) * fft_smem_elems(N);
-    auto k = spectrum_frames_kernel<N>;
-    if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    constexpr int NT = N >= 32 ? fft16_threads(N) : fft_threads(N);
-    k<<<dim3(frames, rows), NT, smem, st>>>(in, in_stride, hist, window, power, consumed, every, first_frame, frames, tw);
-    CSDRB_CUDA(cudaGetLastError());
-    return 1;
-}
-
-template <int N>
-static int launch_frames_real_n(const float* in, long in_stride, const float* hist, const float* window, float* power, long long consumed, int every,
-                                long long first_frame, int frames, int rows, const float2* tw, const float2* rtw, cudaStream_t st)
-{
-    const size_t smem = sizeof(float2) * fft_smem_elems(N);
-    auto k = spectrum_frames_real_kernel<N>;
-    if (smem > 48 * 1024) CSDRB_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k<<<dim3(frames, rows), rfft_threads(N), smem, st>>>(in, in_stride, hist, window, power, consumed, every, first_frame, frames, tw, rtw);
-    CSDRB_CUDA(cudaGetLastError());
-    return 1;
-}
-
-#define CSDRB_SPECTRUM_SIZES(X) X(2) X(4) X(8) X(16) X(32) X(64) X(128) X(256) X(512) X(1024) X(2048) X(4096) X(8192) X(16384)
-
 // One body for both banks.  real = 0: d_in / d_hist_io are float2 (N-sample history); real = 1: float (2N-sample history), fft_fc's framing, no swap.
 static int spectrum_bank_run(const void* d_in, long in_stride, int rows, long n, const float* d_window, const void* h_params_v, void* d_hist_io,
                              float* d_acc_io, void* h_state_io, void* d_out, long out_stride_bytes, void* d_scratch, size_t scratch_bytes, int* launches,
@@ -284,33 +254,26 @@ static int spectrum_bank_run(const void* d_in, long in_stride, int rows, long n,
     }
     const float2 *tw = nullptr, *rtw = nullptr;
     if (f_end > f_first) {
-        if (N >= 32) { if (int rc = get_twiddles16(N, &tw, st)) return rc; }
-        else if (int rc = get_twiddles(N, &tw, st)) return rc;
+        if (int rc = row_fft_twiddles(N, &tw, st)) return rc;
         if (real) { if (int rc = get_rfft_twiddles(N, &rtw, st)) return rc; }
     }
     const float add_db = (float)((double)p->add_db - 10.0 * log10((double)A));        // logaveragepower_cf's add_db -= 10*log10(avgnumber) on a float
     const size_t line_bytes = spectrum_line_bytes(p);
     float* power = static_cast<float*>(d_scratch);
+    const float *xf = static_cast<const float*>(d_in), *hf = static_cast<const float*>(d_hist_io);
+    const float2 *xc = static_cast<const float2*>(d_in), *hc = static_cast<const float2*>(d_hist_io);
+    const size_t smem = sizeof(float2) * fft_smem_elems(N);
     for (long long g0 = f_first; g0 < f_end; g0 += F) {
         const int Fc = (int)(f_end - g0 < F ? f_end - g0 : F);
-        if (real) {
-            const float* x = static_cast<const float*>(d_in);
-            const float* h = static_cast<const float*>(d_hist_io);
-            switch (N) {
-#define X(M) case M: launch_frames_real_n<M>(x, in_stride, h, d_window, power, s->consumed, E, g0, Fc, rows, tw, rtw, st); break;
-                CSDRB_SPECTRUM_SIZES(X)
+        const dim3 grid(Fc, rows);
+        cudaError_t e = cudaSuccess;
+        switch (N) {
+#define X(M) case M: e = real ? launch_kernel(spectrum_frames_real_kernel<M>, grid, fft_threads(M), smem, st, xf, in_stride, hf, d_window, power, s->consumed, E, g0, Fc, tw, rtw) \
+                              : launch_kernel(spectrum_frames_kernel<M>, grid, fft_threads(M), smem, st, xc, in_stride, hc, d_window, power, s->consumed, E, g0, Fc, tw); break;
+            CSDRB_FFT_SIZES(X)
 #undef X
-            }
-        } else {
-            const float2* x = static_cast<const float2*>(d_in);
-            const float2* h = static_cast<const float2*>(d_hist_io);
-            switch (N) {
-#define X(M) case M: launch_frames_n<M>(x, in_stride, h, d_window, power, s->consumed, E, g0, Fc, rows, tw, st); break;
-                CSDRB_SPECTRUM_SIZES(X)
-#undef X
-            }
         }
-        CSDRB_CUDA(cudaGetLastError());
+        CSDRB_CUDA(e);
         ++*launches;
         const int Lc = (int)((g0 + Fc) / A - g0 / A);
         float* db = nullptr;
