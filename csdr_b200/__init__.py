@@ -274,6 +274,9 @@ def lib() -> C.CDLL:
     L.csdrb_serial_line_decoder_bank_f_u8.argtypes = [vp, lg, it, vp, vp, lg, vp, vp, it, C.POINTER(SerialLineParams), it, vp]
     L.csdrb_rtty_baudot2ascii_bank_u8_u8.argtypes = [vp, lg, vp, lg, it, it, vp, vp, vp, vp]
     L.serial_line_decoder_f_u8.argtypes = [C.POINTER(_SerialLine), vp, vp, it]
+    L.firdes_add_peak_c.argtypes = [vp, it, C.c_float, it, it, it]
+    L.csdrb_apply_fir_bank_cc.argtypes = [vp, lg, vp, lg, it, it, vp, it, vp]
+    L.csdrb_bfsk_demod_bank_cf.argtypes = [vp, lg, vp, lg, it, it, vp, vp, it, vp]
     L.csdrb_spectrum_bank_lines.argtypes = [C.POINTER(SpectrumParams), C.POINTER(SpectrumState), lg]; L.csdrb_spectrum_bank_lines.restype = lg
     L.csdrb_spectrum_bank_scratch_bytes.argtypes = [it, lg, C.POINTER(SpectrumParams)]; L.csdrb_spectrum_bank_scratch_bytes.restype = sz
     L.csdrb_spectrum_bank_cf.argtypes = [vp, lg, it, lg, vp, C.POINTER(SpectrumParams), vp, vp, C.POINTER(SpectrumState), vp, lg, vp, sz, vp]
@@ -1167,6 +1170,46 @@ def rtty_baudot2ascii_bank_u8_u8(codes, lengths=None, fig_mode=None):
                                                     lengths.data_ptr() if lengths is not None else None, fig_mode.data_ptr(), count.data_ptr(),
                                                     _stream()), "rtty_baudot2ascii_bank_u8_u8")
     return out, count, fig_mode
+
+
+
+def firdes_peak_c(rate: float, length: int, window: str = "HAMMING") -> np.ndarray:
+    """firdes_add_peak_c(taps, length, rate, window, 0, 1) (libcsdr.c:2219-2258): a windowed complex tone at -rate cycles per sample, scaled so
+    that its magnitudes sum to 1 -- as the reference's build computes it"""
+    t = np.zeros(max(length, 1), np.complex64)
+    lib().firdes_add_peak_c(t.ctypes.data, length, rate, WINDOWS[window], 0, 1)
+    return t[:length]
+
+
+def _tone_rows(x):
+    import torch
+    assert x.dtype == torch.complex64 and x.is_cuda and x.dim() == 2 and x.stride(1) == 1
+    return x.shape
+
+
+def apply_fir_bank_cc(x, taps):
+    """apply_fir_cc per row (libcsdr.c:2261-2273), bit for bit with the reference build: x [C, N] complex64 CUDA, taps [L] complex64 (numpy or
+    CUDA, 2 <= L <= 4096, shared by all rows) -> [C, N - L + 1] complex64, the valid convolution"""
+    import torch
+    ch, n = _tone_rows(x)
+    t = torch.as_tensor(np.asarray(taps, np.complex64) if not torch.is_tensor(taps) else taps, device=x.device).contiguous()
+    out = torch.empty((ch, max(n - t.numel() + 1, 1)), dtype=torch.complex64, device=x.device)
+    m = _check(lib().csdrb_apply_fir_bank_cc(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, t.data_ptr(), t.numel(), _stream()),
+               "apply_fir_bank_cc")
+    return out[:, :m]
+
+
+def bfsk_demod_bank_cf(x, spacing: float, filter_length: int):
+    """bfsk_demod_cf per row (libcsdr.c:2335-2351) with the CLI's taps (csdr.c:3283-3286): Hamming peaks at +spacing/2 (mark) and
+    -spacing/2 (space), spacing in cycles per sample.  x [C, N] complex64 CUDA -> [C, N - L + 1] float32, |mark|^2 - |space|^2"""
+    import torch
+    ch, n = _tone_rows(x)
+    mark = torch.from_numpy(firdes_peak_c(spacing / 2, filter_length)).to(x.device)
+    space = torch.from_numpy(firdes_peak_c(-spacing / 2, filter_length)).to(x.device)
+    out = torch.empty((ch, max(n - filter_length + 1, 1)), dtype=torch.float32, device=x.device)
+    m = _check(lib().csdrb_bfsk_demod_bank_cf(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, mark.data_ptr(), space.data_ptr(),
+                                              filter_length, _stream()), "bfsk_demod_bank_cf")
+    return out[:, :m]
 
 
 def fft_c2c(x, inverse: bool = False):

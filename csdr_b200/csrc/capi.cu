@@ -474,6 +474,35 @@ int csdrb_rtty_baudot2ascii_bank_u8_u8(const unsigned char* d_in, long in_stride
     return rc < 0 ? rc : counted(0, rc);
 }
 
+// tone filters (tone.cu; libcsdr.c:2261-2273, 2335-2351)
+static inline bool misaligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
+
+int csdrb_apply_fir_bank_cc(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int n, const complexf* d_taps,
+                            int taps_length, void* stream)
+{
+    if (too_many_channels(channels, "apply_fir_cc bank")) return -1;
+    if (!d_in || !d_out || !d_taps || misaligned(d_in, 8) || misaligned(d_out, 8) || misaligned(d_taps, 8)) {
+        set_error("apply_fir_cc bank: null or misaligned pointer (complexf needs 8-byte alignment)");
+        return -1;
+    }
+    int rc = launch_apply_fir_bank_cc(reinterpret_cast<const float2*>(d_in), in_stride, reinterpret_cast<float2*>(d_out), out_stride, channels, n,
+                                      reinterpret_cast<const float2*>(d_taps), taps_length, S(stream));
+    return rc < 0 ? rc : counted(rc, channels > 0 ? 1 : 0);
+}
+
+int csdrb_bfsk_demod_bank_cf(const complexf* d_in, long in_stride, float* d_out, long out_stride, int channels, int n, const complexf* d_mark,
+                             const complexf* d_space, int taps_length, void* stream)
+{
+    if (too_many_channels(channels, "bfsk_demod_cf bank")) return -1;
+    if (!d_in || !d_out || !d_mark || !d_space || misaligned(d_in, 8) || misaligned(d_out, 4) || misaligned(d_mark, 8) || misaligned(d_space, 8)) {
+        set_error("bfsk_demod_cf bank: null or misaligned pointer (complexf needs 8-byte, float 4-byte alignment)");
+        return -1;
+    }
+    int rc = launch_bfsk_demod_bank_cf(reinterpret_cast<const float2*>(d_in), in_stride, d_out, out_stride, channels, n,
+                                       reinterpret_cast<const float2*>(d_mark), reinterpret_cast<const float2*>(d_space), taps_length, S(stream));
+    return rc < 0 ? rc : counted(rc, channels > 0 ? 1 : 0);
+}
+
 int csdrb_fft_c2c_batch(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int size, int batch, int inverse, void* stream)
 {
     if (!d_in || !d_out) { set_error("fft: null pointer"); return -1; }

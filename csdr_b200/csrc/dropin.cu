@@ -674,6 +674,34 @@ void timing_recovery_cc(complexf* input, complexf* output, int input_size, float
     state->last_correction_offset = call.state.last_correction_offset;
 }
 
+// ---- tone filters (libcsdr.c:2261-2273, 2335-2351) ---------------------------------------------------------
+int apply_fir_cc(complexf* input, complexf* output, int input_size, complexf* taps, int taps_length)
+{
+    if (input_size < taps_length) return 0;
+    Staging st("apply_fir_cc");
+    const complexf* d_in = st.up(input, input_size);
+    const complexf* d_taps = st.up(taps, taps_length);
+    complexf* d_out = st.alloc<complexf>(input_size - taps_length + 1);
+    const int n_out = st.check(csdrb_apply_fir_bank_cc(d_in, input_size, d_out, input_size, 1, input_size, d_taps, taps_length, st.stream()));
+    st.get(output, d_out, n_out);
+    st.sync();
+    return n_out;
+}
+
+int bfsk_demod_cf(complexf* input, float* output, int input_size, complexf* mark_filter, complexf* space_filter, int taps_length)
+{
+    if (input_size < taps_length) return input_size - taps_length + 1;     // the reference returns the count it would have written
+    Staging st("bfsk_demod_cf");
+    const complexf* d_in = st.up(input, input_size);
+    const complexf* d_mark = st.up(mark_filter, taps_length);
+    const complexf* d_space = st.up(space_filter, taps_length);
+    float* d_out = st.alloc<float>(input_size - taps_length + 1);
+    const int n_out = st.check(csdrb_bfsk_demod_bank_cf(d_in, input_size, d_out, input_size, 1, input_size, d_mark, d_space, taps_length, st.stream()));
+    st.get(output, d_out, n_out);
+    st.sync();
+    return n_out;
+}
+
 // ---- RTTY receive chain -----------------------------------------------------------------------------------
 void serial_line_decoder_f_u8(serial_line_t* s, float* input, unsigned char* output, int input_size)
 {

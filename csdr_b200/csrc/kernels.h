@@ -116,6 +116,13 @@ int launch_serial_line_bank(const float* d_in, long in_stride, int end, int* d_s
 int launch_baudot_bank(const unsigned char* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels, int n, const int* d_lengths,
                        unsigned char* d_mode_io, int* d_count, cudaStream_t st);
 
+// tone filters, tone.cu: the valid convolution of each row with shared complex taps (2 <= L <= kToneMaxTaps, else -2); n - L + 1 per row
+constexpr int kToneMaxTaps = 4096;
+int launch_apply_fir_bank_cc(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n, const float2* d_taps, int L,
+                             cudaStream_t st);
+int launch_bfsk_demod_bank_cf(const float2* d_in, long in_stride, float* d_out, long out_stride, int channels, int n, const float2* d_mark,
+                              const float2* d_space, int L, cudaStream_t st);
+
 // K7/K8/K9 fft.cu.  row_fft_twiddles: the device table of block_row_fft_io<n> (fft16.cuh), cached per device and size.
 int row_fft_twiddles(int n, const float2** out, cudaStream_t st);
 int launch_fft_c2c_batch(const float2* d_in, long in_stride, float2* d_out, long out_stride, int n, int batch, int inverse, cudaStream_t st);

@@ -13,7 +13,8 @@
  * first -- is process plumbing and is not reproduced; tests/test_gpu_zzz_bankd.py compares against the oracle run over the whole stream).
  *
  * usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32|--s16|--real-s16|--real-f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]
- *                   [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty|wfm] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B] [--resample I:D[:BW]]
+ *                   [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty|wfm] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B] [--bfsk SPACING:LENGTH]
+ *                   [--resample I:D[:BW]]
  *                   [--wfm-rate R] [--tau T]
  *                   [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]
  *                   [--waterfall SINK [--fft-size N] [--fft-every E] [--fft-averages A] [--fft-add-db X] [--fft-window W] [--fft-compression adpcm|none]
@@ -34,6 +35,9 @@
  *   at 2.4 Msps: --decimation 1200 --bw 0.001 gives 2 kHz baseband (4001 taps, M = 4 per output period, D*MP = 4800 <= 8000: the fused bank
  *   serves it), and --sps 44 is 45.45 Bd:
  *     rtl_sdr -s 2400000 -f 14080000 - | csdr-bankd --decimation 1200 --bw 0.001 --tail rtty --sps 44 -0.1:ch1.txt 0.05:ch2.txt 0.2:ch3.txt
+ *   --bfsk SPACING:LENGTH demodulates with tone filters instead of the discriminator: the bank gives the complex baseband and each channel runs
+ *   bfsk_demod_cf SPACING LENGTH (a Hamming peak filter of LENGTH taps on mark at +SPACING/2 and one on space at -SPACING/2 cycles per baseband
+ *   sample, |mark|^2 - |space|^2 out) before the decoder; 170 Hz shift at 2 kHz baseband is --bfsk 0.085:44 (a filter about one bit long).
  *   wfm: broadcast FM, the README.md:66 graph's fractional_decimator_ff R | deemphasis_wfm_ff 48000 T | convert_f_s16 behind the discriminator (the bank
  *   runs with fmdemod), s16 audio per channel.  --wfm-rate R (default 5, above 1 and at most 16) brings wideband / D to 48 kHz, the de-emphasis rate;
  *   --tau T (default 50e-6; 75e-6 in the Americas).  Both run in the CLI's calls of 1024 samples (csdrb_wfm_audio_bank_f_s16), so every channel
@@ -549,6 +553,11 @@ typedef struct {
     float *d_rows, *d_carry;
     unsigned char *d_codes, *d_chars, *d_mode, *h_chars;
     int *d_start, *d_count, *d_stuck, *d_char_count, *h_start;                 /* h_start: start[C], stuck[C], char_count[C] */
+    /* --bfsk: the bank gives complexf baseband rows; bfsk_demod_cf with L taps turns them into the rows above.  bb: [C][bs] complexf, the
+     * last L - 1 samples of the previous push (bb_have of them) and then the new ones; mark/space: the taps on the device */
+    int L, bb_have;
+    long bs;
+    complexf *d_bb, *d_bb_carry, *d_mark, *d_space;
 } rtty_tail_t;
 
 static void rtty_tail_init(rtty_tail_t *t, int C, const csdrb_serial_line_params_t *p, int bufsize, int in_cap)
@@ -569,6 +578,25 @@ static void rtty_tail_init(rtty_tail_t *t, int C, const csdrb_serial_line_params
     t->h_chars = csdrb_host_alloc((size_t)C * (size_t)t->cap);
     if (!t->d_rows || !t->d_carry || !t->d_codes || !t->d_chars || !t->d_mode || !t->d_start || !t->d_count || !t->h_start || !t->h_chars)
         die("out of memory");
+}
+
+/* --bfsk SPACING:LENGTH: the taps of `csdr bfsk_demod_cf SPACING LENGTH` (csdr.c:3283-3286), and rows for LENGTH - 1 carried samples plus a push */
+static void rtty_bfsk_init(rtty_tail_t *t, float spacing, int L, int in_cap, void *stream)
+{
+    const int C = t->C;
+    t->L = L;
+    t->bs = ((long)L - 1 + in_cap + 1) & ~1L;
+    complexf *h = malloc(sizeof(complexf) * 2 * (size_t)L);
+    t->d_bb = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->bs);
+    t->d_bb_carry = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)L);
+    t->d_mark = csdrb_device_alloc(sizeof(complexf) * 2 * (size_t)L);
+    if (!h || !t->d_bb || !t->d_bb_carry || !t->d_mark) die("out of memory");
+    t->d_space = t->d_mark + L;
+    firdes_add_peak_c(h, L, spacing / 2, WINDOW_DEFAULT, 0, 1);
+    firdes_add_peak_c(h + L, L, -spacing / 2, WINDOW_DEFAULT, 0, 1);
+    OK(csdrb_copy_h2d(t->d_mark, h, sizeof(complexf) * 2 * (size_t)L, stream));
+    OK(csdrb_stream_synchronize(stream));
+    free(h);
 }
 
 /* n new discriminator samples per channel sit at d_rows + end: decode what fills whole calls, the text to the sinks, keep the rest */
@@ -596,6 +624,19 @@ static void rtty_tail_push(rtty_tail_t *t, channel_t *chan, int n, void *stream)
         OK(csdrb_copy_h2d(t->d_start, t->h_start, sizeof(int) * (size_t)C, stream));
         OK(csdrb_stream_synchronize(stream));
     }
+}
+
+/* --bfsk: n new baseband samples per channel sit at d_bb + bb_have; the bfsk outputs of every complete window go to the decoder's rows */
+static void rtty_bfsk_push(rtty_tail_t *t, channel_t *chan, int n, void *stream)
+{
+    const int have = t->bb_have + n;
+    if (have < t->L) { t->bb_have = have; return; }
+    if (t->end + (long)(have - t->L + 1) > t->rs) die("rtty tail: signal buffer overflow");
+    const int m = csdrb_bfsk_demod_bank_cf(t->d_bb, t->bs, t->d_rows + t->end, t->rs, t->C, have, t->d_mark, t->d_space, t->L, stream);
+    if (m < 0) die("csdrb_bfsk_demod_bank_cf failed");
+    t->bb_have = t->L - 1;
+    rows_to_front(t->d_bb, t->bs, have - t->bb_have, t->bb_have, sizeof(complexf), t->d_bb_carry, t->C, stream);
+    rtty_tail_push(t, chan, m, stream);
 }
 
 /* ---- the WFM tail: fractional_decimator_ff R | deemphasis_wfm_ff 48000 TAU | convert_f_s16 behind the discriminator (README.md:66) --------------
@@ -777,6 +818,8 @@ typedef struct {
     int rs_I, rs_D, sps, rtty_B;                                     /* --resample I:D (rs_I 0: no resampler), --sps N of bpsk31, --rtty-bufsize */
     float rs_bw, wfm_rate, tau;                                      /* --resample's BW, --wfm-rate, --tau */
     csdrb_serial_line_params_t rtty;                                 /* --sps F, --databits, --stopbits of --tail rtty */
+    float bfsk_spacing;                                              /* --bfsk SPACING:LENGTH of --tail rtty (bfsk_L 0: the discriminator) */
+    int bfsk_L;
     waterfall_opts_t wf;
 } opts_t;
 
@@ -791,6 +834,9 @@ typedef struct {
     union { nfm_tail_t nfm; raw_tail_t raw; bb_tail_t bb; bpsk_tail_t bpsk; rtty_tail_t rtty; wfm_tail_t wfm; } u;
 } tail_t;
 
+/* whether the bank demodulates: the tail's choice, except that --tail rtty --bfsk takes the complex baseband */
+static int bank_demod(const opts_t *o) { return kTails[o->tail].demod && !o->bfsk_L; }
+
 /* --devices --tail none without --resample: the rows collected on the host are the output, so that tail needs no device, stream or buffer */
 static int tail_host_fed(int kind, int resample) { return kind == TAIL_NONE && !resample; }
 
@@ -800,7 +846,7 @@ static void tail_init(tail_t *t, const opts_t *o, int C, int in_cap, void *strea
 {
     memset(t, 0, sizeof *t);
     t->kind = o->tail; t->C = C; t->resample = o->rs_I > 0;
-    t->esz = kTails[o->tail].demod ? sizeof(float) : sizeof(complexf);
+    t->esz = bank_demod(o) ? sizeof(float) : sizeof(complexf);
     if (!stream) return;
     if (t->resample) { rs_init(&t->rs, C, o->rs_I, o->rs_D, o->rs_bw, in_cap); in_cap = rs_out_cap(&t->rs); }
     switch (t->kind) {
@@ -810,7 +856,10 @@ static void tail_init(tail_t *t, const opts_t *o, int C, int in_cap, void *strea
     case TAIL_USB: bb_tail_init(&t->u.bb, C, in_cap, o->limit, o->agc_ref, (const float[2]){0.0f, 0.1f}, stream); break;
     case TAIL_LSB: bb_tail_init(&t->u.bb, C, in_cap, o->limit, o->agc_ref, (const float[2]){-0.1f, 0.0f}, stream); break;
     case TAIL_BPSK31: bpsk_tail_init(&t->u.bpsk, C, o->sps, in_cap, o->agc_ref, stream); break;
-    case TAIL_RTTY: rtty_tail_init(&t->u.rtty, C, &o->rtty, o->rtty_B, in_cap); break;
+    case TAIL_RTTY:
+        rtty_tail_init(&t->u.rtty, C, &o->rtty, o->rtty_B, in_cap);
+        if (o->bfsk_L) rtty_bfsk_init(&t->u.rtty, o->bfsk_spacing, o->bfsk_L, in_cap, stream);
+        break;
     case TAIL_WFM: wfm_tail_init(&t->u.wfm, C, o->wfm_rate, o->tau, in_cap); break;
     }
 }
@@ -823,7 +872,9 @@ static void *tail_in(tail_t *t, long *pitch)
     case TAIL_NONE: case TAIL_IQ: *pitch = t->u.raw.pitch; return t->u.raw.d_rows;
     case TAIL_AM: case TAIL_USB: case TAIL_LSB: *pitch = t->u.bb.bs; return t->u.bb.d_bb + t->u.bb.have;
     case TAIL_BPSK31: *pitch = t->u.bpsk.bs; return t->u.bpsk.d_in;
-    case TAIL_RTTY: *pitch = t->u.rtty.rs; return t->u.rtty.d_rows + t->u.rtty.end;
+    case TAIL_RTTY:
+        if (t->u.rtty.L) { *pitch = t->u.rtty.bs; return t->u.rtty.d_bb + t->u.rtty.bb_have; }
+        *pitch = t->u.rtty.rs; return t->u.rtty.d_rows + t->u.rtty.end;
     case TAIL_WFM: default: *pitch = t->u.wfm.rs; return t->u.wfm.d_rows + t->u.wfm.have;
     }
 }
@@ -842,7 +893,10 @@ static void tail_push(tail_t *t, channel_t *chan, int n, void *stream)
         break;
     case TAIL_AM: case TAIL_USB: case TAIL_LSB: bb_tail_push(&t->u.bb, chan, n, stream); break;
     case TAIL_BPSK31: bpsk_tail_push(&t->u.bpsk, chan, n, stream); break;
-    case TAIL_RTTY: rtty_tail_push(&t->u.rtty, chan, n, stream); break;
+    case TAIL_RTTY:
+        if (t->u.rtty.L) rtty_bfsk_push(&t->u.rtty, chan, n, stream);
+        else rtty_tail_push(&t->u.rtty, chan, n, stream);
+        break;
     case TAIL_WFM: wfm_tail_push(&t->u.wfm, chan, n, stream); break;
     }
 }
@@ -865,7 +919,7 @@ static int run_multi(const opts_t *o, channel_t *chan, int C, const float *rates
     const int in_fd = open_input(o->in_spec);
     fprintf(stderr, "csdr-bankd: %d channels over %d devices, decimation %d, %d taps, %s input, blocks of %d samples, tail %s\n", C, o->ndev, D, T,
             kFormatNames[fmt], block, kTails[o->tail].name);
-    csdrb_multi_bank_t *mb = csdrb_multi_bank_create(o->ndev, o->devs, C, rates, D, taps, T, kTails[o->tail].demod, 1024, block);
+    csdrb_multi_bank_t *mb = csdrb_multi_bank_create(o->ndev, o->devs, C, rates, D, taps, T, bank_demod(o), 1024, block);
     if (!mb) die("cannot create the multi-GPU bank");
     const int n_out = (block - T) / D + 1, consumed = n_out * D, keep = block - consumed;
     /* the tail (and the resampler) is audio-rate work (C x the channel rate): the rows every device returned go to the FIRST device once more and
@@ -941,6 +995,7 @@ static int usage(void)
             "usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32|--s16|--real-s16|--real-f32] [--decimation D] [--bw TRANSITION_BW] [--window W]\n"
             "                  [--block SAMPLES]\n"
             "                  [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty|wfm] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B]\n"
+            "                  [--bfsk SPACING:LENGTH]\n"
             "                  [--wfm-rate R] [--tau T] [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]\n"
             "                  RATE:SINK [RATE:SINK ...]\n"
             "  --u8 | --f32 | --s16 the complex input: rtl_sdr's u8 IQ (default), complex float, or complex s16 (Airspy INT16_IQ, SDRplay, ...)\n"
@@ -968,6 +1023,10 @@ static int usage(void)
             "                       by up to B samples; B must exceed F*(1 + N + S) + 2.  An RTTY skimmer at 2.4 Msps:\n"
             "                       csdr-bankd --decimation 1200 --bw 0.001 --tail rtty --sps 44 -0.1:ch1.txt 0.05:ch2.txt 0.2:ch3.txt\n"
             "                       (2 kHz baseband, 4001 taps = 4 per output period, which the fused bank serves; 45.45 Bd; about 8 s of lag)\n"
+            "  --bfsk SPACING:LENGTH  with --tail rtty: tone filters instead of the discriminator, bfsk_demod_cf SPACING LENGTH per channel on the\n"
+            "                       complex baseband (peaks at +-SPACING/2 cycles per baseband sample, Hamming, LENGTH taps, 2..4096).  They hold\n"
+            "                       up in noise below the discriminator's threshold.  170 Hz shift at 2 kHz baseband (2.4 Msps, --decimation 1200):\n"
+            "                       csdr-bankd --decimation 1200 --bw 0.001 --tail rtty --sps 44 --bfsk 0.085:44 -0.1:ch1.txt 0.05:ch2.txt\n"
             "  --resample I:D[:BW]  rational_resampler_ff I D BW (BW default 0.05) right behind the discriminator, for --tail nfm and none: brings\n"
             "                       wideband/decimation to the 48 kHz the NFM de-emphasis is designed for (e.g. 2.048 Msps, --decimation 32,\n"
             "                       --resample 3:4).  With T = taps of BW, the daemon needs (T/I + 1)*I >= 2*D + I - 1 (T >= 2*D + I - 2 suffices),\n"
@@ -1019,6 +1078,12 @@ int main(int argc, char **argv)
         else if (!strcmp(arg, "--databits") && v) { o.rtty.databits = atoi(v); rtty_opts = 1; a++; }
         else if (!strcmp(arg, "--stopbits") && v) { o.rtty.stopbits = (float)atof(v); rtty_opts = 1; a++; }
         else if (!strcmp(arg, "--rtty-bufsize") && v) { o.rtty_B = atoi(v); rtty_opts = 1; a++; }
+        else if (!strcmp(arg, "--bfsk") && v) {
+            if (sscanf(v, "%f:%d", &o.bfsk_spacing, &o.bfsk_L) != 2) die("--bfsk takes SPACING:LENGTH, e.g. 0.085:44");
+            if (!(o.bfsk_spacing > 0.f && o.bfsk_spacing < 1.f)) die("--bfsk SPACING is the mark-space shift in cycles per baseband sample, between 0 and 1");
+            if (o.bfsk_L < 2 || o.bfsk_L > 4096) die("--bfsk LENGTH must be between 2 and 4096 taps");
+            a++;
+        }
         else if (!strcmp(arg, "--wfm-rate") && v) { o.wfm_rate = (float)atof(v); wfm_opts = 1; a++; }
         else if (!strcmp(arg, "--tau") && v) { o.tau = (float)atof(v); wfm_opts = 1; a++; }
         else if (!strcmp(arg, "--waterfall") && v) { o.wf_sink = v; a++; }
@@ -1065,6 +1130,7 @@ int main(int argc, char **argv)
             die("--rtty-bufsize must exceed sps*(1 + databits + stopbits) + 2: a call could not hold one character and would get stuck");
     } else if (o.sps) die("--sps belongs to --tail bpsk31 and --tail rtty");
     if (o.tail != TAIL_RTTY && rtty_opts) die("--databits, --stopbits and --rtty-bufsize belong to --tail rtty");
+    if (o.tail != TAIL_RTTY && o.bfsk_L) die("--bfsk belongs to --tail rtty");
     if (o.tail == TAIL_WFM) {
         /* above 16 a decimator call could consume more than its 1024 samples (the reference then memmoves a negative length): WFM needs about 5 */
         if (!(o.wfm_rate > 1.0f && o.wfm_rate <= 16.0f)) die("--wfm-rate must be above 1 and at most 16 (wideband rate / decimation / 48 kHz)");
@@ -1114,7 +1180,7 @@ int main(int argc, char **argv)
     if (o.ndev > C) die("more devices than channels");
     if (o.ndev > 0) return run_multi(&o, chan, C, rates, taps, T, wfp);
     void *stream = device_stream(o.device);
-    csdrb_ddc_bank_t *bank = csdrb_ddc_bank_create(C, rates, D, taps, T, kTails[o.tail].demod, 1024);   /* 1024 = the CLI's shift_addition_cc call size (csdr.c:911) */
+    csdrb_ddc_bank_t *bank = csdrb_ddc_bank_create(C, rates, D, taps, T, bank_demod(&o), 1024);   /* 1024 = the CLI's shift_addition_cc call size (csdr.c:911) */
     if (!bank) die("cannot create the bank");
 
     /* ---- buffers ----------------------------------------------------------------------------------------------------------------

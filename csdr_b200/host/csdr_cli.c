@@ -1037,6 +1037,83 @@ static int cmd_rtty_baudot2ascii_u8_u8(int argc, char **argv)
     }
 }
 
+/* ---- tone filters (csdr.c:2932-3017, 3271-3301) ---------------------------------------------------------------------------------
+ * peaks_fir_cc and bfsk_demod_cf frame like the reference: one full read, then after every call the consumed output_size samples leave the
+ * front of the buffer and as many are read behind the rest.  The end-of-file test comes before each call, so the output ends with the last
+ * call whose refill was complete: a prefix of the valid convolution of the stream. */
+static int tone_stream(int taps_length, const complexf *taps, const complexf *mark, const complexf *space)
+{
+    complexf *in = must_alloc(sizeof(complexf) * (size_t)block);
+    void *out = must_alloc(sizeof(complexf) * (size_t)block);
+    fread(in, sizeof(complexf), (size_t)block, stdin);
+    for (;;) {
+        if (feof(stdin)) return 0;
+        int n;
+        if (taps) { n = apply_fir_cc(in, out, block, (complexf *)taps, taps_length); fwrite(out, sizeof(complexf), (size_t)n, stdout); }
+        else { n = bfsk_demod_cf(in, out, block, (complexf *)mark, (complexf *)space, taps_length); fwrite(out, sizeof(float), (size_t)n, stdout); }
+        end_of_block();
+        memmove(in, in + n, sizeof(complexf) * (size_t)(block - n));
+        fread(in + (block - n), sizeof(complexf), (size_t)n, stdin);
+    }
+}
+
+static int cmd_firdes_peak_c(int argc, char **argv)                         /* csdr.c:2932-2972 */
+{
+    if (argc <= 3) return complain("need required parameters (rate, length)");
+    float rate;
+    sscanf(argv[2], "%g", &rate);
+    int length;
+    sscanf(argv[3], "%d", &length);
+    if (length % 2 == 0) return complain("number of symmetric FIR filter taps should be odd");
+    window_t window = WINDOW_DEFAULT;
+    if (argc >= 5) window = firdes_get_window_from_string(argv[4]);
+    else { who(); fprintf(stderr, "window = %s\n", firdes_get_string_from_window(window)); }
+    if (argc >= 6 && !strcmp(argv[5], "--octave")) return complain("--octave is not offered here (it plots the filter with GNU Octave)");
+    if (length <= 0) return 0;                                              /* the reference's loops print nothing */
+    complexf *taps = must_alloc(sizeof(complexf) * (size_t)length);
+    firdes_add_peak_c(taps, length, rate, window, 0, 1);
+    for (int i = 0; i < length; i++) printf("(%g)+(%g)*i ", taps[i].i, taps[i].q);
+    return 0;
+}
+
+static int cmd_peaks_fir_cc(int argc, char **argv)                          /* csdr.c:2975-3017 */
+{
+    if (argc <= 2) return complain("need required parameter (taps_length)");
+    int taps_length;
+    sscanf(argv[2], "%d", &taps_length);
+    const int num_peaks = argc - 3;
+    float *peak_rate = must_alloc(sizeof(float) * (size_t)(num_peaks > 0 ? num_peaks : 1));
+    for (int i = 0; i < num_peaks; i++) sscanf(argv[3 + i], "%f", peak_rate + i);
+    if (num_peaks <= 0) return complain("need required parameter (peak_rate) once or multiple times");
+    fflush(stderr);
+    if (!open_block()) return -2;
+    announce_block(block);
+    if (block - taps_length <= 0) return complain("taps_length is below buffer size, decrease taps_length");
+    if (taps_length < 2 || taps_length > 4096) return complain("taps_length must be between 2 and 4096");
+    complexf *taps = must_alloc(sizeof(complexf) * (size_t)taps_length);     /* zero-filled: the peaks add up in it */
+    for (int i = 0; i < num_peaks; i++) firdes_add_peak_c(taps, taps_length, peak_rate[i], WINDOW_DEFAULT, 1, i == num_peaks - 1);
+    return tone_stream(taps_length, taps, NULL, NULL);
+}
+
+static int cmd_bfsk_demod_cf(int argc, char **argv)                         /* csdr.c:3271-3301 */
+{
+    float frequency_shift = 0;
+    if (argc <= 2) return complain("required parameter <frequency_shift> is missing.");
+    sscanf(argv[2], "%f", &frequency_shift);
+    int filter_length = 0;
+    if (argc <= 3) return complain("required parameter <filter_length> is missing.");
+    sscanf(argv[3], "%d", &filter_length);
+    if (!open_block()) return -2;
+    if (!announce_block(1)) return -2;                                      /* the reference announces initialize_buffers()'s 1 */
+    /* the reference designs NaN taps at length 1 (middle = 0) and computes a negative output count from a filter longer than the buffer */
+    if (filter_length < 2 || filter_length > 4096 || filter_length >= block)
+        return complain("filter_length must be between 2 and 4096 and below the buffer size");
+    complexf *mark = must_alloc(sizeof(complexf) * (size_t)filter_length), *space = must_alloc(sizeof(complexf) * (size_t)filter_length);
+    firdes_add_peak_c(mark, filter_length, frequency_shift / 2, WINDOW_DEFAULT, 0, 1);
+    firdes_add_peak_c(space, filter_length, -frequency_shift / 2, WINDOW_DEFAULT, 0, 1);
+    return tone_stream(filter_length, NULL, mark, space);
+}
+
 /* ---- dispatch ------------------------------------------------------------------------------------ */
 static const struct { const char *name; int (*run)(int, char **); const char *syntax; } kCommands[] = {
     {"convert_u8_f", cmd_convert_u8_f, "convert_u8_f"},
@@ -1079,6 +1156,9 @@ static const struct { const char *name; int (*run)(int, char **); const char *sy
     {"psk31_varicode_decoder_u8_u8", cmd_psk31_varicode_decoder_u8_u8, "psk31_varicode_decoder_u8_u8"},
     {"serial_line_decoder_f_u8", cmd_serial_line_decoder_f_u8, "serial_line_decoder_f_u8 <samples_per_bits> [databits [stopbits]]"},
     {"rtty_baudot2ascii_u8_u8", cmd_rtty_baudot2ascii_u8_u8, "rtty_baudot2ascii_u8_u8"},
+    {"firdes_peak_c", cmd_firdes_peak_c, "firdes_peak_c <rate> <length> [window]"},
+    {"peaks_fir_cc", cmd_peaks_fir_cc, "peaks_fir_cc <taps_length> <peak_rate> [peak_rate ...]"},
+    {"bfsk_demod_cf", cmd_bfsk_demod_cf, "bfsk_demod_cf <spacing> <filter_length>"},
     {"fastddc_inv_cc", cmd_fastddc_inv_cc, "fastddc_inv_cc <shift_rate> <decimation> [transition_bw [window]] | --fifo <fifo_path> ... | --fd <fd> ..."},
 };
 

@@ -107,6 +107,32 @@ void firdes_bandpass_c(complexf *output, int length, float lowcut, float highcut
     free(prototype);
 }
 
+/* ---- peak filter (libcsdr.c:2219-2258) as the reference's -O3 -ffast-math build computes it (DESIGN.md section 7) ----------------------
+ * phase steps by (float)((double)-rate * 2pi) in float and wraps against 2pi in double; e_powj becomes sincosf of the float phase; the window
+ * takes (float)(middle - i) times the float reciprocal of middle; the magnitudes sqrt((double)(i*i + q*q)) add in double and round to float
+ * after every tap; the taps are multiplied by the float reciprocal of that sum. */
+void firdes_add_peak_c(complexf *output, int length, float rate, window_t window, int add, int normalize)
+{
+    const int middle = length / 2;
+    const float step = (float)((double)-rate * (2 * M_PI)), inv_middle = 1.0f / (float)middle;
+    float phase = 0;
+    for (int i = 0; i < length; i++) {
+        float c, s;
+        sincosf(phase, &s, &c);
+        const float w = window_value(window, fabsf((float)(middle - i) * inv_middle));
+        if (add) { output[i].i += c * w; output[i].q += s * w; }
+        else { output[i].i = c * w; output[i].q = s * w; }
+        phase += step;
+        while ((double)phase > 2 * M_PI) phase = (float)((double)phase - 2 * M_PI);
+        while (phase < 0) phase = (float)((double)phase + 2 * M_PI);
+    }
+    if (!normalize) return;
+    float sum = 0;
+    for (int i = 0; i < length; i++) sum = (float)((double)sum + sqrt((double)(output[i].i * output[i].i + output[i].q * output[i].q)));
+    const float scale = 1.0f / sum;
+    for (int i = 0; i < length; i++) { output[i].i *= scale; output[i].q *= scale; }
+}
+
 /* ---- integer helpers (libcsdr.c:1220-1243) ----------------------------------------------------- */
 int log2n(int x)
 {

@@ -129,6 +129,15 @@ typedef struct serial_line_s {
 } serial_line_t;
 void serial_line_decoder_f_u8(serial_line_t *s, float *input, unsigned char *output, int input_size);
 
+/* tone filters (libcsdr.c:2219-2273, 2335-2351).  firdes_add_peak_c computes its taps as the reference's -O3 -ffast-math build does (DESIGN.md
+ * section 7): sincosf of the float phase, the window at |(float)(middle - i) * (1/(float)middle)|, the sum of magnitudes in double rounded to
+ * float after every tap, the taps scaled by 1/sum.  apply_fir_cc is bit-exact with that build; bfsk_demod_cf sums in source order and lies
+ * within the bound of tests/test_tone_emulated.py of it.  Both serve 2 <= taps_length <= 4096 and abort with a message outside it; an
+ * input_size below taps_length gives 0 outputs, like the reference. */
+void firdes_add_peak_c(complexf *output, int length, float rate, window_t window, int add, int normalize);
+int  apply_fir_cc(complexf *input, complexf *output, int input_size, complexf *taps, int taps_length);
+int  bfsk_demod_cf(complexf *input, float *output, int input_size, complexf *mark_filter, complexf *space_filter, int taps_length);
+
 /* audio tail of the WFM graph, SURVEY 8(f) rank 1 (libcsdr.h:100-105; libcsdr.c:1081-1097, 1130-1137) */
 float deemphasis_wfm_ff(float *input, float *output, int input_size, float tau, int sample_rate, float last_output);
 void  limit_ff(float *input, float *output, int input_size, float max_amplitude);
@@ -553,6 +562,18 @@ int csdrb_serial_line_decoder_bank_f_u8(const float *d_in, long in_stride, int e
  * Returns 0. */
 int csdrb_rtty_baudot2ascii_bank_u8_u8(const unsigned char *d_in, long in_stride, unsigned char *d_out, long out_stride, int channels, int input_size,
                                        const int *d_lengths, unsigned char *d_fig_mode_io, int *d_count, void *stream);
+
+/* tone filter banks (tone.cu), one row per channel, the taps shared by all rows and on the device.  Row c's input is n complexf at
+ * d_in + c*in_stride; it gives the n - taps_length + 1 outputs of the valid convolution (the caller carries the last taps_length - 1 inputs
+ * between calls) at d_out + c*out_stride.
+ *   apply_fir_bank_cc: apply_fir_cc (libcsdr.c:2261-2273), complexf outputs, bit for bit with the reference build.
+ *   bfsk_demod_bank_cf: bfsk_demod_cf (libcsdr.c:2335-2351), float outputs |mark|^2 - |space|^2 of the two tap sets, summed in source order.
+ * Both return the outputs per row; -1 for a null or misaligned pointer (complexf 8 bytes, float 4), in_stride < n, out_stride < n - taps_length
+ * + 1 or n < taps_length; -2 (nothing launched) for taps_length outside 2..4096. */
+int csdrb_apply_fir_bank_cc(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int n, const complexf *d_taps,
+                            int taps_length, void *stream);
+int csdrb_bfsk_demod_bank_cf(const complexf *d_in, long in_stride, float *d_out, long out_stride, int channels, int n, const complexf *d_mark,
+                             const complexf *d_space, int taps_length, void *stream);
 
 /* K7 batched unnormalised c2c DFT (power-of-two size 2..16384), sign -1 forward / +1 inverse */
 int csdrb_fft_c2c_batch(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int size, int batch, int inverse, void *stream);
