@@ -9,7 +9,7 @@
  *     CSDR_DYNAMIC_BUFSIZE_ON, CSDR_PRINT_BUFSIZES (:394-417)
  *   - optional 8-byte "csdr"+int preamble in and out when dynamic buffer sizes are on (:330-339, :377-392)
  *   - EOF framing: the end-of-file test comes BEFORE the read, so a short final read is still processed and
- *     written as a whole block (:248 and every loop); shift_addition_cc alone stops on an empty read (:907)
+ *     written as a whole block (:248 and every loop); the shift commands also stop on an empty read (:907)
  *   - fflush + sched_yield after every block (:198); F_SETPIPE_SZ 2 MiB, 4096 for small blocks (:427-428, :369-373)
  *   - runtime retune over --fifo <path> / --fd <n>: text lines, non-blocking, last complete line wins (:252-323)
  *   - the stderr lines the reference prints for these commands
@@ -119,108 +119,135 @@ static int poll_control(int fd, const char *format, ...)
     return 1;
 }
 
+/* the starting tuning: the first line on the control channel when there is one (waited for), else argv[2] (and argv[3] for b);
+ * 0 when argv lacks it */
+static int initial_tuning(int ctl, int argc, char **argv, const char *format, float *a, float *b)
+{
+    if (ctl) { while (!poll_control(ctl, format, a, b)) usleep(10000); return 1; }
+    if (argc <= (b ? 3 : 2)) return 0;
+    sscanf(argv[2], "%g", a);
+    if (b) sscanf(argv[3], "%g", b);
+    return 1;
+}
+
+/* ---- shared framing ------------------------------------------------------------------------------ */
+/* One step call per block of the process on the whole buffer, written as out_count items.  The end-of-file test comes before the read, so a
+ * short final read is still processed and written as a whole block, its tail left over from the block before (:248).  Some reference loops
+ * also stop on an empty read (empty_read_stops). */
+static int map_blocks(size_t in_item, size_t out_item, int out_count, int empty_read_stops, void (*step)(void *in, void *out, void *state), void *state)
+{
+    void *in = must_alloc(in_item * (size_t)block), *out = must_alloc(out_item * (size_t)out_count);
+    for (;;) {
+        if (feof(stdin)) return 0;
+        if (!fread(in, in_item, (size_t)block, stdin) && empty_read_stops) return 0;
+        step(in, out, state);
+        fwrite(out, out_item, (size_t)out_count, stdout);
+        end_of_block();
+    }
+}
+
+/* keep the unconsumed tail of a buffer of `size` items at its front and read the `consumed` items behind it */
+static void refill(void *buf, size_t item, int size, int consumed)
+{
+    memmove(buf, (char *)buf + item * (size_t)consumed, item * (size_t)(size - consumed));
+    fread((char *)buf + item * (size_t)(size - consumed), item, (size_t)consumed, stdin);
+}
+
+/* the next FFT frame of `size` items, one starting every `every` items: overlapping frames slide, sparser ones are read whole and the rest
+ * is skipped in pieces of at most one block of complexf samples (whatever the frame's item, see fft_fc) */
+static void read_frame(void *in, size_t item, int size, int every, complexf *skip)
+{
+    if (every <= size) { refill(in, item, size, every); return; }
+    fread(in, item, (size_t)size, stdin);
+    for (int remain = every - size; remain > 0; remain -= block) fread(skip, sizeof(complexf), (size_t)(remain < block ? remain : block), stdin);
+}
+
+/* the pass-through special case of the resamplers (the reference's clone_): blocks of bytes copied through, the EOF test after the write */
+static int clone_blocks(void)
+{
+    char *buf = must_alloc((size_t)block);
+    for (;;) { fread(buf, 1, (size_t)block, stdin); fwrite(buf, 1, (size_t)block, stdout); end_of_block(); if (feof(stdin)) return 0; }
+}
+
+/* the optional window argument at argv[at]; without it the default window is named on stderr */
+static window_t window_arg(int argc, char **argv, int at)
+{
+    if (argc > at) return firdes_get_window_from_string(argv[at]);
+    who(); fprintf(stderr, "window = %s\n", firdes_get_string_from_window(WINDOW_DEFAULT));
+    return WINDOW_DEFAULT;
+}
+
+/* ---- the retunable NCO loop of shift_addition_cc/_fc, shift_unroll_cc and shift_addfast_cc (csdr.c:749-849, :877-934, :3365-3410) ----
+ * The rate comes from argv or the control channel.  Every block is shifted in calls of <= 1024 samples, the phasor re-seeded at each
+ * (:911-918); an empty read ends the stream (:907).  A new rate is polled after a block is written and before it is flushed; it
+ * re-initialises the NCO, and the phase carries on. */
+typedef union { shift_addition_data_t addition; shift_unroll_data_t unroll; shift_addfast_data_t addfast; } nco_t;
+
+static int nco_stream(int argc, char **argv, size_t in_item, void (*init)(nco_t *nco, float rate),
+                      float (*step)(void *in, complexf *out, int n, nco_t *nco, float phase), void (*release)(nco_t *nco))
+{
+    G.wideband = 1;
+    float phase = 0, rate = 0;
+    int ctl = open_control(argc, argv);
+    if (!initial_tuning(ctl, argc, argv, "%g\n", &rate, NULL)) return complain("need required parameter (rate)");
+    if (!announce_block(open_block())) return -2;
+    char *in = must_alloc(in_item * (size_t)block);
+    complexf *out = must_alloc(sizeof(complexf) * (size_t)block);
+    for (;;) {
+        nco_t nco;
+        init(&nco, rate);
+        who(); fprintf(stderr, "reinitialized to %g\n", rate);
+        for (;;) {
+            if (feof(stdin)) return 0;
+            if (!fread(in, in_item, (size_t)block, stdin)) break;
+            for (int done = 0; done < block;) {
+                int n = block - done > 1024 ? 1024 : block - done;
+                phase = step(in + in_item * (size_t)done, out + done, n, &nco, phase);
+                done += n;
+            }
+            fwrite(out, sizeof(complexf), (size_t)block, stdout);
+            if (poll_control(ctl, "%g\n", &rate)) break;
+            end_of_block();
+        }
+        if (release) release(&nco);
+    }
+}
+
 /* ---- commands ------------------------------------------------------------------------------------ */
+static void convert_u8_f_step(void *in, void *out, void *state) { (void)state; convert_u8_f(in, out, block); }
+static void convert_s16_f_step(void *in, void *out, void *state) { (void)state; convert_s16_f(in, out, block); }
+static void convert_f_s16_step(void *in, void *out, void *state) { (void)state; convert_f_s16(in, out, block); }
+
 static int cmd_convert_u8_f(int argc, char **argv)
 {
     (void)argc; (void)argv;
     if (!announce_block(open_block())) return -2;
-    unsigned char *in = must_alloc((size_t)block);
-    float *out = must_alloc(sizeof(float) * (size_t)block);
-    for (;;) {
-        if (feof(stdin)) return 0;
-        fread(in, 1, (size_t)block, stdin);
-        convert_u8_f(in, out, block);
-        fwrite(out, sizeof(float), (size_t)block, stdout);
-        end_of_block();
-    }
+    return map_blocks(1, sizeof(float), block, 0, convert_u8_f_step, NULL);
 }
 
 static int cmd_convert_s16_f(int argc, char **argv)
 {
     (void)argc; (void)argv;
     if (!announce_block(open_block())) return -2;
-    short *in = must_alloc(sizeof(short) * (size_t)block);
-    float *out = must_alloc(sizeof(float) * (size_t)block);
-    for (;;) {
-        if (feof(stdin)) return 0;
-        fread(in, sizeof(short), (size_t)block, stdin);
-        convert_s16_f(in, out, block);
-        fwrite(out, sizeof(float), (size_t)block, stdout);
-        end_of_block();
-    }
+    return map_blocks(sizeof(short), sizeof(float), block, 0, convert_s16_f_step, NULL);
 }
 
 static int cmd_convert_f_s16(int argc, char **argv)
 {
     (void)argc; (void)argv;
     if (!announce_block(open_block())) return -2;
-    float *in = must_alloc(sizeof(float) * (size_t)block);
-    short *out = must_alloc(sizeof(short) * (size_t)block);
-    for (;;) {
-        if (feof(stdin)) return 0;
-        fread(in, sizeof(float), (size_t)block, stdin);
-        convert_f_s16(in, out, block);
-        fwrite(out, sizeof(short), (size_t)block, stdout);
-        end_of_block();
-    }
+    return map_blocks(sizeof(float), sizeof(short), block, 0, convert_f_s16_step, NULL);
 }
 
-static int cmd_shift_addition_cc(int argc, char **argv)
-{
-    G.wideband = 1;
-    float phase = 0, rate = 0;
-    int ctl = open_control(argc, argv);
-    if (ctl) { while (!poll_control(ctl, "%g\n", &rate)) usleep(10000); }
-    else { if (argc <= 2) return complain("need required parameter (rate)"); sscanf(argv[2], "%g", &rate); }
-    if (!announce_block(open_block())) return -2;
-    complexf *in = must_alloc(sizeof(complexf) * (size_t)block), *out = must_alloc(sizeof(complexf) * (size_t)block);
-    for (;;) {
-        shift_addition_data_t nco = shift_addition_init(rate);
-        who(); fprintf(stderr, "reinitialized to %g\n", rate);
-        for (;;) {
-            if (feof(stdin)) return 0;
-            if (!fread(in, sizeof(complexf), (size_t)block, stdin)) break;
-            for (int done = 0; done < block;) {                         /* the phasor is re-seeded every <= 1024 samples (:911-918) */
-                int n = block - done > 1024 ? 1024 : block - done;
-                phase = shift_addition_cc(in + done, out + done, n, nco, phase);
-                done += n;
-            }
-            fwrite(out, sizeof(complexf), (size_t)block, stdout);
-            if (poll_control(ctl, "%g\n", &rate)) break;
-            end_of_block();
-        }
-    }
-}
+static void addition_init(nco_t *nco, float rate) { nco->addition = shift_addition_init(rate); }
+static float addition_cc(void *in, complexf *out, int n, nco_t *nco, float phase) { return shift_addition_cc(in, out, n, nco->addition, phase); }
+static float addition_fc(void *in, complexf *out, int n, nco_t *nco, float phase) { return shift_addition_fc(in, out, n, nco->addition, phase); }
+
+static int cmd_shift_addition_cc(int argc, char **argv) { return nco_stream(argc, argv, sizeof(complexf), addition_init, addition_cc, NULL); }
 
 /* csdr.c:3365-3410: cmd_shift_addition_cc with real input -- the big buffer, 1024-sample calls, the stop on an empty read and the retune
  * between buffers are the same; only the input is one float per sample */
-static int cmd_shift_addition_fc(int argc, char **argv)
-{
-    G.wideband = 1;
-    float phase = 0, rate = 0;
-    int ctl = open_control(argc, argv);
-    if (ctl) { while (!poll_control(ctl, "%g\n", &rate)) usleep(10000); }
-    else { if (argc <= 2) return complain("need required parameter (rate)"); sscanf(argv[2], "%g", &rate); }
-    if (!announce_block(open_block())) return -2;
-    float *in = must_alloc(sizeof(float) * (size_t)block);
-    complexf *out = must_alloc(sizeof(complexf) * (size_t)block);
-    for (;;) {
-        shift_addition_data_t nco = shift_addition_init(rate);
-        who(); fprintf(stderr, "reinitialized to %g\n", rate);
-        for (;;) {
-            if (feof(stdin)) return 0;
-            if (!fread(in, sizeof(float), (size_t)block, stdin)) break;
-            for (int done = 0; done < block;) {
-                int n = block - done > 1024 ? 1024 : block - done;
-                phase = shift_addition_fc(in + done, out + done, n, nco, phase);
-                done += n;
-            }
-            fwrite(out, sizeof(complexf), (size_t)block, stdout);
-            if (poll_control(ctl, "%g\n", &rate)) break;
-            end_of_block();
-        }
-    }
-}
+static int cmd_shift_addition_fc(int argc, char **argv) { return nco_stream(argc, argv, sizeof(float), addition_init, addition_fc, NULL); }
 
 static int cmd_fir_decimate_cc(int argc, char **argv)
 {
@@ -245,116 +272,56 @@ static int cmd_fir_decimate_cc(int argc, char **argv)
         int produced = fir_decimate_cc(in, out, block, factor, taps, taps_length);
         fwrite(out, sizeof(complexf), (size_t)produced, stdout);
         end_of_block();
-        int consumed = factor * produced;                                /* keep the unconsumed tail, refill behind it (:1172-1174) */
-        memmove(in, in + consumed, sizeof(complexf) * (size_t)(block - consumed));
-        fread(in + (block - consumed), sizeof(complexf), (size_t)consumed, stdin);
+        refill(in, sizeof(complexf), block, factor * produced);         /* keep the unconsumed tail, refill behind it (:1172-1174) */
     }
 }
+
+static void fmdemod_step(void *in, void *out, void *last) { *(complexf *)last = fmdemod_quadri_cf(in, out, block, NULL, *(complexf *)last); }
 
 static int cmd_fmdemod_quadri_cf(int argc, char **argv)
 {
     (void)argc; (void)argv;
     if (!announce_block(open_block())) return -2;
-    complexf *in = must_alloc(sizeof(complexf) * (size_t)block);
-    float *out = must_alloc(sizeof(float) * (size_t)block);
     complexf last = {0.f, 0.f};
-    for (;;) {
-        if (feof(stdin)) return 0;
-        fread(in, sizeof(complexf), (size_t)block, stdin);
-        last = fmdemod_quadri_cf(in, out, block, NULL, last);
-        fwrite(out, sizeof(float), (size_t)block, stdout);
-        end_of_block();
-    }
+    return map_blocks(sizeof(complexf), sizeof(float), block, 0, fmdemod_step, &last);
 }
 
-static int cmd_shift_unroll_cc(int argc, char **argv)                      /* csdr.c:800-849 */
-{
-    G.wideband = 1;
-    float phase = 0, rate = 0;
-    int ctl = open_control(argc, argv);
-    if (ctl) { while (!poll_control(ctl, "%g\n", &rate)) usleep(10000); }
-    else { if (argc <= 2) return complain("need required parameter (rate)"); sscanf(argv[2], "%g", &rate); }
-    if (!announce_block(open_block())) return -2;
-    complexf *in = must_alloc(sizeof(complexf) * (size_t)block), *out = must_alloc(sizeof(complexf) * (size_t)block);
-    for (;;) {
-        shift_unroll_data_t table = shift_unroll_init(rate, 1024);
-        who(); fprintf(stderr, "reinitialized to %g\n", rate);
-        for (;;) {
-            if (feof(stdin)) return 0;
-            if (!fread(in, sizeof(complexf), (size_t)block, stdin)) break;
-            for (int done = 0; done < block;) {
-                int n = block - done > 1024 ? 1024 : block - done;
-                phase = shift_unroll_cc(in + done, out + done, n, &table, phase);
-                done += n;
-            }
-            fwrite(out, sizeof(complexf), (size_t)block, stdout);
-            if (poll_control(ctl, "%g\n", &rate)) break;
-            end_of_block();
-        }
-        free(table.dsin); free(table.dcos);
-    }
-}
+static void unroll_init(nco_t *nco, float rate) { nco->unroll = shift_unroll_init(rate, 1024); }
+static float unroll_cc(void *in, complexf *out, int n, nco_t *nco, float phase) { return shift_unroll_cc(in, out, n, &nco->unroll, phase); }
+static void unroll_release(nco_t *nco) { free(nco->unroll.dsin); free(nco->unroll.dcos); }
+
+/* csdr.c:800-849 */
+static int cmd_shift_unroll_cc(int argc, char **argv) { return nco_stream(argc, argv, sizeof(complexf), unroll_init, unroll_cc, unroll_release); }
+
+typedef struct { float rate, phase; shift_table_data_t table; } shift_state_t;
+static void shift_math_step(void *in, void *out, void *s) { shift_state_t *st = s; st->phase = shift_math_cc(in, out, block, st->rate, st->phase); }
+static void shift_table_step(void *in, void *out, void *s) { shift_state_t *st = s; st->phase = shift_table_cc(in, out, block, st->rate, st->table, st->phase); }
 
 static int cmd_shift_math_cc(int argc, char **argv)                        /* csdr.c:703-718 */
 {
     if (argc <= 2) return complain("need required parameter (rate)");
-    float phase = 0, rate = 0; sscanf(argv[2], "%g", &rate);
+    shift_state_t st = {0}; sscanf(argv[2], "%g", &st.rate);
     if (!announce_block(open_block())) return -2;
-    complexf *in = must_alloc(sizeof(complexf) * (size_t)block), *out = must_alloc(sizeof(complexf) * (size_t)block);
-    for (;;) {
-        if (feof(stdin)) return 0;
-        if (!fread(in, sizeof(complexf), (size_t)block, stdin)) return 0;
-        phase = shift_math_cc(in, out, block, rate, phase);
-        fwrite(out, sizeof(complexf), (size_t)block, stdout);
-        end_of_block();
-    }
+    return map_blocks(sizeof(complexf), sizeof(complexf), block, 1, shift_math_step, &st);
 }
 
 static int cmd_shift_table_cc(int argc, char **argv)                       /* csdr.c:725-747 */
 {
     G.wideband = 1;
     if (argc <= 2) return complain("need required parameter (rate)");
-    float phase = 0, rate = 0; sscanf(argv[2], "%g", &rate);
+    shift_state_t st = {0}; sscanf(argv[2], "%g", &st.rate);
     int table_size = 65536; if (argc > 3) sscanf(argv[3], "%d", &table_size);
     if (!announce_block(open_block())) return -2;
-    shift_table_data_t table = shift_table_init(table_size);
+    st.table = shift_table_init(table_size);
     who(); fprintf(stderr, "LUT initialized\n");
-    complexf *in = must_alloc(sizeof(complexf) * (size_t)block), *out = must_alloc(sizeof(complexf) * (size_t)block);
-    for (;;) {
-        if (feof(stdin)) return 0;
-        if (!fread(in, sizeof(complexf), (size_t)block, stdin)) return 0;
-        phase = shift_table_cc(in, out, block, rate, table, phase);
-        fwrite(out, sizeof(complexf), (size_t)block, stdout);
-        end_of_block();
-    }
+    return map_blocks(sizeof(complexf), sizeof(complexf), block, 1, shift_table_step, &st);
 }
 
-static int cmd_shift_addfast_cc(int argc, char **argv)                     /* csdr.c:749-798 */
-{
-    G.wideband = 1;
-    float phase = 0, rate = 0;
-    int ctl = open_control(argc, argv);
-    if (ctl) { while (!poll_control(ctl, "%g\n", &rate)) usleep(10000); }
-    else { if (argc <= 2) return complain("need required parameter (rate)"); sscanf(argv[2], "%g", &rate); }
-    if (!announce_block(open_block())) return -2;
-    complexf *in = must_alloc(sizeof(complexf) * (size_t)block), *out = must_alloc(sizeof(complexf) * (size_t)block);
-    for (;;) {
-        shift_addfast_data_t steps = shift_addfast_init(rate);
-        who(); fprintf(stderr, "reinitialized to %g\n", rate);
-        for (;;) {
-            if (feof(stdin)) return 0;
-            if (!fread(in, sizeof(complexf), (size_t)block, stdin)) break;
-            for (int done = 0; done < block;) {
-                int n = block - done > 1024 ? 1024 : block - done;
-                phase = shift_addfast_cc(in + done, out + done, n, &steps, phase);
-                done += n;
-            }
-            fwrite(out, sizeof(complexf), (size_t)block, stdout);
-            if (poll_control(ctl, "%g\n", &rate)) break;
-            end_of_block();
-        }
-    }
-}
+static void addfast_init(nco_t *nco, float rate) { nco->addfast = shift_addfast_init(rate); }
+static float addfast_cc(void *in, complexf *out, int n, nco_t *nco, float phase) { return shift_addfast_cc(in, out, n, &nco->addfast, phase); }
+
+/* csdr.c:749-798 */
+static int cmd_shift_addfast_cc(int argc, char **argv) { return nco_stream(argc, argv, sizeof(complexf), addfast_init, addfast_cc, NULL); }
 
 static int cmd_decimating_shift_addition_cc(int argc, char **argv)         /* csdr.c:851-875 */
 {
@@ -382,8 +349,7 @@ static int cmd_fft_cc(int argc, char **argv)                               /* cs
     int fft_size = 0; sscanf(argv[2], "%d", &fft_size);
     if (log2n(fft_size) == -1) return complain("fft_size should be power of 2");
     int every = 0; sscanf(argv[3], "%d", &every);
-    window_t window = WINDOW_DEFAULT;
-    if (argc >= 5) window = firdes_get_window_from_string(argv[4]);
+    window_t window = argc >= 5 ? firdes_get_window_from_string(argv[4]) : WINDOW_DEFAULT;
     if (!open_block()) return -2;
     announce_block(fft_size);
     complexf *in = fft_malloc(sizeof(complexf) * (size_t)fft_size), *win = fft_malloc(sizeof(complexf) * (size_t)fft_size);
@@ -394,13 +360,7 @@ static int cmd_fft_cc(int argc, char **argv)                               /* cs
     memset(in, 0, sizeof(complexf) * (size_t)fft_size);
     for (;;) {
         if (feof(stdin)) return 0;
-        if (every > fft_size) {
-            fread(in, sizeof(complexf), (size_t)fft_size, stdin);
-            for (int remain = every - fft_size; remain > 0; remain -= block) fread(skip, sizeof(complexf), (size_t)(remain < block ? remain : block), stdin);
-        } else {
-            memmove(in, in + every, sizeof(complexf) * (size_t)(fft_size - every));
-            fread(in + fft_size - every, sizeof(complexf), (size_t)every, stdin);
-        }
+        read_frame(in, sizeof(complexf), fft_size, every, skip);
         apply_precalculated_window_c(in, win, fft_size, table);
         fft_execute(plan);
         fwrite(out, sizeof(complexf), (size_t)fft_size, stdout);
@@ -421,8 +381,7 @@ static int cmd_fft_fc(int argc, char **argv)
     const int in_size = 2 * out_size;
     int every = 0; sscanf(argv[3], "%d", &every);
     if (every < 1) return complain("out_of_every_n_samples must be at least 1");
-    window_t window = WINDOW_DEFAULT;
-    if (argc >= 5) window = firdes_get_window_from_string(argv[4]);
+    window_t window = argc >= 5 ? firdes_get_window_from_string(argv[4]) : WINDOW_DEFAULT;
     if (!open_block()) return -2;
     announce_block(out_size);
     float *in = fft_malloc(sizeof(float) * (size_t)in_size), *win = fft_malloc(sizeof(float) * (size_t)in_size);
@@ -433,13 +392,7 @@ static int cmd_fft_fc(int argc, char **argv)
     memset(in, 0, sizeof(float) * (size_t)in_size);
     for (;;) {
         if (feof(stdin)) return 0;
-        if (every > in_size) {
-            fread(in, sizeof(float), (size_t)in_size, stdin);
-            for (int remain = every - in_size; remain > 0; remain -= block) fread(skip, sizeof(complexf), (size_t)(remain < block ? remain : block), stdin);
-        } else {
-            memmove(in, in + every, sizeof(float) * (size_t)(in_size - every));
-            fread(in + in_size - every, sizeof(float), (size_t)every, stdin);
-        }
+        read_frame(in, sizeof(float), in_size, every, skip);               /* the skip counts complexf samples, as above */
         apply_precalculated_window_f(in, win, in_size, table);
         fft_execute(plan);
         fwrite(out, sizeof(complexf), (size_t)out_size, stdout);
@@ -447,19 +400,13 @@ static int cmd_fft_fc(int argc, char **argv)
     }
 }
 
+static void logpower_step(void *in, void *out, void *add_db) { logpower_cf(in, out, block, *(float *)add_db); }
+
 static int cmd_logpower_cf(int argc, char **argv)                          /* csdr.c:1645-1661 */
 {
     float add_db = 0; if (argc >= 3) sscanf(argv[2], "%g", &add_db);
     if (!announce_block(open_block())) return -2;
-    complexf *in = must_alloc(sizeof(complexf) * (size_t)block);
-    float *out = must_alloc(sizeof(float) * (size_t)block);
-    for (;;) {
-        if (feof(stdin)) return 0;
-        fread(in, sizeof(complexf), (size_t)block, stdin);
-        logpower_cf(in, out, block, add_db);
-        fwrite(out, sizeof(float), (size_t)block, stdout);
-        end_of_block();
-    }
+    return map_blocks(sizeof(complexf), sizeof(float), block, 0, logpower_step, &add_db);
 }
 
 static int cmd_logaveragepower_cf(int argc, char **argv)                   /* csdr.c:1663-1695 */
@@ -522,53 +469,37 @@ static int cmd_compress_fft_adpcm_f_u8(int argc, char **argv)              /* cs
     }
 }
 
+static void adpcm_step(void *in, void *out, void *st) { *(ima_adpcm_state_t *)st = encode_ima_adpcm_i16_u8(in, out, block, *(ima_adpcm_state_t *)st); }
+
 static int cmd_encode_ima_adpcm(int argc, char **argv)                     /* csdr.c:1891-1904 */
 {
     (void)argc; (void)argv;
     if (!open_block()) return -2;
     announce_block(block / 2);
-    short *in = must_alloc(sizeof(short) * (size_t)block);
-    unsigned char *out = must_alloc((size_t)block / 2 + 1);
     ima_adpcm_state_t st = {0, 0};
-    for (;;) {
-        if (feof(stdin)) return 0;
-        fread(in, sizeof(short), (size_t)block, stdin);
-        st = encode_ima_adpcm_i16_u8(in, out, block, st);
-        fwrite(out, 1, (size_t)block / 2, stdout);
-        end_of_block();
-    }
+    return map_blocks(sizeof(short), 1, block / 2, 0, adpcm_step, &st);
 }
+
+static void limit_step(void *in, void *out, void *max_amplitude) { limit_ff(in, out, block, *(float *)max_amplitude); }
 
 static int cmd_limit_ff(int argc, char **argv)                              /* csdr.c:673-686 */
 {
     float max_amplitude = 1.0f; if (argc >= 3) sscanf(argv[2], "%g", &max_amplitude);
     if (!announce_block(open_block())) return -2;
-    float *in = must_alloc(sizeof(float) * (size_t)block), *out = must_alloc(sizeof(float) * (size_t)block);
-    for (;;) {
-        if (feof(stdin)) return 0;
-        fread(in, sizeof(float), (size_t)block, stdin);
-        limit_ff(in, out, block, max_amplitude);
-        fwrite(out, sizeof(float), (size_t)block, stdout);
-        end_of_block();
-    }
+    return map_blocks(sizeof(float), sizeof(float), block, 0, limit_step, &max_amplitude);
 }
+
+typedef struct { float tau; int sample_rate; float last; } deemphasis_wfm_t;
+static void deemphasis_wfm_step(void *in, void *out, void *s) { deemphasis_wfm_t *d = s; d->last = deemphasis_wfm_ff(in, out, block, d->tau, d->sample_rate, d->last); }
 
 static int cmd_deemphasis_wfm_ff(int argc, char **argv)                     /* csdr.c:1014-1032 */
 {
     if (argc <= 3) return complain("need required parameters (sample rate, tau)");
     if (!announce_block(open_block())) return -2;
-    int sample_rate = 0; sscanf(argv[2], "%d", &sample_rate);
-    float tau = 0; sscanf(argv[3], "%g", &tau);
-    who(); fprintf(stderr, "tau = %g, sample_rate = %d\n", tau, sample_rate);
-    float *in = must_alloc(sizeof(float) * (size_t)block), *out = must_alloc(sizeof(float) * (size_t)block);
-    float last = 0;
-    for (;;) {
-        if (feof(stdin)) return 0;
-        fread(in, sizeof(float), (size_t)block, stdin);
-        last = deemphasis_wfm_ff(in, out, block, tau, sample_rate, last);
-        fwrite(out, sizeof(float), (size_t)block, stdout);
-        end_of_block();
-    }
+    deemphasis_wfm_t d = {0, 0, 0};
+    sscanf(argv[2], "%d", &d.sample_rate); sscanf(argv[3], "%g", &d.tau);
+    who(); fprintf(stderr, "tau = %g, sample_rate = %d\n", d.tau, d.sample_rate);
+    return map_blocks(sizeof(float), sizeof(float), block, 0, deemphasis_wfm_step, &d);
 }
 
 static int cmd_deemphasis_nfm_ff(int argc, char **argv)                     /* csdr.c:1068-1087 */
@@ -607,10 +538,8 @@ static int cmd_fractional_decimator_ff(int argc, char **argv)
                    firdes_get_string_from_window(window));
     if (!open_block()) return -2;
     announce_block((int)(block / rate));
+    if (rate == 1) return clone_blocks();                               /* pass-through special case (:1498, clone_) */
     float *in = must_alloc(sizeof(float) * (size_t)block), *out = must_alloc(sizeof(float) * (size_t)block);
-    if (rate == 1) {                                                    /* pass-through special case (:1498, clone_) */
-        for (;;) { fread(in, 1, (size_t)block, stdin); fwrite(in, 1, (size_t)block, stdout); end_of_block(); if (feof(stdin)) return 0; }
-    }
     int taps_length = 0; float *taps = NULL;
     if (prefilter) {
         taps_length = firdes_filter_len(transition_bw);
@@ -622,8 +551,7 @@ static int cmd_fractional_decimator_ff(int argc, char **argv)
     for (;;) {
         if (feof(stdin)) return 0;
         if (d.input_processed == 0) d.input_processed = block;
-        else memcpy(in, in + d.input_processed, sizeof(float) * (size_t)(block - d.input_processed));
-        fread(in + (block - d.input_processed), sizeof(float), (size_t)d.input_processed, stdin);
+        refill(in, sizeof(float), block, d.input_processed);
         fractional_decimator_ff(in, out, block, &d);
         fwrite(out, sizeof(float), (size_t)d.output_size, stdout);
         end_of_block();
@@ -636,16 +564,14 @@ static int cmd_rational_resampler_ff(int argc, char **argv)                 /* c
     int interpolation = 0, decimation = 0;
     sscanf(argv[2], "%d", &interpolation); sscanf(argv[3], "%d", &decimation);
     float transition_bw = 0.05f; if (argc >= 5) sscanf(argv[4], "%g", &transition_bw);
-    window_t window = WINDOW_DEFAULT;
-    if (argc >= 6) window = firdes_get_window_from_string(argv[5]);
-    else { who(); fprintf(stderr, "window = %s\n", firdes_get_string_from_window(window)); }
+    window_t window = window_arg(argc, argv, 5);
     if (!open_block()) return -2;
-    float *in = must_alloc(sizeof(float) * (size_t)block);
     if (interpolation == 1 && decimation == 1) {                        /* pass-through special case (:1438, clone_) */
         announce_block(block);
-        for (;;) { fread(in, 1, (size_t)block, stdin); fwrite(in, 1, (size_t)block, stdout); end_of_block(); if (feof(stdin)) return 0; }
+        return clone_blocks();
     }
     if (interpolation < 1 || decimation < 1) return complain("interpolation and decimation must be positive integers");
+    float *in = must_alloc(sizeof(float) * (size_t)block);
     const int out_size = (int)((long)block * interpolation / decimation);
     announce_block(out_size);
     float *out = must_alloc(sizeof(float) * (size_t)(out_size > 0 ? out_size : 1));
@@ -656,8 +582,7 @@ static int cmd_rational_resampler_ff(int argc, char **argv)                 /* c
     for (;;) {
         if (feof(stdin)) return 0;
         if (d.input_processed == 0) d.input_processed = block;
-        else memmove(in, in + d.input_processed, sizeof(float) * (size_t)(block - d.input_processed));
-        fread(in + (block - d.input_processed), sizeof(float), (size_t)d.input_processed, stdin);
+        refill(in, sizeof(float), block, d.input_processed);
         d = rational_resampler_ff(in, out, block, interpolation, decimation, taps, taps_length, d.last_taps_delay);
         fwrite(out, sizeof(float), (size_t)d.output_size, stdout);
         end_of_block();
@@ -684,32 +609,22 @@ static int cmd_fastagc_ff(int argc, char **argv)
     }
 }
 
+static void amdemod_step(void *in, void *out, void *state) { (void)state; amdemod_cf(in, out, block); }
+
 static int cmd_amdemod_cf(int argc, char **argv)                            /* csdr.c:1088-1100 */
 {
     (void)argc; (void)argv;
     if (!announce_block(open_block())) return -2;
-    complexf *in = must_alloc(sizeof(complexf) * (size_t)block); float *out = must_alloc(sizeof(float) * (size_t)block);
-    for (;;) {
-        if (feof(stdin)) return 0;
-        fread(in, sizeof(complexf), (size_t)block, stdin);
-        amdemod_cf(in, out, block);
-        fwrite(out, sizeof(float), (size_t)block, stdout);
-        end_of_block();
-    }
+    return map_blocks(sizeof(complexf), sizeof(float), block, 0, amdemod_step, NULL);
 }
+
+static void realpart_step(void *in, void *out, void *state) { (void)state; for (int i = 0; i < block; i++) ((float *)out)[i] = ((complexf *)in)[i].i; }
 
 static int cmd_realpart_cf(int argc, char **argv)                           /* csdr.c:634-645: pure I/O, the I of every sample */
 {
     (void)argc; (void)argv;
     if (!announce_block(open_block())) return -2;
-    float *in = must_alloc(sizeof(float) * 2 * (size_t)block), *out = must_alloc(sizeof(float) * (size_t)block);
-    for (;;) {
-        if (feof(stdin)) return 0;
-        fread(in, sizeof(float) * 2, (size_t)block, stdin);
-        for (int i = 0; i < block; i++) out[i] = in[2 * i];
-        fwrite(out, sizeof(float), (size_t)block, stdout);
-        end_of_block();
-    }
+    return map_blocks(sizeof(complexf), sizeof(float), block, 0, realpart_step, NULL);
 }
 
 static int cmd_fastdcblock_ff(int argc, char **argv)                        /* csdr.c:952-968: its own block size, in place */
@@ -729,41 +644,35 @@ static int cmd_fastdcblock_ff(int argc, char **argv)                        /* c
     }
 }
 
+typedef struct { short hang_time, attack_wait; float reference, attack_rate, decay_rate, max_gain, filter_alpha, last_gain; } agc_args_t;
+static void agc_step(void *in, void *out, void *s)
+{
+    agc_args_t *a = s;
+    a->last_gain = agc_ff(in, out, block, a->reference, a->attack_rate, a->decay_rate, a->max_gain, a->hang_time, a->attack_wait, a->filter_alpha, a->last_gain);
+}
+
 static int cmd_agc_ff(int argc, char **argv)                                /* csdr.c:1337-1373: one agc_ff call per block */
 {
-    short hang_time = 200; if (argc >= 3) sscanf(argv[2], "%hd", &hang_time);
-    float reference = 0.2f; if (argc >= 4) sscanf(argv[3], "%g", &reference);
-    float attack_rate = 0.01f; if (argc >= 5) sscanf(argv[4], "%g", &attack_rate);
-    float decay_rate = 0.0001f; if (argc >= 6) sscanf(argv[5], "%g", &decay_rate);
-    float max_gain = 65536.0f; if (argc >= 7) sscanf(argv[6], "%g", &max_gain);
-    short attack_wait = 0; if (argc >= 8) sscanf(argv[7], "%hd", &attack_wait);
-    float filter_alpha = 0.999f; if (argc >= 9) sscanf(argv[8], "%g", &filter_alpha);
+    agc_args_t a = {200, 0, 0.2f, 0.01f, 0.0001f, 65536.0f, 0.999f, 1.0f};
+    if (argc >= 3) sscanf(argv[2], "%hd", &a.hang_time);
+    if (argc >= 4) sscanf(argv[3], "%g", &a.reference);
+    if (argc >= 5) sscanf(argv[4], "%g", &a.attack_rate);
+    if (argc >= 6) sscanf(argv[5], "%g", &a.decay_rate);
+    if (argc >= 7) sscanf(argv[6], "%g", &a.max_gain);
+    if (argc >= 8) sscanf(argv[7], "%hd", &a.attack_wait);
+    if (argc >= 9) sscanf(argv[8], "%g", &a.filter_alpha);
     if (!announce_block(open_block())) return -2;
-    float *in = must_alloc(sizeof(float) * (size_t)block), *out = must_alloc(sizeof(float) * (size_t)block);
-    float last_gain = 1.0f;
-    for (;;) {
-        if (feof(stdin)) return 0;
-        fread(in, sizeof(float), (size_t)block, stdin);
-        last_gain = agc_ff(in, out, block, reference, attack_rate, decay_rate, max_gain, hang_time, attack_wait, filter_alpha, last_gain);
-        fwrite(out, sizeof(float), (size_t)block, stdout);
-        end_of_block();
-    }
+    return map_blocks(sizeof(float), sizeof(float), block, 0, agc_step, &a);
 }
 
 static int cmd_bandpass_fir_fft_cc(int argc, char **argv)
 {
-    float low_cut = 0, high_cut = 0, transition_bw = 0; window_t window = WINDOW_DEFAULT;
+    float low_cut = 0, high_cut = 0, transition_bw = 0;
     int ctl = open_control(argc, argv);
-    if (ctl) {
-        while (!poll_control(ctl, "%g %g\n", &low_cut, &high_cut)) usleep(10000);
-        if (argc <= 4) return complain("need more required parameters (transition_bw)");
-    } else {
-        if (argc <= 4) return complain("need required parameters (low_cut, high_cut, transition_bw)");
-        sscanf(argv[2], "%g", &low_cut); sscanf(argv[3], "%g", &high_cut);
-    }
+    if (!initial_tuning(ctl, argc, argv, "%g %g\n", &low_cut, &high_cut) || argc <= 4)
+        return complain(ctl ? "need more required parameters (transition_bw)" : "need required parameters (low_cut, high_cut, transition_bw)");
     sscanf(argv[4], "%g", &transition_bw);
-    if (argc >= 6) window = firdes_get_window_from_string(argv[5]);
-    else { who(); fprintf(stderr, "window = %s\n", firdes_get_string_from_window(window)); }
+    window_t window = window_arg(argc, argv, 5);
     int taps_length = firdes_filter_len(transition_bw);
     int fft_size = next_pow2(taps_length);
     if (fft_size - taps_length < 200) fft_size <<= 1;
@@ -802,9 +711,7 @@ static int cmd_fastddc_fwd_cc(int argc, char **argv)
     if (argc <= 2) return complain("need required parameter (decimation)");
     int decimation = 0; sscanf(argv[2], "%d", &decimation);
     float transition_bw = 0.05f; if (argc > 3) sscanf(argv[3], "%g", &transition_bw);
-    window_t window = WINDOW_DEFAULT;
-    if (argc > 4) window = firdes_get_window_from_string(argv[4]);
-    else { who(); fprintf(stderr, "window = %s\n", firdes_get_string_from_window(window)); }
+    window_arg(argc, argv, 4);                                          /* parsed, but the forward transform has no window (:2295) */
     fastddc_t ddc;
     if (fastddc_init(&ddc, transition_bw, decimation, 0)) { complain("error in fastddc_init()"); return 1; }
     fastddc_print(&ddc, "fastddc_fwd_cc");
@@ -818,9 +725,8 @@ static int cmd_fastddc_fwd_cc(int argc, char **argv)
     if (!plan) return complain("FFT size error.");
     for (;;) {
         if (feof(stdin)) return 0;
-        memmove(in, in + ddc.input_size, sizeof(complexf) * (size_t)ddc.overlap_length);      /* overlap-save (:2292) */
-        fread(in + ddc.overlap_length, sizeof(complexf), (size_t)ddc.input_size, stdin);
-        fft_execute(plan);                                                                       /* no window (:2295) */
+        refill(in, sizeof(complexf), ddc.fft_size, ddc.input_size);                             /* overlap-save (:2292) */
+        fft_execute(plan);                                                                      /* no window (:2295) */
         fwrite(out, sizeof(complexf), (size_t)ddc.fft_size, stdout);
         end_of_block();
     }
@@ -828,16 +734,14 @@ static int cmd_fastddc_fwd_cc(int argc, char **argv)
 
 static int cmd_fastddc_inv_cc(int argc, char **argv)
 {
-    float shift_rate = 0; int plus = 0;
+    float shift_rate = 0;
     int ctl = open_control(argc, argv);
-    if (ctl) { while (!poll_control(ctl, "%g\n", &shift_rate)) usleep(10000); plus = 1; }
-    else { if (argc <= 2) return complain("need required parameter (rate)"); sscanf(argv[2], "%g", &shift_rate); }
+    if (!initial_tuning(ctl, argc, argv, "%g\n", &shift_rate, NULL)) return complain("need required parameter (rate)");
+    const int plus = ctl ? 1 : 0;                                        /* "--fd <fd>" takes the place of <shift_rate> */
     if (argc <= 3 + plus) return complain("need required parameter (decimation)");
     int decimation = 0; sscanf(argv[3 + plus], "%d", &decimation);
     float transition_bw = 0.05f; if (argc > 4 + plus) sscanf(argv[4 + plus], "%g", &transition_bw);
-    window_t window = WINDOW_DEFAULT;
-    if (argc > 5 + plus) window = firdes_get_window_from_string(argv[5 + plus]);
-    else { who(); fprintf(stderr, "window = %s\n", firdes_get_string_from_window(window)); }
+    window_t window = window_arg(argc, argv, 5 + plus);
     for (;;) {
         fastddc_t ddc;
         if (fastddc_init(&ddc, transition_bw, decimation, shift_rate)) { complain("error in fastddc_init()"); return 1; }
@@ -872,26 +776,21 @@ static int cmd_fastddc_inv_cc(int argc, char **argv)
     }
 }
 
+typedef struct { float rate, reference, max_gain, gain; } simple_agc_args_t;
+static void simple_agc_step(void *in, void *out, void *s) { simple_agc_args_t *a = s; simple_agc_cc(in, out, block, a->rate, a->reference, a->max_gain, &a->gain); }
+
 static int cmd_simple_agc_cc(int argc, char **argv)                          /* csdr.c:2902-2931 */
 {
-    float rate = 0.f;
+    simple_agc_args_t a = {0.f, 1.f, 65535.f, 1.f};
     if (argc <= 2) return complain("need required parameter (rate)");
-    sscanf(argv[2], "%f", &rate);
-    if (rate <= 0) return complain("rate should be > 0");
-    float reference = 1.f; if (argc > 3) sscanf(argv[3], "%f", &reference);
-    if (reference <= 0) return complain("reference should be > 0");
-    float max_gain = 65535.f; if (argc > 4) sscanf(argv[4], "%f", &max_gain);
-    if (max_gain <= 0) return complain("max_gain should be > 0");
+    sscanf(argv[2], "%f", &a.rate);
+    if (a.rate <= 0) return complain("rate should be > 0");
+    if (argc > 3) sscanf(argv[3], "%f", &a.reference);
+    if (a.reference <= 0) return complain("reference should be > 0");
+    if (argc > 4) sscanf(argv[4], "%f", &a.max_gain);
+    if (a.max_gain <= 0) return complain("max_gain should be > 0");
     if (!announce_block(open_block())) return -2;
-    complexf *in = must_alloc(sizeof(complexf) * (size_t)block), *out = must_alloc(sizeof(complexf) * (size_t)block);
-    float gain = 1.f;
-    for (;;) {
-        if (feof(stdin)) return 0;
-        fread(in, sizeof(complexf), (size_t)block, stdin);
-        simple_agc_cc(in, out, block, rate, reference, max_gain, &gain);
-        fwrite(out, sizeof(complexf), (size_t)block, stdout);
-        end_of_block();
-    }
+    return map_blocks(sizeof(complexf), sizeof(complexf), block, 0, simple_agc_step, &a);
 }
 
 static int cmd_timing_recovery_cc(int argc, char **argv)                     /* csdr.c:2573-2637 */
@@ -932,49 +831,55 @@ static int cmd_timing_recovery_cc(int argc, char **argv)                     /* 
         } else fwrite(out, sizeof(complexf), (size_t)state.output_size, stdout);
         end_of_block();
         buffer_start_counter += (unsigned)state.input_processed;          /* keep the unconsumed tail, refill behind it */
-        memmove(in, in + state.input_processed, sizeof(complexf) * (size_t)(block - state.input_processed));
-        fread(in + (block - state.input_processed), sizeof(complexf), (size_t)state.input_processed, stdin);
+        refill(in, sizeof(complexf), block, state.input_processed);
     }
 }
+
+static void dbpsk_step(void *in, void *out, void *state) { (void)state; dbpsk_decoder_c_u8(in, out, block); }
 
 static int cmd_dbpsk_decoder_c_u8(int argc, char **argv)                     /* csdr.c:3256-3268 */
 {
     (void)argc; (void)argv;
     if (!announce_block(open_block())) return -2;
-    complexf *in = must_alloc(sizeof(complexf) * (size_t)block);
-    unsigned char *out = must_alloc((size_t)block);
-    for (;;) {
-        if (feof(stdin)) return 0;
-        fread(in, sizeof(complexf), (size_t)block, stdin);
-        dbpsk_decoder_c_u8(in, out, block);
-        fwrite(out, 1, (size_t)block, stdout);
-        end_of_block();
-    }
+    return map_blocks(sizeof(complexf), 1, block, 0, dbpsk_step, NULL);
 }
 
-/* csdr.c:2418-2430 pushes one getchar() at a time through psk31_varicode_decoder_push and flushes every character.  Here every read()
- * (whatever the pipe holds, up to one block) goes through the varicode bank, and the characters it decoded are written and flushed at once. */
-static int cmd_psk31_varicode_decoder_u8_u8(int argc, char **argv)
+/* The byte decoders on the GPU: every read() (whatever the pipe holds, up to one block) goes through one call of the decoder bank, which carries
+ * its zero-initialised state_size bytes of state on the device, and the characters it decoded are written and flushed at once.  stdin is
+ * unbuffered, so reading a preamble takes its 8 bytes and no more: whatever follows is left to read(). */
+static int byte_decoder_stream(int (*bank)(const unsigned char *d_in, int n, unsigned char *d_out, void *d_state, int *d_count), size_t state_size)
 {
-    (void)argc; (void)argv;
+    setvbuf(stdin, NULL, _IONBF, 0);
     if (!announce_block(open_block())) return -2;
     unsigned char *in = must_alloc((size_t)block), *out = must_alloc((size_t)block);
     unsigned char *d_in = csdrb_device_alloc((size_t)block), *d_out = csdrb_device_alloc((size_t)block);
-    unsigned long long *d_hist = csdrb_device_alloc(sizeof(unsigned long long));      /* zero-filled: the reference's status_shr = 0 */
+    void *d_state = csdrb_device_alloc(state_size);                           /* zero-filled */
     int *d_count = csdrb_device_alloc(sizeof(int));
-    if (!d_in || !d_out || !d_hist || !d_count) { who(); fprintf(stderr, "%s\n", csdrb_last_error()); return -2; }
+    if (!d_in || !d_out || !d_state || !d_count) { who(); fprintf(stderr, "%s\n", csdrb_last_error()); return -2; }
     for (;;) {
         const ssize_t got = read(STDIN_FILENO, in, (size_t)block);
         if (got <= 0) return 0;
         int count = 0;
-        if (csdrb_copy_h2d(d_in, in, (size_t)got, NULL) < 0 ||
-            csdrb_psk31_varicode_decoder_bank_u8_u8(d_in, got, d_out, got, 1, (int)got, NULL, d_hist, d_count, NULL) < 0 ||
+        if (csdrb_copy_h2d(d_in, in, (size_t)got, NULL) < 0 || bank(d_in, (int)got, d_out, d_state, d_count) < 0 ||
             csdrb_copy_d2h(&count, d_count, sizeof count, NULL) < 0 || csdrb_stream_synchronize(NULL) < 0 ||
             (count > 0 && (csdrb_copy_d2h(out, d_out, (size_t)count, NULL) < 0 || csdrb_stream_synchronize(NULL) < 0))) {
             who(); fprintf(stderr, "%s\n", csdrb_last_error()); return -2;
         }
         if (count > 0) { fwrite(out, 1, (size_t)count, stdout); fflush(stdout); }
     }
+}
+
+static int varicode_bank(const unsigned char *d_in, int n, unsigned char *d_out, void *d_hist, int *d_count)
+{
+    return csdrb_psk31_varicode_decoder_bank_u8_u8(d_in, n, d_out, n, 1, n, NULL, d_hist, d_count, NULL);
+}
+
+/* csdr.c:2418-2430 pushes one getchar() at a time through psk31_varicode_decoder_push and flushes every character; here the varicode bank
+ * decodes whole reads.  Its state is the reference's status_shr, 0 at the start. */
+static int cmd_psk31_varicode_decoder_u8_u8(int argc, char **argv)
+{
+    (void)argc; (void)argv;
+    return byte_decoder_stream(varicode_bank, sizeof(unsigned long long));
 }
 
 static int cmd_serial_line_decoder_f_u8(int argc, char **argv)               /* csdr.c:2490-2530 */
@@ -986,11 +891,9 @@ static int cmd_serial_line_decoder_f_u8(int argc, char **argv)               /* 
     if (serial.samples_per_bits < 1) return complain("samples_per_bits should be at least 1.");
     if (serial.samples_per_bits < 5)
         fprintf(stderr, "%s: warning: this algorithm does not work well if samples_per_bits is too low. It should be at least 5.\n", argv[1]);
-    serial.databits = 8;
-    if (argc > 3) sscanf(argv[3], "%d", &serial.databits);
+    serial.databits = 8; if (argc > 3) sscanf(argv[3], "%d", &serial.databits);
     if (serial.databits > 8 || serial.databits < 1) return complain("databits should be between 1 and 8.");
-    serial.stopbits = 1;
-    if (argc > 4) sscanf(argv[4], "%f", &serial.stopbits);
+    serial.stopbits = 1; if (argc > 4) sscanf(argv[4], "%f", &serial.stopbits);
     if (serial.stopbits < 1) return complain("stopbits should be equal or above 1.");
     serial.bit_sampling_width_ratio = 0.4f;
     if (!announce_block(open_block())) return -2;
@@ -1000,10 +903,7 @@ static int cmd_serial_line_decoder_f_u8(int argc, char **argv)               /* 
      * holds the samples of the call before, and that last call is decoded and written like any other */
     for (;;) {
         if (feof(stdin)) return 0;
-        if (serial.input_used) {
-            memmove(in, in + serial.input_used, sizeof(float) * (size_t)(block - serial.input_used));
-            fread(in + (block - serial.input_used), sizeof(float), (size_t)serial.input_used, stdin);
-        } else fread(in, sizeof(float), (size_t)block, stdin);
+        refill(in, sizeof(float), block, serial.input_used ? serial.input_used : block);
         serial_line_decoder_f_u8(&serial, in, out, block);
         if (serial.input_used == 0) { who(); fprintf(stderr, "error: serial_line_decoder_f_u8() got stuck.\n"); return -3; }
         fwrite(out, 1, (size_t)serial.output_size, stdout);
@@ -1011,30 +911,18 @@ static int cmd_serial_line_decoder_f_u8(int argc, char **argv)               /* 
     }
 }
 
+static int baudot_bank(const unsigned char *d_in, int n, unsigned char *d_out, void *d_mode, int *d_count)
+{
+    return csdrb_rtty_baudot2ascii_bank_u8_u8(d_in, n, d_out, n, 1, n, NULL, d_mode, d_count, NULL);
+}
+
 /* csdr.c:2461-2474 pushes one getchar() at a time through rtty_baudot_decoder_lookup and flushes every character; after the end of the input
- * it pushes up to 255 EOF values (0xFF), which give nothing.  Here every read() (whatever the pipe holds, up to one block) goes through the
- * baudot bank, and the characters it decoded are written and flushed at once. */
+ * it pushes up to 255 EOF values (0xFF), which give nothing.  Here the baudot bank decodes whole reads.  Its state is the letters (0) / figures
+ * mode, letters at the start as fig_mode = 0. */
 static int cmd_rtty_baudot2ascii_u8_u8(int argc, char **argv)
 {
     (void)argc; (void)argv;
-    if (!announce_block(open_block())) return -2;
-    unsigned char *in = must_alloc((size_t)block), *out = must_alloc((size_t)block);
-    unsigned char *d_in = csdrb_device_alloc((size_t)block), *d_out = csdrb_device_alloc((size_t)block);
-    unsigned char *d_mode = csdrb_device_alloc(1);                             /* zero-filled: letters mode, as fig_mode = 0 */
-    int *d_count = csdrb_device_alloc(sizeof(int));
-    if (!d_in || !d_out || !d_mode || !d_count) { who(); fprintf(stderr, "%s\n", csdrb_last_error()); return -2; }
-    for (;;) {
-        const ssize_t got = read(STDIN_FILENO, in, (size_t)block);
-        if (got <= 0) return 0;
-        int count = 0;
-        if (csdrb_copy_h2d(d_in, in, (size_t)got, NULL) < 0 ||
-            csdrb_rtty_baudot2ascii_bank_u8_u8(d_in, got, d_out, got, 1, (int)got, NULL, d_mode, d_count, NULL) < 0 ||
-            csdrb_copy_d2h(&count, d_count, sizeof count, NULL) < 0 || csdrb_stream_synchronize(NULL) < 0 ||
-            (count > 0 && (csdrb_copy_d2h(out, d_out, (size_t)count, NULL) < 0 || csdrb_stream_synchronize(NULL) < 0))) {
-            who(); fprintf(stderr, "%s\n", csdrb_last_error()); return -2;
-        }
-        if (count > 0) { fwrite(out, 1, (size_t)count, stdout); fflush(stdout); }
-    }
+    return byte_decoder_stream(baudot_bank, 1);
 }
 
 /* ---- tone filters (csdr.c:2932-3017, 3271-3301) ---------------------------------------------------------------------------------
@@ -1052,22 +940,17 @@ static int tone_stream(int taps_length, const complexf *taps, const complexf *ma
         if (taps) { n = apply_fir_cc(in, out, block, (complexf *)taps, taps_length); fwrite(out, sizeof(complexf), (size_t)n, stdout); }
         else { n = bfsk_demod_cf(in, out, block, (complexf *)mark, (complexf *)space, taps_length); fwrite(out, sizeof(float), (size_t)n, stdout); }
         end_of_block();
-        memmove(in, in + n, sizeof(complexf) * (size_t)(block - n));
-        fread(in + (block - n), sizeof(complexf), (size_t)n, stdin);
+        refill(in, sizeof(complexf), block, n);
     }
 }
 
 static int cmd_firdes_peak_c(int argc, char **argv)                         /* csdr.c:2932-2972 */
 {
     if (argc <= 3) return complain("need required parameters (rate, length)");
-    float rate;
-    sscanf(argv[2], "%g", &rate);
-    int length;
-    sscanf(argv[3], "%d", &length);
+    float rate; sscanf(argv[2], "%g", &rate);
+    int length; sscanf(argv[3], "%d", &length);
     if (length % 2 == 0) return complain("number of symmetric FIR filter taps should be odd");
-    window_t window = WINDOW_DEFAULT;
-    if (argc >= 5) window = firdes_get_window_from_string(argv[4]);
-    else { who(); fprintf(stderr, "window = %s\n", firdes_get_string_from_window(window)); }
+    window_t window = window_arg(argc, argv, 4);
     if (argc >= 6 && !strcmp(argv[5], "--octave")) return complain("--octave is not offered here (it plots the filter with GNU Octave)");
     if (length <= 0) return 0;                                              /* the reference's loops print nothing */
     complexf *taps = must_alloc(sizeof(complexf) * (size_t)length);
@@ -1079,8 +962,7 @@ static int cmd_firdes_peak_c(int argc, char **argv)                         /* c
 static int cmd_peaks_fir_cc(int argc, char **argv)                          /* csdr.c:2975-3017 */
 {
     if (argc <= 2) return complain("need required parameter (taps_length)");
-    int taps_length;
-    sscanf(argv[2], "%d", &taps_length);
+    int taps_length; sscanf(argv[2], "%d", &taps_length);
     const int num_peaks = argc - 3;
     float *peak_rate = must_alloc(sizeof(float) * (size_t)(num_peaks > 0 ? num_peaks : 1));
     for (int i = 0; i < num_peaks; i++) sscanf(argv[3 + i], "%f", peak_rate + i);
@@ -1097,14 +979,11 @@ static int cmd_peaks_fir_cc(int argc, char **argv)                          /* c
 
 static int cmd_bfsk_demod_cf(int argc, char **argv)                         /* csdr.c:3271-3301 */
 {
-    float frequency_shift = 0;
     if (argc <= 2) return complain("required parameter <frequency_shift> is missing.");
-    sscanf(argv[2], "%f", &frequency_shift);
-    int filter_length = 0;
+    float frequency_shift = 0; sscanf(argv[2], "%f", &frequency_shift);
     if (argc <= 3) return complain("required parameter <filter_length> is missing.");
-    sscanf(argv[3], "%d", &filter_length);
-    if (!open_block()) return -2;
-    if (!announce_block(1)) return -2;                                      /* the reference announces initialize_buffers()'s 1 */
+    int filter_length = 0; sscanf(argv[3], "%d", &filter_length);
+    if (!announce_block(open_block())) return -2;                           /* sendbufsize(initialize_buffers()) (:3286) */
     /* the reference designs NaN taps at length 1 (middle = 0) and computes a negative output count from a filter longer than the buffer */
     if (filter_length < 2 || filter_length > 4096 || filter_length >= block)
         return complain("filter_length must be between 2 and 4096 and below the buffer size");

@@ -43,6 +43,7 @@ test_wfm_graph_of_csdr_fm = g.test_wfm_graph_of_csdr_fm
 test_fft_commands = g.test_fft_commands
 test_spectrum_and_unroll_commands = g.test_spectrum_and_unroll_commands
 test_dynamic_bufsize_preamble = g.test_dynamic_bufsize_preamble
+test_every_command_frames_like_the_reference = g.test_every_command_frames_like_the_reference
 test_reference_binary_runs_on_our_library = g.test_reference_binary_runs_on_our_library
 
 import test_gpu_zz_shift_math as zz  # noqa: E402

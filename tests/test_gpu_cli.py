@@ -3,6 +3,7 @@ libcsdr_b200.so) against the UNMODIFIED reference CLI (oracle/_ref/csdr_ref, bui
 pipe graphs, plus the LD_PRELOAD drop-in: the reference's own binary running on top of our library."""
 import os
 import subprocess
+import tempfile
 from pathlib import Path
 
 import numpy as np
@@ -199,6 +200,108 @@ def test_dynamic_bufsize_preamble(clis):
     a = run_graph(ours, stages, head + z.tobytes(), env); b = run_graph(ref, stages, head + z.tobytes(), env)
     assert a[:8] == b[:8] and len(a) == len(b)                       # the next-stage preamble is forwarded identically
     assert rel(np.frombuffer(a[8:], np.float32), np.frombuffer(b[8:], np.float32)) < 1e-5
+
+
+# Every command of `csdr --help` but firdes_peak_c (it reads no stdin): (bytes per input element, input kind, representative argument lists).
+# The resamplers' pass-through rates are left out: the reference's copy loop never ends at the end of its input.
+FRAMING_CASES = {
+    "convert_u8_f": (1, "u8", [""]),
+    "convert_s16_f": (2, "s16", [""]),
+    "convert_i16_f": (2, "s16", [""]),
+    "convert_f_s16": (4, "f", [""]),
+    "convert_f_i16": (4, "f", [""]),
+    "shift_addition_cc": (8, "f", ["0.1"]),
+    "shift_addition_fc": (4, "f", ["0.1"]),
+    "fir_decimate_cc": (8, "f", ["10 0.05 HAMMING"]),
+    "fmdemod_quadri_cf": (8, "f", [""]),
+    "fractional_decimator_ff": (4, "f", ["1.25"]),
+    "rational_resampler_ff": (4, "f", ["3 4"]),
+    "fastagc_ff": (4, "f", [""]),
+    "limit_ff": (4, "f", [""]),
+    "amdemod_cf": (8, "f", [""]),
+    "realpart_cf": (8, "f", [""]),
+    "fastdcblock_ff": (4, "f", [""]),
+    "agc_ff": (4, "f", [""]),
+    "fft_exchange_sides_ff": (4, "f", ["1024"]),
+    "compress_fft_adpcm_f_u8": (4, "f", ["1024"]),
+    "encode_ima_adpcm_i16_u8": (2, "s16", [""]),
+    "encode_ima_adpcm_s16_u8": (2, "s16", [""]),
+    "shift_unroll_cc": (8, "f", ["0.1"]),
+    "shift_math_cc": (8, "f", ["0.1"]),
+    "shift_table_cc": (8, "f", ["0.1"]),
+    "shift_addfast_cc": (8, "f", ["0.1"]),
+    "decimating_shift_addition_cc": (8, "f", ["0.1 4"]),
+    "fft_cc": (8, "f", ["1024 3000", "512 500 HAMMING"]),
+    "fft_fc": (4, "f", ["512 3000", "512 500 HAMMING"]),
+    "logpower_cf": (8, "f", ["-70"]),
+    "logaveragepower_cf": (8, "f", ["-70 1024 4"]),
+    "deemphasis_wfm_ff": (4, "f", ["48000 50e-6"]),
+    "deemphasis_nfm_ff": (4, "f", ["48000"]),
+    "bandpass_fir_fft_cc": (8, "f", ["-0.1 0.1 0.05"]),
+    "fastddc_fwd_cc": (8, "f", ["8"]),
+    "fastddc_inv_cc": (8, "f", ["0.1 8"]),
+    "simple_agc_cc": (8, "f", ["0.001"]),
+    "timing_recovery_cc": (8, "f", ["GARDNER 16"]),
+    "dbpsk_decoder_c_u8": (8, "f", [""]),
+    "psk31_varicode_decoder_u8_u8": (1, "bits", [""]),
+    "serial_line_decoder_f_u8": (4, "f", ["10"]),
+    "rtty_baudot2ascii_u8_u8": (1, "ita2", [""]),
+    "peaks_fir_cc": (8, "f", ["101 0.1 -0.1"]),
+    "bfsk_demod_cf": (8, "f", ["0.2 31"]),
+}
+# around the EOF edges of both block sizes (1024 and 16384 elements), and several blocks plus a partial one
+FRAMING_LENGTHS = (0, 1, 1024, 1025, 16384, 16385, 40000)
+
+
+def framing_input(kind, nbytes, seed):
+    rng = np.random.default_rng(seed)
+    if kind == "f":
+        return rng.uniform(-1, 1, nbytes // 4).astype(np.float32).tobytes()
+    if kind == "s16":
+        return rng.integers(-32768, 32768, nbytes // 2).astype(np.int16).tobytes()
+    return rng.integers(0, {"u8": 256, "bits": 2, "ita2": 32}[kind], nbytes).astype(np.uint8).tobytes()
+
+
+def command_names(cli):
+    """the command names `csdr --help` lists"""
+    r = subprocess.run([cli, "--help"], stdout=subprocess.PIPE, stderr=subprocess.PIPE, timeout=60)
+    return [line.split()[1] for line in r.stderr.decode().splitlines() if line.startswith("    csdr ")]
+
+
+def framing_runs(cli):
+    """(case, exit code, output length, first 8 output bytes) for every command, argument list and input length, in fixed-size buffer mode
+    and in dynamic mode behind a 4096-element preamble"""
+    from concurrent.futures import ThreadPoolExecutor
+    jobs = []
+    for name, (size, kind, arg_lists) in FRAMING_CASES.items():
+        for args in arg_lists:
+            for n in FRAMING_LENGTHS:
+                data = framing_input(kind, n * size, n)
+                jobs.append(((name, args, n, "fixed"), {}, data))
+                jobs.append(((name, args, n, "dynamic"), {"CSDR_DYNAMIC_BUFSIZE_ON": "1"}, b"csdr" + np.array([4096], np.int32).tobytes() + data))
+
+    def run(job):                                                    # files, not pipes: the CLI shrinks its pipes to one page for small blocks
+        case, env, data = job
+        e = dict(os.environ); e.update(env)
+        with tempfile.TemporaryFile() as fin, tempfile.TemporaryFile() as fout:
+            fin.write(data); fin.seek(0)
+            r = subprocess.run([cli, case[0]] + case[1].split(), stdin=fin, stdout=fout, stderr=subprocess.DEVNULL, env=e, timeout=300)
+            fout.seek(0); out = fout.read()
+        return case, r.returncode, len(out), out[:8]
+
+    with ThreadPoolExecutor(max_workers=min(8, os.cpu_count() or 1)) as ex:
+        return list(ex.map(run, jobs))
+
+
+def test_every_command_frames_like_the_reference(clis):
+    """Block framing of every command against the reference CLI: exit code and output length at input lengths around the EOF edges, and in
+    dynamic buffer-size mode the preamble announced to the next process too."""
+    ours, ref = clis
+    missing = set(command_names(ours)) - set(FRAMING_CASES) - {"firdes_peak_c"}
+    assert not missing, f"commands without a framing case: {sorted(missing)}"
+    bad = [(a, b[1:]) for a, b in zip(framing_runs(ours), framing_runs(ref))
+           if a[1:3] != b[1:3] or (a[0][3] == "dynamic" and a[3] != b[3])]
+    assert not bad, f"{len(bad)} runs frame differently from the reference, e.g. {bad[:8]}"
 
 
 def test_reference_binary_runs_on_our_library(clis):
