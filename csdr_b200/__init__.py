@@ -277,6 +277,8 @@ def lib() -> C.CDLL:
     L.firdes_add_peak_c.argtypes = [vp, it, C.c_float, it, it, it]
     L.csdrb_apply_fir_bank_cc.argtypes = [vp, lg, vp, lg, it, it, vp, it, vp]
     L.csdrb_bfsk_demod_bank_cf.argtypes = [vp, lg, vp, lg, it, it, vp, vp, it, vp]
+    L.csdrb_fir_interpolate_bank_cc.argtypes = [vp, lg, vp, lg, it, it, it, vp, it, vp]
+    L.csdrb_fmmod_bank_fc.argtypes = [vp, lg, vp, lg, it, it, vp, vp]
     L.csdrb_spectrum_bank_lines.argtypes = [C.POINTER(SpectrumParams), C.POINTER(SpectrumState), lg]; L.csdrb_spectrum_bank_lines.restype = lg
     L.csdrb_spectrum_bank_scratch_bytes.argtypes = [it, lg, C.POINTER(SpectrumParams)]; L.csdrb_spectrum_bank_scratch_bytes.restype = sz
     L.csdrb_spectrum_bank_cf.argtypes = [vp, lg, it, lg, vp, C.POINTER(SpectrumParams), vp, vp, C.POINTER(SpectrumState), vp, lg, vp, sz, vp]
@@ -1197,6 +1199,40 @@ def apply_fir_bank_cc(x, taps):
     m = _check(lib().csdrb_apply_fir_bank_cc(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, t.data_ptr(), t.numel(), _stream()),
                "apply_fir_bank_cc")
     return out[:, :m]
+
+
+def fir_interpolate_bank(x, interpolation: int, taps):
+    """fir_interpolate_cc per row (libcsdr.c:579-602): x [C, N] complex64 CUDA, taps [T] float32 (numpy or CUDA, shared by all rows) ->
+    [C, I * (N - ceil((T-1)/I))] complex64, one reference call per row (tap 0 unused, as there).  A stream keeps the inputs a call did not
+    consume, N minus the outputs / I, in front of its next call."""
+    import torch
+    ch, n = _tone_rows(x)
+    t = torch.as_tensor(np.asarray(taps, np.float32) if not torch.is_tensor(taps) else taps, device=x.device)
+    assert not t.is_complex(), "fir_interpolate_bank: real taps"
+    t = t.to(torch.float32).contiguous()
+    groups = max(n - (t.numel() - 1 + interpolation - 1) // interpolation, 0)
+    out = torch.empty((ch, max(groups * interpolation, 1)), dtype=torch.complex64, device=x.device)
+    if ch == 0 or groups == 0:
+        return out[:, :0]
+    m = _check(lib().csdrb_fir_interpolate_bank_cc(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, interpolation, t.data_ptr(),
+                                                   t.numel(), _stream()), "fir_interpolate_bank")
+    return out[:, :m]
+
+
+def fmmod_bank(x, phase=None):
+    """fmmod_fc per row (libcsdr.c:1180-1192): x [C, N] float32 CUDA -> [C, N] complex64 (cos, sin) of the phase advanced by x*PI per sample.
+    phase: a [C] float32 CUDA tensor carried between calls (zeros at stream start), updated in place; None starts from 0."""
+    import torch
+    assert x.dtype == torch.float32 and x.is_cuda and x.dim() == 2 and x.stride(1) == 1
+    ch, n = x.shape
+    if phase is None:
+        phase = torch.zeros(ch, dtype=torch.float32, device=x.device)
+    assert phase.dtype == torch.float32 and phase.is_cuda and phase.numel() == ch and phase.is_contiguous()
+    out = torch.empty((ch, max(n, 1)), dtype=torch.complex64, device=x.device)
+    if ch == 0 or n == 0:
+        return out[:, :0]
+    _check(lib().csdrb_fmmod_bank_fc(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, phase.data_ptr(), _stream()), "fmmod_bank")
+    return out[:, :n]
 
 
 def bfsk_demod_bank_cf(x, spacing: float, filter_length: int):

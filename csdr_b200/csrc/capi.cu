@@ -503,6 +503,31 @@ int csdrb_bfsk_demod_bank_cf(const complexf* d_in, long in_stride, float* d_out,
     return rc < 0 ? rc : counted(rc, channels > 0 ? 1 : 0);
 }
 
+// transmit banks (interpolate.cu; libcsdr.c:579-602, 1180-1192)
+int csdrb_fir_interpolate_bank_cc(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int n, int interpolation,
+                                  const float* d_taps, int taps_length, void* stream)
+{
+    if (too_many_channels(channels, "fir_interpolate bank")) return -1;
+    if (!d_in || !d_out || !d_taps || misaligned(d_in, 8) || misaligned(d_out, 8) || misaligned(d_taps, 4)) {
+        set_error("fir_interpolate bank: null or misaligned pointer (complexf needs 8-byte, float 4-byte alignment)");
+        return -1;
+    }
+    int rc = launch_fir_interpolate_bank_cc(reinterpret_cast<const float2*>(d_in), in_stride, reinterpret_cast<float2*>(d_out), out_stride, channels, n,
+                                            interpolation, d_taps, taps_length, S(stream));
+    return rc < 0 ? rc : counted(rc, channels > 0 && rc > 0 ? 1 : 0);
+}
+
+int csdrb_fmmod_bank_fc(const float* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int n, float* d_phase_io, void* stream)
+{
+    if (too_many_channels(channels, "fmmod bank")) return -1;
+    if (!d_in || !d_out || !d_phase_io || misaligned(d_in, 4) || misaligned(d_out, 8) || misaligned(d_phase_io, 4)) {
+        set_error("fmmod bank: null or misaligned pointer (complexf needs 8-byte, float 4-byte alignment)");
+        return -1;
+    }
+    int rc = launch_fmmod_bank_fc(d_in, in_stride, reinterpret_cast<float2*>(d_out), out_stride, channels, n, d_phase_io, S(stream));
+    return rc < 0 ? rc : counted(rc, channels > 0 && n > 0 ? 1 : 0);
+}
+
 int csdrb_fft_c2c_batch(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int size, int batch, int inverse, void* stream)
 {
     if (!d_in || !d_out) { set_error("fft: null pointer"); return -1; }

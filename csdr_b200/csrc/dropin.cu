@@ -688,6 +688,35 @@ int apply_fir_cc(complexf* input, complexf* output, int input_size, complexf* ta
     return n_out;
 }
 
+int fir_interpolate_cc(complexf* input, complexf* output, int input_size, int interpolation, float* taps, int taps_length)
+{
+    if (input_size <= 0) return 0;
+    Staging st("fir_interpolate_cc");
+    const complexf* d_in = st.up(input, input_size);
+    const float* d_taps = st.up(taps, taps_length);
+    const long groups = (long)input_size - ((long)taps_length - 1 + interpolation - 1) / (interpolation > 0 ? interpolation : 1);
+    complexf* d_out = st.alloc<complexf>(groups > 0 ? groups * interpolation : 0);
+    const int n_out = st.check(csdrb_fir_interpolate_bank_cc(d_in, input_size, d_out, groups > 0 ? groups * interpolation : 0, 1, input_size,
+                                                             interpolation, d_taps, taps_length, st.stream()));
+    st.get(output, d_out, n_out);
+    st.sync();
+    return n_out;
+}
+
+float fmmod_fc(float* input, complexf* output, int input_size, float last_phase)
+{
+    if (input_size <= 0) return last_phase;
+    Staging st("fmmod_fc");
+    const float* d_in = st.up(input, input_size);
+    float* d_phase = st.up(&last_phase, 1);
+    complexf* d_out = st.alloc<complexf>(input_size);
+    st.check(csdrb_fmmod_bank_fc(d_in, input_size, d_out, input_size, 1, input_size, d_phase, st.stream()));
+    st.get(output, d_out, input_size);
+    st.get(&last_phase, d_phase, 1);
+    st.sync();
+    return last_phase;
+}
+
 int bfsk_demod_cf(complexf* input, float* output, int input_size, complexf* mark_filter, complexf* space_filter, int taps_length)
 {
     if (input_size < taps_length) return input_size - taps_length + 1;     // the reference returns the count it would have written

@@ -172,6 +172,11 @@ int launch_spectrum_bank_f(const float* d_in, long in_stride, int rows, long n, 
                            float* d_acc_io, void* h_state_io, void* d_out, long out_stride_bytes, void* d_scratch, size_t scratch_bytes, int* launches,
                            cudaStream_t st);   // the real-input bank: d_window 2N floats, d_hist_io [rows][2N] floats
 
+// transmit banks, interpolate.cu: fir_interpolate_cc rows (returns the outputs per row) and fmmod_fc rows (returns n); -1 for bad arguments
+int launch_fir_interpolate_bank_cc(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n, int interpolation,
+                                   const float* d_taps, int taps_length, cudaStream_t st);
+int launch_fmmod_bank_fc(const float* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n, float* d_phase_io, cudaStream_t st);
+
 // fused shared-input DDC bank, ddc_bank.cu
 int ddc_bank_geometry(int decimation, int taps_length);               // 0 when the bank serves (decimation, taps_length); else -2 with the error set
 size_t ddc_bank_scratch_bytes(int channels, int input_size, int chunk, int offset);

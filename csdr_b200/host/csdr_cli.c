@@ -993,6 +993,45 @@ static int cmd_bfsk_demod_cf(int argc, char **argv)                         /* c
     return tone_stream(filter_length, NULL, mark, space);
 }
 
+/* csdr.c:1179-1229: the big buffer (grown while below twice the taps), no read before the first call -- it interpolates the zero-filled buffer --
+ * then one call per block, its output written, the consumed inputs (output / I) replaced behind the kept tail.  The next process is told the
+ * block times I. */
+static int cmd_fir_interpolate_cc(int argc, char **argv)
+{
+    G.wideband = 1;
+    if (argc <= 2) return complain("need required parameter (interpolation factor)");
+    int factor = 0; sscanf(argv[2], "%d", &factor);
+    if (factor < 1) return complain("the interpolation factor must be at least 1");
+    float transition_bw = 0.05f; if (argc >= 4) sscanf(argv[3], "%g", &transition_bw);
+    if (!(transition_bw >= 0 && transition_bw < 1.f)) return complain("transition_bw must be in [0, 1)");
+    window_t window = window_arg(argc, argv, 4);
+    int taps_length = firdes_filter_len(transition_bw);
+    who(); fprintf(stderr, "taps_length = %d\n", taps_length);
+    while (G.fixed_big < taps_length * 2) G.fixed_big *= 2;
+    if (!open_block()) return -2;
+    announce_block(block * factor);
+    float *taps = must_alloc(sizeof(float) * (size_t)taps_length);
+    firdes_lowpass_f(taps, taps_length, 0.5f / (float)factor, window);
+    complexf *in = must_alloc(sizeof(complexf) * (size_t)block), *out = must_alloc(sizeof(complexf) * (size_t)block * (size_t)factor);
+    for (;;) {
+        if (feof(stdin)) return 0;
+        int produced = fir_interpolate_cc(in, out, block, factor, taps, taps_length);
+        fwrite(out, sizeof(complexf), (size_t)produced, stdout);
+        end_of_block();
+        refill(in, sizeof(complexf), block, produced / factor);
+    }
+}
+
+static void fmmod_step(void *in, void *out, void *phase) { *(float *)phase = fmmod_fc(in, out, block, *(float *)phase); }
+
+static int cmd_fmmod_fc(int argc, char **argv)                               /* csdr.c:2142-2154 */
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    float phase = 0.f;
+    return map_blocks(sizeof(float), sizeof(complexf), block, 0, fmmod_step, &phase);
+}
+
 /* ---- dispatch ------------------------------------------------------------------------------------ */
 static const struct { const char *name; int (*run)(int, char **); const char *syntax; } kCommands[] = {
     {"convert_u8_f", cmd_convert_u8_f, "convert_u8_f"},
@@ -1039,6 +1078,8 @@ static const struct { const char *name; int (*run)(int, char **); const char *sy
     {"peaks_fir_cc", cmd_peaks_fir_cc, "peaks_fir_cc <taps_length> <peak_rate> [peak_rate ...]"},
     {"bfsk_demod_cf", cmd_bfsk_demod_cf, "bfsk_demod_cf <spacing> <filter_length>"},
     {"fastddc_inv_cc", cmd_fastddc_inv_cc, "fastddc_inv_cc <shift_rate> <decimation> [transition_bw [window]] | --fifo <fifo_path> ... | --fd <fd> ..."},
+    {"fir_interpolate_cc", cmd_fir_interpolate_cc, "fir_interpolate_cc <interpolation_factor> [transition_bw [window]]"},
+    {"fmmod_fc", cmd_fmmod_fc, "fmmod_fc"},
 };
 
 static int usage(void)

@@ -138,6 +138,13 @@ void firdes_add_peak_c(complexf *output, int length, float rate, window_t window
 int  apply_fir_cc(complexf *input, complexf *output, int input_size, complexf *taps, int taps_length);
 int  bfsk_demod_cf(complexf *input, float *output, int input_size, complexf *mark_filter, complexf *space_filter, int taps_length);
 
+/* transmit side (libcsdr.c:579-602, 1180-1192).  fir_interpolate_cc sums each output in the source's tap order, every product and sum rounded
+ * (within a float64 per-output bound of the reference build) and returns the reference's count, I outputs per group; tap 0 is never used, as in
+ * the reference.  fmmod_fc follows the reference build's phase chain bit for bit and returns the last phase; its samples are within one float
+ * ulp of the build's sincosf (DESIGN.md section 7). */
+int   fir_interpolate_cc(complexf *input, complexf *output, int input_size, int interpolation, float *taps, int taps_length);
+float fmmod_fc(float *input, complexf *output, int input_size, float last_phase);
+
 /* audio tail of the WFM graph, SURVEY 8(f) rank 1 (libcsdr.h:100-105; libcsdr.c:1081-1097, 1130-1137) */
 float deemphasis_wfm_ff(float *input, float *output, int input_size, float tau, int sample_rate, float last_output);
 void  limit_ff(float *input, float *output, int input_size, float max_amplitude);
@@ -574,6 +581,18 @@ int csdrb_apply_fir_bank_cc(const complexf *d_in, long in_stride, complexf *d_ou
                             int taps_length, void *stream);
 int csdrb_bfsk_demod_bank_cf(const complexf *d_in, long in_stride, float *d_out, long out_stride, int channels, int n, const complexf *d_mark,
                              const complexf *d_space, int taps_length, void *stream);
+
+/* transmit banks (interpolate.cu), one row per channel.
+ *   fir_interpolate_bank_cc: row c is one fir_interpolate_cc call on the n complexf at d_in + c*in_stride with the shared device taps
+ *     (interpolation I, taps_length T): output i*I + ip = sum over si of x[i+si]*taps[(I-ip) + si*I] for (I-ip) + si*I < T, I and Q summed
+ *     separately in tap order without FMA.  Returns the outputs per row, I*(n - ceil((T-1)/I)) or 0, the reference's count; the caller keeps the
+ *     inputs not consumed (n minus the returned count / I) for the next call.  -1 for I < 1, T < 1, a null or misaligned pointer (complexf
+ *     8 bytes, taps 4), in_stride < n or out_stride below the row's outputs.
+ *   fmmod_bank_fc: row c is fmmod_fc on n floats with the phase d_phase_io[c] carried between calls (0 at stream start); complexf out.
+ *     Returns n; -1 for a null or misaligned pointer or strides below n. */
+int csdrb_fir_interpolate_bank_cc(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int n, int interpolation,
+                                  const float *d_taps, int taps_length, void *stream);
+int csdrb_fmmod_bank_fc(const float *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int n, float *d_phase_io, void *stream);
 
 /* K7 batched unnormalised c2c DFT (power-of-two size 2..16384), sign -1 forward / +1 inverse */
 int csdrb_fft_c2c_batch(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int size, int batch, int inverse, void *stream);

@@ -43,3 +43,8 @@ sp7, _ = cb.fastddc_fwd_cc(cplx(7 * d.input_size), d)
 plan.run(sp7); plan.set_shift(2, 0.123); plan.run(sp7); plan.state(); plan.run(sp7); plan.close()
 cb.shift_addition_bank_cc(cplx(2, 600 * 64 + 13), [0.31, -0.07], chunk=64); cb.shift_addition_bank_cc(cplx(1100 * 1024 + 1), [0.2], chunk=1024)
 torch.cuda.synchronize(); print("sanitize_smoke: all kernels ran")
+# transmit banks: fir_interpolate (staged taps and taps past the shared-memory tile, ragged rows, odd strides), fmmod with several wraps per sample
+for I, T, n in ((1, 7, 999), (3, 81, 1001), (50, 401, 333), (256, 2049, 37), (5, 9001, 2000)):
+    cb.fir_interpolate_bank(cplx(3, n + 1)[:, :n], I, cb.firdes_lowpass_f(T, 0.5 / I))
+ph = torch.zeros(5, device=dev); cb.fmmod_bank((torch.rand((5, 1037), device=dev) * 2 - 1) * 9, ph); cb.fmmod_bank(torch.rand((5, 31), device=dev), ph)
+torch.cuda.synchronize()
