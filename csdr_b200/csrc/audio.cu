@@ -595,8 +595,10 @@ __device__ __forceinline__ float agc_target(const float* pk, const FastAgcState&
     return g;
 }
 
+// S16 = true: the output leaves as convert_f_s16 of the scaled sample, as in fastagc_fused_kernel<true>
+template <bool S16>
 __global__ void __launch_bounds__(256)
-fastagc_apply_kernel(const float* __restrict__ in, long in_stride, float* __restrict__ out, long out_stride, int block, int nblocks,
+fastagc_apply_kernel(const float* __restrict__ in, long in_stride, void* __restrict__ out_v, long out_stride, int block, int nblocks,
                      float reference, const FastAgcState* __restrict__ state, const float* __restrict__ hist, const float* __restrict__ peaks)
 {
     const int b = blockIdx.x, c = blockIdx.y, tid = threadIdx.x;
@@ -607,11 +609,12 @@ fastagc_apply_kernel(const float* __restrict__ in, long in_stride, float* __rest
     const float* x = in + (long)c * in_stride;
     const float* h1 = hist + (long)c * 2 * block;
     const float* leaving = b >= 2 ? x + (long)(b - 2) * block : (b == 0 ? h1 : h1 + block);
-    float* y = out + (long)c * out_stride + (long)b * block;
+    const long o = (long)c * out_stride + (long)b * block;
     for (int i = tid; i < block; i += blockDim.x) {
         const float r = __fdiv_rn((float)i, (float)block);
         const float gain = (float)((double)last_gain * (1.0 - (double)r) + (double)__fmul_rn(target, r));
-        y[i] = __fmul_rn(leaving[i], gain);
+        const float v = __fmul_rn(leaving[i], gain);
+        if (S16) static_cast<short*>(out_v)[o + i] = (short)f_to_s16_bits(v); else static_cast<float*>(out_v)[o + i] = v;
     }
 }
 
@@ -710,6 +713,36 @@ fastagc_fused_kernel(const float* __restrict__ in, long in_stride, void* __restr
 
 size_t fastagc_scratch_bytes(int channels, int nblocks) { return (size_t)channels * (size_t)(nblocks > 0 ? nblocks : 1) * sizeof(float); }
 
+// blocks of up to 1024 samples: the fused kernel and the carry (2 launches); longer blocks: peaks, apply and the carry (3 launches).
+// S16 = true: the output is convert_f_s16 of fastagc_ff's, short [channels][out_stride].
+template <bool S16>
+static int launch_fastagc(const float* d_in, long in_stride, void* d_out, long out_stride, int channels, int block, int nblocks,
+                          float reference, void* d_state, float* d_hist, void* d_scratch, size_t scratch_bytes, cudaStream_t st)
+{
+    if (channels <= 0 || nblocks <= 0) return 0;
+    if (block <= 0) { set_error("fastagc: block size must be positive"); return -1; }
+    if (!S16 && d_out == d_in) { set_error("fastagc: in-place operation is not supported (output lags input by two blocks)"); return -1; }
+    if (!d_scratch || scratch_bytes < fastagc_scratch_bytes(channels, nblocks)) { set_error("fastagc: scratch too small"); return -1; }
+    float* peaks = static_cast<float*>(d_scratch);
+    int launches = 2;
+    if (block <= 256 * AGC_PER) {
+        fastagc_fused_kernel<S16><<<dim3((nblocks + AGC_RUN - 1) / AGC_RUN, channels), 256, 0, st>>>(d_in, in_stride, d_out, out_stride, block, nblocks, reference,
+                                                                                                   static_cast<const FastAgcState*>(d_state), d_hist, peaks);
+        CSDRB_CUDA(cudaGetLastError());
+    } else {
+        const dim3 grid(nblocks, channels);
+        fastagc_peaks_kernel<<<grid, 256, 0, st>>>(d_in, in_stride, block, nblocks, peaks);
+        CSDRB_CUDA(cudaGetLastError());
+        fastagc_apply_kernel<S16><<<grid, 256, 0, st>>>(d_in, in_stride, d_out, out_stride, block, nblocks, reference, static_cast<const FastAgcState*>(d_state),
+                                                        d_hist, peaks);
+        CSDRB_CUDA(cudaGetLastError());
+        launches = 3;
+    }
+    fastagc_carry_kernel<<<channels, 256, 0, st>>>(d_in, in_stride, block, nblocks, reference, static_cast<FastAgcState*>(d_state), d_hist, peaks);
+    CSDRB_CUDA(cudaGetLastError());
+    return launches;
+}
+
 // fastagc_ff | convert_f_s16 in one pass (blocks of up to 1024 samples); -2: the block size has no fused kernel
 int launch_fastagc_bank_s16(const float* d_in, long in_stride, short* d_out, long out_stride, int channels, int block, int nblocks,
                             float reference, void* d_state, float* d_hist, void* d_scratch, size_t scratch_bytes, cudaStream_t st)
@@ -717,40 +750,20 @@ int launch_fastagc_bank_s16(const float* d_in, long in_stride, short* d_out, lon
     if (channels <= 0 || nblocks <= 0) return 0;
     if (block <= 0) { set_error("fastagc: block size must be positive"); return -1; }
     if (block > 256 * AGC_PER) return -2;
-    if (!d_scratch || scratch_bytes < fastagc_scratch_bytes(channels, nblocks)) { set_error("fastagc: scratch too small"); return -1; }
-    float* peaks = static_cast<float*>(d_scratch);
-    fastagc_fused_kernel<true><<<dim3((nblocks + AGC_RUN - 1) / AGC_RUN, channels), 256, 0, st>>>(d_in, in_stride, d_out, out_stride, block, nblocks, reference,
-                                                                                                 static_cast<const FastAgcState*>(d_state), d_hist, peaks);
-    CSDRB_CUDA(cudaGetLastError());
-    fastagc_carry_kernel<<<channels, 256, 0, st>>>(d_in, in_stride, block, nblocks, reference, static_cast<FastAgcState*>(d_state), d_hist, peaks);
-    CSDRB_CUDA(cudaGetLastError());
-    return 2;
+    return launch_fastagc<true>(d_in, in_stride, d_out, out_stride, channels, block, nblocks, reference, d_state, d_hist, d_scratch, scratch_bytes, st);
+}
+
+// the same for any block size: blocks over 1024 run peaks, apply with the s16 epilogue and carry (any row stride, no temporary)
+int launch_fastagc_bank_s16_any(const float* d_in, long in_stride, short* d_out, long out_stride, int channels, int block, int nblocks,
+                                float reference, void* d_state, float* d_hist, void* d_scratch, size_t scratch_bytes, cudaStream_t st)
+{
+    return launch_fastagc<true>(d_in, in_stride, d_out, out_stride, channels, block, nblocks, reference, d_state, d_hist, d_scratch, scratch_bytes, st);
 }
 
 int launch_fastagc_bank(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int block, int nblocks,
                         float reference, void* d_state, float* d_hist, void* d_scratch, size_t scratch_bytes, cudaStream_t st)
 {
-    if (channels <= 0 || nblocks <= 0) return 0;
-    if (block <= 0) { set_error("fastagc: block size must be positive"); return -1; }
-    if (d_out == d_in) { set_error("fastagc: in-place operation is not supported (output lags input by two blocks)"); return -1; }
-    if (!d_scratch || scratch_bytes < fastagc_scratch_bytes(channels, nblocks)) { set_error("fastagc: scratch too small"); return -1; }
-    float* peaks = static_cast<float*>(d_scratch);
-    if (block <= 256 * AGC_PER) {
-        fastagc_fused_kernel<false><<<dim3((nblocks + AGC_RUN - 1) / AGC_RUN, channels), 256, 0, st>>>(d_in, in_stride, d_out, out_stride, block, nblocks, reference,
-                                                                                               static_cast<const FastAgcState*>(d_state), d_hist, peaks);
-        CSDRB_CUDA(cudaGetLastError());
-        fastagc_carry_kernel<<<channels, 256, 0, st>>>(d_in, in_stride, block, nblocks, reference, static_cast<FastAgcState*>(d_state), d_hist, peaks);
-        CSDRB_CUDA(cudaGetLastError());
-        return 2;
-    }
-    const dim3 grid(nblocks, channels);
-    fastagc_peaks_kernel<<<grid, 256, 0, st>>>(d_in, in_stride, block, nblocks, peaks);
-    CSDRB_CUDA(cudaGetLastError());
-    fastagc_apply_kernel<<<grid, 256, 0, st>>>(d_in, in_stride, d_out, out_stride, block, nblocks, reference, static_cast<const FastAgcState*>(d_state), d_hist, peaks);
-    CSDRB_CUDA(cudaGetLastError());
-    fastagc_carry_kernel<<<channels, 256, 0, st>>>(d_in, in_stride, block, nblocks, reference, static_cast<FastAgcState*>(d_state), d_hist, peaks);
-    CSDRB_CUDA(cudaGetLastError());
-    return 3;
+    return launch_fastagc<false>(d_in, in_stride, d_out, out_stride, channels, block, nblocks, reference, d_state, d_hist, d_scratch, scratch_bytes, st);
 }
 
 }  // namespace csdrb

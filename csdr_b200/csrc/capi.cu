@@ -135,6 +135,7 @@ int csdrb_fmdemod_quadri_bank_cf(const complexf* d_in, long in_stride, float* d_
 {
     if (too_many_channels(channels, "fmdemod_quadri bank")) return -1;
     if (!d_in || !d_out) { set_error("fmdemod_quadri bank: null pointer"); return -1; }
+    if (channels <= 0 || input_size <= 0) return 0;                  // nothing to do: no launch to count
     return counted(launch_fmdemod_quadri_bank(reinterpret_cast<const float2*>(d_in), in_stride, d_out, out_stride, channels, input_size,
                                               reinterpret_cast<const float2*>(d_last_in), reinterpret_cast<float2*>(d_last_out), S(stream)));
 }
@@ -362,20 +363,14 @@ int csdrb_fastagc_bank_ff(const float* d_in, long in_stride, float* d_out, long 
     return rc < 0 ? rc : counted(0, rc);
 }
 
-// fastagc_ff | convert_f_s16 fused (the last two blocks of the NFM graph, README.md:87).  Block sizes without a fused kernel (> 1024) run the two steps.
+// fastagc_ff | convert_f_s16 fused (the last two blocks of the NFM graph, README.md:87), at every block size
 int csdrb_fastagc_bank_f_s16(const float* d_in, long in_stride, short* d_out, long out_stride, int channels, int block, int nblocks, float reference,
                              csdrb_fastagc_state_t* d_state, float* d_hist, void* d_scratch, size_t scratch_bytes, void* stream)
 {
     if (too_many_channels(channels, "fastagc bank")) return -1;
     if (!d_in || !d_out || !d_state || !d_hist) { set_error("fastagc s16 bank: null pointer"); return -1; }
-    int rc = launch_fastagc_bank_s16(d_in, in_stride, d_out, out_stride, channels, block, nblocks, reference, d_state, d_hist, d_scratch, scratch_bytes, S(stream));
-    if (rc != -2) return rc < 0 ? rc : counted(0, rc);
-    float* tmp = nullptr;                                              // unusual block size: AGC into a stream-ordered temporary, then the conversion row by row
-    const long n = (long)block * nblocks;
-    CSDRB_CUDA(cudaMallocAsync(reinterpret_cast<void**>(&tmp), sizeof(float) * (size_t)n * channels, S(stream)));
-    rc = launch_fastagc_bank(d_in, in_stride, tmp, n, channels, block, nblocks, reference, d_state, d_hist, d_scratch, scratch_bytes, S(stream));
-    for (int c = 0; c < channels && rc >= 0; c++) { const int r2 = launch_convert_f_s16(tmp + (long)c * n, d_out + (long)c * out_stride, n, S(stream)); rc = r2 < 0 ? r2 : rc + 1; }
-    CSDRB_CUDA(cudaFreeAsync(tmp, S(stream)));
+    int rc = launch_fastagc_bank_s16_any(d_in, in_stride, d_out, out_stride, channels, block, nblocks, reference, d_state, d_hist, d_scratch, scratch_bytes,
+                                         S(stream));
     return rc < 0 ? rc : counted(0, rc);
 }
 

@@ -75,6 +75,8 @@ int launch_fractional_decimator_bank(const float* d_in, long in_stride, float* d
 size_t fastagc_scratch_bytes(int channels, int nblocks);
 int launch_fastagc_bank_s16(const float* d_in, long in_stride, short* d_out, long out_stride, int channels, int block, int nblocks,
                             float reference, void* d_state, float* d_hist, void* d_scratch, size_t scratch_bytes, cudaStream_t st);
+int launch_fastagc_bank_s16_any(const float* d_in, long in_stride, short* d_out, long out_stride, int channels, int block, int nblocks,
+                                float reference, void* d_state, float* d_hist, void* d_scratch, size_t scratch_bytes, cudaStream_t st);
 int launch_fastagc_bank(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int block, int nblocks,
                         float reference, void* d_state, float* d_hist, void* d_scratch, size_t scratch_bytes, cudaStream_t st);
 

@@ -184,15 +184,19 @@ class Oracle:
         return y, complex(r.i, r.q)
 
     # ---- fractional decimator (streamed block by block like csdr.c:1510-1522 when block is given)
-    def fractional_decimator_ff(self, x, rate, num_poly_points=12, taps=None, block=None):
+    def fractional_decimator_ff(self, x, rate, num_poly_points=12, taps=None, block=None, where=None, states=None):
+        """``where`` replaces the initial position (a state carried from an earlier call); ``states``, a list, receives
+        (where, input_processed, output_size) after every call."""
         x = np.ascontiguousarray(x, np.float32)
         tp = np.ascontiguousarray(taps, np.float32) if taps is not None else None
         d = self._FracDec()
         self.L.oracle_fractional_decimator_ff_init(C.byref(d), rate, num_poly_points,
                                                    _p(tp, C.c_float) if tp is not None else None,
                                                    tp.size if tp is not None else 0)
+        if where is not None:
+            d.where = where
         return _stream_fracdec(lambda buf, out, n: self.L.oracle_fractional_decimator_ff(_p(buf, C.c_float), _p(out, C.c_float), n, C.byref(d)),
-                               d, x, block)
+                               d, x, block, states)
 
     # ---- fastagc (streamed)
     def fastagc_ff(self, x, block=1024, reference=1.0):
@@ -353,12 +357,15 @@ def next_pow2(x: int) -> int:
     return -1
 
 
-def _stream_fracdec(call, d, x, block):
+def _stream_fracdec(call, d, x, block, states=None):
     """Drive a fractional decimator over ``x``.  block=None: one call on the whole array.
-    Otherwise reproduce the CLI's re-feeding of the unconsumed tail (csdr.c:1510-1522), complete reads only."""
+    Otherwise reproduce the CLI's re-feeding of the unconsumed tail (csdr.c:1510-1522), complete reads only.
+    ``states``, when given, receives (where, input_processed, output_size) after every call."""
+    log = (lambda: states.append((float(d.where), int(d.input_processed), int(d.output_size)))) if states is not None else (lambda: None)
     if block is None:
         out = np.empty(int(x.size / max(d.rate, 1.0)) + 16, np.float32)
         call(x, out, x.size)
+        log()
         return out[:d.output_size].copy()
     buf = np.zeros(block, np.float32); outs = []; pos = 0
     out = np.empty(block, np.float32)
@@ -374,6 +381,7 @@ def _stream_fracdec(call, d, x, block):
         if d.input_processed == 0:
             d.input_processed = block
         call(buf, out, block)
+        log()
         outs.append(out[:d.output_size].copy())
     return np.concatenate(outs) if outs else np.zeros(0, np.float32)
 
