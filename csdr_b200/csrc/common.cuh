@@ -193,9 +193,15 @@ __device__ __forceinline__ float wrap_binade_step(float a)
     return a;
 }
 
+// The wrapped phase from the wrapped magnitude a = |result|: the sign of x, except that a wrap landing exactly on zero gives +0, as the
+// reference's loop does (fl(-2*pi + 2*pi) = +0); only an input of -0.0, which no loop step touches, stays -0.0.
+__device__ __forceinline__ float wrap_sign(float x, float a)
+{
+    return (__float_as_uint(x) >> 31) && (a != 0.f || x == 0.f) ? -a : a;
+}
+
 __device__ __forceinline__ float wrap_phase_pm_pi(float ph)
 {
-    const bool neg = (__float_as_uint(ph) >> 31) != 0u;   // sign bit, so that -0.0 stays -0.0 like the loop leaves it
     float a = fabsf(ph);
     if (!(a < 67108864.f)) return ph;                // |ph| >= 2^26 (or nan): subtracting 2*pi no longer changes it; the reference would spin
     if (a >= 1048576.f) {                            // 2^20 and up: rare
@@ -212,7 +218,7 @@ __device__ __forceinline__ float wrap_phase_pm_pi(float ph)
         a = wrap_binade_step<6>(a);  a = wrap_binade_step<5>(a);  a = wrap_binade_step<4>(a);
     }
     while (a > kPiF) a = __fsub_rn(a, kTwoPiF);                                            // below 16: at most three plain steps
-    return neg ? -a : a;
+    return wrap_sign(ph, a);
 }
 
 // The reference's phase advance over n samples, starting_phase += rate*PI*n (libcsdr_gpl.c:48, :154): fl(fl(rate*PI)*n) ...

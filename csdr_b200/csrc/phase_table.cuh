@@ -147,7 +147,7 @@ __device__ __forceinline__ float wrap_after_add(float x, const WrapTable* __rest
         a = (float)((double)a - t->K[cnt - 1]);             // exact; the result is the float the loop would hold at this point
     }
     while (a > kPiF) a = __fsub_rn(a, kTwoPiF);
-    return (__float_as_uint(x) >> 31) ? -a : a;
+    return wrap_sign(x, a);
 }
 
 
@@ -187,7 +187,7 @@ static __device__ __noinline__ float wrap_after_add_warp_generic(float x, const 
         a = (float)((double)a - K);                                     // exact; the float the loop would hold when it first drops below 16
     }
     while (a > kPiF) a = __fsub_rn(a, kTwoPiF);
-    return (__float_as_uint(x) >> 31) ? -a : a;
+    return wrap_sign(x, a);
 }
 
 // The chain kernels' step.  A chain is pure latency, and a looped step has seven branches (>= 16? in the window? more than 32 pieces?
@@ -209,7 +209,7 @@ __device__ __forceinline__ float wrap_after_add_warp(float x, const WrapLanes& w
     r = r > kPiF ? __fsub_rn(r, kTwoPiF) : r;
     r = r > kPiF ? __fsub_rn(r, kTwoPiF) : r;
     r = r > kPiF ? __fsub_rn(r, kTwoPiF) : r;
-    return (__float_as_uint(x) >> 31) ? -r : r;
+    return wrap_sign(x, r);
 }
 
 struct NoChainSink { __device__ void operator()(int, float) const {} };

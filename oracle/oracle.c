@@ -521,6 +521,56 @@ float oracle_shift_addfast_cc(const ocf32 *in, ocf32 *out, int n, const float *d
 }
 
 /* ------------------------------------------------------------------------------------------------
+ * test helpers of the NCO shift checks (tests/shift_ref.py): the project's own restatement, not reference functions
+ * ---------------------------------------------------------------------------------------------- */
+
+/* The chunk-to-chunk phase chain of shift_addition_cc, shift_addfast_cc and shift_unroll_cc cut into calls of `chunk` samples (the last
+ * one shorter): every call starts at starts[k] and moves the phase by fl(inc * len), wrapped to [-pi, pi] (inc = fl(fl(2 rate) * PI) for
+ * all three).  Returns the phase after the last call. */
+float oracle_shift_chain(float inc, float phase, int n, int chunk, float *starts)
+{
+    for (int k = 0, s = 0; s < n; k++, s += chunk) {
+        const int len = n - s < chunk ? n - s : chunk;
+        starts[k] = phase;
+        phase = wrap_pm_pi(phase + inc * len);
+    }
+    return phase;
+}
+
+/* The per-sample phase of shift_math_cc and shift_table_cc: phases[k] is the phase sample k is rotated by.  Returns the carried phase. */
+float oracle_shift_math_phases(float rate, float phase, int n, float *phases)
+{
+    rate *= 2;
+    const float inc = rate * kPi;
+    for (int k = 0; k < n; k++) {
+        phases[k] = phase;
+        phase += inc;
+        while (phase > 2 * kPi) phase -= 2 * kPi;
+        while (phase < 0) phase += 2 * kPi;
+    }
+    return phase;
+}
+
+/* (float)cos((double)ph), (float)sin((double)ph) for n phases, as every shift kernel seeds its phasor: cs[2k], cs[2k+1].  alt[] holds the
+ * other float neighbour of a component whose double value lies within `ulps` double ulps of a float rounding midpoint (a libm within a few
+ * ulps of this one may round it either way), and the component itself otherwise; returns how many components are that close. */
+long oracle_seed_phasors(const float *ph, long n, float *cs, float *alt, int ulps)
+{
+    long close = 0;
+    for (long k = 0; k < 2 * n; k++) {
+        const double v = (k & 1) ? sin((double)ph[k >> 1]) : cos((double)ph[k >> 1]);
+        const float f = (float)v;
+        cs[k] = alt[k] = f;
+        if (!isfinite(v) || (double)f == v) continue;
+        const float other = nextafterf(f, (double)f < v ? INFINITY : -INFINITY);
+        const double mid = ((double)f + (double)other) / 2;                   /* exact: two floats' sum has at most 25 significant bits */
+        const double ulp = nextafter(fabs(v), INFINITY) - fabs(v);
+        if (fabs(v - mid) <= ulps * ulp) { alt[k] = other; close++; }
+    }
+    return close;
+}
+
+/* ------------------------------------------------------------------------------------------------
  * waterfall compression (SURVEY 8(f) rank 4): IMA ADPCM, 4 bits per value
  * ---------------------------------------------------------------------------------------------- */
 

@@ -93,6 +93,10 @@ float oracle_shift_table_cc(const ocf32 *in, ocf32 *out, int n, float rate, cons
 /* shift_addfast (SURVEY 8(f) rank 3): libcsdr.h:189-197, libcsdr.c:307-317, 396-433.  d9 = dsin[4], dcos[4], phase_increment */
 void  oracle_shift_addfast_init(float rate, float *d9);
 float oracle_shift_addfast_cc(const ocf32 *in, ocf32 *out, int n, const float *d9, float starting_phase);
+/* test helpers of tests/shift_ref.py: the phase chains and the seed phasors of the shift kernels (see oracle.c) */
+float oracle_shift_chain(float inc, float phase, int n, int chunk, float *starts);
+float oracle_shift_math_phases(float rate, float phase, int n, float *phases);
+long  oracle_seed_phasors(const float *ph, long n, float *cs, float *alt, int ulps);
 
 /* waterfall compression (SURVEY 8(f) rank 4): ima_adpcm.c:95-150, csdr.c:1739-1767 */
 void oracle_encode_ima_adpcm_i16_u8(const short *in, unsigned char *out, int n, int *index, int *previous);

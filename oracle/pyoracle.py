@@ -119,6 +119,9 @@ class Oracle:
         L.oracle_shift_math_cc.argtypes = [C.POINTER(_CF), C.POINTER(_CF), C.c_int, C.c_float, C.c_float]; L.oracle_shift_math_cc.restype = C.c_float
         L.oracle_shift_addfast_init.argtypes = [C.c_float, fp]
         L.oracle_shift_addfast_cc.argtypes = [C.POINTER(_CF), C.POINTER(_CF), C.c_int, fp, C.c_float]; L.oracle_shift_addfast_cc.restype = C.c_float
+        L.oracle_shift_chain.argtypes = [C.c_float, C.c_float, C.c_int, C.c_int, fp]; L.oracle_shift_chain.restype = C.c_float
+        L.oracle_shift_math_phases.argtypes = [C.c_float, C.c_float, C.c_int, fp]; L.oracle_shift_math_phases.restype = C.c_float
+        L.oracle_seed_phasors.argtypes = [fp, C.c_long, fp, fp, C.c_int]; L.oracle_seed_phasors.restype = C.c_long
         L.oracle_dft_c2c.argtypes = [C.POINTER(_CF), C.POINTER(_CF), C.c_int, C.c_int]
         L.oracle_apply_fir_fft_cc.argtypes = [C.POINTER(_CF)] * 3 + [C.c_int, C.POINTER(_CF), C.c_int]
         L.oracle_fastddc_init.argtypes = [C.POINTER(self._Ddc), C.c_float, C.c_int, C.c_float]
@@ -298,6 +301,27 @@ class Oracle:
             n = min(chunk, x.size - s0)
             phase = self.L.oracle_shift_addfast_cc(_p(x[s0:], _CF), _p(y[s0:], _CF), n, _p(d, C.c_float), phase)
         return y, float(np.float32(phase))
+
+    # ---- test helpers of the shift checks (tests/shift_ref.py)
+    def shift_chain(self, inc, phase, n, chunk):
+        """(start phase of every call of `chunk` samples, carried phase) of the shift_addition / addfast / unroll chain"""
+        starts = np.empty(max(-(-n // chunk), 1), np.float32)
+        ph = self.L.oracle_shift_chain(inc, phase, n, chunk, _p(starts, C.c_float))
+        return starts[:-(-n // chunk)], np.float32(ph)
+
+    def shift_math_phases(self, rate, phase, n):
+        """(phase of every sample, carried phase) of shift_math_cc / shift_table_cc"""
+        ph = np.empty(max(n, 1), np.float32)
+        end = self.L.oracle_shift_math_phases(rate, phase, n, _p(ph, C.c_float))
+        return ph[:n], np.float32(end)
+
+    def seed_phasors(self, phases, ulps=4):
+        """(seeds [..., 2] float32 = cos, sin of each phase in double, the other rounding of each component within `ulps` of a midpoint
+        (else the seed itself), how many such components)"""
+        ph = np.ascontiguousarray(phases, np.float32)
+        cs = np.empty(ph.shape + (2,), np.float32); alt = np.empty_like(cs)
+        close = self.L.oracle_seed_phasors(_p(ph, C.c_float), ph.size, _p(cs, C.c_float), _p(alt, C.c_float), ulps)
+        return cs, alt, int(close)
 
     # ---- FFT family
     def dft(self, x, forward=True):

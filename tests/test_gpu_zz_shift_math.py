@@ -10,6 +10,8 @@ import pytest
 
 sys.path.insert(0, str(Path(__file__).resolve().parent))
 from test_gpu_cli import clis, rel, run_graph  # noqa: E402,F401  (the CLI suite's fixture and helpers)
+import shift_ref as S  # noqa: E402
+from bitcmp import assert_bits_equal  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 torch = pytest.importorskip("torch")
@@ -43,10 +45,9 @@ def test_shift_math_bank(gpu, oracle):
         x = (rng.uniform(-1, 1, n) + 1j * rng.uniform(-1, 1, n)).astype(np.complex64)
         out, ph = gpu.shift_math_bank_cc(torch.from_numpy(x).cuda(), rates, phases=torch.from_numpy(ph0).cuda())
         out = out.cpu().numpy(); ph = ph.cpu().numpy()
-        for c, r in enumerate(rates):
-            want, wph = oracle.shift_math_cc(x, float(r), float(ph0[c]))
-            assert np.float32(wph).view(np.uint32) == ph[c].view(np.uint32), (n, c)
-            assert _rel(out[c], want) < 1e-7, (n, c)
+        phases = S.expected_chain(oracle, "math", rates, ph0, n, 0)
+        assert_bits_equal(ph, phases[2], f"n={n}: carried phases")
+        S.check_samples(oracle, "math", np.repeat(x[None], rates.size, axis=0), out, rates, None, rates, ph0, n, 0, phases, None, f"shift_math n={n}")
 
 
 def test_shift_math_command(clis):

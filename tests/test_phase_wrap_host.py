@@ -59,3 +59,15 @@ def test_special_values(wrap):
         a, b = np.float32(wrap.wrap_fast(v)), np.float32(wrap.wrap_loop(v))
         assert a.view(np.uint32) == b.view(np.uint32), (v, a, b)
     assert np.isnan(wrap.wrap_fast(float("nan")))
+
+
+def test_wraps_landing_on_zero(wrap):
+    """a phase the loop wraps exactly onto zero ends at +0 from either side (fl(-2 pi + 2 pi) = +0), as the reference's loop leaves it; only
+    an input of -0.0, which no step touches, stays -0.0"""
+    two_pi = np.float32(2) * np.float32(3.14159265358979323846)
+    x = (two_pi * np.arange(1, 2000, dtype=np.float32)).astype(np.float32)
+    x = np.concatenate([x, -x]).astype(np.float32)
+    zeros = [v for v in x if wrap.wrap_loop(float(v)) == 0]
+    assert any(v < 0 for v in zeros) and any(v > 0 for v in zeros), zeros
+    bad = C.c_float(0)
+    assert wrap.wrap_compare(x.ctypes.data, x.size, C.byref(bad)) == 0, bad.value
