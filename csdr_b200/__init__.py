@@ -279,6 +279,11 @@ def lib() -> C.CDLL:
     L.csdrb_bfsk_demod_bank_cf.argtypes = [vp, lg, vp, lg, it, it, vp, vp, it, vp]
     L.csdrb_fir_interpolate_bank_cc.argtypes = [vp, lg, vp, lg, it, it, it, vp, it, vp]
     L.csdrb_fmmod_bank_fc.argtypes = [vp, lg, vp, lg, it, it, vp, vp]
+    L.csdrb_synth_bank_scratch_bytes.argtypes = [it, it, it, it, it, it]; L.csdrb_synth_bank_scratch_bytes.restype = sz
+    L.csdrb_synth_bank_cc.argtypes = [vp, lg, it, it, it, vp, it, vp, vp, it, it, vp, vp, sz, vp]
+    L.csdrb_synth_bank_create.argtypes = [it, C.POINTER(C.c_float), it, C.POINTER(C.c_float), it, it]; L.csdrb_synth_bank_create.restype = vp
+    L.csdrb_synth_bank_destroy.argtypes = [vp]
+    L.csdrb_synth_bank_process.argtypes = [vp, vp, lg, it, vp, vp]
     L.csdrb_spectrum_bank_lines.argtypes = [C.POINTER(SpectrumParams), C.POINTER(SpectrumState), lg]; L.csdrb_spectrum_bank_lines.restype = lg
     L.csdrb_spectrum_bank_scratch_bytes.argtypes = [it, lg, C.POINTER(SpectrumParams)]; L.csdrb_spectrum_bank_scratch_bytes.restype = sz
     L.csdrb_spectrum_bank_cf.argtypes = [vp, lg, it, lg, vp, C.POINTER(SpectrumParams), vp, vp, C.POINTER(SpectrumState), vp, lg, vp, sz, vp]
@@ -1233,6 +1238,72 @@ def fmmod_bank(x, phase=None):
         return out[:, :0]
     _check(lib().csdrb_fmmod_bank_fc(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, phase.data_ptr(), _stream()), "fmmod_bank")
     return out[:, :n]
+
+
+def _synth_rows(x):
+    import torch
+    assert x.dtype == torch.complex64 and x.is_cuda and x.dim() == 2 and x.stride(1) == 1, "synthesis bank: [C, n] complex64 CUDA rows"
+    return x.shape
+
+
+def _real_taps(taps, what):
+    t = np.asarray(taps)
+    if np.iscomplexobj(t):
+        raise TypeError(f"{what}: real taps")
+    return np.ascontiguousarray(t, np.float32)
+
+
+def synth_bank(x, rates, interpolation: int, taps, phases=None, chunk: int = 1024, offset: int = 0):
+    """Synthesis bank (csdrb_synth_bank_cc): x [C, n] complex64 CUDA baseband rows -> (y [G*I] complex64, phases [C]), y the sum over the
+    channels of shift_addition_cc(fir_interpolate_cc(x_c, I, taps), rate_c) in a fixed pairwise tree over the channel index, G = n - ceil((T-1)/I)
+    (or 0).  shift_addition_cc runs once per `chunk` wideband samples counted on the absolute stream: output 0 lies `offset` samples into a chunk,
+    phases[c] is the phase at the start of that chunk (zeros when None) and the returned one the phase at the start of the chunk holding output G*I."""
+    import torch
+    ch, n = _synth_rows(x)
+    rates = np.atleast_1d(np.asarray(rates, np.float32))
+    assert rates.size == ch, "synth_bank: one rate per row"
+    t = torch.from_numpy(_real_taps(taps.cpu().numpy() if torch.is_tensor(taps) else taps, "synth_bank")).to(x.device)
+    params = torch.from_numpy(np.array([shift_addition_init(float(r)) for r in rates], np.float32)).to(x.device)
+    d_phase = torch.zeros(ch, dtype=torch.float32, device=x.device) if phases is None else phases.to(torch.float32).clone()
+    groups = max(n - (t.numel() - 1 + interpolation - 1) // interpolation, 0) if interpolation >= 1 else 0
+    out = torch.empty(max(groups * interpolation, 1), dtype=torch.complex64, device=x.device)
+    scratch = _scratch(lib().csdrb_synth_bank_scratch_bytes(ch, n, interpolation, t.numel(), chunk, offset), x.device)
+    m = _check(lib().csdrb_synth_bank_cc(x.data_ptr(), x.stride(0), ch, n, interpolation, t.data_ptr(), t.numel(), params.data_ptr(), d_phase.data_ptr(),
+                                         chunk, offset, out.data_ptr(), scratch.data_ptr(), scratch.numel(), _stream()), "synth_bank")
+    return out[:m], d_phase
+
+
+class SynthBank:
+    """Streaming synthesis bank (csdrb_synth_bank_*): the rates, taps, phases and the place inside the current NCO chunk live in the object.
+    process(x) takes [C, n] complex64 CUDA rows and returns the G*I wideband outputs; it consumes G = n - ceil((T-1)/I) inputs per row, and the
+    caller presents the last n - G again at the front of the next block (fir_interpolate_cc's block contract)."""
+
+    def __init__(self, rates, interpolation: int, taps, chunk: int = 1024):
+        self.rates = np.ascontiguousarray(np.atleast_1d(rates), np.float32)
+        self.taps = _real_taps(taps, "SynthBank")
+        self.interpolation, self.channels = interpolation, self.rates.size
+        self.h = lib().csdrb_synth_bank_create(self.channels, _fp(self.rates), interpolation, _fp(self.taps), self.taps.size, chunk)
+        if not self.h:
+            raise CsdrB200Error(f"csdrb_synth_bank_create: {lib().csdrb_last_error().decode()}")
+
+    def process(self, x):
+        import torch
+        ch, n = _synth_rows(x)
+        assert ch == self.channels, "SynthBank.process: one row per channel"
+        groups = max(n - (self.taps.size - 1 + self.interpolation - 1) // self.interpolation, 0)
+        out = torch.empty(max(groups * self.interpolation, 1), dtype=torch.complex64, device=x.device)
+        m = _check(lib().csdrb_synth_bank_process(self.h, x.data_ptr(), x.stride(0), n, out.data_ptr(), _stream()), "synth_bank_process")
+        return out[:m]
+
+    def close(self):
+        if getattr(self, "h", None):
+            lib().csdrb_synth_bank_destroy(self.h); self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def bfsk_demod_bank_cf(x, spacing: float, filter_length: int):

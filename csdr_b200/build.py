@@ -90,6 +90,12 @@ def build(force: bool = False, verbose: bool = False) -> Path:
     if bankd_src.exists() and (force or _stale(bankd, [bankd_src, LIB] + headers)):
         subprocess.run(["gcc", "-std=gnu99", "-O2", "-Wall", f"-I{ROOT / 'include'}", str(bankd_src), "-o", str(bankd),
                         f"-L{PKG}", "-lcsdr_b200", "-lm", "-Wl,-rpath,$ORIGIN"], check=True)
+    # host/programs/: programs on the C ABI that are not in the host/*.c list every library build compiles (each has a main())
+    synth_src = HOST / "programs" / "synth.c"
+    synth = PKG / "csdr-synth"
+    if synth_src.exists() and (force or _stale(synth, [synth_src, LIB] + headers)):
+        subprocess.run(["gcc", "-std=gnu99", "-O2", "-Wall", f"-I{ROOT / 'include'}", str(synth_src), "-o", str(synth),
+                        f"-L{PKG}", "-lcsdr_b200", "-lm", "-Wl,-rpath,$ORIGIN"], check=True)
     return LIB
 
 

@@ -523,6 +523,83 @@ int csdrb_fmmod_bank_fc(const float* d_in, long in_stride, complexf* d_out, long
     return rc < 0 ? rc : counted(rc, channels > 0 && n > 0 ? 1 : 0);
 }
 
+// synthesis bank (synth.cu): fir_interpolate_cc | shift_addition_cc per channel, summed over the channels in a fixed pairwise tree
+size_t csdrb_synth_bank_scratch_bytes(int channels, int input_size, int interpolation, int taps_length, int chunk, int offset)
+{
+    return synth_bank_scratch_bytes(channels, input_size, interpolation, taps_length, chunk, offset);
+}
+
+int csdrb_synth_bank_cc(const complexf* d_in, long in_stride, int channels, int input_size, int interpolation, const float* d_taps, int taps_length,
+                        const shift_addition_data_t* d_params, float* d_phase_io, int chunk, int offset, complexf* d_out, void* d_scratch,
+                        size_t scratch_bytes, void* stream)
+{
+    if (!d_in || !d_taps || !d_params || !d_phase_io || !d_out || misaligned(d_in, 8) || misaligned(d_out, 8) || misaligned(d_taps, 4) ||
+        misaligned(d_params, 4) || misaligned(d_phase_io, 4)) {
+        set_error("synth bank: null or misaligned pointer (complexf needs 8-byte, float 4-byte alignment)");
+        return -1;
+    }
+    int launches = 0;
+    int rc = launch_synth_bank(reinterpret_cast<const float2*>(d_in), in_stride, channels, input_size, interpolation, d_taps, taps_length,
+                               reinterpret_cast<const float*>(d_params), d_phase_io, chunk, offset, reinterpret_cast<float2*>(d_out), d_scratch,
+                               scratch_bytes, &launches, S(stream));
+    return rc < 0 ? rc : counted(rc, launches);
+}
+
+// streaming synthesis bank: the state of csdrb_synth_bank_cc between blocks (phases, offset inside the NCO chunk) and its buffers
+struct csdrb_synth_bank_s {
+    int channels = 0, interpolation = 0, taps_length = 0, chunk = 0, offset = 0;
+    float* d_params = nullptr;                        // shift_addition_data_t per channel
+    float* d_taps = nullptr;
+    float* d_phase = nullptr;                         // phase at the start of the chunk holding the next block's first output
+    void* d_scratch = nullptr;
+    size_t scratch_cap = 0;
+};
+
+csdrb_synth_bank_t* csdrb_synth_bank_create(int channels, const float* h_rates, int interpolation, const float* h_taps, int taps_length, int chunk)
+{
+    if (channels < 1 || !h_rates || !h_taps || interpolation < 1 || taps_length < 1 || chunk < 1) {
+        set_error("synth bank create: needs channels >= 1, rates, taps, interpolation >= 1, taps_length >= 1 and chunk >= 1");
+        return nullptr;
+    }
+    auto* b = new csdrb_synth_bank_s();
+    b->channels = channels; b->interpolation = interpolation; b->taps_length = taps_length; b->chunk = chunk;
+    std::vector<shift_addition_data_t> params((size_t)channels);
+    for (int c = 0; c < channels; c++) params[(size_t)c] = shift_addition_init(h_rates[c]);
+    bool ok = cudaMalloc(&b->d_params, sizeof(shift_addition_data_t) * (size_t)channels) == cudaSuccess;
+    ok = ok && cudaMalloc(&b->d_taps, sizeof(float) * (size_t)taps_length) == cudaSuccess;
+    ok = ok && cudaMalloc(&b->d_phase, sizeof(float) * (size_t)channels) == cudaSuccess;
+    ok = ok && cudaMemcpy(b->d_params, params.data(), sizeof(shift_addition_data_t) * (size_t)channels, cudaMemcpyHostToDevice) == cudaSuccess;
+    ok = ok && cudaMemcpy(b->d_taps, h_taps, sizeof(float) * (size_t)taps_length, cudaMemcpyHostToDevice) == cudaSuccess;
+    ok = ok && cudaMemset(b->d_phase, 0, sizeof(float) * (size_t)channels) == cudaSuccess;
+    if (!ok) { set_error("synth bank create: CUDA allocation failed (%s)", cudaGetErrorString(cudaGetLastError())); csdrb_synth_bank_destroy(b); return nullptr; }
+    return b;
+}
+
+void csdrb_synth_bank_destroy(csdrb_synth_bank_t* b)
+{
+    if (!b) return;
+    cudaFree(b->d_params); cudaFree(b->d_taps); cudaFree(b->d_phase); cudaFree(b->d_scratch);
+    delete b;
+}
+
+int csdrb_synth_bank_process(csdrb_synth_bank_t* b, const complexf* d_in, long in_stride, int input_size, complexf* d_out, void* stream)
+{
+    if (!b) { set_error("synth bank process: null bank"); return -1; }
+    const size_t need = synth_bank_scratch_bytes(b->channels, input_size, b->interpolation, b->taps_length, b->chunk, b->offset);
+    if (need > b->scratch_cap) {                      // grow: the previous block may still read the old buffer
+        CSDRB_CUDA(cudaStreamSynchronize(S(stream)));
+        if (b->d_scratch) CSDRB_CUDA(cudaFree(b->d_scratch));
+        b->d_scratch = nullptr; b->scratch_cap = 0;
+        CSDRB_CUDA(cudaMalloc(&b->d_scratch, need));
+        b->scratch_cap = need;
+    }
+    const int rc = csdrb_synth_bank_cc(d_in, in_stride, b->channels, input_size, b->interpolation, b->d_taps, b->taps_length,
+                                       reinterpret_cast<const shift_addition_data_t*>(b->d_params), b->d_phase, b->chunk, b->offset, d_out,
+                                       b->d_scratch, b->scratch_cap, stream);
+    if (rc > 0) b->offset = (int)(((long)b->offset + rc) % b->chunk);
+    return rc;
+}
+
 int csdrb_fft_c2c_batch(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int size, int batch, int inverse, void* stream)
 {
     if (!d_in || !d_out) { set_error("fft: null pointer"); return -1; }

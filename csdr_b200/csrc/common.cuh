@@ -226,4 +226,11 @@ __device__ __forceinline__ float phase_increment(float rate, int n) { return __f
 // ... added to the phase and wrapped into [-PI, PI]: one step of the chain ph <- wrap(fl(ph + inc))
 __device__ __forceinline__ float phase_step(float ph, float inc) { return wrap_phase_pm_pi(__fadd_rn(ph, inc)); }
 
+// groups of I outputs one fir_interpolate_cc call on n inputs gives (libcsdr.c:579-602): interpolate.cu's bank and synth.cu's synthesis bank
+__host__ __device__ inline long interp_groups(int n, int I, int T)
+{
+    const long h = ((long)T - 1 + I - 1) / I;                // ceil((T-1)/I): inputs each group looks ahead
+    return n > h ? (long)n - h : 0;
+}
+
 }  // namespace csdrb

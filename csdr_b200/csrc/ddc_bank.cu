@@ -396,10 +396,16 @@ size_t ddc_bank_scratch_bytes(int channels, int input_size, int chunk, int offse
     const long nchunks = ((long)offset + input_size + chunk - 1) / chunk + 1;
     return (size_t)channels * (size_t)nchunks * (sizeof(float) + sizeof(float2)) + 64 + (size_t)channels * sizeof(WrapTable) + 16;
 }
+static inline size_t ddc_seeds_offset(int channels, int nchunks) { return ((size_t)channels * nchunks * sizeof(float) + 15) & ~(size_t)15; }
 static inline size_t ddc_tables_offset(int channels, int nchunks)        // the per-call wrap tables sit behind the chunk phases and the seeds
 {
-    const size_t seeds_off = ((size_t)channels * nchunks * sizeof(float) + 15) & ~(size_t)15;
-    return (seeds_off + (size_t)channels * nchunks * sizeof(float2) + 15) & ~(size_t)15;
+    return (ddc_seeds_offset(channels, nchunks) + (size_t)channels * nchunks * sizeof(float2) + 15) & ~(size_t)15;
+}
+static inline int ddc_nchunks(int input_size, int chunk, int offset) { return (int)(((long)offset + input_size + chunk - 1) / chunk) + 1; }
+const float2* ddc_prepass_seeds(const void* d_scratch, int channels, int input_size, int chunk, int offset, int* nchunks)
+{
+    *nchunks = ddc_nchunks(input_size, chunk, offset);
+    return reinterpret_cast<const float2*>(static_cast<const char*>(d_scratch) + ddc_seeds_offset(channels, *nchunks));
 }
 int launch_ddc_rechunk(int channels, const float* d_params, float* d_phase_io, int n, cudaStream_t st)
 {
@@ -520,9 +526,9 @@ int launch_ddc_prepass(int input_size, int channels, const float* d_params, floa
     if (chunk <= 0) chunk = input_size;
     if (offset < 0 || offset >= chunk) { set_error("ddc bank: offset must be in [0, chunk)"); return -1; }
     if (scratch_bytes < ddc_bank_scratch_bytes(channels, input_size, chunk, offset) || !d_scratch) { set_error("ddc bank: scratch too small"); return -1; }
-    const int nchunks = (int)(((long)offset + input_size + chunk - 1) / chunk) + 1;
+    const int nchunks = ddc_nchunks(input_size, chunk, offset);
     float* chunk_phase = static_cast<float*>(d_scratch);
-    float2* seeds = reinterpret_cast<float2*>(static_cast<char*>(d_scratch) + (((size_t)channels * nchunks * sizeof(float) + 15) & ~(size_t)15));
+    float2* seeds = reinterpret_cast<float2*>(static_cast<char*>(d_scratch) + ddc_seeds_offset(channels, nchunks));
     int launches = 2;
     if (!d_tables) {                                                    // no persistent tables (one-shot call): build them for this call
         void* tb = static_cast<char*>(d_scratch) + ddc_tables_offset(channels, nchunks);
@@ -563,8 +569,8 @@ static int ddc_main(const TIn* d_wide, int input_size, int channels, const float
     if (n_out == 0) return 0;
     if (chunk <= 0) chunk = input_size;
     if (!ddc_wide_aligned(d_wide)) return -1;
-    const int nchunks = (int)(((long)offset + input_size + chunk - 1) / chunk) + 1;
-    const float2* seeds = reinterpret_cast<const float2*>(static_cast<const char*>(d_scratch) + (((size_t)channels * nchunks * sizeof(float) + 15) & ~(size_t)15));
+    int nchunks;
+    const float2* seeds = ddc_prepass_seeds(d_scratch, channels, input_size, chunk, offset, &nchunks);
     if (int rc = ddc_bank_geometry(decimation, taps_length); rc < 0) return rc;
     int rc = -1;
     const float3* P = reinterpret_cast<const float3*>(d_params);

@@ -25,13 +25,6 @@ constexpr int INTERP_THREADS = 256;
 constexpr int INTERP_TILE = 2048;                            // outputs per CTA
 constexpr int INTERP_SMEM_TAPS = 8192;                       // 32 KB of taps in shared memory; beyond, the read-only cache
 
-// groups of I outputs one reference call on n inputs gives
-__host__ __device__ inline long interp_groups(int n, int I, int T)
-{
-    const long h = ((long)T - 1 + I - 1) / I;                // ceil((T-1)/I): inputs each group looks ahead
-    return n > h ? (long)n - h : 0;
-}
-
 template <bool SMEM_TAPS>
 __global__ void __launch_bounds__(INTERP_THREADS)
 fir_interpolate_kernel(const float2* __restrict__ in, long in_stride, float2* __restrict__ out, long out_stride, long nout, int I,

@@ -179,6 +179,13 @@ int launch_fir_interpolate_bank_cc(const float2* d_in, long in_stride, float2* d
                                    const float* d_taps, int taps_length, cudaStream_t st);
 int launch_fmmod_bank_fc(const float* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n, float* d_phase_io, cudaStream_t st);
 
+// synthesis bank, synth.cu: C channels of fir_interpolate_cc | shift_addition_cc summed in a fixed pairwise tree over the channel index into one
+// wideband row.  Returns G*I outputs (< 0 refused); *launches gets the kernels it launched
+size_t synth_bank_scratch_bytes(int channels, int n, int interpolation, int taps_length, int chunk, int offset);
+int launch_synth_bank(const float2* d_in, long in_stride, int channels, int n, int interpolation, const float* d_taps, int taps_length,
+                      const float* d_params, float* d_phase_io, int chunk, int offset, float2* d_out, void* d_scratch, size_t scratch_bytes,
+                      int* launches, cudaStream_t st);
+
 // fused shared-input DDC bank, ddc_bank.cu
 int ddc_bank_geometry(int decimation, int taps_length);               // 0 when the bank serves (decimation, taps_length); else -2 with the error set
 size_t ddc_bank_scratch_bytes(int channels, int input_size, int chunk, int offset);
@@ -187,6 +194,8 @@ int launch_ddc_rechunk(int channels, const float* d_params, float* d_phase_io, i
 int launch_ddc_tables(int channels, const float* d_params, int chunk, void* d_tables, cudaStream_t st);
 int launch_ddc_prepass(int input_size, int channels, const float* d_params, float* d_phase_io, int chunk, int offset, int decimation,
                        int taps_length, void* d_scratch, size_t scratch_bytes, const void* d_tables, cudaStream_t st);   // d_tables NULL: built per call in d_scratch
+// where launch_ddc_prepass left the (cos, sin) seeds of a block's absolute chunks, [channels][*nchunks], in its scratch
+const float2* ddc_prepass_seeds(const void* d_scratch, int channels, int input_size, int chunk, int offset, int* nchunks);
 int launch_ddc_main(const float2* d_wide, int input_size, int channels, const float* d_params, int chunk, int offset, int decimation,
                     const float* h_taps, int taps_length, int demod, void* d_out, long out_stride, const float2* d_last_in, float2* d_last_out,
                     const void* d_scratch, cudaStream_t st);

@@ -594,6 +594,30 @@ int csdrb_fir_interpolate_bank_cc(const complexf *d_in, long in_stride, complexf
                                   const float *d_taps, int taps_length, void *stream);
 int csdrb_fmmod_bank_fc(const float *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int n, float *d_phase_io, void *stream);
 
+/* Synthesis bank (synth.cu): C baseband channels into ONE wideband stream,
+ *     y = sum over c of shift_addition_cc(fir_interpolate_cc(x_c, I, taps), rate_c)
+ * with the C upshifted intermediates never in memory.  Per channel the contribution is bit for bit csdrb_fir_interpolate_bank_cc followed by
+ * csdrb_shift_addition_bank_cc called once per `chunk` samples, the chunks counted on the absolute stream as in csdrb_ddc_bank: output 0 lies
+ * `offset` samples into a chunk, d_phase_io[c] is the phase at the start of that chunk and on return the phase at the start of the chunk that
+ * contains output G*I.  d_params[c] = shift_addition_init(rate_c) (host), one set of real taps shared by all channels (tap 0 unused, as in
+ * fir_interpolate_cc), row c of the input at d_in + c*in_stride, n inputs per row giving G = n - ceil((T-1)/I) groups (or none).  The channels are
+ * summed in a fixed pairwise tree over the channel index, I and Q separately, each add rounded: level 0 pairs channels (2k, 2k+1), the next level
+ * those sums, and so on; a node with one present child is that child (C = 3: (Y0 + Y1) + Y2; C = 1: Y0 exactly).  The order depends on C alone.
+ *   csdrb_synth_bank_cc returns G*I, the outputs written to d_out; -1 (csdrb_last_error() set, nothing launched, d_phase_io untouched) for I < 1,
+ *   T < 1, channels < 1, n < 0, chunk < 1, offset outside [0, chunk), in_stride < n, more than 2^31 - 1 outputs, a null or misaligned pointer
+ *   or scratch_bytes below csdrb_synth_bank_scratch_bytes() of the same arguments.
+ *   The streaming object owns the rates, the device taps, the phases, the offset and the scratch; process() is csdrb_synth_bank_cc on its state.
+ *   Block contract of fir_interpolate_cc: a call on n inputs per channel consumes G of them (returns G*I), and the caller presents the last n - G
+ *   again at the front of the next block.  create() returns NULL for bad arguments (csdrb_last_error() set). */
+size_t csdrb_synth_bank_scratch_bytes(int channels, int input_size, int interpolation, int taps_length, int chunk, int offset);
+int csdrb_synth_bank_cc(const complexf *d_in, long in_stride, int channels, int input_size, int interpolation, const float *d_taps, int taps_length,
+                        const shift_addition_data_t *d_params, float *d_phase_io, int chunk, int offset, complexf *d_out, void *d_scratch,
+                        size_t scratch_bytes, void *stream);
+typedef struct csdrb_synth_bank_s csdrb_synth_bank_t;
+csdrb_synth_bank_t *csdrb_synth_bank_create(int channels, const float *h_rates, int interpolation, const float *h_taps, int taps_length, int chunk);
+void csdrb_synth_bank_destroy(csdrb_synth_bank_t *bank);
+int  csdrb_synth_bank_process(csdrb_synth_bank_t *bank, const complexf *d_in, long in_stride, int input_size, complexf *d_out, void *stream);
+
 /* K7 batched unnormalised c2c DFT (power-of-two size 2..16384), sign -1 forward / +1 inverse */
 int csdrb_fft_c2c_batch(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int size, int batch, int inverse, void *stream);
 /* The same transform for the sizes above one CTA's shared memory: power-of-two size 32768..1048576 (2^15..2^20), two launches per chunk of

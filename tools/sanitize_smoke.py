@@ -48,3 +48,10 @@ for I, T, n in ((1, 7, 999), (3, 81, 1001), (50, 401, 333), (256, 2049, 37), (5,
     cb.fir_interpolate_bank(cplx(3, n + 1)[:, :n], I, cb.firdes_lowpass_f(T, 0.5 / I))
 ph = torch.zeros(5, device=dev); cb.fmmod_bank((torch.rand((5, 1037), device=dev) * 2 - 1) * 9, ph); cb.fmmod_bank(torch.rand((5, 31), device=dev), ph)
 torch.cuda.synchronize()
+# synthesis bank: the register window at h = 1 and 8, the general path with taps in shared memory and past it, ragged warps, two CTAs of
+# channels (the second tree pass), chunks of 1 and 7 with offsets, n below one group, the streaming object
+for ch, I, T, n, chunk, off in ((1, 1, 1, 300, 7, 3), (33, 50, 401, 40, 1024, 17), (257, 2, 2, 100, 7, 2), (5, 3, 40, 200, 1, 0), (3, 50, 9001, 190, 1024, 0),
+                               (100, 256, 2049, 11, 1024, 1023), (2, 50, 401, 8, 1024, 0)):
+    cb.synth_bank(cplx(ch, n + 1)[:, :n], np.linspace(-0.45, 0.45, ch), I, rng.uniform(-1, 1, T).astype(np.float32), chunk=chunk, offset=off)
+sb = cb.SynthBank(np.linspace(-0.4, 0.4, 40), 50, cb.firdes_lowpass_f(401, 0.01)); w = cplx(40, 3000); sb.process(w[:, :1000].contiguous()); sb.process(w[:, 992:2500].contiguous()); sb.close()
+torch.cuda.synchronize()
