@@ -279,6 +279,14 @@ def lib() -> C.CDLL:
     L.csdrb_bfsk_demod_bank_cf.argtypes = [vp, lg, vp, lg, it, it, vp, vp, it, vp]
     L.csdrb_fir_interpolate_bank_cc.argtypes = [vp, lg, vp, lg, it, it, it, vp, it, vp]
     L.csdrb_fmmod_bank_fc.argtypes = [vp, lg, vp, lg, it, it, vp, vp]
+    L.csdrb_psk31_varicode_encoder_bank_u8_u8.argtypes = [vp, lg, vp, lg, it, it, vp, it, vp, vp, vp]
+    L.csdrb_differential_codec_bank_u8_u8.argtypes = [vp, lg, vp, lg, it, it, vp, it, vp, vp]
+    L.csdrb_psk_modulator_bank_u8_c.argtypes = [vp, lg, vp, lg, it, it, vp, it, vp]
+    L.csdrb_psk31_interpolate_sine_bank_cc.argtypes = [vp, lg, vp, lg, it, it, vp, it, vp, vp]
+    L.psk31_varicode_encoder_u8_u8.argtypes = [vp, vp, it, it, C.POINTER(it), C.POINTER(it)]
+    L.differential_codec.argtypes = [vp, vp, it, it, C.c_ubyte]; L.differential_codec.restype = C.c_ubyte
+    L.psk_modulator_u8_c.argtypes = [vp, vp, it, it]
+    L.psk31_interpolate_sine_cc.argtypes = [vp, vp, it, it, _CF]; L.psk31_interpolate_sine_cc.restype = _CF
     L.csdrb_synth_bank_scratch_bytes.argtypes = [it, it, it, it, it, it]; L.csdrb_synth_bank_scratch_bytes.restype = sz
     L.csdrb_synth_bank_cc.argtypes = [vp, lg, it, it, it, vp, it, vp, vp, it, it, vp, vp, sz, vp]
     L.csdrb_synth_bank_create.argtypes = [it, C.POINTER(C.c_float), it, C.POINTER(C.c_float), it, it]; L.csdrb_synth_bank_create.restype = vp
@@ -1238,6 +1246,68 @@ def fmmod_bank(x, phase=None):
         return out[:, :0]
     _check(lib().csdrb_fmmod_bank_fc(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, phase.data_ptr(), _stream()), "fmmod_bank")
     return out[:, :n]
+
+
+def _u8_rows(x):
+    import torch
+    assert x.dtype == torch.uint8 and x.is_cuda and x.dim() == 2 and x.stride(1) == 1
+    return x.shape
+
+
+def psk31_varicode_encoder_bank_u8_u8(text, lengths=None, output_max_size=None):
+    """psk31_varicode_encoder_u8_u8 per row (libcsdr.c:1551-1575): text [C, N] uint8 (row c holds lengths[c] bytes) -> (bits [C, M] uint8, one
+    byte 0/1 per bit, input_processed [C] int32, output_size [C] int32).  M = output_max_size, by default 12*N: every character fits (the longest
+    code has 10 bits, then two 0 bits).  output_size can be passed on as the next bank's lengths."""
+    import torch
+    ch, n = _u8_rows(text)
+    m = 12 * n if output_max_size is None else output_max_size
+    out = torch.zeros((ch, max(m, 1)), dtype=torch.uint8, device=text.device)
+    processed = torch.zeros(ch, dtype=torch.int32, device=text.device)
+    size = torch.zeros(ch, dtype=torch.int32, device=text.device)
+    _check(lib().csdrb_psk31_varicode_encoder_bank_u8_u8(text.data_ptr(), text.stride(0), out.data_ptr(), out.stride(0), ch, n,
+                                                         lengths.data_ptr() if lengths is not None else None, m, processed.data_ptr(),
+                                                         size.data_ptr(), _stream()), "psk31_varicode_encoder_bank_u8_u8")
+    return out[:, :max(m, 0)], processed, size
+
+
+def differential_codec_bank_u8_u8(x, encode: bool, lengths=None, state=None):
+    """differential_codec per row (libcsdr.c:1828-1843): x [C, N] uint8 -> (out [C, N] uint8, state [C] uint8).  state: the codec state
+    carried between calls (zeros at stream start), a [C] uint8 CUDA tensor updated in place; None starts from 0."""
+    import torch
+    ch, n = _u8_rows(x)
+    state = torch.zeros(ch, dtype=torch.uint8, device=x.device) if state is None else state
+    assert state.dtype == torch.uint8 and state.is_cuda and state.numel() == ch and state.is_contiguous()
+    out = torch.zeros((ch, max(n, 1)), dtype=torch.uint8, device=x.device)
+    _check(lib().csdrb_differential_codec_bank_u8_u8(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n,
+                                                     lengths.data_ptr() if lengths is not None else None, int(bool(encode)), state.data_ptr(),
+                                                     _stream()), "differential_codec_bank_u8_u8")
+    return out[:, :n], state
+
+
+def psk_modulator_bank_u8_c(x, n_psk: int, lengths=None):
+    """psk_modulator_u8_c per row (libcsdr.c:1772-1782): symbols x [C, N] uint8 -> [C, N] complex64, (cos, sin)(b * 2pi/n_psk), 1 <= n_psk <= 256"""
+    import torch
+    ch, n = _u8_rows(x)
+    out = torch.zeros((ch, max(n, 1)), dtype=torch.complex64, device=x.device)
+    _check(lib().csdrb_psk_modulator_bank_u8_c(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n,
+                                               lengths.data_ptr() if lengths is not None else None, n_psk, _stream()), "psk_modulator_bank_u8_c")
+    return out[:, :n]
+
+
+def psk31_interpolate_sine_bank_cc(x, interpolation: int, lengths=None, last=None):
+    """psk31_interpolate_sine_cc per row (libcsdr.c:1793-1808): x [C, N] complex64 -> ([C, N*interpolation] complex64, last [C] complex64).
+    last: the previous input of each row carried between calls (zeros at stream start), a [C] complex64 CUDA tensor updated in place."""
+    import torch
+    assert x.dtype == torch.complex64 and x.is_cuda and x.dim() == 2 and x.stride(1) == 1
+    ch, n = x.shape
+    last = torch.zeros(ch, dtype=torch.complex64, device=x.device) if last is None else last
+    assert last.dtype == torch.complex64 and last.is_cuda and last.numel() == ch and last.is_contiguous()
+    m = n * max(interpolation, 0)
+    out = torch.zeros((ch, max(m, 1)), dtype=torch.complex64, device=x.device)
+    _check(lib().csdrb_psk31_interpolate_sine_bank_cc(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n,
+                                                      lengths.data_ptr() if lengths is not None else None, interpolation, last.data_ptr(),
+                                                      _stream()), "psk31_interpolate_sine_bank_cc")
+    return out[:, :m], last
 
 
 def _synth_rows(x):

@@ -72,6 +72,7 @@ static inline bool too_many_channels(int channels, const char* who)
     set_error("%s: %d channels in one call (at most 65535; split the bank)", who, channels);
     return true;
 }
+static inline bool misaligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
 static inline bool null_io(const void* in, const void* out, const char* who) { if (in && out) return false; set_error("%s: null pointer", who); return true; }
 int csdrb_convert_u8_f(const unsigned char* d_in, float* d_out, long n, void* stream)
 {
@@ -449,6 +450,49 @@ int csdrb_psk31_varicode_decoder_bank_u8_u8(const unsigned char* d_in, long in_s
     return rc < 0 ? rc : counted(0, rc);
 }
 
+// BPSK31 transmit chain (psk31_tx.cu; libcsdr.c:1551-1575, 1828-1843, 1772-1782, 1793-1808)
+int csdrb_psk31_varicode_encoder_bank_u8_u8(const unsigned char* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels,
+                                            int input_size, const int* d_lengths, int output_max_size, int* d_input_processed, int* d_output_size,
+                                            void* stream)
+{
+    if (null_io(d_in, d_out, "varicode encoder bank")) return -1;
+    if (!d_input_processed || !d_output_size) { set_error("varicode encoder bank: null pointer"); return -1; }
+    int rc = launch_varicode_encoder_bank(d_in, in_stride, d_out, out_stride, channels, input_size, d_lengths, output_max_size, d_input_processed,
+                                          d_output_size, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
+int csdrb_differential_codec_bank_u8_u8(const unsigned char* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels,
+                                        int input_size, const int* d_lengths, int encode, unsigned char* d_state_io, void* stream)
+{
+    if (null_io(d_in, d_out, "differential codec bank")) return -1;
+    if (!d_state_io) { set_error("differential codec bank: null pointer"); return -1; }
+    int rc = launch_differential_codec_bank(d_in, in_stride, d_out, out_stride, channels, input_size, d_lengths, encode, d_state_io, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
+int csdrb_psk_modulator_bank_u8_c(const unsigned char* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int input_size,
+                                  const int* d_lengths, int n_psk, void* stream)
+{
+    if (too_many_channels(channels, "psk modulator bank")) return -1;
+    if (!d_in || !d_out || misaligned(d_out, 8)) { set_error("psk modulator bank: null or misaligned pointer (complexf needs 8-byte alignment)"); return -1; }
+    int rc = launch_psk_modulator_bank(d_in, in_stride, reinterpret_cast<float2*>(d_out), out_stride, channels, input_size, d_lengths, n_psk, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
+int csdrb_psk31_interpolate_sine_bank_cc(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int input_size,
+                                         const int* d_lengths, int interpolation, complexf* d_last_io, void* stream)
+{
+    if (too_many_channels(channels, "psk31_interpolate_sine bank")) return -1;
+    if (!d_in || !d_out || !d_last_io || misaligned(d_in, 8) || misaligned(d_out, 8) || misaligned(d_last_io, 8)) {
+        set_error("psk31_interpolate_sine bank: null or misaligned pointer (complexf needs 8-byte alignment)");
+        return -1;
+    }
+    int rc = launch_psk31_interpolate_sine_bank(reinterpret_cast<const float2*>(d_in), in_stride, reinterpret_cast<float2*>(d_out), out_stride, channels,
+                                                input_size, d_lengths, interpolation, reinterpret_cast<float2*>(d_last_io), S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
 // RTTY receive chain (rtty.cu; libcsdr.c:1662-1729, 1608-1616)
 int csdrb_serial_line_decoder_bank_f_u8(const float* d_in, long in_stride, int end, int* d_start_io, unsigned char* d_out, long out_stride, int* d_count,
                                         int* d_stuck, int channels, const csdrb_serial_line_params_t* params, int bufsize, void* stream)
@@ -470,7 +514,6 @@ int csdrb_rtty_baudot2ascii_bank_u8_u8(const unsigned char* d_in, long in_stride
 }
 
 // tone filters (tone.cu; libcsdr.c:2261-2273, 2335-2351)
-static inline bool misaligned(const void* p, size_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) != 0; }
 
 int csdrb_apply_fir_bank_cc(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int n, const complexf* d_taps,
                             int taps_length, void* stream)

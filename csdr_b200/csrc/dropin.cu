@@ -717,6 +717,69 @@ float fmmod_fc(float* input, complexf* output, int input_size, float last_phase)
     return last_phase;
 }
 
+// ---- BPSK31 transmit chain (libcsdr.c:1551-1575, 1828-1843, 1772-1782, 1793-1808) ------------------------------------------------
+void psk31_varicode_encoder_u8_u8(unsigned char* input, unsigned char* output, int input_size, int output_max_size, int* input_processed,
+                                  int* output_size)
+{
+    *input_processed = 0;
+    *output_size = 0;
+    if (input_size <= 0) return;
+    Staging st("psk31_varicode_encoder_u8_u8");
+    const unsigned char* d_in = st.up(input, input_size);
+    const int room = output_max_size > 0 ? output_max_size : 0;
+    unsigned char* d_out = st.alloc<unsigned char>(room);
+    int* d_counts = st.alloc<int>(2);
+    st.check(csdrb_psk31_varicode_encoder_bank_u8_u8(d_in, input_size, d_out, room, 1, input_size, nullptr, output_max_size, d_counts, d_counts + 1,
+                                                     st.stream()));
+    int counts[2];
+    st.get(counts, d_counts, 2);
+    st.sync();
+    st.get(output, d_out, counts[1]);
+    st.sync();
+    *input_processed = counts[0];
+    *output_size = counts[1];
+}
+
+unsigned char differential_codec(unsigned char* input, unsigned char* output, int input_size, int encode, unsigned char state)
+{
+    if (input_size <= 0) return state;
+    Staging st("differential_codec");
+    const unsigned char* d_in = st.up(input, input_size);
+    unsigned char* d_state = st.up(&state, 1);
+    unsigned char* d_out = st.alloc<unsigned char>(input_size);
+    st.check(csdrb_differential_codec_bank_u8_u8(d_in, input_size, d_out, input_size, 1, input_size, nullptr, encode, d_state, st.stream()));
+    st.get(output, d_out, input_size);
+    st.get(&state, d_state, 1);
+    st.sync();
+    return state;
+}
+
+void psk_modulator_u8_c(unsigned char* input, complexf* output, int input_size, int n_psk)
+{
+    if (input_size <= 0) return;
+    Staging st("psk_modulator_u8_c");
+    const unsigned char* d_in = st.up(input, input_size);
+    complexf* d_out = st.alloc<complexf>(input_size);
+    st.check(csdrb_psk_modulator_bank_u8_c(d_in, input_size, d_out, input_size, 1, input_size, nullptr, n_psk, st.stream()));
+    st.get(output, d_out, input_size);
+    st.sync();
+}
+
+complexf psk31_interpolate_sine_cc(complexf* input, complexf* output, int input_size, int interpolation, complexf last_input)
+{
+    if (input_size <= 0) return last_input;
+    Staging st("psk31_interpolate_sine_cc");
+    const complexf* d_in = st.up(input, input_size);
+    complexf* d_last = st.up(&last_input, 1);
+    const long nout = (long)input_size * (interpolation > 0 ? interpolation : 0);
+    complexf* d_out = st.alloc<complexf>(nout);
+    st.check(csdrb_psk31_interpolate_sine_bank_cc(d_in, input_size, d_out, nout, 1, input_size, nullptr, interpolation, d_last, st.stream()));
+    st.get(output, d_out, nout);
+    st.get(&last_input, d_last, 1);
+    st.sync();
+    return last_input;
+}
+
 int bfsk_demod_cf(complexf* input, float* output, int input_size, complexf* mark_filter, complexf* space_filter, int taps_length)
 {
     if (input_size < taps_length) return input_size - taps_length + 1;     // the reference returns the count it would have written

@@ -110,6 +110,17 @@ int launch_dbpsk_bank(const float2* d_in, long in_stride, unsigned char* d_out, 
 int launch_varicode_bank(const unsigned char* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels, int n, const int* d_lengths,
                          unsigned long long* d_hist_io, int* d_count, cudaStream_t st);
 
+// BPSK31 transmit chain, psk31_tx.cu: one row per channel, d_lengths optional (NULL: n for every row); each returns the launches it made
+extern "C" int csdrb_psk31_sine_rates(int interpolation, float* rates);   // host/psk31_rates.c: the build's rate table; -1 without libmvec
+int launch_varicode_encoder_bank(const unsigned char* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels, int n,
+                                 const int* d_lengths, int output_max_size, int* d_input_processed, int* d_output_size, cudaStream_t st);
+int launch_differential_codec_bank(const unsigned char* d_in, long in_stride, unsigned char* d_out, long out_stride, int channels, int n,
+                                   const int* d_lengths, int encode, unsigned char* d_state_io, cudaStream_t st);
+int launch_psk_modulator_bank(const unsigned char* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n, const int* d_lengths,
+                              int n_psk, cudaStream_t st);
+int launch_psk31_interpolate_sine_bank(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n, const int* d_lengths,
+                                       int interpolation, float2* d_last_io, cudaStream_t st);
+
 // RTTY receive chain, rtty.cu.  SerialLineParams has the layout of csdrb_serial_line_params_t.
 struct SerialLineParams { float samples_per_bits; int databits; float stopbits, bit_sampling_width_ratio; };
 int serial_line_max_outputs(float samples_per_bits, int databits, float stopbits, int input_size);   // characters input_size samples can hold at most

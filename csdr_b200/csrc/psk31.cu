@@ -10,6 +10,7 @@
 // disassembly; these kernels follow it operation for operation, with explicit _rn intrinsics so that nothing is contracted into an FMA.
 #include "common.cuh"
 #include "kernels.h"
+#include "varicode.cuh"
 
 namespace csdrb {
 
@@ -241,28 +242,7 @@ int launch_dbpsk_bank(const float2* d_in, long in_stride, unsigned char* d_out, 
 // (code << 2) == shr & (2^(bitcount+4) - 1), else 0.  Its early return tests `shr & (0xFFF == 0)`, i.e. `shr & 0`, and never fires.  The
 // longest code has 10 bits, so the character at bit i is a function of bits i-13..i; bits before the call come from the carried register.
 //
-// The varicode table of PSK31 (G3PLX's specification), ASCII 0..127: code bits, most significant first, and their number.
-struct Varicode { unsigned short code; unsigned char bits; };
-#define VC(s) {(unsigned short)0b##s, (unsigned char)(sizeof(#s) - 1)}
-__constant__ Varicode kVaricode[128] = {
-    VC(1010101011), VC(1011011011), VC(1011101101), VC(1101110111), VC(1011101011), VC(1101011111), VC(1011101111), VC(1011111101),
-    VC(1011111111), VC(11101111),   VC(11101),      VC(1101101111), VC(1011011101), VC(11111),      VC(1101110101), VC(1110101011),
-    VC(1011110111), VC(1011110101), VC(1110101101), VC(1110101111), VC(1101011011), VC(1101101011), VC(1101101101), VC(1101010111),
-    VC(1101111011), VC(1101111101), VC(1110110111), VC(1101010101), VC(1101011101), VC(1110111011), VC(1011111011), VC(1101111111),
-    VC(1),          VC(111111111),  VC(101011111),  VC(111110101),  VC(111011011),  VC(1011010101), VC(1010111011), VC(101111111),
-    VC(11111011),   VC(11110111),   VC(101101111),  VC(111011111),  VC(1110101),    VC(110101),     VC(1010111),    VC(110101111),
-    VC(10110111),   VC(10111101),   VC(11101101),   VC(11111111),   VC(101110111),  VC(101011011),  VC(101101011),  VC(110101101),
-    VC(110101011),  VC(110110111),  VC(11110101),   VC(110111101),  VC(111101101),  VC(1010101),    VC(111010111),  VC(1010101111),
-    VC(1010111101), VC(1111101),    VC(11101011),   VC(10101101),   VC(10110101),   VC(1110111),    VC(11011011),   VC(11111101),
-    VC(101010101),  VC(1111111),    VC(111111101),  VC(101111101),  VC(11010111),   VC(10111011),   VC(11011101),   VC(10101011),
-    VC(11010101),   VC(111011101),  VC(10101111),   VC(1101111),    VC(1101101),    VC(101010111),  VC(110110101),  VC(101011101),
-    VC(101110101),  VC(101111011),  VC(1010101101), VC(111110111),  VC(111101111),  VC(111111011),  VC(1010111111), VC(101101101),
-    VC(1011011111), VC(1011),       VC(1011111),    VC(101111),     VC(101101),     VC(11),         VC(111101),     VC(1011011),
-    VC(101011),     VC(1101),       VC(111101011),  VC(10111111),   VC(11011),      VC(111011),     VC(1111),       VC(111),
-    VC(111111),     VC(110111111),  VC(10101),      VC(10111),      VC(101),        VC(110111),     VC(1111011),    VC(1101011),
-    VC(11011111),   VC(1011101),    VC(111010101),  VC(1010110111), VC(110111011),  VC(1010110101), VC(1011010111), VC(1110110101),
-};
-#undef VC
+// The table, kVaricode, is shared with the encoder (varicode.cuh).
 constexpr int kVaricodeWindow = 14;                                        // longest code (10 bits) + the two zero bits on either side
 
 __device__ __forceinline__ unsigned char varicode_char(unsigned w)

@@ -13,6 +13,8 @@
  *   - fflush + sched_yield after every block (:198); F_SETPIPE_SZ 2 MiB, 4096 for small blocks (:427-428, :369-373)
  *   - runtime retune over --fifo <path> / --fd <n>: text lines, non-blocking, last complete line wins (:252-323)
  *   - the stderr lines the reference prints for these commands
+ *   - psk31_varicode_encoder_u8_u8 as the reference's loop runs: after the first block it re-encodes that block once per read (:2797 refills
+ *     the wrong buffer), so its bytes equal the reference CLI's for every input
  * Everything else the reference CLI offers (100+ other commands) is out of scope (SURVEY.md section 2.1 #6).
  */
 #define _GNU_SOURCE
@@ -1032,6 +1034,70 @@ static int cmd_fmmod_fc(int argc, char **argv)                               /* 
     return map_blocks(sizeof(float), sizeof(complexf), block, 0, fmmod_step, &phase);
 }
 
+/* ---- BPSK31 transmit chain (csdr.c:2684-2701, 2727-2746, 2780-2800, 2816-2833) ---------------------------------------------------
+ * psk31_varicode_encoder_u8_u8 | differential_encoder_u8_u8 | psk_modulator_u8_c 2 | psk31_interpolate_sine_cc <sps>, the pipe of the reference's
+ * BER harness.  The codec, the modulator and the interpolator are per-block maps with their state carried; the next process is told the block
+ * (codec, modulator) or the block times the interpolation. */
+static void psk_modulator_step(void *in, void *out, void *n_psk) { psk_modulator_u8_c(in, out, block, *(int *)n_psk); }
+
+static int cmd_psk_modulator_u8_c(int argc, char **argv)
+{
+    if (argc <= 2) return complain("need required parameter (n_psk)");
+    int n_psk = 0; sscanf(argv[2], "%d", &n_psk);
+    if (n_psk <= 0 || n_psk > 256) return complain("n_psk should be between 1 and 256");
+    if (!announce_block(open_block())) return -2;
+    return map_blocks(1, sizeof(complexf), block, 0, psk_modulator_step, &n_psk);
+}
+
+typedef struct { int interpolation; complexf last; } sine_state_t;
+static void sine_step(void *in, void *out, void *s) { sine_state_t *st = s; st->last = psk31_interpolate_sine_cc(in, out, block, st->interpolation, st->last); }
+
+static int cmd_psk31_interpolate_sine_cc(int argc, char **argv)
+{
+    if (argc <= 2) return complain("need required parameter (interpolation)");
+    sine_state_t st = {0, {0.f, 0.f}}; sscanf(argv[2], "%d", &st.interpolation);
+    if (st.interpolation <= 0) return complain("interpolation should be >0");
+    if (!open_block()) return -2;
+    announce_block(block * st.interpolation);
+    return map_blocks(sizeof(complexf), sizeof(complexf), block * st.interpolation, 0, sine_step, &st);
+}
+
+typedef struct { int encode; unsigned char state; } codec_state_t;
+static void codec_step(void *in, void *out, void *s) { codec_state_t *st = s; st->state = differential_codec(in, out, block, st->encode, st->state); }
+
+static int codec_stream(int encode)
+{
+    if (!announce_block(open_block())) return -2;
+    codec_state_t st = {encode, 0};
+    return map_blocks(1, 1, block, 0, codec_step, &st);
+}
+static int cmd_differential_encoder_u8_u8(int argc, char **argv) { (void)argc; (void)argv; return codec_stream(1); }
+static int cmd_differential_decoder_u8_u8(int argc, char **argv) { (void)argc; (void)argv; return codec_stream(0); }
+
+/* The reference's encoder loop as it runs (csdr.c:2780-2800), so that a pipe graph keeps its bytes: one read into a zero-filled block, then
+ * encode the block, write, the end-of-file test, and a refill that reads the consumed bytes into a buffer that is never encoded (csdr.c:2797
+ * reads into input_buffer, not local_input_buffer).  Every block after the first therefore repeats the first block's bits, once per further
+ * read, until the end of the input; a short first read encodes the zero padding as NUL characters.  Text longer than one block belongs to the
+ * drop-in or the bank, which encode every byte. */
+static int cmd_psk31_varicode_encoder_u8_u8(int argc, char **argv)
+{
+    (void)argc; (void)argv;
+    if (!open_block()) return -2;
+    announce_block(block * 8);
+    const int output_max_size = block * 30;
+    unsigned char *in = must_alloc((size_t)block), *out = must_alloc((size_t)output_max_size), *refilled = must_alloc((size_t)block);
+    fread(in, 1, (size_t)block, stdin);
+    for (;;) {
+        int input_processed = 0, output_size = 0;
+        psk31_varicode_encoder_u8_u8(in, out, block, output_max_size, &input_processed, &output_size);
+        fwrite(out, 1, (size_t)output_size, stdout);
+        if (feof(stdin)) return 0;
+        memmove(in, in + input_processed, (size_t)(block - input_processed));
+        fread(refilled, 1, (size_t)input_processed, stdin);
+        end_of_block();
+    }
+}
+
 /* ---- dispatch ------------------------------------------------------------------------------------ */
 static const struct { const char *name; int (*run)(int, char **); const char *syntax; } kCommands[] = {
     {"convert_u8_f", cmd_convert_u8_f, "convert_u8_f"},
@@ -1080,6 +1146,11 @@ static const struct { const char *name; int (*run)(int, char **); const char *sy
     {"fastddc_inv_cc", cmd_fastddc_inv_cc, "fastddc_inv_cc <shift_rate> <decimation> [transition_bw [window]] | --fifo <fifo_path> ... | --fd <fd> ..."},
     {"fir_interpolate_cc", cmd_fir_interpolate_cc, "fir_interpolate_cc <interpolation_factor> [transition_bw [window]]"},
     {"fmmod_fc", cmd_fmmod_fc, "fmmod_fc"},
+    {"psk31_varicode_encoder_u8_u8", cmd_psk31_varicode_encoder_u8_u8, "psk31_varicode_encoder_u8_u8"},
+    {"differential_encoder_u8_u8", cmd_differential_encoder_u8_u8, "differential_encoder_u8_u8"},
+    {"differential_decoder_u8_u8", cmd_differential_decoder_u8_u8, "differential_decoder_u8_u8"},
+    {"psk_modulator_u8_c", cmd_psk_modulator_u8_c, "psk_modulator_u8_c <n_psk>"},
+    {"psk31_interpolate_sine_cc", cmd_psk31_interpolate_sine_cc, "psk31_interpolate_sine_cc <interpolation>"},
 };
 
 static int usage(void)

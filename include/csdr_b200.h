@@ -145,6 +145,17 @@ int  bfsk_demod_cf(complexf *input, float *output, int input_size, complexf *mar
 int   fir_interpolate_cc(complexf *input, complexf *output, int input_size, int interpolation, float *taps, int taps_length);
 float fmmod_fc(float *input, complexf *output, int input_size, float last_phase);
 
+/* BPSK31 transmit chain (libcsdr.h:343-347; libcsdr.c:1551-1575, 1772-1808, 1828-1843), the reference's own pipe
+ * psk31_varicode_encoder_u8_u8 | differential_encoder_u8_u8 | psk_modulator_u8_c 2 | psk31_interpolate_sine_cc <sps>.  The encoder, the
+ * differential codec and the interpolator are bit for bit the reference build.  psk_modulator_u8_c is the float of the double cos/sin of the
+ * build's float phase: bit for bit the build for n_psk 2, 4 and 8 with symbols below n_psk, within 2 float ulps of it elsewhere (the build's
+ * own scalar and vector paths differ by that much, DESIGN.md section 7). */
+void          psk31_varicode_encoder_u8_u8(unsigned char *input, unsigned char *output, int input_size, int output_max_size, int *input_processed,
+                                           int *output_size);
+unsigned char differential_codec(unsigned char *input, unsigned char *output, int input_size, int encode, unsigned char state);
+void          psk_modulator_u8_c(unsigned char *input, complexf *output, int input_size, int n_psk);
+complexf      psk31_interpolate_sine_cc(complexf *input, complexf *output, int input_size, int interpolation, complexf last_input);
+
 /* audio tail of the WFM graph, SURVEY 8(f) rank 1 (libcsdr.h:100-105; libcsdr.c:1081-1097, 1130-1137) */
 float deemphasis_wfm_ff(float *input, float *output, int input_size, float tau, int sample_rate, float last_output);
 void  limit_ff(float *input, float *output, int input_size, float max_amplitude);
@@ -548,6 +559,27 @@ int csdrb_dbpsk_decoder_bank_c_u8(const complexf *d_in, long in_stride, unsigned
  * to d_count[c].  d_hist_io[c] is the decoder's shift register (0 at stream start).  out_stride >= input_size.  Returns 0. */
 int csdrb_psk31_varicode_decoder_bank_u8_u8(const unsigned char *d_in, long in_stride, unsigned char *d_out, long out_stride, int channels,
                                             int input_size, const int *d_lengths, unsigned long long *d_hist_io, int *d_count, void *stream);
+
+/* BPSK31 transmit chain banks (psk31_tx.cu), one row per channel.  Row c holds d_lengths[c] <= input_size elements (d_lengths NULL: input_size
+ * each), so the encoder's d_output_size can feed the next bank's d_lengths directly.  Refusals return -1 with csdrb_last_error() set, launch
+ * nothing and leave every _io array unchanged; an empty row leaves its state or last input unchanged.  Returns 0 on success.
+ *
+ * psk31_varicode_encoder bank: psk31_varicode_encoder_u8_u8 on each row with output_max_size bits of room; the bits (one byte each, 0 or 1) go
+ * to row c of d_out, d_input_processed[c] and d_output_size[c] receive the reference's counts.  out_stride >= output_max_size. */
+int csdrb_psk31_varicode_encoder_bank_u8_u8(const unsigned char *d_in, long in_stride, unsigned char *d_out, long out_stride, int channels,
+                                            int input_size, const int *d_lengths, int output_max_size, int *d_input_processed, int *d_output_size,
+                                            void *stream);
+/* differential codec bank: differential_codec(row, encode, d_state_io[c]) per row (0 at stream start); d_state_io[c] receives the state the
+ * reference returns (in decode mode the last byte itself).  out_stride >= input_size; d_out must not alias d_in. */
+int csdrb_differential_codec_bank_u8_u8(const unsigned char *d_in, long in_stride, unsigned char *d_out, long out_stride, int channels,
+                                        int input_size, const int *d_lengths, int encode, unsigned char *d_state_io, void *stream);
+/* psk_modulator bank: one complexf per symbol byte, n_psk 1..256 (the CLI's range); the constellation contract of psk_modulator_u8_c above. */
+int csdrb_psk_modulator_bank_u8_c(const unsigned char *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int input_size,
+                                  const int *d_lengths, int n_psk, void *stream);
+/* psk31_interpolate_sine bank: psk31_interpolate_sine_cc per row, interpolation >= 1 outputs per input; d_last_io[c] is the reference's
+ * last_input (0 at stream start), replaced by the row's last input.  out_stride >= input_size * interpolation. */
+int csdrb_psk31_interpolate_sine_bank_cc(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int input_size,
+                                         const int *d_lengths, int interpolation, complexf *d_last_io, void *stream);
 
 /* RTTY receive chain banks (rtty.cu), one row per channel.
  *

@@ -47,6 +47,12 @@ torch.cuda.synchronize(); print("sanitize_smoke: all kernels ran")
 for I, T, n in ((1, 7, 999), (3, 81, 1001), (50, 401, 333), (256, 2049, 37), (5, 9001, 2000)):
     cb.fir_interpolate_bank(cplx(3, n + 1)[:, :n], I, cb.firdes_lowpass_f(T, 0.5 / I))
 ph = torch.zeros(5, device=dev); cb.fmmod_bank((torch.rand((5, 1037), device=dev) * 2 - 1) * 9, ph); cb.fmmod_bank(torch.rand((5, 31), device=dev), ph)
+# BPSK31 transmit banks at awkward sizes: rows across scan chunks, a cut encoder, odd lengths, both interpolator rate paths
+txt = torch.randint(0, 256, (3, 1031), dtype=torch.uint8, device=dev)
+cb.psk31_varicode_encoder_bank_u8_u8(txt); cb.psk31_varicode_encoder_bank_u8_u8(txt, output_max_size=777)
+cb.differential_codec_bank_u8_u8(txt, True); cb.differential_codec_bank_u8_u8(txt, False)
+cb.psk_modulator_bank_u8_c(txt, 256)
+cb.psk31_interpolate_sine_bank_cc(cplx(3, 37), 257); cb.psk31_interpolate_sine_bank_cc(cplx(2, 3), 9001)
 torch.cuda.synchronize()
 # synthesis bank: the register window at h = 1 and 8, the general path with taps in shared memory and past it, ragged warps, two CTAs of
 # channels (the second tree pass), chunks of 1 and 7 with offsets, n below one group, the streaming object
