@@ -279,6 +279,13 @@ def lib() -> C.CDLL:
     L.csdrb_bfsk_demod_bank_cf.argtypes = [vp, lg, vp, lg, it, it, vp, vp, it, vp]
     L.csdrb_fir_interpolate_bank_cc.argtypes = [vp, lg, vp, lg, it, it, it, vp, it, vp]
     L.csdrb_fmmod_bank_fc.argtypes = [vp, lg, vp, lg, it, it, vp, vp]
+    L.csdrb_gain_bank_ff.argtypes = [vp, lg, vp, lg, it, it, C.c_float, vp]
+    L.csdrb_dsb_bank_fc.argtypes = [vp, lg, vp, lg, it, it, C.c_float, vp]
+    L.csdrb_add_dcoffset_bank_cc.argtypes = [vp, lg, vp, lg, it, it, vp]
+    L.csdrb_fixed_amplitude_bank_cc.argtypes = [vp, lg, vp, lg, it, it, C.c_float, vp]
+    L.gain_ff.argtypes = [vp, vp, it, C.c_float]
+    L.add_dcoffset_cc.argtypes = [vp, vp, it]
+    L.fixed_amplitude_cc.argtypes = [vp, vp, it, C.c_float]
     L.csdrb_psk31_varicode_encoder_bank_u8_u8.argtypes = [vp, lg, vp, lg, it, it, vp, it, vp, vp, vp]
     L.csdrb_differential_codec_bank_u8_u8.argtypes = [vp, lg, vp, lg, it, it, vp, it, vp, vp]
     L.csdrb_psk_modulator_bank_u8_c.argtypes = [vp, lg, vp, lg, it, it, vp, it, vp]
@@ -1246,6 +1253,51 @@ def fmmod_bank(x, phase=None):
         return out[:, :0]
     _check(lib().csdrb_fmmod_bank_fc(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, phase.data_ptr(), _stream()), "fmmod_bank")
     return out[:, :n]
+
+
+def _mod_rows(x, dtype, what):
+    import torch
+    assert x.dtype == dtype and x.is_cuda and x.dim() == 2 and x.stride(1) == 1, f"{what}: [C, N] {dtype} CUDA rows"
+    return x.shape
+
+
+def gain_bank(x, gain: float, out=None):
+    """gain_ff per row (libcsdr.c:1139): x [C, N] float32 CUDA -> [C, N] float32 gain*x, bit for bit the reference build.  out may be x (in place)."""
+    import torch
+    ch, n = _mod_rows(x, torch.float32, "gain_bank")
+    out = torch.empty((ch, n), dtype=torch.float32, device=x.device) if out is None else out
+    _check(lib().csdrb_gain_bank_ff(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, gain, _stream()), "gain_bank")
+    return out
+
+
+def dsb_bank(x, q_value: float = 0.0):
+    """the dsb_fc command per row (csdr.c:2084-2102): x [C, N] float32 CUDA -> [C, N] complex64 (x, q_value)"""
+    import torch
+    ch, n = _mod_rows(x, torch.float32, "dsb_bank")
+    out = torch.empty((ch, n), dtype=torch.complex64, device=x.device)
+    _check(lib().csdrb_dsb_bank_fc(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, q_value, _stream()), "dsb_bank")
+    return out
+
+
+def add_dcoffset_bank(x, out=None):
+    """add_dcoffset_cc per row (libcsdr.c:1174) as the reference build runs it: x [C, N] complex64 CUDA -> [C, N] complex64
+    ((i + 1)*0.5, q*0.5) in float, bit for bit.  out may be x (in place)."""
+    import torch
+    ch, n = _mod_rows(x, torch.complex64, "add_dcoffset_bank")
+    out = torch.empty((ch, n), dtype=torch.complex64, device=x.device) if out is None else out
+    _check(lib().csdrb_add_dcoffset_bank_cc(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, _stream()), "add_dcoffset_bank")
+    return out
+
+
+def fixed_amplitude_bank(x, new_amplitude: float, out=None):
+    """fixed_amplitude_cc per row (libcsdr.c:1194): x [C, N] complex64 CUDA -> [C, N] complex64 x*A/|x| (0 where |x| is not positive), the
+    source's sqrt and division correctly rounded (DESIGN.md section 7).  out may be x (in place)."""
+    import torch
+    ch, n = _mod_rows(x, torch.complex64, "fixed_amplitude_bank")
+    out = torch.empty((ch, n), dtype=torch.complex64, device=x.device) if out is None else out
+    _check(lib().csdrb_fixed_amplitude_bank_cc(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, new_amplitude, _stream()),
+           "fixed_amplitude_bank")
+    return out
 
 
 def _u8_rows(x):

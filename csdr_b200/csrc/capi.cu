@@ -566,6 +566,34 @@ int csdrb_fmmod_bank_fc(const float* d_in, long in_stride, complexf* d_out, long
     return rc < 0 ? rc : counted(rc, channels > 0 && n > 0 ? 1 : 0);
 }
 
+// amplitude modulator banks (modulate.cu; libcsdr.c:1139-1142, 1174-1178, 1194-1208, csdr.c:2084-2102): the launcher returns its launches
+int csdrb_gain_bank_ff(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int n, float gain, void* stream)
+{
+    const int rc = launch_gain_bank_ff(d_in, in_stride, d_out, out_stride, channels, n, gain, S(stream));
+    return rc < 0 ? rc : counted(n, rc);
+}
+
+int csdrb_dsb_bank_fc(const float* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int n, float q_value, void* stream)
+{
+    const int rc = launch_dsb_bank_fc(d_in, in_stride, reinterpret_cast<float2*>(d_out), out_stride, channels, n, q_value, S(stream));
+    return rc < 0 ? rc : counted(n, rc);
+}
+
+int csdrb_add_dcoffset_bank_cc(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int n, void* stream)
+{
+    const int rc = launch_add_dcoffset_bank_cc(reinterpret_cast<const float2*>(d_in), in_stride, reinterpret_cast<float2*>(d_out), out_stride, channels,
+                                               n, S(stream));
+    return rc < 0 ? rc : counted(n, rc);
+}
+
+int csdrb_fixed_amplitude_bank_cc(const complexf* d_in, long in_stride, complexf* d_out, long out_stride, int channels, int n, float new_amplitude,
+                                  void* stream)
+{
+    const int rc = launch_fixed_amplitude_bank_cc(reinterpret_cast<const float2*>(d_in), in_stride, reinterpret_cast<float2*>(d_out), out_stride,
+                                                  channels, n, new_amplitude, S(stream));
+    return rc < 0 ? rc : counted(n, rc);
+}
+
 // synthesis bank (synth.cu): fir_interpolate_cc | shift_addition_cc per channel, summed over the channels in a fixed pairwise tree
 size_t csdrb_synth_bank_scratch_bytes(int channels, int input_size, int interpolation, int taps_length, int chunk, int offset)
 {

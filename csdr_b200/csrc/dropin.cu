@@ -717,6 +717,26 @@ float fmmod_fc(float* input, complexf* output, int input_size, float last_phase)
     return last_phase;
 }
 
+// ---- the other modulators (libcsdr.c:1139-1142, 1174-1178, 1194-1208): one-row banks; input == output is staged like any other call ----------
+void gain_ff(float* input, float* output, int input_size, float gain)
+{
+    elementwise("gain_ff", input, output, input_size,
+                [=](const float* in, float* out, long n, void* s) { return csdrb_gain_bank_ff(in, n, out, n, 1, (int)n, gain, s); });
+}
+
+void add_dcoffset_cc(complexf* input, complexf* output, int input_size)
+{
+    elementwise("add_dcoffset_cc", input, output, input_size,
+                [](const complexf* in, complexf* out, long n, void* s) { return csdrb_add_dcoffset_bank_cc(in, n, out, n, 1, (int)n, s); });
+}
+
+void fixed_amplitude_cc(complexf* input, complexf* output, int input_size, float new_amplitude)
+{
+    elementwise("fixed_amplitude_cc", input, output, input_size, [=](const complexf* in, complexf* out, long n, void* s) {
+        return csdrb_fixed_amplitude_bank_cc(in, n, out, n, 1, (int)n, new_amplitude, s);
+    });
+}
+
 // ---- BPSK31 transmit chain (libcsdr.c:1551-1575, 1828-1843, 1772-1782, 1793-1808) ------------------------------------------------
 void psk31_varicode_encoder_u8_u8(unsigned char* input, unsigned char* output, int input_size, int output_max_size, int* input_processed,
                                   int* output_size)

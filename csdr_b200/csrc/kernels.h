@@ -189,6 +189,12 @@ int launch_spectrum_bank_f(const float* d_in, long in_stride, int rows, long n, 
 int launch_fir_interpolate_bank_cc(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n, int interpolation,
                                    const float* d_taps, int taps_length, cudaStream_t st);
 int launch_fmmod_bank_fc(const float* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n, float* d_phase_io, cudaStream_t st);
+// modulate.cu: gain_ff, dsb_fc, add_dcoffset_cc and fixed_amplitude_cc rows; each returns the launches it made (0 or 1), -1 for bad arguments
+int launch_gain_bank_ff(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int n, float gain, cudaStream_t st);
+int launch_dsb_bank_fc(const float* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n, float q_value, cudaStream_t st);
+int launch_add_dcoffset_bank_cc(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n, cudaStream_t st);
+int launch_fixed_amplitude_bank_cc(const float2* d_in, long in_stride, float2* d_out, long out_stride, int channels, int n, float amplitude,
+                                   cudaStream_t st);
 
 // synthesis bank, synth.cu: C channels of fir_interpolate_cc | shift_addition_cc summed in a fixed pairwise tree over the channel index into one
 // wideband row.  Returns G*I outputs (< 0 refused); *launches gets the kernels it launched

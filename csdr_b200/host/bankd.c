@@ -82,6 +82,7 @@
  */
 #define _GNU_SOURCE
 #include "csdr_b200.h"
+#include "ssb_filter.h"
 
 #include <errno.h>
 #include <fcntl.h>
@@ -369,7 +370,6 @@ static void raw_tail_push(raw_tail_t *t, channel_t *chan, int n, void *stream)
  *   bb   : [C][bs] complexf : [remainder (< unit samples) | new baseband]   unit = 1024 (am) or the overlap-add input size (usb/lsb)
  *   mid  : [C][bs] float (am: DC-blocked envelope) or complexf (usb/lsb: filtered baseband) over the whole units
  *   pcm  : [C][whole] s16 */
-#define SSB_BW 0.05f                                      /* bandpass_fir_fft_cc transition bandwidth of README.md:110 */
 
 typedef struct {
     int C, unit, have, fft_size;                                  /* fft_size 0: am, else the usb/lsb bandpass */
@@ -391,22 +391,11 @@ static void bb_tail_init(bb_tail_t *t, int C, int out_cap, float limit, float ag
     const csdrb_agc_params_t p = {agc_ref, 0.01f, 0.0001f, 65536.0f, 200, 0, 0.999f, 1024};
     t->agc = p;
     t->unit = 1024;
-    if (band) {                                                      /* bandpass_fir_fft_cc geometry, csdr.c:1822-1831 */
-        const int T = firdes_filter_len(SSB_BW);
-        int N = next_pow2(T);
-        if (N - T < 200) N <<= 1;
-        t->fft_size = N; t->unit = N - T + 1;
-        complexf *h_taps = calloc((size_t)N, sizeof(complexf));
-        if (!h_taps) die("out of memory");
-        firdes_bandpass_c(h_taps, T, band[0], band[1], WINDOW_HAMMING);
-        complexf *d_taps = csdrb_device_alloc(sizeof(complexf) * (size_t)N);
-        t->d_taps_fft = csdrb_device_alloc(sizeof(complexf) * (size_t)N);
-        t->d_ola_tail = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)N);   /* zero-filled: the overlap tail is zero at stream start (csdr.c:1860) */
-        if (!d_taps || !t->d_taps_fft || !t->d_ola_tail) die("out of memory");
-        OK(csdrb_copy_h2d(d_taps, h_taps, sizeof(complexf) * (size_t)N, stream));
-        OK(csdrb_fft_c2c_batch(d_taps, N, t->d_taps_fft, N, N, 1, 0, stream));       /* the forward FFT of the zero-padded taps (csdr.c:1869) */
-        OK(csdrb_stream_synchronize(stream));
-        csdrb_device_free(d_taps); free(h_taps);
+    if (band) {                                                      /* bandpass_fir_fft_cc geometry and taps, ssb_filter.h */
+        t->d_taps_fft = ssb_taps_fft(band[0], band[1], &t->fft_size, &t->unit, stream);
+        if (!t->d_taps_fft) die("SSB filter taps failed");
+        t->d_ola_tail = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->fft_size);   /* zero-filled: the overlap tail is zero at stream start (csdr.c:1860) */
+        if (!t->d_ola_tail) die("out of memory");
     }
     t->bs = ((long)t->unit + out_cap + 3) & ~3L;
     t->d_bb = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)t->bs);

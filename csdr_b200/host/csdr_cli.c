@@ -1034,6 +1034,57 @@ static int cmd_fmmod_fc(int argc, char **argv)                               /* 
     return map_blocks(sizeof(float), sizeof(complexf), block, 0, fmmod_step, &phase);
 }
 
+/* ---- the amplitude modulators (csdr.c:658-671, 2084-2102, 2129-2140, 2156-2172): per-block maps of the reference's framing ----------------- */
+static void gain_step(void *in, void *out, void *gain) { gain_ff(in, out, block, *(float *)gain); }
+
+static int cmd_gain_ff(int argc, char **argv)
+{
+    if (argc <= 2) return complain("need required parameter (gain)");
+    float gain = 0.f; sscanf(argv[2], "%g", &gain);
+    if (!announce_block(open_block())) return -2;
+    return map_blocks(sizeof(float), sizeof(float), block, 0, gain_step, &gain);
+}
+
+/* dsb_fc has no library function: the dsb bank on device copies of the block */
+typedef struct { float q_value; float *d_in; complexf *d_out; } dsb_state_t;
+static void dsb_step(void *in, void *out, void *s)
+{
+    dsb_state_t *d = s;
+    if (csdrb_copy_h2d(d->d_in, in, sizeof(float) * (size_t)block, NULL) < 0 || csdrb_dsb_bank_fc(d->d_in, block, d->d_out, block, 1, block, d->q_value, NULL) < 0 ||
+        csdrb_copy_d2h(out, d->d_out, sizeof(complexf) * (size_t)block, NULL) < 0 || csdrb_stream_synchronize(NULL) < 0) {
+        who(); fprintf(stderr, "%s\n", csdrb_last_error()); exit(-2);
+    }
+}
+
+static int cmd_dsb_fc(int argc, char **argv)
+{
+    dsb_state_t d = {0.f, NULL, NULL};
+    if (argc >= 3) sscanf(argv[2], "%g", &d.q_value);
+    if (!announce_block(open_block())) return -2;
+    d.d_in = csdrb_device_alloc(sizeof(float) * (size_t)block); d.d_out = csdrb_device_alloc(sizeof(complexf) * (size_t)block);
+    if (!d.d_in || !d.d_out) { who(); fprintf(stderr, "%s\n", csdrb_last_error()); return -2; }
+    return map_blocks(sizeof(float), sizeof(complexf), block, 0, dsb_step, &d);
+}
+
+static void dcoffset_step(void *in, void *out, void *state) { (void)state; add_dcoffset_cc(in, out, block); }
+
+static int cmd_add_dcoffset_cc(int argc, char **argv)
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    return map_blocks(sizeof(complexf), sizeof(complexf), block, 0, dcoffset_step, NULL);
+}
+
+static void fixed_amplitude_step(void *in, void *out, void *a) { fixed_amplitude_cc(in, out, block, *(float *)a); }
+
+static int cmd_fixed_amplitude_cc(int argc, char **argv)
+{
+    if (argc <= 2) return complain("need required parameter (new_amplitude)");
+    float new_amplitude = 0.f; sscanf(argv[2], "%g", &new_amplitude);
+    if (!announce_block(open_block())) return -2;
+    return map_blocks(sizeof(complexf), sizeof(complexf), block, 0, fixed_amplitude_step, &new_amplitude);
+}
+
 /* ---- BPSK31 transmit chain (csdr.c:2684-2701, 2727-2746, 2780-2800, 2816-2833) ---------------------------------------------------
  * psk31_varicode_encoder_u8_u8 | differential_encoder_u8_u8 | psk_modulator_u8_c 2 | psk31_interpolate_sine_cc <sps>, the pipe of the reference's
  * BER harness.  The codec, the modulator and the interpolator are per-block maps with their state carried; the next process is told the block
@@ -1146,6 +1197,10 @@ static const struct { const char *name; int (*run)(int, char **); const char *sy
     {"fastddc_inv_cc", cmd_fastddc_inv_cc, "fastddc_inv_cc <shift_rate> <decimation> [transition_bw [window]] | --fifo <fifo_path> ... | --fd <fd> ..."},
     {"fir_interpolate_cc", cmd_fir_interpolate_cc, "fir_interpolate_cc <interpolation_factor> [transition_bw [window]]"},
     {"fmmod_fc", cmd_fmmod_fc, "fmmod_fc"},
+    {"gain_ff", cmd_gain_ff, "gain_ff <gain>"},
+    {"dsb_fc", cmd_dsb_fc, "dsb_fc [q_value]"},
+    {"add_dcoffset_cc", cmd_add_dcoffset_cc, "add_dcoffset_cc"},
+    {"fixed_amplitude_cc", cmd_fixed_amplitude_cc, "fixed_amplitude_cc <new_amplitude>"},
     {"psk31_varicode_encoder_u8_u8", cmd_psk31_varicode_encoder_u8_u8, "psk31_varicode_encoder_u8_u8"},
     {"differential_encoder_u8_u8", cmd_differential_encoder_u8_u8, "differential_encoder_u8_u8"},
     {"differential_decoder_u8_u8", cmd_differential_decoder_u8_u8, "differential_decoder_u8_u8"},

@@ -144,6 +144,12 @@ int  bfsk_demod_cf(complexf *input, float *output, int input_size, complexf *mar
  * ulp of the build's sincosf (DESIGN.md section 7). */
 int   fir_interpolate_cc(complexf *input, complexf *output, int input_size, int interpolation, float *taps, int taps_length);
 float fmmod_fc(float *input, complexf *output, int input_size, float last_phase);
+/* the rest of the library's modulators (libcsdr.c:1139, 1174, 1194): gain_ff and add_dcoffset_cc are bit for bit the reference build;
+ * fixed_amplitude_cc is the source's sqrt/division form correctly rounded, within a float64 bound of the build (DESIGN.md section 7).
+ * input == output is allowed. */
+void  gain_ff(float *input, float *output, int input_size, float gain);
+void  add_dcoffset_cc(complexf *input, complexf *output, int input_size);
+void  fixed_amplitude_cc(complexf *input, complexf *output, int input_size, float new_amplitude);
 
 /* BPSK31 transmit chain (libcsdr.h:343-347; libcsdr.c:1551-1575, 1772-1808, 1828-1843), the reference's own pipe
  * psk31_varicode_encoder_u8_u8 | differential_encoder_u8_u8 | psk_modulator_u8_c 2 | psk31_interpolate_sine_cc <sps>.  The encoder, the
@@ -625,6 +631,24 @@ int csdrb_bfsk_demod_bank_cf(const complexf *d_in, long in_stride, float *d_out,
 int csdrb_fir_interpolate_bank_cc(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int n, int interpolation,
                                   const float *d_taps, int taps_length, void *stream);
 int csdrb_fmmod_bank_fc(const float *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int n, float *d_phase_io, void *stream);
+
+/* amplitude modulator banks (modulate.cu), one row per channel, row c of the input at d_in + c*in_stride and of the output at d_out + c*out_stride
+ * (strides in elements).  With fmmod_bank_fc and bandpass_fir_fft_bank_cc they make the reference's transmit pipes: AM `gain_ff G | dsb_fc |
+ * add_dcoffset_cc`, DSB `gain_ff G | dsb_fc`, USB/LSB `gain_ff G | dsb_fc | bandpass_fir_fft_cc 0 0.1 0.05` (-0.1 0 0.05), FM `gain_ff G | fmmod_fc`.
+ *   gain_bank_ff: gain_ff (libcsdr.c:1139), y = gain*x, bit for bit the reference build.
+ *   dsb_bank_fc: the dsb_fc command's loop (csdr.c:2084-2102), y = (x, q_value): a real signal as the I of a complex one.
+ *   add_dcoffset_bank_cc: add_dcoffset_cc (libcsdr.c:1174) as the -ffast-math build runs it, y = ((i + 1.0f)*0.5f, q*0.5f) in float, bit for bit.
+ *   fixed_amplitude_bank_cc: fixed_amplitude_cc (libcsdr.c:1194), the source's expression correctly rounded: s = i*i + q*q, a = sqrt(s),
+ *     g = a > 0 ? new_amplitude/a : 0, y = (i*g, q*g).  The build's rsqrtss seed differs between CPUs; both lie within a float64 bound of
+ *     new_amplitude*x/|x| (DESIGN.md section 7).
+ * Each returns n; -1 (csdrb_last_error() set, nothing launched) for n < 0, channels < 0, a stride below n, a null pointer with work to do, a
+ * misaligned one (complexf 8 bytes, float 4) or d_in == d_out with unequal strides (gain, add_dcoffset, fixed_amplitude: in place with equal
+ * strides is allowed; dsb_fc is never in place). */
+int csdrb_gain_bank_ff(const float *d_in, long in_stride, float *d_out, long out_stride, int channels, int n, float gain, void *stream);
+int csdrb_dsb_bank_fc(const float *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int n, float q_value, void *stream);
+int csdrb_add_dcoffset_bank_cc(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int n, void *stream);
+int csdrb_fixed_amplitude_bank_cc(const complexf *d_in, long in_stride, complexf *d_out, long out_stride, int channels, int n, float new_amplitude,
+                                  void *stream);
 
 /* Synthesis bank (synth.cu): C baseband channels into ONE wideband stream,
  *     y = sum over c of shift_addition_cc(fir_interpolate_cc(x_c, I, taps), rate_c)

@@ -61,3 +61,11 @@ for ch, I, T, n, chunk, off in ((1, 1, 1, 300, 7, 3), (33, 50, 401, 40, 1024, 17
     cb.synth_bank(cplx(ch, n + 1)[:, :n], np.linspace(-0.45, 0.45, ch), I, rng.uniform(-1, 1, T).astype(np.float32), chunk=chunk, offset=off)
 sb = cb.SynthBank(np.linspace(-0.4, 0.4, 40), 50, cb.firdes_lowpass_f(401, 0.01)); w = cplx(40, 3000); sb.process(w[:, :1000].contiguous()); sb.process(w[:, 992:2500].contiguous()); sb.close()
 torch.cuda.synchronize()
+# amplitude modulator banks: 128-bit rows, rows off 16-byte alignment (odd strides, offset starts), ragged tails, in place
+r = (torch.rand((3, 1037), device=dev) * 2 - 1)
+cb.gain_bank(r[:, :1035], 0.7); cb.gain_bank(r[:, 1:1030], 2.0); cb.gain_bank(r, 0.5, out=r)
+cb.dsb_bank(r[:, :1033], 0.1); cb.dsb_bank(r[:, 3:], 0.0)
+z = cplx(3, 1037)
+cb.add_dcoffset_bank(z[:, :1035]); cb.add_dcoffset_bank(z[:, 1:]); cb.add_dcoffset_bank(z, out=z)
+cb.fixed_amplitude_bank(z[:, :1031], 2.0); cb.fixed_amplitude_bank(z[:, 1:], 1.0); cb.fixed_amplitude_bank(z, 0.5, out=z)
+torch.cuda.synchronize()
