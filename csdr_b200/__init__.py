@@ -142,6 +142,10 @@ def lib() -> C.CDLL:
     L.csdrb_convert_u8_f.argtypes = [vp, vp, lg, vp]
     L.csdrb_convert_s16_f.argtypes = [vp, vp, lg, vp]
     L.csdrb_convert_f_s16.argtypes = [vp, vp, lg, vp]
+    for name in ("csdrb_convert_s8_f", "csdrb_convert_f_s8", "csdrb_convert_f_u8"):
+        getattr(L, name).argtypes = [vp, vp, lg, vp]
+    L.csdrb_convert_s24_f.argtypes = [vp, vp, lg, it, vp]
+    L.csdrb_convert_f_s24.argtypes = [vp, vp, lg, it, vp]
     L.csdrb_fir_decimate_bank_cc.argtypes = [vp, lg, vp, lg, it, it, it, C.POINTER(C.c_float), it, it, vp]
     L.csdrb_fmdemod_quadri_bank_cf.argtypes = [vp, lg, vp, lg, it, it, vp, vp, vp]
     L.csdrb_stream_synchronize.argtypes = [vp]
@@ -261,6 +265,11 @@ def lib() -> C.CDLL:
     L.convert_u8_f.argtypes = [vp, vp, it]
     L.convert_s16_f.argtypes = [vp, vp, it]
     L.convert_f_s16.argtypes = [vp, vp, it]
+    L.convert_s8_f.argtypes = [vp, vp, it]
+    L.convert_f_s8.argtypes = [vp, vp, it]
+    L.convert_f_u8.argtypes = [vp, vp, it]
+    L.convert_s24_f.argtypes = [vp, vp, it, it]
+    L.convert_f_s24.argtypes = [vp, vp, it, it]
     L.fir_decimate_cc.argtypes = [vp, vp, it, it, C.POINTER(C.c_float), it]
     L.fmdemod_quadri_cf.argtypes = [vp, vp, it, vp, _CF]; L.fmdemod_quadri_cf.restype = _CF
     L.csdrb_simple_agc_bank_cc.argtypes = [vp, lg, vp, lg, it, it, C.c_float, C.c_float, C.c_float, vp, vp]
@@ -398,6 +407,54 @@ def convert_f_s16(x, out=None):
     assert x.dtype == torch.float32 and x.is_cuda and x.is_contiguous()
     out = torch.empty(x.shape, dtype=torch.int16, device=x.device) if out is None else out
     _check(lib().csdrb_convert_f_s16(x.data_ptr(), out.data_ptr(), x.numel(), _stream()), "convert_f_s16")
+    return out
+
+
+def convert_s8_f(x, out=None):
+    """HackRF-style signed 8-bit values -> float32 of the same shape: (float)b * (1.0f/127.0f), as the reference build computes it."""
+    import torch
+    assert x.dtype == torch.int8 and x.is_cuda and x.is_contiguous()
+    out = torch.empty(x.shape, dtype=torch.float32, device=x.device) if out is None else out
+    _check(lib().csdrb_convert_s8_f(x.data_ptr(), out.data_ptr(), x.numel(), _stream()), "convert_s8_f")
+    return out
+
+
+def convert_f_s8(x, out=None):
+    """float32 -> int8 of the same shape: x*127 truncated, the low byte kept (out of range wraps, NaN/Inf give 0)."""
+    import torch
+    assert x.dtype == torch.float32 and x.is_cuda and x.is_contiguous()
+    out = torch.empty(x.shape, dtype=torch.int8, device=x.device) if out is None else out
+    _check(lib().csdrb_convert_f_s8(x.data_ptr(), out.data_ptr(), x.numel(), _stream()), "convert_f_s8")
+    return out
+
+
+def convert_f_u8(x, out=None):
+    """float32 -> uint8 of the same shape: x*255*0.5 + 128 truncated, the low byte kept (out of range wraps, NaN/Inf give 0)."""
+    import torch
+    assert x.dtype == torch.float32 and x.is_cuda and x.is_contiguous()
+    out = torch.empty(x.shape, dtype=torch.uint8, device=x.device) if out is None else out
+    _check(lib().csdrb_convert_f_u8(x.data_ptr(), out.data_ptr(), x.numel(), _stream()), "convert_f_u8")
+    return out
+
+
+def convert_s24_f(x, bigendian=False, out=None):
+    """24-bit samples, a uint8 tensor of 3n bytes -> n float32.  ``bigendian`` is the reference's flag: False reads the most significant
+    byte first, True the least significant byte first (on x86 the flag does the opposite of its name)."""
+    import torch
+    assert x.dtype == torch.uint8 and x.is_cuda and x.is_contiguous() and x.numel() % 3 == 0
+    n = x.numel() // 3
+    out = torch.empty(n, dtype=torch.float32, device=x.device) if out is None else out
+    _check(lib().csdrb_convert_s24_f(x.data_ptr(), out.data_ptr(), n, int(bool(bigendian)), _stream()), "convert_s24_f")
+    return out
+
+
+def convert_f_s24(x, bigendian=False, out=None):
+    """n float32 -> 3n uint8 bytes of 24-bit samples: x*8388607 truncated, the low three bytes kept, in the order ``bigendian`` gives (as in
+    convert_s24_f)."""
+    import torch
+    assert x.dtype == torch.float32 and x.is_cuda and x.is_contiguous()
+    out = torch.empty(3 * x.numel(), dtype=torch.uint8, device=x.device) if out is None else out
+    _check(lib().csdrb_convert_f_s24(x.data_ptr(), out.data_ptr(), x.numel(), int(bool(bigendian)), _stream()), "convert_f_s24")
     return out
 
 
@@ -560,6 +617,31 @@ class libcsdr:
     def convert_f_s16(x):
         x = np.ascontiguousarray(x, np.float32); y = np.empty(x.size, np.int16)
         lib().convert_f_s16(x.ctypes.data, y.ctypes.data, x.size); return y
+
+    @staticmethod
+    def convert_s8_f(x):
+        x = np.ascontiguousarray(x, np.int8); y = np.empty(x.size, np.float32)
+        lib().convert_s8_f(x.ctypes.data, y.ctypes.data, x.size); return y
+
+    @staticmethod
+    def convert_f_s8(x):
+        x = np.ascontiguousarray(x, np.float32); y = np.empty(x.size, np.int8)
+        lib().convert_f_s8(x.ctypes.data, y.ctypes.data, x.size); return y
+
+    @staticmethod
+    def convert_f_u8(x):
+        x = np.ascontiguousarray(x, np.float32); y = np.empty(x.size, np.uint8)
+        lib().convert_f_u8(x.ctypes.data, y.ctypes.data, x.size); return y
+
+    @staticmethod
+    def convert_s24_f(x, bigendian=False):
+        x = np.ascontiguousarray(x, np.uint8); y = np.empty(x.size // 3, np.float32)
+        lib().convert_s24_f(x.ctypes.data, y.ctypes.data, y.size, int(bool(bigendian))); return y
+
+    @staticmethod
+    def convert_f_s24(x, bigendian=False):
+        x = np.ascontiguousarray(x, np.float32); y = np.empty(3 * x.size, np.uint8)
+        lib().convert_f_s24(x.ctypes.data, y.ctypes.data, x.size, int(bool(bigendian))); return y
 
     @staticmethod
     def fir_decimate_cc(x, decimation, taps):

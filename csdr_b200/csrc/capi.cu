@@ -86,6 +86,36 @@ int csdrb_convert_f_s16(const float* d_in, short* d_out, long n, void* stream)
 {
     return null_io(d_in, d_out, "convert_f_s16") ? -1 : counted(launch_convert_f_s16(d_in, d_out, n, S(stream)));
 }
+// the other sample formats: byte buffers at any address, float buffers 4-byte aligned; a null pointer, a misaligned float buffer or n < 0 is
+// refused before anything is launched
+static inline bool bad_io(const void* in, const void* out, const float* floats, long n, const char* who)
+{
+    if (null_io(in, out, who)) return true;
+    if (misaligned(floats, 4)) { set_error("%s: float buffer not 4-byte aligned", who); return true; }
+    if (n >= 0) return false;
+    set_error("%s: negative count %ld", who, n);
+    return true;
+}
+int csdrb_convert_s8_f(const signed char* d_in, float* d_out, long n, void* stream)
+{
+    return bad_io(d_in, d_out, d_out, n, "convert_s8_f") ? -1 : counted(launch_convert_s8_f(reinterpret_cast<const unsigned char*>(d_in), d_out, n, S(stream)), n > 0);
+}
+int csdrb_convert_f_s8(const float* d_in, signed char* d_out, long n, void* stream)
+{
+    return bad_io(d_in, d_out, d_in, n, "convert_f_s8") ? -1 : counted(launch_convert_f_s8(d_in, reinterpret_cast<unsigned char*>(d_out), n, S(stream)), n > 0);
+}
+int csdrb_convert_f_u8(const float* d_in, unsigned char* d_out, long n, void* stream)
+{
+    return bad_io(d_in, d_out, d_in, n, "convert_f_u8") ? -1 : counted(launch_convert_f_u8(d_in, d_out, n, S(stream)), n > 0);
+}
+int csdrb_convert_s24_f(const unsigned char* d_in, float* d_out, long n, int bigendian, void* stream)
+{
+    return bad_io(d_in, d_out, d_out, n, "convert_s24_f") ? -1 : counted(launch_convert_s24_f(d_in, d_out, n, bigendian, S(stream)), n > 0);
+}
+int csdrb_convert_f_s24(const float* d_in, unsigned char* d_out, long n, int bigendian, void* stream)
+{
+    return bad_io(d_in, d_out, d_in, n, "convert_f_s24") ? -1 : counted(launch_convert_f_s24(d_in, d_out, n, bigendian, S(stream)), n > 0);
+}
 
 int csdrb_fir_bank_variants(void) { return fir_bank_variant_count(); }
 

@@ -143,14 +143,22 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 
 #endif  // CSDRB_HOST_EMULATION
 
+// ---- x86's truncating conversions to int32, cvttss2si (float) and cvttsd2si (double) --------------------------------------------
+// Toward zero; NaN, +-Inf and values outside the int32 range give the "integer indefinite" INT_MIN.  The reference build converts every float
+// to a narrower integer this way and stores the low bytes, so out of range wraps and INT_MIN stores zeros.  __float2int_rz saturates instead
+// (+Inf would give INT_MAX), hence the explicit range check.
+__device__ __forceinline__ int x86_trunc_i32(float s)
+{
+    return (s >= 2147483648.0f || s < -2147483648.0f || s != s) ? (-2147483647 - 1) : __float2int_rz(s);
+}
+__device__ __forceinline__ int x86_trunc_i32(double t)
+{
+    return (t >= 2147483648.0 || t <= -2147483649.0 || t != t) ? (-2147483647 - 1) : (int)t;
+}
+
 // ---- convert_f_s16 of one value (libcsdr.c:2390-2398): float multiply by 32767, truncate toward zero, keep the low 16 bits of the int32 ----
 // (what cvttss2si + a 16-bit store do on the reference's x86 build; out-of-range / NaN -> INT_MIN -> 0)
-__device__ __forceinline__ unsigned f_to_s16_bits(float x)
-{
-    const float s = __fmul_rn(x, 32767.0f);
-    const int w = (s >= 2147483648.0f || s < -2147483648.0f || s != s) ? (-2147483647 - 1) : __float2int_rz(s);
-    return (unsigned)w & 0xffffu;
-}
+__device__ __forceinline__ unsigned f_to_s16_bits(float x) { return (unsigned)x86_trunc_i32(__fmul_rn(x, 32767.0f)) & 0xffffu; }
 
 // ---- the reference's complex rotation: two rounded products, then a rounded difference / sum ----------------------------
 //   (p.x*v.x - p.y*v.y, p.y*v.x + p.x*v.y)   e.g. libcsdr_gpl.c:39-45: the sample times the phasor, and the phasor recursion with v = (cosd, sind)

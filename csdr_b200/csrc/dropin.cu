@@ -98,16 +98,17 @@ private:
     size_t next_ = 0;
 };
 
-// the drop-ins that turn n input elements into n output elements with one Part B call f(d_in, d_out, n, stream)
+// the drop-ins that turn n values into n values with one Part B call f(d_in, d_out, n, stream); a value is in_items In elements on the way in
+// and out_items Out elements on the way out (3 bytes of s24)
 template <class In, class Out, class F>
-void elementwise(const char* who, const In* input, Out* output, int n, F f)
+void elementwise(const char* who, const In* input, Out* output, int n, F f, int in_items = 1, int out_items = 1)
 {
     if (n <= 0) return;
     Staging st(who);
-    const In* d_in = st.up(input, n);
-    Out* d_out = st.alloc<Out>(n);
+    const In* d_in = st.up(input, (long)n * in_items);
+    Out* d_out = st.alloc<Out>((long)n * out_items);
     st.check(f(d_in, d_out, n, st.stream()));
-    st.get(output, d_out, n);
+    st.get(output, d_out, (long)n * out_items);
     st.sync();
 }
 
@@ -127,6 +128,19 @@ void convert_s16_f(short* input, float* output, int input_size) { elementwise("c
 void convert_i16_f(short* input, float* output, int input_size) { convert_s16_f(input, output, input_size); }
 void convert_f_s16(float* input, short* output, int input_size) { elementwise("convert_f_s16", input, output, input_size, csdrb_convert_f_s16); }
 void convert_f_i16(float* input, short* output, int input_size) { convert_f_s16(input, output, input_size); }
+void convert_s8_f(signed char* input, float* output, int input_size) { elementwise("convert_s8_f", input, output, input_size, csdrb_convert_s8_f); }
+void convert_f_s8(float* input, signed char* output, int input_size) { elementwise("convert_f_s8", input, output, input_size, csdrb_convert_f_s8); }
+void convert_f_u8(float* input, unsigned char* output, int input_size) { elementwise("convert_f_u8", input, output, input_size, csdrb_convert_f_u8); }
+void convert_f_s24(float* input, unsigned char* output, int input_size, int bigendian)
+{
+    elementwise("convert_f_s24", input, output, input_size,
+                [bigendian](const float* d_in, unsigned char* d_out, long n, void* s) { return csdrb_convert_f_s24(d_in, d_out, n, bigendian, s); }, 1, 3);
+}
+void convert_s24_f(unsigned char* input, float* output, int input_size, int bigendian)
+{
+    elementwise("convert_s24_f", input, output, input_size,
+                [bigendian](const unsigned char* d_in, float* d_out, long n, void* s) { return csdrb_convert_s24_f(d_in, d_out, n, bigendian, s); }, 3, 1);
+}
 
 int fir_decimate_cc(complexf* input, complexf* output, int input_size, int decimation, float* taps, int taps_length)
 {

@@ -1,11 +1,11 @@
 // elementwise.cu -- K1 sample-format conversions and K4 fmdemod_quadri_cf.
 //
-// K1 replaces convert_u8_f / convert_s16_f / convert_f_s16 (libcsdr.c:2363-2366, 2373-2376, 2390-2398).
+// K1 replaces convert_u8_f / convert_s16_f / convert_f_s16 (libcsdr.c:2363-2366, 2373-2376, 2390-2398), and the other sample formats
+// convert_s8_f / convert_f_s8 / convert_f_u8 / convert_s24_f / convert_f_s24 (libcsdr.c:2368-2437).
 // K4 replaces fmdemod_quadri_cf (libcsdr.c:1040-1071) for C channels per launch.
 // All are pure streaming kernels: 128-bit global accesses, grid-stride, nothing staged.
 #include "common.cuh"
 #include "kernels.h"
-#include <limits.h>
 
 namespace csdrb {
 
@@ -81,6 +81,122 @@ __global__ void __launch_bounds__(256) convert_f_s16_kernel(const float* __restr
     for (long i = nvec * 8 + (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) out[i] = (short)f_to_s16_bits(in[i]);
 }
 
+// ---- the other sample formats: convert_s8_f, convert_f_s8, convert_f_u8, convert_s24_f, convert_f_s24 (libcsdr.c:2368-2437) -------------
+// The arithmetic of the reference's -O3 -ffast-math x86 build, value for value:
+//   s8 -> f32   (float)b * (1.0f/127.0f): the build multiplies by the float-rounded reciprocal of SCHAR_MAX instead of dividing
+//   f32 -> s8   x * 127.0f, truncated as cvttss2si does, low byte
+//   f32 -> u8   (double)(x * 255.0f) * 0.5 + 128.0 (float product, double sum), truncated as cvttsd2si does, low byte
+//   f32 -> s24  x * 8388607.0f (INT_MAX >> 8), truncated as cvttss2si does, low three bytes
+//   s24 -> f32  the three bytes as the top of an int32 (exact as a float) times the build's constant 0x30000001 = (float)(1/2147483392.0f),
+//               2147483392 being (float)(INT_MAX - 256)
+// s24 byte order: the reference's `bigendian` flag names the opposite of what it does on x86.  Without it the most significant byte comes
+// first (big-endian); with it the least significant one.  The kernels take the flag with the reference's meaning.
+constexpr float kS8Recip = 1.0f / 127.0f;
+constexpr float kS24Recip = 1.0f / 2147483392.0f;
+
+__device__ __forceinline__ float s8_to_f(unsigned b) { return __fmul_rn((float)(int)(signed char)b, kS8Recip); }
+__device__ __forceinline__ unsigned f_to_s8_bits(float x) { return (unsigned)x86_trunc_i32(__fmul_rn(x, 127.0f)) & 0xffu; }
+// x*255 rounds once in float; *0.5 is exact in double, so the sum rounds once whether or not it is contracted into an FMA
+__device__ __forceinline__ unsigned f_to_u8_bits(float x) { return (unsigned)x86_trunc_i32((double)__fmul_rn(x, 255.0f) * 0.5 + 128.0) & 0xffu; }
+
+// v = the sample's three bytes in stream order, packed little-endian (b0 | b1 << 8 | b2 << 16).  LSB_FIRST = the reference's `bigendian`.
+template <bool LSB_FIRST>
+__device__ __forceinline__ float s24_to_f(unsigned v)
+{
+    const unsigned w = LSB_FIRST ? v << 8 : (v & 0xffu) << 24 | (v & 0xff00u) << 8 | (v & 0xff0000u) >> 8;
+    return __fmul_rn((float)(int)w, kS24Recip);
+}
+// the sample's three bytes in stream order, packed the same way: the low three bytes of the truncated int32 (INT_MIN stores zeros)
+template <bool LSB_FIRST>
+__device__ __forceinline__ unsigned f_to_s24_bytes(float x)
+{
+    const unsigned t = (unsigned)x86_trunc_i32(__fmul_rn(x, 8388607.0f));
+    return LSB_FIRST ? t & 0xffffffu : (t & 0xffu) << 16 | (t & 0xff00u) | (t >> 16 & 0xffu);
+}
+
+// Each format is a policy for one grid-stride loop: a lane converts a group of four values per step, four steps in flight, with whole-word
+// global accesses -- one 32-bit word of s8 bytes, three of s24 bytes, one float4 of floats in; one float4, or one or three 32-bit words out.
+// ngroups = 0 when a buffer lacks the alignment of its group accesses: then every value takes the per-value path (byte accesses).
+struct S8ToF {
+    using In = unsigned char; using Out = float; using Group = unsigned;
+    static __device__ __forceinline__ Group load(const In* in, long g) { return __ldg(reinterpret_cast<const unsigned*>(in) + g); }
+    static __device__ __forceinline__ void store(Out* out, long g, Group w)
+    {
+        st_na_f4(reinterpret_cast<float4*>(out) + g, make_float4(s8_to_f(w & 255u), s8_to_f((w >> 8) & 255u), s8_to_f((w >> 16) & 255u), s8_to_f(w >> 24)));
+    }
+    static __device__ __forceinline__ void one(const In* in, Out* out, long i) { out[i] = s8_to_f(in[i]); }
+};
+
+template <bool U8>
+struct FToByte {
+    using In = float; using Out = unsigned char; using Group = float4;
+    static __device__ __forceinline__ unsigned bits(float x) { return U8 ? f_to_u8_bits(x) : f_to_s8_bits(x); }
+    static __device__ __forceinline__ Group load(const In* in, long g) { return __ldg(reinterpret_cast<const float4*>(in) + g); }
+    static __device__ __forceinline__ void store(Out* out, long g, Group a)
+    {
+        reinterpret_cast<unsigned*>(out)[g] = bits(a.x) | bits(a.y) << 8 | bits(a.z) << 16 | bits(a.w) << 24;
+    }
+    static __device__ __forceinline__ void one(const In* in, Out* out, long i) { out[i] = (unsigned char)bits(in[i]); }
+};
+
+struct Words3 { unsigned a, b, c; };                                      // 12 bytes: four s24 samples
+
+template <bool LSB_FIRST>
+struct S24ToF {
+    using In = unsigned char; using Out = float; using Group = Words3;
+    static __device__ __forceinline__ Group load(const In* in, long g)
+    {
+        const unsigned* p = reinterpret_cast<const unsigned*>(in) + 3 * g;
+        return {__ldg(p), __ldg(p + 1), __ldg(p + 2)};
+    }
+    static __device__ __forceinline__ void store(Out* out, long g, Group w)
+    {
+        st_na_f4(reinterpret_cast<float4*>(out) + g,
+                 make_float4(s24_to_f<LSB_FIRST>(w.a & 0xffffffu), s24_to_f<LSB_FIRST>(w.a >> 24 | (w.b & 0xffffu) << 8),
+                             s24_to_f<LSB_FIRST>(w.b >> 16 | (w.c & 0xffu) << 16), s24_to_f<LSB_FIRST>(w.c >> 8)));
+    }
+    static __device__ __forceinline__ void one(const In* in, Out* out, long i)
+    {
+        const In* p = in + 3 * i;
+        out[i] = s24_to_f<LSB_FIRST>((unsigned)p[0] | (unsigned)p[1] << 8 | (unsigned)p[2] << 16);
+    }
+};
+
+template <bool LSB_FIRST>
+struct FToS24 {
+    using In = float; using Out = unsigned char; using Group = float4;
+    static __device__ __forceinline__ Group load(const In* in, long g) { return __ldg(reinterpret_cast<const float4*>(in) + g); }
+    static __device__ __forceinline__ void store(Out* out, long g, Group a)
+    {
+        const unsigned v0 = f_to_s24_bytes<LSB_FIRST>(a.x), v1 = f_to_s24_bytes<LSB_FIRST>(a.y), v2 = f_to_s24_bytes<LSB_FIRST>(a.z),
+                       v3 = f_to_s24_bytes<LSB_FIRST>(a.w);
+        unsigned* p = reinterpret_cast<unsigned*>(out) + 3 * g;
+        p[0] = v0 | v1 << 24; p[1] = v1 >> 8 | v2 << 16; p[2] = v2 >> 16 | v3 << 8;
+    }
+    static __device__ __forceinline__ void one(const In* in, Out* out, long i)
+    {
+        const unsigned v = f_to_s24_bytes<LSB_FIRST>(in[i]);
+        Out* p = out + 3 * i;
+        p[0] = (Out)v; p[1] = (Out)(v >> 8); p[2] = (Out)(v >> 16);
+    }
+};
+
+template <class P>
+__global__ void __launch_bounds__(256) convert_groups_kernel(const typename P::In* __restrict__ in, typename P::Out* __restrict__ out, long n, long ngroups)
+{
+    const long stride = (long)gridDim.x * blockDim.x;
+    long g = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    for (; g + 3 * stride < ngroups; g += 4 * stride) {
+        typename P::Group w[4];
+#pragma unroll
+        for (int u = 0; u < 4; u++) w[u] = P::load(in, g + u * stride);
+#pragma unroll
+        for (int u = 0; u < 4; u++) P::store(out, g + u * stride, w[u]);
+    }
+    for (; g < ngroups; g += stride) P::store(out, g, P::load(in, g));
+    for (long i = ngroups * 4 + (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) P::one(in, out, i);
+}
+
 // ---- waterfall compression (SURVEY 8(f) rank 4): IMA ADPCM, 4 bits per value ------------------------------------------------------------
 // encode_ima_adpcm_i16_u8 (ima_adpcm.c:95-150) is a predictor/step-index recursion, sequential by definition; OpenWebRX runs one per audio stream and one
 // per waterfall line (csdr.c:1745-1767, state reset every line), so the bank form is one thread per row.  Integer arithmetic: bit-exact.
@@ -143,8 +259,7 @@ __global__ void compress_fft_adpcm_rows_kernel(const float* __restrict__ in, lon
 #pragma unroll
         for (int h = 0; h < 2; h++) {
             const int i = 2 * k + h;
-            const float s = __fmul_rn(x[i < PAD ? 0 : i - PAD], 100.0f);
-            const int w = (s >= 2147483648.0f || s < -2147483648.0f || s != s) ? INT_MIN : __float2int_rz(s);
+            const int w = x86_trunc_i32(__fmul_rn(x[i < PAD ? 0 : i - PAD], 100.0f));
             code[h] = ima_encode_one((int)(short)(w & 0xffff), index, previous);
         }
         y[k] = (unsigned char)(code[0] | (code[1] << 4));
@@ -181,6 +296,29 @@ int launch_convert_f_s16(const float* d_in, short* d_out, long n, cudaStream_t s
     convert_f_s16_kernel<<<grid_for(n / 8 + 1, 256), 256, 0, st>>>(d_in, d_out, n);
     CSDRB_CUDA(cudaGetLastError());
     return 0;
+}
+
+// byte buffers at any address, float buffers 4-byte aligned: the group path where the input and output pointers have in_align / out_align, the per-value path otherwise
+template <class P>
+static int launch_convert_groups(const typename P::In* d_in, typename P::Out* d_out, long n, uintptr_t in_align, uintptr_t out_align, cudaStream_t st)
+{
+    if (n <= 0) return 0;
+    const bool grouped = !(reinterpret_cast<uintptr_t>(d_in) & (in_align - 1)) && !(reinterpret_cast<uintptr_t>(d_out) & (out_align - 1));
+    const long ngroups = grouped ? n / 4 : 0;
+    convert_groups_kernel<P><<<grid_for(grouped ? n / 16 + 1 : n / 4 + 1, 256), 256, 0, st>>>(d_in, d_out, n, ngroups);
+    CSDRB_CUDA(cudaGetLastError());
+    return 0;
+}
+int launch_convert_s8_f(const unsigned char* d_in, float* d_out, long n, cudaStream_t st) { return launch_convert_groups<S8ToF>(d_in, d_out, n, 4, 16, st); }
+int launch_convert_f_s8(const float* d_in, unsigned char* d_out, long n, cudaStream_t st) { return launch_convert_groups<FToByte<false>>(d_in, d_out, n, 16, 4, st); }
+int launch_convert_f_u8(const float* d_in, unsigned char* d_out, long n, cudaStream_t st) { return launch_convert_groups<FToByte<true>>(d_in, d_out, n, 16, 4, st); }
+int launch_convert_s24_f(const unsigned char* d_in, float* d_out, long n, int bigendian, cudaStream_t st)
+{
+    return bigendian ? launch_convert_groups<S24ToF<true>>(d_in, d_out, n, 4, 16, st) : launch_convert_groups<S24ToF<false>>(d_in, d_out, n, 4, 16, st);
+}
+int launch_convert_f_s24(const float* d_in, unsigned char* d_out, long n, int bigendian, cudaStream_t st)
+{
+    return bigendian ? launch_convert_groups<FToS24<true>>(d_in, d_out, n, 16, 4, st) : launch_convert_groups<FToS24<false>>(d_in, d_out, n, 16, 4, st);
 }
 
 // ---- limit_ff (libcsdr.c:1130-1137): clamp to +-max; NaN -> +max like the reference build's minss/maxss (see oracle.c) ----

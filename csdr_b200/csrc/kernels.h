@@ -17,6 +17,12 @@ int launch_fir_decimate_bank_u8(const unsigned char* d_in, long in_stride, float
 int launch_convert_u8_f(const unsigned char* d_in, float* d_out, long n, cudaStream_t st);
 int launch_convert_s16_f(const short* d_in, float* d_out, long n, cudaStream_t st);
 int launch_convert_f_s16(const float* d_in, short* d_out, long n, cudaStream_t st);
+// the other sample formats: byte buffers at any address, float buffers 4-byte aligned; s24 counts values (3 bytes each), bigendian as the reference's flag
+int launch_convert_s8_f(const unsigned char* d_in, float* d_out, long n, cudaStream_t st);
+int launch_convert_f_s8(const float* d_in, unsigned char* d_out, long n, cudaStream_t st);
+int launch_convert_f_u8(const float* d_in, unsigned char* d_out, long n, cudaStream_t st);
+int launch_convert_s24_f(const unsigned char* d_in, float* d_out, long n, int bigendian, cudaStream_t st);
+int launch_convert_f_s24(const float* d_in, unsigned char* d_out, long n, int bigendian, cudaStream_t st);
 int launch_fmdemod_quadri_bank(const float2* d_in, long in_stride, float* d_out, long out_stride, int channels, int n,
                                const float2* d_last_in, float2* d_last_out, cudaStream_t st);
 

@@ -12,7 +12,7 @@
  * as ONE continuous stream (the CLI's per-process block framing -- stale tail blocks at EOF, the zero block deemphasis_nfm_ff emits
  * first -- is process plumbing and is not reproduced; tests/test_gpu_zzz_bankd.py compares against the oracle run over the whole stream).
  *
- * usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32|--s16|--real-s16|--real-f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]
+ * usage: csdr-bankd [--in -|HOST:PORT] [--u8|--s8|--f32|--s16|--real-s16|--real-f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]
  *                   [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty|wfm] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B] [--bfsk SPACING:LENGTH]
  *                   [--resample I:D[:BW]]
  *                   [--wfm-rate R] [--tau T]
@@ -51,9 +51,9 @@
  *   wideband rate / D is not 48 kHz, --resample I:D[:BW] puts rational_resampler_ff I D BW right behind the discriminator (tails nfm and none; see
  *   --help for the geometries it serves), e.g. 2.048 Msps with --decimation 32 --resample 3:4, or 10 Msps with --decimation 200 --resample 24:25:0.02.
  *   RATE  shift_addition_cc rate (fraction of the wideband sample rate), SINK a path (file or FIFO) or tcp:PORT (one listener).
- *   Input formats: --u8 (default) rtl_sdr's unsigned 8-bit IQ, --f32 complex float, --s16 complex signed 16-bit (Airspy INT16_IQ, SDRplay, LimeSDR,
- *   PlutoSDR; convert_s16_f in front of the complex bank), and REAL streams as direct-sampling receivers (RX888 / SDDC, Airspy real modes, ADC
- *   boards) deliver them: --real-s16 (convert_s16_f) and --real-f32.  A real stream runs csdrb_ddc_bank_process_f, per channel
+ *   Input formats: --u8 (default) rtl_sdr's unsigned 8-bit IQ, --s8 HackRF's signed 8-bit IQ (convert_s8_f in front of the complex bank), --f32
+ *   complex float, --s16 complex signed 16-bit (Airspy INT16_IQ, SDRplay, LimeSDR, PlutoSDR; convert_s16_f in front of the complex bank), and
+ *   REAL streams as direct-sampling receivers (RX888 / SDDC, Airspy real modes, ADC boards) deliver them: --real-s16 (convert_s16_f) and --real-f32.  A real stream runs csdrb_ddc_bank_process_f, per channel
  *     convert_s16_f | shift_addition_fc r | fir_decimate_cc D bw W | <tail>
  *   and every tail works behind it.  A station at frequency f of a real stream sampled at fs is tuned with RATE = -f/fs (shift_addition_fc moves
  *   it to 0 Hz); +f/fs selects its mirror image, the conjugate: sidebands swapped and the discriminator negated.  E.g. 7.074 MHz FT8 from an RX888 at
@@ -784,10 +784,11 @@ static void close_sinks(channel_t *chan, int C, waterfall_t *wf)
 
 /* ---- options: main() parses and validates them, both loops read them ------------------------------------------------------------------------ */
 /* wideband input formats (--u8 ...), their bytes per sample on the wire and their names */
-enum { IN_U8, IN_F32, IN_S16, IN_REAL_S16, IN_REAL_F32 };
-static const int kWireBytes[] = {2, 8, 4, 2, 4};
-static const char *kFormatNames[] = {"u8", "f32", "s16", "real s16", "real f32"};
+enum { IN_U8, IN_F32, IN_S16, IN_REAL_S16, IN_REAL_F32, IN_S8 };
+static const int kWireBytes[] = {2, 8, 4, 2, 4, 2};
+static const char *kFormatNames[] = {"u8", "f32", "s16", "real s16", "real f32", "s8"};
 #define S16_RECIP (1.0f / 32767.0f)                       /* convert_s16_f: the reference build multiplies by the float reciprocal (csdrb_convert_s16_f) */
+#define S8_RECIP (1.0f / 127.0f)                          /* convert_s8_f: likewise (csdrb_convert_s8_f) */
 
 /* the tails (--tail NAME): whether the bank demodulates for them (float discriminator rows, else cf32 baseband rows), whether --resample
  * may run in front of them, and their AGC reference when --agc-ref is not given: fastagc_ff's default (csdr.c:1388), agc_ff's (csdr.c:1342),
@@ -945,8 +946,10 @@ static int run_multi(const opts_t *o, channel_t *chan, int C, const float *rates
             ok = read_block(in_fd, raw, (size_t)fresh * (size_t)kWireBytes[fmt]);
             const short *s16 = (const short *)raw;
             const float *f32 = (const float *)raw;
+            const signed char *s8 = (const signed char *)raw;
             if (ok) for (int i = 0; i < fresh; i++) {
                 if (fmt == IN_U8) { dst[i].i = lut[raw[2 * i]]; dst[i].q = lut[raw[2 * i + 1]]; }
+                else if (fmt == IN_S8) { dst[i].i = (float)s8[2 * i] * S8_RECIP; dst[i].q = (float)s8[2 * i + 1] * S8_RECIP; }
                 else if (fmt == IN_S16) { dst[i].i = (float)s16[2 * i] * S16_RECIP; dst[i].q = (float)s16[2 * i + 1] * S16_RECIP; }
                 else if (fmt == IN_REAL_S16) { dst[i].i = (float)s16[i] * S16_RECIP; dst[i].q = 0.0f; }
                 else { dst[i].i = f32[i]; dst[i].q = 0.0f; }
@@ -981,13 +984,17 @@ static int run_multi(const opts_t *o, channel_t *chan, int C, const float *rates
 static int usage(void)
 {
     fprintf(stderr,
-            "usage: csdr-bankd [--in -|HOST:PORT] [--u8|--f32|--s16|--real-s16|--real-f32] [--decimation D] [--bw TRANSITION_BW] [--window W]\n"
+            "usage: csdr-bankd [--in -|HOST:PORT] [--u8|--s8|--f32|--s16|--real-s16|--real-f32] [--decimation D] [--bw TRANSITION_BW] [--window W]\n"
             "                  [--block SAMPLES]\n"
             "                  [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty|wfm] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B]\n"
             "                  [--bfsk SPACING:LENGTH]\n"
             "                  [--wfm-rate R] [--tau T] [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]\n"
             "                  RATE:SINK [RATE:SINK ...]\n"
             "  --u8 | --f32 | --s16 the complex input: rtl_sdr's u8 IQ (default), complex float, or complex s16 (Airspy INT16_IQ, SDRplay, ...)\n"
+            "  --s8                 HackRF's signed 8-bit IQ (hackrf_transfer -r -), convert_s8_f in front of the bank.  Three NFM channels\n"
+            "                       at 10 Msps (50 kHz channels, resampled to 48 kHz):\n"
+            "                       hackrf_transfer -r - -s 10000000 -f 145500000 | csdr-bankd --s8 --decimation 200 --resample 24:25\n"
+            "                       -0.05:a.s16 0.0:b.s16 0.1:c.s16\n"
             "  --real-s16 | --real-f32  a REAL stream from a direct-sampling receiver (RX888 / SDDC, Airspy real modes, ADC boards): per channel\n"
             "                       convert_s16_f | shift_addition_fc RATE | fir_decimate_cc D bw | <tail>.  A station at f Hz of a real stream\n"
             "                       sampled at fs is tuned with RATE = -f/fs; +f/fs gives it conjugated (sidebands swapped, discriminator negated).\n"
@@ -1051,6 +1058,7 @@ int main(int argc, char **argv)
         const char *arg = argv[a];
         const char *v = a + 1 < argc ? argv[a + 1] : NULL;
         if (!strcmp(arg, "--u8")) o.fmt = IN_U8;
+        else if (!strcmp(arg, "--s8")) o.fmt = IN_S8;
         else if (!strcmp(arg, "--f32")) o.fmt = IN_F32;
         else if (!strcmp(arg, "--s16")) o.fmt = IN_S16;
         else if (!strcmp(arg, "--real-s16")) o.fmt = IN_REAL_S16;
@@ -1181,7 +1189,7 @@ int main(int argc, char **argv)
     unsigned char *h_in = csdrb_host_alloc(in_bytes);
     const int wide_cap = block + T + D + 16;
     unsigned char *d_wide[2] = {csdrb_device_alloc(ssz * (size_t)wide_cap), csdrb_device_alloc(ssz * (size_t)wide_cap)};
-    const int raw_in = fmt == IN_U8 || fmt == IN_S16 || fmt == IN_REAL_S16;
+    const int raw_in = fmt == IN_U8 || fmt == IN_S8 || fmt == IN_S16 || fmt == IN_REAL_S16;
     unsigned char *d_raw = raw_in ? csdrb_device_alloc(in_bytes + 16) : NULL;
     float *d_stage = fmt == IN_REAL_S16 ? csdrb_device_alloc(sizeof(float) * (size_t)block + 16) : NULL;
     const int out_cap = wide_cap / D + 2;                          /* bank outputs one block can add */
@@ -1209,6 +1217,7 @@ int main(int argc, char **argv)
         float *fresh = (float *)(d_wide[cur] + ssz * (size_t)keep);
         if (raw_in) OK(csdrb_copy_h2d(d_raw, h_in, fresh_bytes, stream));
         if (fmt == IN_U8) OK(csdrb_convert_u8_f(d_raw, fresh, 2L * fresh_n, stream));
+        else if (fmt == IN_S8) OK(csdrb_convert_s8_f((const signed char *)d_raw, fresh, 2L * fresh_n, stream));
         else if (fmt == IN_S16) OK(csdrb_convert_s16_f((const short *)d_raw, fresh, 2L * fresh_n, stream));
         else if (fmt == IN_REAL_S16 && !((size_t)fresh & 15)) OK(csdrb_convert_s16_f((const short *)d_raw, fresh, fresh_n, stream));
         else if (fmt == IN_REAL_S16) {

@@ -241,6 +241,49 @@ static int cmd_convert_f_s16(int argc, char **argv)
     return map_blocks(sizeof(float), sizeof(short), block, 0, convert_f_s16_step, NULL);
 }
 
+/* convert_s8_f, convert_f_s8, convert_f_u8 (csdr.c:546-581) and convert_s24_f / convert_f_s24 [--bigendian] (:606-633): one call per block,
+ * s24 values 3 bytes each.  `--bigendian` is the reference's flag, whose meaning on x86 is the opposite of its name (include/csdr_b200.h). */
+static void convert_s8_f_step(void *in, void *out, void *state) { (void)state; convert_s8_f(in, out, block); }
+static void convert_f_s8_step(void *in, void *out, void *state) { (void)state; convert_f_s8(in, out, block); }
+static void convert_f_u8_step(void *in, void *out, void *state) { (void)state; convert_f_u8(in, out, block); }
+static void convert_s24_f_step(void *in, void *out, void *bigendian) { convert_s24_f(in, out, block, *(int *)bigendian); }
+static void convert_f_s24_step(void *in, void *out, void *bigendian) { convert_f_s24(in, out, block, *(int *)bigendian); }
+
+static int cmd_convert_s8_f(int argc, char **argv)
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    return map_blocks(1, sizeof(float), block, 0, convert_s8_f_step, NULL);
+}
+
+static int cmd_convert_f_s8(int argc, char **argv)
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    return map_blocks(sizeof(float), 1, block, 0, convert_f_s8_step, NULL);
+}
+
+static int cmd_convert_f_u8(int argc, char **argv)
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    return map_blocks(sizeof(float), 1, block, 0, convert_f_u8_step, NULL);
+}
+
+static int cmd_convert_s24_f(int argc, char **argv)
+{
+    int bigendian = argc > 2 && !strcmp(argv[2], "--bigendian");
+    if (!announce_block(open_block())) return -2;
+    return map_blocks(3, sizeof(float), block, 0, convert_s24_f_step, &bigendian);
+}
+
+static int cmd_convert_f_s24(int argc, char **argv)
+{
+    int bigendian = argc > 2 && !strcmp(argv[2], "--bigendian");
+    if (!announce_block(open_block())) return -2;
+    return map_blocks(sizeof(float), 3, block, 0, convert_f_s24_step, &bigendian);
+}
+
 static void addition_init(nco_t *nco, float rate) { nco->addition = shift_addition_init(rate); }
 static float addition_cc(void *in, complexf *out, int n, nco_t *nco, float phase) { return shift_addition_cc(in, out, n, nco->addition, phase); }
 static float addition_fc(void *in, complexf *out, int n, nco_t *nco, float phase) { return shift_addition_fc(in, out, n, nco->addition, phase); }
@@ -1156,6 +1199,11 @@ static const struct { const char *name; int (*run)(int, char **); const char *sy
     {"convert_i16_f", cmd_convert_s16_f, "convert_i16_f"},
     {"convert_f_s16", cmd_convert_f_s16, "convert_f_s16"},
     {"convert_f_i16", cmd_convert_f_s16, "convert_f_i16"},
+    {"convert_s8_f", cmd_convert_s8_f, "convert_s8_f"},
+    {"convert_f_s8", cmd_convert_f_s8, "convert_f_s8"},
+    {"convert_f_u8", cmd_convert_f_u8, "convert_f_u8"},
+    {"convert_s24_f", cmd_convert_s24_f, "convert_s24_f [--bigendian]"},
+    {"convert_f_s24", cmd_convert_f_s24, "convert_f_s24 [--bigendian]"},
     {"shift_addition_cc", cmd_shift_addition_cc, "shift_addition_cc <rate> | --fifo <fifo_path> | --fd <fd>"},
     {"shift_addition_fc", cmd_shift_addition_fc, "shift_addition_fc <rate> | --fifo <fifo_path> | --fd <fd>"},
     {"fir_decimate_cc", cmd_fir_decimate_cc, "fir_decimate_cc <decimation_factor> [transition_bw [window]]"},

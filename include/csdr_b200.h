@@ -52,6 +52,12 @@ void convert_s16_f(short *input, float *output, int input_size);
 void convert_i16_f(short *input, float *output, int input_size);
 void convert_f_s16(float *input, short *output, int input_size);
 void convert_f_i16(float *input, short *output, int input_size);
+/* the other sample formats (libcsdr.h:221-223, 228-229; libcsdr.c:2368-2437): HackRF's s8 IQ, rtl_tcp-style u8 out, 24-bit sound cards */
+void convert_s8_f(signed char *input, float *output, int input_size);
+void convert_f_s8(float *input, signed char *output, int input_size);
+void convert_f_u8(float *input, unsigned char *output, int input_size);
+void convert_f_s24(float *input, unsigned char *output, int input_size, int bigendian);
+void convert_s24_f(unsigned char *input, float *output, int input_size, int bigendian);
 
 /* NCO shift by phasor recursion (libcsdr_gpl.h:26-46; libcsdr_gpl.c:27-52, 81-89, 126-160) */
 typedef struct shift_addition_data_s { float sindelta; float cosdelta; float rate; } shift_addition_data_t;
@@ -256,6 +262,17 @@ int csdrb_copy2d_h2d(void *d_dst, size_t dst_pitch_bytes, const void *h_src, siz
 int csdrb_convert_u8_f(const unsigned char *d_in, float *d_out, long n, void *stream);
 int csdrb_convert_s16_f(const short *d_in, float *d_out, long n, void *stream);
 int csdrb_convert_f_s16(const float *d_in, short *d_out, long n, void *stream);
+/* The other sample formats (libcsdr.c:2368-2437), bit for bit the reference's x86 build, on device buffers (bytes at any
+ * address, floats 4-byte aligned); n counts values
+ * (an s24 value is 3 bytes).  f32 -> s8/u8/s24 truncate toward zero and keep the low bytes of the int32 as x86's cvttss2si/cvttsd2si give it:
+ * out of range wraps, NaN and +-Inf store zeros.  `bigendian` is the reference flag passed straight through; on x86 it selects the opposite
+ * order of its name: 0 = most significant byte first, 1 = least significant byte first.  Returns 0; -1 for a null pointer, a misaligned float
+ * buffer or n < 0, with nothing launched.  n = 0 does nothing. */
+int csdrb_convert_s8_f(const signed char *d_in, float *d_out, long n, void *stream);
+int csdrb_convert_f_s8(const float *d_in, signed char *d_out, long n, void *stream);
+int csdrb_convert_f_u8(const float *d_in, unsigned char *d_out, long n, void *stream);
+int csdrb_convert_s24_f(const unsigned char *d_in, float *d_out, long n, int bigendian, void *stream);
+int csdrb_convert_f_s24(const float *d_in, unsigned char *d_out, long n, int bigendian, void *stream);
 
 /* K3 fir_decimate_cc bank: channel c reads d_in + c*in_stride (input_size samples) and writes
  * d_out + c*out_stride; all channels share h_taps (HOST pointer, copied into the launch).
