@@ -25,6 +25,11 @@ class _CF(C.Structure):
     _fields_ = [("i", C.c_float), ("q", C.c_float)]
 
 
+class _DcBlock(C.Structure):
+    """dcblock_preserve_t"""
+    _fields_ = [("last_input", C.c_float), ("last_output", C.c_float)]
+
+
 class _Shift(C.Structure):
     _fields_ = [("sindelta", C.c_float), ("cosdelta", C.c_float), ("rate", C.c_float)]
 
@@ -272,6 +277,14 @@ def lib() -> C.CDLL:
     L.convert_f_s24.argtypes = [vp, vp, it, it]
     L.fir_decimate_cc.argtypes = [vp, vp, it, it, C.POINTER(C.c_float), it]
     L.fmdemod_quadri_cf.argtypes = [vp, vp, it, vp, _CF]; L.fmdemod_quadri_cf.restype = _CF
+    L.csdrb_fmdemod_quadri_novect_bank_cf.argtypes = [vp, lg, vp, lg, it, it, vp, vp, vp]
+    L.csdrb_fmdemod_atan_bank_cf.argtypes = [vp, lg, vp, lg, it, it, vp, vp, vp]
+    L.csdrb_amdemod_estimator_bank_cf.argtypes = [vp, lg, vp, lg, it, it, C.c_float, C.c_float, vp]
+    L.csdrb_dcblock_bank_ff.argtypes = [vp, lg, vp, lg, it, it, C.c_float, vp, vp]
+    L.fmdemod_quadri_novect_cf.argtypes = [vp, vp, it, _CF]; L.fmdemod_quadri_novect_cf.restype = _CF
+    L.fmdemod_atan_cf.argtypes = [vp, vp, it, C.c_float]; L.fmdemod_atan_cf.restype = C.c_float
+    L.amdemod_estimator_cf.argtypes = [vp, vp, it, C.c_float, C.c_float]
+    L.dcblock_ff.argtypes = [vp, vp, it, C.c_float, _DcBlock]; L.dcblock_ff.restype = _DcBlock
     L.csdrb_simple_agc_bank_cc.argtypes = [vp, lg, vp, lg, it, it, C.c_float, C.c_float, C.c_float, vp, vp]
     L.csdrb_timing_recovery_bank_cc.argtypes = [vp, lg, vp, vp, it, vp, lg, vp, vp, it, C.POINTER(TimingRecoveryParams), vp, vp]
     L.csdrb_dbpsk_decoder_bank_c_u8.argtypes = [vp, lg, vp, lg, it, it, vp, vp, vp, vp]
@@ -566,6 +579,88 @@ def fmdemod_quadri_bank_cf(x, last=None, out=None, return_last: bool = False):
     return (res, last_out) if return_last else res
 
 
+def _device_rows(t, shape, dtype, device, what: str):
+    """t as the device buffer a bank reads or writes through its raw pointer: a contiguous CUDA tensor of this dtype and shape"""
+    import torch
+    if not (isinstance(t, torch.Tensor) and t.is_cuda and t.device == device and t.dtype == dtype and tuple(t.shape) == tuple(shape)
+            and t.is_contiguous()):
+        got = f"{tuple(t.shape)} {t.dtype} on {t.device}, contiguous={t.is_contiguous()}" if isinstance(t, torch.Tensor) else type(t).__name__
+        raise ValueError(f"{what} must be a contiguous {dtype} CUDA tensor of shape {tuple(shape)} on {device}, got {got}")
+    return t
+
+
+def fmdemod_quadri_novect_bank_cf(x, last=None, out=None, return_last: bool = False):
+    """fmdemod_quadri_novect_cf per row: fmdemod_quadri_bank_cf's bits except where I*I + Q*Q rounds to 0 (NaN or +-Inf there, not 0)."""
+    import torch
+    xr, ptr, stride, ch, n = _as_cf32_rows(x)
+    if out is None:
+        out = torch.empty((ch, n + (n & 1)), dtype=torch.float32, device=xr.device)
+    if not (out.is_cuda and out.device == xr.device and out.dtype == torch.float32 and out.dim() == 2 and out.stride(1) == 1 and out.shape[0] == ch
+            and out.shape[1] >= n):
+        raise ValueError(f"out must be a float32 CUDA tensor [{ch}, >= {n}] with contiguous rows on {xr.device}")
+    if last is not None:
+        _device_rows(last, (ch,), torch.complex64, xr.device, "last")
+    last_out = torch.empty(ch, dtype=torch.complex64, device=xr.device) if return_last else None
+    _check(lib().csdrb_fmdemod_quadri_novect_bank_cf(ptr, stride, out.data_ptr(), out.stride(0), ch, n,
+                                                     last.data_ptr() if last is not None else None,
+                                                     last_out.data_ptr() if last_out is not None else None, _stream()),
+           "fmdemod_quadri_novect_bank_cf")
+    res = out[:, :n]
+    return (res, last_out) if return_last else res
+
+
+def fmdemod_atan_bank_cf(x, last=None, out=None, return_last: bool = False):
+    """fmdemod_atan_cf per row: [C, N] cf32 -> [C, N] f32, the phase difference over pi.  ``last`` is a [C] float32 CUDA tensor (the phase
+    before each row; None = 0); with ``return_last`` also the [C] phases of the rows' last samples, to pass as ``last`` next time."""
+    import torch
+    xr, ptr, stride, ch, n = _as_cf32_rows(x)
+    if out is None:
+        out = torch.empty((ch, n), dtype=torch.float32, device=xr.device)
+    if not (out.is_cuda and out.device == xr.device and out.dtype == torch.float32 and out.dim() == 2 and out.stride(1) == 1 and out.shape[0] == ch
+            and out.shape[1] >= n):
+        raise ValueError(f"out must be a float32 CUDA tensor [{ch}, >= {n}] with contiguous rows on {xr.device}")
+    if last is not None:
+        _device_rows(last, (ch,), torch.float32, xr.device, "last")
+    last_out = torch.empty(ch, dtype=torch.float32, device=xr.device) if return_last else None
+    _check(lib().csdrb_fmdemod_atan_bank_cf(ptr, stride, out.data_ptr(), out.stride(0), ch, n,
+                                            last.data_ptr() if last is not None else None,
+                                            last_out.data_ptr() if last_out is not None else None, _stream()),
+           "fmdemod_atan_bank_cf")
+    res = out[:, :n]
+    return (res, last_out) if return_last else res
+
+
+def amdemod_estimator_bank_cf(x, alpha: float = 0.0, beta: float = 0.0, out=None):
+    """amdemod_estimator_cf per row: [C, N] cf32 -> [C, N] f32, alpha*max(|I|,|Q|) + beta*min(|I|,|Q|) (alpha = 0: the reference's defaults)."""
+    import torch
+    xr, ptr, stride, ch, n = _as_cf32_rows(x)
+    if out is None:
+        out = torch.empty((ch, n), dtype=torch.float32, device=xr.device)
+    if not (out.is_cuda and out.device == xr.device and out.dtype == torch.float32 and out.dim() == 2 and out.stride(1) == 1 and out.shape[0] == ch
+            and out.shape[1] >= n):
+        raise ValueError(f"out must be a float32 CUDA tensor [{ch}, >= {n}] with contiguous rows on {xr.device}")
+    _check(lib().csdrb_amdemod_estimator_bank_cf(ptr, stride, out.data_ptr(), out.stride(0), ch, n, alpha, beta, _stream()), "amdemod_estimator_bank_cf")
+    return out[:, :n]
+
+
+def dcblock_bank_ff(x, a: float = 0.0, state=None, return_state: bool = False, out=None):
+    """dcblock_ff per row: x [C, N] float32 -> y [C, N].  ``state`` is a [C, 2] float32 CUDA tensor of dcblock_preserve_t {last_input,
+    last_output} (None = zeros, the stream start); with ``return_state`` also the updated state to pass next time.  a = 0 means 0.999."""
+    import torch
+    if not (isinstance(x, torch.Tensor) and x.dtype == torch.float32 and x.is_cuda and x.dim() == 2 and x.stride(1) == 1):
+        raise ValueError("x must be a float32 CUDA tensor [C, N] with contiguous rows")
+    ch, n = x.shape
+    if out is None:
+        out = torch.empty((ch, n), dtype=torch.float32, device=x.device)
+    elif not (out.is_cuda and out.device == x.device and out.dtype == torch.float32 and out.dim() == 2 and out.stride(1) == 1
+              and out.shape[0] == ch and out.shape[1] >= n and (out.data_ptr() != x.data_ptr() or out.stride(0) == x.stride(0))):
+        raise ValueError(f"out must be a float32 CUDA tensor [{ch}, >= {n}] with contiguous rows on {x.device} (x itself for in place)")
+    state = torch.zeros((ch, 2), dtype=torch.float32, device=x.device) if state is None else \
+        _device_rows(state, (ch, 2), torch.float32, x.device, "state").clone()
+    _check(lib().csdrb_dcblock_bank_ff(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), ch, n, a, state.data_ptr(), _stream()), "dcblock_bank_ff")
+    return (out, state) if return_state else out
+
+
 # --------------------------------------------------------------------------------------------------
 # libcsdr drop-in calls on HOST arrays (Part A of the C ABI) -- what the reference's callers bind
 # --------------------------------------------------------------------------------------------------
@@ -741,6 +836,29 @@ class libcsdr:
     def amdemod_cf(x):
         x = np.ascontiguousarray(x, np.complex64); y = np.empty(x.size, np.float32)
         lib().amdemod_cf(x.ctypes.data, y.ctypes.data, x.size); return y
+
+    @staticmethod
+    def amdemod_estimator_cf(x, alpha=0.0, beta=0.0):
+        x = np.ascontiguousarray(x, np.complex64); y = np.empty(x.size, np.float32)
+        lib().amdemod_estimator_cf(x.ctypes.data, y.ctypes.data, x.size, alpha, beta); return y
+
+    @staticmethod
+    def dcblock_ff(x, a=0.0, preserved=(0.0, 0.0)):
+        """one call: (y, (last_input, last_output))"""
+        x = np.ascontiguousarray(x, np.float32); y = np.empty_like(x)
+        r = lib().dcblock_ff(x.ctypes.data, y.ctypes.data, x.size, a, _DcBlock(*preserved)); return y, (r.last_input, r.last_output)
+
+    @staticmethod
+    def fmdemod_atan_cf(x, last_phase=0.0):
+        """one call: (y, the last sample's phase)"""
+        x = np.ascontiguousarray(x, np.complex64); y = np.empty(x.size, np.float32)
+        r = lib().fmdemod_atan_cf(x.ctypes.data, y.ctypes.data, x.size, last_phase); return y, float(np.float32(r))
+
+    @staticmethod
+    def fmdemod_quadri_novect_cf(x, last=0j):
+        x = np.ascontiguousarray(x, np.complex64); y = np.empty(x.size, np.float32)
+        r = lib().fmdemod_quadri_novect_cf(x.ctypes.data, y.ctypes.data, x.size, _CF(np.float32(last.real), np.float32(last.imag)))
+        return y, complex(r.i, r.q)
 
     @staticmethod
     def fastdcblock_ff(x, last_dc=0.0):

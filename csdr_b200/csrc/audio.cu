@@ -257,13 +257,33 @@ int launch_fractional_decimator_bank(const float* d_in, long in_stride, float* d
     return 2;
 }
 
-// ---------------------------------------------------------------------------------------------- de-emphasis
-// deemphasis_wfm_ff (libcsdr.c:1081-1097): y[i] = alpha*x[i] + (1-alpha)*y[i-1] -- a float recursion whose rounding sequence is
-// the result, so it stays sequential per channel: lane = channel, a warp moves 32 channels through a padded shared tile so that
-// global accesses are coalesced rows while each lane walks its own row (same scheme as the NCO kernel).
-__global__ void __launch_bounds__(128)
-deemphasis_wfm_bank_kernel(const float* __restrict__ in, long in_stride, float* __restrict__ out, long out_stride, int channels, int n,
-                           float alpha, float keep, float* __restrict__ last_io)
+// ---------------------------------------------------------------------------------------------- first-order recursions
+// deemphasis_wfm_ff (libcsdr.c:1081-1097): y[i] = alpha*x[i] + (1-alpha)*y[i-1], and dcblock_ff (libcsdr.c:903-918): y[i] = (x[i] - x[i-1]) +
+// a*y[i-1] -- float recursions whose rounding sequence is the result, so they stay sequential per channel: lane = channel, a warp moves 32
+// channels through a padded shared tile so that global accesses are coalesced rows while each lane walks its own row (same scheme as the NCO
+// kernel).  recursion_rows is that scheme; Step gives the per-channel State, how a carried state starts (begin) and one sample's step; every tile is read whole before it is
+// written, so d_in == d_out with equal strides is allowed.
+struct DeemphasisStep {
+    using State = float;                                               // y[i-1]
+    float alpha, keep;
+    __device__ __forceinline__ State begin(State y) const { return y != y ? 0.f : y; }   // NaN carry restarts from 0 (libcsdr.c:1092)
+    __device__ __forceinline__ float operator()(State& y, float x) const { y = __fadd_rn(__fmul_rn(alpha, x), __fmul_rn(keep, y)); return y; }
+};
+struct DcBlockStep {
+    using State = DcBlockState;                                        // {x[i-1], y[i-1]}: dcblock_preserve_t
+    float a;
+    __device__ __forceinline__ State begin(State s) const { return s; }
+    __device__ __forceinline__ float operator()(State& s, float x) const
+    {
+        s.last_output = __fadd_rn(__fsub_rn(x, s.last_input), __fmul_rn(a, s.last_output));
+        s.last_input = x;
+        return s.last_output;
+    }
+};
+
+template <class Step>
+__device__ __forceinline__ void recursion_rows(const float* __restrict__ in, long in_stride, float* __restrict__ out, long out_stride, int channels,
+                                               int n, Step step, typename Step::State* __restrict__ state_io)
 {
     __shared__ float tile_all[4][32 * 33];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -272,8 +292,7 @@ deemphasis_wfm_bank_kernel(const float* __restrict__ in, long in_stride, float* 
     if (c0 >= channels) return;
     const int rows = min(32, channels - c0);
     const bool live = lane < rows;
-    float y = live ? last_io[c0 + lane] : 0.f;
-    if (y != y) y = 0.f;                                               // NaN carry restarts from 0 (libcsdr.c:1092)
+    typename Step::State s = live ? step.begin(state_io[c0 + lane]) : typename Step::State{};
     for (int t0 = 0; t0 < n; t0 += 32) {
         const int len = min(32, n - t0);
         for (int r0 = 0; r0 < rows; r0 += 8) {                       // eight rows' loads in flight before the first shared store
@@ -286,13 +305,27 @@ deemphasis_wfm_bank_kernel(const float* __restrict__ in, long in_stride, float* 
         __syncwarp();
         if (live) {
             float* row = tile + lane * 33;
-            for (int j = 0; j < len; j++) { y = __fadd_rn(__fmul_rn(alpha, row[j]), __fmul_rn(keep, y)); row[j] = y; }
+            for (int j = 0; j < len; j++) row[j] = step(s, row[j]);
         }
         __syncwarp();
         for (int r = 0; r < rows; r++) if (lane < len) out[(long)(c0 + r) * out_stride + t0 + lane] = tile[r * 33 + lane];
         __syncwarp();
     }
-    if (live) last_io[c0 + lane] = y;
+    if (live) state_io[c0 + lane] = s;
+}
+
+__global__ void __launch_bounds__(128)
+deemphasis_wfm_bank_kernel(const float* __restrict__ in, long in_stride, float* __restrict__ out, long out_stride, int channels, int n, DeemphasisStep step,
+                           float* __restrict__ last_io)
+{
+    recursion_rows(in, in_stride, out, out_stride, channels, n, step, last_io);
+}
+
+__global__ void __launch_bounds__(128)
+dcblock_bank_kernel(const float* __restrict__ in, long in_stride, float* __restrict__ out, long out_stride, int channels, int n, DcBlockStep step,
+                    DcBlockState* __restrict__ state_io)
+{
+    recursion_rows(in, in_stride, out, out_stride, channels, n, step, state_io);
 }
 
 int launch_deemphasis_wfm_bank(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int n, float tau, int sample_rate,
@@ -303,7 +336,18 @@ int launch_deemphasis_wfm_bank(const float* d_in, long in_stride, float* d_out, 
     const float dt = (float)(1.0 / sample_rate);                        // same promotions as libcsdr.c:1090-1091
     const float alpha = dt / (tau + dt);
     const float keep = 1 - alpha;
-    deemphasis_wfm_bank_kernel<<<(channels + 127) / 128, 128, 0, st>>>(d_in, in_stride, d_out, out_stride, channels, n, alpha, keep, d_last_io);
+    deemphasis_wfm_bank_kernel<<<(channels + 127) / 128, 128, 0, st>>>(d_in, in_stride, d_out, out_stride, channels, n, DeemphasisStep{alpha, keep}, d_last_io);
+    CSDRB_CUDA(cudaGetLastError());
+    return 1;
+}
+
+int launch_dcblock_bank(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int n, float a, void* d_state_io,
+                        cudaStream_t st)
+{
+    if (channels <= 0 || n <= 0) return 0;
+    if (a == 0.f) a = 0.999f;                                            // libcsdr.c:909
+    dcblock_bank_kernel<<<(channels + 127) / 128, 128, 0, st>>>(d_in, in_stride, d_out, out_stride, channels, n, DcBlockStep{a},
+                                                                  static_cast<DcBlockState*>(d_state_io));
     CSDRB_CUDA(cudaGetLastError());
     return 1;
 }

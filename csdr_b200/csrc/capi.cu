@@ -170,7 +170,63 @@ int csdrb_fmdemod_quadri_bank_cf(const complexf* d_in, long in_stride, float* d_
     return counted(launch_fmdemod_quadri_bank(reinterpret_cast<const float2*>(d_in), in_stride, d_out, out_stride, channels, input_size,
                                               reinterpret_cast<const float2*>(d_last_in), reinterpret_cast<float2*>(d_last_out), S(stream)));
 }
+int csdrb_fmdemod_quadri_novect_bank_cf(const complexf* d_in, long in_stride, float* d_out, long out_stride, int channels,
+                                        int input_size, const complexf* d_last_in, complexf* d_last_out, void* stream)
+{
+    if (too_many_channels(channels, "fmdemod_quadri_novect bank")) return -1;
+    if (!d_in || !d_out) { set_error("fmdemod_quadri_novect bank: null pointer"); return -1; }
+    if (channels <= 0 || input_size <= 0) return 0;
+    return counted(launch_fmdemod_quadri_novect_bank(reinterpret_cast<const float2*>(d_in), in_stride, d_out, out_stride, channels, input_size,
+                                                     reinterpret_cast<const float2*>(d_last_in), reinterpret_cast<float2*>(d_last_out), S(stream)));
+}
 
+// the demodulator banks of demod.cu and dcblock: 0 = go ahead, 1 = nothing to do, -1 = refused (nothing launched)
+static int demod_args(const char* who, const void* d_in, size_t in_align, long in_stride, const void* d_out, long out_stride, int channels, int n,
+                      const void* d_state, bool in_place_ok)
+{
+    if (too_many_channels(channels, who)) return -1;
+    if (channels < 0 || n < 0 || in_stride < n || out_stride < n) { set_error("%s: needs channels >= 0, n >= 0 and row strides of at least n", who); return -1; }
+    if (!d_in || !d_out) { set_error("%s: null pointer", who); return -1; }
+    if (misaligned(d_in, in_align) || misaligned(d_out, 4) || misaligned(d_state, 4)) { set_error("%s: misaligned pointer", who); return -1; }
+    if (d_in == d_out && (!in_place_ok || (channels > 1 && in_stride != out_stride))) {
+        set_error(in_place_ok ? "%s: in place only with equal strides" : "%s: d_in and d_out must differ", who);
+        return -1;
+    }
+    return channels == 0 || n == 0 ? 1 : 0;
+}
+
+int csdrb_fmdemod_atan_bank_cf(const complexf* d_in, long in_stride, float* d_out, long out_stride, int channels, int input_size,
+                               const float* d_last_phase_in, float* d_last_phase_out, void* stream)
+{
+    const char* who = "fmdemod_atan bank";
+    int rc = demod_args(who, d_in, 8, in_stride, d_out, out_stride, channels, input_size, d_last_phase_in, false);
+    if (rc == 0 && misaligned(d_last_phase_out, 4)) { set_error("%s: misaligned pointer", who); rc = -1; }
+    if (rc) return rc < 0 ? rc : 0;
+    rc = launch_fmdemod_atan_bank(reinterpret_cast<const float2*>(d_in), in_stride, d_out, out_stride, channels, input_size, d_last_phase_in,
+                                  d_last_phase_out, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
+
+int csdrb_amdemod_estimator_bank_cf(const complexf* d_in, long in_stride, float* d_out, long out_stride, int channels, int input_size,
+                                    float alpha, float beta, void* stream)
+{
+    const int rc = demod_args("amdemod_estimator bank", d_in, 8, in_stride, d_out, out_stride, channels, input_size, nullptr, false);
+    if (rc) return rc < 0 ? rc : 0;
+    const int k = launch_amdemod_estimator_bank(reinterpret_cast<const float2*>(d_in), in_stride, d_out, out_stride, channels, input_size, alpha, beta,
+                                                S(stream));
+    return k < 0 ? k : counted(0, k);
+}
+
+int csdrb_dcblock_bank_ff(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int input_size, float a,
+                          dcblock_preserve_t* d_state_io, void* stream)
+{
+    const char* who = "dcblock bank";
+    int rc = demod_args(who, d_in, 4, in_stride, d_out, out_stride, channels, input_size, d_state_io, true);
+    if (rc >= 0 && !d_state_io) { set_error("%s: null state", who); rc = -1; }
+    if (rc) return rc < 0 ? rc : 0;
+    rc = launch_dcblock_bank(d_in, in_stride, d_out, out_stride, channels, input_size, a, d_state_io, S(stream));
+    return rc < 0 ? rc : counted(0, rc);
+}
 
 // ---- host-buffer bank call: the e2e path -------------------------------------------------------------
 // Streams a [channels][input_size] HOST bank through the device in channel chunks on three streams so

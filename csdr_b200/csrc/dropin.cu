@@ -170,6 +170,56 @@ complexf fmdemod_quadri_cf(complexf* input, float* output, int input_size, float
     return input[input_size - 1];
 }
 
+complexf fmdemod_quadri_novect_cf(complexf* input, float* output, int input_size, complexf last_sample)
+{
+    if (input_size <= 0) return last_sample;
+    Staging st("fmdemod_quadri_novect_cf");
+    const complexf* d_in = st.up(input, input_size);
+    const complexf* d_last = st.up(&last_sample, 1);
+    float* d_out = st.alloc<float>(input_size);
+    st.check(csdrb_fmdemod_quadri_novect_bank_cf(d_in, (input_size + 1) & ~1, d_out, (input_size + 1) & ~1, 1, input_size, d_last, nullptr, st.stream()));
+    st.get(output, d_out, input_size);
+    st.sync();
+    return input[input_size - 1];
+}
+
+float fmdemod_atan_cf(complexf* input, float* output, int input_size, float last_phase)
+{
+    if (input_size <= 0) return last_phase;
+    Staging st("fmdemod_atan_cf");
+    const complexf* d_in = st.up(input, input_size);
+    float* d_phase = st.up(&last_phase, 1);                               // in: the carried phase; out: the last sample's
+    float* d_out = st.alloc<float>(input_size);
+    float* d_phase_out = st.alloc<float>(1);
+    st.check(csdrb_fmdemod_atan_bank_cf(d_in, input_size, d_out, input_size, 1, input_size, d_phase, d_phase_out, st.stream()));
+    st.get(output, d_out, input_size);
+    st.get(&last_phase, d_phase_out, 1);
+    st.sync();
+    return last_phase;
+}
+
+void amdemod_estimator_cf(complexf* input, float* output, int input_size, float alpha, float beta)
+{
+    elementwise("amdemod_estimator_cf", input, output, input_size, [=](const complexf* in, float* out, long n, void* s) {
+        return csdrb_amdemod_estimator_bank_cf(in, n, out, n, 1, (int)n, alpha, beta, s);
+    });
+}
+
+// input == output gives what separate buffers give, not libcsdr's in-place result (include/csdr_b200.h)
+dcblock_preserve_t dcblock_ff(float* input, float* output, int input_size, float a, dcblock_preserve_t preserved)
+{
+    if (input_size <= 0) return preserved;
+    Staging st("dcblock_ff");
+    const float* d_in = st.up(input, input_size);
+    dcblock_preserve_t* d_state = st.up(&preserved, 1);
+    float* d_out = st.alloc<float>(input_size);
+    st.check(csdrb_dcblock_bank_ff(d_in, input_size, d_out, input_size, 1, input_size, a, d_state, st.stream()));
+    st.get(output, d_out, input_size);
+    st.get(&preserved, d_state, 1);
+    st.sync();
+    return preserved;
+}
+
 // ---- shift / fractional decimator / fastagc ----------------------------------------------------------
 float shift_addition_cc(complexf* input, complexf* output, int input_size, shift_addition_data_t d, float starting_phase)
 {

@@ -404,14 +404,20 @@ int launch_power(const float2* d_in_c, const float* d_in_f, float* d_out, long n
 // exactly as the C expression promotes it (libcsdr.c:1065).
 #define FMDEMOD_K 0.340447550238101026565118445432744920253753662109375
 
+// Guard = false is fmdemod_quadri_novect_cf (libcsdr.c:1024-1037) as the reference build computes it: the numerator as I*(Q-Qp) + Q*(Ip-I),
+// which differs from the guarded form only in the sign of a zero (equal consecutive samples with I < 0), and den = 0 divided by (NaN for 0/0,
+// else +-Inf) instead of giving 0.
+template <bool Guard>
 __device__ __forceinline__ float quadri(float2 cur, float2 prev)
 {
-    const float dq = __fsub_rn(cur.y, prev.y), di = __fsub_rn(cur.x, prev.x);
-    const float num = __fsub_rn(__fmul_rn(cur.x, dq), __fmul_rn(cur.y, di));
+    const float dq = __fsub_rn(cur.y, prev.y);
+    const float num = Guard ? __fsub_rn(__fmul_rn(cur.x, dq), __fmul_rn(cur.y, __fsub_rn(cur.x, prev.x)))
+                            : __fadd_rn(__fmul_rn(cur.x, dq), __fmul_rn(cur.y, __fsub_rn(prev.x, cur.x)));
     const float den = __fadd_rn(__fmul_rn(cur.x, cur.x), __fmul_rn(cur.y, cur.y));
-    return den != 0.f ? (float)(FMDEMOD_K * (double)num / (double)den) : 0.f;
+    return !Guard || den != 0.f ? (float)(FMDEMOD_K * (double)num / (double)den) : 0.f;
 }
 
+template <bool Guard>
 __global__ void __launch_bounds__(256)
 fmdemod_quadri_bank_kernel(const float2* __restrict__ in, long in_stride, float* __restrict__ out, long out_stride, int n,
                            const float2* __restrict__ last_in, float2* __restrict__ last_out)
@@ -429,17 +435,18 @@ fmdemod_quadri_bank_kernel(const float2* __restrict__ in, long in_stride, float*
             const float4 q = reinterpret_cast<const float4*>(x)[v];
             const float2 a = make_float2(q.x, q.y), b = make_float2(q.z, q.w);
             const float2 p = v ? x[2 * v - 1] : carry;
-            reinterpret_cast<float2*>(y)[v] = make_float2(quadri(a, p), quadri(b, a));   // y is 8-byte aligned when out_stride is even
+            reinterpret_cast<float2*>(y)[v] = make_float2(quadri<Guard>(a, p), quadri<Guard>(b, a));   // y is 8-byte aligned when out_stride is even
         }
-        if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0) y[n - 1] = quadri(x[n - 1], n > 1 ? x[n - 2] : carry);
+        if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0) y[n - 1] = quadri<Guard>(x[n - 1], n > 1 ? x[n - 2] : carry);
     } else {
-        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) y[i] = quadri(x[i], i ? x[i - 1] : carry);
+        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) y[i] = quadri<Guard>(x[i], i ? x[i - 1] : carry);
     }
     if (last_out && blockIdx.x == 0 && threadIdx.x == 0 && n > 0) last_out[ch] = x[n - 1];
 }
 
-int launch_fmdemod_quadri_bank(const float2* d_in, long in_stride, float* d_out, long out_stride, int channels, int n,
-                               const float2* d_last_in, float2* d_last_out, cudaStream_t st)
+template <bool Guard>
+static int launch_quadri(const float2* d_in, long in_stride, float* d_out, long out_stride, int channels, int n, const float2* d_last_in,
+                         float2* d_last_out, cudaStream_t st)
 {
     if (channels <= 0 || n <= 0) return 0;
     if ((reinterpret_cast<uintptr_t>(d_out) & 7) || (out_stride & 1) ) {
@@ -451,9 +458,20 @@ int launch_fmdemod_quadri_bank(const float2* d_in, long in_stride, float* d_out,
         set_error("fmdemod_quadri bank: last_in and last_out must not alias"); return -1;
     }
     int gx = (n / 2 + 255) / 256; if (gx < 1) gx = 1; if (gx > 64) gx = 64;
-    fmdemod_quadri_bank_kernel<<<dim3(gx, channels), 256, 0, st>>>(d_in, in_stride, d_out, out_stride, n, d_last_in, d_last_out);
+    fmdemod_quadri_bank_kernel<Guard><<<dim3(gx, channels), 256, 0, st>>>(d_in, in_stride, d_out, out_stride, n, d_last_in, d_last_out);
     CSDRB_CUDA(cudaGetLastError());
     return 0;
+}
+
+int launch_fmdemod_quadri_bank(const float2* d_in, long in_stride, float* d_out, long out_stride, int channels, int n,
+                               const float2* d_last_in, float2* d_last_out, cudaStream_t st)
+{
+    return launch_quadri<true>(d_in, in_stride, d_out, out_stride, channels, n, d_last_in, d_last_out, st);
+}
+int launch_fmdemod_quadri_novect_bank(const float2* d_in, long in_stride, float* d_out, long out_stride, int channels, int n,
+                                      const float2* d_last_in, float2* d_last_out, cudaStream_t st)
+{
+    return launch_quadri<false>(d_in, in_stride, d_out, out_stride, channels, n, d_last_in, d_last_out, st);
 }
 
 }  // namespace csdrb

@@ -25,12 +25,20 @@ int launch_convert_s24_f(const unsigned char* d_in, float* d_out, long n, int bi
 int launch_convert_f_s24(const float* d_in, unsigned char* d_out, long n, int bigendian, cudaStream_t st);
 int launch_fmdemod_quadri_bank(const float2* d_in, long in_stride, float* d_out, long out_stride, int channels, int n,
                                const float2* d_last_in, float2* d_last_out, cudaStream_t st);
+// fmdemod_quadri_novect_cf: the same kernel without the den != 0 guard (den = 0 divides: NaN or +-Inf)
+int launch_fmdemod_quadri_novect_bank(const float2* d_in, long in_stride, float* d_out, long out_stride, int channels, int n,
+                                      const float2* d_last_in, float2* d_last_out, cudaStream_t st);
 
 int launch_adpcm_encode_rows(const short* d_in, long in_stride, unsigned char* d_out, long out_stride, int rows, int n, void* d_state_io, cudaStream_t st);
 int launch_compress_fft_adpcm_rows(const float* d_in, long in_stride, unsigned char* d_out, long out_stride, int rows, int fft_size, cudaStream_t st);
 int launch_limit_ff(const float* d_in, float* d_out, long n, float max_amplitude, cudaStream_t st);
 int launch_deemphasis_wfm_bank(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int n, float tau, int sample_rate,
                                float* d_last_io, cudaStream_t st);
+// dcblock_ff with the de-emphasis bank's scheme; DcBlockState has the layout of dcblock_preserve_t (include/csdr_b200.h), DcBlockState[channels]
+// on the device; a = 0 means 0.999
+struct DcBlockState { float last_input, last_output; };
+int launch_dcblock_bank(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int n, float a, void* d_state_io,
+                        cudaStream_t st);
 // WFM audio tail `fractional_decimator_ff R 12 | deemphasis_wfm_ff SR TAU | convert_f_s16`, audio.cu.  Parameters and state are the host
 // csdrb_wfm_audio_params_t / csdrb_wfm_audio_state_t; both return the s16 samples per row (< 0 refused).
 int wfm_audio_outputs(const void* h_params, const void* h_state, int n, int* consumed_out);
@@ -93,6 +101,13 @@ int rational_resampler_state(int input_size, int interpolation, int decimation, 
 int launch_rational_resampler_bank(const float* d_in, long in_stride, float* d_out, long out_stride, int channels, int input_size,
                                    int interpolation, int decimation, const float* h_taps, int taps_length, int last_taps_delay,
                                    int* h_state, cudaStream_t st);
+
+// fmdemod_atan_cf and amdemod_estimator_cf, demod.cu.  The atan bank carries one float phase per channel (d_last_in NULL: 0; d_last_out NULL:
+// not written; the two must not alias); the estimator takes alpha == 0 as the reference's default pair.
+int launch_fmdemod_atan_bank(const float2* d_in, long in_stride, float* d_out, long out_stride, int channels, int n, const float* d_last_in,
+                             float* d_last_out, cudaStream_t st);
+int launch_amdemod_estimator_bank(const float2* d_in, long in_stride, float* d_out, long out_stride, int channels, int n, float alpha, float beta,
+                                  cudaStream_t st);
 
 // AM / SSB receiver blocks, agc.cu.  AgcParams / AgcState have the layout of csdrb_agc_params_t / csdrb_agc_state_t (include/csdr_b200.h).
 struct AgcParams { float reference, attack_rate, decay_rate, max_gain; int hang_time, attack_wait_time; float gain_filter_alpha; int chunk; };

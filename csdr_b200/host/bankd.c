@@ -14,7 +14,7 @@
  *
  * usage: csdr-bankd [--in -|HOST:PORT] [--u8|--s8|--f32|--s16|--real-s16|--real-f32] [--decimation D] [--bw TRANSITION_BW] [--window W] [--block SAMPLES]
  *                   [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty|wfm] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B] [--bfsk SPACING:LENGTH]
- *                   [--resample I:D[:BW]]
+ *                   [--resample I:D[:BW]] [--fm-demod quadri|atan]
  *                   [--wfm-rate R] [--tau T]
  *                   [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]
  *                   [--waterfall SINK [--fft-size N] [--fft-every E] [--fft-averages A] [--fft-add-db X] [--fft-window W] [--fft-compression adpcm|none]
@@ -46,6 +46,12 @@
  *     rtl_sdr -s 2400000 -f 89300000 - | csdr-bankd --decimation 10 --bw 0.05 --tail wfm -0.085:a.s16 0.0:b.s16 0.2:c.s16
  *   and the whole 88-108 MHz band from a 20 Msps receiver, about 100 stations (250 kHz channels, 999 taps = 13 per output period):
  *     ... | csdr-bankd --decimation 80 --bw 0.004 --tail wfm --wfm-rate 5.2083333 -0.45:s1.s16 -0.44:s2.s16 ...
+ *   --fm-demod quadri|atan picks the FM discriminator of the nfm, none, wfm and rtty tails.  quadri (default) is the bank's fmdemod_quadri_cf,
+ *   K*|z[n-1]|/|z[n]|*sin(dphi) with K = 0.3404: sin() bends loud broadcast FM (75 kHz deviation in a 240 kHz channel takes dphi to 1.96 rad,
+ *   harmonics about -13 dB below the tone).  atan runs the bank with the complex baseband (as --bfsk does) and fmdemod_atan_cf on it, dphi/pi,
+ *   straight up to +-pi; per channel the stream is then ... | fir_decimate_cc D bw W | fmdemod_atan_cf | <the rest of the tail>, the phase
+ *   carried from block to block.  At small deviation atan's level is 1/(pi*K) = 0.935 of quadri's, about 7 % lower on the none and wfm tails;
+ *   the NFM AGC absorbs it.  Not with --bfsk, nor with the iq, am, usb, lsb and bpsk31 tails, which take the baseband.
  *   --decimation: any even D (default 50) whose filter the fused bank serves: M = ceil(taps / D) <= 24 and D * M (rounded up to the kernel's
  *   bucket) <= 8000 taps, see csdrb_ddc_bank in include/csdr_b200.h.  The NFM tail's deemphasis_nfm_ff stays at 48000 whatever D gives: where
  *   wideband rate / D is not 48 kHz, --resample I:D[:BW] puts rational_resampler_ff I D BW right behind the discriminator (tails nfm and none; see
@@ -810,38 +816,63 @@ typedef struct {
     csdrb_serial_line_params_t rtty;                                 /* --sps F, --databits, --stopbits of --tail rtty */
     float bfsk_spacing;                                              /* --bfsk SPACING:LENGTH of --tail rtty (bfsk_L 0: the discriminator) */
     int bfsk_L;
+    int fm_atan;                                                     /* --fm-demod atan: fmdemod_atan_cf instead of the bank's quadri-correlator */
     waterfall_opts_t wf;
 } opts_t;
+
+/* --fm-demod atan: the bank gives complexf baseband rows, and fmdemod_atan_cf turns them into the discriminator rows of the resampler or the tail,
+ * each channel's phase carried from call to call (phase[cur] in, phase[cur ^ 1] out: the bank's in and out must not alias; zero at stream start)
+ *   bb : [C][bs] complexf, the new baseband samples from the front of every row */
+typedef struct { complexf *d_bb; long bs; float *d_phase[2]; int cur; } atan_stage_t;
+
+static void atan_stage_init(atan_stage_t *a, int C, int in_cap)
+{
+    a->bs = ((long)in_cap + 3) & ~3L;
+    a->d_bb = csdrb_device_alloc(sizeof(complexf) * (size_t)C * (size_t)a->bs);
+    a->d_phase[0] = csdrb_device_alloc(sizeof(float) * (size_t)C);
+    a->d_phase[1] = csdrb_device_alloc(sizeof(float) * (size_t)C);
+    if (!a->d_bb || !a->d_phase[0] || !a->d_phase[1]) die("out of memory");
+}
+
+/* n new baseband samples per channel at the front of d_bb: their discriminator output to dst (row pitch in floats) */
+static void atan_stage_push(atan_stage_t *a, int C, int n, float *dst, long pitch, void *stream)
+{
+    OK(csdrb_fmdemod_atan_bank_cf(a->d_bb, a->bs, dst, pitch, C, n, a->d_phase[a->cur], a->d_phase[a->cur ^ 1], stream));
+    a->cur ^= 1;
+}
 
 /* ---- the tail interface: the only code past option validation that knows which tail runs ----------------------------------------------------
  * tail_in gives the device rows where the next bank outputs land (the resampler's input with --resample); tail_push runs the resampler if on
  * and the tail over the n samples per channel put there and writes the sinks; tail_push_host does both for rows in host memory (--devices).
  * All buffers are on ONE device: the single-GPU path's own, the first device of --devices. */
 typedef struct {
-    int kind, C, resample;
+    int kind, C, resample, atan;
     size_t esz;                                                      /* one bank output sample: float (demodulated) or complexf */
+    atan_stage_t fm;
     rs_stage_t rs;
     union { nfm_tail_t nfm; raw_tail_t raw; bb_tail_t bb; bpsk_tail_t bpsk; rtty_tail_t rtty; wfm_tail_t wfm; } u;
 } tail_t;
 
-/* whether the bank demodulates: the tail's choice, except that --tail rtty --bfsk takes the complex baseband */
-static int bank_demod(const opts_t *o) { return kTails[o->tail].demod && !o->bfsk_L; }
+/* whether the bank demodulates: the tail's choice, except that --tail rtty --bfsk and --fm-demod atan take the complex baseband */
+static int bank_demod(const opts_t *o) { return kTails[o->tail].demod && !o->bfsk_L && !o->fm_atan; }
 
-/* --devices --tail none without --resample: the rows collected on the host are the output, so that tail needs no device, stream or buffer */
-static int tail_host_fed(int kind, int resample) { return kind == TAIL_NONE && !resample; }
+/* --devices --tail none without --resample or --fm-demod atan: the rows collected on the host are the output, so that tail needs no device,
+ * stream or buffer */
+static int tail_host_fed(int kind, int resample, int atan) { return kind == TAIL_NONE && !resample && !atan; }
 
 /* in_cap: the most samples per channel one block adds; stream NULL for a host-fed tail, which allocates nothing.  The per-tail inits fill the
  * state zeroed here. */
 static void tail_init(tail_t *t, const opts_t *o, int C, int in_cap, void *stream)
 {
     memset(t, 0, sizeof *t);
-    t->kind = o->tail; t->C = C; t->resample = o->rs_I > 0;
+    t->kind = o->tail; t->C = C; t->resample = o->rs_I > 0; t->atan = o->fm_atan;
     t->esz = bank_demod(o) ? sizeof(float) : sizeof(complexf);
     if (!stream) return;
+    if (t->atan) atan_stage_init(&t->fm, C, in_cap);
     if (t->resample) { rs_init(&t->rs, C, o->rs_I, o->rs_D, o->rs_bw, in_cap); in_cap = rs_out_cap(&t->rs); }
     switch (t->kind) {
     case TAIL_NFM: nfm_tail_init(&t->u.nfm, C, in_cap, o->limit, o->agc_ref); break;
-    case TAIL_NONE: case TAIL_IQ: raw_tail_init(&t->u.raw, C, in_cap, t->esz); break;
+    case TAIL_NONE: case TAIL_IQ: raw_tail_init(&t->u.raw, C, in_cap, t->kind == TAIL_NONE ? sizeof(float) : sizeof(complexf)); break;
     case TAIL_AM: bb_tail_init(&t->u.bb, C, in_cap, o->limit, o->agc_ref, NULL, stream); break;
     case TAIL_USB: bb_tail_init(&t->u.bb, C, in_cap, o->limit, o->agc_ref, (const float[2]){0.0f, 0.1f}, stream); break;
     case TAIL_LSB: bb_tail_init(&t->u.bb, C, in_cap, o->limit, o->agc_ref, (const float[2]){-0.1f, 0.0f}, stream); break;
@@ -854,7 +885,8 @@ static void tail_init(tail_t *t, const opts_t *o, int C, int in_cap, void *strea
     }
 }
 
-static void *tail_in(tail_t *t, long *pitch)
+/* where the discriminator output (or, for iq, am, usb, lsb, bpsk31 and rtty --bfsk, the baseband) goes next */
+static void *demod_in(tail_t *t, long *pitch)
 {
     if (t->resample) { *pitch = t->rs.rs; return t->rs.d_in + t->rs.have; }
     switch (t->kind) {
@@ -869,9 +901,20 @@ static void *tail_in(tail_t *t, long *pitch)
     }
 }
 
+static void *tail_in(tail_t *t, long *pitch)
+{
+    if (t->atan) { *pitch = t->fm.bs; return t->fm.d_bb; }
+    return demod_in(t, pitch);
+}
+
 /* n new bank outputs per channel sit at tail_in: through the resampler if on, then the tail, output to the sinks */
 static void tail_push(tail_t *t, channel_t *chan, int n, void *stream)
 {
+    if (t->atan) {
+        long pitch;
+        float *dst = demod_in(t, &pitch);
+        atan_stage_push(&t->fm, t->C, n, dst, pitch, stream);
+    }
     switch (t->kind) {
     case TAIL_NFM:
         if (t->resample) n = rs_push(&t->rs, n, t->u.nfm.d_demod + t->u.nfm.a_have, t->u.nfm.ds, stream);
@@ -895,7 +938,7 @@ static void tail_push(tail_t *t, channel_t *chan, int n, void *stream)
 static void tail_push_host(tail_t *t, channel_t *chan, const unsigned char *h_rows, int n, void *stream)
 {
     const size_t width = t->esz * (size_t)n;
-    if (tail_host_fed(t->kind, t->resample)) { write_rows(chan, t->C, h_rows, width, NULL); return; }
+    if (tail_host_fed(t->kind, t->resample, t->atan)) { write_rows(chan, t->C, h_rows, width, NULL); return; }
     long pitch;
     void *d_in = tail_in(t, &pitch);
     OK(csdrb_copy2d_h2d(d_in, t->esz * (size_t)pitch, h_rows, width, width, (size_t)t->C, stream));
@@ -915,7 +958,7 @@ static int run_multi(const opts_t *o, channel_t *chan, int C, const float *rates
     /* the tail (and the resampler) is audio-rate work (C x the channel rate): the rows every device returned go to the FIRST device once more and
      * through the same tail as in the single-GPU path */
     tail_t tail;
-    void *tail_stream = tail_host_fed(o->tail, o->rs_I > 0) ? NULL : device_stream(o->devs[0]);
+    void *tail_stream = tail_host_fed(o->tail, o->rs_I > 0, o->fm_atan) ? NULL : device_stream(o->devs[0]);
     tail_init(&tail, o, C, n_out + 2, tail_stream);
     float lut[256];
     for (int i = 0; i < 256; i++) lut[i] = (float)((float)i / (UCHAR_MAX / 2.0) - 1.0);      /* convert_u8_f, libcsdr.c:2365 */
@@ -987,7 +1030,7 @@ static int usage(void)
             "usage: csdr-bankd [--in -|HOST:PORT] [--u8|--s8|--f32|--s16|--real-s16|--real-f32] [--decimation D] [--bw TRANSITION_BW] [--window W]\n"
             "                  [--block SAMPLES]\n"
             "                  [--tail nfm|none|am|usb|lsb|iq|bpsk31|rtty|wfm] [--sps N] [--databits N] [--stopbits S] [--rtty-bufsize B]\n"
-            "                  [--bfsk SPACING:LENGTH]\n"
+            "                  [--bfsk SPACING:LENGTH] [--fm-demod quadri|atan]\n"
             "                  [--wfm-rate R] [--tau T] [--resample I:D[:BW]] [--limit L] [--agc-ref R] [--device N | --devices N0,N1,...]\n"
             "                  RATE:SINK [RATE:SINK ...]\n"
             "  --u8 | --f32 | --s16 the complex input: rtl_sdr's u8 IQ (default), complex float, or complex s16 (Airspy INT16_IQ, SDRplay, ...)\n"
@@ -1023,6 +1066,12 @@ static int usage(void)
             "                       complex baseband (peaks at +-SPACING/2 cycles per baseband sample, Hamming, LENGTH taps, 2..4096).  They hold\n"
             "                       up in noise below the discriminator's threshold.  170 Hz shift at 2 kHz baseband (2.4 Msps, --decimation 1200):\n"
             "                       csdr-bankd --decimation 1200 --bw 0.001 --tail rtty --sps 44 --bfsk 0.085:44 -0.1:ch1.txt 0.05:ch2.txt\n"
+            "  --fm-demod quadri|atan  the FM discriminator of --tail nfm, none, wfm and rtty.  quadri (default): the bank's fmdemod_quadri_cf,\n"
+            "                       K*|z[n-1]|/|z[n]|*sin(dphi) with K = 0.3404, which bends loud broadcast FM (75 kHz deviation at 240 kHz\n"
+            "                       channels: harmonics about -13 dB).  atan: fmdemod_atan_cf on the bank's baseband, dphi/pi, straight up to\n"
+            "                       +-pi.  At small deviation its level is about 7 %% lower than quadri's (1/pi against K): the none and wfm\n"
+            "                       outputs come out that much quieter, the NFM AGC absorbs it.  Not with --bfsk or the baseband tails.  Broadcast FM:\n"
+            "                       rtl_sdr -s 2400000 -f 89300000 - | csdr-bankd --decimation 10 --bw 0.05 --tail wfm --fm-demod atan 0.0:a.s16\n"
             "  --resample I:D[:BW]  rational_resampler_ff I D BW (BW default 0.05) right behind the discriminator, for --tail nfm and none: brings\n"
             "                       wideband/decimation to the 48 kHz the NFM de-emphasis is designed for (e.g. 2.048 Msps, --decimation 32,\n"
             "                       --resample 3:4).  With T = taps of BW, the daemon needs (T/I + 1)*I >= 2*D + I - 1 (T >= 2*D + I - 2 suffices),\n"
@@ -1081,6 +1130,12 @@ int main(int argc, char **argv)
             if (o.bfsk_L < 2 || o.bfsk_L > 4096) die("--bfsk LENGTH must be between 2 and 4096 taps");
             a++;
         }
+        else if (!strcmp(arg, "--fm-demod") && v) {
+            if (!strcmp(v, "atan")) o.fm_atan = 1;
+            else if (!strcmp(v, "quadri")) o.fm_atan = 0;
+            else die("--fm-demod is quadri or atan");
+            a++;
+        }
         else if (!strcmp(arg, "--wfm-rate") && v) { o.wfm_rate = (float)atof(v); wfm_opts = 1; a++; }
         else if (!strcmp(arg, "--tau") && v) { o.tau = (float)atof(v); wfm_opts = 1; a++; }
         else if (!strcmp(arg, "--waterfall") && v) { o.wf_sink = v; a++; }
@@ -1128,6 +1183,8 @@ int main(int argc, char **argv)
     } else if (o.sps) die("--sps belongs to --tail bpsk31 and --tail rtty");
     if (o.tail != TAIL_RTTY && rtty_opts) die("--databits, --stopbits and --rtty-bufsize belong to --tail rtty");
     if (o.tail != TAIL_RTTY && o.bfsk_L) die("--bfsk belongs to --tail rtty");
+    if (o.fm_atan && !kTails[o.tail].demod) die("--fm-demod atan works with --tail nfm, none, wfm and rtty only (the iq, am, usb, lsb and bpsk31 tails take the baseband)");
+    if (o.fm_atan && o.bfsk_L) die("--fm-demod atan and --bfsk are two different demodulators: choose one");
     if (o.tail == TAIL_WFM) {
         /* above 16 a decimator call could consume more than its 1024 samples (the reference then memmoves a negative length): WFM needs about 5 */
         if (!(o.wfm_rate > 1.0f && o.wfm_rate <= 16.0f)) die("--wfm-rate must be above 1 and at most 16 (wideband rate / decimation / 48 kHz)");

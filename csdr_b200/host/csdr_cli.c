@@ -135,13 +135,15 @@ static int initial_tuning(int ctl, int argc, char **argv, const char *format, fl
 /* ---- shared framing ------------------------------------------------------------------------------ */
 /* One step call per block of the process on the whole buffer, written as out_count items.  The end-of-file test comes before the read, so a
  * short final read is still processed and written as a whole block, its tail left over from the block before (:248).  Some reference loops
- * also stop on an empty read (empty_read_stops). */
+ * also stop on an empty read (empty_read_stops = 1); fmdemod_atan_cf tests end of file right after its read, so a short final read is
+ * dropped and only whole blocks come out (empty_read_stops = 2, :976). */
 static int map_blocks(size_t in_item, size_t out_item, int out_count, int empty_read_stops, void (*step)(void *in, void *out, void *state), void *state)
 {
     void *in = must_alloc(in_item * (size_t)block), *out = must_alloc(out_item * (size_t)out_count);
     for (;;) {
         if (feof(stdin)) return 0;
         if (!fread(in, in_item, (size_t)block, stdin) && empty_read_stops) return 0;
+        if (empty_read_stops == 2 && feof(stdin)) return 0;
         step(in, out, state);
         fwrite(out, out_item, (size_t)out_count, stdout);
         end_of_block();
@@ -661,6 +663,44 @@ static int cmd_amdemod_cf(int argc, char **argv)                            /* c
     (void)argc; (void)argv;
     if (!announce_block(open_block())) return -2;
     return map_blocks(sizeof(complexf), sizeof(float), block, 0, amdemod_step, NULL);
+}
+
+/* fmdemod_atan_cf (csdr.c:970-983, whole blocks only), fmdemod_quadri_novect_cf (:999-1012), amdemod_estimator_cf (:1101-1112) and
+ * dcblock_ff (:938-950): the carried phase, sample and filter state start at zero */
+static void atan_step(void *in, void *out, void *last) { *(float *)last = fmdemod_atan_cf(in, out, block, *(float *)last); }
+static void novect_step(void *in, void *out, void *last) { *(complexf *)last = fmdemod_quadri_novect_cf(in, out, block, *(complexf *)last); }
+static void estimator_step(void *in, void *out, void *state) { (void)state; amdemod_estimator_cf(in, out, block, 0.f, 0.f); }
+static void dcblock_step(void *in, void *out, void *dcp) { *(dcblock_preserve_t *)dcp = dcblock_ff(in, out, block, 0.f, *(dcblock_preserve_t *)dcp); }
+
+static int cmd_fmdemod_atan_cf(int argc, char **argv)
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    float last_phase = 0.f;
+    return map_blocks(sizeof(complexf), sizeof(float), block, 2, atan_step, &last_phase);
+}
+
+static int cmd_fmdemod_quadri_novect_cf(int argc, char **argv)
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    complexf last = {0.f, 0.f};
+    return map_blocks(sizeof(complexf), sizeof(float), block, 0, novect_step, &last);
+}
+
+static int cmd_amdemod_estimator_cf(int argc, char **argv)
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    return map_blocks(sizeof(complexf), sizeof(float), block, 0, estimator_step, NULL);
+}
+
+static int cmd_dcblock_ff(int argc, char **argv)
+{
+    (void)argc; (void)argv;
+    if (!announce_block(open_block())) return -2;
+    dcblock_preserve_t dcp = {0.f, 0.f};
+    return map_blocks(sizeof(float), sizeof(float), block, 0, dcblock_step, &dcp);
 }
 
 static void realpart_step(void *in, void *out, void *state) { (void)state; for (int i = 0; i < block; i++) ((float *)out)[i] = ((complexf *)in)[i].i; }
@@ -1213,6 +1253,10 @@ static const struct { const char *name; int (*run)(int, char **); const char *sy
     {"fastagc_ff", cmd_fastagc_ff, "fastagc_ff [block_size [reference]]"},
     {"limit_ff", cmd_limit_ff, "limit_ff [max_amplitude]"},
     {"amdemod_cf", cmd_amdemod_cf, "amdemod_cf"},
+    {"amdemod_estimator_cf", cmd_amdemod_estimator_cf, "amdemod_estimator_cf"},
+    {"fmdemod_atan_cf", cmd_fmdemod_atan_cf, "fmdemod_atan_cf"},
+    {"fmdemod_quadri_novect_cf", cmd_fmdemod_quadri_novect_cf, "fmdemod_quadri_novect_cf"},
+    {"dcblock_ff", cmd_dcblock_ff, "dcblock_ff"},
     {"realpart_cf", cmd_realpart_cf, "realpart_cf"},
     {"fastdcblock_ff", cmd_fastdcblock_ff, "fastdcblock_ff [block_size (<= 49152)]"},
     {"agc_ff", cmd_agc_ff, "agc_ff [hang_time [reference [attack_rate [decay_rate [max_gain [attack_wait [filter_alpha]]]]]]]"},

@@ -76,6 +76,24 @@ int fir_decimate_cc(complexf *input, complexf *output, int input_size, int decim
 /* FM demodulator (libcsdr.h:95; libcsdr.c:1040-1071): `temp` is accepted and ignored */
 complexf fmdemod_quadri_cf(complexf *input, float *output, int input_size, float *temp, complexf last_sample);
 
+/* the other demodulators of libcsdr.h:95-116 (libcsdr.c:875-918, 1004-1037), computed as the reference's -O3 -ffast-math build computes them
+ * (DESIGN.md section 7).  fmdemod_atan_cf returns the last sample's phase (pass it back as last_phase; 0 at stream start); its phase is CUDA's
+ * double atan2 rounded to float, which can differ from the reference's by one float ulp on about 1e-8 of samples.  fmdemod_quadri_novect_cf
+ * is fmdemod_quadri_cf without the guard on a zero |x|^2 (NaN or +-Inf there) and returns the last input sample.  amdemod_estimator_cf takes
+ * alpha == 0 as the reference's default pair, beta ignored then.  dcblock_ff with a == 0 uses 0.999; preserved is {0, 0} at stream start.
+ * dcblock_ff in place (input == output) gives what separate buffers give.  libcsdr's loop differs there: it reads input[i-1] after writing
+ * output[i-1], so in place it computes y[i] = (x[i] - y[i-1]) + a*y[i-1] and returns last_input = y[n-1]; this drop-in does not reproduce that
+ * (no caller of the reference runs dcblock_ff in place). */
+float fmdemod_atan_cf(complexf *input, float *output, int input_size, float last_phase);
+complexf fmdemod_quadri_novect_cf(complexf *input, float *output, int input_size, complexf last_sample);
+void amdemod_estimator_cf(complexf *input, float *output, int input_size, float alpha, float beta);
+typedef struct dcblock_preserve_s
+{
+    float last_input;
+    float last_output;
+} dcblock_preserve_t;
+dcblock_preserve_t dcblock_ff(float *input, float *output, int input_size, float a, dcblock_preserve_t preserved);
+
 /* fractional decimator (libcsdr.h:151-170; libcsdr.c:715-793) */
 typedef struct fractional_decimator_ff_s {
     float where; int input_processed; int output_size; int num_poly_points;
@@ -305,6 +323,32 @@ int csdrb_fir_decimate_bank_u8_host(const unsigned char *h_in, long in_stride, c
  * d_last_out[c] receives its last sample (may be NULL; must not alias d_last_in). */
 int csdrb_fmdemod_quadri_bank_cf(const complexf *d_in, long in_stride, float *d_out, long out_stride, int channels,
                                  int input_size, const complexf *d_last_in, complexf *d_last_out, void *stream);
+/* fmdemod_quadri_novect_cf bank: the same call, the same bits except where I*I + Q*Q rounds to 0, which fmdemod_quadri_novect_cf divides by
+ * (NaN for 0/0, +-Inf otherwise) where the bank above gives 0. */
+int csdrb_fmdemod_quadri_novect_bank_cf(const complexf *d_in, long in_stride, float *d_out, long out_stride, int channels,
+                                        int input_size, const complexf *d_last_in, complexf *d_last_out, void *stream);
+
+/* fmdemod_atan_cf bank (libcsdr.c:1004-1019): y = wrap(arg x[i] - arg x[i-1]) / pi, so +-1 is +-half the channel's sample rate.
+ * d_last_phase_in[c] is the phase before channel c's block (NULL = 0, the stream start), d_last_phase_out[c] receives its last sample's phase
+ * (may be NULL; must not alias d_last_phase_in).  Bit for bit the reference build except where CUDA's double atan2 and the host's round to
+ * different floats (within 2 ulp of double of a float rounding midpoint, about 1e-8 of samples).  Rows at any 8-byte (in) / 4-byte (out)
+ * address; d_in == d_out is not allowed.  Returns 0; a negative code (csdrb_last_error()) with nothing launched for a null pointer, a
+ * misalignment, more than 65535 channels, strides below input_size or aliased phase buffers. */
+int csdrb_fmdemod_atan_bank_cf(const complexf *d_in, long in_stride, float *d_out, long out_stride, int channels, int input_size,
+                               const float *d_last_phase_in, float *d_last_phase_out, void *stream);
+
+/* amdemod_estimator_cf bank (libcsdr.c:875-901): y = alpha*max(|I|,|Q|) + beta*min(|I|,|Q|), with the build's selections on NaN (a NaN takes
+ * |Q| in rows of 2 samples or more, the build's SSE loops, and |I| in a row of one sample, its scalar loop); alpha == 0 takes
+ * the reference's defaults (0.947543636291, 0.392485425092) and ignores beta.  Bit for bit the reference build.  Refusals as above. */
+int csdrb_amdemod_estimator_bank_cf(const complexf *d_in, long in_stride, float *d_out, long out_stride, int channels, int input_size,
+                                    float alpha, float beta, void *stream);
+
+/* dcblock_ff bank (libcsdr.c:903-918): y[0] = (x[0] - s.last_input) + a*s.last_output, y[i] = (x[i] - x[i-1]) + a*y[i-1]; a == 0 means 0.999.
+ * d_state_io[c] is channel c's dcblock_preserve_t ({0, 0} at stream start), updated to {x[n-1], y[n-1]}.  Sequential per channel, bit for bit
+ * the reference build; calls over consecutive pieces of a stream give the bits of one long call.  In place (d_in == d_out with equal strides)
+ * is allowed and gives what separate buffers give.  Refusals as above. */
+int csdrb_dcblock_bank_ff(const float *d_in, long in_stride, float *d_out, long out_stride, int channels, int input_size, float a,
+                          dcblock_preserve_t *d_state_io, void *stream);
 
 /* K2 shift_addition_cc bank.  in_stride == 0: every channel shifts the SAME wideband input (ddcd use case).
  * d_params[c] = shift_addition_init(rate_c) computed on the host (bit-exact sin/cos deltas); d_phase_io[c] is the

@@ -69,3 +69,11 @@ z = cplx(3, 1037)
 cb.add_dcoffset_bank(z[:, :1035]); cb.add_dcoffset_bank(z[:, 1:]); cb.add_dcoffset_bank(z, out=z)
 cb.fixed_amplitude_bank(z[:, :1031], 2.0); cb.fixed_amplitude_bank(z[:, 1:], 1.0); cb.fixed_amplitude_bank(z, 0.5, out=z)
 torch.cuda.synchronize()
+# demodulator banks: atan tiles with ragged ends and rows off 16-byte alignment, novect, the estimator's pair and single paths, dcblock in place
+z = cplx(3, 2051)
+for n in (1, 5, 1023, 1025, 2051): cb.fmdemod_atan_bank_cf(z[:, :n]); cb.fmdemod_atan_bank_cf(z[:, 1:n + 1] if n < 2051 else z[:, :n], last=torch.zeros(3, device=dev))
+cb.fmdemod_atan_bank_cf(z, return_last=True); cb.fmdemod_quadri_novect_bank_cf(z[:, :2049]); cb.fmdemod_quadri_novect_bank_cf(z[:, 1:], return_last=True)
+cb.amdemod_estimator_bank_cf(z[:, :1]); cb.amdemod_estimator_bank_cf(z[:, 1:1030], 0.5, 0.25); cb.amdemod_estimator_bank_cf(z)
+r = (torch.rand((37, 1037), device=dev) * 2 - 1)
+cb.dcblock_bank_ff(r[:, :1035]); cb.dcblock_bank_ff(r[:, 1:1030].contiguous(), 0.9, return_state=True); cb.dcblock_bank_ff(r, out=r)
+torch.cuda.synchronize()
